@@ -11,6 +11,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <limits>
+
 namespace cosmo {
 
 constexpr int kBlock = 256;           // threads per block for every reducing kernel
@@ -150,6 +152,17 @@ __device__ __forceinline__ T nanmax(T a, T b) {
 
 template <typename T>
 __device__ __forceinline__ T tabs(T a) { return a < 0 ? -a : a; }
+
+// exponent e with |x| < 2^e for the largest |x| of a block (0 for 0, inf or NaN), clamped so that 2^-e and 2^e are both
+// normal numbers of T: scaling by 2^-e is exact and brings the maximum into [0.5, 1)
+template <typename T>
+__device__ __forceinline__ int pow2_exponent(T mx) {
+  constexpr double kMax = sizeof(T) == 8 ? 1.7976931348623157e308 : 3.4028234663852886e38;
+  constexpr int lim = std::numeric_limits<T>::max_exponent - 2;
+  int e = 0;
+  if (mx > T(0) && (double)mx <= kMax) frexp((double)mx, &e);
+  return e < -lim ? -lim : (e > lim ? lim : e);
+}
 
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {

@@ -869,7 +869,7 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
     n_soc_chunks_ = (int)cs.size();
     soc_off_.upload(soc_off, stream_); soc_dim_.upload(soc_dim, stream_);
     soc_chunk_start_.upload(cs, stream_); soc_chunk_len_.upload(cl, stream_); soc_cone_chunk_ptr_.upload(ptr, stream_);
-    soc_norm_.alloc(n_soc_); soc_norm2_.alloc(n_soc_); soc_chunk_sum_.alloc(std::max(n_soc_chunks_, 1));
+    soc_norm_.alloc(n_soc_); soc_norm2_.alloc(n_soc_); soc_chunk_sum_.alloc(2 * std::max(n_soc_chunks_, 1));   // (scaled sum, exponent) per chunk
     sync();
   }
   psd_.init(psd_descs, stream_);

@@ -145,8 +145,9 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
   const T inv_sqrt2 = T(0.70710678118654752440);
   const T sqrt2 = T(1.41421356237309504880);
 
-  // ---- load: X = mat(x) ----
-  T fro = 0;
+  // ---- load: X = mat(x) 2^-pe, pe even: the power of two nearest max |X| (exact; every projection is positively
+  // homogeneous, so nothing below overflows or underflows whatever the scale of x, and the result is unscaled at the end)
+  T mx = 0;
   for (int e = threadIdx.x; e < N * N; e += blockDim.x) {
     const int i = e % N, j = e / N;
     T v;
@@ -161,6 +162,21 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
     }
     A[i + j * ld] = v;
     V[i + j * ld] = (i == j) ? T(1) : T(0);
+    mx = fmax(mx, tabs(v));
+  }
+  for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  mx = red[0];
+  for (int w = 1; w < kWarpsPerBlock; ++w) mx = fmax(mx, red[w]);
+  const int pe = pow2_exponent(mx) & ~1;          // even: sqrt(lambda 2^-pe) = sqrt(lambda) 2^(-pe/2) exactly
+  const T down = (T)ldexp(1.0, -pe), up = (T)ldexp(1.0, pe);
+  __syncthreads();
+  T fro = 0;
+  for (int e = threadIdx.x; e < N * N; e += blockDim.x) {
+    const int i = e % N, j = e / N;
+    const T v = A[i + j * ld] * down;
+    A[i + j * ld] = v;
     fro += v * v;
   }
   fro = warp_sum(fro);
@@ -244,7 +260,7 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
     if (threadIdx.x == 0) {
       T f = red[0];
       for (int w = 1; w < kWarpsPerBlock; ++w) f = fmax(f, red[w]);
-      lam_max[blockIdx.x] = f;
+      lam_max[blockIdx.x] = f * up;
     }
     return;
   }
@@ -278,10 +294,10 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
       if (!imag) {
         for (int k = 0; k < N; ++k) acc += V[i + k * ld] * V[j + k * ld] + V[Nc + i + k * ld] * V[Nc + j + k * ld];
         acc *= T(0.5);
-        s[d.off + e] = (i == j) ? acc : sqrt2 * acc;
+        s[d.off + e] = ((i == j) ? acc : sqrt2 * acc) * up;
       } else {
         for (int k = 0; k < N; ++k) acc += V[Nc + i + k * ld] * V[j + k * ld] - V[i + k * ld] * V[Nc + j + k * ld];
-        s[d.off + e] = sqrt2 * T(0.5) * acc;
+        s[d.off + e] = sqrt2 * T(0.5) * acc * up;
       }
     }
   } else if (d.triangle) {
@@ -294,7 +310,7 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
       const int i = e - j * (j + 1) / 2;
       T acc = 0;
       for (int k = 0; k < N; ++k) acc += V[i + k * ld] * V[j + k * ld];
-      s[d.off + e] = (i == j) ? acc : sqrt2 * acc;
+      s[d.off + e] = ((i == j) ? acc : sqrt2 * acc) * up;
     }
   } else {
     for (int e = threadIdx.x; e < N * N; e += blockDim.x) {
@@ -302,7 +318,7 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
       const int a = i < j ? i : j, b = i < j ? j : i;
       T acc = 0;
       for (int k = 0; k < N; ++k) acc += V[a + k * ld] * V[b + k * ld];
-      s[d.off + e] = acc;
+      s[d.off + e] = acc * up;
     }
   }
 }
@@ -310,12 +326,49 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
 // ---------------------------------------------------------------------------
 // Large cones: matrix + eigenvectors in global memory, one kernel triple per round.
 // ---------------------------------------------------------------------------
+// Entries a large cone stores: N (N + 1) / 2 (triangle), N^2 (square), Nc^2 (Hermitian, N = 2 Nc).
+__host__ __device__ inline long long psd_cone_dim(const PsdConeDesc& d) {
+  return d.triangle == 1 ? (long long)d.N * (d.N + 1) / 2 : (d.triangle == 2 ? (long long)(d.N / 2) * (d.N / 2) : (long long)d.N * d.N);
+}
+
+// *mx_bits = max(*mx_bits, max |x[0..dim)|) as the bit pattern of a non-negative double (ordered like the value; a NaN
+// orders above inf).  *mx_bits must be 0 before the first block runs.
+template <typename T>
+__global__ void __launch_bounds__(kBlock) psd_cone_max_kernel(const T* __restrict__ x, long long dim, unsigned long long* __restrict__ mx_bits) {
+  __shared__ double red[kWarpsPerBlock];
+  double mx = 0.0;
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < dim; k += (long long)gridDim.x * blockDim.x) {
+    const double v = fabs((double)x[k]);
+    mx = (v > mx || v != v) ? v : mx;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    const double w = __shfl_xor_sync(0xffffffffu, mx, o);
+    mx = (w > mx || w != w) ? w : mx;
+  }
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long b = 0;
+    for (int w = 0; w < kWarpsPerBlock; ++w) b = max(b, (unsigned long long)__double_as_longlong(red[w]));
+    atomicMax(mx_bits, b);
+  }
+}
+
+// A = mat(x) 2^-pe, V = I, partial sums of |A|_F^2.  pe (even) is the exponent of the power of two nearest max |x|
+// (psd_cone_max_kernel): the scaling is exact, the projection is positively homogeneous, so the eigensolvers and the
+// Newton-Schulz iteration work on a matrix of norm ~1 whatever the scale of x; *up = 2^pe undoes it on the output
+// (psd_unscale_kernel).
 template <typename T>
 __global__ void __launch_bounds__(kBlock) psd_large_load_kernel(PsdConeDesc d, const T* __restrict__ ws, T* __restrict__ A,
-                                                                T* __restrict__ V, T* __restrict__ fro_partials) {
+                                                                T* __restrict__ V, T* __restrict__ fro_partials,
+                                                                const unsigned long long* __restrict__ mx_bits, double* __restrict__ up) {
   const int N = d.N;
   const T* x = ws + d.off;
   const T inv_sqrt2 = T(0.70710678118654752440);
+  const double mxv = __longlong_as_double((long long)*mx_bits);
+  const int pe = (mxv == mxv) ? (pow2_exponent((T)mxv) & ~1) : 0;
+  const T down = (T)ldexp(1.0, -pe);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *up = ldexp(1.0, pe);
   T fro = 0;
   const long long total = (long long)N * N;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
@@ -330,6 +383,7 @@ __global__ void __launch_bounds__(kBlock) psd_large_load_kernel(PsdConeDesc d, c
     } else {
       v = (x[(long long)j * N + i] + x[(long long)i * N + j]) / T(2);
     }
+    v *= down;
     A[e] = v;
     V[e] = (i == j) ? T(1) : T(0);
     fro += v * v;
@@ -354,6 +408,14 @@ __global__ void psd_large_thr_kernel(const T* __restrict__ fro_partials, int npa
     *thr = (T)(PsdEps<T>::v) * sqrt(f);
     *rotated = 0;
   }
+}
+
+// s[0..dim) *= 2^pe: the projection of the prescaled matrix back to the scale of the input
+template <typename T>
+__global__ void __launch_bounds__(kBlock) psd_unscale_kernel(T* __restrict__ s, long long dim, const double* __restrict__ up) {
+  const double f = *up;
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < dim; k += (long long)gridDim.x * blockDim.x)
+    s[k] = (T)((double)s[k] * f);
 }
 
 template <typename T>
@@ -771,11 +833,11 @@ __global__ void __launch_bounds__(256) psd_large_syrk_kernel(PsdConeDesc d, cons
 }
 
 template <typename T>
-__global__ void psd_large_lammax_kernel(int N, const T* __restrict__ A, T* __restrict__ out) {
+__global__ void psd_large_lammax_kernel(int N, const T* __restrict__ A, const double* __restrict__ up, T* __restrict__ out) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     T mx = -INFINITY;
     for (int i = 0; i < N; ++i) mx = fmax(mx, A[i + (long long)i * N]);
-    *out = mx;
+    *out = (T)((double)mx * *up);
   }
 }
 
@@ -801,6 +863,8 @@ struct PsdBatch {
   T *A_d = nullptr, *V_d = nullptr, *cs_d = nullptr, *fro_d = nullptr, *thr_d = nullptr, *lam_large_d = nullptr;
   int* rot_d = nullptr;
   int* rot_h = nullptr;  // pinned
+  unsigned long long* mx_d = nullptr;   // max |entry| of the cone being projected (psd_cone_max_kernel)
+  double* up_d = nullptr;               // 2^pe: the prescaling of that cone (psd_large_load_kernel)
   // warm start across ADMM iterations (single large cone): eigenvectors of the previous projection
   T *Vw_d = nullptr, *T_d = nullptr;
   bool warm_valid = false;
@@ -822,6 +886,7 @@ struct PsdBatch {
   ~PsdBatch() {
     cudaFree(small_d); cudaFree(lam_small_d); cudaFree(fail_d); cudaFree(A_d); cudaFree(V_d); cudaFree(cs_d);
     cudaFree(fro_d); cudaFree(thr_d); cudaFree(lam_large_d); cudaFree(rot_d); cudaFree(R_d); cudaFree(act_d); cudaFree(Vw_d); cudaFree(T_d);
+    cudaFree(mx_d); cudaFree(up_d);
     if (rot_h) cudaFreeHost(rot_h);
   }
   bool empty() const { return small_h.empty() && large_h.empty(); }
@@ -855,6 +920,8 @@ struct PsdBatch {
       ck(cudaMalloc(&thr_d, sizeof(T)), "cudaMalloc thr");
       ck(cudaMalloc(&lam_large_d, large_h.size() * sizeof(T)), "cudaMalloc lam");
       ck(cudaMalloc(&rot_d, sizeof(int)), "cudaMalloc rot");
+      ck(cudaMalloc(&mx_d, sizeof(unsigned long long)), "cudaMalloc psd max");
+      ck(cudaMalloc(&up_d, sizeof(double)), "cudaMalloc psd scale");
       {
         const char* e = getenv("COSMO_B200_PSD_WARM");
         warm_enabled = !(e && e[0] == '0');
@@ -882,6 +949,23 @@ struct PsdBatch {
   }
   void reset_warm_start() { warm_valid = false; warm_count = 0; }
 
+  // A_d = mat(ws[cone]) 2^-pe, V_d = I, fro_d = partial sums of |A_d|_F^2 (g of them), up_d = 2^pe
+  void load_large(const PsdConeDesc& d, const T* ws, cudaStream_t st, long long& launches) {
+    const int N = d.N;
+    const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
+    const long long dim = psd_cone_dim(d);
+    const int gm = (int)std::min<long long>((dim + kBlock - 1) / kBlock, kMaxGrid);
+    ck(cudaMemsetAsync(mx_d, 0, sizeof(unsigned long long), st), "memset psd max");
+    psd_cone_max_kernel<T><<<gm, kBlock, 0, st>>>(ws + d.off, dim, mx_d);
+    psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, ws, A_d, V_d, fro_d, mx_d, up_d);
+    launches += 2;
+  }
+  void unscale_large(const PsdConeDesc& d, T* s, cudaStream_t st, long long& launches) {
+    const long long dim = psd_cone_dim(d);
+    psd_unscale_kernel<T><<<(int)std::min<long long>((dim + kBlock - 1) / kBlock, kMaxGrid), kBlock, 0, st>>>(s + d.off, dim, up_d);
+    ++launches;
+  }
+
   // eigen-decompose one large cone into A_d (diagonal = eigenvalues) and V_d (block Jacobi)
   void large_eig(const PsdConeDesc& d, const T* ws, cudaStream_t st, int max_sweeps, long long& launches,
                  bool allow_warm = false) {
@@ -890,9 +974,9 @@ struct PsdBatch {
     if (Nb & 1) ++Nb;                                 // even number of blocks (zero padding decouples)
     const int npairs = Nb / 2;
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-    psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, ws, A_d, V_d, fro_d);
+    load_large(d, ws, st, launches);
     psd_large_thr_kernel<T><<<1, 32, 0, st>>>(fro_d, g, thr_d, rot_d);
-    launches += 2;
+    ++launches;
     // Warm start (ADMM iterates move slowly): rotate X into the eigenbasis of the previous projection,
     // A <- V0' X V0 is then nearly diagonal and a couple of sweeps finish the job; V starts at V0.
     // A cold start every 16th call bounds the drift of V's orthogonality.
@@ -946,9 +1030,12 @@ struct PsdBatch {
       if (tc_enabled && !sign_enabled && d.N >= tc_min_n) {
         const int N = d.N;
         const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-        psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, ws, A_d, V_d, fro_d);
-        ++launches;
-        if (tc_.project(d, A_d, fro_d, g, V_d, s, st, launches)) { ++tc_projections; continue; }
+        load_large(d, ws, st, launches);
+        if (tc_.project(d, A_d, fro_d, g, V_d, s, st, launches)) {
+          unscale_large(d, s, st, launches);
+          ++tc_projections;
+          continue;
+        }
         ++tc_fallbacks;
         if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd-tc] fallback to block Jacobi: %s\n", tc_.err.c_str());
         cudaGetLastError();
@@ -956,9 +1043,12 @@ struct PsdBatch {
       if (sign_enabled && d.triangle != 2) {   // experimental: Pi_+(X) = (X + sign(X) X) / 2 by Newton-Schulz products, no eigenvectors
         const int N = d.N;
         const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-        psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, ws, A_d, V_d, fro_d);
-        ++launches;
-        if (sign_.project(d, A_d, fro_d, g, V_d, s, st, launches)) { ++sign_projections; continue; }
+        load_large(d, ws, st, launches);
+        if (sign_.project(d, A_d, fro_d, g, V_d, s, st, launches)) {
+          unscale_large(d, s, st, launches);
+          ++sign_projections;
+          continue;
+        }
         ++sign_fallbacks;
       }
       large_eig(d, ws, st, max_sweeps, launches, /*allow_warm=*/true);
@@ -976,6 +1066,7 @@ struct PsdBatch {
       } else {
         psd_large_syrk_kernel<T><<<gt, 256, 0, st>>>(d, V_d, s);
       }
+      unscale_large(d, s, st, launches);
       ck(cudaGetLastError(), "psd large reconstruct");
       launches += 2;
     }
@@ -998,7 +1089,7 @@ struct PsdBatch {
     }
     for (size_t k = 0; k < large_h.size(); ++k) {
       large_eig(large_h[k], v, st, max_sweeps, launches);
-      psd_large_lammax_kernel<T><<<1, 32, 0, st>>>(large_h[k].N, A_d, lam_large_d + k);
+      psd_large_lammax_kernel<T><<<1, 32, 0, st>>>(large_h[k].N, A_d, up_d, lam_large_d + k);
       ++launches;
       T l;
       ck(cudaMemcpyAsync(&l, lam_large_d + k, sizeof(T), cudaMemcpyDeviceToHost, st), "copy lam");

@@ -209,9 +209,17 @@ __global__ void __launch_bounds__(256) slice_rows_kernel(const T* __restrict__ M
   mx = red[0];
   for (int w = 1; w < 8; ++w) mx = fmax(mx, red[w]);
   int e = 0;
-  if (mx > 0.0 && mx < 1.0e300) frexp(mx, &e);   // mx = f 2^e, f in [0.5, 1)  =>  |x| < 2^e
+  if (mx > 0.0 && mx <= 1.7976931348623157e308) frexp(mx, &e);   // mx = f 2^e, f in [0.5, 1)  =>  |x| < 2^e
+  // Contract: every row whose maximum is a normal number is sliced exactly as at scale 1 (same digits, scale[r] a power
+  // of two).  scale[r] = 2^(e - 6) is subnormal for e < -1016 but still exact (powers of two down to 2^-1074 are), and the
+  // epilogue forms acc * sA * sB left to right, so the product keeps its accuracy relative to |A| |B|.  Rows whose maximum
+  // is itself subnormal are sliced as if it were 2^-1022 (e = -1021): their digits have fewer significant bits, i.e. they
+  // are exact to 2^-7K * 2^-1021 in absolute terms, not relative to the row maximum.
+  e = e < -1021 ? -1021 : e;
   if (threadIdx.x == 0) scale[r] = ldexp(1.0, e - 6);
-  const double inv = ldexp(1.0, 6 - e);
+  // 2^(6 - e) as two factors: over the whole normal range each factor is a normal number, and x * inv0 * inv1 is the
+  // exact power-of-two scaling (2^(6 - e) alone overflows for e < -1017)
+  const double inv0 = ldexp(1.0, (6 - e) / 2), inv1 = ldexp(1.0, (6 - e) - (6 - e) / 2);
   int8_t* out_row = slices + (size_t)r * Np * kSlices;
   for (int c0 = threadIdx.x * 8; c0 < N; c0 += blockDim.x * 8) {
     unsigned long long u[8];
@@ -220,7 +228,7 @@ __global__ void __launch_bounds__(256) slice_rows_kernel(const T* __restrict__ M
     for (int j = 0; j < 8; ++j) {
       double x = 0.0;
       if (c0 + j < N) x = staged ? sp[j] : (double)row[c0 + j];
-      u[j] = slice_fixed<K>(x * inv);
+      u[j] = slice_fixed<K>(x * inv0 * inv1);
     }
     int8_t* dst = out_row + (size_t)(c0 >> 5) * (kSlices * 32) + (c0 & 31);
 #pragma unroll

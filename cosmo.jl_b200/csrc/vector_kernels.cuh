@@ -186,16 +186,31 @@ __global__ void __launch_bounds__(kBlock) proj_rhs_vec2_kernel(ProjRhsArgs<doubl
   }
 }
 
-// SOC norms, stage 1: one block per chunk of a cone's tail (deterministic tree).
+constexpr int kSocZeroExp = -100000;   // exponent recorded for an all-zero chunk (exact in float and double)
+
+// SOC norms, stage 1: one block per chunk of a cone's tail (deterministic tree).  The squares are summed after scaling
+// the chunk by the power of two 2^-e nearest its maximum (exact), so the sum neither overflows nor underflows anywhere in
+// the range of T; chunk_sum[2 c] = the scaled sum, chunk_sum[2 c + 1] = e.
 template <typename T>
 __global__ void __launch_bounds__(kBlock) soc_chunk_kernel(const T* __restrict__ ws, const int* __restrict__ chunk_start,
                                                            const int* __restrict__ chunk_len, T* __restrict__ chunk_sum) {
   __shared__ T sm[kWarpsPerBlock];
   const int c = blockIdx.x;
   const int start = chunk_start[c], len = chunk_len[c];
+  T mx = 0;
+  for (int i = threadIdx.x; i < len; i += blockDim.x) mx = fmax(mx, tabs(ws[start + i]));
+  for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  mx = sm[0];
+  for (int w = 1; w < kWarpsPerBlock; ++w) mx = fmax(mx, sm[w]);
+  __syncthreads();
+  // an all-zero chunk contributes nothing and must not set the common exponent of the cone: kSocZeroExp keeps it out
+  const int e = (mx == T(0)) ? kSocZeroExp : pow2_exponent(mx);
+  const T inv = (mx == T(0)) ? T(1) : (T)ldexp(1.0, -e);
   T acc = 0;
   for (int i = threadIdx.x; i < len; i += blockDim.x) {
-    const T v = ws[start + i];
+    const T v = ws[start + i] * inv;
     acc += v * v;
   }
   acc = warp_sum(acc);
@@ -204,19 +219,26 @@ __global__ void __launch_bounds__(kBlock) soc_chunk_kernel(const T* __restrict__
   if (threadIdx.x == 0) {
     T v = sm[0];
     for (int w = 1; w < kWarpsPerBlock; ++w) v += sm[w];
-    chunk_sum[c] = v;
+    chunk_sum[2 * c] = v;
+    chunk_sum[2 * c + 1] = (T)e;
   }
 }
 
-// SOC norms, stage 2: one thread per cone folds its chunks in order.
+// SOC norms, stage 2: one thread per cone folds its chunks in order, relative to the largest chunk exponent E:
+// norm = 2^E sqrt(sum_c s_c 4^(e_c - E)).
 template <typename T>
 __global__ void soc_final_kernel(const T* __restrict__ chunk_sum, const int* __restrict__ cone_chunk_ptr, int ncones,
                                  T* __restrict__ norm) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= ncones) return;
+  int E = kSocZeroExp;
+  for (int c = cone_chunk_ptr[k]; c < cone_chunk_ptr[k + 1]; ++c) E = max(E, (int)chunk_sum[2 * c + 1]);
   T v = 0;
-  for (int c = cone_chunk_ptr[k]; c < cone_chunk_ptr[k + 1]; ++c) v += chunk_sum[c];
-  norm[k] = sqrt(v);
+  for (int c = cone_chunk_ptr[k]; c < cone_chunk_ptr[k + 1]; ++c) {
+    const int ec = (int)chunk_sum[2 * c + 1];
+    if (ec != kSocZeroExp) v += chunk_sum[2 * c] * (T)ldexp(1.0, 2 * (ec - E));
+  }
+  norm[k] = (v == T(0)) ? T(0) : (T)ldexp((double)sqrt(v), E);
 }
 
 // w_x <- w_x + alpha (x_tl - w_x)              (solver.jl:63), ping-pong buffers

@@ -42,6 +42,7 @@ class OracleEngine:
         self.P, self.q = sp.csc_matrix(P), np.array(q, dtype=float)
         self.A, self.b = sp.csc_matrix(A), np.array(b, dtype=float)
         self.m, self.n = self.A.shape
+        self.dtype = np.dtype(dtype)
         self.cones = cones_from_tuples(sets)
         self.st = settings
         self.scaled = D is not None
@@ -77,7 +78,7 @@ class OracleEngine:
     def project(self, ws):
         out = np.array(ws, dtype=float).copy()
         O.project(out, self.cones)
-        return out
+        return out.astype(self.dtype)
 
     def solve(self):
         st = self.st

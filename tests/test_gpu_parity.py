@@ -12,17 +12,9 @@ from cosmo_b200 import engine as E
 from oracle import cosmo_oracle as O
 from oracle.bridge import to_oracle_cones
 from tests import golden_problems as G
+from tests.gpu_helpers import _engine, _hermitian_ws, _psd_test_matrix, _tuples
 
 pytestmark = pytest.mark.gpu
-
-
-def _tuples(sets):
-    return [cosmo_b200.model.set_tuple(S) for S in sets]
-
-
-def _engine(P, q, A, b, sets, dtype=np.float64, **kw):
-    st = cosmo_b200.Settings(**kw).to_struct()
-    return E.Engine(P, q, A, b, _tuples(sets), st, dtype=dtype)
 
 
 def _ragged_matrix(rng, m, n):
@@ -271,29 +263,6 @@ def test_tc_gemm_matches_dgemm(N, slices, groups, bound):
     assert np.array_equal(got, got.T)                                   # mirrored store: exactly symmetric
     assert abs(fr[0] - np.sum(got * got)) <= 1e-12 * np.sum(got * got)  # fused |C|_F^2
     assert abs(fr[1] - np.sum((np.eye(N) - got) ** 2)) <= 1e-12 * np.sum((np.eye(N) - got) ** 2)
-
-
-def _psd_test_matrix(kind, N, rng):
-    B = rng.standard_normal((N, N))
-    if kind == "wigner":
-        return (B + B.T) / 2
-    if kind == "rank_deficient":
-        k = max(N // 10, 2)
-        return B[:, :k] @ B[:, :k].T - B[:, k:2 * k] @ B[:, k:2 * k].T
-    if kind == "shifted":
-        return (B + B.T) / 2 + 3.0 * np.sqrt(N) * np.eye(N)
-    if kind == "zero":
-        return np.zeros((N, N))
-    if kind == "admm_like":      # w_s = s - mu / rho near a solution: PSD part, scaled negative part, a cluster near zero
-        Q, _ = np.linalg.qr(B)
-        lam = np.concatenate([np.abs(rng.standard_normal(N // 3)), -10.0 * np.abs(rng.standard_normal(N // 3)),
-                              1e-7 * rng.standard_normal(N - 2 * (N // 3))])
-        return (Q * lam) @ Q.T
-    if kind == "graded":         # eigenvalues spread over 12 orders of magnitude, both signs
-        Q, _ = np.linalg.qr(B)
-        lam = np.logspace(0, -12, N) * np.where(np.arange(N) % 2 == 0, 1.0, -1.0)
-        return (Q * lam) @ Q.T
-    raise ValueError(kind)
 
 
 @pytest.mark.parametrize("kind", ["wigner", "rank_deficient", "shifted", "zero", "admm_like", "graded"])
@@ -966,17 +935,6 @@ def test_psd_tensor_core_large_and_fallback(monkeypatch):
     st = eng.psd_stats()
     assert st["tc_projections"] == 0 and st["tc_fallbacks"] == 1, st
     assert np.linalg.norm(got - ref) / np.linalg.norm(ws) < 1e-12
-
-
-def _hermitian_ws(N, rng, kind):
-    Z = rng.standard_normal((N, N)) + 1j * rng.standard_normal((N, N))
-    H = (Z + Z.conj().T) / 2
-    if kind == "shifted":
-        H = H - 0.3 * np.sqrt(N) * np.eye(N)
-    elif kind == "low_rank_plus_noise":          # an ADMM-like iterate: a PSD part plus a small indefinite perturbation
-        Y = rng.standard_normal((N, N // 4)) + 1j * rng.standard_normal((N, N // 4))
-        H = Y @ Y.conj().T / N + 1e-3 * H
-    return O.extract_upper_triangle_complex(H, np.sqrt(2.0)), H
 
 
 @pytest.mark.parametrize("Nc,kind", [(49, "shifted"), (100, "wigner"), (100, "low_rank_plus_noise"), (193, "shifted")])

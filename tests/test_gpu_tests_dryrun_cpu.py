@@ -1,5 +1,6 @@
 """Dry run of GPU test bodies on the CPU: the CUDA engine is replaced by the oracle-backed stand-in of
-tests/oracle_engine.py and the functions of tests/test_gpu_parity.py are called directly.  What this checks is the
+tests/oracle_engine.py and the functions of tests/test_gpu_parity.py, tests/test_gpu_float32.py and
+tests/test_gpu_scale_edges.py are called directly.  What this checks is the
 Python side of those tests (imports, helpers, fixtures, the host glue they drive) -- a NameError in a GPU test would
 otherwise only show up on the next GPU run.  Assertion failures are tolerated where the stand-in legitimately differs
 from the engine (it ignores the D/E unscaling of the termination test); every other exception fails the test."""
@@ -16,9 +17,18 @@ CASES = ["test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_t
          "test_accelerated_iterates_match_oracle", "test_accelerator_rho_adaption_limits", "test_g1_simple_qp",
          "test_g2_box_statuses", "test_g3_hs21_with_soc_and_merging", "test_g14_model_updates_and_warm_start",
          "test_project_composite_matches_oracle", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
-         "test_project_psd_sign_function_path"]
+         "test_project_psd_sign_function_path",
+         "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_soc_float32",
+         "test_gpu_float32::test_project_exp_pow_cones_float32", "test_gpu_float32::test_project_psd_small_batch_float32",
+         "test_gpu_float32::test_project_psd_tensor_core_path_float32_kinds", "test_gpu_float32::test_complex_psd_float32",
+         "test_gpu_float32::test_g1_float32", "test_gpu_float32::test_g2_statuses_float32",
+         "test_gpu_float32::test_g15_g16_float32", "test_gpu_float32::test_g14_model_updates_float32",
+         "test_gpu_float32::test_closest_correlation_float32",
+         "test_gpu_scale_edges::test_homogeneity_ladder", "test_gpu_scale_edges::test_mixed_large_cone_shapes_share_the_workspace",
+         "test_gpu_scale_edges::test_small_kernel_tensor_core_boundary"]
 MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_through_the_clique_batch",
-             "test_project_exp_pow_cones", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue"}
+             "test_project_exp_pow_cones", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
+             "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_project_psd_small_batch_float32"}
 
 
 def _calls(fn):
@@ -38,8 +48,9 @@ def test_gpu_test_body_runs_against_the_oracle_stand_in(name, monkeypatch):
     monkeypatch.setattr(M._eng, "Engine", OracleEngine)
     monkeypatch.setattr(E, "Engine", OracleEngine)
     monkeypatch.setenv("COSMO_B200_TEST_EXPERIMENTAL", "1")
-    T = importlib.import_module("tests.test_gpu_parity")
-    fn = getattr(T, name)
+    module, _, func = name.rpartition("::")      # "module::test" for the other GPU modules, a bare name for the parity module
+    T = importlib.import_module("tests." + (module or "test_gpu_parity"))
+    fn = getattr(T, func)
     kwargs = _calls(fn)
     if "monkeypatch" in inspect.signature(fn).parameters:
         kwargs["monkeypatch"] = monkeypatch
