@@ -113,6 +113,158 @@ __global__ void __launch_bounds__(kBlock) aa_apply_kernel(int dim, T* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The other variants of anderson_accelerator.jl: AndersonAccelerator{T, Type2{NormalEquations} | Type1,
+// RollingMemory | RestartedMemory, NoRegularizer | TikonovRegularizer | FrobeniusNormRegularizer}.
+// Restated from the published methods (type-II: Walker & Ni 2011; type-I and its Frobenius-norm regularisation:
+// Fu, Zhang & Boyd 2020), parity with COSMOAccelerators.jl UNPINNED like the QR variant above.  With the history
+// columns X_j = x - x_last, F_j = f - f_last, G_j = g - g_last each iteration solves the l x l system
+//   Type2{NormalEquations}: M = F'F, rhs = F'f        Type1: M = X'F, rhs = X'f
+// (M + shift I) eta = rhs by LU with partial pivoting, shift = lambda (Tikonov) or lambda (|A|_F^2 + |B|_F^2) for
+// M = A'B (Frobenius), and the candidate is g - G eta.  M is kept on the device in physical column order; a new
+// column j refreshes row j and column j of M against the whole window (RollingMemory overwrites column iter mod mem).
+// ---------------------------------------------------------------------------------------------------------------
+enum { AA_GRAM_COLS = 8, AA_GRAM_NR = 3 * AA_GRAM_COLS + 2, AA_GRAM_MAX_CHUNKS = 4 };
+
+// CA.update! of the normal-equation variants: f = x - g; after a restart only (x_last, g_last, f_last) are stored;
+// otherwise G[:, j] = g - g_last, F[:, j] = f - f_last and, for Type1 (Xj != nullptr), X[:, j] = x - x_last.
+// out[0] = |f|^2 over [lo, dim) for the safeguard.
+template <typename T>
+__global__ void __launch_bounds__(kBlock) aa_hist_kernel(int dim, int lo, const T* __restrict__ g, const T* __restrict__ x,
+                                                         T* __restrict__ f, T* __restrict__ f_last, T* __restrict__ g_last,
+                                                         T* __restrict__ x_last, T* __restrict__ Gj, T* __restrict__ Fj,
+                                                         T* __restrict__ Xj, int init, RedBuf<T> rb) {
+  T accS[1] = {0};
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dim; i += gridDim.x * blockDim.x) {
+    const T gi = g[i], xi = x[i];
+    const T fi = xi - gi;
+    f[i] = fi;
+    if (!init) {
+      Gj[i] = gi - g_last[i];
+      Fj[i] = fi - f_last[i];
+      if (Xj) Xj[i] = xi - x_last[i];
+    }
+    g_last[i] = gi;
+    f_last[i] = fi;
+    if (x_last) x_last[i] = xi;
+    if (i >= lo) accS[0] += fi * fi;
+  }
+  reduce_and_finalize<T, 1, 0>(accS, (const T*)nullptr, rb, NoFin());
+}
+
+// The fused Gram + right-hand-side pass over window columns c = c0 .. c0 + ncols - 1 (ncols <= 8) of A (X for
+// Type1, F for Type2) and B = F, the new column j and f; each history column is read once:
+//   out[c] = <A_j, B_c> (row j of M),  out[8 + c] = <A_c, B_j> (column j of M, Type1 only),  out[16 + c] = <A_c, f>,
+//   out[24] = |A_j|^2,  out[25] = |B_j|^2 (Type1 only; the Frobenius regulariser).   Sums over [lo, dim).
+template <typename T, bool TYPE1>
+__global__ void __launch_bounds__(kBlock) aa_gram_kernel(int dim, int lo, const T* __restrict__ A, const T* __restrict__ B,
+                                                         size_t ld, int j, int c0, int ncols, const T* __restrict__ f,
+                                                         RedBuf<T> rb) {
+  T acc[AA_GRAM_NR];
+#pragma unroll
+  for (int k = 0; k < AA_GRAM_NR; ++k) acc[k] = T(0);
+  const T* Aj = A + (size_t)j * ld;
+  const T* Bj = B + (size_t)j * ld;
+  for (int i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < dim; i += gridDim.x * blockDim.x) {
+    const T aj = Aj[i], fi = f[i];
+    const T bj = TYPE1 ? Bj[i] : aj;
+#pragma unroll
+    for (int c = 0; c < AA_GRAM_COLS; ++c)
+      if (c < ncols) {
+        const T a = A[(size_t)(c0 + c) * ld + i];
+        const T b = TYPE1 ? B[(size_t)(c0 + c) * ld + i] : a;
+        acc[c] += aj * b;
+        if (TYPE1) acc[AA_GRAM_COLS + c] += a * bj;
+        acc[2 * AA_GRAM_COLS + c] += a * fi;
+      }
+    acc[3 * AA_GRAM_COLS] += aj * aj;
+    if (TYPE1) acc[3 * AA_GRAM_COLS + 1] += bj * bj;
+  }
+  reduce_and_finalize<T, AA_GRAM_NR, 0, NoFin, kWarpsPerBlock, AA_GRAM_NR>(acc, (const T*)nullptr, rb, NoFin());
+}
+
+// One warp (lane r owns row r, l <= 32).  Scatters the reduced Gram pass `gsc` (AA_GRAM_NR scalars per chunk of 8
+// columns) into row and column j of M (row-major, leading dimension mem) and the column norms; with `solve`, factors
+// M[0:l, 0:l] + shift I by LU with partial pivoting (first largest |pivot|), solves for eta and applies the
+// acceptance test of aa_solve_kernel: no zero or non-finite pivot, eta finite, |eta|_2 <= 1e4.  flag[0] = 1 / 0.
+// reg: 0 none, 1 Tikonov (shift = lambda), 2 Frobenius (shift = lambda sum_c (nrmA[c] + nrmB[c])).
+template <typename T>
+__global__ void __launch_bounds__(32) aa_ne_solve_kernel(const T* __restrict__ gsc, T* __restrict__ M, T* __restrict__ nrmA,
+                                                         T* __restrict__ nrmB, int mem, int j, int l, int type1, int reg,
+                                                         T lambda, int solve, T* __restrict__ eta, T* __restrict__ flag) {
+  __shared__ T S[32][33];
+  __shared__ T rhs[32];
+  const int r = threadIdx.x;
+  if (r < l) {
+    const T* o = gsc + (r / AA_GRAM_COLS) * AA_GRAM_NR;
+    const int k = r % AA_GRAM_COLS;
+    M[(size_t)j * mem + r] = o[k];
+    if (r != j) M[(size_t)r * mem + j] = type1 ? o[AA_GRAM_COLS + k] : o[k];
+    rhs[r] = o[2 * AA_GRAM_COLS + k];
+  }
+  if (r == 0) {
+    nrmA[j] = gsc[3 * AA_GRAM_COLS];
+    nrmB[j] = type1 ? gsc[3 * AA_GRAM_COLS + 1] : gsc[3 * AA_GRAM_COLS];
+  }
+  __threadfence_block();
+  __syncwarp();
+  if (!solve) return;
+  T shift = T(0);
+  if (reg == 1) shift = lambda;
+  if (reg == 2) shift = lambda * warp_sum(r < l ? nrmA[r] + nrmB[r] : T(0));
+  bool ok = true;
+  if (r < l) {
+    for (int c = 0; c < l; ++c) {
+      const T v = M[(size_t)r * mem + c] + (c == r ? shift : T(0));
+      S[r][c] = v;
+      if (!isfinite(v)) ok = false;
+    }
+    if (!isfinite(rhs[r])) ok = false;
+  }
+  ok = __all_sync(0xffffffffu, ok);
+  __syncwarp();
+  for (int k = 0; k < l && ok; ++k) {
+    T v = (r >= k && r < l) ? tabs(S[r][k]) : T(-1);
+    if (v != v) v = T(INFINITY);
+    int idx = r;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const T ov = __shfl_xor_sync(0xffffffffu, v, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+      if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+    }
+    const T piv = S[idx][k];
+    __syncwarp();   // every lane has read the pivot before the row swap below rewrites S[idx][k]
+    if (piv == T(0) || !isfinite(piv)) { ok = false; break; }
+    if (idx != k) {
+      if (r < l) { const T t = S[k][r]; S[k][r] = S[idx][r]; S[idx][r] = t; }
+      if (r == 0) { const T t = rhs[k]; rhs[k] = rhs[idx]; rhs[idx] = t; }
+    }
+    __syncwarp();
+    if (r > k && r < l) {
+      const T fct = S[r][k] / S[k][k];
+      S[r][k] = fct;
+      for (int c = k + 1; c < l; ++c) S[r][c] -= fct * S[k][c];
+      rhs[r] -= fct * rhs[k];
+    }
+    __syncwarp();
+  }
+  if (r != 0) return;
+  if (ok) {
+    for (int i = l - 1; i >= 0; --i) {
+      T v = rhs[i];
+      for (int k = i + 1; k < l; ++k) v -= S[i][k] * rhs[k];
+      rhs[i] = v / S[i][i];
+    }
+    T nrm2 = 0;
+    for (int i = 0; i < l; ++i) nrm2 += rhs[i] * rhs[i];
+    const T nrm = sqrt(nrm2);
+    if (!isfinite(nrm) || nrm > T(1e4)) ok = false;
+    for (int i = 0; i < l; ++i) eta[i] = rhs[i];
+  }
+  flag[0] = ok ? T(1) : T(0);
+}
+
 // compute_accelerated_res_norm! (accelerator_interface.jl:120-123): f = w_prev - w, out[0] = |f|^2
 template <typename T>
 __global__ void __launch_bounds__(kBlock) aa_res_kernel(int dim, int lo, const T* __restrict__ w_prev, const T* __restrict__ w,

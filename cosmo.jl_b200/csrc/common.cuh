@@ -182,12 +182,13 @@ __device__ __forceinline__ T warp_nanmax(T v) {
 // Must be called by all kBlock threads of every block of the grid.
 // `slot` / `nslots`: position of this block's partial and the number of participating blocks
 // (default: every block of the grid, indexed by blockIdx.x).
-template <typename T, int NS, int NM, typename Fin, int NWARPS = kWarpsPerBlock>
+// MAXR: slots per block the partials buffer of `rb` holds (kMaxRed for the engine's shared buffer).
+template <typename T, int NS, int NM, typename Fin, int NWARPS = kWarpsPerBlock, int MAXR = kMaxRed>
 __device__ __forceinline__ void reduce_and_finalize(const T* accS, const T* accM, const RedBuf<T>& rb,
                                                     const Fin& fin, int slot = -1, int nslots = -1) {
   if (slot < 0) { slot = blockIdx.x; nslots = gridDim.x; }
   constexpr int NR = NS + NM;
-  static_assert(NR >= 1 && NR <= kMaxRed, "reduction slots");
+  static_assert(NR >= 1 && NR <= MAXR, "reduction slots");
   __shared__ T sm[NWARPS][NR];
   __shared__ int is_last;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

@@ -206,6 +206,8 @@ class EngineBase {
   virtual void comm_init(int nranks, int rank, const void* id128) = 0;
   virtual void p2p_export(void* blob128) = 0;
   virtual void p2p_attach(const void* blobs, int nranks) = 0;
+  virtual void set_accelerator(const cosmo_b200_accelerator* acc) = 0;
+  virtual void accelerator_stats(int64_t* out6) = 0;
 };
 
 template <typename T>
@@ -235,6 +237,8 @@ class Engine : public EngineBase {
   void comm_init(int nranks, int rank, const void* id128) override;
   void p2p_export(void* blob128) override;
   void p2p_attach(const void* blobs, int nranks) override;
+  void set_accelerator(const cosmo_b200_accelerator* acc) override;
+  void accelerator_stats(int64_t* out6) override;
 
  private:
   // ---- problem ----
@@ -275,10 +279,21 @@ class Engine : public EngineBase {
   int aa_iter_ = 0;            // columns filled since the last restart
   bool aa_init_ = true, aa_success_ = false, aa_active_ = false;
   long long aa_accelerated_ = 0, aa_declined_ = 0;
+  // variant and activation reason (cosmo_b200_set_accelerator); the default runs aa_update / aa_accelerate above
+  cosmo_b200_accelerator acc_{COSMO_B200_AA_TYPE2_QR, COSMO_B200_AA_RESTARTED_MEMORY, COSMO_B200_AA_NO_REGULARIZER,
+                              COSMO_B200_AA_IMMEDIATE, 0.0, 2, 0.0};
+  long long aa_rejected_ = 0, aa_rho_restarts_ = 0, aa_mem_restarts_ = 0, aa_activated_at_ = 0;
+  // normal-equation variants: F is stored in aaQ_, M in aaR_ (row-major, leading dimension aa_mem_)
+  DevBuf<T> aaX_, aa_xlast_, aa_nrm_, aa_gsc_, aa_gpart_;
+  int aa_j_ = 0;               // column written by the last aa_update_ne
+  bool aa_fresh_ = false;      // aa_update_ne wrote a column that aa_accelerate_ne has not used yet
+  bool aa_ne() const { return acc_.type != COSMO_B200_AA_TYPE2_QR; }
   void aa_prepare();
-  void aa_restart() { aa_iter_ = 0; aa_init_ = true; }
+  void aa_restart() { aa_iter_ = 0; aa_init_ = true; aa_fresh_ = false; }
   void aa_update(const T* g, const T* x);
   bool aa_accelerate(T* g);
+  void aa_update_ne(const T* g, const T* x);
+  bool aa_accelerate_ne(T* g);
   // ---- state ----
   DevBuf<T> W_[2];           // operator variable, ping-pong (w / w_prev)
   int cur_ = 0, prev_ = 1;
@@ -1659,9 +1674,21 @@ void Engine<T>::aa_prepare() {   // _make_accelerator!, setup.jl:10-14 (built on
     if (!h_aa_) CUDA_TRY(cudaMallocHost(&h_aa_, AA_SC_COUNT * sizeof(T)));
     aa_mem_ = mem;
   }
+  if (aa_ne()) {
+    if (aa_gsc_.n == 0) {
+      aa_gsc_.alloc((size_t)AA_GRAM_MAX_CHUNKS * AA_GRAM_NR);
+      aa_gpart_.alloc((size_t)kMaxGrid * AA_GRAM_NR);
+      aa_nrm_.alloc(64);
+    }
+    if (acc_.type == COSMO_B200_AA_TYPE1) {
+      if (aa_xlast_.n != (size_t)dim) aa_xlast_.alloc(dim);
+      if (aaX_.n != (size_t)dim * mem) aaX_.alloc((size_t)dim * mem, false);
+    }
+  }
   aa_restart();               // setup.jl:47-49
   aa_active_ = false; aa_success_ = false;
   aa_accelerated_ = aa_declined_ = 0;
+  aa_rejected_ = aa_rho_restarts_ = aa_mem_restarts_ = aa_activated_at_ = 0;
 }
 
 // CA.update!(aa, g = w, x = w_prev): history columns + QR update by modified Gram-Schmidt
@@ -1678,7 +1705,7 @@ void Engine<T>::aa_update(const T* g, const T* x) {
     return;
   }
   int j = aa_iter_ % aa_mem_;
-  if (j == 0 && aa_iter_ != 0) aa_iter_ = 0;   // RestartedMemory: the history is full, start again
+  if (j == 0 && aa_iter_ != 0) { aa_iter_ = 0; ++aa_mem_restarts_; }   // RestartedMemory: the history is full, start again
   T* Gj = aaG_.p + (size_t)j * dim;
   T* q = aaQ_.p + (size_t)j * dim;
   aa_update_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, Gj, q, 0,
@@ -1718,7 +1745,95 @@ bool Engine<T>::aa_accelerate(T* g) {
   check_launch("aa_apply");
   CUDA_TRY(cudaMemcpyAsync(h_aa_ + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
   sync();
-  return h_aa_[AA_FLAG] != T(0);
+  if (h_aa_[AA_FLAG] == T(0)) { ++aa_rejected_; return false; }
+  return true;
+}
+
+// CA.update! of the normal-equation variants (aa.cuh): history columns only; M follows in aa_accelerate_ne
+template <typename T>
+void Engine<T>::aa_update_ne(const T* g, const T* x) {
+  const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
+  const int grid = vgrid(dim);
+  const bool type1 = acc_.type == COSMO_B200_AA_TYPE1;
+  T* xl = type1 ? aa_xlast_.p : nullptr;
+  if (aa_init_) {
+    aa_hist_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, xl, (T*)nullptr,
+                                                    (T*)nullptr, (T*)nullptr, 1, red_ptr(aa_sc_.p + AA_F2));
+    check_launch("aa_hist");
+    allreduce_sum(aa_sc_.p + AA_F2, 1);
+    aa_init_ = false;
+    aa_fresh_ = false;
+    return;
+  }
+  const int j = aa_iter_ % aa_mem_;
+  if (acc_.memory == COSMO_B200_AA_RESTARTED_MEMORY && j == 0 && aa_iter_ != 0) { aa_iter_ = 0; ++aa_mem_restarts_; }
+  aa_hist_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, xl,
+                                                  aaG_.p + (size_t)j * dim, aaQ_.p + (size_t)j * dim,
+                                                  type1 ? aaX_.p + (size_t)j * dim : nullptr, 0, red_ptr(aa_sc_.p + AA_F2));
+  check_launch("aa_hist");
+  allreduce_sum(aa_sc_.p + AA_F2, 1);
+  aa_j_ = j;
+  ++aa_iter_;
+  if (aa_iter_ >= 2 * aa_mem_) aa_iter_ -= aa_mem_;   // RollingMemory: keeps iter mod mem and min(iter, mem)
+  aa_fresh_ = true;
+}
+
+// CA.accelerate! of the normal-equation variants: one fused Gram + rhs pass (ceil(l/8) launches, one allreduce), the
+// one-warp LU solve, then the candidate through aa_apply_kernel
+template <typename T>
+bool Engine<T>::aa_accelerate_ne(T* g) {
+  if (!aa_fresh_) return false;
+  aa_fresh_ = false;
+  const int l = std::min(aa_iter_, aa_mem_);
+  const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
+  const int grid = vgrid(dim);
+  const bool type1 = acc_.type == COSMO_B200_AA_TYPE1;
+  const int nch = (l + AA_GRAM_COLS - 1) / AA_GRAM_COLS;
+  for (int ch = 0; ch < nch; ++ch) {
+    const int c0 = ch * AA_GRAM_COLS, nc = std::min((int)AA_GRAM_COLS, l - c0);
+    RedBuf<T> rb{aa_gpart_.p, aa_gsc_.p + (size_t)ch * AA_GRAM_NR, ticket_.p};
+    if (type1)
+      aa_gram_kernel<T, true><<<grid, kBlock, 0, stream_>>>(dim, lo, aaX_.p, aaQ_.p, (size_t)dim, aa_j_, c0, nc, aa_f_.p, rb);
+    else
+      aa_gram_kernel<T, false><<<grid, kBlock, 0, stream_>>>(dim, lo, aaQ_.p, aaQ_.p, (size_t)dim, aa_j_, c0, nc, aa_f_.p, rb);
+    check_launch("aa_gram");
+  }
+  allreduce_sum(aa_gsc_.p, (size_t)nch * AA_GRAM_NR);
+  const bool solve = l >= std::max(st_.accelerator_min_mem, 1);
+  aa_ne_solve_kernel<T><<<1, 32, 0, stream_>>>(aa_gsc_.p, aaR_.p, aa_nrm_.p, aa_nrm_.p + aa_mem_, aa_mem_, aa_j_, l, type1 ? 1 : 0,
+                                               acc_.regularizer, (T)acc_.lambda, solve ? 1 : 0, aa_eta_.p, aa_sc_.p + AA_FLAG);
+  check_launch("aa_ne_solve");
+  if (!solve) return false;
+  aa_apply_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, g, aaG_.p, (size_t)dim, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
+  check_launch("aa_apply");
+  CUDA_TRY(cudaMemcpyAsync(h_aa_ + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  if (h_aa_[AA_FLAG] == T(0)) { ++aa_rejected_; return false; }
+  return true;
+}
+
+template <typename T>
+void Engine<T>::set_accelerator(const cosmo_b200_accelerator* a) {
+  if (!a) {
+    acc_ = cosmo_b200_accelerator{COSMO_B200_AA_TYPE2_QR, COSMO_B200_AA_RESTARTED_MEMORY, COSMO_B200_AA_NO_REGULARIZER,
+                                  COSMO_B200_AA_IMMEDIATE, 0.0, 2, 0.0};
+    return;
+  }
+  if (a->type < COSMO_B200_AA_TYPE2_QR || a->type > COSMO_B200_AA_TYPE1 || a->memory < 0 || a->memory > 1 ||
+      a->regularizer < 0 || a->regularizer > 2 || a->activation < 0 || a->activation > 2)
+    throw EngineError{COSMO_B200_ERR_INVALID, "accelerator: unknown type, memory, regularizer or activation"};
+  if (!(a->lambda >= 0.0)) throw EngineError{COSMO_B200_ERR_INVALID, "accelerator: lambda must be a non-negative number"};
+  if (a->type == COSMO_B200_AA_TYPE2_QR && a->memory == COSMO_B200_AA_ROLLING_MEMORY)
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "accelerator: Type2{QRDecomp} with RollingMemory is not supported"};
+  if (a->type == COSMO_B200_AA_TYPE2_QR && a->regularizer != COSMO_B200_AA_NO_REGULARIZER)
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "accelerator: Type2{QRDecomp} takes no regularizer"};
+  acc_ = *a;
+}
+
+template <typename T>
+void Engine<T>::accelerator_stats(int64_t* out) {
+  out[0] = aa_accelerated_; out[1] = aa_declined_; out[2] = aa_rejected_;
+  out[3] = aa_rho_restarts_; out[4] = aa_mem_restarts_; out[5] = aa_activated_at_;
 }
 
 // ---------------------------------------------------------------------------
@@ -1796,12 +1911,21 @@ void Engine<T>::solve(cosmo_b200_result* out) {
 
   while (iter + safeguarding_iter < st_.max_iter) {
     ++iter;
-    // acceleration_pre! (accelerator_interface.jl:58-75), ImmediateActivation (:24-28)
+    // acceleration_pre! (accelerator_interface.jl:58-75), ImmediateActivation / IterActivation (:24-33)
     if (use_aa) {
-      if (!aa_active_ && iter >= 2) aa_active_ = true;
+      if (!aa_active_ && ((acc_.activation == COSMO_B200_AA_IMMEDIATE && iter >= 2) ||
+                          (acc_.activation == COSMO_B200_AA_ITER && iter >= acc_.start_iter))) {
+        aa_active_ = true;
+        aa_activated_at_ = iter;
+      }
       if (aa_active_) {
-        aa_update(W_[cur_].p, W_[prev_].p);
-        aa_success_ = aa_accelerate(W_[cur_].p);   // overwrites w with the candidate
+        if (aa_ne()) {
+          aa_update_ne(W_[cur_].p, W_[prev_].p);
+          aa_success_ = aa_accelerate_ne(W_[cur_].p);
+        } else {
+          aa_update(W_[cur_].p, W_[prev_].p);
+          aa_success_ = aa_accelerate(W_[cur_].p);   // overwrites w with the candidate
+        }
         if (aa_success_) ++aa_accelerated_;
       }
     }
@@ -1835,7 +1959,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
       const bool adapted = adapt_rho(W_[src].p);
       res_time += now_s() - t0;
       if (adapted) {
-        if (use_aa) aa_restart();   // the operator changed: CA.restart! (solver.jl:272-275)
+        if (use_aa) { aa_restart(); ++aa_rho_restarts_; }   // the operator changed: CA.restart! (solver.jl:272-275)
         // w[n+1:end] = mu ./ rho + s (solver.jl:278), kept apart from w_prev
         ws_from_mu_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, rho_vec_.p, mu_.p, s_.p, W_[dst].p + n);
         check_launch("ws_from_mu");
@@ -1873,6 +1997,14 @@ void Engine<T>::solve(cosmo_b200_result* out) {
       res_time += now_s() - t0;
       cost = info[4];
       if (fabs(cost) > 1e20) { status = COSMO_B200_UNSOLVED; break; }
+      // AccuracyActivation (accelerator_interface.jl:38-46), checked first thing in has_converged (residuals.jl:129)
+      if (use_aa && !aa_active_ && acc_.activation == COSMO_B200_AA_ACCURACY) {
+        const double tol = acc_.start_accuracy;
+        if (info[0] < tol + tol * info[2] && info[1] < tol + tol * info[3]) {
+          aa_active_ = true;
+          aa_activated_at_ = iter;
+        }
+      }
       if (st_.verbose & 1) printf("%lld\t%.4e\t%.4e\t%.4e\t%.4e\n", iter, cost, info[0], info[1], rho_);
       // has_converged (residuals.jl:127-140): a known optimal value, when given, must be met as well
       const bool obj_ok = (st_.obj_true != st_.obj_true) || fabs(st_.obj_true - cost) <= st_.obj_true_tol;
@@ -2159,6 +2291,13 @@ int cosmo_b200_get_w(cosmo_b200_handle* h, void* out) {
 int cosmo_b200_psd_stats(cosmo_b200_handle* h, int64_t out[8]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->psd_stats(out));
+}
+int cosmo_b200_set_accelerator(cosmo_b200_handle* h, const cosmo_b200_accelerator* acc) {
+  ABI_GUARD(h, h->impl->set_accelerator(acc));
+}
+int cosmo_b200_accelerator_stats(cosmo_b200_handle* h, int64_t out[6]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->accelerator_stats(out));
 }
 int cosmo_b200_get_scaling(cosmo_b200_handle* h, void* D, void* E, double* c) {
   ABI_GUARD(h, h->impl->get_scaling(D, E, c));

@@ -23,6 +23,10 @@ STATUS = {0: "Undetermined", 1: "Solved", 2: "Max_iter_reached", 3: "Time_limit_
           4: "Primal_infeasible", 5: "Dual_infeasible", 6: "Unsolved"}
 KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES = 0, 1, 2
 ACC_EMPTY, ACC_ANDERSON = 0, 1
+AA_TYPE2_QR, AA_TYPE2_NORMAL, AA_TYPE1 = 0, 1, 2
+AA_RESTARTED_MEMORY, AA_ROLLING_MEMORY = 0, 1
+AA_NO_REGULARIZER, AA_TIKONOV, AA_FROBENIUS = 0, 1, 2
+AA_IMMEDIATE, AA_ITER, AA_ACCURACY = 0, 1, 2
 
 
 class EngineError(RuntimeError):
@@ -80,6 +84,11 @@ class ResultStruct(C.Structure):
                 ("kernel_launches", C.c_int64)]
 
 
+class AcceleratorStruct(C.Structure):
+    _fields_ = [("type", C.c_int32), ("memory", C.c_int32), ("regularizer", C.c_int32), ("activation", C.c_int32),
+                ("lambda_", C.c_double), ("start_iter", C.c_int64), ("start_accuracy", C.c_double)]
+
+
 EXPORTS = [
     "cosmo_b200_abi_version", "cosmo_b200_default_settings", "cosmo_b200_create", "cosmo_b200_destroy",
     "cosmo_b200_last_error", "cosmo_b200_update_settings", "cosmo_b200_warm_start", "cosmo_b200_update_qb",
@@ -87,6 +96,7 @@ EXPORTS = [
     "cosmo_b200_residuals", "cosmo_b200_spmv", "cosmo_b200_spmv_bench", "cosmo_b200_get_rho_vec", "cosmo_b200_get_w",
     "cosmo_b200_comm_unique_id", "cosmo_b200_comm_init", "cosmo_b200_comm_p2p_export", "cosmo_b200_comm_p2p_attach",
     "cosmo_b200_tc_gemm_test", "cosmo_b200_psd_stats", "cosmo_b200_get_scaling",
+    "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats",
 ]
 
 _lib = None
@@ -134,6 +144,8 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_comm_p2p_attach.argtypes = [vp, vp, C.c_int32]
     lib.cosmo_b200_psd_stats.argtypes = [vp, C.POINTER(C.c_int64)]
     lib.cosmo_b200_get_scaling.argtypes = [vp, vp, vp, C.POINTER(C.c_double)]
+    lib.cosmo_b200_set_accelerator.argtypes = [vp, C.POINTER(AcceleratorStruct)]
+    lib.cosmo_b200_accelerator_stats.argtypes = [vp, C.POINTER(C.c_int64)]
     lib.cosmo_b200_tc_gemm_test.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32,
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]
     for name in EXPORTS:
@@ -291,6 +303,10 @@ class Engine:
     def reset(self):
         self._check(self._lib.cosmo_b200_reset(self._h))
 
+    def set_accelerator(self, acc: Optional[AcceleratorStruct]):
+        """cosmo_b200_set_accelerator: the Anderson variant and activation reason (None: the default)."""
+        self._check(self._lib.cosmo_b200_set_accelerator(self._h, None if acc is None else C.byref(acc)))
+
     def comm_init(self, nranks, rank, unique_id: Optional[bytes]):
         buf = C.create_string_buffer(unique_id, 128) if unique_id is not None else None
         self._check(self._lib.cosmo_b200_comm_init(self._h, nranks, rank, C.cast(buf, C.c_void_p) if buf else None))
@@ -389,6 +405,15 @@ class Engine:
         keys = ("tc_projections", "tc_fallbacks", "tc_last_steps", "tc_last_checks", "sign_projections", "sign_fallbacks",
                 "jacobi_last_sweeps", "tc_slices")
         return dict(zip(keys, [int(v) for v in out]))
+
+    def accelerator_stats(self):
+        """Accelerator events of the last solve (cosmo_b200_accelerator_stats), keyed by ACCELERATOR_STATS."""
+        out = (C.c_int64 * 6)()
+        self._check(self._lib.cosmo_b200_accelerator_stats(self._h, out))
+        return dict(zip(ACCELERATOR_STATS, [int(v) for v in out]))
+
+
+ACCELERATOR_STATS = ("accepted", "declined", "rejected", "rho_restarts", "memory_restarts", "activated_at")
 
 
 def tc_gemm(A, B, slices=8, groups=0, reps=0):

@@ -15,7 +15,7 @@ from __future__ import annotations
 import math
 import time
 from dataclasses import dataclass, field
-from typing import List, Optional, Sequence, Union
+from typing import List, Optional, Sequence, Tuple, Union
 
 import os
 
@@ -247,11 +247,18 @@ class Settings:
     tol_constant: float = 1.0
     tol_exponent: float = 1.5
     psd_max_sweeps: int = 30
-    # "EmptyAccelerator" | "AndersonAccelerator" (= AndersonAccelerator{T, Type2{QRDecomp}, RestartedMemory,
-    # NoRegularizer} with ImmediateActivation, the reference's default family, settings.jl:136-138)
+    # "EmptyAccelerator" | "AndersonAccelerator" (settings.jl:136-138).  The AndersonAccelerator{T, type, memory,
+    # regularizer} parameters and the activation reason (accelerator_interface.jl:1-48) follow; the defaults give the
+    # reference's default AndersonAccelerator{T, Type2{QRDecomp}, RestartedMemory, NoRegularizer}, ImmediateActivation.
     accelerator: str = "EmptyAccelerator"
     accelerator_mem: int = 15
     accelerator_min_mem: int = 3
+    accelerator_type: str = "Type2{QRDecomp}"             # | "Type2{NormalEquations}" | "Type1"
+    accelerator_memory: str = "RestartedMemory"           # | "RollingMemory"
+    accelerator_regularizer: str = "NoRegularizer"        # | "TikonovRegularizer" | "FrobeniusNormRegularizer"
+    accelerator_lambda: float = 1e-8                      # regulariser weight
+    accelerator_activation: Union[str, Tuple[str, float]] = "ImmediateActivation"   # | ("IterActivation", k) |
+    #                                                                                   ("AccuracyActivation", tol)
     safeguard: bool = True
     safeguard_tol: float = 2.0
     # chordal decomposition of PsdConeTriangle constraints (settings.jl:50-53,129-135; host side, chordal.py).
@@ -263,6 +270,41 @@ class Settings:
 
     _KKT = {"CGIndirectKKTSolver": _eng.KKT_CG, "MINRESIndirectKKTSolver": _eng.KKT_MINRES,
             "IndirectReducedKKTSolver:MINRES": _eng.KKT_MINRES_REDUCED}
+    _AA_TYPE = {"Type2{QRDecomp}": _eng.AA_TYPE2_QR, "Type2{NormalEquations}": _eng.AA_TYPE2_NORMAL, "Type1": _eng.AA_TYPE1}
+    _AA_MEMORY = {"RestartedMemory": _eng.AA_RESTARTED_MEMORY, "RollingMemory": _eng.AA_ROLLING_MEMORY}
+    _AA_REG = {"NoRegularizer": _eng.AA_NO_REGULARIZER, "TikonovRegularizer": _eng.AA_TIKONOV,
+               "FrobeniusNormRegularizer": _eng.AA_FROBENIUS}
+
+    def accelerator_struct(self) -> Optional["_eng.AcceleratorStruct"]:
+        """The cosmo_b200_accelerator of these settings; None for the default variant (nothing to set).  Validates the
+        combination: Type2{QRDecomp} with RollingMemory or a regulariser -> ERR_UNSUPPORTED, lambda < 0 -> ERR_INVALID."""
+        for value, table, what in ((self.accelerator_type, self._AA_TYPE, "type"),
+                                   (self.accelerator_memory, self._AA_MEMORY, "memory"),
+                                   (self.accelerator_regularizer, self._AA_REG, "regularizer")):
+            if value not in table:
+                raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "accelerator %s %r is not an AndersonAccelerator parameter" % (what, value))
+        act = self.accelerator_activation
+        kind, arg = (act, None) if isinstance(act, str) else (tuple(act) if len(act) == 2 else (None, None))
+        if kind not in ("ImmediateActivation", "IterActivation", "AccuracyActivation") or (kind == "ImmediateActivation") != (arg is None):
+            raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "accelerator_activation %r is not an activation reason" % (act,))
+        if not self.accelerator_lambda >= 0:
+            raise _eng.EngineError(_eng.ERR_INVALID, "accelerator_lambda must be a non-negative number")
+        a = _eng.AcceleratorStruct()
+        a.type = self._AA_TYPE[self.accelerator_type]
+        a.memory = self._AA_MEMORY[self.accelerator_memory]
+        a.regularizer = self._AA_REG[self.accelerator_regularizer]
+        a.lambda_ = float(self.accelerator_lambda)
+        a.activation = {"ImmediateActivation": _eng.AA_IMMEDIATE, "IterActivation": _eng.AA_ITER,
+                        "AccuracyActivation": _eng.AA_ACCURACY}[kind]
+        a.start_iter = int(arg) if kind == "IterActivation" else 2
+        a.start_accuracy = float(arg) if kind == "AccuracyActivation" else 0.0
+        if a.type == _eng.AA_TYPE2_QR and a.memory != _eng.AA_RESTARTED_MEMORY:
+            raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "Type2{QRDecomp} with RollingMemory is not supported (no QR downdate)")
+        if a.type == _eng.AA_TYPE2_QR and a.regularizer != _eng.AA_NO_REGULARIZER:
+            raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "Type2{QRDecomp} takes no regularizer")
+        if a.type == _eng.AA_TYPE2_QR and a.activation == _eng.AA_IMMEDIATE:
+            return None
+        return a
 
     def to_struct(self) -> "_eng.SettingsStruct":
         if self.kkt_solver not in self._KKT:
@@ -271,9 +313,10 @@ class Settings:
                                    "CGIndirectKKTSolver / MINRESIndirectKKTSolver" % self.kkt_solver)
         if self.accelerator not in ("EmptyAccelerator", "AndersonAccelerator"):
             raise _eng.EngineError(_eng.ERR_UNSUPPORTED,
-                                   "accelerator %r: the engine implements EmptyAccelerator and AndersonAccelerator"
-                                   "{T, Type2{QRDecomp}, RestartedMemory, NoRegularizer}" % self.accelerator)
+                                   "accelerator %r: the engine implements EmptyAccelerator and AndersonAccelerator "
+                                   "(variant in accelerator_type / _memory / _regularizer)" % self.accelerator)
         if self.accelerator == "AndersonAccelerator":
+            self.accelerator_struct()
             if self.accelerator_mem <= 2:
                 raise ValueError("Memory has to be bigger than two.")      # AndersonAccelerator ctor (DomainError)
             if self.accelerator_mem > 32:
@@ -551,6 +594,7 @@ class Model:
             self.D, self.E, self.c = D, E, c
         else:
             self.engine.update_settings(st.to_struct())
+        configure_accelerator(self.engine, st)
         # scale_variables! (scaling.jl:118-123)
         if self._dec is not None:
             # The decomposed problem keeps its own iterates between solves.  A warm start given in the ORIGINAL
@@ -597,6 +641,15 @@ class Model:
         if self.engine is not None:
             self.engine.close()
         self.__init__(self.dtype, self.device)
+
+
+def configure_accelerator(engine, st: Settings):
+    """Hand the Anderson variant of `st` to the engine (_make_accelerator!, setup.jl:10-14).  An engine that never ran
+    a non-default variant is left alone; one that did is reset to the default."""
+    acc = st.accelerator_struct() if st.accelerator == "AndersonAccelerator" else None
+    if acc is not None or getattr(engine, "_custom_accelerator", False):
+        engine.set_accelerator(acc)
+        engine._custom_accelerator = acc is not None
 
 
 def assemble(model: Model, P, q, constraints, settings: Optional[Settings] = None, x0=None, y0=None):

@@ -110,6 +110,7 @@ def create_engine(shard: Shard, settings: M.Settings, device: int = 0, dist=None
     tuples = [M.set_tuple(S) for S in shard.sets]
     eng = _eng.Engine(shard.P, shard.q, shard.A, shard.b, tuples, settings.to_struct(), D=D,
                       E=None if E is None else np.asarray(E)[shard.rows], c=c, dtype=dtype, device=device)
+    M.configure_accelerator(eng, settings)
     if shard.world > 1:
         if dist is None:
             raise _eng.EngineError(_eng.ERR_INVALID, "world > 1 needs an initialised torch.distributed module")

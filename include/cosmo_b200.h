@@ -89,6 +89,24 @@ enum {
 /* accelerators (COSMOAccelerators.jl types selectable through settings.accelerator) */
 enum { COSMO_B200_ACC_EMPTY = 0, COSMO_B200_ACC_ANDERSON = 1 };
 
+/* AndersonAccelerator{T, type, memory, regularizer} parameters and the activation reason (accelerator_interface.jl:1-48) */
+enum { COSMO_B200_AA_TYPE2_QR = 0, COSMO_B200_AA_TYPE2_NORMAL = 1, COSMO_B200_AA_TYPE1 = 2 };
+enum { COSMO_B200_AA_RESTARTED_MEMORY = 0, COSMO_B200_AA_ROLLING_MEMORY = 1 };
+enum { COSMO_B200_AA_NO_REGULARIZER = 0, COSMO_B200_AA_TIKONOV = 1, COSMO_B200_AA_FROBENIUS = 2 };
+enum { COSMO_B200_AA_IMMEDIATE = 0, COSMO_B200_AA_ITER = 1, COSMO_B200_AA_ACCURACY = 2 };
+
+/* ws.accelerator's type parameters and ws.activation_reason (settings.jl:96-98,136-138) */
+typedef struct {
+  int32_t type;          /* COSMO_B200_AA_TYPE2_QR | _TYPE2_NORMAL (Type2{NormalEquations}) | _TYPE1 */
+  int32_t memory;        /* COSMO_B200_AA_RESTARTED_MEMORY | _ROLLING_MEMORY (not with TYPE2_QR) */
+  int32_t regularizer;   /* COSMO_B200_AA_NO_REGULARIZER | _TIKONOV | _FROBENIUS (not with TYPE2_QR) */
+  int32_t activation;    /* COSMO_B200_AA_IMMEDIATE | _ITER (IterActivation) | _ACCURACY (AccuracyActivation) */
+  double lambda;         /* regulariser weight (>= 0; 1e-8 is the value the Julia shim passes by default) */
+  int64_t start_iter;    /* IterActivation: active once iter >= start_iter */
+  double start_accuracy; /* AccuracyActivation: active after the first termination check with r_prim < tol + tol
+                            max_norm_prim and r_dual < tol + tol max_norm_dual */
+} cosmo_b200_accelerator;
+
 /* KKT plugins (src/linear_solver/kktsolver_indirect.jl:173-189) */
 enum {
   COSMO_B200_KKT_CG = 0,             /* CGIndirectKKTSolver      (reduced system, CG)      :3-88   */
@@ -159,7 +177,7 @@ typedef struct {
   int32_t psd_max_sweeps;            /* Jacobi eigensolver sweep cap (engine-specific) */
   /* accelerator (settings.jl:96-98,136-138; accelerator_interface.jl:58-114) */
   int32_t accelerator;         /* COSMO_B200_ACC_EMPTY | COSMO_B200_ACC_ANDERSON (Type2{QRDecomp}, RestartedMemory,
-                                  NoRegularizer, ImmediateActivation) */
+                                  NoRegularizer, ImmediateActivation unless cosmo_b200_set_accelerator chose another) */
   int32_t accelerator_mem;     /* history length `mem` (reference default 15) */
   int32_t accelerator_min_mem; /* columns needed before a candidate is formed (package default 3) */
   int32_t safeguard;           /* settings.safeguard */
@@ -231,6 +249,17 @@ int cosmo_b200_update_qb(cosmo_b200_handle* h, const void* q, const void* b);
 int cosmo_b200_update_rho(cosmo_b200_handle* h, const void* rho_vec, double rho);
 /* empty_model!-like reset of iterates, rho, CG warm start and call counter */
 int cosmo_b200_reset(cosmo_b200_handle* h);
+/* _make_accelerator! (setup.jl:10-14) for settings.accelerator = AndersonAccelerator{T, type, memory, regularizer} with
+   activation_reason (accelerator_interface.jl:1-48); read when settings.accelerator == COSMO_B200_ACC_ANDERSON and kept
+   across update_settings.  NULL restores the default (Type2{QRDecomp}, RestartedMemory, NoRegularizer,
+   ImmediateActivation).  TYPE2_QR with rolling memory or a regulariser: COSMO_B200_ERR_UNSUPPORTED; lambda < 0 or an
+   unknown enum: COSMO_B200_ERR_INVALID. */
+int cosmo_b200_set_accelerator(cosmo_b200_handle* h, const cosmo_b200_accelerator* acc);
+/* what the reference logs in accelerator.acceleration_status (accelerator_interface.jl:95-111, solver.jl:272-275)
+   for the last solve: out = {accepted candidates (num_accelerated_steps), safeguard declines, rejected solves
+   (singular, non-finite or |eta| > 1e4), restarts after a rho adaptation, memory restarts, iteration at which the
+   accelerator became active (0: never)} */
+int cosmo_b200_accelerator_stats(cosmo_b200_handle* h, int64_t out[6]);
 
 /* ---- the hot loop (solver.jl:125-167) ------------------------------------ */
 int cosmo_b200_solve(cosmo_b200_handle* h, cosmo_b200_result* out);
