@@ -208,6 +208,8 @@ class EngineBase {
   virtual void p2p_attach(const void* blobs, int nranks) = 0;
   virtual void set_accelerator(const cosmo_b200_accelerator* acc) = 0;
   virtual void accelerator_stats(int64_t* out6) = 0;
+  virtual void infeasibility_test(int which, const void* delta, double* out8) = 0;
+  virtual void psd_lambda_max(const void* v, double* lam) = 0;
 };
 
 template <typename T>
@@ -239,6 +241,8 @@ class Engine : public EngineBase {
   void p2p_attach(const void* blobs, int nranks) override;
   void set_accelerator(const cosmo_b200_accelerator* acc) override;
   void accelerator_stats(int64_t* out6) override;
+  void infeasibility_test(int which, const void* delta, double* out8) override;
+  void psd_lambda_max(const void* v, double* lam) override;
 
  private:
   // ---- problem ----
@@ -397,6 +401,7 @@ class Engine : public EngineBase {
   bool adapt_rho(const T* x);
   bool primal_infeasible();
   bool dual_infeasible();
+  double inf_rec_[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // what the last primal_infeasible / dual_infeasible computed
   void recover_mu(const T* w_prev) {
     recover_mu_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_vec_.p, w_prev + n_, s_.p, mu_.p);
     check_launch("recover_mu");
@@ -1556,22 +1561,32 @@ bool Engine<T>::adapt_rho(const T* x) {
   return false;
 }
 
-// is_primal_infeasible! (infeasibility.jl:1-29); dy_ holds delta_y
+// is_primal_infeasible! (infeasibility.jl:1-29); dy_ holds delta_y.  inf_rec_ records what the test computed
+// (cosmo_b200_infeasibility_test): {verdict, last gate reached (1: norm, 2: A'dy, 4: cone tests), |E dy|_inf,
+// |Dinv A'dy|_inf, dy'b (of the normalized -dy / |E dy|_inf), Box support sum, failed families (rows 1, SOC 2, PSD 4,
+// Exp/Pow 8), PSD cones whose eigensolver missed psd_max_sweeps}
 template <typename T>
 bool Engine<T>::primal_infeasible() {
   const T eps = (T)st_.eps_prim_inf;
+  double* rec = inf_rec_;
+  for (int k = 0; k < 8; ++k) rec[k] = (k == 0 || k >= 6) ? 0.0 : NAN;
+  rec[1] = 1;
   scaled_norminf_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, scaled_ ? E_.p : nullptr, dy_.p, red(SC_TMP0));
   check_launch("norminf_dy");
   allreduce_max(sc_.p + SC_TMP0, 1);
   read_scalars(SC_TMP0, 1);
   const double norm_dy = (double)h_sc_[SC_TMP0];
+  rec[2] = norm_dy;
   if (!(norm_dy > st_.eps_prim_inf)) return false;
+  rec[1] = 2;
   launch_spmv(At_, dy_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n_, EpiStore<T>{nullptr, vec_n_.p}, red(SC_TMP0), "spmv_At_dy");
   allreduce_sum(vec_n_.p, n_);
   scaled_norminf_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, scaled_ ? Dinv_.p : nullptr, vec_n_.p, red(SC_TMP0));
   check_launch("norminf_Atdy");
   read_scalars(SC_TMP0, 1);
+  rec[3] = (double)h_sc_[SC_TMP0];
   if (!((double)h_sc_[SC_TMP0] <= st_.eps_prim_inf * norm_dy)) return false;
+  rec[1] = 4;
   scal_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, (T)(-1.0 / norm_dy), dy_.p);
   check_launch("scal_dy");
   dot_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, dy_.p, b_.p, red(SC_TMP0));
@@ -1607,26 +1622,41 @@ bool Engine<T>::primal_infeasible() {
   const double dyt_b = (double)h_sc_[SC_TMP0];
   const double box_sum = (double)h_sc_[SC_TMP1];
   const bool cone_bad = (h_sc_[SC_TMP2] != 0) || (h_sc_[SC_TMP3] != 0) || (h_sc_[SC_TMP4] != 0) || (h_sc_[SC_TMP5] != 0);
+  rec[4] = dyt_b;
+  rec[5] = box_sum;
+  rec[6] = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) + (h_sc_[SC_TMP5] != 0 ? 8 : 0);
+  rec[7] = psd_.cert_unconverged;
   const double sF = (cone_bad ? INFINITY : 0.0) + box_sum - dyt_b;
+  rec[0] = sF <= st_.eps_prim_inf ? 1.0 : 0.0;
   return sF <= st_.eps_prim_inf;
 }
 
-// is_dual_infeasible! (infeasibility.jl:32-68); dx_ holds delta_x
+// is_dual_infeasible! (infeasibility.jl:32-68); dx_ holds delta_x.  inf_rec_: {verdict, last gate reached (1: norm,
+// 2: q'dx, 3: P dx, 4: cone tests), |D dx|_inf, q'dx, |Dinv P dx|_inf, NaN, failed families, unconverged PSD cones}
 template <typename T>
 bool Engine<T>::dual_infeasible() {
   const T eps = (T)st_.eps_dual_inf;
+  double* rec = inf_rec_;
+  for (int k = 0; k < 8; ++k) rec[k] = (k == 0 || k >= 6) ? 0.0 : NAN;
+  rec[1] = 1;
   scaled_norminf_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, scaled_ ? D_.p : nullptr, dx_.p, red(SC_TMP0));
   check_launch("norminf_dx");
   dot_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, q_.p, dx_.p, red(SC_TMP1));
   check_launch("dot_q_dx");
   read_scalars(SC_TMP0, 2);
   const double norm_dx = (double)h_sc_[SC_TMP0];
+  rec[2] = norm_dx;
+  rec[3] = (double)h_sc_[SC_TMP1];
   if (!(norm_dx > st_.eps_dual_inf)) return false;
+  rec[1] = 2;
   if (!((double)h_sc_[SC_TMP1] / (norm_dx * c_) < -st_.eps_dual_inf)) return false;
+  rec[1] = 3;
   launch_spmv(P_, dx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n_,
               EpiStoreScaledMax<T>{nullptr, nullptr, scaled_ ? Dinv_.p : nullptr}, red(SC_TMP0), "spmv_P_dx");
   read_scalars(SC_TMP0, 1);
+  rec[4] = (double)h_sc_[SC_TMP0];
   if (!((double)h_sc_[SC_TMP0] / (norm_dx * c_) <= st_.eps_dual_inf)) return false;
+  rec[1] = 4;
   launch_spmv(A_, dx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m_, EpiStore<T>{nullptr, vec_m_.p}, red(SC_TMP0), "spmv_A_dx");
   if (scaled_) {
     scale_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, Einv_.p, vec_m_.p, vec_m_.p);
@@ -1654,6 +1684,9 @@ bool Engine<T>::dual_infeasible() {
   CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_ + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
   if (nranks_ > 1) allreduce_max(sc_.p + SC_TMP2, 4);
   read_scalars(SC_TMP2, 4);
+  rec[6] = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) + (h_sc_[SC_TMP5] != 0 ? 8 : 0);
+  rec[7] = psd_.cert_unconverged;
+  rec[0] = rec[6] == 0 ? 1.0 : 0.0;
   return (h_sc_[SC_TMP2] == 0) && (h_sc_[SC_TMP3] == 0) && (h_sc_[SC_TMP4] == 0) && (h_sc_[SC_TMP5] == 0);
 }
 
@@ -2182,6 +2215,29 @@ void Engine<T>::psd_stats(int64_t* o) {
 template <typename T>
 void Engine<T>::get_w(void* out) { download_vec(out, W_[cur_].p, (size_t)n_ + m_); sync(); }
 
+template <typename T>
+void Engine<T>::infeasibility_test(int which, const void* delta, double* out) {
+  CUDA_TRY(cudaSetDevice(device_));
+  if (which == 0) {
+    upload_vec(dy_, delta, m_);
+    primal_infeasible();
+  } else if (which == 1) {
+    upload_vec(dx_, delta, n_);
+    dual_infeasible();
+  } else {
+    throw EngineError{COSMO_B200_ERR_INVALID, "infeasibility_test: which must be 0 (primal) or 1 (dual)"};
+  }
+  for (int k = 0; k < 8; ++k) out[k] = inf_rec_[k];
+}
+
+template <typename T>
+void Engine<T>::psd_lambda_max(const void* v, double* lam) {
+  CUDA_TRY(cudaSetDevice(device_));
+  upload_vec(vec_m_, v, m_);
+  if (!psd_.empty()) psd_.lambda_max(vec_m_.p, stream_, st_.psd_max_sweeps, launches_, lam);
+  sync();
+}
+
 }  // namespace cosmo
 
 // ============================================================================
@@ -2298,6 +2354,14 @@ int cosmo_b200_set_accelerator(cosmo_b200_handle* h, const cosmo_b200_accelerato
 int cosmo_b200_accelerator_stats(cosmo_b200_handle* h, int64_t out[6]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->accelerator_stats(out));
+}
+int cosmo_b200_infeasibility_test(cosmo_b200_handle* h, int32_t which, const void* delta, double out[8]) {
+  if (!delta || !out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->infeasibility_test(which, delta, out));
+}
+int cosmo_b200_psd_lambda_max(cosmo_b200_handle* h, const void* v, double* lam) {
+  if (!v || !lam) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->psd_lambda_max(v, lam));
 }
 int cosmo_b200_get_scaling(cosmo_b200_handle* h, void* D, void* E, double* c) {
   ABI_GUARD(h, h->impl->get_scaling(D, E, c));

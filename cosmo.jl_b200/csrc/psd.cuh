@@ -117,6 +117,11 @@ __global__ void __launch_bounds__(kBlock) psd_embedding_store_kernel(PsdConeDesc
 // ---------------------------------------------------------------------------
 // Small cones: one CTA per cone, everything in shared memory.
 //   mode 0: s[cone] = Pi_PSD(ws[cone]);  mode 1: lam_max[cone] = max eigenvalue of mat(ws[cone])
+// mode 0 symmetrizes a square cone as project! does (symmetrize_upper!); mode 1 reads its upper triangle only, as the
+// certificate is_pos_def! -> cholesky!(Hermitian(X)) does (convexset.jl:324-336, algebra.jl:226-233): delta y and
+// A delta x are not symmetric on the rows of a square cone in general.  In mode 1 a cone whose Jacobi sweeps did not
+// converge within max_sweeps gets lam_max = +inf (not certified: the diagonal of a partly rotated matrix can
+// underestimate lambda_max) and increments *fail_flag.
 // ---------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __restrict__ descs, const T* __restrict__ ws,
@@ -157,6 +162,9 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
       if (a != b) v *= inv_sqrt2;
     } else if (d.triangle == 2) {
       v = hermitian_embedding_entry(x, N >> 1, i, j);
+    } else if (mode == 1) {
+      const int a = i < j ? i : j, b = i < j ? j : i;
+      v = x[(long long)b * N + a];                                      // Hermitian(X, :U)
     } else {
       v = (x[(long long)j * N + i] + x[(long long)i * N + j]) / T(2);   // symmetrize_upper!, algebra.jl:201-208
     }
@@ -248,9 +256,13 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
     if (!rotated) { converged = true; break; }
     __syncthreads();
   }
-  if (!converged && threadIdx.x == 0 && fail_flag) atomicExch(fail_flag, 1);
+  if (!converged && threadIdx.x == 0 && fail_flag) atomicAdd(fail_flag, 1);
 
   if (mode == 1) {
+    if (!converged) {
+      if (threadIdx.x == 0) lam_max[blockIdx.x] = T(INFINITY);
+      return;
+    }
     T mx = -INFINITY;
     for (int i = threadIdx.x; i < N; i += blockDim.x) mx = fmax(mx, A[i + i * ld]);
 #pragma unroll
@@ -357,9 +369,10 @@ __global__ void __launch_bounds__(kBlock) psd_cone_max_kernel(const T* __restric
 // A = mat(x) 2^-pe, V = I, partial sums of |A|_F^2.  pe (even) is the exponent of the power of two nearest max |x|
 // (psd_cone_max_kernel): the scaling is exact, the projection is positively homogeneous, so the eigensolvers and the
 // Newton-Schulz iteration work on a matrix of norm ~1 whatever the scale of x; *up = 2^pe undoes it on the output
-// (psd_unscale_kernel).
+// (psd_unscale_kernel).  A square cone is symmetrized as project! does, or with upper = 1 reflected from its upper
+// triangle as the certificate reads it (see psd_small_kernel).
 template <typename T>
-__global__ void __launch_bounds__(kBlock) psd_large_load_kernel(PsdConeDesc d, const T* __restrict__ ws, T* __restrict__ A,
+__global__ void __launch_bounds__(kBlock) psd_large_load_kernel(PsdConeDesc d, int upper, const T* __restrict__ ws, T* __restrict__ A,
                                                                 T* __restrict__ V, T* __restrict__ fro_partials,
                                                                 const unsigned long long* __restrict__ mx_bits, double* __restrict__ up) {
   const int N = d.N;
@@ -380,6 +393,9 @@ __global__ void __launch_bounds__(kBlock) psd_large_load_kernel(PsdConeDesc d, c
       const int a = i < j ? i : j, b = i < j ? j : i;
       v = x[svec_pos(a, b)];
       if (a != b) v *= inv_sqrt2;
+    } else if (upper) {
+      const int a = i < j ? i : j, b = i < j ? j : i;
+      v = x[(long long)b * N + a];
     } else {
       v = (x[(long long)j * N + i] + x[(long long)i * N + j]) / T(2);
     }
@@ -882,6 +898,9 @@ struct PsdBatch {
   T* R_d = nullptr;      // npairs * 64 * 64 pivot rotations
   int* act_d = nullptr;  // per pair: pivot needed work this round
   std::vector<T> lam_host;
+  std::vector<int> small_idx, large_idx;   // position of each small / large cone among all PSD cones (set order)
+  std::vector<double> lam_all;
+  int cert_unconverged = 0;                // cones whose eigensolver missed max_sweeps in the last lambda_max call
 
   ~PsdBatch() {
     cudaFree(small_d); cudaFree(lam_small_d); cudaFree(fail_d); cudaFree(A_d); cudaFree(V_d); cudaFree(cs_d);
@@ -896,7 +915,11 @@ struct PsdBatch {
   }
 
   void init(const std::vector<PsdConeDesc>& descs, cudaStream_t st) {
-    for (const auto& d : descs) (d.N <= kPsdSmallMax ? small_h : large_h).push_back(d);
+    for (size_t k = 0; k < descs.size(); ++k) {
+      const bool small = descs[k].N <= kPsdSmallMax;
+      (small ? small_h : large_h).push_back(descs[k]);
+      (small ? small_idx : large_idx).push_back((int)k);
+    }
     if (!small_h.empty()) {
       for (const auto& d : small_h) small_maxN = std::max(small_maxN, d.N);
       ck(cudaMalloc(&small_d, small_h.size() * sizeof(PsdConeDesc)), "cudaMalloc psd descs");
@@ -950,14 +973,15 @@ struct PsdBatch {
   void reset_warm_start() { warm_valid = false; warm_count = 0; }
 
   // A_d = mat(ws[cone]) 2^-pe, V_d = I, fro_d = partial sums of |A_d|_F^2 (g of them), up_d = 2^pe
-  void load_large(const PsdConeDesc& d, const T* ws, cudaStream_t st, long long& launches) {
+  // upper: reflect a square cone from its upper triangle (the certificate) instead of symmetrizing it (the projection)
+  void load_large(const PsdConeDesc& d, const T* ws, cudaStream_t st, long long& launches, bool upper = false) {
     const int N = d.N;
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
     const long long dim = psd_cone_dim(d);
     const int gm = (int)std::min<long long>((dim + kBlock - 1) / kBlock, kMaxGrid);
     ck(cudaMemsetAsync(mx_d, 0, sizeof(unsigned long long), st), "memset psd max");
     psd_cone_max_kernel<T><<<gm, kBlock, 0, st>>>(ws + d.off, dim, mx_d);
-    psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, ws, A_d, V_d, fro_d, mx_d, up_d);
+    psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, upper ? 1 : 0, ws, A_d, V_d, fro_d, mx_d, up_d);
     launches += 2;
   }
   void unscale_large(const PsdConeDesc& d, T* s, cudaStream_t st, long long& launches) {
@@ -966,15 +990,16 @@ struct PsdBatch {
     ++launches;
   }
 
-  // eigen-decompose one large cone into A_d (diagonal = eigenvalues) and V_d (block Jacobi)
-  void large_eig(const PsdConeDesc& d, const T* ws, cudaStream_t st, int max_sweeps, long long& launches,
-                 bool allow_warm = false) {
+  // eigen-decompose one large cone into A_d (diagonal = eigenvalues) and V_d (block Jacobi).  certificate: load a
+  // square cone from its upper triangle and return false instead of throwing PsdError when max_sweeps is not enough.
+  bool large_eig(const PsdConeDesc& d, const T* ws, cudaStream_t st, int max_sweeps, long long& launches,
+                 bool allow_warm = false, bool certificate = false) {
     const int N = d.N;
     int Nb = (N + kBjB - 1) / kBjB;
     if (Nb & 1) ++Nb;                                 // even number of blocks (zero padding decouples)
     const int npairs = Nb / 2;
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-    load_large(d, ws, st, launches);
+    load_large(d, ws, st, launches, certificate);
     psd_large_thr_kernel<T><<<1, 32, 0, st>>>(fro_d, g, thr_d, rot_d);
     ++launches;
     // Warm start (ADMM iterates move slowly): rotate X into the eigenbasis of the previous projection,
@@ -1008,13 +1033,17 @@ struct PsdBatch {
     last_sweeps = sweep;
     if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd] N=%d warm=%d sweeps=%d\n", N, (int)warm, sweep);
     ck(cudaGetLastError(), "psd block-Jacobi kernels");
-    if (!converged) throw PsdError{"block Jacobi eigensolver did not converge within psd_max_sweeps"};
+    if (!converged) {
+      if (certificate) return false;
+      throw PsdError{"block Jacobi eigensolver did not converge within psd_max_sweeps"};
+    }
     if (allow_warm && Vw_d) {
       ck(cudaMemcpyAsync(Vw_d, V_d, (size_t)N * N * sizeof(T), cudaMemcpyDeviceToDevice, st), "save V0");
       warm_valid = true;
       warm_N = N;
       ++warm_count;
     }
+    return true;
   }
 
   // s[cone rows] = Pi_PSD(ws[cone rows]) for every PSD cone
@@ -1076,27 +1105,45 @@ struct PsdBatch {
   // positive definite (is_pos_def!/is_neg_def!, algebra.jl:226-238; convexset.jl:324-336,415-425)
   bool certificate(const T* v, bool /*negate*/, double tol, cudaStream_t st, int max_sweeps, long long& launches) {
     if (empty()) return true;
-    if (max_sweeps <= 0) max_sweeps = 30;
+    lam_all.resize(small_h.size() + large_h.size());
+    lambda_max(v, st, max_sweeps, launches, lam_all.data());
     bool ok = true;
+    for (double l : lam_all) if (!(l < tol)) ok = false;
+    return ok;
+  }
+
+  // lam[k] = lambda_max of the k-th PSD cone (set order) of mat(v), read as the certificate reads it (a square cone
+  // from its upper triangle); +inf for a cone whose eigensolver did not converge within max_sweeps (counted in
+  // cert_unconverged).  Small cones: psd_small_kernel mode 1; large cones: block Jacobi + psd_large_lammax_kernel.
+  void lambda_max(const T* v, cudaStream_t st, int max_sweeps, long long& launches, double* lam) {
+    if (max_sweeps <= 0) max_sweeps = 30;
+    cert_unconverged = 0;
     if (!small_h.empty()) {
+      ck(cudaMemsetAsync(fail_d, 0, sizeof(int), st), "memset fail flag");
       psd_small_kernel<T><<<(int)small_h.size(), kBlock, small_smem(), st>>>(small_d, v, nullptr, 1, lam_small_d, max_sweeps, fail_d);
       ck(cudaGetLastError(), "psd_small_kernel");
       ++launches;
       lam_host.resize(small_h.size());
+      int fails = 0;
       ck(cudaMemcpyAsync(lam_host.data(), lam_small_d, small_h.size() * sizeof(T), cudaMemcpyDeviceToHost, st), "copy lam");
+      ck(cudaMemcpyAsync(&fails, fail_d, sizeof(int), cudaMemcpyDeviceToHost, st), "copy fail flag");
       ck(cudaStreamSynchronize(st), "sync");
-      for (T l : lam_host) if (!((double)l < tol)) ok = false;
+      for (size_t k = 0; k < small_h.size(); ++k) lam[small_idx[k]] = (double)lam_host[k];
+      cert_unconverged += fails;
     }
     for (size_t k = 0; k < large_h.size(); ++k) {
-      large_eig(large_h[k], v, st, max_sweeps, launches);
+      if (!large_eig(large_h[k], v, st, max_sweeps, launches, /*allow_warm=*/false, /*certificate=*/true)) {
+        lam[large_idx[k]] = INFINITY;
+        ++cert_unconverged;
+        continue;
+      }
       psd_large_lammax_kernel<T><<<1, 32, 0, st>>>(large_h[k].N, A_d, up_d, lam_large_d + k);
       ++launches;
       T l;
       ck(cudaMemcpyAsync(&l, lam_large_d + k, sizeof(T), cudaMemcpyDeviceToHost, st), "copy lam");
       ck(cudaStreamSynchronize(st), "sync");
-      if (!((double)l < tol)) ok = false;
+      lam[large_idx[k]] = (double)l;
     }
-    return ok;
   }
 
   bool failed(cudaStream_t st) {

@@ -96,7 +96,8 @@ EXPORTS = [
     "cosmo_b200_residuals", "cosmo_b200_spmv", "cosmo_b200_spmv_bench", "cosmo_b200_get_rho_vec", "cosmo_b200_get_w",
     "cosmo_b200_comm_unique_id", "cosmo_b200_comm_init", "cosmo_b200_comm_p2p_export", "cosmo_b200_comm_p2p_attach",
     "cosmo_b200_tc_gemm_test", "cosmo_b200_psd_stats", "cosmo_b200_get_scaling",
-    "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats",
+    "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats", "cosmo_b200_infeasibility_test",
+    "cosmo_b200_psd_lambda_max",
 ]
 
 _lib = None
@@ -146,6 +147,8 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_get_scaling.argtypes = [vp, vp, vp, C.POINTER(C.c_double)]
     lib.cosmo_b200_set_accelerator.argtypes = [vp, C.POINTER(AcceleratorStruct)]
     lib.cosmo_b200_accelerator_stats.argtypes = [vp, C.POINTER(C.c_int64)]
+    lib.cosmo_b200_infeasibility_test.argtypes = [vp, C.c_int32, vp, C.POINTER(C.c_double)]
+    lib.cosmo_b200_psd_lambda_max.argtypes = [vp, vp, C.POINTER(C.c_double)]
     lib.cosmo_b200_tc_gemm_test.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32,
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]
     for name in EXPORTS:
@@ -206,6 +209,7 @@ class Engine:
         P.sort_indices()
         A.sort_indices()
         self.m, self.n = A.shape
+        self.n_psd = sum(1 for t in sets if t[0] in (PSD_SQUARE, PSD_TRIANGLE, PSD_TRIANGLE_COMPLEX) and int(t[1]) > 0)
         base = 1 if julia_indexing else 0
         keep = []  # keep host arrays alive during create
 
@@ -412,6 +416,30 @@ class Engine:
         self._check(self._lib.cosmo_b200_accelerator_stats(self._h, out))
         return dict(zip(ACCELERATOR_STATS, [int(v) for v in out]))
 
+
+    def infeasibility_test(self, which, delta):
+        """cosmo_b200_infeasibility_test: is_primal_infeasible! (which = 0, delta = delta_y, m) or is_dual_infeasible!
+        (which = 1, delta = delta_x, n) on the engine's data; returns a dict keyed by INFEASIBILITY_RECORD."""
+        delta = self._vec(delta, self.m if which == 0 else self.n)
+        out = (C.c_double * 8)()
+        self._check(self._lib.cosmo_b200_infeasibility_test(self._h, int(which), _ptr(delta), out))
+        rec = dict(zip(INFEASIBILITY_RECORD, list(out)))
+        for k in ("verdict", "gate", "families", "psd_unconverged"):
+            rec[k] = int(rec[k])
+        return rec
+
+    def psd_lambda_max(self, v):
+        """cosmo_b200_psd_lambda_max: lambda_max of every PSD cone of mat(v) (set order) as the certificate computes it."""
+        v = self._vec(v, self.m)
+        lam = np.zeros(max(self.n_psd, 1), dtype=np.float64)
+        self._check(self._lib.cosmo_b200_psd_lambda_max(self._h, _ptr(v), lam.ctypes.data_as(C.POINTER(C.c_double))))
+        return lam[:self.n_psd]
+
+
+# cosmo_b200_infeasibility_test's out[8]: "gate2" is |Dinv A'dy|_inf (primal) or q'dx (dual), "gate3" dy'b of the
+# normalized -dy (primal) or |Dinv P dx|_inf (dual); "families" has bit 0 rows, 1 SOC, 2 PSD, 3 Exp/Pow
+INFEASIBILITY_RECORD = ("verdict", "gate", "norm", "gate2", "gate3", "box_sum", "families", "psd_unconverged")
+FAMILY_ROWS, FAMILY_SOC, FAMILY_PSD, FAMILY_C3 = 1, 2, 4, 8
 
 ACCELERATOR_STATS = ("accepted", "declined", "rejected", "rho_restarts", "memory_restarts", "activated_at")
 

@@ -285,6 +285,20 @@ int cosmo_b200_get_rho_vec(cosmo_b200_handle* h, void* rho_vec);
 int cosmo_b200_get_scaling(cosmo_b200_handle* h, void* D, void* E, double* c);
 /* read back the operator variable w = [w_x; w_s] (n+m) */
 int cosmo_b200_get_w(cosmo_b200_handle* h, void* w);
+/* is_primal_infeasible! (which = 0, delta = delta_y: this rank's m rows) or is_dual_infeasible! (which = 1,
+   delta = delta_x: n) (infeasibility.jl:1-68) on the given delta, with the engine's D, E, c, b, q and eps_*_inf.
+   out = {verdict (1: infeasible), last gate reached (1: norm, 2: A'dy resp. q'dx, 3: P dx (dual only), 4: cone tests),
+          |E dy|_inf resp. |D dx|_inf, |Dinv A'dy|_inf resp. q'dx, dy'b of the normalized -dy resp. |Dinv P dx|_inf,
+          Box support sum (primal), failed certificate families (bit 0: Zero/Nonnegatives/Box rows, 1: SOC, 2: PSD,
+          3: Exp/Pow and their duals), PSD cones whose eigensolver missed psd_max_sweeps (counted as not certified)};
+   a value that the test did not reach is NaN.  Uses the engine's dx / dy scratch vectors, as cosmo_b200_residuals
+   does: call it between solves, not inside one.  With several ranks every rank calls it. */
+int cosmo_b200_infeasibility_test(cosmo_b200_handle* h, int32_t which, const void* delta, double out[8]);
+/* lam[k] = largest eigenvalue of mat(v[rows of the k-th PSD cone]) for every PSD cone of this rank, in set order, as
+   the infeasibility certificate computes it: a PsdCone read from its upper triangle (is_pos_def!, convexset.jl:324-336),
+   the same prescaling and eigensolver path (shared-memory Jacobi up to N = 96, block Jacobi beyond); +inf where the
+   eigensolver did not converge within psd_max_sweeps.  v has the m rows of this rank. */
+int cosmo_b200_psd_lambda_max(cosmo_b200_handle* h, const void* v, double* lam);
 
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */

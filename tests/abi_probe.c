@@ -40,5 +40,10 @@ int main(void) {
   printf("create_null %d\n", rc);
   const char* msg = cosmo_b200_last_error(NULL);
   printf("last_error %s\n", msg ? msg : "(null)");
+  /* the test hooks refuse a null handle or null buffers the same way */
+  double out8[8], lam = 0.0, v = 0.0;
+  printf("infeasibility_null %d %d\n", cosmo_b200_infeasibility_test(NULL, 0, &v, out8),
+         cosmo_b200_infeasibility_test(NULL, 0, NULL, NULL));
+  printf("lambda_max_null %d %d\n", cosmo_b200_psd_lambda_max(NULL, &v, &lam), cosmo_b200_psd_lambda_max(NULL, NULL, &lam));
   return 0;
 }

@@ -340,3 +340,147 @@ def g17_complex_least_eigenvalue():
 
 
 G17_OBJ = 1.0 - np.sqrt(2.0)
+
+
+# ---------------------------------------------------------------------------
+# Infeasible problems of test/UnitTests/InfeasibilityTests/ (primal_infeasible_1/2/3, dual_infeasible_1/2).
+# The reference draws its data from MersenneTwister streams that cannot be reproduced here, so these builders follow
+# the construction of each file (sizes, sparsity, the feasible or unbounded part and the row that breaks it) with
+# numpy's generator and a fixed seed.  The seeds are ones for which the CPU oracle (EmptyAccelerator and
+# AndersonAccelerator, scaling 0 and 10) reaches the status the reference's file asserts.
+# ---------------------------------------------------------------------------
+def _sprand(rng, m, n, density):
+    """sprand(rng, m, n, density): uniform [0, 1) values at a Bernoulli pattern"""
+    mask = rng.random((m, n)) < density
+    return sp.csr_matrix(np.where(mask, rng.random((m, n)), 0.0))
+
+
+def _pos_def(rng, n, a_min=0.1, a_max=2.0):
+    """generate_pos_def_matrix (COSMOTestUtils.jl:11-19): Q diag(eigs) Q' with eigs uniform in [a_min, a_max]"""
+    Q, _ = np.linalg.qr(rng.random((n, n)))
+    X = (Q * (rng.random(n) * (a_max - a_min) + a_min)) @ Q.T
+    return 0.5 * (X + X.T)
+
+
+def _svec_upper(X):
+    """the PsdConeTriangle vector of a symmetric matrix (upper triangle by columns, sqrt 2 off the diagonal)"""
+    N = X.shape[0]
+    return np.concatenate([np.concatenate([X[:j, j] * np.sqrt(2.0), [X[j, j]]]) for j in range(N)])
+
+
+def primal_infeasible_1(seed=74747):
+    """primal_infeasible_1.jl: x >= 0, A >= 0, b < 0, s in R+ (one Nonnegatives constraint)."""
+    rng = np.random.default_rng(seed)
+    n = int(rng.integers(5, 51))
+    m = 2 * n
+    A = sp.vstack([_sprand(rng, m, n, 0.8), -sp.identity(n)]).tocsr()
+    b = np.concatenate([-rng.random(m), np.zeros(n)])
+    P = _pos_def(rng, n)
+    ytrue, xtrue = rng.random(m + n), rng.random(n)
+    q = -P @ xtrue - A.T @ ytrue
+    return P, q, [O.Constraint(-A, b, O.Nonnegatives(m + n))]
+
+
+def primal_infeasible_2(seed=29, r=None, triangle=False, m1=None):
+    """primal_infeasible_2.jl: ZeroSet rows with a feasible right-hand side, x >= 0, and a PsdCone whose constant part
+    is entrywise negative (A >= 0, x >= 0: the diagonal is negative).  The PSD rows of A are arbitrary, so delta_y is not
+    symmetric on the square cone.  triangle=True: the same with a PsdConeTriangle; r: the side (r >= 97 for the large
+    path); m1: the number of ZeroSet rows (the reference uses r^2)."""
+    rng = np.random.default_rng(seed)
+    n = int(rng.integers(10, 51))
+    r = int(rng.integers(2, 11)) if r is None else r
+    m2 = r * (r + 1) // 2 if triangle else r * r
+    m1 = m2 if m1 is None else m1
+    A = _sprand(rng, m1 + m2, n, 0.8) * 50
+    xtrue = rng.random(n) * 50
+    b1 = A[:m1] @ xtrue
+    b3 = -rng.random(m2)
+    P = _pos_def(rng, n)
+    Afull = sp.vstack([A[:m1], -sp.identity(n), A[m1:]]).tocsr()
+    Y3 = _pos_def(rng, r)
+    ytrue = np.concatenate([rng.standard_normal(m1) * 50, rng.random(n) * 50,
+                            _svec_upper(Y3) if triangle else Y3.reshape(-1, order="F")])
+    q = -P @ xtrue - Afull.T @ ytrue
+    cone = O.PsdConeTriangle(m2) if triangle else O.PsdCone(m2)
+    return P, q, [O.Constraint(-A[:m1], b1, O.ZeroSet(m1)), O.Constraint(sp.identity(n), np.zeros(n), O.Nonnegatives(n)),
+                  O.Constraint(-A[m1:], b3, cone)]
+
+
+def primal_infeasible_3(seed=1313, psd=True):
+    """primal_infeasible_3.jl: ZeroSet + SecondOrderCone + PsdCone around a feasible point, then the SOC's first row is
+    replaced by 0 x + (-1): t = -1 < 0.  The reference accepts Primal_infeasible or Max_iter_reached.
+    psd=False: the SOC-only variant (ZeroSet + SecondOrderCone)."""
+    rng = np.random.default_rng(seed)
+    n = int(rng.integers(10, 51))
+    m1, m2, r = int(rng.integers(2, 11)), int(rng.integers(3, 11)), int(rng.integers(4, 11))
+    m3 = r * r if psd else 0
+    A = (_sprand(rng, m1 + m2 + m3, n, 0.8) * 50).tolil()
+    xtrue = rng.random(n) * 50
+    s = np.concatenate([np.zeros(m1), rng.random(m2), _pos_def(rng, r).reshape(-1, order="F") if psd else []])
+    b = A @ xtrue + s
+    A[m1, :] = 0
+    b[m1] = -1.0
+    A = A.tocsr()
+    P = _pos_def(rng, n)
+    y2 = rng.random(m2 - 1) * 50
+    ytrue = np.concatenate([rng.random(m1) * 50, [np.linalg.norm(y2) + 1.0], y2,
+                            _pos_def(rng, r, 0.1, 5.0).reshape(-1, order="F") if psd else []])
+    q = -P @ xtrue - A.T @ ytrue
+    cons = [O.Constraint(-A[:m1], b[:m1], O.ZeroSet(m1)), O.Constraint(-A[m1:m1 + m2], b[m1:m1 + m2], O.SecondOrderCone(m2))]
+    if psd:
+        cons.append(O.Constraint(-A[m1 + m2:], b[m1 + m2:], O.PsdCone(m3)))
+    return P, q, cons
+
+
+def dual_infeasible_1(seed=1):
+    """dual_infeasible_1.jl: the last variable has cost -1 and appears in no constraint (P = 0)."""
+    rng = np.random.default_rng(seed)
+    n = int(rng.integers(5, 51))
+    m = 2 * n
+    A = (_sprand(rng, m, n, 0.7) * 50).tolil()
+    A[:, n - 1] = 0
+    A = A.tocsr()
+    q = rng.random(n) * 50
+    q[-1] = -1.0
+    b = A @ (rng.random(n) * 50) + rng.random(m) * 50
+    return sp.csr_matrix((n, n)), q, [O.Constraint(-A, b, O.Nonnegatives(m))]
+
+
+def dual_infeasible_2(seed=8):
+    """dual_infeasible_2.jl: ZeroSet + Nonnegatives + SecondOrderCone + PsdCone around a feasible point, x1 unbounded
+    below (cost -1, in no row but the Nonnegatives row x1 >= ... that lets it decrease)."""
+    rng = np.random.default_rng(seed)
+    n = int(rng.integers(10, 51))
+    m1, m2, m3, r = int(rng.integers(2, 11)), 1, int(rng.integers(3, 11)), int(rng.integers(4, 11))
+    m4 = r * r
+    A = (_sprand(rng, m1 + m2 + m3 + m4, n, 0.8) * 50).tolil()
+    xtrue = rng.random(n) * 50
+    s3 = rng.random(m3 - 1)
+    s = np.concatenate([np.zeros(m1), [rng.random()], [np.linalg.norm(s3) + 1.0], s3, _pos_def(rng, r).reshape(-1, order="F")])
+    A[:, 0] = 0
+    A[m1, :] = 0
+    A[m1, 0] = -1.0
+    A = A.tocsr()
+    b = A @ xtrue + s
+    b[m1] = 0.0
+    q = np.concatenate([[-1.0], rng.random(n - 1)])
+    o = np.cumsum([0, m1, m2, m3, m4])
+    return sp.csr_matrix((n, n)), q, [O.Constraint(-A[o[0]:o[1]], b[o[0]:o[1]], O.ZeroSet(m1)),
+                                      O.Constraint(-A[o[1]:o[2]], b[o[1]:o[2]], O.Nonnegatives(m2)),
+                                      O.Constraint(-A[o[2]:o[3]], b[o[2]:o[3]], O.SecondOrderCone(m3)),
+                                      O.Constraint(-A[o[3]:o[4]], b[o[3]:o[4]], O.PsdCone(m4))]
+
+
+# (name, builder, statuses the reference's file accepts)
+INFEASIBILITY_PROBLEMS = [
+    ("primal_infeasible_1", primal_infeasible_1, ("Primal_infeasible",)),
+    ("primal_infeasible_2", primal_infeasible_2, ("Primal_infeasible",)),
+    ("primal_infeasible_2_triangle", lambda: primal_infeasible_2(seed=2024, triangle=True), ("Primal_infeasible",)),
+    # N = 100 > 96: the block-Jacobi certificate.  The oracle detects it with EmptyAccelerator only (with
+    # AndersonAccelerator it reaches max_iter on every seed tried), so the solve tests run it without acceleration
+    ("primal_infeasible_2_large_psd", lambda: primal_infeasible_2(seed=97, r=100, triangle=True, m1=20), ("Primal_infeasible",)),
+    ("primal_infeasible_3", primal_infeasible_3, ("Primal_infeasible", "Max_iter_reached")),
+    ("primal_infeasible_3_soc", lambda: primal_infeasible_3(psd=False), ("Primal_infeasible", "Max_iter_reached")),
+    ("dual_infeasible_1", dual_infeasible_1, ("Dual_infeasible",)),
+    ("dual_infeasible_2", dual_infeasible_2, ("Dual_infeasible",)),
+]

@@ -3,7 +3,8 @@
 It exists to exercise, without a GPU, the Python side of everything that normally talks to the CUDA engine: the host
 glue of Model (scaling, decomposition, warm starts) and the bodies of the GPU tests themselves (so a typo in a GPU
 test is found by the CPU run, not at the next GPU run).  It implements the part of the call surface those users need:
-ctor, update_settings, warm_start, update_qb, project, solve, w, rho_vec, scaling, close."""
+ctor, update_settings, warm_start, update_qb, project, solve, w, rho_vec, scaling, close, and the infeasibility hooks
+infeasibility_test and psd_lambda_max."""
 import numpy as np
 import scipy.sparse as sp
 
@@ -12,6 +13,8 @@ from oracle import cosmo_oracle as O
 
 _PLAIN = {E.ZERO: O.ZeroSet, E.NONNEG: O.Nonnegatives, E.SOC: O.SecondOrderCone, E.PSD_SQUARE: O.PsdCone,
           E.PSD_TRIANGLE: O.PsdConeTriangle, E.PSD_TRIANGLE_COMPLEX: O.ComplexPsdConeTriangle}
+_FAMILY = {O.ZeroSet: E.FAMILY_ROWS, O.Nonnegatives: E.FAMILY_ROWS, O.Box: E.FAMILY_ROWS, O.SecondOrderCone: E.FAMILY_SOC,
+           O.PsdCone: E.FAMILY_PSD, O.PsdConeTriangle: E.FAMILY_PSD, O.ComplexPsdConeTriangle: E.FAMILY_PSD}
 
 
 def cones_from_tuples(sets):
@@ -69,7 +72,7 @@ class OracleEngine:
     def warm_start(self, x, s, mu):
         self._warm = (np.array(x), np.array(s), np.array(mu))
 
-    def update_qb(self, q, b):
+    def update_qb(self, q=None, b=None):
         if q is not None:
             self.q = np.array(q, dtype=float)
         if b is not None:
@@ -97,6 +100,61 @@ class OracleEngine:
         out.rho, out.rho_updates, out.times = 0.1, list(r.info.rho_updates), {"iter_time_device": 0.0}
         out.kkt_inner_iterations = out.kkt_multiplications = out.kernel_launches = 0
         return out
+
+    def infeasibility_test(self, which, delta):
+        """cosmo_b200_infeasibility_test through the oracle's scaled_norm / in_dual / in_pol_recc / support_function"""
+        D, Em, c = self._scal
+        eps = (self.st.eps_prim_inf if which == 0 else self.st.eps_dual_inf) if self.st is not None else 1e-4
+        d = np.array(delta, dtype=float)
+        rec = dict(zip(E.INFEASIBILITY_RECORD, [0, 1, np.nan, np.nan, np.nan, np.nan, 0, 0]))
+        norm = O.scaled_norm(Em if which == 0 else D, d, np.inf)
+        rec["norm"] = norm
+        if which == 1:
+            rec["gate2"] = float(self.q @ d)
+        if not norm > eps:
+            return rec
+        rec["gate"] = 2
+        if which == 0:
+            rec["gate2"] = float(np.max(np.abs((self.A.T @ d) / D)))
+            if not rec["gate2"] <= eps * norm:
+                return rec
+            v = d * (-1.0 / norm)
+            rec["gate3"] = float(v @ self.b)
+        else:
+            if not rec["gate2"] / (norm * c) < -eps:
+                return rec
+            rec["gate"] = 3
+            rec["gate3"] = float(np.max(np.abs((self.P @ d) / D)))
+            if not rec["gate3"] / (norm * c) <= eps:
+                return rec
+            v = (self.A @ d) / Em / norm
+        rec["gate"] = 4
+        fams, box = 0, 0.0
+        for rng, cone in zip(O.row_ranges(self.cones), self.cones):
+            x = v[rng]
+            if which == 0 and isinstance(cone, O.Box):
+                box += O.support_function(x, cone, eps)
+                continue
+            ok = O.support_function(x, cone, eps) == 0.0 if which == 0 else O.in_pol_recc(x, cone, eps)
+            if not ok:
+                fams |= _FAMILY.get(type(cone), E.FAMILY_C3)
+        rec["families"] = fams
+        if which == 0:
+            rec["box_sum"] = box
+            rec["verdict"] = int((np.inf if fams else 0.0) + box - rec["gate3"] <= eps)
+        else:
+            rec["verdict"] = int(fams == 0)
+        return rec
+
+    def psd_lambda_max(self, v):
+        """lambda_max of the upper reflection of every PSD cone (the matrix the oracle's _is_pos_def factorizes)"""
+        lam = []
+        for rng, cone in zip(O.row_ranges(self.cones), self.cones):
+            if isinstance(cone, (O.PsdCone, O.PsdConeTriangle, O.ComplexPsdConeTriangle)):
+                X = O._cone_matrix(np.array(v[rng], dtype=float), cone)
+                U = np.triu(X)
+                lam.append(float(np.linalg.eigvalsh(U + np.triu(U, 1).conj().T)[-1]))
+        return np.array(lam)
 
     def w(self):
         return self._w

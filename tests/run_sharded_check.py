@@ -1,9 +1,11 @@
 """Launched under torchrun (one rank per GPU) by tests/test_gpu_sharded.py: solves the same
-problems row-sharded over WORLD_SIZE GPUs and checks them against the CPU oracle on rank 0."""
+problems row-sharded over WORLD_SIZE GPUs and checks them against the CPU oracle on rank 0, then runs the
+infeasibility certificates of a composite set (every cone family) row-sharded against one unsharded engine."""
 import os
 import sys
 
 import numpy as np
+import scipy.sparse as sp
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
@@ -23,6 +25,77 @@ def gather_rows(local, rows, m, world):
     for r, v in parts:
         full[r] = v
     return full
+
+
+def _composite():
+    """one set of every family (a large PSD cone among them) and, per case, a point v on the rows (leading
+    Nonnegatives row -1, so |v|_inf = 1) where no family, one family or every family fails its certificate"""
+    M = cosmo_b200.model
+    sets = [M.Nonnegatives(4), M.Box(np.array([-1.0, -2.0, -3.0]), np.array([1.0, np.inf, 3.0])), M.SecondOrderCone(3),
+            M.PsdCone(9), M.PsdConeTriangle(6), M.PsdConeTriangle(5050), M.ExponentialCone(), M.DualExponentialCone(),
+            M.PowerCone(0.3), M.DualPowerCone(0.6)]
+    tri100 = np.concatenate([np.concatenate([np.zeros(j), [-0.5]]) for j in range(100)])
+    # the square cone is not symmetric (upper entry 0.2, lower -0.7): certified from its upper triangle
+    base = [np.array([-1.0, -0.5, -0.5, -0.5]), np.zeros(3), np.array([-1.0, 0.3, 0.4]),
+            np.array([-0.5, -0.7, 0, 0.2, -0.5, 0, 0, 0, -0.5]), np.array([-0.5, 0, -0.5, 0, 0, -0.5]), tri100,
+            np.array([0.5, 0.0, -1.0]), np.array([0.0, -0.5, -1.0]), np.array([-0.5, -0.5, 0.0]), np.array([-0.5, -0.5, 0.0])]
+    bad = {0: np.array([-1.0, -0.5, 0.5, -0.5]), 2: np.array([1.0, 0.3, 0.4]), 5: -tri100, 6: np.array([-0.5, 0.0, -1.0])}
+    cases = [np.concatenate(base)]
+    for i, vb in bad.items():
+        parts = list(base)
+        parts[i] = vb
+        cases.append(np.concatenate(parts))
+    allbad = list(base)
+    for i, vb in bad.items():
+        allbad[i] = vb
+    cases.append(np.concatenate(allbad))
+    return sets, cases
+
+
+def check_infeasibility_hook(rank, world, local_rank):
+    """cosmo_b200_infeasibility_test on row-sharded engines against one unsharded engine on rank 0: the verdict, the
+    gate reached, the norms and the failed-family bitmask must be equal, dy'b and the Box support sum (allreduce(sum)
+    over the ranks) equal to 1e-14 of their magnitude.  Primal: A = 0, b != 0, delta_y = -v; dual: A = I, P = 0,
+    q = -v, delta_x = v (the exact-gate rigs of tests/test_gpu_infeasibility.py)."""
+    sets, cases = _composite()
+    m = sum(S.dim for S in sets)
+    b = np.random.default_rng(3).uniform(-1e-4, 1e-4, m)
+    st = cosmo_b200.Settings(scaling=0, eps_prim_inf=2.0 ** -10, eps_dual_inf=2.0 ** -10)
+    rigs = {0: (sp.csc_matrix((1, 1)), np.zeros(1), sp.csc_matrix((m, 1)), b),
+            1: (sp.csc_matrix((m, m)), np.zeros(m), sp.identity(m, format="csc"), np.zeros(m))}
+    ok = True
+    for which, (P, q, A, bb) in rigs.items():
+        sh = sharding.make_shard(P, q, A, bb, sets, rank, world)
+        eng = sharding.create_engine(sh, st, device=local_rank, dist=dist)
+        one = sharding.create_engine(sharding.make_shard(P, q, A, bb, sets, 0, 1), st, device=local_rank) if rank == 0 else None
+        for k, v in enumerate(cases):
+            if which == 0:
+                rec = eng.infeasibility_test(0, -v[sh.rows])
+            else:
+                eng.update_qb(q=-v)
+                rec = eng.infeasibility_test(1, v)
+            recs = [None] * world
+            dist.all_gather_object(recs, rec)
+            if rank == 0:
+                if which == 1:
+                    one.update_qb(q=-v)
+                ref = one.infeasibility_test(which, -v if which == 0 else v)
+                mag_b = float(np.sum(np.abs(v * b)))
+                good = all(r["verdict"] == ref["verdict"] and r["gate"] == ref["gate"] == 4 and r["families"] == ref["families"]
+                           and r["norm"] == ref["norm"] and r["psd_unconverged"] == ref["psd_unconverged"] == 0
+                           and (which == 1 or (abs(r["gate3"] - ref["gate3"]) <= 1e-14 * mag_b
+                                               and abs(r["box_sum"] - ref["box_sum"]) <= 1e-14 * 4.0))
+                           for r in recs)
+                good = good and ref["families"] == ([0, 1, 2, 4, 8, 15][k])
+                print("infeasibility_hook which=%d case=%d world=%d families=%s/%d verdict=%s/%d dyb=%s/%.17g box=%s/%.17g %s" % (
+                    which, k, world, [r["families"] for r in recs], ref["families"], [r["verdict"] for r in recs], ref["verdict"],
+                    [r["gate3"] for r in recs], ref["gate3"], [r["box_sum"] for r in recs], ref["box_sum"],
+                    "OK" if good else "MISMATCH"), flush=True)
+                ok = ok and good
+        eng.close()
+        if one is not None:
+            one.close()
+    return ok
 
 
 def main():
@@ -86,6 +159,7 @@ def main():
                 "OK" if good else "MISMATCH"), flush=True)
             ok = ok and good
         eng.close()
+    ok = check_infeasibility_hook(rank, world, local_rank) and ok
     flag = torch.tensor([1 if ok else 0], device="cuda")
     dist.broadcast(flag, src=0)
     dist.destroy_process_group()

@@ -144,6 +144,7 @@ def test_c_header_layout_matches_ctypes_mirror(tmp_path):
     assert checked >= 35
     assert vals["abi"] == "4" and vals["defaults"] == "0.1 1e-06 1.6 5000 0 15 2"
     assert int(vals["create_null"]) == E.ERR_INVALID and "null" in vals["last_error"]
+    assert vals["infeasibility_null"] == vals["lambda_max_null"] == "%d %d" % (E.ERR_INVALID, E.ERR_INVALID)
 
 
 def _build_c_example(tmp_path):

@@ -1,6 +1,6 @@
 """Dry run of GPU test bodies on the CPU: the CUDA engine is replaced by the oracle-backed stand-in of
 tests/oracle_engine.py and the functions of tests/test_gpu_parity.py, tests/test_gpu_float32.py and
-tests/test_gpu_scale_edges.py are called directly.  What this checks is the
+tests/test_gpu_scale_edges.py and tests/test_gpu_infeasibility.py are called directly.  What this checks is the
 Python side of those tests (imports, helpers, fixtures, the host glue they drive) -- a NameError in a GPU test would
 otherwise only show up on the next GPU run.  Assertion failures are tolerated where the stand-in legitimately differs
 from the engine (it ignores the D/E unscaling of the termination test); every other exception fails the test."""
@@ -25,10 +25,29 @@ CASES = ["test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_t
          "test_gpu_float32::test_g15_g16_float32", "test_gpu_float32::test_g14_model_updates_float32",
          "test_gpu_float32::test_closest_correlation_float32",
          "test_gpu_scale_edges::test_homogeneity_ladder", "test_gpu_scale_edges::test_mixed_large_cone_shapes_share_the_workspace",
-         "test_gpu_scale_edges::test_small_kernel_tensor_core_boundary"]
+         "test_gpu_scale_edges::test_small_kernel_tensor_core_boundary",
+         "test_gpu_infeasibility::test_gate_quantities_match_the_reference",
+         "test_gpu_infeasibility::test_gates_reached_on_either_side_pin_E_D_and_c",
+         "test_gpu_infeasibility::test_rows_at_the_tolerance_edge",
+         "test_gpu_infeasibility::test_soc_exact_boundary_points_are_certified",
+         "test_gpu_infeasibility::test_psd_verdicts_at_the_tolerance",
+         "test_gpu_infeasibility::test_nonsymmetric_square_psd_certificate_reads_the_upper_triangle",
+         "test_gpu_infeasibility::test_exp_pow_verdicts_near_the_boundary",
+         "test_gpu_infeasibility::test_composite_bitmask_names_exactly_the_failing_family",
+         "test_gpu_infeasibility::test_soc_margins_dimensions_and_scale",
+         "test_gpu_infeasibility::test_psd_lambda_max_small_and_large_paths",
+         "test_gpu_infeasibility::test_psd_lambda_max_homogeneity_ladder",
+         "test_gpu_infeasibility::test_unconverged_eigensolver_is_not_certified",
+         "test_gpu_infeasibility::test_reference_infeasible_problems_status_and_iterations",
+         "test_gpu_infeasibility::test_reference_infeasible_problems_float32"]
 MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_through_the_clique_batch",
              "test_project_exp_pow_cones", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
-             "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_project_psd_small_batch_float32"}
+             "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_project_psd_small_batch_float32",
+             "test_gpu_infeasibility::test_gate_quantities_match_the_reference",
+             "test_gpu_infeasibility::test_gates_reached_on_either_side_pin_E_D_and_c",
+             "test_gpu_infeasibility::test_rows_at_the_tolerance_edge",
+             "test_gpu_infeasibility::test_soc_exact_boundary_points_are_certified",
+             "test_gpu_infeasibility::test_composite_bitmask_names_exactly_the_failing_family"}
 
 
 def _calls(fn):
