@@ -31,6 +31,7 @@
 #include "vector_kernels.cuh"
 #include "ruiz.cuh"
 #include "cg_persistent.cuh"
+#include "ldl.cuh"
 
 namespace cosmo {
 
@@ -210,6 +211,7 @@ class EngineBase {
   virtual void accelerator_stats(int64_t* out6) = 0;
   virtual void infeasibility_test(int which, const void* delta, double* out8) = 0;
   virtual void psd_lambda_max(const void* v, double* lam) = 0;
+  virtual void ldl_stats(double* out8) = 0;
 };
 
 template <typename T>
@@ -218,7 +220,11 @@ class Engine : public EngineBase {
   Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st);
   ~Engine() override;
   void update_settings(const cosmo_b200_settings& st) override {
-    if (st.sigma != st_.sigma) destroy_cg_graphs();   // sigma is baked into the captured kernel arguments
+    if (st.sigma != st_.sigma) {   // sigma is baked into the captured kernel arguments
+      destroy_cg_graphs();
+      destroy_ldl_factor_graph();
+      ldl_dirty_ = true;
+    }
     st_ = st;
   }
   void warm_start(const void* x, const void* s, const void* mu) override;
@@ -243,6 +249,7 @@ class Engine : public EngineBase {
   void accelerator_stats(int64_t* out6) override;
   void infeasibility_test(int which, const void* delta, double* out8) override;
   void psd_lambda_max(const void* v, double* lam) override;
+  void ldl_stats(double* out8) override;
 
  private:
   // ---- problem ----
@@ -324,6 +331,26 @@ class Engine : public EngineBase {
   void cg_iteration_launches(const int* done);
   void build_cg_graphs(const int* done);
   void destroy_cg_graphs();
+  // direct LDL' plugin (ldl.cuh): symbolic analysis on the host, factor and solves as captured graphs
+  bool ldl_ready_ = false;
+  bool ldl_dirty_ = true;          // rho_vec_ or sigma changed since the last factorisation
+  std::vector<ldl::Segment> ldl_fseg_, ldl_bseg_;
+  std::vector<int> ldl_fptr_h_, ldl_bptr_h_;
+  int ldl_N_ = 0, ldl_ws_ctas_ = 1, ldl_solve_nodes_ = 0, ldl_factor_nodes_ = 0;
+  long long ldl_nnzK_ = 0, ldl_nnzL_ = 0, ldl_factorizations_ = 0;
+  double ldl_symbolic_s_ = 0.0, ldl_factor_s_ = 0.0;
+  DevBuf<int64_t> ldl_Kp_, ldl_Ksp_, ldl_Ksrc_, ldl_Lp_, ldl_Rp_, ldl_Rmap_;
+  DevBuf<int> ldl_Ki_, ldl_Li_, ldl_Rj_, ldl_fcols_, ldl_fptr_, ldl_bcols_, ldl_bptr_, ldl_perm_, ldl_flags_;
+  DevBuf<T> ldl_Kx_, ldl_Lx_, ldl_Rx_, ldl_D_, ldl_Dinv_, ldl_ws_, ldl_y_;
+  cudaGraphExec_t ldl_factor_graph_ = nullptr, ldl_solve_graph_ = nullptr;
+  cudaEvent_t ldl_ev_[2] = {nullptr, nullptr};
+  void ldl_setup();
+  void ldl_factor();
+  void ldl_solve();
+  void destroy_ldl_factor_graph() {
+    if (ldl_factor_graph_) cudaGraphExecDestroy(ldl_factor_graph_);
+    ldl_factor_graph_ = nullptr;
+  }
   long long kkt_counter_ = 1;   // S.iteration_counter
   int last_cg_iters_ = 1;
   long long total_inner_ = 0, total_mults_ = 0;
@@ -926,6 +953,11 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   }
   classify_and_set_rho(true);
   sync();
+  // QdldlKKTSolver's constructor factors K (kktsolver.jl:293-306): a non-convex P or a singular K fails the create
+  if (st_.kkt_solver == COSMO_B200_KKT_LDL) {
+    ldl_setup();
+    ldl_factor();
+  }
   create_time_ = now_s() - t_ctor0;
   auto_rho_interval_ = 0;
 }
@@ -941,6 +973,9 @@ void Engine<T>::destroy_cg_graphs() {
 template <typename T>
 Engine<T>::~Engine() {
   destroy_cg_graphs();
+  destroy_ldl_factor_graph();
+  if (ldl_solve_graph_) cudaGraphExecDestroy(ldl_solve_graph_);
+  for (cudaEvent_t e : ldl_ev_) if (e) cudaEventDestroy(e);
   for (void* p : ipc_opened_) cudaIpcCloseMemHandle(p);
   if (comm_ && g_nccl.CommDestroy) g_nccl.CommDestroy(comm_);
   if (h_sc_) cudaFreeHost(h_sc_);
@@ -981,6 +1016,7 @@ void Engine<T>::classify_and_set_rho(bool reset_rho, bool rebuild_vec) {
   }
   rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
   check_launch("rho_vec");
+  ldl_dirty_ = true;
 }
 
 // scale_ruiz! (scaling.jl:21-116) on the resident data; see ruiz.cuh
@@ -1094,6 +1130,7 @@ template <typename T>
 void Engine<T>::update_rho(const void* rho_vec, double rho) {
   if (rho_vec) upload_vec(rho_vec_, rho_vec, m_);
   rho_ = rho;
+  ldl_dirty_ = true;   // update_rho! -> refactor! (kktsolver.jl:310-313), done before the next KKT solve
   sync();
 }
 
@@ -1130,6 +1167,8 @@ void Engine<T>::allreduce_max(T* buf, size_t count) {
 template <typename T>
 void Engine<T>::comm_init(int nranks, int rank, const void* id128) {
   if (nranks < 1 || rank < 0 || rank >= nranks) throw EngineError{COSMO_B200_ERR_INVALID, "bad rank / nranks"};
+  if (st_.kkt_solver == COSMO_B200_KKT_LDL)
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU (use CG or reduced MINRES when sharded)"};
   nranks_ = nranks; rank_ = rank;
   if (nranks == 1) return;
   std::string e;
@@ -1295,12 +1334,14 @@ template <typename T>
 void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
   const bool lead = (rank_ == 0);
   const bool full = (st_.kkt_solver == COSMO_B200_KKT_MINRES);
-  if (st_.kkt_solver != COSMO_B200_KKT_CG && st_.kkt_solver != COSMO_B200_KKT_MINRES_REDUCED && !full)
+  const bool direct = (st_.kkt_solver == COSMO_B200_KKT_LDL);
+  if (st_.kkt_solver != COSMO_B200_KKT_CG && st_.kkt_solver != COSMO_B200_KKT_MINRES_REDUCED && !full && !direct)
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "unknown kkt_solver"};
   if (full && nranks_ > 1)
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "full-KKT MINRES is single-GPU in this build (use CG or reduced MINRES when sharded)"};
-  if (full) {
-    kkt_minres(true);   // xsol_ = y1, nu_ = y2
+  if (full || direct) {
+    if (direct) ldl_solve();   // xsol_ = y1, nu_ = y2
+    else kkt_minres(true);
     if (fused_tail) {
       admm_tail_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, nu_.p, rho_vec_.p, s_.p, w_src + n_, w_dst + n_, (T)st_.alpha);
       check_launch("admm_tail");
@@ -1555,6 +1596,7 @@ bool Engine<T>::adapt_rho(const T* x) {
     rho_ = new_rho;
     rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
     check_launch("rho_vec");
+    ldl_dirty_ = true;
     rho_updates_.push_back(new_rho);
     return true;
   }
@@ -2140,11 +2182,167 @@ void Engine<T>::kkt_solve(const void* rhs, void* sol, int64_t* inner) {
   download_vec(sol, xsol_.p, n_);
   download_vec(static_cast<T*>(sol) + n_, nu_.p, m_);
   sync();
-  if (inner) {
+  if (inner && st_.kkt_solver == COSMO_B200_KKT_LDL) {
+    *inner = 0;
+  } else if (inner) {
     CUDA_TRY(cudaMemcpyAsync(h_isc_, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     *inner = h_isc_[ISC_IT];
   }
+}
+
+// ---- direct LDL' plugin (ldl.cuh) -----------------------------------------------------------------------------
+// Symbolic analysis of the resident pattern (host), upload of L's structure and the schedules, device buffers.
+template <typename T>
+void Engine<T>::ldl_setup() {
+  CUDA_TRY(cudaSetDevice(device_));
+  const double t0 = now_s();
+  std::vector<int> Prow(n_ + 1), Pcol(P_.nnz), Arow(n_ + 1), Acol(At_.nnz);
+  CUDA_TRY(cudaMemcpyAsync(Prow.data(), P_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(Arow.data(), At_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  if (P_.nnz) CUDA_TRY(cudaMemcpyAsync(Pcol.data(), P_.col.p, P_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  if (At_.nnz) CUDA_TRY(cudaMemcpyAsync(Acol.data(), At_.col.p, At_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  ldl::Symbolic S;
+  ldl::analyze(n_, m_, Prow, Pcol, Arow, Acol, S);
+  ldl_symbolic_s_ = now_s() - t0;
+  const int N = S.N;
+  ldl_N_ = N;
+  ldl_nnzK_ = S.nnz_triu_K();
+  ldl_nnzL_ = S.nnz_L();
+  // one dense workspace of length N per resident factor CTA: as many CTAs as the widest level, at most two per SM
+  int maxw = 1;
+  for (const ldl::Segment& s : S.fseg)
+    if (!s.run) maxw = std::max(maxw, S.fptr[s.l1] - S.fptr[s.l0]);
+  ldl_ws_ctas_ = std::max(1, std::min(maxw, 2 * num_sms_));
+  const double ts = (double)sizeof(T);
+  const double need = (double)ldl_nnzL_ * (2 * ts + 4 + 4 + 8) + (double)ldl_nnzK_ * (ts + 4 + 8) + (double)S.Ksrc.size() * 8 +
+                      (double)(N + 1) * 8 * 3 + (double)N * (ts * 3 + 4 * 5) + (double)ldl_ws_ctas_ * N * ts;
+  size_t free_b = 0, total_b = 0;
+  CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+  if (need > 0.9 * (double)free_b) {
+    char b[256];
+    snprintf(b, sizeof(b), "the direct LDL' factor does not fit in device memory: nnz(L) = %lld needs %.2f GB, %.2f GB free",
+             ldl_nnzL_, need * 1e-9, (double)free_b * 1e-9);
+    throw EngineError{COSMO_B200_ERR_ALLOC, b};
+  }
+  ldl_Kp_.upload(S.Kp, stream_); ldl_Ki_.upload(S.Ki, stream_); ldl_Ksp_.upload(S.Ksp, stream_); ldl_Ksrc_.upload(S.Ksrc, stream_);
+  ldl_Lp_.upload(S.Lp, stream_); ldl_Li_.upload(S.Li, stream_);
+  ldl_Rp_.upload(S.Rp, stream_); ldl_Rj_.upload(S.Rj, stream_); ldl_Rmap_.upload(S.Rmap, stream_);
+  ldl_fcols_.upload(S.fcols, stream_); ldl_fptr_.upload(S.fptr, stream_);
+  ldl_bcols_.upload(S.bcols, stream_); ldl_bptr_.upload(S.bptr, stream_);
+  ldl_perm_.upload(S.perm, stream_);
+  ldl_Kx_.alloc(std::max<long long>(ldl_nnzK_, 1), false);
+  ldl_Lx_.alloc(std::max<long long>(ldl_nnzL_, 1), false);
+  ldl_Rx_.alloc(std::max<long long>(ldl_nnzL_, 1), false);
+  ldl_D_.alloc(std::max(N, 1)); ldl_Dinv_.alloc(std::max(N, 1)); ldl_y_.alloc(std::max(N, 1));
+  ldl_ws_.alloc((size_t)ldl_ws_ctas_ * std::max(N, 1));   // zeroed: every column clears what it touched
+  ldl_flags_.alloc(2);
+  sync();
+  ldl_fseg_ = S.fseg; ldl_bseg_ = S.bseg;
+  ldl_fptr_h_ = S.fptr; ldl_bptr_h_ = S.bptr;
+  if (!ldl_ev_[0]) { CUDA_TRY(cudaEventCreate(&ldl_ev_[0])); CUDA_TRY(cudaEventCreate(&ldl_ev_[1])); }
+  destroy_ldl_factor_graph();
+  if (ldl_solve_graph_) { cudaGraphExecDestroy(ldl_solve_graph_); ldl_solve_graph_ = nullptr; }
+  ldl_ready_ = true;
+  ldl_dirty_ = true;
+}
+
+// Assemble K from the resident (scaled) P_, At_, rho_vec_ and sigma and factor it: one captured graph, replayed on
+// every refactorisation.  Reads back the pivot counts (the only host synchronisation of the plugin).
+template <typename T>
+void Engine<T>::ldl_factor() {
+  if (!ldl_ready_) ldl_setup();
+  if (!ldl_factor_graph_) {
+    cudaGraph_t g = nullptr;
+    CUDA_TRY(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
+    int nodes = 0;
+    ldl_reset_flags_kernel<<<1, 32, 0, stream_>>>(ldl_flags_.p); ++nodes;
+    ldl_assemble_kernel<T><<<vgrid(ldl_nnzK_), kBlock, 0, stream_>>>(ldl_nnzK_, ldl_Ksp_.p, ldl_Ksrc_.p, P_.val.p, At_.val.p,
+                                                                     rho_vec_.p, (T)st_.sigma, ldl_Kx_.p);
+    ++nodes;
+    LdlFactorArgs<T> a;
+    a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p;
+    a.Kp = ldl_Kp_.p; a.Ki = ldl_Ki_.p; a.Kx = ldl_Kx_.p;
+    a.Lp = ldl_Lp_.p; a.Li = ldl_Li_.p; a.Lx = ldl_Lx_.p;
+    a.Rp = ldl_Rp_.p; a.Rj = ldl_Rj_.p; a.Rmap = ldl_Rmap_.p;
+    a.D = ldl_D_.p; a.Dinv = ldl_Dinv_.p; a.ws = ldl_ws_.p; a.N = ldl_N_; a.flags = ldl_flags_.p;
+    for (const ldl::Segment& s : ldl_fseg_) {
+      a.l0 = s.l0; a.l1 = s.l1;
+      const int grid = s.run ? 1 : std::min(ldl_fptr_h_[s.l1] - ldl_fptr_h_[s.l0], ldl_ws_ctas_);
+      ldl_factor_kernel<T><<<grid, kBlock, 0, stream_>>>(a);
+      ++nodes;
+    }
+    if (ldl_nnzL_) {
+      ldl_csr_gather_kernel<T><<<vgrid(ldl_nnzL_), kBlock, 0, stream_>>>(ldl_nnzL_, ldl_Rmap_.p, ldl_Lx_.p, ldl_Rx_.p);
+      ++nodes;
+    }
+    CUDA_TRY(cudaStreamEndCapture(stream_, &g));
+    CUDA_TRY(cudaGraphInstantiate(&ldl_factor_graph_, g, 0));
+    CUDA_TRY(cudaGraphDestroy(g));
+    ldl_factor_nodes_ = nodes;
+  }
+  int flags[2] = {0, 0};
+  CUDA_TRY(cudaEventRecord(ldl_ev_[0], stream_));
+  CUDA_TRY(cudaGraphLaunch(ldl_factor_graph_, stream_));
+  CUDA_TRY(cudaEventRecord(ldl_ev_[1], stream_));
+  CUDA_TRY(cudaMemcpyAsync(flags, ldl_flags_.p, sizeof(flags), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  launches_ += ldl_factor_nodes_;
+  float ms = 0.f;
+  CUDA_TRY(cudaEventElapsedTime(&ms, ldl_ev_[0], ldl_ev_[1]));
+  ldl_factor_s_ = ms * 1e-3;
+  ++ldl_factorizations_;
+  if (flags[1] != 0) {
+    char b[160];
+    snprintf(b, sizeof(b), "LDL' factorisation of the KKT matrix met %d zero or non-finite pivots", flags[1]);
+    throw EngineError{COSMO_B200_ERR_NUMERICAL, b};
+  }
+  // positive_inertia(ldlfact) == n (kktsolver.jl:300-303)
+  if (flags[0] != n_) throw EngineError{COSMO_B200_ERR_INVALID, "Objective function is not convex."};
+  ldl_dirty_ = false;
+}
+
+// [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: forward and backward levels replayed as one graph
+template <typename T>
+void Engine<T>::ldl_solve() {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU"};
+  if (!ldl_ready_) ldl_setup();
+  if (ldl_dirty_) ldl_factor();
+  if (!ldl_solve_graph_) {
+    cudaGraph_t g = nullptr;
+    CUDA_TRY(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
+    int nodes = 0;
+    LdlSolveArgs<T> a;
+    a.Dinv = ldl_Dinv_.p; a.perm = ldl_perm_.p; a.rhs = ls_.p; a.y = ldl_y_.p; a.out1 = xsol_.p; a.out2 = nu_.p; a.n = n_;
+    auto grid = [&](const std::vector<int>& ptr, const ldl::Segment& s) {
+      return s.run ? 1 : (int)std::min<long long>(((long long)ptr[s.l1] - ptr[s.l0] + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid);
+    };
+    a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p; a.ptr = ldl_Rp_.p; a.idx = ldl_Rj_.p; a.val = ldl_Rx_.p;
+    for (const ldl::Segment& s : ldl_fseg_) {
+      a.l0 = s.l0; a.l1 = s.l1;
+      ldl_forward_kernel<T><<<grid(ldl_fptr_h_, s), kBlock, 0, stream_>>>(a);
+      ++nodes;
+    }
+    a.cols = ldl_bcols_.p; a.lptr = ldl_bptr_.p; a.ptr = ldl_Lp_.p; a.idx = ldl_Li_.p; a.val = ldl_Lx_.p;
+    for (const ldl::Segment& s : ldl_bseg_) {
+      a.l0 = s.l0; a.l1 = s.l1;
+      ldl_backward_kernel<T><<<grid(ldl_bptr_h_, s), kBlock, 0, stream_>>>(a);
+      ++nodes;
+    }
+    CUDA_TRY(cudaStreamEndCapture(stream_, &g));
+    CUDA_TRY(cudaGraphInstantiate(&ldl_solve_graph_, g, 0));
+    CUDA_TRY(cudaGraphDestroy(g));
+    ldl_solve_nodes_ = nodes;
+  }
+  CUDA_TRY(cudaGraphLaunch(ldl_solve_graph_, stream_));
+  launches_ += ldl_solve_nodes_;
+}
+
+template <typename T>
+void Engine<T>::ldl_stats(double* o) {
+  o[0] = ldl_N_; o[1] = (double)ldl_nnzK_; o[2] = (double)ldl_nnzL_; o[3] = ldl_fptr_h_.empty() ? 0 : (double)ldl_fptr_h_.size() - 1;
+  o[4] = ldl_solve_nodes_; o[5] = (double)ldl_factorizations_; o[6] = ldl_factor_s_; o[7] = ldl_symbolic_s_;
 }
 
 template <typename T>
@@ -2365,6 +2563,38 @@ int cosmo_b200_psd_lambda_max(cosmo_b200_handle* h, const void* v, double* lam) 
 }
 int cosmo_b200_get_scaling(cosmo_b200_handle* h, void* D, void* E, double* c) {
   ABI_GUARD(h, h->impl->get_scaling(D, E, c));
+}
+int cosmo_b200_ldl_stats(cosmo_b200_handle* h, double out[8]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->ldl_stats(out));
+}
+int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* p, int64_t* perm, int64_t* parent, int64_t* colcount, int64_t* level) {
+  if (!p || !perm || !parent || !colcount || !level) { cosmo::g_create_error = "null argument"; return COSMO_B200_ERR_INVALID; }
+  try {
+    if (p->m < 0 || p->n < 0 || p->A.nrows != p->m || p->A.ncols != p->n || p->P.nrows != p->n || p->P.ncols != p->n)
+      throw cosmo::EngineError{COSMO_B200_ERR_INVALID, "P must be n x n and A m x n"};
+    cosmo::HostCsr a, at, pp, ppt;
+    if (p->dtype == COSMO_B200_F64) {
+      cosmo::csc_to_host_csrs<double>(p->A, p->index_base, a, at);
+      cosmo::csc_to_host_csrs<double>(p->P, p->index_base, pp, ppt);
+    } else if (p->dtype == COSMO_B200_F32) {
+      cosmo::csc_to_host_csrs<float>(p->A, p->index_base, a, at);
+      cosmo::csc_to_host_csrs<float>(p->P, p->index_base, pp, ppt);
+    } else {
+      throw cosmo::EngineError{COSMO_B200_ERR_UNSUPPORTED, "dtype must be Float64 or Float32"};
+    }
+    cosmo::ldl::Symbolic S;
+    cosmo::ldl::analyze((int)p->n, (int)p->m, pp.rowptr, pp.col, at.rowptr, at.col, S);
+    for (int j = 0; j < S.N; ++j) {
+      perm[j] = S.perm[j];
+      parent[j] = S.parent[j];
+      colcount[j] = S.Lp[j + 1] - S.Lp[j];
+      level[j] = S.level[j];
+    }
+    return COSMO_B200_OK;
+  } catch (const cosmo::EngineError& e) { cosmo::g_create_error = e.msg; return e.code; }
+  catch (const std::bad_alloc&) { cosmo::g_create_error = "host allocation failed"; return COSMO_B200_ERR_ALLOC; }
+  catch (...) { cosmo::g_create_error = "unknown error"; return COSMO_B200_ERR_INVALID; }
 }
 int cosmo_b200_comm_unique_id(void* id128) {
   if (!id128) return COSMO_B200_ERR_INVALID;

@@ -21,7 +21,7 @@ F64, F32 = 0, 1
 ZERO, NONNEG, BOX, SOC, PSD_SQUARE, PSD_TRIANGLE, EXP, DUAL_EXP, POW, DUAL_POW, PSD_TRIANGLE_COMPLEX = range(11)
 STATUS = {0: "Undetermined", 1: "Solved", 2: "Max_iter_reached", 3: "Time_limit_reached",
           4: "Primal_infeasible", 5: "Dual_infeasible", 6: "Unsolved"}
-KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES = 0, 1, 2
+KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES, KKT_LDL = 0, 1, 2, 3
 ACC_EMPTY, ACC_ANDERSON = 0, 1
 AA_TYPE2_QR, AA_TYPE2_NORMAL, AA_TYPE1 = 0, 1, 2
 AA_RESTARTED_MEMORY, AA_ROLLING_MEMORY = 0, 1
@@ -97,7 +97,7 @@ EXPORTS = [
     "cosmo_b200_comm_unique_id", "cosmo_b200_comm_init", "cosmo_b200_comm_p2p_export", "cosmo_b200_comm_p2p_attach",
     "cosmo_b200_tc_gemm_test", "cosmo_b200_psd_stats", "cosmo_b200_get_scaling",
     "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats", "cosmo_b200_infeasibility_test",
-    "cosmo_b200_psd_lambda_max",
+    "cosmo_b200_psd_lambda_max", "cosmo_b200_ldl_stats", "cosmo_b200_ldl_symbolic",
 ]
 
 _lib = None
@@ -149,6 +149,9 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_accelerator_stats.argtypes = [vp, C.POINTER(C.c_int64)]
     lib.cosmo_b200_infeasibility_test.argtypes = [vp, C.c_int32, vp, C.POINTER(C.c_double)]
     lib.cosmo_b200_psd_lambda_max.argtypes = [vp, vp, C.POINTER(C.c_double)]
+    lib.cosmo_b200_ldl_stats.argtypes = [vp, C.POINTER(C.c_double)]
+    i64p = C.POINTER(C.c_int64)
+    lib.cosmo_b200_ldl_symbolic.argtypes = [C.POINTER(ProblemStruct), i64p, i64p, i64p, i64p]
     lib.cosmo_b200_tc_gemm_test.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32,
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]
     for name in EXPORTS:
@@ -435,13 +438,52 @@ class Engine:
         self._check(self._lib.cosmo_b200_psd_lambda_max(self._h, _ptr(v), lam.ctypes.data_as(C.POINTER(C.c_double))))
         return lam[:self.n_psd]
 
+    def ldl_stats(self):
+        """State of the direct LDL' plugin (cosmo_b200_ldl_stats), keyed by LDL_STATS."""
+        out = (C.c_double * 8)()
+        self._check(self._lib.cosmo_b200_ldl_stats(self._h, out))
+        rec = dict(zip(LDL_STATS, list(out)))
+        for k in LDL_STATS[:6]:
+            rec[k] = int(rec[k])
+        return rec
+
 
 # cosmo_b200_infeasibility_test's out[8]: "gate2" is |Dinv A'dy|_inf (primal) or q'dx (dual), "gate3" dy'b of the
 # normalized -dy (primal) or |Dinv P dx|_inf (dual); "families" has bit 0 rows, 1 SOC, 2 PSD, 3 Exp/Pow
 INFEASIBILITY_RECORD = ("verdict", "gate", "norm", "gate2", "gate3", "box_sum", "families", "psd_unconverged")
 FAMILY_ROWS, FAMILY_SOC, FAMILY_PSD, FAMILY_C3 = 1, 2, 4, 8
 
+LDL_STATS = ("N", "nnz_triu_K", "nnz_L", "levels", "solve_nodes", "factorizations", "factor_time", "symbolic_time")
+
 ACCELERATOR_STATS = ("accepted", "declined", "rejected", "rho_restarts", "memory_restarts", "activated_at")
+
+
+def ldl_symbolic(P, A):
+    """cosmo_b200_ldl_symbolic: the host symbolic analysis of K = [P + sigma I, A'; A, -diag(1/rho)] (no GPU needed).
+    Returns (perm, parent, colcount, level), each of length n + m and in pivot order."""
+    import scipy.sparse as sp
+    lib = load_library()
+    P = sp.csc_matrix(P, dtype=np.float64)
+    A = sp.csc_matrix(A, dtype=np.float64)
+    P.sort_indices()
+    A.sort_indices()
+    m, n = A.shape
+    keep = []
+
+    def csc(M):
+        arrs = [np.ascontiguousarray(M.indptr, dtype=np.int64), np.ascontiguousarray(M.indices, dtype=np.int64),
+                np.ascontiguousarray(M.data, dtype=np.float64)]
+        keep.extend(arrs)
+        return CscStruct(M.shape[0], M.shape[1], _ptr(arrs[0]), _ptr(arrs[1]), _ptr(arrs[2]))
+
+    prob = ProblemStruct()
+    prob.dtype, prob.index_base, prob.m, prob.n = F64, 0, m, n
+    prob.P, prob.A = csc(P), csc(A)
+    out = [np.zeros(n + m, dtype=np.int64) for _ in range(4)]
+    rc = lib.cosmo_b200_ldl_symbolic(C.byref(prob), *[o.ctypes.data_as(C.POINTER(C.c_int64)) for o in out])
+    if rc != OK:
+        raise EngineError(rc, (lib.cosmo_b200_last_error(None) or b"").decode())
+    return tuple(out)
 
 
 def tc_gemm(A, B, slices=8, groups=0, reps=0):

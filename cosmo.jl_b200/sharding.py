@@ -107,6 +107,8 @@ def create_engine(shard: Shard, settings: M.Settings, device: int = 0, dist=None
                   dtype=np.float64) -> _eng.Engine:
     """Build the per-rank engine; with world > 1 rank 0 creates the ncclUniqueId and
     `torch.distributed` (the plumbing) broadcasts its 128 bytes."""
+    if shard.world > 1 and settings.kkt_solver == "DeviceLdlKKTSolver":
+        raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU (use CG or reduced MINRES when sharded)")
     tuples = [M.set_tuple(S) for S in shard.sets]
     eng = _eng.Engine(shard.P, shard.q, shard.A, shard.b, tuples, settings.to_struct(), D=D,
                       E=None if E is None else np.asarray(E)[shard.rows], c=c, dtype=dtype, device=device)

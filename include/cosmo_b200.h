@@ -111,7 +111,9 @@ typedef struct {
 enum {
   COSMO_B200_KKT_CG = 0,             /* CGIndirectKKTSolver      (reduced system, CG)      :3-88   */
   COSMO_B200_KKT_MINRES_REDUCED = 1, /* IndirectReducedKKTSolver(solver_type = :MINRES)    :3-88   */
-  COSMO_B200_KKT_MINRES = 2          /* MINRESIndirectKKTSolver  (full KKT, MINRES)        :90-162 */
+  COSMO_B200_KKT_MINRES = 2,         /* MINRESIndirectKKTSolver  (full KKT, MINRES)        :90-162 */
+  COSMO_B200_KKT_LDL = 3             /* direct LDL' of the full KKT matrix on the device, the counterpart of
+                                        QdldlKKTSolver (kktsolver.jl:285-320); single-GPU */
 };
 
 /* SparseMatrixCSC{T,Int64} as Julia stores it */
@@ -299,6 +301,23 @@ int cosmo_b200_infeasibility_test(cosmo_b200_handle* h, int32_t which, const voi
    the same prescaling and eigensolver path (shared-memory Jacobi up to N = 96, block Jacobi beyond); +inf where the
    eigensolver did not converge within psd_max_sweeps.  v has the m rows of this rank. */
 int cosmo_b200_psd_lambda_max(cosmo_b200_handle* h, const void* v, double* lam);
+
+/* ---- direct LDL' KKT plugin (kkt_solver = COSMO_B200_KKT_LDL) ------------- */
+/* K = [P + sigma I, A'; A, -diag(1/rho)] (N = n + m) is ordered by minimum degree and analysed on the host at create;
+   the factorisation (at create, then lazily before the first KKT solve after rho_vec or sigma changed: adapt_rho,
+   update_rho, reset, update_settings) and both triangular solves run on the device.  A factor that does not fit in
+   device memory fails the create with COSMO_B200_ERR_ALLOC; a factorisation with fewer or more than n positive pivots
+   fails with COSMO_B200_ERR_INVALID ("Objective function is not convex."), a zero or non-finite pivot with
+   COSMO_B200_ERR_NUMERICAL.  cosmo_b200_kkt_solve reports 0 inner iterations.
+   out = {N, nnz of the upper triangle of K, nnz of L (strictly lower), levels of the elimination tree, kernel launches
+   per solve, factorisations so far, device seconds of the last factorisation, host seconds of the symbolic analysis};
+   all 0 on a handle that never used the plugin. */
+int cosmo_b200_ldl_stats(cosmo_b200_handle* h, double out[8]);
+/* The symbolic analysis alone, on the host (no GPU needed).  Every array has N = n + m entries, in pivot order k:
+   perm[k] = original index of pivot k (x: 0..n-1, y: n..N-1), parent[k] = parent of k in the elimination tree of the
+   permuted K (-1: root), colcount[k] = entries of column k of L below the diagonal, level[k] = 0 for a leaf, else
+   1 + the largest level of its children.  Errors through cosmo_b200_last_error(NULL). */
+int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* prob, int64_t* perm, int64_t* parent, int64_t* colcount, int64_t* level);
 
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
