@@ -319,11 +319,8 @@ class Engine : public EngineBase {
   int cur_maxit_ = -1;
   // CUDA graphs of 1, 2, 4, 8 CG iterations (the inner loop is launch-bound for small problems)
   cudaGraphExec_t cg_graph_[4] = {nullptr, nullptr, nullptr, nullptr};
-  bool use_graphs_ = true;
-  bool graph_multi_ = true;
   // persistent cooperative CG kernel for launch-latency-bound (small / medium, non-windowed) problems
-  bool use_persistent_ = true;
-  int persist_grid_ = 0, persist_lanes_ = 0, persist_ctas_per_sm_ = 2;
+  int persist_grid_ = 0, persist_lanes_ = 0;
   DevBuf<T> persist_part_;
   long long persist_solves_ = 0;
   bool persistent_cg_ok();
@@ -358,8 +355,6 @@ class Engine : public EngineBase {
   DevBuf<T> vec_m_, vec_n_, vec_n2_, dy_, dx_, ypart_;
   DevBuf<unsigned> chunk_ticket_;
   int num_sms_ = 132;
-  bool use_windows_ = true;
-  int win_group_ = 16;
   DevBuf<T> sc_;       // device scalars
   DevBuf<int> isc_;
   DevBuf<T> partials_;
@@ -486,7 +481,7 @@ void Engine<T>::build_csr(DevCsr<T>& dst, const HostCsr& h) {
 // the gathers become (nearly) bank-conflict free.
 namespace {
 struct WinGroupScratch {
-  std::vector<int> cap, load, order;
+  std::vector<int> cap, load;
   std::vector<unsigned short> used;
   std::vector<std::vector<int>> members;
   std::vector<int> bucket[16];
@@ -495,8 +490,8 @@ struct WinGroupScratch {
 
 template <typename T>
 static void win_fill_segment(const int* cols, const double* vals, const int* idx, int k, int wbase, long long start,
-                             unsigned short* wc, T* wv, WinGroupScratch& S, int GL) {
-  // GL = lanes that share one shared-memory wavefront (16: half-warp, 8: quarter-warp)
+                             unsigned short* wc, T* wv, WinGroupScratch& S) {
+  constexpr int GL = 16;                // lanes that share one shared-memory wavefront: a half-warp
   const int kpad = (k + 7) & ~7;
   if (kpad == 0) return;
   const int lanes_total = kpad / 8;
@@ -574,7 +569,7 @@ static void win_fill_segment(const int* cols, const double* vals, const int* idx
 template <typename T>
 void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h) {
   dst.windowed = false;
-  if (!use_windows_ || h.nrows == 0 || h.ncols == 0) return;
+  if (h.nrows == 0 || h.ncols == 0) return;
   const long long nnz = (long long)h.col.size();
   const int Wmax = (int)(204800 / sizeof(T));
   const int nwin = (h.ncols + Wmax - 1) / Wmax;
@@ -631,7 +626,7 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h) {
       for (int k = h.rowptr[r]; k < h.rowptr[r + 1]; ++k) seg[h.col[k] / W].push_back(k);
       for (int w = 0; w < nwin; ++w)
         win_fill_segment<T>(h.col.data(), h.val.data(), seg[w].data(), (int)seg[w].size(), w * W,
-                            rp[(size_t)w * (nr + 1) + r], wc.data(), wv.data(), S, win_group_);
+                            rp[(size_t)w * (nr + 1) + r], wc.data(), wv.data(), S);
     }
   });
   // contiguous row chunks per CTA, balanced by padded nnz (+ per-row overhead)
@@ -747,20 +742,6 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   CUDA_TRY(cudaSetDevice(device_));
   CUDA_TRY(cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, device_));
   if (num_sms_ < 1 || num_sms_ > kMaxGrid) num_sms_ = 132;
-  {
-    const char* e = getenv("COSMO_B200_NO_WINDOWS");
-    use_windows_ = !(e && e[0] == '1');
-    const char* ng = getenv("COSMO_B200_NO_GRAPH");
-    use_graphs_ = !(ng && ng[0] == '1');
-    const char* np_ = getenv("COSMO_B200_NO_PERSISTENT");
-    use_persistent_ = !(np_ && np_[0] == '1');
-    const char* pc = getenv("COSMO_B200_PERSIST_CTAS");
-    if (pc && atoi(pc) > 0) persist_ctas_per_sm_ = atoi(pc);
-    const char* gm = getenv("COSMO_B200_GRAPH_MULTI");
-    graph_multi_ = !(gm && gm[0] == '0');
-    const char* g = getenv("COSMO_B200_WIN_GROUP");
-    if (g && atoi(g) == 8) win_group_ = 8;
-  }
   CUDA_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
   CUDA_TRY(cudaEventCreate(&ev0_));
   CUDA_TRY(cudaEventCreate(&ev1_));
@@ -1382,22 +1363,17 @@ void Engine<T>::kkt_cg(const int* done) {
   cg_init_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, rhsb_.p, cb_.p, r_.p, u_.p, red(SC_RES2),
                                                       CgInitFin<T>{sc_.p, isc_.p, (T)tol_num, p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
   check_launch("cg_init");
-  // NCCL collectives are capturable too; COSMO_B200_GRAPH_MULTI=0 restores eager launches when sharded
-  const bool graphs = use_graphs_ && (nranks_ == 1 || graph_multi_);
-  if (graphs && !cg_graph_[0]) build_cg_graphs(done);
+  // NCCL collectives are capturable too: sharded runs replay the same graphs
+  if (!cg_graph_[0]) build_cg_graphs(done);
   int chunk = std::max(last_cg_iters_, 0);
   for (;;) {
-    if (graphs) {
-      int left = chunk;
-      for (int b = 3; b >= 0; --b)
-        while (left >= (1 << b)) {
-          CUDA_TRY(cudaGraphLaunch(cg_graph_[b], stream_));
-          launches_ += (long long)(1 << b) * (At_.windowed && P_.nnz > 0 ? 5 : 4);
-          left -= (1 << b);
-        }
-    } else {
-      for (int i = 0; i < chunk; ++i) cg_iteration_launches(done);
-    }
+    int left = chunk;
+    for (int b = 3; b >= 0; --b)
+      while (left >= (1 << b)) {
+        CUDA_TRY(cudaGraphLaunch(cg_graph_[b], stream_));
+        launches_ += (long long)(1 << b) * (At_.windowed && P_.nnz > 0 ? 5 : 4);
+        left -= (1 << b);
+      }
     CUDA_TRY(cudaMemcpyAsync(h_isc_, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     if (h_isc_[ISC_DONE]) break;
@@ -1411,7 +1387,7 @@ void Engine<T>::kkt_cg(const int* done) {
 
 template <typename T>
 bool Engine<T>::persistent_cg_ok() {
-  if (!use_persistent_ || nranks_ != 1 || A_.windowed || At_.windowed) return false;
+  if (nranks_ != 1 || A_.windowed || At_.windowed) return false;
   const long long work = A_.nnz + At_.nnz + P_.nnz + 4LL * ((long long)n_ + m_);
   if (work > 6000000LL) return false;           // bigger problems are bandwidth-bound: separate kernels win
   if (persist_grid_ == 0) {
@@ -1427,7 +1403,7 @@ bool Engine<T>::persistent_cg_ok() {
     const long long per = kBlock / la;
     const long long need = std::max<long long>(1, (std::max(n_, m_) + per - 1) / per);
     // a grid barrier costs more the more CTAs take part: at most two CTAs per SM
-    persist_grid_ = (int)std::max<long long>(1, std::min<long long>(std::min<long long>((long long)nb, persist_ctas_per_sm_) * num_sms_, need));
+    persist_grid_ = (int)std::max<long long>(1, std::min<long long>(std::min<long long>((long long)nb, 2) * num_sms_, need));
     if (nb <= 0) { persist_grid_ = -1; return false; }
     persist_part_.alloc((size_t)persist_grid_ * 4);
   }
@@ -1636,7 +1612,6 @@ bool Engine<T>::primal_infeasible() {
   cone_rows_certificate_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, 0, dy_.p, row_class_.p, box_l_.p, box_u_.p, eps, red(SC_TMP1));
   check_launch("cone_cert_primal");
   // SOC: -v in K*  <=>  |v[2:]| <= tol - v[1]  ;  PSD: -V + tol I positive definite
-  T flag = 0;
   if (n_soc_) {
     soc_norms(dy_.p, soc_norm2_.p);
     soc_cert_kernel<T><<<1, kBlock, 0, stream_>>>(n_soc_, soc_off_.p, soc_norm2_.p, dy_.p, eps, sc_.p + SC_TMP3);
@@ -1651,7 +1626,6 @@ bool Engine<T>::primal_infeasible() {
     CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP5, 0, sizeof(T), stream_));
   }
   const bool psd_ok = psd_.certificate(dy_.p, /*negate=*/true, (double)eps, stream_, st_.psd_max_sweeps, launches_);
-  (void)flag;
   // the PSD verdict is a host bool of THIS rank: put it next to the device flags so that the
   // max-allreduce makes every rank take the same decision
   h_sc_[SC_TMP4] = psd_ok ? T(0) : T(1);
@@ -2408,7 +2382,7 @@ void Engine<T>::get_rho_vec(void* out) { download_vec(out, rho_vec_.p, m_); sync
 template <typename T>
 void Engine<T>::psd_stats(int64_t* o) {
   o[0] = psd_.tc_projections; o[1] = psd_.tc_fallbacks; o[2] = psd_.tc_.last_steps; o[3] = psd_.tc_.last_checks;
-  o[4] = psd_.sign_projections; o[5] = psd_.sign_fallbacks; o[6] = psd_.last_sweeps; o[7] = psd_.tc_.gemm.k;
+  o[4] = 0; o[5] = 0; o[6] = psd_.last_sweeps; o[7] = psd_.tc_.gemm.k;
 }
 template <typename T>
 void Engine<T>::get_w(void* out) { download_vec(out, W_[cur_].p, (size_t)n_ + m_); sync(); }

@@ -858,7 +858,6 @@ __global__ void psd_large_lammax_kernel(int N, const T* __restrict__ A, const do
 }
 
 }  // namespace cosmo
-#include "psd_sign.cuh"
 #include "psd_tc.cuh"
 namespace cosmo {
 
@@ -886,14 +885,9 @@ struct PsdBatch {
   bool warm_valid = false;
   int warm_N = 0;
   long long warm_count = 0;
-  bool warm_enabled = true;
   int last_sweeps = 0;
-  PsdSign<T> sign_;      // experimental GEMM-only projection (psd_sign.cuh), COSMO_B200_PSD_SIGN=1
-  bool sign_enabled = PsdSign<T>::enabled();
-  long long sign_projections = 0, sign_fallbacks = 0;
   PsdTc<T> tc_;          // tensor-core projection (psd_tc.cuh): Newton-Schulz on int8-sliced wgmma products
   bool tc_enabled = PsdTc<T>::enabled();
-  int tc_min_n = PsdTc<T>::min_n();
   long long tc_projections = 0, tc_fallbacks = 0;
   T* R_d = nullptr;      // npairs * 64 * 64 pivot rotations
   int* act_d = nullptr;  // per pair: pivot needed work this round
@@ -945,11 +939,7 @@ struct PsdBatch {
       ck(cudaMalloc(&rot_d, sizeof(int)), "cudaMalloc rot");
       ck(cudaMalloc(&mx_d, sizeof(unsigned long long)), "cudaMalloc psd max");
       ck(cudaMalloc(&up_d, sizeof(double)), "cudaMalloc psd scale");
-      {
-        const char* e = getenv("COSMO_B200_PSD_WARM");
-        warm_enabled = !(e && e[0] == '0');
-      }
-      if (large_h.size() == 1 && warm_enabled) {
+      if (large_h.size() == 1) {
         ck(cudaMalloc(&Vw_d, nn * sizeof(T)), "cudaMalloc psd Vw");
         ck(cudaMalloc(&T_d, nn * sizeof(T)), "cudaMalloc psd T");
       }
@@ -1056,7 +1046,7 @@ struct PsdBatch {
       ++launches;
     }
     for (const auto& d : large_h) {
-      if (tc_enabled && !sign_enabled && d.N >= tc_min_n) {
+      if (tc_enabled) {
         const int N = d.N;
         const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
         load_large(d, ws, st, launches);
@@ -1068,17 +1058,6 @@ struct PsdBatch {
         ++tc_fallbacks;
         if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd-tc] fallback to block Jacobi: %s\n", tc_.err.c_str());
         cudaGetLastError();
-      }
-      if (sign_enabled && d.triangle != 2) {   // experimental: Pi_+(X) = (X + sign(X) X) / 2 by Newton-Schulz products, no eigenvectors
-        const int N = d.N;
-        const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-        load_large(d, ws, st, launches);
-        if (sign_.project(d, A_d, fro_d, g, V_d, s, st, launches)) {
-          unscale_large(d, s, st, launches);
-          ++sign_projections;
-          continue;
-        }
-        ++sign_fallbacks;
       }
       large_eig(d, ws, st, max_sweeps, launches, /*allow_warm=*/true);
       const int N = d.N;
@@ -1144,13 +1123,6 @@ struct PsdBatch {
       ck(cudaStreamSynchronize(st), "sync");
       lam[large_idx[k]] = (double)l;
     }
-  }
-
-  bool failed(cudaStream_t st) {
-    int f = 0;
-    ck(cudaMemcpyAsync(&f, fail_d, sizeof(int), cudaMemcpyDeviceToHost, st), "copy fail");
-    ck(cudaStreamSynchronize(st), "sync");
-    return f != 0;
   }
 };
 

@@ -144,7 +144,7 @@ struct PsdTc {
   // rate, so a projection that needed more than sched_len + 6 steps was laid out too optimistically (l0 /= 10 and that
   // value is not tried again for 25 projections), one that finished on schedule lets every 2nd call probe l0 * 10.
   // Measured on config C4 (N = 2000): 24 / 21 / 19 / 22 / 25 steps for l0 = 1e-7 / 1e-6 / 1e-5 / 1e-4 / 1e-3.
-  double l0_cur = -1.0, l0_cap = 1e-2;
+  double l0_cur = 1e-7, l0_cap = 1e-2;
   int cap_hold = 0, good_streak = 0;
   static int sched_len(double l, double alpha_max) {
     int k = 0;
@@ -168,23 +168,16 @@ struct PsdTc {
     const char* e = getenv(name);
     return (e && *e) ? atoi(e) : def;
   }
-  static double env_double(const char* name, double def) {
-    const char* e = getenv(name);
-    return (e && *e) ? atof(e) : def;
-  }
   // COSMO_B200_PSD_TC=0 switches the tensor-core path off (block Jacobi for every large cone)
   static bool enabled() {
     const char* e = getenv("COSMO_B200_PSD_TC");
     return !(e && e[0] == '0');
   }
-  static int min_n() { return env_int("COSMO_B200_PSD_TC_MIN_N", 97); }   // measured: faster than block Jacobi from N = 100 on (2.1 vs 4.1 ms)
 
   bool ensure(int N, cudaStream_t st) {
     if (!configured) {
       // fp64 model: 8 slices, 10 groups (products exact to ~2^-56 of the row maxima); fp32 model: 6 slices, 8 groups (2^-42)
-      const int k = env_int("COSMO_B200_TC_SLICES", sizeof(T) == 8 ? 8 : 6);
-      const int g = env_int("COSMO_B200_TC_GROUPS", k == 8 ? 10 : (k == 7 ? 7 : k + 2));
-      if (!gemm.configure(k, g, st)) { err = gemm.err; return false; }
+      if (!gemm.configure(sizeof(T) == 8 ? 8 : 6, sizeof(T) == 8 ? 10 : 8, st)) { err = gemm.err; return false; }
       bool ok = cudaMalloc(&state_d, 8 * sizeof(double)) == cudaSuccess && cudaMalloc(&const_d, 8 * sizeof(double)) == cudaSuccess &&
                 cudaMalloc(&x2_d, sizeof(double)) == cudaSuccess && cudaMallocHost(&state_h, 8 * sizeof(double)) == cudaSuccess;
       if (!ok) { err = "PsdTc: cudaMalloc"; return false; }
@@ -227,11 +220,9 @@ struct PsdTc {
     if (!ensure(N, st)) return false;
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
     const int ntiles = gemm.ntiles;
-    const bool adapt = env_int("COSMO_B200_TC_ADAPT", 1) != 0;
-    if (l0_cur < 0.0 || !adapt) l0_cur = env_double("COSMO_B200_TC_L0", 1e-7);
     const double l0 = l0_cur;
     const double l_rearm = 1e-3;                         // a failed check re-arms the schedule for three more decades
-    const double alpha_max = env_double("COSMO_B200_TC_ALPHA_MAX", 1.5);
+    const double alpha_max = 1.5;                        // see the header
     const double tol = 1e-7;                              // quadratic convergence: the step after delta < tol reaches ~delta^2
     const double rtol = sizeof(T) == 8 ? 5e-13 : 1e-7;    // accepted weighted residual
     const int cap = env_int("COSMO_B200_TC_MAX_STEPS", 80);
@@ -305,17 +296,15 @@ struct PsdTc {
       prev = delta;
     }
     last_steps = it; last_checks = checks; last_delta = delta; last_resid = resid; last_phases = phases;
-    if (adapt) {
-      const bool on_schedule = (phases == 1) && it <= sched_len(l0, alpha_max) + 6;
-      if (on_schedule) {
-        if (cap_hold > 0 && --cap_hold == 0) l0_cap = 1e-2;
-        if (++good_streak >= 2) { good_streak = 0; l0_cur = std::min(l0 * 10.0, l0_cap); }
-      } else {
-        good_streak = 0;
-        l0_cap = std::max(l0 * 0.1, 1e-12);              // this optimism failed: stay below it for the next 25 projections
-        cap_hold = 25;
-        l0_cur = std::max(l0 * (phases > 1 ? 1e-2 : 0.1), 1e-12);
-      }
+    const bool on_schedule = (phases == 1) && it <= sched_len(l0, alpha_max) + 6;
+    if (on_schedule) {
+      if (cap_hold > 0 && --cap_hold == 0) l0_cap = 1e-2;
+      if (++good_streak >= 2) { good_streak = 0; l0_cur = std::min(l0 * 10.0, l0_cap); }
+    } else {
+      good_streak = 0;
+      l0_cap = std::max(l0 * 0.1, 1e-12);                // this optimism failed: stay below it for the next 25 projections
+      cap_hold = 25;
+      l0_cur = std::max(l0 * (phases > 1 ? 1e-2 : 0.1), 1e-12);
     }
     if (!have_P) {
       ok = ok && gemm.slice(S, slS, st);

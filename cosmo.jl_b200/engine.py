@@ -409,9 +409,8 @@ class Engine:
         """Which path projected the large PSD cones so far (cosmo_b200_psd_stats)."""
         out = (C.c_int64 * 8)()
         self._check(self._lib.cosmo_b200_psd_stats(self._h, out))
-        keys = ("tc_projections", "tc_fallbacks", "tc_last_steps", "tc_last_checks", "sign_projections", "sign_fallbacks",
-                "jacobi_last_sweeps", "tc_slices")
-        return dict(zip(keys, [int(v) for v in out]))
+        keys = ("tc_projections", "tc_fallbacks", "tc_last_steps", "tc_last_checks", None, None, "jacobi_last_sweeps", "tc_slices")
+        return {k: int(v) for k, v in zip(keys, out) if k}
 
     def accelerator_stats(self):
         """Accelerator events of the last solve (cosmo_b200_accelerator_stats), keyed by ACCELERATOR_STATS."""

@@ -17,8 +17,6 @@ import time
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Tuple, Union
 
-import os
-
 import numpy as np
 import scipy.sparse as sp
 
@@ -582,16 +580,10 @@ class Model:
                     self._x2 = np.concatenate([self.x, np.zeros(A2.shape[1] - self.n)])
                     self._s2, self._mu2 = np.zeros(A2.shape[0]), np.zeros(A2.shape[0])
             m2, n2 = A0.shape
-            host_ruiz = os.environ.get("COSMO_B200_HOST_RUIZ") == "1"
-            if st.scaling != 0 and host_ruiz:      # the NumPy restatement (kept for the sharded path and as a cross-check)
-                P, q, A, b, sets, D, E, c = ruiz_equilibrate(P0, q0, A0, b0, sets0, st)
-                self.engine = _eng.Engine(P, q, A, b, [set_tuple(S) for S in sets], st.to_struct(), D=D, E=E, c=c,
-                                          dtype=self.dtype, device=self.device)
-            else:
-                # scale_ruiz! runs on the device (csrc/ruiz.cuh): the engine ingests the unscaled data and hands D, E, c back
-                self.engine = _eng.Engine(P0, q0, A0, b0, [set_tuple(S) for S in sets0], st.to_struct(),
-                                          dtype=self.dtype, device=self.device, equilibrate=(st.scaling != 0))
-                D, E, c = self.engine.scaling() if st.scaling != 0 else (np.ones(n2), np.ones(m2), 1.0)
+            # scale_ruiz! runs on the device (csrc/ruiz.cuh): the engine ingests the unscaled data and hands D, E, c back
+            self.engine = _eng.Engine(P0, q0, A0, b0, [set_tuple(S) for S in sets0], st.to_struct(),
+                                      dtype=self.dtype, device=self.device, equilibrate=(st.scaling != 0))
+            D, E, c = self.engine.scaling() if st.scaling != 0 else (np.ones(n2), np.ones(m2), 1.0)
             self.D, self.E, self.c = D, E, c
         else:
             self.engine.update_settings(st.to_struct())

@@ -332,8 +332,8 @@ int cosmo_b200_comm_p2p_attach(cosmo_b200_handle* h, const void* blobs, int32_t 
 
 /* ---- diagnostics ---------------------------------------------------------- */
 /* Which path projected the large PSD cones (N > 96) so far: out = {tensor-core projections, tensor-core fallbacks to
-   block Jacobi, Newton-Schulz steps of the last one, weighted-residual checks of the last one, FP64-FMA sign
-   projections, their fallbacks, block-Jacobi sweeps of the last eigensolve, int8 slices per operand}. */
+   block Jacobi, Newton-Schulz steps of the last one, weighted-residual checks of the last one, 0, 0 (unused, always
+   zero), block-Jacobi sweeps of the last eigensolve, int8 slices per operand}. */
 int cosmo_b200_psd_stats(cosmo_b200_handle* h, int64_t out[8]);
 /* The product kernel of the large-cone PSD projection on its own: C = A B for symmetric, commuting N x N fp64
    matrices (column-major) through `k` int8 slices on wgmma (csrc/tc_gemm.cuh; the reference's counterpart is the

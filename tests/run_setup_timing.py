@@ -19,7 +19,3 @@ for scaling in (0, 10):
     t2 = time.perf_counter()
     print("scaling=%d make_shard %.3f s, Engine() %.3f s" % (scaling, t1 - t0, t2 - t1), flush=True)
     eng.close()
-if os.environ.get("HOST_RUIZ"):
-    t0 = time.perf_counter()
-    cosmo_b200.ruiz_equilibrate(P, q, A, b, sets, cosmo_b200.Settings())
-    print("host NumPy ruiz_equilibrate %.3f s" % (time.perf_counter() - t0))

@@ -1,8 +1,6 @@
-"""NumPy models of two device code paths that have not run on a GPU yet (DESIGN.md section 9), kept as CPU tests so
-that the claims "control flow validated in NumPy" / "index maps checked by emulation" stay reproducible:
+"""NumPy model of a device code path that has not run on a GPU yet (DESIGN.md section 9), kept as a CPU test so that
+the claim "index maps checked by emulation" stays reproducible:
 
-* csrc/psd_sign.cuh -- Pi_+(X) = (X + sign(X) X) / 2 by Newton-Schulz steps with the rigorous scaling
-  (|X|_F, then beta = |S^2|_F^(1/2) whenever beta < 1) and the stopping rules of PsdSign::project;
 * psd_small_kernel, d.triangle == 2 -- load / store index maps of the real embedding of a Hermitian matrix.
 
 The functions below follow the CUDA code statement by statement (same scalars, same tests, same order)."""
@@ -11,80 +9,6 @@ import math
 import numpy as np
 
 from oracle import cosmo_oracle as O
-
-
-def sign_project(X, tol=1e-7, rtol=5e-13, cap=64):
-    """PsdSign<double>::project"""
-    N = len(X)
-    fro = math.sqrt((X * X).sum())
-    S = X * (1.0 / fro if fro > 0 else 0.0)                     # sg_scale_kernel
-    prev, it, gemms, next_check, resid = 1e300, 0, 0, 24, None
-    while True:
-        T = S @ S                                               # sym_gemm_kernel<SG_SQ>
-        gemms += 1
-        f, d = (T * T).sum(), ((np.eye(N) - T) ** 2).sum()
-        if not (f > 0):                                         # sg_delta_kernel
-            delta, ib, ib2 = (0.0 if f == 0 else f), 1.0, 1.0
-        else:
-            beta = math.sqrt(math.sqrt(f))
-            if beta < 1:
-                delta, ib, ib2 = 2.0, 1.0 / beta, 1.0 / (beta * beta)
-            else:
-                delta, ib, ib2 = math.sqrt(d / N), 1.0, 1.0
-        S = 0.5 * ib * (3.0 * S - ib2 * (S @ T))                # sym_gemm_kernel<SG_UPD>
-        gemms += 1
-        it += 1
-        if delta != delta:
-            return None, it, gemms, resid
-        if delta < tol:
-            W = S @ X
-            gemms += 1
-            break
-        if (it >= next_check and delta > 0.98 * prev) or it >= cap:
-            W = S @ X                                           # SG_MUL
-            R = S @ W                                           # SG_RES
-            gemms += 2
-            resid = math.sqrt(((R - X) ** 2).sum()) / (fro if fro > 0 else 1.0)
-            if resid < rtol or (it >= cap and resid < 1e3 * rtol):
-                break
-            if it >= cap:
-                return None, it, gemms, resid                   # caller falls back to the eigensolver
-            next_check = it + 8
-        prev = delta
-    return 0.5 * (X + W), it, gemms, resid                      # sg_store_kernel
-
-
-def _ref(X):
-    w, V = np.linalg.eigh(X)
-    return (V * np.maximum(w, 0)) @ V.T
-
-
-def test_sign_function_projection_control_flow():
-    rng = np.random.default_rng(0)
-    B = rng.standard_normal((200, 200))
-    v = rng.standard_normal(120)
-    Q, _ = np.linalg.qr(rng.standard_normal((150, 150)))
-    spec = lambda lam: (Q * lam) @ Q.T   # noqa: E731
-    geo = 10.0 ** -np.arange(0, 15, 0.2)[:75]
-    cases = {
-        "wigner": ((B + B.T) / 2, 30, 2e-14),
-        "zero": (np.zeros((50, 50)), 1, 0.0),
-        "rank1_pos": (np.outer(v, v), 24, 2e-14),
-        "rank1_neg": (-np.outer(v, v), 24, 2e-14),
-        "zeros_in_spectrum": (spec(np.concatenate([np.linspace(1, 2, 50), np.zeros(50), -np.linspace(0.5, 3, 50)])), 24, 2e-14),
-        "identity": (3.0 * np.eye(64), 10, 2e-14),
-        "one_huge": (spec(np.concatenate([[1e6], rng.standard_normal(149)])), 60, 2e-14),
-        "one_tiny": (spec(np.concatenate([np.linspace(1, 2, 75), -np.linspace(1, 2, 74), [1e-9]])), 64, 2e-14),
-        "geometric_to_1e-15": (spec(np.concatenate([geo, -geo])), 64, 1e-11),
-    }
-    for name, (X, max_steps, bound) in cases.items():
-        X = (X + X.T) / 2
-        P, steps, gemms, resid = sign_project(X)
-        assert P is not None, name
-        nrm = np.linalg.norm(X) or 1.0
-        assert np.linalg.norm(P - _ref(X)) / nrm <= bound, (name, np.linalg.norm(P - _ref(X)) / nrm)
-        assert steps <= max_steps and gemms <= 2 * steps + 1 + 2 * max((steps - 24) // 8 + 2, 0), (name, steps, gemms)
-        assert np.allclose(P, P.T, atol=1e-12 * nrm)
 
 
 def _svec_pos(i, j):

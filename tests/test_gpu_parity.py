@@ -214,9 +214,8 @@ def test_project_psd_large_path(N):
 
 
 @pytest.mark.parametrize("kind", ["wigner", "rank_deficient", "shifted", "zero"])
-def test_project_psd_sign_function_path(kind, monkeypatch):
+def test_project_psd_tensor_core_path_n150(kind):
     # Pi_+(X) = (X + sign(X) X) / 2 with sign(X) by Newton-Schulz products; same bar as the eigensolver path
-    monkeypatch.setenv("COSMO_B200_PSD_SIGN", "1")
     rng = np.random.default_rng(21)
     N = 150
     B = rng.standard_normal((N, N))
@@ -237,6 +236,8 @@ def test_project_psd_sign_function_path(kind, monkeypatch):
     got = eng.project(ws)
     nrm = np.linalg.norm(ws) + 1e-300
     assert np.linalg.norm(got - ref) / nrm < 1e-12
+    st = eng.psd_stats()
+    assert st["tc_projections"] == 2 and st["tc_fallbacks"] == 0, st
 
 
 # ---------------------------------------------------------------------------

@@ -17,7 +17,7 @@ CASES = ["test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_t
          "test_accelerated_iterates_match_oracle", "test_accelerator_rho_adaption_limits", "test_g1_simple_qp",
          "test_g2_box_statuses", "test_g3_hs21_with_soc_and_merging", "test_g14_model_updates_and_warm_start",
          "test_project_composite_matches_oracle", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
-         "test_project_psd_sign_function_path",
+         "test_project_psd_tensor_core_path_n150",
          "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_soc_float32",
          "test_gpu_float32::test_project_exp_pow_cones_float32", "test_gpu_float32::test_project_psd_small_batch_float32",
          "test_gpu_float32::test_project_psd_tensor_core_path_float32_kinds", "test_gpu_float32::test_complex_psd_float32",
@@ -66,7 +66,6 @@ def _calls(fn):
 def test_gpu_test_body_runs_against_the_oracle_stand_in(name, monkeypatch):
     monkeypatch.setattr(M._eng, "Engine", OracleEngine)
     monkeypatch.setattr(E, "Engine", OracleEngine)
-    monkeypatch.setenv("COSMO_B200_TEST_EXPERIMENTAL", "1")
     module, _, func = name.rpartition("::")      # "module::test" for the other GPU modules, a bare name for the parity module
     T = importlib.import_module("tests." + (module or "test_gpu_parity"))
     fn = getattr(T, func)
