@@ -24,6 +24,7 @@
 
 #include "../../include/cosmo_b200.h"
 #include "common.cuh"
+#include "host.cuh"
 #include "psd.cuh"
 #include "cone3.cuh"
 #include "aa.cuh"
@@ -36,22 +37,6 @@
 namespace cosmo {
 
 static thread_local std::string g_create_error;
-
-struct EngineError {
-  int code;
-  std::string msg;
-};
-
-#define CUDA_TRY(expr)                                                                              \
-  do {                                                                                              \
-    cudaError_t _e = (expr);                                                                        \
-    if (_e != cudaSuccess) {                                                                        \
-      char _b[512];                                                                                 \
-      snprintf(_b, sizeof(_b), "CUDA error %s at %s:%d: %s", cudaGetErrorName(_e), __FILE__,        \
-               __LINE__, cudaGetErrorString(_e));                                                   \
-      throw EngineError{COSMO_B200_ERR_CUDA, _b};                                                   \
-    }                                                                                               \
-  } while (0)
 
 static inline double now_s() {
   return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
@@ -92,19 +77,13 @@ constexpr int kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2;
 // waits for a timer (one event synchronisation per kCap phases).
 struct PhaseTimer {
   static constexpr int kCap = 64;
-  cudaEvent_t a[kCap], b[kCap];
+  Event a[kCap], b[kCap];
   int n = 0;
-  bool created = false, on = false;
+  bool on = false;
   double total_ms = 0.0;
-  ~PhaseTimer() {
-    if (created) for (int i = 0; i < kCap; ++i) { cudaEventDestroy(a[i]); cudaEventDestroy(b[i]); }
-  }
   void enable(bool e) {
     on = e;
-    if (on && !created) {
-      for (int i = 0; i < kCap; ++i) { cudaEventCreate(&a[i]); cudaEventCreate(&b[i]); }
-      created = true;
-    }
+    if (on) for (int i = 0; i < kCap; ++i) { a[i].create(); b[i].create(); }
     n = 0; total_ms = 0.0;
   }
   void begin(cudaStream_t st) { if (on) cudaEventRecord(a[n], st); }
@@ -118,37 +97,6 @@ struct PhaseTimer {
     cudaEventSynchronize(b[n - 1]);
     for (int i = 0; i < n; ++i) { float ms = 0.f; cudaEventElapsedTime(&ms, a[i], b[i]); total_ms += ms; }
     n = 0;
-  }
-};
-
-// ---- device buffer -----------------------------------------------------------
-template <typename U>
-struct DevBuf {
-  U* p = nullptr;
-  size_t n = 0;
-  DevBuf() {}
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { if (p) cudaFree(p); }
-  void alloc(size_t count, bool zero = true) {
-    if (p) { cudaFree(p); p = nullptr; }
-    n = count;
-    size_t bytes = (count + 8) * sizeof(U);   // +8: bulk (TMA) copies round the tail up to 16 bytes
-    cudaError_t e = cudaMalloc(&p, bytes);
-    if (e != cudaSuccess) throw EngineError{COSMO_B200_ERR_ALLOC, std::string("cudaMalloc failed: ") + cudaGetErrorString(e)};
-    if (zero) {
-      // cudaMemset runs on the legacy default stream, which does NOT order against the engine's
-      // non-blocking stream: wait for it here or a later kernel may race with the pending fill.
-      CUDA_TRY(cudaMemset(p, 0, bytes));
-      CUDA_TRY(cudaDeviceSynchronize());
-    }
-  }
-  void upload(const U* host, size_t count, cudaStream_t st) {
-    if (count) CUDA_TRY(cudaMemcpyAsync(p, host, count * sizeof(U), cudaMemcpyHostToDevice, st));
-  }
-  void upload(const std::vector<U>& h, cudaStream_t st) {
-    if (n < h.size()) alloc(h.size(), false);
-    upload(h.data(), h.size(), st);
   }
 };
 
@@ -285,7 +233,7 @@ class Engine : public EngineBase {
   }
   // ---- accelerator (aa.cuh) ----
   DevBuf<T> aaG_, aaQ_, aaR_, aa_eta_, aa_glast_, aa_f_, aa_flast_, aa_sc_;
-  T* h_aa_ = nullptr;          // pinned mirror of aa_sc_
+  PinnedBuf<T> h_aa_;          // mirror of aa_sc_
   int aa_mem_ = 0;             // allocated history length (min(mem, dim)), 0 = not allocated
   int aa_iter_ = 0;            // columns filled since the last restart
   bool aa_init_ = true, aa_success_ = false, aa_active_ = false;
@@ -318,7 +266,7 @@ class Engine : public EngineBase {
   DevBuf<T> mr_[6], mr_x_, mr_c_, mr_b_;   // MINRES Lanczos / direction vectors, solution, operator output, rhs
   int cur_maxit_ = -1;
   // CUDA graphs of 1, 2, 4, 8 CG iterations (the inner loop is launch-bound for small problems)
-  cudaGraphExec_t cg_graph_[4] = {nullptr, nullptr, nullptr, nullptr};
+  GraphExec cg_graph_[4];
   // persistent cooperative CG kernel for launch-latency-bound (small / medium, non-windowed) problems
   int persist_grid_ = 0, persist_lanes_ = 0;
   DevBuf<T> persist_part_;
@@ -339,15 +287,12 @@ class Engine : public EngineBase {
   DevBuf<int64_t> ldl_Kp_, ldl_Ksp_, ldl_Ksrc_, ldl_Lp_, ldl_Rp_, ldl_Rmap_;
   DevBuf<int> ldl_Ki_, ldl_Li_, ldl_Rj_, ldl_fcols_, ldl_fptr_, ldl_bcols_, ldl_bptr_, ldl_perm_, ldl_flags_;
   DevBuf<T> ldl_Kx_, ldl_Lx_, ldl_Rx_, ldl_D_, ldl_Dinv_, ldl_ws_, ldl_y_;
-  cudaGraphExec_t ldl_factor_graph_ = nullptr, ldl_solve_graph_ = nullptr;
-  cudaEvent_t ldl_ev_[2] = {nullptr, nullptr};
+  GraphExec ldl_factor_graph_, ldl_solve_graph_;
+  Event ldl_ev_[2];
   void ldl_setup();
   void ldl_factor();
   void ldl_solve();
-  void destroy_ldl_factor_graph() {
-    if (ldl_factor_graph_) cudaGraphExecDestroy(ldl_factor_graph_);
-    ldl_factor_graph_ = nullptr;
-  }
+  void destroy_ldl_factor_graph() { ldl_factor_graph_.reset(); }
   long long kkt_counter_ = 1;   // S.iteration_counter
   int last_cg_iters_ = 1;
   long long total_inner_ = 0, total_mults_ = 0;
@@ -359,10 +304,10 @@ class Engine : public EngineBase {
   DevBuf<int> isc_;
   DevBuf<T> partials_;
   DevBuf<unsigned> ticket_;
-  T* h_sc_ = nullptr;  // pinned mirrors
-  int* h_isc_ = nullptr;
+  PinnedBuf<T> h_sc_;  // host mirrors
+  PinnedBuf<int> h_isc_;
   cudaStream_t stream_ = nullptr;
-  cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
+  Event ev0_, ev1_;
   long long launches_ = 0;
   // multi-GPU
   int nranks_ = 1, rank_ = 0;
@@ -429,7 +374,7 @@ class Engine : public EngineBase {
     check_launch("recover_mu");
   }
   void read_scalars(int first, int count) {
-    CUDA_TRY(cudaMemcpyAsync(h_sc_ + first, sc_.p + first, count * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+    CUDA_TRY(cudaMemcpyAsync(h_sc_.p + first, sc_.p + first, count * sizeof(T), cudaMemcpyDeviceToHost, stream_));
     sync();
   }
 };
@@ -743,10 +688,10 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   CUDA_TRY(cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, device_));
   if (num_sms_ < 1 || num_sms_ > kMaxGrid) num_sms_ = 132;
   CUDA_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-  CUDA_TRY(cudaEventCreate(&ev0_));
-  CUDA_TRY(cudaEventCreate(&ev1_));
-  CUDA_TRY(cudaMallocHost(&h_sc_, SC_COUNT * sizeof(T)));
-  CUDA_TRY(cudaMallocHost(&h_isc_, ISC_COUNT * sizeof(int)));
+  ev0_.create();
+  ev1_.create();
+  h_sc_.alloc(SC_COUNT);
+  h_isc_.alloc(ISC_COUNT);
 
   // ---- sets -> row tables -------------------------------------------------
   long long off = 0;
@@ -945,25 +890,13 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
 
 template <typename T>
 void Engine<T>::destroy_cg_graphs() {
-  for (auto& g : cg_graph_) {
-    if (g) cudaGraphExecDestroy(g);
-    g = nullptr;
-  }
+  for (auto& g : cg_graph_) g.reset();
 }
 
 template <typename T>
 Engine<T>::~Engine() {
-  destroy_cg_graphs();
-  destroy_ldl_factor_graph();
-  if (ldl_solve_graph_) cudaGraphExecDestroy(ldl_solve_graph_);
-  for (cudaEvent_t e : ldl_ev_) if (e) cudaEventDestroy(e);
   for (void* p : ipc_opened_) cudaIpcCloseMemHandle(p);
   if (comm_ && g_nccl.CommDestroy) g_nccl.CommDestroy(comm_);
-  if (h_sc_) cudaFreeHost(h_sc_);
-  if (h_isc_) cudaFreeHost(h_isc_);
-  if (h_aa_) cudaFreeHost(h_aa_);
-  if (ev0_) cudaEventDestroy(ev0_);
-  if (ev1_) cudaEventDestroy(ev1_);
   if (stream_) cudaStreamDestroy(stream_);
 }
 
@@ -1302,7 +1235,7 @@ template <typename T>
 void Engine<T>::set_maxit(int v) {
   if (cur_maxit_ == v) return;
   h_isc_[ISC_MAXIT] = v;
-  CUDA_TRY(cudaMemcpyAsync(isc_.p + ISC_MAXIT, h_isc_ + ISC_MAXIT, sizeof(int), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(cudaMemcpyAsync(isc_.p + ISC_MAXIT, h_isc_.p + ISC_MAXIT, sizeof(int), cudaMemcpyHostToDevice, stream_));
   sync();
   cur_maxit_ = v;
 }
@@ -1374,7 +1307,7 @@ void Engine<T>::kkt_cg(const int* done) {
         launches_ += (long long)(1 << b) * (At_.windowed && P_.nnz > 0 ? 5 : 4);
         left -= (1 << b);
       }
-    CUDA_TRY(cudaMemcpyAsync(h_isc_, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+    CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     if (h_isc_[ISC_DONE]) break;
     chunk = 1;
@@ -1449,14 +1382,8 @@ void Engine<T>::build_cg_graphs(const int* done) {
   cg_iteration_launches(done);
   sync();
   const long long saved = launches_;
-  for (int b = 0; b < 4; ++b) {
-    cudaGraph_t graph = nullptr;
-    CUDA_TRY(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-    for (int i = 0; i < (1 << b); ++i) cg_iteration_launches(done);
-    CUDA_TRY(cudaStreamEndCapture(stream_, &graph));
-    CUDA_TRY(cudaGraphInstantiate(&cg_graph_[b], graph, 0));
-    CUDA_TRY(cudaGraphDestroy(graph));
-  }
+  for (int b = 0; b < 4; ++b)
+    capture_graph(cg_graph_[b], stream_, [&] { for (int i = 0; i < (1 << b); ++i) cg_iteration_launches(done); });
   launches_ = saved;
 }
 
@@ -1515,7 +1442,7 @@ void Engine<T>::kkt_minres(bool full) {
       T* t = v_prev; v_prev = v_curr; v_curr = v_next; v_next = t;
       t = w_prev; w_prev = w_curr; w_curr = w_next; w_next = t;
     }
-    CUDA_TRY(cudaMemcpyAsync(h_isc_, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+    CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     if (h_isc_[ISC_DONE]) break;
     chunk = 1;
@@ -1629,7 +1556,7 @@ bool Engine<T>::primal_infeasible() {
   // the PSD verdict is a host bool of THIS rank: put it next to the device flags so that the
   // max-allreduce makes every rank take the same decision
   h_sc_[SC_TMP4] = psd_ok ? T(0) : T(1);
-  CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_ + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_.p + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
   if (nranks_ > 1) {
     allreduce_sum(sc_.p + SC_TMP0, 2);   // dy'b, box support sum
     allreduce_max(sc_.p + SC_TMP2, 4);   // flags: rows, SOC, PSD, Exp/Pow
@@ -1697,7 +1624,7 @@ bool Engine<T>::dual_infeasible() {
   }
   const bool psd_ok = psd_.certificate(vec_m_.p, /*negate=*/true, (double)eps, stream_, st_.psd_max_sweeps, launches_);
   h_sc_[SC_TMP4] = psd_ok ? T(0) : T(1);
-  CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_ + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_.p + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
   if (nranks_ > 1) allreduce_max(sc_.p + SC_TMP2, 4);
   read_scalars(SC_TMP2, 4);
   rec[6] = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) + (h_sc_[SC_TMP5] != 0 ? 8 : 0);
@@ -1720,7 +1647,7 @@ void Engine<T>::aa_prepare() {   // _make_accelerator!, setup.jl:10-14 (built on
     aaG_.alloc((size_t)dim * mem, false); aaQ_.alloc((size_t)dim * mem, false);
     aaR_.alloc((size_t)mem * mem); aa_eta_.alloc(32);
     aa_glast_.alloc(dim); aa_f_.alloc(dim); aa_flast_.alloc(dim); aa_sc_.alloc(AA_SC_COUNT);
-    if (!h_aa_) CUDA_TRY(cudaMallocHost(&h_aa_, AA_SC_COUNT * sizeof(T)));
+    if (!h_aa_.p) h_aa_.alloc(AA_SC_COUNT);
     aa_mem_ = mem;
   }
   if (aa_ne()) {
@@ -1792,7 +1719,7 @@ bool Engine<T>::aa_accelerate(T* g) {
   check_launch("aa_solve");
   aa_apply_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, g, aaG_.p, (size_t)dim, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
   check_launch("aa_apply");
-  CUDA_TRY(cudaMemcpyAsync(h_aa_ + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(h_aa_.p + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
   sync();
   if (h_aa_[AA_FLAG] == T(0)) { ++aa_rejected_; return false; }
   return true;
@@ -1855,7 +1782,7 @@ bool Engine<T>::aa_accelerate_ne(T* g) {
   if (!solve) return false;
   aa_apply_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, g, aaG_.p, (size_t)dim, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
   check_launch("aa_apply");
-  CUDA_TRY(cudaMemcpyAsync(h_aa_ + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(h_aa_.p + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
   sync();
   if (h_aa_[AA_FLAG] == T(0)) { ++aa_rejected_; return false; }
   return true;
@@ -2026,7 +1953,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
       aa_res_kernel<T><<<vgrid(dim), kBlock, 0, stream_>>>(dim, lo, W_[prev_].p, W_[cur_].p, aa_f_.p, red_ptr(aa_sc_.p + AA_FACC2));
       check_launch("aa_res");
       allreduce_sum(aa_sc_.p + AA_FACC2, 1);
-      CUDA_TRY(cudaMemcpyAsync(h_aa_, aa_sc_.p, 2 * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+      CUDA_TRY(cudaMemcpyAsync(h_aa_.p, aa_sc_.p, 2 * sizeof(T), cudaMemcpyDeviceToHost, stream_));
       sync();
       const double nrm_f = sqrt((double)h_aa_[AA_F2]), nrm_f_acc = sqrt((double)h_aa_[AA_FACC2]);
       if (nrm_f_acc > nrm_f * st_.safeguard_tol) {
@@ -2093,7 +2020,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
     status = COSMO_B200_MAX_ITER_REACHED;
   }
   if (persist_solves_ > 0) {   // inner-iteration statistics of the persistent CG kernel live on the device
-    CUDA_TRY(cudaMemcpyAsync(h_isc_ + ISC_TOTAL, isc_.p + ISC_TOTAL, sizeof(int), cudaMemcpyDeviceToHost, stream_));
+    CUDA_TRY(cudaMemcpyAsync(h_isc_.p + ISC_TOTAL, isc_.p + ISC_TOTAL, sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     total_inner_ += h_isc_[ISC_TOTAL];
     total_mults_ += h_isc_[ISC_TOTAL] + persist_solves_;
@@ -2159,7 +2086,7 @@ void Engine<T>::kkt_solve(const void* rhs, void* sol, int64_t* inner) {
   if (inner && st_.kkt_solver == COSMO_B200_KKT_LDL) {
     *inner = 0;
   } else if (inner) {
-    CUDA_TRY(cudaMemcpyAsync(h_isc_, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+    CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     *inner = h_isc_[ISC_IT];
   }
@@ -2215,9 +2142,10 @@ void Engine<T>::ldl_setup() {
   sync();
   ldl_fseg_ = S.fseg; ldl_bseg_ = S.bseg;
   ldl_fptr_h_ = S.fptr; ldl_bptr_h_ = S.bptr;
-  if (!ldl_ev_[0]) { CUDA_TRY(cudaEventCreate(&ldl_ev_[0])); CUDA_TRY(cudaEventCreate(&ldl_ev_[1])); }
+  ldl_ev_[0].create();
+  ldl_ev_[1].create();
   destroy_ldl_factor_graph();
-  if (ldl_solve_graph_) { cudaGraphExecDestroy(ldl_solve_graph_); ldl_solve_graph_ = nullptr; }
+  ldl_solve_graph_.reset();
   ldl_ready_ = true;
   ldl_dirty_ = true;
 }
@@ -2228,32 +2156,29 @@ template <typename T>
 void Engine<T>::ldl_factor() {
   if (!ldl_ready_) ldl_setup();
   if (!ldl_factor_graph_) {
-    cudaGraph_t g = nullptr;
-    CUDA_TRY(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
     int nodes = 0;
-    ldl_reset_flags_kernel<<<1, 32, 0, stream_>>>(ldl_flags_.p); ++nodes;
-    ldl_assemble_kernel<T><<<vgrid(ldl_nnzK_), kBlock, 0, stream_>>>(ldl_nnzK_, ldl_Ksp_.p, ldl_Ksrc_.p, P_.val.p, At_.val.p,
-                                                                     rho_vec_.p, (T)st_.sigma, ldl_Kx_.p);
-    ++nodes;
-    LdlFactorArgs<T> a;
-    a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p;
-    a.Kp = ldl_Kp_.p; a.Ki = ldl_Ki_.p; a.Kx = ldl_Kx_.p;
-    a.Lp = ldl_Lp_.p; a.Li = ldl_Li_.p; a.Lx = ldl_Lx_.p;
-    a.Rp = ldl_Rp_.p; a.Rj = ldl_Rj_.p; a.Rmap = ldl_Rmap_.p;
-    a.D = ldl_D_.p; a.Dinv = ldl_Dinv_.p; a.ws = ldl_ws_.p; a.N = ldl_N_; a.flags = ldl_flags_.p;
-    for (const ldl::Segment& s : ldl_fseg_) {
-      a.l0 = s.l0; a.l1 = s.l1;
-      const int grid = s.run ? 1 : std::min(ldl_fptr_h_[s.l1] - ldl_fptr_h_[s.l0], ldl_ws_ctas_);
-      ldl_factor_kernel<T><<<grid, kBlock, 0, stream_>>>(a);
+    capture_graph(ldl_factor_graph_, stream_, [&] {
+      ldl_reset_flags_kernel<<<1, 32, 0, stream_>>>(ldl_flags_.p); ++nodes;
+      ldl_assemble_kernel<T><<<vgrid(ldl_nnzK_), kBlock, 0, stream_>>>(ldl_nnzK_, ldl_Ksp_.p, ldl_Ksrc_.p, P_.val.p, At_.val.p,
+                                                                       rho_vec_.p, (T)st_.sigma, ldl_Kx_.p);
       ++nodes;
-    }
-    if (ldl_nnzL_) {
-      ldl_csr_gather_kernel<T><<<vgrid(ldl_nnzL_), kBlock, 0, stream_>>>(ldl_nnzL_, ldl_Rmap_.p, ldl_Lx_.p, ldl_Rx_.p);
-      ++nodes;
-    }
-    CUDA_TRY(cudaStreamEndCapture(stream_, &g));
-    CUDA_TRY(cudaGraphInstantiate(&ldl_factor_graph_, g, 0));
-    CUDA_TRY(cudaGraphDestroy(g));
+      LdlFactorArgs<T> a;
+      a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p;
+      a.Kp = ldl_Kp_.p; a.Ki = ldl_Ki_.p; a.Kx = ldl_Kx_.p;
+      a.Lp = ldl_Lp_.p; a.Li = ldl_Li_.p; a.Lx = ldl_Lx_.p;
+      a.Rp = ldl_Rp_.p; a.Rj = ldl_Rj_.p; a.Rmap = ldl_Rmap_.p;
+      a.D = ldl_D_.p; a.Dinv = ldl_Dinv_.p; a.ws = ldl_ws_.p; a.N = ldl_N_; a.flags = ldl_flags_.p;
+      for (const ldl::Segment& s : ldl_fseg_) {
+        a.l0 = s.l0; a.l1 = s.l1;
+        const int grid = s.run ? 1 : std::min(ldl_fptr_h_[s.l1] - ldl_fptr_h_[s.l0], ldl_ws_ctas_);
+        ldl_factor_kernel<T><<<grid, kBlock, 0, stream_>>>(a);
+        ++nodes;
+      }
+      if (ldl_nnzL_) {
+        ldl_csr_gather_kernel<T><<<vgrid(ldl_nnzL_), kBlock, 0, stream_>>>(ldl_nnzL_, ldl_Rmap_.p, ldl_Lx_.p, ldl_Rx_.p);
+        ++nodes;
+      }
+    });
     ldl_factor_nodes_ = nodes;
   }
   int flags[2] = {0, 0};
@@ -2284,29 +2209,26 @@ void Engine<T>::ldl_solve() {
   if (!ldl_ready_) ldl_setup();
   if (ldl_dirty_) ldl_factor();
   if (!ldl_solve_graph_) {
-    cudaGraph_t g = nullptr;
-    CUDA_TRY(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
     int nodes = 0;
-    LdlSolveArgs<T> a;
-    a.Dinv = ldl_Dinv_.p; a.perm = ldl_perm_.p; a.rhs = ls_.p; a.y = ldl_y_.p; a.out1 = xsol_.p; a.out2 = nu_.p; a.n = n_;
-    auto grid = [&](const std::vector<int>& ptr, const ldl::Segment& s) {
-      return s.run ? 1 : (int)std::min<long long>(((long long)ptr[s.l1] - ptr[s.l0] + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid);
-    };
-    a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p; a.ptr = ldl_Rp_.p; a.idx = ldl_Rj_.p; a.val = ldl_Rx_.p;
-    for (const ldl::Segment& s : ldl_fseg_) {
-      a.l0 = s.l0; a.l1 = s.l1;
-      ldl_forward_kernel<T><<<grid(ldl_fptr_h_, s), kBlock, 0, stream_>>>(a);
-      ++nodes;
-    }
-    a.cols = ldl_bcols_.p; a.lptr = ldl_bptr_.p; a.ptr = ldl_Lp_.p; a.idx = ldl_Li_.p; a.val = ldl_Lx_.p;
-    for (const ldl::Segment& s : ldl_bseg_) {
-      a.l0 = s.l0; a.l1 = s.l1;
-      ldl_backward_kernel<T><<<grid(ldl_bptr_h_, s), kBlock, 0, stream_>>>(a);
-      ++nodes;
-    }
-    CUDA_TRY(cudaStreamEndCapture(stream_, &g));
-    CUDA_TRY(cudaGraphInstantiate(&ldl_solve_graph_, g, 0));
-    CUDA_TRY(cudaGraphDestroy(g));
+    capture_graph(ldl_solve_graph_, stream_, [&] {
+      LdlSolveArgs<T> a;
+      a.Dinv = ldl_Dinv_.p; a.perm = ldl_perm_.p; a.rhs = ls_.p; a.y = ldl_y_.p; a.out1 = xsol_.p; a.out2 = nu_.p; a.n = n_;
+      auto grid = [&](const std::vector<int>& ptr, const ldl::Segment& s) {
+        return s.run ? 1 : (int)std::min<long long>(((long long)ptr[s.l1] - ptr[s.l0] + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid);
+      };
+      a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p; a.ptr = ldl_Rp_.p; a.idx = ldl_Rj_.p; a.val = ldl_Rx_.p;
+      for (const ldl::Segment& s : ldl_fseg_) {
+        a.l0 = s.l0; a.l1 = s.l1;
+        ldl_forward_kernel<T><<<grid(ldl_fptr_h_, s), kBlock, 0, stream_>>>(a);
+        ++nodes;
+      }
+      a.cols = ldl_bcols_.p; a.lptr = ldl_bptr_.p; a.ptr = ldl_Lp_.p; a.idx = ldl_Li_.p; a.val = ldl_Lx_.p;
+      for (const ldl::Segment& s : ldl_bseg_) {
+        a.l0 = s.l0; a.l1 = s.l1;
+        ldl_backward_kernel<T><<<grid(ldl_bptr_h_, s), kBlock, 0, stream_>>>(a);
+        ++nodes;
+      }
+    });
     ldl_solve_nodes_ = nodes;
   }
   CUDA_TRY(cudaGraphLaunch(ldl_solve_graph_, stream_));
@@ -2420,13 +2342,18 @@ struct cosmo_b200_handle {
   std::string err;
 };
 
+// The code of the exception in flight, its message into `msg`: call it from a catch block.
+static int error_code(std::string& msg) {
+  try { throw; }
+  catch (const cosmo::EngineError& e) { msg = e.msg; return e.code; }
+  catch (const std::bad_alloc&) { msg = "host allocation failed"; return COSMO_B200_ERR_ALLOC; }
+  catch (...) { msg = "unknown error"; return COSMO_B200_ERR_INVALID; }
+}
+
 #define ABI_GUARD(h, body)                                                   \
   if (!(h) || !(h)->impl) return COSMO_B200_ERR_INVALID;                     \
   try { body; return COSMO_B200_OK; }                                        \
-  catch (const cosmo::EngineError& e) { (h)->err = e.msg; return e.code; }   \
-  catch (const cosmo::PsdError& e) { (h)->err = e.msg; return COSMO_B200_ERR_NUMERICAL; } \
-  catch (const std::bad_alloc&) { (h)->err = "host allocation failed"; return COSMO_B200_ERR_ALLOC; } \
-  catch (...) { (h)->err = "unknown error"; return COSMO_B200_ERR_INVALID; }
+  catch (...) { return error_code((h)->err); }
 
 extern "C" {
 
@@ -2463,10 +2390,7 @@ int cosmo_b200_create(cosmo_b200_handle** out, const cosmo_b200_problem* prob, c
     h->impl = impl;
     *out = h;
     return COSMO_B200_OK;
-  } catch (const cosmo::EngineError& e) { cosmo::g_create_error = e.msg; return e.code; }
-  catch (const cosmo::PsdError& e) { cosmo::g_create_error = e.msg; return COSMO_B200_ERR_CUDA; }
-  catch (const std::bad_alloc&) { cosmo::g_create_error = "host allocation failed"; return COSMO_B200_ERR_ALLOC; }
-  catch (...) { cosmo::g_create_error = "unknown error"; return COSMO_B200_ERR_INVALID; }
+  } catch (...) { return error_code(cosmo::g_create_error); }
 }
 
 void cosmo_b200_destroy(cosmo_b200_handle* h) {
@@ -2566,18 +2490,18 @@ int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* p, int64_t* perm, int64_t*
       level[j] = S.level[j];
     }
     return COSMO_B200_OK;
-  } catch (const cosmo::EngineError& e) { cosmo::g_create_error = e.msg; return e.code; }
-  catch (const std::bad_alloc&) { cosmo::g_create_error = "host allocation failed"; return COSMO_B200_ERR_ALLOC; }
-  catch (...) { cosmo::g_create_error = "unknown error"; return COSMO_B200_ERR_INVALID; }
+  } catch (...) { return error_code(cosmo::g_create_error); }
 }
 int cosmo_b200_comm_unique_id(void* id128) {
   if (!id128) return COSMO_B200_ERR_INVALID;
-  std::string e;
-  if (!cosmo::g_nccl.load(e)) { cosmo::g_create_error = e; return COSMO_B200_ERR_NCCL; }
-  cosmo::NcclUniqueId id;
-  if (cosmo::g_nccl.GetUniqueId(&id) != 0) { cosmo::g_create_error = "ncclGetUniqueId failed"; return COSMO_B200_ERR_NCCL; }
-  memcpy(id128, &id, sizeof(id));
-  return COSMO_B200_OK;
+  try {
+    std::string e;
+    if (!cosmo::g_nccl.load(e)) throw cosmo::EngineError{COSMO_B200_ERR_NCCL, e};
+    cosmo::NcclUniqueId id;
+    if (cosmo::g_nccl.GetUniqueId(&id) != 0) throw cosmo::EngineError{COSMO_B200_ERR_NCCL, "ncclGetUniqueId failed"};
+    memcpy(id128, &id, sizeof(id));
+    return COSMO_B200_OK;
+  } catch (...) { return error_code(cosmo::g_create_error); }
 }
 int cosmo_b200_comm_init(cosmo_b200_handle* h, int32_t nranks, int32_t rank, const void* id128) {
   if (nranks > 1 && !id128) return COSMO_B200_ERR_INVALID;
@@ -2597,59 +2521,55 @@ int cosmo_b200_comm_p2p_attach(cosmo_b200_handle* h, const void* blobs, int32_t 
 int cosmo_b200_tc_gemm_test(int32_t N, int32_t k, int32_t kstep, int32_t gpb, const double* A, const double* B, double* C,
                             int32_t reps, double* ms_per_product, double* frob2) {
   if (N <= 0 || !A || !B || !C) return COSMO_B200_ERR_INVALID;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cosmo::g_create_error = "no CUDA device"; return COSMO_B200_ERR_CUDA; }
-  cudaStream_t st;
-  if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) return COSMO_B200_ERR_CUDA;
-  int rc = COSMO_B200_OK;
-  double *A_d = nullptr, *B_d = nullptr, *C_d = nullptr, *coef_d = nullptr, *part_d = nullptr;
-  {
-    cosmo::tc::OzakiGemm<double> g;
-    cosmo::tc::Sliced sa, sb;
+  (void)gpb;
+  cudaStream_t st = nullptr;
+  try {
+    using namespace cosmo;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw EngineError{COSMO_B200_ERR_CUDA, "no CUDA device"};
+    CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    tc::OzakiGemm<double> g;
+    tc::Sliced sa, sb;
+    DevBuf<double> A_d, B_d, C_d, coef_d, part_d;
     const size_t nn = (size_t)N * N;
     const double coef[3] = {1.0, 0.0, 0.0};
-    (void)gpb;
-    bool ok = g.configure(k, kstep > 0 ? kstep : (k == 8 ? 10 : (k == 7 ? 7 : k + 2)), st) && g.set_shape(N, st);
-    ok = ok && cudaMalloc(&A_d, nn * 8) == cudaSuccess && cudaMalloc(&B_d, nn * 8) == cudaSuccess && cudaMalloc(&C_d, nn * 8) == cudaSuccess &&
-         cudaMalloc(&coef_d, 3 * 8) == cudaSuccess && cudaMalloc(&part_d, (size_t)2 * (g.ntiles + 1) * 8) == cudaSuccess;
-    ok = ok && sa.ensure(g.Np) && sb.ensure(g.Np) && sa.clear(g.Np, st) && sb.clear(g.Np, st);
-    ok = ok && cudaMemcpyAsync(A_d, A, nn * 8, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-         cudaMemcpyAsync(B_d, B, nn * 8, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-         cudaMemcpyAsync(coef_d, coef, 3 * 8, cudaMemcpyHostToDevice, st) == cudaSuccess &&
-         cudaMemsetAsync(C_d, 0, nn * 8, st) == cudaSuccess;
-    ok = ok && g.slice(A_d, sa, st) && g.slice(B_d, sb, st);
-    ok = ok && g.gemm(sa, sb, C_d, nullptr, nullptr, 1, coef_d, part_d, st);
-    ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
-    if (ok && reps > 0 && ms_per_product) {
-      cudaEvent_t e0, e1;
-      cudaEventCreate(&e0); cudaEventCreate(&e1);
-      cudaEventRecord(e0, st);
-      for (int r = 0; r < reps && ok; ++r) ok = g.gemm(sa, sb, C_d, nullptr, nullptr, 1, coef_d, part_d, st);
-      cudaEventRecord(e1, st);
-      ok = ok && cudaEventSynchronize(e1) == cudaSuccess;
+    g.configure(k, kstep > 0 ? kstep : (k == 8 ? 10 : (k == 7 ? 7 : k + 2)));
+    g.set_shape(N, st);
+    A_d.alloc(nn, false); B_d.alloc(nn, false); C_d.alloc(nn, false); coef_d.alloc(3, false);
+    part_d.alloc((size_t)2 * (g.ntiles + 1), false);
+    sa.ensure(g.Np); sb.ensure(g.Np); sa.clear(g.Np, st); sb.clear(g.Np, st);
+    A_d.upload(A, nn, st); B_d.upload(B, nn, st); coef_d.upload(coef, 3, st);
+    CUDA_TRY(cudaMemsetAsync(C_d.p, 0, nn * 8, st));
+    g.slice(A_d.p, sa, st); g.slice(B_d.p, sb, st);
+    g.gemm(sa, sb, C_d.p, nullptr, nullptr, 1, coef_d.p, part_d.p, st);
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (reps > 0 && ms_per_product) {
+      Event e0, e1; e0.create(); e1.create();
+      CUDA_TRY(cudaEventRecord(e0, st));
+      for (int r = 0; r < reps; ++r) g.gemm(sa, sb, C_d.p, nullptr, nullptr, 1, coef_d.p, part_d.p, st);
+      CUDA_TRY(cudaEventRecord(e1, st));
+      CUDA_TRY(cudaEventSynchronize(e1));
       float ms = 0.f;
-      cudaEventElapsedTime(&ms, e0, e1);
+      CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
       *ms_per_product = ms / reps;
-      cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
-    ok = ok && cudaMemcpyAsync(C, C_d, nn * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess;
-    if (ok && frob2) {
+    CUDA_TRY(cudaMemcpyAsync(C, C_d.p, nn * 8, cudaMemcpyDeviceToHost, st));
+    if (frob2) {
       std::vector<double> part(2 * g.ntiles);
-      ok = cudaMemcpyAsync(part.data(), part_d, part.size() * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
-           cudaStreamSynchronize(st) == cudaSuccess;
+      CUDA_TRY(cudaMemcpyAsync(part.data(), part_d.p, part.size() * 8, cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
       frob2[0] = frob2[1] = 0.0;
       for (int i = 0; i < g.ntiles; ++i) { frob2[0] += part[2 * i]; frob2[1] += part[2 * i + 1]; }
     }
-    ok = ok && cudaStreamSynchronize(st) == cudaSuccess;
-    if (!ok) {
-      cudaError_t e = cudaGetLastError();
-      cosmo::g_create_error = "tc_gemm_test: " + (g.err.empty() ? std::string(cudaGetErrorString(e)) : g.err);
-      rc = COSMO_B200_ERR_CUDA;
-    }
+    CUDA_TRY(cudaStreamSynchronize(st));
+  } catch (...) {
+    if (st) cudaStreamDestroy(st);
+    const int rc = error_code(cosmo::g_create_error);
+    cosmo::g_create_error = "tc_gemm_test: " + cosmo::g_create_error;
+    return rc;
   }
-  cudaFree(A_d); cudaFree(B_d); cudaFree(C_d); cudaFree(coef_d); cudaFree(part_d);
   cudaStreamDestroy(st);
-  return rc;
+  return COSMO_B200_OK;
 }
 
 }  // extern "C"

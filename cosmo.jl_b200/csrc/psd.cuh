@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "host.cuh"
 
 namespace cosmo {
 
@@ -864,24 +865,22 @@ namespace cosmo {
 // ---------------------------------------------------------------------------
 // Host-side batch object
 // ---------------------------------------------------------------------------
-struct PsdError { std::string msg; };
-
 template <typename T>
 struct PsdBatch {
   std::vector<PsdConeDesc> small_h, large_h;
-  PsdConeDesc* small_d = nullptr;
-  T* lam_small_d = nullptr;
-  int* fail_d = nullptr;
+  DevBuf<PsdConeDesc> small_d;
+  DevBuf<T> lam_small_d;
+  DevBuf<int> fail_d;
   int small_maxN = 0;
   // large-cone workspace (sized for the largest cone, cones processed one after another)
   int large_maxN = 0;
-  T *A_d = nullptr, *V_d = nullptr, *cs_d = nullptr, *fro_d = nullptr, *thr_d = nullptr, *lam_large_d = nullptr;
-  int* rot_d = nullptr;
-  int* rot_h = nullptr;  // pinned
-  unsigned long long* mx_d = nullptr;   // max |entry| of the cone being projected (psd_cone_max_kernel)
-  double* up_d = nullptr;               // 2^pe: the prescaling of that cone (psd_large_load_kernel)
+  DevBuf<T> A_d, V_d, cs_d, fro_d, thr_d, lam_large_d;
+  DevBuf<int> rot_d;
+  PinnedBuf<int> rot_h;
+  DevBuf<unsigned long long> mx_d;   // max |entry| of the cone being projected (psd_cone_max_kernel)
+  DevBuf<double> up_d;               // 2^pe: the prescaling of that cone (psd_large_load_kernel)
   // warm start across ADMM iterations (single large cone): eigenvectors of the previous projection
-  T *Vw_d = nullptr, *T_d = nullptr;
+  DevBuf<T> Vw_d, T_d;
   bool warm_valid = false;
   int warm_N = 0;
   long long warm_count = 0;
@@ -889,24 +888,14 @@ struct PsdBatch {
   PsdTc<T> tc_;          // tensor-core projection (psd_tc.cuh): Newton-Schulz on int8-sliced wgmma products
   bool tc_enabled = PsdTc<T>::enabled();
   long long tc_projections = 0, tc_fallbacks = 0;
-  T* R_d = nullptr;      // npairs * 64 * 64 pivot rotations
-  int* act_d = nullptr;  // per pair: pivot needed work this round
+  DevBuf<T> R_d;         // npairs * 64 * 64 pivot rotations
+  DevBuf<int> act_d;     // per pair: pivot needed work this round
   std::vector<T> lam_host;
   std::vector<int> small_idx, large_idx;   // position of each small / large cone among all PSD cones (set order)
   std::vector<double> lam_all;
   int cert_unconverged = 0;                // cones whose eigensolver missed max_sweeps in the last lambda_max call
 
-  ~PsdBatch() {
-    cudaFree(small_d); cudaFree(lam_small_d); cudaFree(fail_d); cudaFree(A_d); cudaFree(V_d); cudaFree(cs_d);
-    cudaFree(fro_d); cudaFree(thr_d); cudaFree(lam_large_d); cudaFree(rot_d); cudaFree(R_d); cudaFree(act_d); cudaFree(Vw_d); cudaFree(T_d);
-    cudaFree(mx_d); cudaFree(up_d);
-    if (rot_h) cudaFreeHost(rot_h);
-  }
   bool empty() const { return small_h.empty() && large_h.empty(); }
-
-  static void ck(cudaError_t e, const char* what) {
-    if (e != cudaSuccess) throw PsdError{std::string(what) + ": " + cudaGetErrorString(e)};
-  }
 
   void init(const std::vector<PsdConeDesc>& descs, cudaStream_t st) {
     for (size_t k = 0; k < descs.size(); ++k) {
@@ -916,45 +905,34 @@ struct PsdBatch {
     }
     if (!small_h.empty()) {
       for (const auto& d : small_h) small_maxN = std::max(small_maxN, d.N);
-      ck(cudaMalloc(&small_d, small_h.size() * sizeof(PsdConeDesc)), "cudaMalloc psd descs");
-      ck(cudaMemcpyAsync(small_d, small_h.data(), small_h.size() * sizeof(PsdConeDesc), cudaMemcpyHostToDevice, st), "copy psd descs");
-      ck(cudaMalloc(&lam_small_d, small_h.size() * sizeof(T)), "cudaMalloc lam");
+      small_d.upload(small_h, st);
+      lam_small_d.alloc(small_h.size(), false);
       // the attribute belongs to the function on the device, not to this engine: always raise it to the worst case
       // of kPsdSmallMax, or a second engine with smaller cones would lower the limit under a live one
       const size_t ld_max = (size_t)(kPsdSmallMax | 1);
       const size_t smem = (2 * ld_max * kPsdSmallMax + 2 * (size_t)(kPsdSmallMax / 2 + 2)) * sizeof(T);
-      ck(cudaFuncSetAttribute(psd_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "smem attr");
+      CUDA_TRY(cudaFuncSetAttribute(psd_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    ck(cudaMalloc(&fail_d, sizeof(int)), "cudaMalloc fail flag");
-    ck(cudaMemsetAsync(fail_d, 0, sizeof(int), st), "memset");
+    fail_d.alloc(1, false);
+    CUDA_TRY(cudaMemsetAsync(fail_d.p, 0, sizeof(int), st));
     if (!large_h.empty()) {
       for (const auto& d : large_h) large_maxN = std::max(large_maxN, d.N);
       const size_t nn = (size_t)large_maxN * large_maxN;
-      ck(cudaMalloc(&A_d, nn * sizeof(T)), "cudaMalloc psd A");
-      ck(cudaMalloc(&V_d, nn * sizeof(T)), "cudaMalloc psd V");
-      ck(cudaMalloc(&cs_d, (size_t)(large_maxN + 2) * sizeof(T)), "cudaMalloc cs");
-      ck(cudaMalloc(&fro_d, kMaxGrid * sizeof(T)), "cudaMalloc fro");
-      ck(cudaMalloc(&thr_d, sizeof(T)), "cudaMalloc thr");
-      ck(cudaMalloc(&lam_large_d, large_h.size() * sizeof(T)), "cudaMalloc lam");
-      ck(cudaMalloc(&rot_d, sizeof(int)), "cudaMalloc rot");
-      ck(cudaMalloc(&mx_d, sizeof(unsigned long long)), "cudaMalloc psd max");
-      ck(cudaMalloc(&up_d, sizeof(double)), "cudaMalloc psd scale");
-      if (large_h.size() == 1) {
-        ck(cudaMalloc(&Vw_d, nn * sizeof(T)), "cudaMalloc psd Vw");
-        ck(cudaMalloc(&T_d, nn * sizeof(T)), "cudaMalloc psd T");
-      }
-      ck(cudaMallocHost(&rot_h, sizeof(int)), "cudaMallocHost rot");
+      A_d.alloc(nn, false); V_d.alloc(nn, false); cs_d.alloc(large_maxN + 2, false); fro_d.alloc(kMaxGrid, false);
+      thr_d.alloc(1, false); lam_large_d.alloc(large_h.size(), false); rot_d.alloc(1, false); rot_h.alloc(1);
+      mx_d.alloc(1, false); up_d.alloc(1, false);
+      if (large_h.size() == 1) { Vw_d.alloc(nn, false); T_d.alloc(nn, false); }
       int Nb = (large_maxN + kBjB - 1) / kBjB;
       if (Nb & 1) ++Nb;
-      ck(cudaMalloc(&R_d, (size_t)(Nb / 2) * kBjP * kBjP * sizeof(T)), "cudaMalloc R");
-      ck(cudaMalloc(&act_d, (size_t)(Nb / 2) * sizeof(int)), "cudaMalloc act");
+      R_d.alloc((size_t)(Nb / 2) * kBjP * kBjP, false);
+      act_d.alloc(Nb / 2, false);
       const int smem_pivot = (int)((2 * (size_t)(kBjP + 1) * kBjP + kBjP + 2) * sizeof(T));
       const int smem_upd = (int)(((size_t)kBjP * kBjP + (size_t)kBjTilesPerCta * kBjLd * kBjP) * sizeof(T));
-      ck(cudaFuncSetAttribute(bj_pivot_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_pivot), "smem attr pivot");
-      ck(cudaFuncSetAttribute(bj_cols_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_upd), "smem attr cols");
-      ck(cudaFuncSetAttribute(bj_rows_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_upd), "smem attr rows");
+      CUDA_TRY(cudaFuncSetAttribute(bj_pivot_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_pivot));
+      CUDA_TRY(cudaFuncSetAttribute(bj_cols_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_upd));
+      CUDA_TRY(cudaFuncSetAttribute(bj_rows_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_upd));
     }
-    ck(cudaStreamSynchronize(st), "sync");
+    CUDA_TRY(cudaStreamSynchronize(st));
   }
   size_t small_smem() const {
     const size_t ld = (size_t)(small_maxN | 1);
@@ -969,19 +947,19 @@ struct PsdBatch {
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
     const long long dim = psd_cone_dim(d);
     const int gm = (int)std::min<long long>((dim + kBlock - 1) / kBlock, kMaxGrid);
-    ck(cudaMemsetAsync(mx_d, 0, sizeof(unsigned long long), st), "memset psd max");
-    psd_cone_max_kernel<T><<<gm, kBlock, 0, st>>>(ws + d.off, dim, mx_d);
-    psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, upper ? 1 : 0, ws, A_d, V_d, fro_d, mx_d, up_d);
+    CUDA_TRY(cudaMemsetAsync(mx_d.p, 0, sizeof(unsigned long long), st));
+    psd_cone_max_kernel<T><<<gm, kBlock, 0, st>>>(ws + d.off, dim, mx_d.p);
+    psd_large_load_kernel<T><<<g, kBlock, 0, st>>>(d, upper ? 1 : 0, ws, A_d.p, V_d.p, fro_d.p, mx_d.p, up_d.p);
     launches += 2;
   }
   void unscale_large(const PsdConeDesc& d, T* s, cudaStream_t st, long long& launches) {
     const long long dim = psd_cone_dim(d);
-    psd_unscale_kernel<T><<<(int)std::min<long long>((dim + kBlock - 1) / kBlock, kMaxGrid), kBlock, 0, st>>>(s + d.off, dim, up_d);
+    psd_unscale_kernel<T><<<(int)std::min<long long>((dim + kBlock - 1) / kBlock, kMaxGrid), kBlock, 0, st>>>(s + d.off, dim, up_d.p);
     ++launches;
   }
 
   // eigen-decompose one large cone into A_d (diagonal = eigenvalues) and V_d (block Jacobi).  certificate: load a
-  // square cone from its upper triangle and return false instead of throwing PsdError when max_sweeps is not enough.
+  // square cone from its upper triangle and return false instead of throwing ERR_NUMERICAL when max_sweeps is not enough.
   bool large_eig(const PsdConeDesc& d, const T* ws, cudaStream_t st, int max_sweeps, long long& launches,
                  bool allow_warm = false, bool certificate = false) {
     const int N = d.N;
@@ -990,17 +968,17 @@ struct PsdBatch {
     const int npairs = Nb / 2;
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
     load_large(d, ws, st, launches, certificate);
-    psd_large_thr_kernel<T><<<1, 32, 0, st>>>(fro_d, g, thr_d, rot_d);
+    psd_large_thr_kernel<T><<<1, 32, 0, st>>>(fro_d.p, g, thr_d.p, rot_d.p);
     ++launches;
     // Warm start (ADMM iterates move slowly): rotate X into the eigenbasis of the previous projection,
     // A <- V0' X V0 is then nearly diagonal and a couple of sweeps finish the job; V starts at V0.
     // A cold start every 16th call bounds the drift of V's orthogonality.
-    const bool warm = allow_warm && Vw_d && warm_valid && warm_N == N && (warm_count % 16 != 0);
+    const bool warm = allow_warm && Vw_d.p && warm_valid && warm_N == N && (warm_count % 16 != 0);
     if (warm) {
       dim3 gg((N + 127) / 128, (N + 127) / 128);
-      bj_gemm_kernel<T, false><<<gg, kBlock, 0, st>>>(N, A_d, Vw_d, T_d);     // T = X V0
-      bj_gemm_kernel<T, true><<<gg, kBlock, 0, st>>>(N, Vw_d, T_d, A_d);      // A = V0' T
-      ck(cudaMemcpyAsync(V_d, Vw_d, (size_t)N * N * sizeof(T), cudaMemcpyDeviceToDevice, st), "copy V0");
+      bj_gemm_kernel<T, false><<<gg, kBlock, 0, st>>>(N, A_d.p, Vw_d.p, T_d.p);     // T = X V0
+      bj_gemm_kernel<T, true><<<gg, kBlock, 0, st>>>(N, Vw_d.p, T_d.p, A_d.p);      // A = V0' T
+      CUDA_TRY(cudaMemcpyAsync(V_d.p, Vw_d.p, (size_t)N * N * sizeof(T), cudaMemcpyDeviceToDevice, st));
       launches += 2;
     }
     const size_t smem_pivot = (2 * (size_t)(kBjP + 1) * kBjP + kBjP + 2) * sizeof(T);
@@ -1010,25 +988,25 @@ struct PsdBatch {
     int sweep = 0;
     for (; sweep < max_sweeps && !converged; ++sweep) {
       for (int r = 0; r < Nb - 1; ++r) {
-        bj_pivot_kernel<T><<<npairs, 512, smem_pivot, st>>>(N, Nb, r, A_d, thr_d, R_d, act_d, rot_d, 1);
-        bj_cols_kernel<T><<<dim3(tiles, npairs, 2), kBlock, smem_upd, st>>>(N, Nb, r, A_d, V_d, R_d, act_d);
-        bj_rows_kernel<T><<<dim3(tiles, npairs, 1), kBlock, smem_upd, st>>>(N, Nb, r, A_d, R_d, act_d);
+        bj_pivot_kernel<T><<<npairs, 512, smem_pivot, st>>>(N, Nb, r, A_d.p, thr_d.p, R_d.p, act_d.p, rot_d.p, 1);
+        bj_cols_kernel<T><<<dim3(tiles, npairs, 2), kBlock, smem_upd, st>>>(N, Nb, r, A_d.p, V_d.p, R_d.p, act_d.p);
+        bj_rows_kernel<T><<<dim3(tiles, npairs, 1), kBlock, smem_upd, st>>>(N, Nb, r, A_d.p, R_d.p, act_d.p);
         launches += 3;
       }
-      ck(cudaMemcpyAsync(rot_h, rot_d, sizeof(int), cudaMemcpyDeviceToHost, st), "copy rot");
-      ck(cudaMemsetAsync(rot_d, 0, sizeof(int), st), "memset rot");
-      ck(cudaStreamSynchronize(st), "sync");
-      if (*rot_h == 0) converged = true;
+      CUDA_TRY(cudaMemcpyAsync(rot_h.p, rot_d.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaMemsetAsync(rot_d.p, 0, sizeof(int), st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      if (rot_h[0] == 0) converged = true;
     }
     last_sweeps = sweep;
     if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd] N=%d warm=%d sweeps=%d\n", N, (int)warm, sweep);
-    ck(cudaGetLastError(), "psd block-Jacobi kernels");
+    CUDA_TRY(cudaGetLastError());
     if (!converged) {
       if (certificate) return false;
-      throw PsdError{"block Jacobi eigensolver did not converge within psd_max_sweeps"};
+      throw EngineError{COSMO_B200_ERR_NUMERICAL, "block Jacobi eigensolver did not converge within psd_max_sweeps"};
     }
-    if (allow_warm && Vw_d) {
-      ck(cudaMemcpyAsync(Vw_d, V_d, (size_t)N * N * sizeof(T), cudaMemcpyDeviceToDevice, st), "save V0");
+    if (allow_warm && Vw_d.p) {
+      CUDA_TRY(cudaMemcpyAsync(Vw_d.p, V_d.p, (size_t)N * N * sizeof(T), cudaMemcpyDeviceToDevice, st));
       warm_valid = true;
       warm_N = N;
       ++warm_count;
@@ -1041,8 +1019,8 @@ struct PsdBatch {
     if (empty()) return;
     if (max_sweeps <= 0) max_sweeps = 30;
     if (!small_h.empty()) {
-      psd_small_kernel<T><<<(int)small_h.size(), kBlock, small_smem(), st>>>(small_d, ws, s, 0, lam_small_d, max_sweeps, fail_d);
-      ck(cudaGetLastError(), "psd_small_kernel");
+      psd_small_kernel<T><<<(int)small_h.size(), kBlock, small_smem(), st>>>(small_d.p, ws, s, 0, lam_small_d.p, max_sweeps, fail_d.p);
+      CUDA_TRY(cudaGetLastError());
       ++launches;
     }
     for (const auto& d : large_h) {
@@ -1050,32 +1028,30 @@ struct PsdBatch {
         const int N = d.N;
         const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
         load_large(d, ws, st, launches);
-        if (tc_.project(d, A_d, fro_d, g, V_d, s, st, launches)) {
+        if (tc_.project(d, A_d.p, fro_d.p, g, V_d.p, s, st, launches)) {
           unscale_large(d, s, st, launches);
           ++tc_projections;
           continue;
         }
         ++tc_fallbacks;
-        if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd-tc] fallback to block Jacobi: %s\n", tc_.err.c_str());
-        cudaGetLastError();
       }
       large_eig(d, ws, st, max_sweeps, launches, /*allow_warm=*/true);
       const int N = d.N;
       const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-      psd_large_scale_kernel<T><<<g, kBlock, 0, st>>>(N, A_d, V_d);
+      psd_large_scale_kernel<T><<<g, kBlock, 0, st>>>(N, A_d.p, V_d.p);
       dim3 gt((N + 31) / 32, (N + 31) / 32);
       if (d.triangle == 2) {
         // Hermitian cone: reconstruct the projected embedding as a square matrix in A_d (its eigenvalues are no longer
         // needed), then read A+ and B+ off its blocks
         const PsdConeDesc sq{0, N, 0};
-        psd_large_syrk_kernel<T><<<gt, 256, 0, st>>>(sq, V_d, A_d);
-        psd_embedding_store_kernel<T, T><<<g, kBlock, 0, st>>>(d, A_d, s);
+        psd_large_syrk_kernel<T><<<gt, 256, 0, st>>>(sq, V_d.p, A_d.p);
+        psd_embedding_store_kernel<T, T><<<g, kBlock, 0, st>>>(d, A_d.p, s);
         ++launches;
       } else {
-        psd_large_syrk_kernel<T><<<gt, 256, 0, st>>>(d, V_d, s);
+        psd_large_syrk_kernel<T><<<gt, 256, 0, st>>>(d, V_d.p, s);
       }
       unscale_large(d, s, st, launches);
-      ck(cudaGetLastError(), "psd large reconstruct");
+      CUDA_TRY(cudaGetLastError());
       launches += 2;
     }
   }
@@ -1098,15 +1074,15 @@ struct PsdBatch {
     if (max_sweeps <= 0) max_sweeps = 30;
     cert_unconverged = 0;
     if (!small_h.empty()) {
-      ck(cudaMemsetAsync(fail_d, 0, sizeof(int), st), "memset fail flag");
-      psd_small_kernel<T><<<(int)small_h.size(), kBlock, small_smem(), st>>>(small_d, v, nullptr, 1, lam_small_d, max_sweeps, fail_d);
-      ck(cudaGetLastError(), "psd_small_kernel");
+      CUDA_TRY(cudaMemsetAsync(fail_d.p, 0, sizeof(int), st));
+      psd_small_kernel<T><<<(int)small_h.size(), kBlock, small_smem(), st>>>(small_d.p, v, nullptr, 1, lam_small_d.p, max_sweeps, fail_d.p);
+      CUDA_TRY(cudaGetLastError());
       ++launches;
       lam_host.resize(small_h.size());
       int fails = 0;
-      ck(cudaMemcpyAsync(lam_host.data(), lam_small_d, small_h.size() * sizeof(T), cudaMemcpyDeviceToHost, st), "copy lam");
-      ck(cudaMemcpyAsync(&fails, fail_d, sizeof(int), cudaMemcpyDeviceToHost, st), "copy fail flag");
-      ck(cudaStreamSynchronize(st), "sync");
+      CUDA_TRY(cudaMemcpyAsync(lam_host.data(), lam_small_d.p, small_h.size() * sizeof(T), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaMemcpyAsync(&fails, fail_d.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
       for (size_t k = 0; k < small_h.size(); ++k) lam[small_idx[k]] = (double)lam_host[k];
       cert_unconverged += fails;
     }
@@ -1116,11 +1092,11 @@ struct PsdBatch {
         ++cert_unconverged;
         continue;
       }
-      psd_large_lammax_kernel<T><<<1, 32, 0, st>>>(large_h[k].N, A_d, up_d, lam_large_d + k);
+      psd_large_lammax_kernel<T><<<1, 32, 0, st>>>(large_h[k].N, A_d.p, up_d.p, lam_large_d.p + k);
       ++launches;
       T l;
-      ck(cudaMemcpyAsync(&l, lam_large_d + k, sizeof(T), cudaMemcpyDeviceToHost, st), "copy lam");
-      ck(cudaStreamSynchronize(st), "sync");
+      CUDA_TRY(cudaMemcpyAsync(&l, lam_large_d.p + k, sizeof(T), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
       lam[large_idx[k]] = (double)l;
     }
   }

@@ -17,8 +17,8 @@
 // Eigenvalues that are numerically zero never reach +-1 and do not have to (they enter the projection with weight
 // |lambda|): once the unweighted measure delta = rms(1 - s_i^2) stalls, the weighted residual
 // |S (S X) - X|_F / |X|_F -- twice an upper bound of the projection error -- decides.
-// Anything unexpected (NaN, no convergence within the cap) returns false and the caller falls back to the
-// block-Jacobi eigensolver.
+// A NaN, no convergence within the cap or a workspace that does not fit in memory returns false and the caller falls
+// back to the block-Jacobi eigensolver; CUDA failures throw.
 #pragma once
 #include "tc_gemm.cuh"
 
@@ -133,9 +133,8 @@ template <typename T>
 struct PsdTc {
   tc::OzakiGemm<double> gemm;     // the iteration runs in fp64 for every model type (fp32 iterates would cost accuracy, not time)
   tc::Sliced slS, slY, slX;
-  double *S0_d = nullptr, *S1_d = nullptr, *U_d = nullptr, *Xd_d = nullptr;
-  double *state_d = nullptr, *partial_d = nullptr, *const_d = nullptr, *x2_d = nullptr;
-  double* state_h = nullptr;   // pinned
+  DevBuf<double> S0_d, S1_d, U_d, Xd_d, state_d, partial_d, const_d, x2_d;
+  PinnedBuf<double> state_h;
   int capN = 0, shapeN = 0;
   int last_steps = 0, last_checks = 0, last_phases = 0;
   double last_delta = 0, last_resid = -1;
@@ -158,12 +157,7 @@ struct PsdTc {
     return k;
   }
   bool configured = false;
-  std::string err;
 
-  ~PsdTc() {
-    cudaFree(S0_d); cudaFree(S1_d); cudaFree(U_d); cudaFree(Xd_d); cudaFree(state_d); cudaFree(partial_d); cudaFree(const_d); cudaFree(x2_d);
-    if (state_h) cudaFreeHost(state_h);
-  }
   static int env_int(const char* name, int def) {
     const char* e = getenv(name);
     return (e && *e) ? atoi(e) : def;
@@ -173,51 +167,56 @@ struct PsdTc {
     const char* e = getenv("COSMO_B200_PSD_TC");
     return !(e && e[0] == '0');
   }
+  // the projection is left to block Jacobi
+  static bool fall_back(const char* why) {
+    if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd-tc] fallback to block Jacobi: %s\n", why);
+    return false;
+  }
 
-  bool ensure(int N, cudaStream_t st) {
+  void ensure(int N, cudaStream_t st) {
     if (!configured) {
       // fp64 model: 8 slices, 10 groups (products exact to ~2^-56 of the row maxima); fp32 model: 6 slices, 8 groups (2^-42)
-      if (!gemm.configure(sizeof(T) == 8 ? 8 : 6, sizeof(T) == 8 ? 10 : 8, st)) { err = gemm.err; return false; }
-      bool ok = cudaMalloc(&state_d, 8 * sizeof(double)) == cudaSuccess && cudaMalloc(&const_d, 8 * sizeof(double)) == cudaSuccess &&
-                cudaMalloc(&x2_d, sizeof(double)) == cudaSuccess && cudaMallocHost(&state_h, 8 * sizeof(double)) == cudaSuccess;
-      if (!ok) { err = "PsdTc: cudaMalloc"; return false; }
+      gemm.configure(sizeof(T) == 8 ? 8 : 6, sizeof(T) == 8 ? 10 : 8);
+      state_d.alloc(8, false); const_d.alloc(8, false); x2_d.alloc(1, false);
+      state_h.alloc(8);
       const double c[8] = {1.0, 0.0, 0.0, 0.5, 0.5, 0.0, 0.0, 0.0};   // [0..2]: plain product, [3..5]: (X + S X) / 2
-      if (cudaMemcpyAsync(const_d, c, sizeof(c), cudaMemcpyHostToDevice, st) != cudaSuccess) { err = "PsdTc: copy"; return false; }
-      cudaStreamSynchronize(st);
+      const_d.upload(c, 8, st);
+      CUDA_TRY(cudaStreamSynchronize(st));
       configured = true;
     }
     if (N > capN) {
-      cudaFree(S0_d); cudaFree(S1_d); cudaFree(U_d); cudaFree(Xd_d); cudaFree(partial_d);
-      S0_d = S1_d = U_d = Xd_d = nullptr; partial_d = nullptr;
       capN = 0;
       const size_t nn = (size_t)N * N;
       const int nt = (N + tc::kTile - 1) / tc::kTile;
-      bool ok = cudaMalloc(&S0_d, nn * sizeof(double)) == cudaSuccess && cudaMalloc(&S1_d, nn * sizeof(double)) == cudaSuccess &&
-                cudaMalloc(&U_d, nn * sizeof(double)) == cudaSuccess &&
-                cudaMalloc(&partial_d, (size_t)nt * (nt + 1) * sizeof(double)) == cudaSuccess;
-      if (sizeof(T) != 8) ok = ok && cudaMalloc(&Xd_d, nn * sizeof(double)) == cudaSuccess;
+      S0_d.alloc(nn, false); S1_d.alloc(nn, false); U_d.alloc(nn, false);
+      partial_d.alloc((size_t)nt * (nt + 1), false);
+      if (sizeof(T) != 8) Xd_d.alloc(nn, false);
       const int Np = nt * tc::kTile;
-      ok = ok && slS.ensure(Np) && slY.ensure(Np) && slX.ensure(Np);
-      if (!ok) { err = "PsdTc: out of memory"; return false; }
+      slS.ensure(Np); slY.ensure(Np); slX.ensure(Np);
       capN = N;
       shapeN = 0;
     }
     if (shapeN != N) {
-      if (!gemm.set_shape(N, st)) { err = gemm.err; return false; }
+      gemm.set_shape(N, st);
       const int Np = gemm.Np;
       // the padding rows / columns of the slices must be zero; the shape of the cone changed, so clear everything
-      if (!slS.clear(Np, st) || !slY.clear(Np, st) || !slX.clear(Np, st)) { err = "PsdTc: memset"; return false; }
+      slS.clear(Np, st); slY.clear(Np, st); slX.clear(Np, st);
       shapeN = N;
     }
-    return true;
   }
 
   // X_in: N x N symmetric (ld = N) of the model type, fro_partials: partial sums of |X|_F^2.  Writes the projection in
-  // the layout of the cone into s_out.
+  // the layout of the cone into s_out.  false: NaN, no convergence within the step cap, or no memory for the workspace
+  // (block Jacobi needs less); every other failure throws.
   bool project(const PsdConeDesc& d, const T* X_in, const T* fro_partials, int nfro, T* /*scratch*/, T* s_out, cudaStream_t st,
                long long& launches) {
     const int N = d.N;
-    if (!ensure(N, st)) return false;
+    try {
+      ensure(N, st);
+    } catch (const EngineError& e) {
+      if (e.code != COSMO_B200_ERR_ALLOC) throw;
+      return fall_back(e.msg.c_str());
+    }
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
     const int ntiles = gemm.ntiles;
     const double l0 = l0_cur;
@@ -226,26 +225,25 @@ struct PsdTc {
     const double tol = 1e-7;                              // quadratic convergence: the step after delta < tol reaches ~delta^2
     const double rtol = sizeof(T) == 8 ? 5e-13 : 1e-7;    // accepted weighted residual
     const int cap = env_int("COSMO_B200_TC_MAX_STEPS", 80);
-    bool ok = true;
     const double* X_d;
     if (sizeof(T) == 8) {
       X_d = reinterpret_cast<const double*>(X_in);
-      ns_norm_kernel<T><<<1, kBlock, 0, st>>>(fro_partials, nfro, x2_d);
-      ns_scale_kernel<T><<<g, kBlock, 0, st>>>(N, X_in, S0_d, (double*)nullptr, x2_d);
+      ns_norm_kernel<T><<<1, kBlock, 0, st>>>(fro_partials, nfro, x2_d.p);
+      ns_scale_kernel<T><<<g, kBlock, 0, st>>>(N, X_in, S0_d.p, (double*)nullptr, x2_d.p);
     } else {
-      X_d = Xd_d;
-      ns_norm_kernel<T><<<1, kBlock, 0, st>>>(fro_partials, nfro, x2_d);
-      ns_scale_kernel<T><<<g, kBlock, 0, st>>>(N, X_in, S0_d, Xd_d, x2_d);
+      X_d = Xd_d.p;
+      ns_norm_kernel<T><<<1, kBlock, 0, st>>>(fro_partials, nfro, x2_d.p);
+      ns_scale_kernel<T><<<g, kBlock, 0, st>>>(N, X_in, S0_d.p, Xd_d.p, x2_d.p);
     }
     {
       double init[8] = {0, 0, 0, l0, 2.0, 0, 1.0, alpha_max};
-      memcpy(state_h, init, sizeof(init));
-      ok = ok && cudaMemcpyAsync(state_d, state_h, 8 * sizeof(double), cudaMemcpyHostToDevice, st) == cudaSuccess;
+      memcpy(state_h.p, init, sizeof(init));
+      CUDA_TRY(cudaMemcpyAsync(state_d.p, state_h.p, 8 * sizeof(double), cudaMemcpyHostToDevice, st));
     }
-    ok = ok && gemm.slice(X_d, slX, st);
+    gemm.slice(X_d, slX, st);
     launches += 2;
-    double* S = S0_d;
-    double* Sn = S1_d;
+    double* S = S0_d.p;
+    double* Sn = S1_d.p;
     double prev = 1e300, resid = -1.0, prev_resid = 1e300, delta = 2.0;
     // the host has nothing to decide while the schedule is still far from its taper: those steps are enqueued without
     // reading the state back (coefficients and scalings live on the device)
@@ -253,43 +251,41 @@ struct PsdTc {
     int it = 0, next_check = -1, checks = 0, phases = 1;
     bool have_P = false;
     for (;;) {
-      ok = ok && gemm.slice(S, slS, st);
-      ok = ok && gemm.gemm(slS, slS, U_d, nullptr, nullptr, 1, const_d, partial_d, st);        // Y = S S
-      ns_coef_kernel<0><<<1, 32, 0, st>>>(partial_d, ntiles, N, state_d);
-      ok = ok && gemm.slice(U_d, slY, st);
-      ok = ok && gemm.gemm(slS, slY, Sn, S, nullptr, 0, state_d, nullptr, st);                  // S' = c1 S + c0 S Y
+      gemm.slice(S, slS, st);
+      gemm.gemm(slS, slS, U_d.p, nullptr, nullptr, 1, const_d.p, partial_d.p, st);        // Y = S S
+      ns_coef_kernel<0><<<1, 32, 0, st>>>(partial_d.p, ntiles, N, state_d.p);
+      gemm.slice(U_d.p, slY, st);
+      gemm.gemm(slS, slY, Sn, S, nullptr, 0, state_d.p, nullptr, st);                    // S' = c1 S + c0 S Y
       launches += 5;
-      if (!ok) { err = gemm.err; return false; }
       if (phases == 1 && it + 1 < nosync_until) { std::swap(S, Sn); ++it; continue; }
-      if (cudaMemcpyAsync(state_h, state_d, 8 * sizeof(double), cudaMemcpyDeviceToHost, st) != cudaSuccess) return false;
-      if (cudaStreamSynchronize(st) != cudaSuccess) { err = std::string("PsdTc: ") + cudaGetErrorString(cudaGetLastError()); return false; }
+      CUDA_TRY(cudaMemcpyAsync(state_h.p, state_d.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
       std::swap(S, Sn);
       ++it;
       delta = state_h[4];
-      if (!(delta == delta)) { err = "PsdTc: NaN"; return false; }
+      if (!(delta == delta)) return fall_back("NaN");
       if (delta < tol) break;
       // the scaling schedule has run out (l ~ 1) and delta stalls: a cluster of (numerically) zero eigenvalues
       const bool schedule_done = state_h[3] > 0.999;
       if (next_check < 0 && schedule_done) next_check = it + 1;
       if ((next_check >= 0 && it >= next_check && delta > 0.9 * prev) || it >= cap) {
-        ok = ok && gemm.slice(S, slS, st);
-        ok = ok && gemm.gemm(slS, slX, U_d, X_d, nullptr, 0, const_d + 3, nullptr, st);           // P = (X + S X) / 2
-        ok = ok && residual_of_candidate(X_d, Sn, st, launches);
+        gemm.slice(S, slS, st);
+        gemm.gemm(slS, slX, U_d.p, X_d, nullptr, 0, const_d.p + 3, nullptr, st);           // P = (X + S X) / 2
+        residual_of_candidate(X_d, Sn, st, launches);
         launches += 2;
-        if (!ok) { if (err.empty()) err = gemm.err; return false; }
-        if (cudaMemcpyAsync(state_h, state_d, 8 * sizeof(double), cudaMemcpyDeviceToHost, st) != cudaSuccess) return false;
-        if (cudaStreamSynchronize(st) != cudaSuccess) return false;
+        CUDA_TRY(cudaMemcpyAsync(state_h.p, state_d.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
         resid = state_h[4];
         ++checks;
-        if (!(resid == resid)) { err = "PsdTc: NaN"; return false; }
+        if (!(resid == resid)) return fall_back("NaN");
         // accept: below the tolerance, or within 100x of it and no longer improving (the floor of the arithmetic)
         if (resid < rtol || (resid < 1e2 * rtol && resid > 0.5 * prev_resid)) { have_P = true; break; }
-        if (it >= cap) { err = "PsdTc: no convergence"; return false; }
+        if (it >= cap) return fall_back("no convergence");
         prev_resid = resid;
         // eigenvalues below the schedule's range are still on their way: run the aggressive schedule again from l_rearm
         // (the converged part of the spectrum bounces inside [0.56, 1] meanwhile and settles in the taper)
         state_h[3] = l_rearm;
-        if (cudaMemcpyAsync(state_d + 3, state_h + 3, sizeof(double), cudaMemcpyHostToDevice, st) != cudaSuccess) return false;
+        CUDA_TRY(cudaMemcpyAsync(state_d.p + 3, state_h.p + 3, sizeof(double), cudaMemcpyHostToDevice, st));
         ++phases;
         next_check = -1;
       }
@@ -307,30 +303,29 @@ struct PsdTc {
       l0_cur = std::max(l0 * (phases > 1 ? 1e-2 : 0.1), 1e-12);
     }
     if (!have_P) {
-      ok = ok && gemm.slice(S, slS, st);
-      ok = ok && gemm.gemm(slS, slX, U_d, X_d, nullptr, 0, const_d + 3, nullptr, st);
+      gemm.slice(S, slS, st);
+      gemm.gemm(slS, slX, U_d.p, X_d, nullptr, 0, const_d.p + 3, nullptr, st);
       launches += 2;
-      if (!ok) { err = gemm.err; return false; }
     }
-    if (d.triangle == 2) psd_embedding_store_kernel<T, double><<<g, kBlock, 0, st>>>(d, U_d, s_out);
-    else ns_store_kernel<T><<<g, kBlock, 0, st>>>(d, U_d, s_out);
+    if (d.triangle == 2) psd_embedding_store_kernel<T, double><<<g, kBlock, 0, st>>>(d, U_d.p, s_out);
+    else ns_store_kernel<T><<<g, kBlock, 0, st>>>(d, U_d.p, s_out);
     ++launches;
     if (getenv("COSMO_B200_PSD_DEBUG"))
       fprintf(stderr, "[psd-tc] N=%d steps=%d checks=%d phases=%d delta=%g resid=%g l0=%g next l0=%g\n", N, it, checks, phases, delta,
               resid, l0, l0_cur);
-    return cudaGetLastError() == cudaSuccess;
+    CUDA_TRY(cudaGetLastError());
+    return true;
   }
 
   // state[4] <- |S W - X|_F / |X|_F with W = 2 P - X, P in U_d, S sliced in slS.  Wbuf: scratch N x N.
-  bool residual_of_candidate(const double* X_d, double* Wbuf, cudaStream_t st, long long& launches) {
+  void residual_of_candidate(const double* X_d, double* Wbuf, cudaStream_t st, long long& launches) {
     const int N = gemm.N;
     const int g = (int)std::min<long long>(((long long)N * N + kBlock - 1) / kBlock, kMaxGrid);
-    ns_w_from_p_kernel<0><<<g, kBlock, 0, st>>>((long long)N * N, U_d, X_d, Wbuf);
-    bool ok = gemm.slice(Wbuf, slY, st);
-    ok = ok && gemm.gemm(slS, slY, nullptr, nullptr, X_d, 0, const_d, partial_d, st);
-    ns_residual_kernel<0><<<1, 32, 0, st>>>(partial_d, gemm.ntiles, x2_d, state_d);
+    ns_w_from_p_kernel<0><<<g, kBlock, 0, st>>>((long long)N * N, U_d.p, X_d, Wbuf);
+    gemm.slice(Wbuf, slY, st);
+    gemm.gemm(slS, slY, nullptr, nullptr, X_d, 0, const_d.p, partial_d.p, st);
+    ns_residual_kernel<0><<<1, 32, 0, st>>>(partial_d.p, gemm.ntiles, x2_d.p, state_d.p);
     launches += 4;
-    return ok;
   }
 };
 

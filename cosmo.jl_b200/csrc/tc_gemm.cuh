@@ -35,6 +35,8 @@
 #include <vector>
 #include <algorithm>
 
+#include "host.cuh"
+
 namespace cosmo {
 namespace tc {
 
@@ -415,85 +417,70 @@ inline EncodeTiledFn encode_tiled_fn() {
 
 // One sliced operand: int8 [Np][Np / 32][8][32] + Np scales, and its tensor map for the current Np.
 struct Sliced {
-  int8_t* d = nullptr;
-  double* scale = nullptr;
+  DevBuf<int8_t> d;
+  DevBuf<double> scale;
   CUtensorMap map;
   int capNp = 0, mapNp = 0;
-  ~Sliced() { cudaFree(d); cudaFree(scale); }
-  bool ensure(int Np) {
-    if (Np <= capNp) return true;
-    cudaFree(d); cudaFree(scale);
-    d = nullptr; scale = nullptr; capNp = 0; mapNp = 0;
-    if (cudaMalloc(&d, (size_t)kSlices * Np * Np) != cudaSuccess || cudaMalloc(&scale, (size_t)Np * sizeof(double)) != cudaSuccess) return false;
+  void ensure(int Np) {
+    if (Np <= capNp) return;
+    capNp = 0; mapNp = 0;
+    d.alloc((size_t)kSlices * Np * Np, false);
+    scale.alloc(Np, false);
     capNp = Np;
-    return true;
   }
   // zero padding rows / columns and unused slices: called when the shape of the cone changes
-  bool clear(int Np, cudaStream_t st) {
+  void clear(int Np, cudaStream_t st) {
     mapNp = 0;
-    return cudaMemsetAsync(d, 0, (size_t)kSlices * Np * Np, st) == cudaSuccess &&
-           cudaMemsetAsync(scale, 0, (size_t)Np * sizeof(double), st) == cudaSuccess;
+    CUDA_TRY(cudaMemsetAsync(d.p, 0, (size_t)kSlices * Np * Np, st));
+    CUDA_TRY(cudaMemsetAsync(scale.p, 0, (size_t)Np * sizeof(double), st));
   }
-  bool make_map(int Np) {
-    if (mapNp == Np) return true;
+  void make_map(int Np) {
+    if (mapNp == Np) return;
     EncodeTiledFn enc = encode_tiled_fn();
-    if (!enc) return false;
+    if (!enc) throw EngineError{COSMO_B200_ERR_CUDA, "cuTensorMapEncodeTiled is not available"};
     const cuuint64_t dims[2] = {(cuuint64_t)Np * kSlices, (cuuint64_t)Np};
     const cuuint64_t strides[1] = {(cuuint64_t)Np * kSlices};
     const cuuint32_t box[2] = {128, (cuuint32_t)kTile};
     const cuuint32_t estr[2] = {1, 1};
-    if (enc(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, d, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    if (enc(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, d.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return false;
+      throw EngineError{COSMO_B200_ERR_CUDA, "cuTensorMapEncodeTiled failed"};
     mapNp = Np;
-    return true;
   }
 };
 
 template <typename T>
 struct OzakiGemm {
-  int2* tiles_d = nullptr;
+  DevBuf<int2> tiles_d;
   int tilesNp = 0, ntiles = 0;
   int k = 8, g = 10, num_sms = 132;
   int N = 0, Np = 0;
-  bool ready = false;
-  std::string err;
-  ~OzakiGemm() { cudaFree(tiles_d); }
 
   static constexpr int smem_bytes() { return kUnits * kUnitBytes + 1024; }
   // supported (slices, groups): (8, 10) exact-fp64 default, (8, 8) and (7, 7) classical truncations, (6, 8) and (4, 6)
   // for the fp32 model type
   template <int K, int G>
-  static bool set_attr() {
-    return cudaFuncSetAttribute(ozaki_gemm_kernel<T, K, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes()) == cudaSuccess;
+  static void set_attr() {
+    CUDA_TRY(cudaFuncSetAttribute(ozaki_gemm_kernel<T, K, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes()));
   }
   template <int K>
-  static bool set_slice_attr() {
-    return cudaFuncSetAttribute(slice_rows_kernel<T, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSliceStageMaxBytes) == cudaSuccess;
+  static void set_slice_attr() {
+    CUDA_TRY(cudaFuncSetAttribute(slice_rows_kernel<T, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSliceStageMaxBytes));
   }
   static bool supported(int k_, int g_) {
     return (k_ == 8 && (g_ == 10 || g_ == 8)) || (k_ == 7 && g_ == 7) || (k_ == 6 && g_ == 8) || (k_ == 4 && g_ == 6);
   }
-  bool configure(int k_, int g_, cudaStream_t st) {
-    (void)st;
-    if (!supported(k_, g_)) { err = "tc::OzakiGemm: unsupported (slices, groups)"; return false; }
+  void configure(int k_, int g_) {
+    if (!supported(k_, g_)) throw EngineError{COSMO_B200_ERR_INVALID, "tc::OzakiGemm: unsupported (slices, groups)"};
     k = k_; g = g_;
     int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     // per device, every time: function attributes are per device and cheap to set
-    if (!(set_attr<8, 10>() && set_attr<8, 8>() && set_attr<7, 7>() && set_attr<6, 8>() && set_attr<4, 6>())) {
-      err = "cudaFuncSetAttribute(ozaki_gemm_kernel)";
-      return false;
-    }
-    if (!(set_slice_attr<8>() && set_slice_attr<7>() && set_slice_attr<6>() && set_slice_attr<4>())) {
-      err = "cudaFuncSetAttribute(slice_rows_kernel)";
-      return false;
-    }
-    ready = true;
-    return true;
+    set_attr<8, 10>(); set_attr<8, 8>(); set_attr<7, 7>(); set_attr<6, 8>(); set_attr<4, 6>();
+    set_slice_attr<8>(); set_slice_attr<7>(); set_slice_attr<6>(); set_slice_attr<4>();
   }
-  bool set_shape(int N_, cudaStream_t st) {
+  void set_shape(int N_, cudaStream_t st) {
     N = N_;
     Np = (N + kTile - 1) / kTile * kTile;
     if (tilesNp != Np) {
@@ -501,33 +488,32 @@ struct OzakiGemm {
       std::vector<int2> tl;
       for (int bj = 0; bj < nt; ++bj)
         for (int bi = 0; bi <= bj; ++bi) tl.push_back(make_int2(bi, bj));
-      cudaFree(tiles_d);
-      tiles_d = nullptr;
-      if (cudaMalloc(&tiles_d, tl.size() * sizeof(int2)) != cudaSuccess) { err = "cudaMalloc tiles"; return false; }
-      if (cudaMemcpyAsync(tiles_d, tl.data(), tl.size() * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess) { err = "copy tiles"; return false; }
-      cudaStreamSynchronize(st);
+      tilesNp = 0;
+      tiles_d.alloc(tl.size(), false);
+      tiles_d.upload(tl.data(), tl.size(), st);
+      CUDA_TRY(cudaStreamSynchronize(st));
       ntiles = (int)tl.size();
       tilesNp = Np;
     }
-    return true;
   }
   // slices of an N x N symmetric matrix (ld = N) into `sl` (padding rows / columns must have been cleared)
-  bool slice(const T* M, Sliced& sl, cudaStream_t st) {
+  void slice(const T* M, Sliced& sl, cudaStream_t st) {
     const int staged = slice_stage_bytes(N) <= (size_t)kSliceStageMaxBytes ? 1 : 0;
     const size_t sm = staged ? slice_stage_bytes(N) : 0;
-    if (k == 8) slice_rows_kernel<T, 8><<<N, 256, sm, st>>>(M, N, Np, sl.d, sl.scale, staged);
-    else if (k == 7) slice_rows_kernel<T, 7><<<N, 256, sm, st>>>(M, N, Np, sl.d, sl.scale, staged);
-    else if (k == 6) slice_rows_kernel<T, 6><<<N, 256, sm, st>>>(M, N, Np, sl.d, sl.scale, staged);
-    else slice_rows_kernel<T, 4><<<N, 256, sm, st>>>(M, N, Np, sl.d, sl.scale, staged);
-    return cudaGetLastError() == cudaSuccess;
+    if (k == 8) slice_rows_kernel<T, 8><<<N, 256, sm, st>>>(M, N, Np, sl.d.p, sl.scale.p, staged);
+    else if (k == 7) slice_rows_kernel<T, 7><<<N, 256, sm, st>>>(M, N, Np, sl.d.p, sl.scale.p, staged);
+    else if (k == 6) slice_rows_kernel<T, 6><<<N, 256, sm, st>>>(M, N, Np, sl.d.p, sl.scale.p, staged);
+    else slice_rows_kernel<T, 4><<<N, 256, sm, st>>>(M, N, Np, sl.d.p, sl.scale.p, staged);
+    CUDA_TRY(cudaGetLastError());
   }
   // out = c0 (A B) + c1 D + c2 I   (+ reductions into partial[2 * ntiles])
-  bool gemm(Sliced& A, Sliced& B, T* out, const T* D, const T* E, int e_identity, const double* coef_d, double* partial,
+  void gemm(Sliced& A, Sliced& B, T* out, const T* D, const T* E, int e_identity, const double* coef_d, double* partial,
             cudaStream_t st) {
-    if (!A.make_map(Np) || !B.make_map(Np)) { err = "cuTensorMapEncodeTiled failed"; return false; }
+    A.make_map(Np);
+    B.make_map(Np);
     GemmArgs<T> a;
     a.N = N; a.Np = Np; a.ntiles = ntiles; a.store = out ? 1 : 0;
-    a.tiles = tiles_d; a.scaleA = A.scale; a.scaleB = B.scale; a.out = out; a.D = D; a.E = E; a.e_identity = e_identity;
+    a.tiles = tiles_d.p; a.scaleA = A.scale.p; a.scaleB = B.scale.p; a.out = out; a.D = D; a.E = E; a.e_identity = e_identity;
     a.coef = coef_d; a.partial = partial;
     const int grid = std::min(ntiles, num_sms);
     if (k == 8 && g == 10) ozaki_gemm_kernel<T, 8, 10><<<grid, kThreads, smem_bytes(), st>>>(A.map, B.map, a);
@@ -535,9 +521,7 @@ struct OzakiGemm {
     else if (k == 7) ozaki_gemm_kernel<T, 7, 7><<<grid, kThreads, smem_bytes(), st>>>(A.map, B.map, a);
     else if (k == 6) ozaki_gemm_kernel<T, 6, 8><<<grid, kThreads, smem_bytes(), st>>>(A.map, B.map, a);
     else ozaki_gemm_kernel<T, 4, 6><<<grid, kThreads, smem_bytes(), st>>>(A.map, B.map, a);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { err = std::string("ozaki_gemm_kernel launch: ") + cudaGetErrorString(e); return false; }
-    return true;
+    CUDA_TRY(cudaGetLastError());
   }
 };
 

@@ -938,6 +938,23 @@ def test_psd_tensor_core_large_and_fallback(monkeypatch):
     assert np.linalg.norm(got - ref) / np.linalg.norm(ws) < 1e-12
 
 
+def test_block_jacobi_non_convergence_is_a_numerical_error(monkeypatch):
+    """tensor cores off and psd_max_sweeps = 1 on a Wigner matrix of side 150: block Jacobi misses the sweep cap, and
+    project() and solve() fail with ERR_NUMERICAL, as the reference fails when LAPACK does not converge
+    (convexset.jl:186)."""
+    monkeypatch.setenv("COSMO_B200_PSD_TC", "0")
+    N = 150
+    ws = G._svec(_psd_test_matrix("wigner", N, np.random.default_rng(60)))
+    sets = [cosmo_b200.PsdConeTriangle(N * (N + 1) // 2)]
+    eng = _engine(sp.identity(1, format="csc"), np.zeros(1), sp.csc_matrix((ws.size, 1)), ws, sets, psd_max_sweeps=1)
+    for call in (lambda: eng.project(ws), eng.solve):
+        with pytest.raises(E.EngineError) as ei:
+            call()
+        assert ei.value.code == E.ERR_NUMERICAL, ei.value
+        assert "block Jacobi eigensolver did not converge within psd_max_sweeps" in str(ei.value)
+    eng.close()
+
+
 @pytest.mark.parametrize("Nc,kind", [(49, "shifted"), (100, "wigner"), (100, "low_rank_plus_noise"), (193, "shifted")])
 def test_complex_psd_cone_large_through_the_tensor_core_path(Nc, kind):
     """PsdConeTriangle{T, Complex{T}} beyond the shared-memory path (2 Nc > 96): the real embedding [[A, -B], [B, A]]
