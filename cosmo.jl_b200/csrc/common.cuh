@@ -94,6 +94,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
       : "memory");
 }
 
+// ---- programmatic dependent launch (launch_pdl in host.cuh) -----------------
+// A kernel launched with launch_pdl may start while the kernel before it in the stream is still running.  Until
+// pdl_wait() returns it may touch only data that stay constant during the solve (matrix slabs, row partitions, shape
+// arguments): pdl_wait() blocks until every earlier kernel of the stream has completed and its writes are visible.
+// Without a programmatic predecessor (first launch, after a collective, a copy or an event) it returns at once.
+// pdl_launch_dependents() lets the next launch_pdl kernel start being scheduled; its CTAs take SMs as ours leave.
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // ---- peer-memory exchange (NVLink / NVSwitch) -------------------------------
 // One exchange buffer per rank, mapped into every peer through CUDA IPC:
 //   data : 2 slots x stride elements (the rank's partial n-vector + its partial dot at [n])

@@ -295,6 +295,11 @@ class Engine : public EngineBase {
   void destroy_ldl_factor_graph() { ldl_factor_graph_.reset(); }
   long long kkt_counter_ = 1;   // S.iteration_counter
   int last_cg_iters_ = 1;
+  // tm_ = rho .* (A xsol_), stored by the fused ADMM tail: the next CG solve of the same solve() starts from it instead
+  // of recomputing the product.  It never outlives one solve() call: solve() and kkt_solve() clear it on entry (so
+  // warm_start, reset, update_qb/update_rho/update_settings in between cannot leave it stale), a rho adaptation clears
+  // it, and kkt_core consumes it and sets it again only from a tail that stored tm_ for the chained CG loop.
+  bool tm_valid_ = false;
   long long total_inner_ = 0, total_mults_ = 0;
   // scratch
   DevBuf<T> vec_m_, vec_n_, vec_n2_, dy_, dx_, ypart_;
@@ -356,12 +361,14 @@ class Engine : public EngineBase {
 
   template <typename Epi>
   void launch_spmv(const DevCsr<T>& M1, const T* x1, const DevCsr<T>* M2, const T* x2, int nrows, const Epi& epi,
-                   RedBuf<T> rb, const char* name);
+                   RedBuf<T> rb, const char* name, T* pbuf = nullptr);
+  template <typename Epi, int PL>
+  void launch_win(const DevCsr<T>& M1, const T* x1, CsrView<T> v2, const T* x2, const Epi& epi, RedBuf<T> rb, T* pbuf);
   void project_device(const T* w, bool with_rhs, const T* ws_rhs);
   void soc_norms(const T* ws, T* norm_out);
   void kkt_core(bool fused_tail, const T* w_src, T* w_dst);
   void kkt_op_stage2(const int* done, const T* u, const T* t_in, T* c_out, bool exchange = false);
-  void kkt_cg(const int* done);
+  void kkt_cg(const int* done, bool tm_ready);
   void kkt_minres(bool full);
   void set_maxit(int v);
   void compute_residuals(const T* x, const T* s, const T* mu, bool ignore_scaling, double out[5]);
@@ -1147,28 +1154,45 @@ void Engine<T>::p2p_attach(const void* blobs, int nranks) {
 template <typename T>
 template <typename Epi>
 void Engine<T>::launch_spmv(const DevCsr<T>& M1, const T* x1, const DevCsr<T>* M2, const T* x2, int nrows,
-                            const Epi& epi, RedBuf<T> rb, const char* name) {
+                            const Epi& epi, RedBuf<T> rb, const char* name, T* pbuf) {
   const CsrView<T> v2 = M2 ? M2->view() : CsrView<T>{nullptr, nullptr, nullptr};
   if (M1.windowed) {
-    const size_t smem = (size_t)M1.W * sizeof(T);
-    // function attributes are per device: one flag per (T, Epi) instantiation AND device ordinal
-    static bool configured[64] = {false};
-    const int dev_slot = device_ & 63;
-    if (!configured[dev_slot] || device_ >= 64) {
-      CUDA_TRY(cudaFuncSetAttribute(spmv_win_kernel<T, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204800));
-      configured[dev_slot] = true;
+    // a second matrix on the windowed path: the P rows of the reduced KKT operator, summed with P's own lane count
+    // into pbuf (M2 must be plain CSR)
+    if (M2 == nullptr) {
+      launch_win<Epi, 0>(M1, x1, v2, x2, epi, rb, nullptr);
+    } else if constexpr (std::is_same<Epi, EpiKktOp<T>>::value) {
+      if (M2->windowed || pbuf == nullptr) throw EngineError{COSMO_B200_ERR_INVALID, "windowed SpMV: P rows need plain CSR and a buffer"};
+      if (M2->lanes == 32) launch_win<Epi, 32>(M1, x1, v2, x2, epi, rb, pbuf);
+      else if (M2->lanes == 8) launch_win<Epi, 8>(M1, x1, v2, x2, epi, rb, pbuf);
+      else launch_win<Epi, 2>(M1, x1, v2, x2, epi, rb, pbuf);
+    } else {
+      throw EngineError{COSMO_B200_ERR_INVALID, "windowed SpMV: a second matrix is only folded into the KKT operator"};
     }
-    spmv_win_kernel<T, Epi><<<M1.nctas, kWinThreads, smem, stream_>>>(M1.wview(), x1, v2, x2, epi, rb, ypart_.p,
-                                                                      chunk_ticket_.p);
     check_launch(name);
     return;
   }
   const int lanes = M1.lanes;
   const int grid = sgrid(nrows, lanes);
-  if (lanes == 32) spmv_kernel<T, 32, Epi><<<grid, kBlock, 0, stream_>>>(M1.view(), x1, v2, x2, nrows, epi, rb);
-  else if (lanes == 8) spmv_kernel<T, 8, Epi><<<grid, kBlock, 0, stream_>>>(M1.view(), x1, v2, x2, nrows, epi, rb);
-  else spmv_kernel<T, 2, Epi><<<grid, kBlock, 0, stream_>>>(M1.view(), x1, v2, x2, nrows, epi, rb);
+  auto kernel = lanes == 32 ? spmv_kernel<T, 32, Epi> : lanes == 8 ? spmv_kernel<T, 8, Epi> : spmv_kernel<T, 2, Epi>;
+  launch_pdl(kernel, grid, kBlock, 0, stream_, M1.view(), x1, v2, x2, nrows, epi, rb);
   check_launch(name);
+}
+
+template <typename T>
+template <typename Epi, int PL>
+void Engine<T>::launch_win(const DevCsr<T>& M1, const T* x1, CsrView<T> v2, const T* x2, const Epi& epi, RedBuf<T> rb,
+                           T* pbuf) {
+  const size_t smem = (size_t)M1.W * sizeof(T);
+  // function attributes are per device: one flag per (T, Epi, PL) instantiation AND device ordinal
+  static bool configured[64] = {false};
+  const int dev_slot = device_ & 63;
+  if (!configured[dev_slot] || device_ >= 64) {
+    CUDA_TRY(cudaFuncSetAttribute(spmv_win_kernel<T, Epi, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204800));
+    configured[dev_slot] = true;
+  }
+  launch_pdl(spmv_win_kernel<T, Epi, PL>, M1.nctas, kWinThreads, smem, stream_, M1.wview(), x1, v2, x2, epi, rb, ypart_.p,
+             chunk_ticket_.p, pbuf);
 }
 
 template <typename T>
@@ -1211,15 +1235,19 @@ void Engine<T>::kkt_op_stage2(const int* done, const T* u, const T* t_in, T* c_o
   const DevCsr<T>* M2 = nullptr;
   const T* pu = nullptr;
   if (At_.windowed) {
-    // the slab kernel cannot walk P's rows without unbalancing its window-0 CTAs: P u goes first
+    // P u lands in vec_n2_ and enters through the epilogue's `add`: the slab kernel sums the P rows of each chunk
+    // (spread over the chunk's window CTAs) before streaming; a column-windowed P keeps its own launch
     if (lead && P_.nnz > 0) {
-      launch_spmv(P_, u, (const DevCsr<T>*)nullptr, (const T*)nullptr, n_, EpiStore<T>{done, vec_n2_.p}, red(SC_TMP0), "spmv_P");
       pu = vec_n2_.p;
+      if (P_.windowed)
+        launch_spmv(P_, u, (const DevCsr<T>*)nullptr, (const T*)nullptr, n_, EpiStore<T>{done, vec_n2_.p}, red(SC_TMP0), "spmv_P");
+      else
+        M2 = &P_;
     }
   } else if (lead) {
     M2 = &P_;
   }
-  launch_spmv(At_, t_in, M2, u, n_, EpiKktOp<T>{done, c_out, u, sig, pu}, red_ptr(cb_.p + n_), "spmv_kkt_op");
+  launch_spmv(At_, t_in, M2, u, n_, EpiKktOp<T>{done, c_out, u, sig, pu}, red_ptr(cb_.p + n_), "spmv_kkt_op", vec_n2_.p);
   if (px) {
     // one-shot allreduce over NVLink: push [c; u'c] into every peer's exchange buffer (coalesced 16-byte remote
     // stores), the consumers (cg_init / cg_update_xr) wait for the flags and sum their local segments in rank order
@@ -1253,6 +1281,8 @@ void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "unknown kkt_solver"};
   if (full && nranks_ > 1)
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "full-KKT MINRES is single-GPU in this build (use CG or reduced MINRES when sharded)"};
+  const bool tm_ready = tm_valid_;
+  tm_valid_ = false;
   if (full || direct) {
     if (direct) ldl_solve();   // xsol_ = y1, nu_ = y2
     else kkt_minres(true);
@@ -1266,13 +1296,19 @@ void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
   launch_spmv(At_, t0_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n_,
               EpiAddVec<T>{nullptr, rhsb_.p, lead ? ls_.p : nullptr}, red(SC_TMP0), "spmv_rhs");
   allreduce_sum(rhsb_.p, n_);
-  if (st_.kkt_solver == COSMO_B200_KKT_CG) kkt_cg(isc_.p + ISC_DONE);
+  const bool cg = (st_.kkt_solver == COSMO_B200_KKT_CG);
+  if (cg) kkt_cg(isc_.p + ISC_DONE, tm_ready);
   else kkt_minres(false);
   kkt_counter_ += 1;
   if (fused_tail) {
+    // the tail also keeps tm = rho .* (A xsol) for the warm start of the next CG solve of the chained loop (the
+    // persistent CG kernel computes its own; reduced MINRES uses tm_ as scratch)
+    const bool keep_tm = cg && !persistent_cg_ok();
     launch_spmv(A_, xsol_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m_,
-                EpiAdmmTail<T>{nullptr, ls_.p + n_, rho_vec_.p, s_.p, w_src + n_, w_dst + n_, (T)st_.alpha}, red(SC_TMP0),
-                "spmv_admm_tail");
+                EpiAdmmTail<T>{nullptr, ls_.p + n_, rho_vec_.p, s_.p, w_src + n_, w_dst + n_, (T)st_.alpha,
+                               keep_tm ? tm_.p : nullptr},
+                red(SC_TMP0), "spmv_admm_tail");
+    tm_valid_ = keep_tm;
   } else {
     launch_spmv(A_, xsol_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m_,
                 EpiY2<T>{nullptr, nu_.p, ls_.p + n_, rho_vec_.p}, red(SC_TMP0), "spmv_y2");
@@ -1281,20 +1317,22 @@ void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
 
 // cg!(previous_solution, L, y1; abstol = tol_k/|y1|, reltol = 0) (kktsolver_indirect.jl:70)
 template <typename T>
-void Engine<T>::kkt_cg(const int* done) {
+void Engine<T>::kkt_cg(const int* done, bool tm_ready) {
   set_maxit(n_);   // IterativeSolvers default maxiter = size(A, 2)
   if (persistent_cg_ok()) {
     launch_persistent_cg(st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent));
     return;
   }
-  // c = L x0 (warm start => one product for the initial residual)
-  launch_spmv(A_, xsol_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m_, EpiScale<T>{nullptr, tm_.p, rho_vec_.p},
-              red(SC_TMP0), "spmv_A_scale");
+  // c = L x0 (warm start => one product for the initial residual); tm = rho .* (A x0) is left by the previous
+  // iteration's fused tail when nothing changed since (the product is still counted: the reference computes it)
+  if (!tm_ready)
+    launch_spmv(A_, xsol_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m_, EpiScale<T>{nullptr, tm_.p, rho_vec_.p},
+                red(SC_TMP0), "spmv_A_scale");
   kkt_op_stage2(nullptr, xsol_.p, tm_.p, cb_.p, true);
   if (!p2p_) allreduce_sum(cb_.p, n_ + 1);
   const double tol_num = st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent);
-  cg_init_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, rhsb_.p, cb_.p, r_.p, u_.p, red(SC_RES2),
-                                                      CgInitFin<T>{sc_.p, isc_.p, (T)tol_num, p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
+  launch_pdl(cg_init_kernel<T>, vgrid(n_), kBlock, 0, stream_, n_, (const T*)rhsb_.p, (const T*)cb_.p, r_.p, u_.p, red(SC_RES2),
+             CgInitFin<T>{sc_.p, isc_.p, (T)tol_num, p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
   check_launch("cg_init");
   // NCCL collectives are capturable too: sharded runs replay the same graphs
   if (!cg_graph_[0]) build_cg_graphs(done);
@@ -1304,7 +1342,7 @@ void Engine<T>::kkt_cg(const int* done) {
     for (int b = 3; b >= 0; --b)
       while (left >= (1 << b)) {
         CUDA_TRY(cudaGraphLaunch(cg_graph_[b], stream_));
-        launches_ += (long long)(1 << b) * (At_.windowed && P_.nnz > 0 ? 5 : 4);
+        launches_ += (long long)(1 << b) * (At_.windowed && P_.windowed && P_.nnz > 0 && rank_ == 0 ? 5 : 4);
         left -= (1 << b);
       }
     CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
@@ -1362,14 +1400,15 @@ void Engine<T>::launch_persistent_cg(double tol_num) {
 // one CG iteration: u = r + beta u ; c = L u ; alpha = res^2/u'c ; x += alpha u ; r -= alpha c
 template <typename T>
 void Engine<T>::cg_iteration_launches(const int* done) {
-  cg_update_u_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, r_.p, u_.p, sc_.p, isc_.p);
+  launch_pdl(cg_update_u_kernel<T>, vgrid(n_), kBlock, 0, stream_, n_, (const T*)r_.p, u_.p, (const T*)sc_.p, (const int*)isc_.p);
   check_launch("cg_update_u");
   launch_spmv(A_, u_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m_, EpiScale<T>{done, tm_.p, rho_vec_.p}, red(SC_TMP0),
               "spmv_A_scale");
   kkt_op_stage2(done, u_.p, tm_.p, cb_.p, true);
   if (!p2p_) allreduce_sum(cb_.p, n_ + 1);
-  cg_update_xr_kernel<T><<<vgrid(n_), kBlock, 0, stream_>>>(n_, u_.p, cb_.p, cb_.p + n_, xsol_.p, r_.p, sc_.p, isc_.p, red(SC_RES2),
-                                                         CgStepFin<T>{sc_.p, isc_.p, p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
+  launch_pdl(cg_update_xr_kernel<T>, vgrid(n_), kBlock, 0, stream_, n_, (const T*)u_.p, (const T*)cb_.p, (const T*)cb_.p + n_,
+             xsol_.p, r_.p, (const T*)sc_.p, (const int*)isc_.p, red(SC_RES2),
+             CgStepFin<T>{sc_.p, isc_.p, p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
   check_launch("cg_update_xr");
 }
 
@@ -1497,6 +1536,7 @@ bool Engine<T>::adapt_rho(const T* x) {
   new_rho = std::min(std::max(new_rho, st_.RHO_MIN), st_.RHO_MAX);
   if (new_rho > st_.adaptive_rho_tolerance * rho_ || new_rho < (1.0 / st_.adaptive_rho_tolerance) * rho_) {
     rho_ = new_rho;
+    tm_valid_ = false;
     rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
     check_launch("rho_vec");
     ldl_dirty_ = true;
@@ -1823,6 +1863,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
   const long long launches0 = launches_;
   total_inner_ = 0; total_mults_ = 0;
   persist_solves_ = 0;
+  tm_valid_ = false;
   CUDA_TRY(cudaMemsetAsync(isc_.p + ISC_TOTAL, 0, sizeof(int), stream_));
   int status = COSMO_B200_UNDETERMINED;
   double cost = INFINITY;
@@ -2076,6 +2117,7 @@ void Engine<T>::project(const void* ws, void* s_out) {
 template <typename T>
 void Engine<T>::kkt_solve(const void* rhs, void* sol, int64_t* inner) {
   CUDA_TRY(cudaSetDevice(device_));
+  tm_valid_ = false;
   upload_vec(ls_, rhs, (size_t)n_ + m_);
   scale_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_vec_.p, ls_.p + n_, t0_.p);
   check_launch("scale_x2");
@@ -2265,8 +2307,14 @@ void Engine<T>::spmv(int which, const void* x, void* y) {
     upload_vec(dx_, x, n_);
     launch_spmv(P_, dx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n_, EpiStore<T>{nullptr, vec_n_.p}, red(SC_TMP0), "spmv_P");
     download_vec(y, vec_n_.p, n_);
+  } else if (which == 3) {
+    // second stage of the reduced KKT operator: y = A' x2 + P x1 + sigma x1, x = [x1; x2] (the CG kernel's pass)
+    upload_vec(dx_, x, n_);
+    upload_vec(dy_, static_cast<const T*>(x) + n_, m_);
+    kkt_op_stage2(nullptr, dx_.p, dy_.p, vec_n_.p);
+    download_vec(y, vec_n_.p, n_);
   } else {
-    throw EngineError{COSMO_B200_ERR_INVALID, "spmv: which must be 0 (A), 1 (A') or 2 (P)"};
+    throw EngineError{COSMO_B200_ERR_INVALID, "spmv: which must be 0 (A), 1 (A'), 2 (P) or 3 (A' x2 + P x1 + sigma x1)"};
   }
   sync();
 }

@@ -8,6 +8,7 @@
 #include <stdio.h>
 
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/cosmo_b200.h"
@@ -94,6 +95,24 @@ struct GraphExec {
   void reset() { if (g) cudaGraphExecDestroy(g); g = nullptr; }
   operator cudaGraphExec_t() const { return g; }
 };
+
+// Launch `kernel` on `st` as a programmatic dependent of the kernel before it: it may be scheduled as soon as that kernel
+// calls pdl_launch_dependents() (common.cuh), and must itself call pdl_wait() before it touches anything an earlier kernel
+// of the stream reads or writes.  Stream capture records the programmatic edge in the graph.
+template <typename... KArgs, typename... Args>
+void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
+}
 
 // Stream-capture what `launches()` enqueues on `st` into `out`.
 template <typename F>

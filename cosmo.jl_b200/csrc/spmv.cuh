@@ -78,6 +78,8 @@ __device__ __forceinline__ T group_sum(T v) {
 template <typename T, int LANES, typename Epi>
 __global__ void __launch_bounds__(kBlock) spmv_kernel(CsrView<T> M1, const T* __restrict__ x1, CsrView<T> M2,
                                                       const T* __restrict__ x2, int nrows, Epi epi, RedBuf<T> rb) {
+  pdl_launch_dependents();
+  pdl_wait();
   if (epi.done != nullptr && *epi.done) return;
   constexpr int GROUPS = kBlock / LANES;
   const int lane = threadIdx.x % LANES;
@@ -171,13 +173,20 @@ __device__ __forceinline__ T win_row_rest(const unsigned short* __restrict__ col
 // slab w and writes per-window partial sums.  The last of the nwin CTAs of a chunk to finish
 // (per-chunk ticket) folds the partials in window order -- deterministic -- and runs the epilogue
 // (one thread per row); only those "finishing" CTAs take part in the scalar reduction, whose
-// partials are indexed by chunk, not by CTA.  (The small P-row product of the reduced KKT
-// operator is computed by a separate launch and enters through the epilogue's `add` vector.)
-template <typename T, typename Epi>
+// partials are indexed by chunk, not by CTA.
+//
+// PL > 0 (the reduced KKT operator): the P-row product p = M2 x2 of chunk j's rows is spread over the nwin CTAs of the
+// chunk, PL lanes per row, and stored in `pbuf`, which the epilogue reads as its `add` vector.  With nwin > 1 each CTA
+// sums its share after streaming its slab, and the finishing CTA reads them after the chunk ticket; with nwin == 1
+// the CTA sums them before streaming, behind a CTA barrier.  Every P row is summed exactly as
+// spmv_kernel<T, PL, EpiStore> sums it (row_partial + group_sum with the same PL), so the result is bitwise that of a
+// separate P launch.  PL = 0: no P rows (M2, x2 and pbuf unused).
+template <typename T, typename Epi, int PL = 0>
 __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M, const T* __restrict__ x, CsrView<T> M2,
                                                                   const T* __restrict__ x2, Epi epi, RedBuf<T> rb,
-                                                                  T* __restrict__ ypart, unsigned* __restrict__ chunk_ticket) {
-  if (epi.done != nullptr && *epi.done) return;
+                                                                  T* __restrict__ ypart, unsigned* __restrict__ chunk_ticket,
+                                                                  T* pbuf) {
+  pdl_launch_dependents();
   extern __shared__ __align__(128) unsigned char win_smem[];
   T* xs = reinterpret_cast<T*>(win_smem);
   __shared__ __align__(8) uint64_t bar;
@@ -188,13 +197,23 @@ __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M,
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
     mbar_fence_init();
-    int cnt = M.ncols - w * M.W;
-    if (cnt > M.W) cnt = M.W;
-    const unsigned bytes = ((unsigned)cnt * (unsigned)sizeof(T) + 15u) & ~15u;   // source buffers are padded
-    mbar_expect_tx(&bar, bytes);
-    bulk_load_g2s(xs, x + (size_t)w * M.W, bytes, &bar);
   }
   __syncthreads();
+  // Up to the first pdl_wait() (in `stage_x`) only the constant slab arrays are read: the barrier setup, the row
+  // pointers and (PL = 0) the first row pair's columns and values overlap the tail of the kernel before this one.  The
+  // x-slice, the done flag, x2 and every output are touched after it.  stage_x() waits, then issues the bulk copy.
+  auto stage_x = [&]() -> bool {
+    pdl_wait();
+    if (epi.done != nullptr && *epi.done) return false;
+    if (threadIdx.x == 0) {
+      int cnt = M.ncols - w * M.W;
+      if (cnt > M.W) cnt = M.W;
+      const unsigned bytes = ((unsigned)cnt * (unsigned)sizeof(T) + 15u) & ~15u;   // source buffers are padded
+      mbar_expect_tx(&bar, bytes);
+      bulk_load_g2s(xs, x + (size_t)w * M.W, bytes, &bar);
+    }
+    return true;
+  };
   const int r0 = M.cta_row_start[chunk], r1 = M.cta_row_start[chunk + 1];
   T accS[Epi::NS > 0 ? Epi::NS : 1];
   T accM[Epi::NM > 0 ? Epi::NM : 1];
@@ -225,7 +244,32 @@ __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M,
       e_b = __ldg(rp + row + 1);
     }
   };
+  // this CTA's share of the chunk's P rows (called block-uniformly, after the wait)
+  auto p_rows = [&]() {
+    constexpr int G = kWinThreads / (PL > 0 ? PL : 1);
+    const int plane = threadIdx.x % (PL > 0 ? PL : 1), group = threadIdx.x / (PL > 0 ? PL : 1);
+    // `base` is block-uniform so every lane of a warp runs the same number of trips (full-mask shuffles)
+    for (int base = r0 + w * G; base < r1; base += M.nwin * G) {
+      const int row = base + group;
+      const bool valid = row < r1;
+      T s = 0;
+      if (valid) s += row_partial<T, (PL > 0 ? PL : 1)>(M2, x2, row, plane);
+      s = group_sum<T, (PL > 0 ? PL : 1)>(s);
+      if (valid && plane == 0) pbuf[row] = s;
+    }
+  };
   fetch_ptrs(0, sa, ea, sb, eb);
+  bool staged = false;
+  if constexpr (PL > 0) {
+    if (single) {
+      // the epilogue runs in the streaming loop: wait, start the x-slice copy, sum the P rows under it, and make them
+      // visible to the whole CTA before streaming
+      if (!stage_x()) return;
+      staged = true;
+      p_rows();
+      __syncthreads();
+    }
+  }
   for (int k = 0; k < nmine; k += 2) {
     const bool has_b = (k + 1 < nmine);
     const int ja = sa + lane * 8, jb = sb + lane * 8;
@@ -238,7 +282,11 @@ __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M,
     if (lb) { cxb = __ldcs(reinterpret_cast<const uint4*>(M.col + jb)); load8_coalesced(M.val + sb, min(32, (eb - sb) >> 3), lane, vb); }
     const int csa = sa, cea = ea, csb = sb, ceb = eb;
     fetch_ptrs(k + 2, sa, ea, sb, eb);          // next pair
-    if (!waited) { mbar_wait(&bar, 0); waited = true; }
+    if (!waited) {
+      if (!staged && !stage_x()) return;
+      mbar_wait(&bar, 0);
+      waited = true;
+    }
     T pa = la ? win_fma8<T>(va, cxa, xs) : T(0);
     T pb = lb ? win_fma8<T>(vb, cxb, xs) : T(0);
     if (cea - csa > 256) pa += win_row_rest<T>(M.col, M.val, xs, csa, cea, lane);
@@ -258,7 +306,15 @@ __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M,
       else yw[row] = keep;
     }
   }
-  if (!waited) mbar_wait(&bar, 0);   // never leave a bulk copy in flight
+  if (!waited) {   // warps without rows: the x-slice is still staged by thread 0, never left in flight
+    if (!staged && !stage_x()) return;
+    mbar_wait(&bar, 0);
+  }
+  // nwin > 1: the P rows fill the time between this CTA's last row and the chunk ticket; the finishing CTA reads them
+  // after the ticket's fences
+  if constexpr (PL > 0) {
+    if (!single) p_rows();
+  }
 
   if (!single) {
     __threadfence();
@@ -317,10 +373,11 @@ struct EpiKktOp {
   T* c;
   const T* u;
   T sigma;
-  const T* add;   // optional precomputed P u (nullptr: P rows are traversed by the same kernel)
+  const T* add;   // optional P u, computed by the P rows of the windowed kernel or by a separate launch (nullptr: the
+                  // plain kernel traverses P's rows itself); read through L2, other CTAs of the same kernel may write it
   __device__ void row(int r, T s, T* accS, T*) const {
     const T ur = u[r];
-    const T v = (add ? s + add[r] : s) + sigma * ur;
+    const T v = (add ? s + __ldcg(add + r) : s) + sigma * ur;
     c[r] = v;
     accS[0] += ur * v;
   }
@@ -366,6 +423,7 @@ struct EpiKktFullLower {
 //   nu   = rho .* (A y1 - x2)               (kktsolver_indirect.jl:80-83)
 //   s_tl = 2 s - w_s - nu ./ rho            (solver.jl:55)
 //   w_s  = w_s + alpha (s_tl - s)           (solver.jl:64)
+//   tm   = rho .* (A y1)                    (optional: the warm-start product of the next CG solve, as EpiScale)
 template <typename T>
 struct EpiAdmmTail {
   static constexpr int NS = 0, NM = 0;
@@ -376,8 +434,10 @@ struct EpiAdmmTail {
   const T* ws_in;
   T* ws_out;
   T alpha;
+  T* tm;          // may be nullptr
   __device__ void row(int r, T sum, T*, T*) const {
     const T rh = rho[r];
+    if (tm) tm[r] = rh * sum;
     const T nu = rh * (sum - x2[r]);
     const T sr = s[r], w = ws_in[r];
     const T s_tl = T(2) * sr - w - nu / rh;

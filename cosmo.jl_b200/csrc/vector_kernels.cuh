@@ -355,6 +355,8 @@ template <typename T>
 __global__ void __launch_bounds__(kBlock) cg_init_kernel(int n, const T* __restrict__ rhs, const T* __restrict__ c,
                                                          T* __restrict__ r, T* __restrict__ u, RedBuf<T> rb,
                                                          CgInitFin<T> fin, bool p2p, P2pView<T> xv) {
+  pdl_launch_dependents();
+  pdl_wait();
   T accS[2] = {0, 0};
   T accM[1] = {0};
   unsigned slot = 0;
@@ -379,6 +381,8 @@ __global__ void __launch_bounds__(kBlock) cg_init_kernel(int n, const T* __restr
 template <typename T>
 __global__ void __launch_bounds__(kBlock) cg_update_u_kernel(int n, const T* __restrict__ r, T* __restrict__ u,
                                                              const T* __restrict__ sc, const int* __restrict__ isc) {
+  pdl_launch_dependents();
+  pdl_wait();
   if (isc[ISC_DONE]) return;
   const T res = sc[SC_RES], prev = sc[SC_PREV];
   const T beta = (res * res) / (prev * prev);
@@ -407,6 +411,8 @@ __global__ void __launch_bounds__(kBlock) cg_update_xr_kernel(int n, const T* __
                                                               T* __restrict__ r, const T* __restrict__ sc,
                                                               const int* __restrict__ isc, RedBuf<T> rb,
                                                               CgStepFin<T> fin, bool p2p, P2pView<T> xv) {
+  pdl_launch_dependents();
+  pdl_wait();
   if (isc[ISC_DONE]) return;
   const T res = sc[SC_RES];
   unsigned slot = 0;

@@ -375,7 +375,7 @@ class Engine:
         return tuple(out)
 
     def spmv(self, which, x):
-        size_in = self.m if which == 1 else self.n
+        size_in = self.m if which == 1 else self.n + self.m if which == 3 else self.n
         size_out = self.m if which == 0 else self.n
         x = self._vec(x, size_in)
         y = np.empty(size_out, dtype=self.dtype)

@@ -275,7 +275,8 @@ int cosmo_b200_kkt_solve(cosmo_b200_handle* h, const void* rhs, void* sol, int64
    for given (x, s, mu); out = {r_prim, r_dual, max_norm_prim, max_norm_dual, cost} */
 int cosmo_b200_residuals(cosmo_b200_handle* h, const void* x, const void* s, const void* mu,
                          int32_t ignore_scaling, double out[5]);
-/* y = M x for M in {0: A, 1: A', 2: P} (the mul! calls at kktsolver_indirect.jl:53-63) */
+/* y = M x for M in {0: A, 1: A', 2: P} (the mul! calls at kktsolver_indirect.jl:53-63); 3: y = A' x2 + P x1 + sigma x1
+   for x = [x1; x2] in R^{n+m}, y in R^n (the second half of the reduced KKT operator, kktsolver_indirect.jl:61-63) */
 int cosmo_b200_spmv(cosmo_b200_handle* h, int32_t which, const void* x, void* y);
 /* time `reps` back-to-back launches of one SpMV kernel with CUDA events; returns ms per launch */
 int cosmo_b200_spmv_bench(cosmo_b200_handle* h, int32_t which, int32_t reps, double* ms_per_launch,
