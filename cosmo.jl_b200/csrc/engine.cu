@@ -17,6 +17,7 @@
 
 #include <algorithm>
 #include <functional>
+#include <mutex>
 #include <thread>
 #include <chrono>
 #include <string>
@@ -111,10 +112,18 @@ struct DevCsr {
   bool windowed = false;
   int nwin = 0, W = 0, nctas = 0;
   DevBuf<int> w_rowptr, w_cta_rows;
-  DevBuf<unsigned short> w_col;
+  DevBuf<unsigned short> w_col;   // 10 B layout
   DevBuf<T> w_val;
-  long long w_elems = 0;
-  WcsrView<T> wview() const { return WcsrView<T>{w_rowptr.p, w_col.p, w_val.p, w_cta_rows.p, nwin, W, nrows, ncols}; }
+  bool packed = false;            // 9 B layout (fp64 only, win_pack.h): w_word + w_colhi + w_esc replace w_val + w_col
+  int ebase = 0;
+  DevBuf<unsigned long long> w_word;
+  DevBuf<unsigned char> w_colhi;
+  DevBuf<double> w_esc;
+  long long w_elems = 0, w_nesc = 0;
+  WcsrView<T> wview() const {
+    return WcsrView<T>{w_rowptr.p, w_col.p, w_val.p, w_word.p, w_colhi.p, w_esc.p, winpack::exp_offset(ebase), w_cta_rows.p,
+                       nwin, W, nrows, ncols};
+  }
   CsrView<T> view() const { return CsrView<T>{rowptr.p, col.p, val.p}; }
   double spmv_bytes() const {  // SURVEY.md 8d: 12 nnz + 4 (rows+1) + 8 cols + 8 rows   (fp64)
     return (double)nnz * (sizeof(T) + 4) + 4.0 * (nrows + 1) + (double)sizeof(T) * ncols + (double)sizeof(T) * nrows;
@@ -354,7 +363,7 @@ class Engine : public EngineBase {
   void upload_vec(DevBuf<T>& dst, const void* host, size_t count);
   void download_vec(void* host, const T* src, size_t count);
   void build_csr(DevCsr<T>& dst, const HostCsr& h);
-  void build_windows(DevCsr<T>& dst, const HostCsr& h);
+  void build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packed);
   void classify_and_set_rho(bool reset_rho, bool rebuild_vec = true);
   void allreduce_sum(T* buf, size_t count);
   void allreduce_max(T* buf, size_t count);
@@ -364,6 +373,8 @@ class Engine : public EngineBase {
                    RedBuf<T> rb, const char* name, T* pbuf = nullptr);
   template <typename Epi, int PL>
   void launch_win(const DevCsr<T>& M1, const T* x1, CsrView<T> v2, const T* x2, const Epi& epi, RedBuf<T> rb, T* pbuf);
+  template <typename Epi, int PL, bool PACKED>
+  void launch_win_layout(const DevCsr<T>& M1, const T* x1, CsrView<T> v2, const T* x2, const Epi& epi, RedBuf<T> rb, T* pbuf);
   void project_device(const T* w, bool with_rhs, const T* ws_rhs);
   void soc_norms(const T* ws, T* norm_out);
   void kkt_core(bool fused_tail, const T* w_src, T* w_dst);
@@ -518,9 +529,78 @@ static void win_fill_segment(const int* cols, const double* vals, const int* idx
   }
 }
 
+// The 9 B layout of an fp64 slab (win_pack.h), built from the 10 B one in place: every 8-byte value becomes its packed
+// word at the same position, and the high column bits go to `colhi` at the column's position.  Escapes are numbered in
+// slab order (window-major, then row, then entry order of the segment), so the table does not depend on the thread
+// count.  Returns false, and leaves wv untouched, when more than 1/kEscDen of the stored entries would be escapes.
+namespace {
+struct WinPacked {
+  int ebase = 0;
+  std::vector<unsigned char> colhi;
+  std::vector<double> esc;
+};
+}  // namespace
+
+template <typename RowLoop>
+static bool win_pack(const std::vector<double>& hval, const std::vector<int>& rp, int nr, int nwin, long long total,
+                     const std::vector<unsigned short>& wc, std::vector<double>& wv, WinPacked& out, RowLoop parallel_rows) {
+  namespace wp = winpack;
+  // exponent window: the kCodes consecutive binades that hold the most finite normal values of the matrix
+  std::vector<long long> hist(2048, 0);
+  {
+    std::mutex mu;
+    parallel_rows([&](int a, int b) {
+      std::vector<long long> hl(2048, 0);
+      const long long k0 = (long long)hval.size() * a / nr, k1 = (long long)hval.size() * b / nr;
+      for (long long k = k0; k < k1; ++k) hl[wp::normal_exponent(hval[k])]++;
+      std::lock_guard<std::mutex> g(mu);
+      for (int e = 0; e < 2048; ++e) hist[e] += hl[e];
+    });
+  }
+  const int ebase = wp::pick_ebase(hist.data());
+  // escapes per row segment, in slab order
+  std::vector<long long> esc_off((size_t)nwin * nr + 1, 0);
+  parallel_rows([&](int a, int b) {
+    for (int w = 0; w < nwin; ++w)
+      for (int r = a; r < b; ++r) {
+        long long c = 0;
+        for (int p = rp[(size_t)w * (nr + 1) + r]; p < rp[(size_t)w * (nr + 1) + r + 1]; ++p) c += wp::code_of(wv[p], ebase) == wp::kEscape;
+        esc_off[(size_t)w * nr + r + 1] = c;
+      }
+  });
+  for (size_t i = 1; i < esc_off.size(); ++i) esc_off[i] += esc_off[i - 1];
+  const long long nesc = esc_off.back();
+  if (nesc * wp::kEscDen > total) return false;
+  out.ebase = ebase;
+  out.colhi.assign((size_t)total + 8, 0);
+  out.esc.assign((size_t)nesc, 0.0);
+  parallel_rows([&](int a, int b) {
+    for (int w = 0; w < nwin; ++w)
+      for (int r = a; r < b; ++r) {
+        const int s = rp[(size_t)w * (nr + 1) + r], kpad = rp[(size_t)w * (nr + 1) + r + 1] - s;
+        long long ei = esc_off[(size_t)w * nr + r];
+        for (int idx = 0; idx < kpad; ++idx) {   // the entry order of the kernel: step, lane, slot
+          const int st = idx >> 8, l = (idx & 255) >> 3, i = idx & 7;
+          const int ls = std::min(32, (kpad >> 3) - 32 * st);
+          const long long pc = (long long)s + idx;
+          const long long pv = (long long)s + (long long)st * 256 + (long long)(i / 2) * (2 * ls) + (long long)l * 2 + (i % 2);
+          const double v = wv[pv];
+          const unsigned col = wc[pc];
+          uint32_t slot = 0;
+          if (wp::code_of(v, ebase) == wp::kEscape) { slot = (uint32_t)ei; out.esc[(size_t)ei++] = v; }
+          const uint64_t word = wp::encode_word(v, col, ebase, slot);
+          memcpy(&wv[pv], &word, 8);
+          out.colhi[pc] = wp::encode_colhi(col);
+        }
+      }
+  });
+  return true;
+}
+
 template <typename T>
-void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h) {
+void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packed) {
   dst.windowed = false;
+  dst.packed = false;
   if (h.nrows == 0 || h.ncols == 0) return;
   const long long nnz = (long long)h.col.size();
   const int Wmax = (int)(204800 / sizeof(T));
@@ -600,9 +680,31 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h) {
   dst.nwin = nwin; dst.W = W; dst.nctas = nctas; dst.w_elems = total;
   dst.w_rowptr.upload(rp, stream_);
   dst.w_cta_rows.upload(cta_rows, stream_);
-  dst.w_col.upload(wc, stream_);
-  dst.w_val.upload(wv, stream_);
-  sync();
+  // fp64: the 9 B layout unless the values need too many escapes, or device equilibration will rewrite the slab values
+  // in place (ruiz_apply_win_kernel works on the 10 B layout)
+  if constexpr (sizeof(T) == sizeof(double)) {
+    WinPacked pk;
+    if (allow_packed && W - 1 <= (int)winpack::kMaxCol && win_pack(h.val, rp, nr, nwin, total, wc, wv, pk, parallel_rows)) {
+      dst.packed = true;
+      dst.ebase = pk.ebase;
+      dst.w_nesc = (long long)pk.esc.size();
+      dst.w_word.alloc(wv.size(), false);
+      dst.w_word.upload(reinterpret_cast<const unsigned long long*>(wv.data()), wv.size(), stream_);
+      dst.w_colhi.upload(pk.colhi, stream_);
+      dst.w_esc.upload(pk.esc, stream_);
+      sync();
+    }
+  }
+  if (!dst.packed) {
+    dst.w_col.upload(wc, stream_);
+    dst.w_val.upload(wv, stream_);
+    sync();
+  }
+  if (getenv("COSMO_B200_SETUP_DEBUG") != nullptr) {
+    const double bytes = (double)total * (dst.packed ? 9 : sizeof(T) + 2) + 8.0 * dst.w_nesc;
+    fprintf(stderr, "[setup] windows %d x %d, %d rows: %s layout, ebase %d, %lld escapes, slab %.1f MB\n", nwin, W, nr,
+            dst.packed ? "9 B" : sizeof(T) == 8 ? "10 B" : "6 B", dst.ebase, dst.w_nesc, bytes / 1e6);
+  }
   dst.windowed = true;
 }
 
@@ -797,16 +899,18 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
       if (dbg) { const double t = now_s(); fprintf(stderr, "[setup] %-22s %.3f s\n", what, t - tp); tp = t; }
     };
     lap("cone tables");
+    // device equilibration rewrites the slab values in place, which only the 10 B slab layout allows
+    const bool pack_ok = !((p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0);
     HostCsr a, at, pp, ppt;
     csc_to_host_csrs<T>(p.A, p.index_base, a, at);
     lap("csc -> csr (A, A')");
     build_csr(A_, a);
     lap("upload csr A");
-    build_windows(A_, a);
+    build_windows(A_, a, pack_ok);
     lap("windows A");
     build_csr(At_, at);
     lap("upload csr A'");
-    build_windows(At_, at);
+    build_windows(At_, at, pack_ok);
     lap("windows A'");
     csc_to_host_csrs<T>(p.P, p.index_base, pp, ppt);
     build_csr(P_, pp);
@@ -984,6 +1088,7 @@ void Engine<T>::equilibrate() {
     }
   }
   // apply D, E, c to every copy of the data
+  if (A_.packed || At_.packed) throw EngineError{COSMO_B200_ERR_INVALID, "device equilibration of a packed (9 B) slab"};
   ruiz_apply_csr_kernel<T><<<wgrid(m), kBlock, 0, stream_>>>(m, A_.rowptr.p, A_.col.p, A_.val.p, E_.p, D_.p, (const T*)nullptr);
   ruiz_apply_csr_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, At_.val.p, D_.p, E_.p, (const T*)nullptr);
   ruiz_apply_csr_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.val.p, D_.p, D_.p, cdev.p);
@@ -1183,15 +1288,28 @@ template <typename T>
 template <typename Epi, int PL>
 void Engine<T>::launch_win(const DevCsr<T>& M1, const T* x1, CsrView<T> v2, const T* x2, const Epi& epi, RedBuf<T> rb,
                            T* pbuf) {
+  if constexpr (sizeof(T) == sizeof(double)) {
+    if (M1.packed) {
+      launch_win_layout<Epi, PL, true>(M1, x1, v2, x2, epi, rb, pbuf);
+      return;
+    }
+  }
+  launch_win_layout<Epi, PL, false>(M1, x1, v2, x2, epi, rb, pbuf);
+}
+
+template <typename T>
+template <typename Epi, int PL, bool PACKED>
+void Engine<T>::launch_win_layout(const DevCsr<T>& M1, const T* x1, CsrView<T> v2, const T* x2, const Epi& epi,
+                                  RedBuf<T> rb, T* pbuf) {
   const size_t smem = (size_t)M1.W * sizeof(T);
-  // function attributes are per device: one flag per (T, Epi, PL) instantiation AND device ordinal
+  // function attributes are per device: one flag per (T, PACKED, Epi, PL) instantiation AND device ordinal
   static bool configured[64] = {false};
   const int dev_slot = device_ & 63;
   if (!configured[dev_slot] || device_ >= 64) {
-    CUDA_TRY(cudaFuncSetAttribute(spmv_win_kernel<T, Epi, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204800));
+    CUDA_TRY(cudaFuncSetAttribute(spmv_win_kernel<T, PACKED, Epi, PL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 204800));
     configured[dev_slot] = true;
   }
-  launch_pdl(spmv_win_kernel<T, Epi, PL>, M1.nctas, kWinThreads, smem, stream_, M1.wview(), x1, v2, x2, epi, rb, ypart_.p,
+  launch_pdl(spmv_win_kernel<T, PACKED, Epi, PL>, M1.nctas, kWinThreads, smem, stream_, M1.wview(), x1, v2, x2, epi, rb, ypart_.p,
              chunk_ticket_.p, pbuf);
 }
 

@@ -16,6 +16,7 @@
 // 4-element boundary so that the streams stay 16/32-byte aligned.
 #pragma once
 #include "common.cuh"
+#include "win_pack.h"
 
 namespace cosmo {
 
@@ -118,18 +119,26 @@ __global__ void __launch_bounds__(kBlock) spmv_kernel(CsrView<T> M1, const T* __
 // `nwin` column slabs ("windows") of width W <= 25.6k doubles; a persistent CTA
 // per SM pulls the W-slice of x into its 200 KB of shared memory with one TMA
 // bulk copy (cp.async.bulk + mbarrier), then streams its rows of that slab
-// from HBM (8-byte values + 16-bit window-local column indices, rows padded to
-// 8 entries so every lane issues aligned 128-bit loads; values are laid out so
-// that each warp-wide load instruction covers one contiguous 512-byte run) and
-// gathers from shared memory.  Partial row sums are carried between
-// windows in a small global vector; the epilogue runs on the last window.
-// Algorithmic HBM traffic drops from 12 to 10 B/nnz (+1.4 % padding).
+// from HBM and gathers from shared memory.  Rows are padded to 8 entries so
+// every lane issues aligned loads; values are laid out so that each warp-wide
+// load instruction covers one contiguous 512-byte run.  Partial row sums are
+// carried between windows in a small global vector; the epilogue runs on the
+// last window.  Two slab layouts (the PACKED template argument):
+//   10 B per entry: 8-byte values + 16-bit window-local column indices.
+//    9 B per entry (fp64 only, win_pack.h): an 8-byte word holding sign, a 4-bit exponent code, the low 7 column bits
+//                   and the mantissa, where the value sits in the 10 B layout, and one byte of high column bits, where
+//                   the column sits.  The decode is exact, so both layouts compute the same sums bit for bit.
+// Streamed HBM traffic is 10 or 9 B/nnz (+1.4 % padding on C2), against 12 for plain CSR.
 // ---------------------------------------------------------------------------
 template <typename T>
 struct WcsrView {
   const int* rowptr;            // nwin * (nrows + 1), element offsets (multiples of 8)
-  const unsigned short* col;    // window-local column index
-  const T* val;
+  const unsigned short* col;    // 10 B layout: window-local column index
+  const T* val;                 // 10 B layout: value
+  const unsigned long long* word;   // 9 B layout: packed words (win_pack.h)
+  const unsigned char* colhi;       // 9 B layout: column bits 7-14
+  const double* esc;                // 9 B layout: escaped values
+  unsigned kexp;                    // 9 B layout: winpack::exp_offset(ebase)
   const int* cta_row_start;     // gridDim.x + 1 contiguous row chunks, balanced by nnz
   int nwin, W, nrows, ncols;
 };
@@ -137,32 +146,85 @@ struct WcsrView {
 constexpr int kWinThreads = 1024;
 constexpr int kWinWarps = kWinThreads / 32;
 
-// gather-FMA of one lane's 8 (value, local column) pairs against the staged x slice
-template <typename T>
-__device__ __forceinline__ T win_fma8(const T (&v)[8], const uint4& c, const T* xs) {
-  T s0 = v[0] * xs[c.x & 0xffffu];
-  T s1 = v[1] * xs[c.x >> 16];
-  s0 += v[2] * xs[c.y & 0xffffu];
-  s1 += v[3] * xs[c.y >> 16];
-  s0 += v[4] * xs[c.z & 0xffffu];
-  s1 += v[5] * xs[c.z >> 16];
-  s0 += v[6] * xs[c.w & 0xffffu];
-  s1 += v[7] * xs[c.w >> 16];
+// One lane's 8 entries of a slab step, as loaded: `v` from the value (or word) stream, `c` from the column stream.
+// val(i) / col(i) give entry i; the packed layout decodes it here, right before its FMA.
+template <typename T, bool PACKED>
+struct WinStep {
+  using Col = uint4;
+  T v[8];
+  Col c;
+  __device__ __forceinline__ void clear() {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = T(0);
+    c = make_uint4(0, 0, 0, 0);
+  }
+  __device__ __forceinline__ void load(const WcsrView<T>& M, int s, int L, int lane) {
+    c = __ldcs(reinterpret_cast<const uint4*>(M.col + s + lane * 8));
+    load8_coalesced(M.val + s, L, lane, v);
+  }
+  __device__ __forceinline__ T val(const WcsrView<T>&, int i) const { return v[i]; }
+  __device__ __forceinline__ unsigned col(int i) const {
+    const unsigned w = i < 2 ? c.x : i < 4 ? c.y : i < 6 ? c.z : c.w;
+    return (i & 1) ? w >> 16 : w & 0xffffu;
+  }
+};
+template <>
+struct WinStep<double, true> {
+  double v[8];   // packed words, loaded through the double path of load8_coalesced
+  uint2 c;       // 8 column-high bytes
+  __device__ __forceinline__ void clear() {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = 0.0;
+    c = make_uint2(0, 0);
+  }
+  __device__ __forceinline__ void load(const WcsrView<double>& M, int s, int L, int lane) {
+    c = __ldcs(reinterpret_cast<const uint2*>(M.colhi + s + lane * 8));
+    load8_coalesced(reinterpret_cast<const double*>(M.word) + s, L, lane, v);
+  }
+  // an escape reads its value from the table with a predicated load, not a branch
+  __device__ __forceinline__ double val(const WcsrView<double>& M, int i) const {
+    const unsigned hi = (unsigned)__double2hiint(v[i]), lo = (unsigned)__double2loint(v[i]);
+    double d = __hiloint2double((int)winpack::decode_hi(hi, M.kexp), (int)lo);
+    if (winpack::is_escape(hi)) d = __ldg(M.esc + lo);
+    return d;
+  }
+  __device__ __forceinline__ unsigned col(int i) const {
+    const unsigned hb = __byte_perm(i < 4 ? c.x : c.y, 0u, (unsigned)(i & 3) | 0x4440u);
+    return winpack::decode_col((unsigned)__double2hiint(v[i]), hb);
+  }
+};
+
+__device__ __forceinline__ double win_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ float win_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double win_fma(double a, double b, double c) { return __fma_rn(a, b, c); }
+__device__ __forceinline__ float win_fma(float a, float b, float c) { return __fmaf_rn(a, b, c); }
+
+// gather-FMA of one lane's 8 entries against the staged x slice.  The roundings are spelled out, so that both layouts
+// (and every build) sum in the same order: s0 = v0 x0 + v2 x2 + v4 x4 + v6 x6 with the product v2 x2 rounded and the
+// others fused, s1 likewise over the odd slots.
+template <typename T, bool PACKED>
+__device__ __forceinline__ T win_fma8(const WinStep<T, PACKED>& e, const WcsrView<T>& M, const T* xs) {
+  T s0 = win_mul(e.val(M, 2), xs[e.col(2)]);
+  T s1 = win_mul(e.val(M, 3), xs[e.col(3)]);
+  s0 = win_fma(e.val(M, 0), xs[e.col(0)], s0);
+  s1 = win_fma(e.val(M, 1), xs[e.col(1)], s1);
+  s0 = win_fma(e.val(M, 4), xs[e.col(4)], s0);
+  s1 = win_fma(e.val(M, 5), xs[e.col(5)], s1);
+  s0 = win_fma(e.val(M, 6), xs[e.col(6)], s0);
+  s1 = win_fma(e.val(M, 7), xs[e.col(7)], s1);
   return s0 + s1;
 }
 
 // steps beyond the first 256 entries of a row segment (long rows)
-template <typename T>
-__device__ __forceinline__ T win_row_rest(const unsigned short* __restrict__ col, const T* __restrict__ val, const T* xs,
-                                          int start, int end, int lane) {
+template <typename T, bool PACKED>
+__device__ __forceinline__ T win_row_rest(const WcsrView<T>& M, const T* xs, int start, int end, int lane) {
   T s = 0;
   for (int j0 = start + 256; j0 < end; j0 += 256) {
     const int L = min(32, (end - j0) >> 3);
     if (lane < L) {
-      const uint4 c = __ldcs(reinterpret_cast<const uint4*>(col + j0 + lane * 8));
-      T v[8];
-      load8_coalesced(val + j0, L, lane, v);
-      s += win_fma8<T>(v, c, xs);
+      WinStep<T, PACKED> e;
+      e.load(M, j0, L, lane);
+      s += win_fma8<T, PACKED>(e, M, xs);
     }
   }
   return s;
@@ -181,7 +243,7 @@ __device__ __forceinline__ T win_row_rest(const unsigned short* __restrict__ col
 // the CTA sums them before streaming, behind a CTA barrier.  Every P row is summed exactly as
 // spmv_kernel<T, PL, EpiStore> sums it (row_partial + group_sum with the same PL), so the result is bitwise that of a
 // separate P launch.  PL = 0: no P rows (M2, x2 and pbuf unused).
-template <typename T, typename Epi, int PL = 0>
+template <typename T, bool PACKED, typename Epi, int PL = 0>
 __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M, const T* __restrict__ x, CsrView<T> M2,
                                                                   const T* __restrict__ x2, Epi epi, RedBuf<T> rb,
                                                                   T* __restrict__ ypart, unsigned* __restrict__ chunk_ticket,
@@ -274,25 +336,25 @@ __global__ void __launch_bounds__(kWinThreads, 1) spmv_win_kernel(WcsrView<T> M,
     const bool has_b = (k + 1 < nmine);
     const int ja = sa + lane * 8, jb = sb + lane * 8;
     const bool la = ja < ea, lb = jb < eb;
-    uint4 cxa = make_uint4(0, 0, 0, 0), cxb = make_uint4(0, 0, 0, 0);
-    T va[8], vb[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { va[i] = T(0); vb[i] = T(0); }
-    if (la) { cxa = __ldcs(reinterpret_cast<const uint4*>(M.col + ja)); load8_coalesced(M.val + sa, min(32, (ea - sa) >> 3), lane, va); }
-    if (lb) { cxb = __ldcs(reinterpret_cast<const uint4*>(M.col + jb)); load8_coalesced(M.val + sb, min(32, (eb - sb) >> 3), lane, vb); }
-    const int csa = sa, cea = ea, csb = sb, ceb = eb;
+    WinStep<T, PACKED> stepa, stepb;
+    stepa.clear();
+    stepb.clear();
+    if (la) stepa.load(M, sa, min(32, (ea - sa) >> 3), lane);
+    if (lb) stepb.load(M, sb, min(32, (eb - sb) >> 3), lane);
+    // long segments (> one 256-entry step) re-read their row pointers after the first step instead of holding them
+    const bool longa = ea - sa > 256, longb = eb - sb > 256;
     fetch_ptrs(k + 2, sa, ea, sb, eb);          // next pair
     if (!waited) {
       if (!staged && !stage_x()) return;
       mbar_wait(&bar, 0);
       waited = true;
     }
-    T pa = la ? win_fma8<T>(va, cxa, xs) : T(0);
-    T pb = lb ? win_fma8<T>(vb, cxb, xs) : T(0);
-    if (cea - csa > 256) pa += win_row_rest<T>(M.col, M.val, xs, csa, cea, lane);
-    if (ceb - csb > 256) pb += win_row_rest<T>(M.col, M.val, xs, csb, ceb, lane);
+    T pa = la ? win_fma8<T, PACKED>(stepa, M, xs) : T(0);
+    T pb = lb ? win_fma8<T, PACKED>(stepb, M, xs) : T(0);
     const int rowa = r0 + warp + k * kWinWarps;
     const int rowb = rowa + kWinWarps;
+    if (longa) pa += win_row_rest<T, PACKED>(M, xs, __ldg(rp + rowa), __ldg(rp + rowa + 1), lane);
+    if (longb) pb += win_row_rest<T, PACKED>(M, xs, __ldg(rp + rowb), __ldg(rp + rowb + 1), lane);
     // paired reduction: lanes 0-15 fold row a, lanes 16-31 fold row b (5 shuffles for 2 rows)
     const bool hi = (lane & 16) != 0;
     T keep = hi ? pb : pa;
