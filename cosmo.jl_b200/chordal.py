@@ -591,29 +591,8 @@ def psd_complete(Y: np.ndarray, tree: CliqueTree, assume_symmetric: bool = False
     if not assume_symmetric:                 # the reference reads the upper triangle
         W = np.triu(W) + np.triu(W, 1).T
     N = W.shape[0]
-    ncl = len(tree.cliques)
-    children: List[List[int]] = [[] for _ in range(ncl)]
-    roots = []
-    for k, p in enumerate(tree.parent):
-        (children[p] if p >= 0 else roots).append(k)
     # traversal order (parents first) and the renumbering it induces
-    order_k: List[int] = []
-    stack = list(reversed(roots))
-    while stack:
-        k = stack.pop()
-        order_k.append(k)
-        stack.extend(reversed(children[k]))
-    new_of = np.full(N, -1, dtype=np.int64)
-    nxt = 0
-    residuals: Dict[int, np.ndarray] = {}
-    for k in order_k:
-        c = np.asarray(tree.cliques[k], dtype=np.int64)
-        fresh = c[new_of[c] < 0]
-        residuals[k] = fresh
-        new_of[fresh] = np.arange(nxt, nxt + len(fresh))
-        nxt += len(fresh)
-    rest = np.nonzero(new_of < 0)[0]                       # vertices in no clique (cannot happen for a clique tree)
-    new_of[rest] = np.arange(nxt, nxt + len(rest))
+    order_k, new_of, residuals = _traversal(tree, N)
     perm = np.argsort(new_of)                              # perm[new] = old
     W = W[np.ix_(perm, perm)]
     seen = 0
@@ -706,6 +685,218 @@ def _mat_to_svec(X: np.ndarray) -> np.ndarray:
     j = np.arange(N, dtype=np.int64)
     v[j * (j + 1) // 2 + j] = np.diagonal(X)
     return v
+
+
+def _traversal(tree: CliqueTree, N: int):
+    """The clique order of `psd_complete` (parents first, children in order), its renumbering `new_of` (visited vertices
+    form a leading block) and the residual of every clique."""
+    ncl = len(tree.cliques)
+    children: List[List[int]] = [[] for _ in range(ncl)]
+    roots = []
+    for k, p in enumerate(tree.parent):
+        (children[p] if p >= 0 else roots).append(k)
+    order_k: List[int] = []
+    stack = list(reversed(roots))
+    while stack:
+        k = stack.pop()
+        order_k.append(k)
+        stack.extend(reversed(children[k]))
+    new_of = np.full(N, -1, dtype=np.int64)
+    nxt = 0
+    residuals: Dict[int, np.ndarray] = {}
+    for k in order_k:
+        c = np.asarray(tree.cliques[k], dtype=np.int64)
+        fresh = c[new_of[c] < 0]
+        residuals[k] = fresh
+        new_of[fresh] = np.arange(nxt, nxt + len(fresh))
+        nxt += len(fresh)
+    rest = np.nonzero(new_of < 0)[0]
+    new_of[rest] = np.arange(nxt, nxt + len(rest))
+    return order_k, new_of, residuals
+
+
+@dataclass
+class CompletionSchedule:
+    """`psd_complete` of one N x N matrix as flat int64 arrays.  Step t (traversal order) completes the residual
+    nu = new indices lo..hi-1 against the leading block 0..lo-1 (lo = hi of the step before, 0 for the first):
+        W[r, nu] = W[r, alpha] Z,  W[alpha, alpha] Z = W[alpha, nu],   for every r < lo outside the clique,
+    with alpha = idx[a0:a1] (the separator, new numbering) and idx[k0:k1] the clique's other members below lo, whose
+    entries are known and stay as they are."""
+    N: int
+    row_offset: int            # first original row of the cone (0 for a bare matrix)
+    dim: int                   # rows of the cone: N(N+1)/2 (PsdConeTriangle); N*N (PsdCone) is refused
+    new_of: np.ndarray         # N: old vertex -> traversal position
+    steps: np.ndarray          # (n_steps, 6): lo, hi, a0, a1, k0, k1
+    idx: np.ndarray
+
+
+@dataclass
+class DecompositionArrays:
+    """The map of `reverse` as flat int64 arrays (decomposition_arrays): plain rows are copied; an original row of a
+    decomposed cone gets s = 0.0 + the clique rows s_src[s_ptr[i]:s_ptr[i+1]] in that order and mu = mu_src[i] (the
+    last of them, the row the host loop writes last); rows in no clique stay 0."""
+    n_orig: int
+    m_orig: int
+    n: int                     # decomposed problem
+    m: int
+    plain: np.ndarray          # (n_plain, 3): old_start, new_start, dim
+    row: np.ndarray            # original rows of the decomposed cones, increasing
+    s_ptr: np.ndarray          # len(row) + 1
+    s_src: np.ndarray          # decomposed rows
+    mu_src: np.ndarray         # len(row)
+    cones: List[CompletionSchedule] = field(default_factory=list)
+
+
+def completion_schedule(tree: CliqueTree, N: int, row_offset: int = 0) -> CompletionSchedule:
+    order_k, new_of, residuals = _traversal(tree, N)
+    steps, idx = [], []
+    seen = 0
+    for k in order_k:
+        nn = len(residuals[k])
+        alpha = new_of[np.asarray(tree.sep[k], dtype=np.int64)] if tree.parent[k] >= 0 else np.zeros(0, dtype=np.int64)
+        c_new = new_of[np.asarray(tree.cliques[k], dtype=np.int64)]
+        other = c_new[(c_new < seen) & ~np.isin(c_new, alpha)]
+        a0 = len(idx)
+        idx.extend(alpha.tolist())
+        k0 = len(idx)
+        idx.extend(other.tolist())
+        steps.append((seen, seen + nn, a0, k0, k0, len(idx)))
+        seen += nn
+    return CompletionSchedule(int(N), int(row_offset), int(N) * (int(N) + 1) // 2, new_of, np.array(steps, dtype=np.int64).reshape(-1, 6),
+                              np.array(idx, dtype=np.int64))
+
+
+def decomposition_arrays(info: DecompositionInfo, n: Optional[int] = None, m: Optional[int] = None) -> DecompositionArrays:
+    """Flatten `info` for the device reverse (cosmo_b200_set_decomposition).  n, m: size of the decomposed problem
+    (default: what the blocks and row map imply)."""
+    plain = np.array(info.row_map_plain, dtype=np.int64).reshape(-1, 3)
+    orig_l, src_l = [], []
+    cones = []
+    m_imp = int((plain[:, 1] + plain[:, 2]).max()) if len(plain) else 0
+    for k, blocks in info.blocks.items():                      # set order, then clique order: the host's loop
+        S = info.sets_orig[k]
+        off = info.cone_offsets[k]
+        for start, c in blocks:
+            c = np.asarray(c, dtype=np.int64)
+            nc = len(c)
+            ai, bj = svec_to_ij(np.arange(nc * (nc + 1) // 2, dtype=np.int64))
+            gi, gj = c[ai], c[bj]
+            orig_l.append(off + gj * (gj + 1) // 2 + gi)
+            src_l.append(start + np.arange(nc * (nc + 1) // 2, dtype=np.int64))
+            m_imp = max(m_imp, start + nc * (nc + 1) // 2)
+        sched = completion_schedule(info.trees[k], S.sqrt_dim, off)
+        sched.dim = S.dim                                      # a PsdCone would show N*N here and be refused
+        cones.append(sched)
+    orig = np.concatenate(orig_l) if orig_l else np.zeros(0, dtype=np.int64)
+    src = np.concatenate(src_l) if src_l else np.zeros(0, dtype=np.int64)
+    perm = np.argsort(orig, kind="stable")                     # keeps the host's summation order within a row
+    orig, src = orig[perm], src[perm]
+    row, first, counts = np.unique(orig, return_index=True, return_counts=True)
+    s_ptr = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    mu_src = src[s_ptr[1:] - 1] if len(row) else np.zeros(0, dtype=np.int64)
+    return DecompositionArrays(int(info.n_orig), int(info.m_orig), int(n if n is not None else info.n_orig + info.num_overlaps),
+                               int(m if m is not None else m_imp), plain, row.astype(np.int64), s_ptr, src.astype(np.int64),
+                               mu_src.astype(np.int64), cones)
+
+
+def validate_schedule(c: CompletionSchedule, m_orig: Optional[int] = None) -> None:
+    """The checks cosmo_b200_set_decomposition / cosmo_b200_psd_complete apply to a schedule: ValueError if one fails."""
+    N = int(c.N)
+    if N < 1:
+        raise ValueError("schedule: N must be positive")
+    if m_orig is not None and c.dim == N * N and N > 1:
+        raise NotImplementedError("schedule: the square PsdCone layout is not supported")
+    if m_orig is not None and (c.dim != N * (N + 1) // 2 or not (0 <= c.row_offset and c.row_offset + c.dim <= m_orig)):
+        raise ValueError("schedule: cone rows out of range")
+    new_of = np.asarray(c.new_of)
+    if new_of.shape != (N,) or not np.array_equal(np.sort(new_of), np.arange(N)):
+        raise ValueError("schedule: new_of is not a permutation of 0..N-1")
+    st = np.asarray(c.steps).reshape(-1, 6)
+    idx = np.asarray(c.idx)
+    lo_expect = 0
+    for t, (lo, hi, a0, a1, k0, k1) in enumerate(st.tolist()):
+        if lo != lo_expect or hi < lo or hi > N:
+            raise ValueError("schedule: step %d does not continue the leading block" % t)
+        if not (0 <= a0 <= a1 == k0 <= k1 <= len(idx)):
+            raise ValueError("schedule: step %d index ranges are inconsistent" % t)
+        known = idx[a0:k1]
+        if len(known) and (known.min() < 0 or known.max() >= lo):
+            raise ValueError("schedule: step %d refers to a vertex outside the leading block" % t)
+        lo_expect = hi
+
+
+def validate_decomposition_arrays(d: DecompositionArrays) -> None:
+    """Every index in range and the maps consistent (the checks the C ABI applies): ValueError otherwise."""
+    if min(d.n_orig, d.m_orig, d.n, d.m) < 0 or d.n_orig > d.n:
+        raise ValueError("decomposition: bad dimensions")
+    pl = np.asarray(d.plain).reshape(-1, 3)
+    if len(pl) and ((pl < 0).any() or (pl[:, 0] + pl[:, 2] > d.m_orig).any() or (pl[:, 1] + pl[:, 2] > d.m).any()):
+        raise ValueError("decomposition: plain rows out of range")
+    row, s_ptr, s_src, mu_src = (np.asarray(a) for a in (d.row, d.s_ptr, d.s_src, d.mu_src))
+    if len(row) and (row.min() < 0 or row.max() >= d.m_orig or (np.diff(row) <= 0).any()):
+        raise ValueError("decomposition: rows out of range or not increasing")
+    if s_ptr.shape != (len(row) + 1,) or s_ptr[0] != 0 or (np.diff(s_ptr) <= 0).any() or s_ptr[-1] != len(s_src):
+        raise ValueError("decomposition: s_ptr is inconsistent")
+    if len(s_src) and (s_src.min() < 0 or s_src.max() >= d.m):
+        raise ValueError("decomposition: s_src out of range")
+    if mu_src.shape != row.shape or (len(row) and not np.array_equal(mu_src, s_src[s_ptr[1:] - 1])):
+        raise ValueError("decomposition: mu_src is not the last clique row of each row")
+    cover = np.zeros(d.m_orig, dtype=np.int8)
+    for old, _, dim in pl.tolist():
+        cover[old:old + dim] += 1
+    cover[row] += 1
+    if (cover > 1).any():
+        raise ValueError("decomposition: an original row is written twice")
+    for c in d.cones:
+        validate_schedule(c, d.m_orig)
+
+
+def reverse_from_arrays(d: DecompositionArrays, x2, s2, mu2):
+    """`reverse(..., complete_dual=False)` replayed from the flat map (what the device gather pass computes)."""
+    x = np.asarray(x2, dtype=np.float64)[:d.n_orig].copy()
+    s = np.zeros(d.m_orig)
+    mu = np.zeros(d.m_orig)
+    s2 = np.asarray(s2, dtype=np.float64)
+    mu2 = np.asarray(mu2, dtype=np.float64)
+    for old, new, dim in np.asarray(d.plain).reshape(-1, 3).tolist():
+        s[old:old + dim] = s2[new:new + dim]
+        mu[old:old + dim] = mu2[new:new + dim]
+    cnt = np.diff(d.s_ptr)
+    acc = np.zeros(len(d.row))
+    for t in range(int(cnt.max()) if len(cnt) else 0):       # position t of every row's list, in list order
+        has = cnt > t
+        acc[has] += s2[d.s_src[d.s_ptr[:-1][has] + t]]
+    s[d.row] = acc
+    mu[d.row] = mu2[d.mu_src]
+    return x, s, mu
+
+
+def psd_complete_from_schedule(Y: np.ndarray, c: CompletionSchedule) -> np.ndarray:
+    """`psd_complete(Y, tree, assume_symmetric=True)` replayed from the flat schedule."""
+    new_of = np.asarray(c.new_of)
+    perm = np.argsort(new_of)
+    W = np.array(Y, dtype=np.float64)[np.ix_(perm, perm)]
+    for lo, hi, a0, a1, k0, k1 in np.asarray(c.steps).reshape(-1, 6).tolist():
+        if lo == 0 or hi == lo:
+            continue
+        al = c.idx[a0:a1]
+        if len(al):
+            Waa = W[np.ix_(al, al)]
+            Wan = W[al, lo:hi]
+            try:
+                Z = np.linalg.solve(Waa, Wan)
+                if not np.all(np.isfinite(Z)):
+                    raise np.linalg.LinAlgError
+            except np.linalg.LinAlgError:
+                Z = np.linalg.pinv(Waa) @ Wan
+            blk = W[:lo, al] @ Z
+        else:
+            blk = np.zeros((lo, hi - lo))
+        known = c.idx[a0:k1]
+        blk[known, :] = W[known, lo:hi]
+        W[:lo, lo:hi] = blk
+        W[lo:hi, :lo] = blk.T
+    return W[np.ix_(new_of, new_of)]
 
 
 def reverse(info: DecompositionInfo, x2, s2, mu2, complete_dual: bool = False):

@@ -34,6 +34,7 @@
 #include "ruiz.cuh"
 #include "cg_persistent.cuh"
 #include "ldl.cuh"
+#include "chordal_rev.cuh"
 
 namespace cosmo {
 
@@ -169,6 +170,8 @@ class EngineBase {
   virtual void infeasibility_test(int which, const void* delta, double* out8) = 0;
   virtual void psd_lambda_max(const void* v, double* lam) = 0;
   virtual void ldl_stats(double* out8) = 0;
+  virtual void set_decomposition(const cosmo_b200_decomposition* d) = 0;
+  virtual void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) = 0;
 };
 
 template <typename T>
@@ -207,6 +210,8 @@ class Engine : public EngineBase {
   void infeasibility_test(int which, const void* delta, double* out8) override;
   void psd_lambda_max(const void* v, double* lam) override;
   void ldl_stats(double* out8) override;
+  void set_decomposition(const cosmo_b200_decomposition* d) override;
+  void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) override;
 
  private:
   // ---- problem ----
@@ -270,6 +275,8 @@ class Engine : public EngineBase {
   double rho_ = 0.1;
   std::vector<double> rho_updates_;
   bool is_optimized_ = false;
+  bool have_solution_ = false;   // xs_, s_, mu_ hold what the last solve() returned (cleared by reset / warm_start)
+  rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   // KKT (reduced CG)
   DevBuf<T> ls_, t0_, tm_, xsol_, rhsb_, cb_, r_, u_, nu_;
   DevBuf<T> mr_[6], mr_x_, mr_c_, mr_b_;   // MINRES Lanczos / direction vectors, solution, operator output, rhs
@@ -1134,6 +1141,7 @@ void Engine<T>::get_scaling(void* D, void* E, double* c) {
 
 template <typename T>
 void Engine<T>::warm_start(const void* x, const void* s, const void* mu) {
+  have_solution_ = false;
   if (x) upload_vec(xs_, x, n_);
   if (s) upload_vec(s_, s, m_);
   if (mu) upload_vec(mu_, mu, m_);
@@ -1172,6 +1180,7 @@ void Engine<T>::reset() {
   kkt_counter_ = 1;
   last_cg_iters_ = 1;
   is_optimized_ = false;
+  have_solution_ = false;
   psd_.reset_warm_start();
   classify_and_set_rho(true);
   sync();
@@ -2186,6 +2195,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
   }
   // x = view(w_prev, 1:n): keep it for the next warm start and hand it out
   CUDA_TRY(cudaMemcpyAsync(xs_.p, W_[prev_].p, n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  have_solution_ = true;
   if (out) {
     if (out->x) download_vec(out->x, W_[prev_].p, n);
     if (out->s) download_vec(out->s, s_.p, m);
@@ -2498,6 +2508,26 @@ void Engine<T>::psd_lambda_max(const void* v, double* lam) {
   sync();
 }
 
+template <typename T>
+void Engine<T>::set_decomposition(const cosmo_b200_decomposition* d) {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "set_decomposition: the reverse of a decomposition is single-GPU"};
+  CUDA_TRY(cudaSetDevice(device_));
+  if (!d) rev_.clear();
+  else rev_.set(*d, n_, m_, stream_);
+}
+
+// reverse_scaling! + reverse_decomposition! (+ psd_completion!) of the iterates the last solve left in HBM
+template <typename T>
+void Engine<T>::reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "reverse_decomposition: the reverse of a decomposition is single-GPU"};
+  if (!rev_.has_map()) throw EngineError{COSMO_B200_ERR_INVALID, "reverse_decomposition: no decomposition map (cosmo_b200_set_decomposition)"};
+  if (!have_solution_)
+    throw EngineError{COSMO_B200_ERR_INVALID, "reverse_decomposition: no solve since the engine was created, reset or warm-started"};
+  CUDA_TRY(cudaSetDevice(device_));
+  rev_.run<T>(xs_.p, s_.p, mu_.p, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, complete_dual != 0,
+              x, s, mu, stats4, stream_, device_);
+}
+
 }  // namespace cosmo
 
 // ============================================================================
@@ -2680,6 +2710,72 @@ int cosmo_b200_comm_p2p_export(cosmo_b200_handle* h, void* blob128) {
 int cosmo_b200_comm_p2p_attach(cosmo_b200_handle* h, const void* blobs, int32_t nranks) {
   if (!blobs) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->p2p_attach(blobs, nranks));
+}
+
+int cosmo_b200_set_decomposition(cosmo_b200_handle* h, const cosmo_b200_decomposition* d) {
+  ABI_GUARD(h, h->impl->set_decomposition(d));
+}
+int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
+  ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));
+}
+
+// psd_complete! of a bare column-major N x N matrix (upper triangle read) on the current device
+int cosmo_b200_psd_complete(int64_t N, const cosmo_b200_completion* sc, double* Y, int64_t stats[4]) {
+  if (!sc || !Y || N < 1 || sc->N != N) {
+    cosmo::g_create_error = "psd_complete: null argument, or N is not the schedule's";
+    return COSMO_B200_ERR_INVALID;
+  }
+  cudaStream_t st = nullptr;
+  try {
+    using namespace cosmo;
+    int ndev = 0, dev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) throw EngineError{COSMO_B200_ERR_CUDA, "no CUDA device"};
+    CUDA_TRY(cudaGetDevice(&dev));
+    rev::check_schedule(*sc, -1, 0);
+    CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    {
+      rev::Cone cone;
+      rev::upload_cone(cone, *sc, st);
+      DevBuf<double> Yd, W, z;
+      DevBuf<int> cnt;
+      const size_t nn = (size_t)N * N;
+      rev::ensure(Yd, nn, N);
+      rev::ensure(W, nn, N);
+      z.alloc(std::max<int64_t>(cone.z_total, 1), false);
+      cnt.alloc(1);
+      Yd.upload(Y, nn, st);
+      Event e0, e1;
+      e0.create();
+      e1.create();
+      CUDA_TRY(cudaEventRecord(e0, st));
+      rev::permute_in_kernel<<<rev::grid_for((int64_t)nn), rev::kThreads, 0, st>>>(N, Yd.p, cone.new_of.p, W.p);
+      CUDA_TRY(cudaGetLastError());
+      rev::complete(cone, W.p, z.p, cnt.p, st, dev);
+      rev::permute_out_kernel<<<rev::grid_for((int64_t)nn), rev::kThreads, 0, st>>>(N, W.p, cone.new_of.p, Yd.p);
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(cudaEventRecord(e1, st));
+      int fallbacks = 0;
+      CUDA_TRY(cudaMemcpyAsync(Y, Yd.p, nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaMemcpyAsync(&fallbacks, cnt.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      float ms = 0.f;
+      CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+      if (stats) {
+        stats[0] = 1;
+        stats[1] = fallbacks;
+        stats[2] = (int64_t)(nn * sizeof(double));
+        stats[3] = (int64_t)llround(1000.0 * ms);
+      }
+    }
+  } catch (...) {
+    if (st) cudaStreamDestroy(st);
+    const int rc = error_code(cosmo::g_create_error);
+    if (cosmo::g_create_error.rfind("psd_complete", 0) != 0 && cosmo::g_create_error.rfind("completion", 0) != 0)
+      cosmo::g_create_error = "psd_complete: " + cosmo::g_create_error;
+    return rc;
+  }
+  cudaStreamDestroy(st);
+  return COSMO_B200_OK;
 }
 
 // ---- diagnostics of the tensor-core PSD path (tc_gemm.cuh, psd_tc.cuh) ----------------------------------------

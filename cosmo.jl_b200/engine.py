@@ -89,6 +89,34 @@ class AcceleratorStruct(C.Structure):
                 ("lambda_", C.c_double), ("start_iter", C.c_int64), ("start_accuracy", C.c_double)]
 
 
+class CompletionStruct(C.Structure):
+    _fields_ = [("N", C.c_int64), ("row_offset", C.c_int64), ("dim", C.c_int64), ("new_of", C.c_void_p),
+                ("n_steps", C.c_int64), ("steps", C.c_void_p), ("n_idx", C.c_int64), ("idx", C.c_void_p)]
+
+
+class DecompositionStruct(C.Structure):
+    _fields_ = [("n_orig", C.c_int64), ("m_orig", C.c_int64), ("n", C.c_int64), ("m", C.c_int64),
+                ("n_plain", C.c_int64), ("plain", C.c_void_p), ("n_rows", C.c_int64), ("row", C.c_void_p),
+                ("s_ptr", C.c_void_p), ("s_src", C.c_void_p), ("mu_src", C.c_void_p),
+                ("n_cones", C.c_int64), ("cones", C.c_void_p)]
+
+
+def _i64(a, keep):
+    a = np.ascontiguousarray(a, dtype=np.int64)
+    keep.append(a)
+    return _ptr(a)
+
+
+def completion_struct(c, keep) -> CompletionStruct:
+    """cosmo_b200_completion of a chordal.CompletionSchedule; the arrays it points to are appended to `keep`."""
+    st = np.asarray(c.steps, dtype=np.int64).reshape(-1, 6)
+    return CompletionStruct(int(c.N), int(c.row_offset), int(c.dim), _i64(c.new_of, keep), st.shape[0], _i64(st, keep),
+                            len(c.idx), _i64(c.idx, keep))
+
+
+# cosmo_b200_reverse_decomposition / cosmo_b200_psd_complete stats[4]
+REVERSE_STATS = ("cones_completed", "pinv_fallbacks", "workspace_bytes", "device_us")
+
 EXPORTS = [
     "cosmo_b200_abi_version", "cosmo_b200_default_settings", "cosmo_b200_create", "cosmo_b200_destroy",
     "cosmo_b200_last_error", "cosmo_b200_update_settings", "cosmo_b200_warm_start", "cosmo_b200_update_qb",
@@ -98,6 +126,7 @@ EXPORTS = [
     "cosmo_b200_tc_gemm_test", "cosmo_b200_psd_stats", "cosmo_b200_get_scaling",
     "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats", "cosmo_b200_infeasibility_test",
     "cosmo_b200_psd_lambda_max", "cosmo_b200_ldl_stats", "cosmo_b200_ldl_symbolic",
+    "cosmo_b200_set_decomposition", "cosmo_b200_reverse_decomposition", "cosmo_b200_psd_complete",
 ]
 
 _lib = None
@@ -154,6 +183,9 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_ldl_symbolic.argtypes = [C.POINTER(ProblemStruct), i64p, i64p, i64p, i64p]
     lib.cosmo_b200_tc_gemm_test.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32,
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    lib.cosmo_b200_set_decomposition.argtypes = [vp, C.POINTER(DecompositionStruct)]
+    lib.cosmo_b200_reverse_decomposition.argtypes = [vp, C.c_int32, vp, vp, vp, i64p]
+    lib.cosmo_b200_psd_complete.argtypes = [C.c_int64, C.POINTER(CompletionStruct), vp, i64p]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if name not in ("cosmo_b200_destroy", "cosmo_b200_last_error"):
@@ -264,6 +296,7 @@ class Engine:
         if rc != OK:
             raise EngineError(rc, (self._lib.cosmo_b200_last_error(None) or b"").decode())
         self._h = h
+        self.n_orig, self.m_orig = 0, 0     # the original problem of a decomposition map (set_decomposition)
         del keep
 
     # ---- lifecycle --------------------------------------------------------
@@ -445,6 +478,49 @@ class Engine:
         for k in LDL_STATS[:6]:
             rec[k] = int(rec[k])
         return rec
+
+    # ---- reverse of a chordal decomposition ---------------------------------
+    def set_decomposition(self, d):
+        """cosmo_b200_set_decomposition: hand over the map of a chordal.DecompositionArrays (None clears it)."""
+        if d is None:
+            self._check(self._lib.cosmo_b200_set_decomposition(self._h, None))
+            self.n_orig, self.m_orig = 0, 0
+            return
+        keep = []
+        cones = (CompletionStruct * max(len(d.cones), 1))()
+        for k, c in enumerate(d.cones):
+            cones[k] = completion_struct(c, keep)
+        sptr = np.asarray(d.s_ptr, dtype=np.int64)
+        ds = DecompositionStruct(int(d.n_orig), int(d.m_orig), int(d.n), int(d.m),
+                                 np.asarray(d.plain).reshape(-1, 3).shape[0], _i64(d.plain, keep),
+                                 len(d.row), _i64(d.row, keep), _i64(sptr, keep), _i64(d.s_src, keep),
+                                 _i64(d.mu_src, keep), len(d.cones), C.cast(cones, C.c_void_p))
+        self._check(self._lib.cosmo_b200_set_decomposition(self._h, C.byref(ds)))
+        self.n_orig, self.m_orig = int(d.n_orig), int(d.m_orig)
+
+    def reverse_decomposition(self, complete_dual=False, x=True, s=True, mu=True):
+        """cosmo_b200_reverse_decomposition: the unscaled (x, s, mu) of the original problem in fp64 from the iterates of
+        the last solve (a False argument skips that output: None in its place), and the stats keyed by REVERSE_STATS."""
+        out = [np.empty(n, dtype=np.float64) if want else None
+               for want, n in ((x, self.n_orig), (s, self.m_orig), (mu, self.m_orig))]
+        stats = (C.c_int64 * 4)()
+        self._check(self._lib.cosmo_b200_reverse_decomposition(self._h, int(bool(complete_dual)), *[_ptr(a) for a in out],
+                                                               stats))
+        return out[0], out[1], out[2], dict(zip(REVERSE_STATS, [int(v) for v in stats]))
+
+
+def psd_complete(Y, schedule):
+    """cosmo_b200_psd_complete: the device completion of the symmetric matrix Y (upper triangle read) along a
+    chordal.CompletionSchedule.  Returns (completed matrix, stats keyed by REVERSE_STATS)."""
+    lib = load_library()
+    W = np.array(Y, dtype=np.float64, order="F", copy=True)
+    keep = []
+    cs = completion_struct(schedule, keep)
+    stats = (C.c_int64 * 4)()
+    rc = lib.cosmo_b200_psd_complete(int(cs.N), C.byref(cs), W.ctypes.data_as(C.c_void_p), stats)
+    if rc != OK:
+        raise EngineError(rc, (lib.cosmo_b200_last_error(None) or b"").decode())
+    return W, dict(zip(REVERSE_STATS, [int(v) for v in stats]))
 
 
 # cosmo_b200_infeasibility_test's out[8]: "gate2" is |Dinv A'dy|_inf (primal) or q'dx (dual), "gate3" dy'b of the

@@ -265,6 +265,9 @@ class Settings:
     merge_strategy: str = "CliqueGraphMerge"   # "NoMerge" | "ParentChildMerge" | "CliqueGraphMerge"
     complete_dual: bool = False
     compact_transformation: bool = True         # the only transformation restated
+    # engine-specific: reverse the decomposition (reverse_scaling!, reverse_decomposition!, psd_completion!) on the
+    # device from the iterates the solve left there, instead of chordal.reverse on the host
+    reverse_on_device: bool = False
 
     _KKT = {"CGIndirectKKTSolver": _eng.KKT_CG, "MINRESIndirectKKTSolver": _eng.KKT_MINRES,
             "IndirectReducedKKTSolver:MINRES": _eng.KKT_MINRES_REDUCED, "DeviceLdlKKTSolver": _eng.KKT_LDL}
@@ -585,6 +588,8 @@ class Model:
                                       dtype=self.dtype, device=self.device, equilibrate=(st.scaling != 0))
             D, E, c = self.engine.scaling() if st.scaling != 0 else (np.ones(n2), np.ones(m2), 1.0)
             self.D, self.E, self.c = D, E, c
+            if self._dec is not None and st.reverse_on_device:
+                self.engine.set_decomposition(_chordal.decomposition_arrays(self._dec, n2, m2))
         else:
             self.engine.update_settings(st.to_struct())
         configure_accelerator(self.engine, st)
@@ -621,7 +626,10 @@ class Model:
         if self._dec is not None:   # reverse_decomposition! (+ psd_completion!), chordal_decomposition.jl:129-151
             from . import chordal as _chordal
             self._x2, self._s2, self._mu2 = x.copy(), s.copy(), mu.copy()
-            x, s, mu = _chordal.reverse(self._dec, x, s, mu, complete_dual=self.settings.complete_dual)
+            if self.settings.reverse_on_device:
+                x, s, mu, _ = self.engine.reverse_decomposition(complete_dual=self.settings.complete_dual)
+            else:
+                x, s, mu = _chordal.reverse(self._dec, x, s, mu, complete_dual=self.settings.complete_dual)
         self.x, self.s, self.mu = x.copy(), s.copy(), mu.copy()
         times = dict(out.times)
         times["setup_time"] = setup_time

@@ -320,6 +320,62 @@ int cosmo_b200_ldl_stats(cosmo_b200_handle* h, double out[8]);
    1 + the largest level of its children.  Errors through cosmo_b200_last_error(NULL). */
 int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* prob, int64_t* perm, int64_t* parent, int64_t* colcount, int64_t* level);
 
+/* ---- reverse of a chordal decomposition (reverse_decomposition! + psd_completion!,
+        chordal_decomposition.jl:129-311) ------------------------------------ */
+/* psd_complete! of one decomposed PsdConeTriangle: the clique tree in traversal order (parents first, children in
+   order).  Vertices are renumbered in the order the traversal first meets them (new_of), so the vertices visited before
+   step t are the leading block 0..lo-1.  Step t = steps[6t .. 6t+5] = {lo, hi, a0, a1, k0, k1}: its residual nu is the
+   new indices lo..hi-1 (lo = hi of the step before, 0 for the first), its separator alpha = idx[a0..a1-1] and the other
+   clique members below lo are idx[k0..k1-1] (a1 == k0).  The step sets, for every r < lo outside the clique,
+       W[r, nu] = W[nu, r]' = W[r, alpha] Z,   W[alpha, alpha] Z = W[alpha, nu],
+   and leaves every entry inside the clique as it is. */
+typedef struct {
+  int64_t N;               /* side of the matrix */
+  int64_t row_offset;      /* first row of the cone in the original problem (cosmo_b200_psd_complete ignores it) */
+  int64_t dim;             /* rows of the cone: N(N+1)/2 (PsdConeTriangle); a square PsdCone (N*N) is not supported */
+  const int64_t* new_of;   /* N: traversal position of every vertex, a permutation of 0..N-1 */
+  int64_t n_steps;
+  const int64_t* steps;    /* 6 * n_steps */
+  int64_t n_idx;
+  const int64_t* idx;      /* new indices, each below the lo of its step */
+} cosmo_b200_completion;
+
+/* The map from the decomposed problem (the handle's n, m) back to the original one (n_orig, m_orig), 0-based:
+   x = the first n_orig entries; plain rows are copied; original row row[i] of a decomposed cone gets
+   s = 0.0 + s'[s_src[s_ptr[i]]] + ... + s'[s_src[s_ptr[i+1]-1]] in that order and mu = mu'[mu_src[i]], which must be the
+   last entry of that list (the clique the host loop writes last); rows in no clique are 0. */
+typedef struct {
+  int64_t n_orig, m_orig;
+  int64_t n, m;            /* must equal the handle's n, m */
+  int64_t n_plain;
+  const int64_t* plain;    /* 3 * n_plain: old_start, new_start, dim */
+  int64_t n_rows;
+  const int64_t* row;      /* n_rows original rows, strictly increasing, none inside a plain block */
+  const int64_t* s_ptr;    /* n_rows + 1, s_ptr[0] = 0, every list non-empty */
+  const int64_t* s_src;    /* s_ptr[n_rows] rows of the decomposed problem */
+  const int64_t* mu_src;   /* n_rows */
+  int64_t n_cones;         /* decomposed cones (PsdConeTriangle) */
+  const cosmo_b200_completion* cones;
+} cosmo_b200_decomposition;
+
+/* Copies the map to the device (NULL clears it).  Every index is checked: out-of-range or inconsistent maps return
+   COSMO_B200_ERR_INVALID; a cone with the square PsdCone layout (dim = N*N) and a sharded handle (nranks > 1) return
+   COSMO_B200_ERR_UNSUPPORTED. */
+int cosmo_b200_set_decomposition(cosmo_b200_handle* h, const cosmo_b200_decomposition* d);
+/* reverse_scaling! + reverse_decomposition! (+ psd_completion! when complete_dual != 0) of the x, s, mu that the last
+   cosmo_b200_solve left on the device: x = D x', s = s' / E, mu = (E mu') / c widened to fp64, then the map.  Writes x
+   (n_orig), s and mu (m_orig) in fp64 into caller buffers; NULL skips a buffer (a NULL mu skips the completion).
+   stats (may be NULL) = {cones completed, separator solves that fell back to the pseudo-inverse, bytes of the dense
+   workspace, device microseconds of the kernels (CUDA events; the copies to the caller's buffers excluded)}.  The dense N x N fp64 workspace of the largest cone is allocated on
+   first use and kept; if it does not fit: COSMO_B200_ERR_ALLOC.  No map, or no solve since create / reset / warm_start:
+   COSMO_B200_ERR_INVALID. */
+int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu,
+                                     int64_t stats[4]);
+/* The completion alone on a dense column-major N x N fp64 matrix Y (host memory, read from its upper triangle,
+   overwritten with the symmetric completion); the parity hook of the kernels.  No handle: uses the current device.
+   stats as above.  Errors through cosmo_b200_last_error(NULL). */
+int cosmo_b200_psd_complete(int64_t N, const cosmo_b200_completion* schedule, double* Y, int64_t stats[4]);
+
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
 int cosmo_b200_comm_unique_id(void* id128);
