@@ -35,6 +35,7 @@
 #include "cg_persistent.cuh"
 #include "ldl.cuh"
 #include "chordal_rev.cuh"
+#include "mat_update.cuh"
 
 namespace cosmo {
 
@@ -121,6 +122,12 @@ struct DevCsr {
   DevBuf<unsigned char> w_colhi;
   DevBuf<double> w_esc;
   long long w_elems = 0, w_nesc = 0;
+  bool packable = false;          // the 9 B layout may hold this slab (fp64, no device equilibration, 15-bit columns)
+  // where every stored value comes from (cosmo_b200_update_matrices): CSR position -> CSC index (none when the CSR is
+  // the CSC order itself, as for A'), slab column position -> CSC index of the matrix or -1 for padding.  Device copies
+  // made by the first update (upload_value_maps); h_src holds the CSR(P) map from create until then.
+  std::vector<int> h_src;
+  DevBuf<int> d_src, d_wsrc;
   WcsrView<T> wview() const {
     return WcsrView<T>{w_rowptr.p, w_col.p, w_val.p, w_word.p, w_colhi.p, w_esc.p, winpack::exp_offset(ebase), w_cta_rows.p,
                        nwin, W, nrows, ncols};
@@ -141,6 +148,7 @@ struct HostCsr {
   int nrows = 0, ncols = 0;
   std::vector<int> rowptr, col;
   std::vector<double> val;  // staged in double, narrowed on upload when T=float
+  std::vector<int> src;     // CSR position -> CSC index (csc_to_host_csrs with record_src; empty otherwise)
 };
 
 class EngineBase {
@@ -150,6 +158,7 @@ class EngineBase {
   virtual void update_settings(const cosmo_b200_settings& st) = 0;
   virtual void warm_start(const void* x, const void* s, const void* mu) = 0;
   virtual void update_qb(const void* q, const void* b) = 0;
+  virtual void update_matrices(const void* Px, long long nnzP, const void* Ax, long long nnzA, const void* q, const void* b) = 0;
   virtual void update_rho(const void* rho_vec, double rho) = 0;
   virtual void reset() = 0;
   virtual void solve(cosmo_b200_result* out) = 0;
@@ -189,6 +198,7 @@ class Engine : public EngineBase {
   }
   void warm_start(const void* x, const void* s, const void* mu) override;
   void update_qb(const void* q, const void* b) override;
+  void update_matrices(const void* Px, long long nnzP, const void* Ax, long long nnzA, const void* q, const void* b) override;
   void update_rho(const void* rho_vec, double rho) override;
   void reset() override;
   void solve(cosmo_b200_result* out) override;
@@ -226,6 +236,7 @@ class Engine : public EngineBase {
   DevBuf<T> q_, b_, D_, Dinv_, E_, Einv_;
   std::vector<double> hb_;                       // host copy of b (row classification)
   std::vector<double> hl_, hu_;                  // host box bounds (m-length, +-inf elsewhere)
+  std::vector<double> hl0_, hu0_;                // the unscaled box bounds of an equilibrating engine (update_matrices)
   std::vector<cosmo_b200_set> sets_;             // type + dim only
   std::vector<int> set_off_;
   // cones
@@ -371,6 +382,9 @@ class Engine : public EngineBase {
   void download_vec(void* host, const T* src, size_t count);
   void build_csr(DevCsr<T>& dst, const HostCsr& h);
   void build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packed);
+  void update_slab(DevCsr<T>& M, int ebase);
+  void upload_value_maps();
+  bool maps_ready_ = false;        // d_src / d_wsrc of A_, At_, P_ are on the device
   void classify_and_set_rho(bool reset_rho, bool rebuild_vec = true);
   void allreduce_sum(T* buf, size_t count);
   void allreduce_max(T* buf, size_t count);
@@ -459,8 +473,8 @@ struct WinGroupScratch {
 }  // namespace
 
 template <typename T>
-static void win_fill_segment(const int* cols, const double* vals, const int* idx, int k, int wbase, long long start,
-                             unsigned short* wc, T* wv, WinGroupScratch& S) {
+static void win_fill_segment(const int* cols, const double* vals, const int* src, const int* idx, int k, int wbase,
+                             long long start, unsigned short* wc, T* wv, int* wsrc, WinGroupScratch& S) {
   constexpr int GL = 16;                // lanes that share one shared-memory wavefront: a half-warp
   const int kpad = (k + 7) & ~7;
   if (kpad == 0) return;
@@ -523,14 +537,16 @@ static void win_fill_segment(const int* cols, const double* vals, const int* idx
       const long long pos_v = start + (long long)st * 256 + (long long)(i / EPL) * (EPL * ls) + (long long)lane * EPL + (i % EPL);
       if (t < S.load[g]) {
         const int e = S.members[g][t];
-        wc[pos_c] = (unsigned short)(cols[e] - wbase);
-        wv[pos_v] = (T)vals[e];
+        if (wc) wc[pos_c] = (unsigned short)(cols[e] - wbase);
+        if (wv) wv[pos_v] = (T)vals[e];
+        if (wsrc) wsrc[pos_c] = src ? src[e] : e;
       } else {   // padding: zero value on a bank this group does not use yet
         int r0 = 0;
         while (r0 < 15 && ((S.used[g] >> r0) & 1)) ++r0;
         S.used[g] |= (unsigned short)(1u << r0);
-        wc[pos_c] = (unsigned short)r0;
-        wv[pos_v] = T(0);
+        if (wc) wc[pos_c] = (unsigned short)r0;
+        if (wv) wv[pos_v] = T(0);
+        if (wsrc) wsrc[pos_c] = -1;
       }
     }
   }
@@ -604,6 +620,46 @@ static bool win_pack(const std::vector<double>& hval, const std::vector<int>& rp
   return true;
 }
 
+// fn(a, b) on contiguous ranges [a, b) of nr rows, one host thread each
+static void parallel_rows(int nr, const std::function<void(int, int)>& fn) {
+  const int nthreads = (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
+  std::vector<std::thread> th;
+  const int chunk = (nr + nthreads - 1) / nthreads;
+  for (int t = 0; t < nthreads; ++t) {
+    const int a = t * chunk, b = std::min(nr, a + chunk);
+    if (a < b) th.emplace_back(fn, a, b);
+  }
+  for (auto& x : th) x.join();
+}
+
+// Pass 2 of build_windows: the bank-aware placement of every row segment of a CSR (rowptr, col) into the slab laid out
+// by rp.  It depends on the pattern alone, so update_matrices runs it again without values (wc = wv = nullptr) to learn
+// which entry every slot holds: wsrc[slot] = src[k] (k itself when src is null), -1 for padding.
+template <typename T>
+static void win_place(const int* rowptr, const int* col, const double* vals, const int* src, int nr, int nwin, int W,
+                      const std::vector<int>& rp, unsigned short* wc, T* wv, int* wsrc) {
+  parallel_rows(nr, [&](int a, int b) {
+    WinGroupScratch S;
+    std::vector<std::vector<int>> seg(nwin);
+    for (int r = a; r < b; ++r) {
+      for (int w = 0; w < nwin; ++w) seg[w].clear();
+      for (int k = rowptr[r]; k < rowptr[r + 1]; ++k) seg[col[k] / W].push_back(k);
+      for (int w = 0; w < nwin; ++w)
+        win_fill_segment<T>(col, vals, src, seg[w].data(), (int)seg[w].size(), w * W, rp[(size_t)w * (nr + 1) + r], wc, wv,
+                            wsrc, S);
+    }
+  });
+}
+
+// the slab layout line of COSMO_B200_SETUP_DEBUG (create and update_matrices)
+template <typename T>
+static void report_windows(const DevCsr<T>& d) {
+  if (getenv("COSMO_B200_SETUP_DEBUG") == nullptr) return;
+  const double bytes = (double)d.w_elems * (d.packed ? 9 : sizeof(T) + 2) + 8.0 * d.w_nesc;
+  fprintf(stderr, "[setup] windows %d x %d, %d rows: %s layout, ebase %d, %lld escapes, slab %.1f MB\n", d.nwin, d.W, d.nrows,
+          d.packed ? "9 B" : sizeof(T) == 8 ? "10 B" : "6 B", d.ebase, d.w_nesc, bytes / 1e6);
+}
+
 template <typename T>
 void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packed) {
   dst.windowed = false;
@@ -621,18 +677,9 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
   const int nr = h.nrows;
   std::vector<int> rp((size_t)nwin * (nr + 1), 0);
   std::vector<long long> row_cost(nr, 0);
-  const int nthreads = (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
-  auto parallel_rows = [&](const std::function<void(int, int)>& fn) {
-    std::vector<std::thread> th;
-    const int chunk = (nr + nthreads - 1) / nthreads;
-    for (int t = 0; t < nthreads; ++t) {
-      const int a = t * chunk, b = std::min(nr, a + chunk);
-      if (a < b) th.emplace_back(fn, a, b);
-    }
-    for (auto& x : th) x.join();
-  };
+  auto rows = [&](const std::function<void(int, int)>& fn) { parallel_rows(nr, fn); };
   // pass 1: padded segment lengths
-  parallel_rows([&](int a, int b) {
+  rows([&](int a, int b) {
     std::vector<int> cnt(nwin);
     for (int r = a; r < b; ++r) {
       std::fill(cnt.begin(), cnt.end(), 0);
@@ -656,18 +703,7 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
   const long long total = run;
   std::vector<unsigned short> wc((size_t)total + 8, 0);
   std::vector<T> wv((size_t)total + 8, T(0));
-  // pass 2: bank-aware placement of every row segment
-  parallel_rows([&](int a, int b) {
-    WinGroupScratch S;
-    std::vector<std::vector<int>> seg(nwin);
-    for (int r = a; r < b; ++r) {
-      for (int w = 0; w < nwin; ++w) seg[w].clear();
-      for (int k = h.rowptr[r]; k < h.rowptr[r + 1]; ++k) seg[h.col[k] / W].push_back(k);
-      for (int w = 0; w < nwin; ++w)
-        win_fill_segment<T>(h.col.data(), h.val.data(), seg[w].data(), (int)seg[w].size(), w * W,
-                            rp[(size_t)w * (nr + 1) + r], wc.data(), wv.data(), S);
-    }
-  });
+  win_place<T>(h.rowptr.data(), h.col.data(), h.val.data(), nullptr, nr, nwin, W, rp, wc.data(), wv.data(), nullptr);
   // contiguous row chunks per CTA, balanced by padded nnz (+ per-row overhead)
   // one CTA per (row chunk, window): chunks are contiguous row ranges balanced by padded nnz
   const int nchunks = std::max(1, num_sms_ / nwin);
@@ -691,7 +727,8 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
   // in place (ruiz_apply_win_kernel works on the 10 B layout)
   if constexpr (sizeof(T) == sizeof(double)) {
     WinPacked pk;
-    if (allow_packed && W - 1 <= (int)winpack::kMaxCol && win_pack(h.val, rp, nr, nwin, total, wc, wv, pk, parallel_rows)) {
+    dst.packable = allow_packed && W - 1 <= (int)winpack::kMaxCol;
+    if (dst.packable && win_pack(h.val, rp, nr, nwin, total, wc, wv, pk, rows)) {
       dst.packed = true;
       dst.ebase = pk.ebase;
       dst.w_nesc = (long long)pk.esc.size();
@@ -707,18 +744,14 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
     dst.w_val.upload(wv, stream_);
     sync();
   }
-  if (getenv("COSMO_B200_SETUP_DEBUG") != nullptr) {
-    const double bytes = (double)total * (dst.packed ? 9 : sizeof(T) + 2) + 8.0 * dst.w_nesc;
-    fprintf(stderr, "[setup] windows %d x %d, %d rows: %s layout, ebase %d, %lld escapes, slab %.1f MB\n", nwin, W, nr,
-            dst.packed ? "9 B" : sizeof(T) == 8 ? "10 B" : "6 B", dst.ebase, dst.w_nesc, bytes / 1e6);
-  }
+  report_windows(dst);
   dst.windowed = true;
 }
 
 // Julia CSC -> (a) CSR of the transpose (zero conversion: same arrays, rebased)
 //              (b) CSR of the matrix itself (stable counting-sort transposition)
 template <typename T>
-static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, HostCsr& csr_t) {
+static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, HostCsr& csr_t, bool record_src = false) {
   const long long nr = M.nrows, nc = M.ncols;
   if (nr < 0 || nc < 0 || nr >= (1LL << 31) - 8 || nc >= (1LL << 31) - 8)
     throw EngineError{COSMO_B200_ERR_INVALID, "matrix dimensions out of int32 range"};
@@ -738,6 +771,8 @@ static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, Ho
   csr.rowptr.assign(nr + 1, 0);
   csr.col.resize(nnz);
   csr.val.resize(nnz);
+  if (record_src) csr.src.resize(nnz);
+  int* const srcp = record_src ? csr.src.data() : nullptr;
   // Stable counting-sort transposition, parallel over column blocks: thread t counts the rows of its columns, a prefix
   // over (row, thread) gives every thread its own slots in every row, so the scatter needs no synchronisation and the
   // entries of a row stay ordered by column whatever the thread count (deterministic).
@@ -782,6 +817,7 @@ static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, Ho
         const int dstk = next[csr_t.col[k]]++;
         csr.col[dstk] = (int)j;
         csr.val[dstk] = csr_t.val[k];
+        if (srcp) srcp[dstk] = k;
       }
   });
 }
@@ -919,8 +955,10 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
     lap("upload csr A'");
     build_windows(At_, at, pack_ok);
     lap("windows A'");
-    csc_to_host_csrs<T>(p.P, p.index_base, pp, ppt);
+    // P's CSC order is not resident: its CSR -> CSC map is kept for update_matrices (A's is derived from A')
+    csc_to_host_csrs<T>(p.P, p.index_base, pp, ppt, true);
     build_csr(P_, pp);
+    P_.h_src.swap(pp.src);
     lap("P");
     // A' and P rows are traversed by the same lane group in the fused operator kernel
     double mean = n_ ? (double)(At_.nnz + P_.nnz) / n_ : 0.0;
@@ -993,6 +1031,7 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   // (setup.jl:27-33 -> scale_ruiz!); the host reads D, E, c back with cosmo_b200_get_scaling
   if ((p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0) {
     if (scaled_) throw EngineError{COSMO_B200_ERR_INVALID, "COSMO_B200_PROBLEM_EQUILIBRATE expects D = Dinv = E = Einv = NULL"};
+    hl0_ = hl_; hu0_ = hu_;
     equilibrate();
   }
   classify_and_set_rho(true);
@@ -1160,6 +1199,176 @@ void Engine<T>::update_qb(const void* q, const void* b) {
   sync();
 }
 
+// New values of P and/or A on the resident pattern, left in the state a create with the new data and the current
+// settings leaves (mat_update.cuh): same scaling, rho vector, zero iterates, KKT call counter at 1, a fresh factor.
+template <typename T>
+void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, long long nnzA, const void* q, const void* b) {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "update_matrices: a sharded handle holds only a slice of the data"};
+  if ((Px && nnzP != P_.nnz) || (Ax && nnzA != At_.nnz))
+    throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices: nnz differs from the pattern given at create (a new pattern needs a new engine)"};
+  // Ruiz restarts from identity on the unscaled data, and the engine keeps only the scaled values
+  if (device_scaled_ && !(Px && Ax && q && b))
+    throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices: an equilibrating engine needs the unscaled P, A, q and b"};
+  CUDA_TRY(cudaSetDevice(device_));
+  const double t0 = now_s();
+  upload_value_maps();
+  auto gather = [&](DevCsr<T>& M, const T* v) {
+    matup::gather_kernel<T><<<vgrid(M.nnz), kBlock, 0, stream_>>>(M.nnz, M.d_src.p, v, M.val.p);
+    check_launch("update_matrices gather");
+  };
+  if (Ax) {
+    upload_vec(At_.val, Ax, (size_t)At_.nnz);   // CSR(A') is the CSC order of A
+    gather(A_, At_.val.p);
+    int ebase = 0;
+    if constexpr (sizeof(T) == sizeof(double)) {
+      if ((A_.windowed && A_.packable) || (At_.windowed && At_.packable)) {   // one exponent window for A and A'
+        DevBuf<unsigned long long> hist;
+        hist.alloc(2048);
+        matup::exp_hist_kernel<<<std::min(vgrid(At_.nnz), 4 * num_sms_), kBlock, 0, stream_>>>(At_.nnz, At_.val.p, hist.p);
+        check_launch("update_matrices exp_hist");
+        std::vector<long long> h(2048);
+        CUDA_TRY(cudaMemcpyAsync(h.data(), hist.p, 2048 * sizeof(long long), cudaMemcpyDeviceToHost, stream_));
+        sync();
+        ebase = winpack::pick_ebase(h.data());
+      }
+    }
+    update_slab(A_, ebase);
+    update_slab(At_, ebase);
+  }
+  if (Px) {
+    DevBuf<T> px;
+    px.alloc((size_t)P_.nnz, false);
+    upload_vec(px, Px, (size_t)P_.nnz);
+    gather(P_, px.p);
+    sync();
+  }
+  if (q) upload_vec(q_, q, n_);
+  if (b) {
+    upload_vec(b_, b, m_);
+    for (int i = 0; i < m_; ++i) hb_[i] = (double)static_cast<const T*>(b)[i];
+  }
+  if (device_scaled_) {
+    std::vector<T> l(hl0_.begin(), hl0_.end()), u(hu0_.begin(), hu0_.end());
+    upload_vec(box_l_, l.data(), m_);
+    upload_vec(box_u_, u.data(), m_);
+    equilibrate();
+  }
+  sync();
+  destroy_cg_graphs();   // the slab and escape-table pointers they captured may have changed
+  reset();
+  auto_rho_interval_ = 0;
+  if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_factor();   // reset() marked the factor dirty; a non-convex P fails here
+  create_time_ = now_s() - t0;
+}
+
+// The value maps of update_matrices, made once and kept on the device.  Creating an engine records only the CSR(P) map
+// (P's CSC order is not resident); the others follow from the resident pattern: CSR(A) position -> CSC index by the
+// stable counting sort of csc_to_host_csrs over A' (the CSC pattern itself), and slab slot -> CSC index, -1 for
+// padding, by running build_windows' placement again on the same CSR pattern and row layout.  Padding cannot be told
+// from a stored zero by its content, but the placement is a function of the pattern, so it places every entry where
+// create placed it.  Engines that never update pay nothing for the maps, in time or memory.
+template <typename T>
+void Engine<T>::upload_value_maps() {
+  if (maps_ready_) return;
+  auto down = [&](std::vector<int>& v, const int* d, size_t cnt) {
+    v.resize(cnt);
+    if (cnt) CUDA_TRY(cudaMemcpyAsync(v.data(), d, cnt * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  };
+  std::vector<int> arow, acol, atrow, atcol;
+  down(atrow, At_.rowptr.p, (size_t)n_ + 1);
+  down(atcol, At_.col.p, (size_t)At_.nnz);
+  down(arow, A_.rowptr.p, (size_t)m_ + 1);
+  if (A_.windowed) down(acol, A_.col.p, (size_t)A_.nnz);
+  sync();
+  std::vector<int> asrc((size_t)A_.nnz);
+  {
+    std::vector<int> next(arow.begin(), arow.end() - 1);
+    for (int j = 0; j < n_; ++j)
+      for (int k = atrow[j]; k < atrow[j + 1]; ++k) asrc[next[atcol[k]]++] = k;
+  }
+  A_.d_src.upload(asrc, stream_);
+  P_.d_src.upload(P_.h_src, stream_);
+  auto slab = [&](DevCsr<T>& M, const std::vector<int>& row, const std::vector<int>& col, const int* src) {
+    if (!M.windowed) return;
+    std::vector<int> rp;
+    down(rp, M.w_rowptr.p, (size_t)M.nwin * (M.nrows + 1));
+    sync();
+    std::vector<int> wsrc((size_t)M.w_elems + 8, -1);
+    win_place<T>(row.data(), col.data(), nullptr, src, M.nrows, M.nwin, M.W, rp, nullptr, nullptr, wsrc.data());
+    M.d_wsrc.upload(wsrc, stream_);
+    sync();
+  };
+  slab(A_, arow, acol, asrc.data());
+  slab(At_, atrow, atcol, nullptr);
+  sync();
+  std::vector<int>().swap(P_.h_src);
+  maps_ready_ = true;
+}
+
+// New slab values of a windowed matrix from the CSC values in At_.val, in the layout create would choose for them.
+template <typename T>
+void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
+  if (!M.windowed) return;
+  const long long nseg = (long long)M.nwin * M.nrows;
+  const int grid = (int)std::min<long long>((nseg * 32 + kBlock - 1) / kBlock, kMaxGrid);
+  if constexpr (sizeof(T) == sizeof(double)) {
+    if (M.packable) {
+      DevBuf<int> cnt;
+      cnt.alloc((size_t)nseg, false);
+      matup::slab_esc_count_kernel<<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, ebase, cnt.p);
+      check_launch("update_matrices esc_count");
+      std::vector<int> hc((size_t)nseg);
+      CUDA_TRY(cudaMemcpyAsync(hc.data(), cnt.p, (size_t)nseg * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+      sync();
+      std::vector<long long> off((size_t)nseg + 1, 0);   // escape slots in slab order: window, row, entry
+      for (long long g = 0; g < nseg; ++g) off[g + 1] = off[g] + hc[g];
+      const long long nesc = off.back();
+      if (nesc * winpack::kEscDen <= M.w_elems) {
+        DevBuf<long long> doff;
+        doff.upload(off, stream_);
+        if ((long long)M.w_esc.n < nesc) M.w_esc.alloc((size_t)nesc, false);
+        if (!M.packed) {   // 10 B -> 9 B: the columns come from w_col
+          M.w_word.alloc((size_t)M.w_elems + 8);
+          M.w_colhi.alloc((size_t)M.w_elems + 8);
+          matup::slab_encode_kernel<true><<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, ebase,
+                                                                       doff.p, M.w_col.p, M.w_word.p, M.w_colhi.p, M.w_esc.p);
+          check_launch("update_matrices encode");
+          sync();
+          M.w_col.release();
+          M.w_val.release();
+        } else {
+          matup::slab_encode_kernel<false><<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, ebase,
+                                                                        doff.p, nullptr, M.w_word.p, M.w_colhi.p, M.w_esc.p);
+          check_launch("update_matrices encode");
+          sync();
+        }
+        M.packed = true;
+        M.ebase = ebase;
+        M.w_nesc = nesc;
+        report_windows(M);
+        return;
+      }
+      if (M.packed) {   // 9 B -> 10 B: decode the columns before the words go
+        M.w_col.alloc((size_t)M.w_elems + 8);
+        matup::slab_unpack_col_kernel<<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.w_word.p, M.w_colhi.p, M.w_col.p);
+        check_launch("update_matrices unpack_col");
+        M.w_val.alloc((size_t)M.w_elems + 8);
+        sync();
+        M.w_word.release();
+        M.w_colhi.release();
+        M.w_esc.release();
+        M.packed = false;
+        M.ebase = 0;
+        M.w_nesc = 0;
+      }
+    }
+  }
+  matup::slab_gather_kernel<T><<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, M.w_val.p);
+  check_launch("update_matrices slab_gather");
+  sync();
+  report_windows(M);
+}
+
 template <typename T>
 void Engine<T>::update_rho(const void* rho_vec, double rho) {
   if (rho_vec) upload_vec(rho_vec_, rho_vec, m_);
@@ -1206,6 +1415,7 @@ void Engine<T>::comm_init(int nranks, int rank, const void* id128) {
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU (use CG or reduced MINRES when sharded)"};
   nranks_ = nranks; rank_ = rank;
   if (nranks == 1) return;
+  std::vector<int>().swap(P_.h_src);   // update_matrices refuses sharded handles
   std::string e;
   if (!g_nccl.load(e)) throw EngineError{COSMO_B200_ERR_NCCL, e};
   NcclUniqueId id;
@@ -2605,6 +2815,10 @@ int cosmo_b200_update_settings(cosmo_b200_handle* h, const cosmo_b200_settings* 
 }
 int cosmo_b200_warm_start(cosmo_b200_handle* h, const void* x, const void* s, const void* mu) { ABI_GUARD(h, h->impl->warm_start(x, s, mu)); }
 int cosmo_b200_update_qb(cosmo_b200_handle* h, const void* q, const void* b) { ABI_GUARD(h, h->impl->update_qb(q, b)); }
+int cosmo_b200_update_matrices(cosmo_b200_handle* h, const void* Px, int64_t nnzP, const void* Ax, int64_t nnzA, const void* q,
+                               const void* b) {
+  ABI_GUARD(h, h->impl->update_matrices(Px, nnzP, Ax, nnzA, q, b));
+}
 int cosmo_b200_update_rho(cosmo_b200_handle* h, const void* rho_vec, double rho) { ABI_GUARD(h, h->impl->update_rho(rho_vec, rho)); }
 int cosmo_b200_reset(cosmo_b200_handle* h) { ABI_GUARD(h, h->impl->reset()); }
 int cosmo_b200_solve(cosmo_b200_handle* h, cosmo_b200_result* out) { ABI_GUARD(h, h->impl->solve(out)); }

@@ -55,6 +55,11 @@ struct DevBuf {
       CUDA_TRY(cudaDeviceSynchronize());
     }
   }
+  void release() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    n = 0;
+  }
   void upload(const U* host, size_t count, cudaStream_t st) {
     if (count) CUDA_TRY(cudaMemcpyAsync(p, host, count * sizeof(U), cudaMemcpyHostToDevice, st));
   }

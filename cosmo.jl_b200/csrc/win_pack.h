@@ -11,7 +11,8 @@
 //               Inf, NaN with its payload, every exponent outside [ebase, ebase + 13])
 // The decode is lossless: it returns the stored double bit for bit.  It touches only the high 32 bits of the word; the
 // low word (mantissa bits 0-31, or the escape index) passes through.  Plain C++ with __host__ __device__ functions,
-// so a host program can check the very functions the kernel calls.
+// so a host program can check the very functions the kernel calls, and the device re-encoder of an update
+// (mat_update.cuh) writes the words the host builder writes.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -44,11 +45,11 @@ WP_HD bool is_escape(uint32_t hi) { return (hi & 0x78000000u) == 0x78000000u; }
 // window-local column from the high word and the column-high byte
 WP_HD uint32_t decode_col(uint32_t hi, uint32_t colhi) { return ((hi >> 20) & 0x7Fu) | (colhi << 7); }
 
-inline uint64_t bits_of(double v) { uint64_t u; memcpy(&u, &v, 8); return u; }
-inline double double_of(uint64_t u) { double v; memcpy(&v, &u, 8); return v; }
+WP_HD uint64_t bits_of(double v) { uint64_t u; memcpy(&u, &v, 8); return u; }
+WP_HD double double_of(uint64_t u) { double v; memcpy(&v, &u, 8); return v; }
 
 // biased exponent of a finite normal value, 0 otherwise (zero, subnormal, Inf, NaN)
-inline int normal_exponent(double v) {
+WP_HD int normal_exponent(double v) {
   const int e = (int)((bits_of(v) >> 52) & 0x7FF);
   return (e == 0 || e == 0x7FF) ? 0 : e;
 }
@@ -66,7 +67,7 @@ inline int pick_ebase(const long long* hist) {
 }
 
 // exponent code of a value: 0 for +-0, 1-14 inside the window, kEscape otherwise
-inline unsigned code_of(double v, int ebase) {
+WP_HD unsigned code_of(double v, int ebase) {
   const uint64_t u = bits_of(v);
   if ((u << 1) == 0) return 0u;
   const int e = (int)((u >> 52) & 0x7FF);
@@ -75,13 +76,13 @@ inline unsigned code_of(double v, int ebase) {
 }
 
 // the packed word of (v, col); an escape stores esc_index in the low 32 bits, the caller stores v at esc[esc_index]
-inline uint64_t encode_word(double v, uint32_t col, int ebase, uint32_t esc_index) {
+WP_HD uint64_t encode_word(double v, uint32_t col, int ebase, uint32_t esc_index) {
   const uint64_t u = bits_of(v);
   const unsigned code = code_of(v, ebase);
   const uint64_t mant = code == kEscape ? (uint64_t)esc_index : (u & 0x000FFFFFFFFFFFFFull);
   return (u & 0x8000000000000000ull) | ((uint64_t)code << 59) | ((uint64_t)(col & 0x7Fu) << 52) | mant;
 }
-inline uint8_t encode_colhi(uint32_t col) { return (uint8_t)(col >> 7); }
+WP_HD uint8_t encode_colhi(uint32_t col) { return (uint8_t)(col >> 7); }
 
 // host reference of the device decode (same functions): the double and the column of one entry
 inline double decode_value(uint64_t word, const double* esc, int ebase) {

@@ -120,6 +120,7 @@ REVERSE_STATS = ("cones_completed", "pinv_fallbacks", "workspace_bytes", "device
 EXPORTS = [
     "cosmo_b200_abi_version", "cosmo_b200_default_settings", "cosmo_b200_create", "cosmo_b200_destroy",
     "cosmo_b200_last_error", "cosmo_b200_update_settings", "cosmo_b200_warm_start", "cosmo_b200_update_qb",
+    "cosmo_b200_update_matrices",
     "cosmo_b200_update_rho", "cosmo_b200_reset", "cosmo_b200_solve", "cosmo_b200_project", "cosmo_b200_kkt_solve",
     "cosmo_b200_residuals", "cosmo_b200_spmv", "cosmo_b200_spmv_bench", "cosmo_b200_get_rho_vec", "cosmo_b200_get_w",
     "cosmo_b200_comm_unique_id", "cosmo_b200_comm_init", "cosmo_b200_comm_p2p_export", "cosmo_b200_comm_p2p_attach",
@@ -158,6 +159,7 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_update_settings.argtypes = [vp, C.POINTER(SettingsStruct)]
     lib.cosmo_b200_warm_start.argtypes = [vp, vp, vp, vp]
     lib.cosmo_b200_update_qb.argtypes = [vp, vp, vp]
+    lib.cosmo_b200_update_matrices.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, vp]
     lib.cosmo_b200_update_rho.argtypes = [vp, vp, C.c_double]
     lib.cosmo_b200_reset.argtypes = [vp]
     lib.cosmo_b200_solve.argtypes = [vp, C.POINTER(ResultStruct)]
@@ -335,6 +337,15 @@ class Engine:
     def update_qb(self, q=None, b=None):
         q, b = self._vec(q, self.n), self._vec(b, self.m)
         self._check(self._lib.cosmo_b200_update_qb(self._h, _ptr(q), _ptr(b)))
+
+    def update_matrices(self, Px=None, Ax=None, q=None, b=None):
+        """cosmo_b200_update_matrices: new values of P and A on the pattern of create -- ``Px`` / ``Ax`` are the ``data``
+        arrays of the CSC matrices with sorted indices -- and optionally q and b (None: unchanged).  The engine is left
+        as a new Engine with these data would be; an equilibrating engine needs all four, unscaled."""
+        Px, Ax = [None if a is None else np.ascontiguousarray(a, dtype=self.dtype).ravel() for a in (Px, Ax)]
+        q, b = self._vec(q, self.n), self._vec(b, self.m)
+        self._check(self._lib.cosmo_b200_update_matrices(self._h, _ptr(Px), 0 if Px is None else Px.size, _ptr(Ax),
+                                                         0 if Ax is None else Ax.size, _ptr(q), _ptr(b)))
 
     def update_rho(self, rho_vec, rho):
         rv = self._vec(rho_vec, self.m)

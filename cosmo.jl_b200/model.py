@@ -444,6 +444,12 @@ def ruiz_equilibrate(P, q, A, b, sets, st: Settings):
     return P, q, A, b, new_sets, D, E, c
 
 
+def _sorted_csc(M) -> sp.csc_matrix:
+    """M as a float64 CSC matrix with sorted row indices (a copy when they had to be sorted)."""
+    M = sp.csc_matrix(M, dtype=np.float64)
+    return M if M.has_sorted_indices else M.sorted_indices()
+
+
 # ---------------------------------------------------------------------------
 # Model (COSMO.Model = Workspace, src/types.jl:348-403)
 # ---------------------------------------------------------------------------
@@ -491,8 +497,8 @@ class Model:
 
     # set!(model, P, q, A, b, convex_sets, settings), interface.jl:218-250: model form A x + s = b
     def set(self, P, q, A, b, convex_sets: Sequence[AbstractConvexSet], settings: Optional[Settings] = None):
-        A = sp.csc_matrix(A, dtype=np.float64)
-        P = sp.csc_matrix(P, dtype=np.float64)
+        A = _sorted_csc(A)
+        P = _sorted_csc(P)
         m, n = A.shape
         if sum(S.dim for S in convex_sets) != m:
             raise ValueError("set dimension is not m")
@@ -534,10 +540,13 @@ class Model:
         self.mu[:] = -y0
         self._x2 = None
 
-    # update!(model; q, b), interface.jl:187-211
-    def update(self, q=None, b=None):
+    # update!(model; q, b), interface.jl:187-211, extended by new values of P and A on the pattern given to set!
+    def update(self, q=None, b=None, *, P=None, A=None):
         if not self.is_assembled:
             raise RuntimeError("Model has to be assembled once before one can start updating q or b.")
+        if P is not None or A is not None:
+            self._update_matrices(q, b, P, A)
+            return
         if q is not None:
             q = np.asarray(q, dtype=np.float64)
             if q.shape != (self.n,):
@@ -559,6 +568,47 @@ class Model:
             qs = (self.D * self.q0) * self.c if q is not None else None
             bs = self.E * self.b0 if b is not None else None
             self.engine.update_qb(qs, bs)
+
+    def _update_matrices(self, q, b, P, A):
+        """update(q, b, P=, A=): the new values go to the live engine (cosmo_b200_update_matrices), which ends up as a
+        new engine with these data would be; the iterates of the model stay as the next warm start."""
+        new = {}
+        for name, M, old in (("P", P, self.P0), ("A", A, self.A0)):
+            if M is None:
+                continue
+            M = _sorted_csc(M)
+            if M.shape != old.shape or not (np.array_equal(M.indptr, old.indptr) and np.array_equal(M.indices, old.indices)):
+                raise ValueError("The sparsity pattern of %s differs from the one the model was set up with: use set! "
+                                 "(Model.set) for a new pattern." % name)
+            new[name] = M
+        if q is not None:
+            q = np.asarray(q, dtype=np.float64)
+            if q.shape != (self.n,):
+                raise ValueError("The dimension of q, does not agree with the model dimension, n.")
+        if b is not None:
+            b = np.asarray(b, dtype=np.float64)
+            if b.shape != (self.m,):
+                raise ValueError("The dimension of b, does not agree with the model dimension, m.")
+        self.P0, self.A0 = new.get("P", self.P0), new.get("A", self.A0)
+        if q is not None:
+            self.q0 = q.copy()
+        if b is not None:
+            self.b0 = b.copy()
+        if self.engine is None:
+            return
+        if self._dec is not None:
+            # the decomposed problem is rebuilt from the new data at the next optimize!, as update(q, b) does
+            self._x2 = None
+            self.engine.close()
+            self.engine = None
+            return
+        if self._engine_equilibrates:
+            # Ruiz runs again on the device from the unscaled data: every vector goes with the matrices
+            self.engine.update_matrices(self.P0.data, self.A0.data, self.q0, self.b0)
+            self.D, self.E, self.c = self.engine.scaling()
+        else:
+            self.engine.update_matrices(new["P"].data if "P" in new else None, new["A"].data if "A" in new else None,
+                                        q, b)
 
     # setup! (setup.jl:18-64): scaling + engine creation (the KKT "factorisation" analogue)
     def _setup(self):
@@ -584,8 +634,10 @@ class Model:
                     self._s2, self._mu2 = np.zeros(A2.shape[0]), np.zeros(A2.shape[0])
             m2, n2 = A0.shape
             # scale_ruiz! runs on the device (csrc/ruiz.cuh): the engine ingests the unscaled data and hands D, E, c back
+            # how the engine was created, not the settings of a later solve, decides what update(P=, A=) hands over
+            self._engine_equilibrates = st.scaling != 0
             self.engine = _eng.Engine(P0, q0, A0, b0, [set_tuple(S) for S in sets0], st.to_struct(),
-                                      dtype=self.dtype, device=self.device, equilibrate=(st.scaling != 0))
+                                      dtype=self.dtype, device=self.device, equilibrate=self._engine_equilibrates)
             D, E, c = self.engine.scaling() if st.scaling != 0 else (np.ones(n2), np.ones(m2), 1.0)
             self.D, self.E, self.c = D, E, c
             if self._dec is not None and st.reverse_on_device:

@@ -247,6 +247,25 @@ int cosmo_b200_update_settings(cosmo_b200_handle* h, const cosmo_b200_settings* 
 int cosmo_b200_warm_start(cosmo_b200_handle* h, const void* x, const void* s, const void* mu);
 /* update!(model, q=, b=) (interface.jl:187-211), already scaled; NULL = leave unchanged */
 int cosmo_b200_update_qb(cosmo_b200_handle* h, const void* q, const void* b);
+/* New values of P and A on the sparsity pattern given at create, an engine extension: the closest reference entry point
+   is update!(model, q=, b=) (interface.jl:187-211), which takes only q and b.  Px and Ax are the nzval arrays in the
+   CSC order of create (element type T, nnzP / nnzA entries, which must equal create's: otherwise
+   COSMO_B200_ERR_INVALID and nothing changes); q and b as for cosmo_b200_update_qb; NULL = leave unchanged.  Afterwards
+   the handle is bit for bit in the state cosmo_b200_create with the new data and the handle's current settings leaves:
+   the same scaling, rho vector (rho_updates = [settings.rho]), zero iterates and CG warm start, KKT call counter 1,
+   cleared accelerator history and PSD warm starts, and under COSMO_B200_KKT_LDL a fresh factor (a non-convex P:
+   COSMO_B200_ERR_INVALID "Objective function is not convex.").  Warm-start it as a new engine.  Not reset, because
+   they describe the engine's history rather than its state: the setup time a later solve reports is the duration of
+   this call (and so is the figure the automatic adaptive_rho_interval rule reads when settings.setup_time is 0), and
+   the statistics counters (factorisations, kernel launches) keep counting.  The first call also derives the value
+   maps from the resident pattern and keeps them on the device (a one-off cost about that of the slab placement).
+   An engine created with COSMO_B200_PROBLEM_EQUILIBRATE (and scaling != 0) re-runs Ruiz from identity on the unscaled
+   data, so it needs all four of Px, Ax, q and b, unscaled (COSMO_B200_ERR_INVALID otherwise); its Box bounds are the
+   unscaled ones given at create.  With caller-supplied D, E the values are taken as given, like create does.  A
+   decomposition map (cosmo_b200_set_decomposition) stays; reverse_decomposition needs a solve first.  After
+   cosmo_b200_comm_init with nranks > 1: COSMO_B200_ERR_UNSUPPORTED. */
+int cosmo_b200_update_matrices(cosmo_b200_handle* h, const void* Px, int64_t nnzP, const void* Ax, int64_t nnzA,
+                               const void* q, const void* b);
 /* update_rho!(kkt_solver, rho_vec) (kktsolver_indirect.jl:164-166): overrides the row penalties */
 int cosmo_b200_update_rho(cosmo_b200_handle* h, const void* rho_vec, double rho);
 /* empty_model!-like reset of iterates, rho, CG warm start and call counter */
