@@ -16,8 +16,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
 #include <functional>
-#include <mutex>
 #include <thread>
 #include <chrono>
 #include <string>
@@ -144,11 +144,11 @@ static int pick_lanes(double mean_row) {
   return 2;
 }
 
+// a sparsity pattern; the values go to the device separately (mat_update.cuh)
 struct HostCsr {
   int nrows = 0, ncols = 0;
   std::vector<int> rowptr, col;
-  std::vector<double> val;  // staged in double, narrowed on upload when T=float
-  std::vector<int> src;     // CSR position -> CSC index (csc_to_host_csrs with record_src; empty otherwise)
+  std::vector<int> src;     // CSR position -> CSC index (csr_transpose; empty for the CSC pattern itself)
 };
 
 class EngineBase {
@@ -381,7 +381,10 @@ class Engine : public EngineBase {
   void upload_vec(DevBuf<T>& dst, const void* host, size_t count);
   void download_vec(void* host, const T* src, size_t count);
   void build_csr(DevCsr<T>& dst, const HostCsr& h);
-  void build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packed);
+  void build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src, bool allow_packed);
+  void gather_csr(DevCsr<T>& M, const T* v);
+  void load_P(const void* Px);
+  int exponent_window();
   void update_slab(DevCsr<T>& M, int ebase);
   void upload_value_maps();
   bool maps_ready_ = false;        // d_src / d_wsrc of A_, At_, P_ are on the device
@@ -439,18 +442,8 @@ void Engine<T>::build_csr(DevCsr<T>& dst, const HostCsr& h) {
   dst.rowptr.alloc(h.nrows + 1, false);
   dst.col.alloc(dst.nnz + 4, true);   // +4: the vector path never reads past nnz, padding keeps ASAN-style tools quiet
   dst.val.alloc(dst.nnz + 4, true);
-  CUDA_TRY(cudaMemcpyAsync(dst.rowptr.p, h.rowptr.data(), (h.nrows + 1) * sizeof(int), cudaMemcpyHostToDevice, stream_));
-  if (dst.nnz) {
-    CUDA_TRY(cudaMemcpyAsync(dst.col.p, h.col.data(), dst.nnz * sizeof(int), cudaMemcpyHostToDevice, stream_));
-    if (sizeof(T) == sizeof(double)) {
-      CUDA_TRY(cudaMemcpyAsync(dst.val.p, h.val.data(), dst.nnz * sizeof(double), cudaMemcpyHostToDevice, stream_));
-      sync();
-    } else {
-      std::vector<float> tmp(h.val.begin(), h.val.end());
-      CUDA_TRY(cudaMemcpyAsync(dst.val.p, tmp.data(), dst.nnz * sizeof(float), cudaMemcpyHostToDevice, stream_));
-      sync();
-    }
-  }
+  dst.rowptr.upload(h.rowptr.data(), h.nrows + 1, stream_);
+  dst.col.upload(h.col.data(), dst.nnz, stream_);
   sync();
 }
 
@@ -472,9 +465,8 @@ struct WinGroupScratch {
 };
 }  // namespace
 
-template <typename T>
-static void win_fill_segment(const int* cols, const double* vals, const int* src, const int* idx, int k, int wbase,
-                             long long start, unsigned short* wc, T* wv, int* wsrc, WinGroupScratch& S) {
+static void win_fill_segment(const int* cols, const int* src, const int* idx, int k, int wbase, long long start,
+                             unsigned short* wc, int* wsrc, WinGroupScratch& S) {
   constexpr int GL = 16;                // lanes that share one shared-memory wavefront: a half-warp
   const int kpad = (k + 7) & ~7;
   if (kpad == 0) return;
@@ -528,96 +520,23 @@ static void win_fill_segment(const int* cols, const double* vals, const int* src
     const int st = g / GPS, h = (g % GPS) / 8, i = g % 8;
     const int nl = S.cap[g];
     for (int t = 0; t < nl; ++t) {
-      // column index: lane-contiguous (one 16-byte load per lane); value: instruction-coalesced
-      // (load k of lane l at k * EPL * L + l * EPL, see load8_coalesced)
+      // column position: lane-contiguous (one 16-byte load per lane); the value of the same entry sits at its
+      // instruction-coalesced position (matup::value_pos)
       const int lane = GL * h + t;
-      const int ls = std::min(32, lanes_total - 32 * st);
-      constexpr int EPL = 16 / (int)sizeof(T);
       const long long pos_c = start + (long long)st * 256 + (long long)lane * 8 + i;
-      const long long pos_v = start + (long long)st * 256 + (long long)(i / EPL) * (EPL * ls) + (long long)lane * EPL + (i % EPL);
       if (t < S.load[g]) {
         const int e = S.members[g][t];
         if (wc) wc[pos_c] = (unsigned short)(cols[e] - wbase);
-        if (wv) wv[pos_v] = (T)vals[e];
-        if (wsrc) wsrc[pos_c] = src ? src[e] : e;
+        wsrc[pos_c] = src ? src[e] : e;
       } else {   // padding: zero value on a bank this group does not use yet
         int r0 = 0;
         while (r0 < 15 && ((S.used[g] >> r0) & 1)) ++r0;
         S.used[g] |= (unsigned short)(1u << r0);
         if (wc) wc[pos_c] = (unsigned short)r0;
-        if (wv) wv[pos_v] = T(0);
-        if (wsrc) wsrc[pos_c] = -1;
+        wsrc[pos_c] = -1;
       }
     }
   }
-}
-
-// The 9 B layout of an fp64 slab (win_pack.h), built from the 10 B one in place: every 8-byte value becomes its packed
-// word at the same position, and the high column bits go to `colhi` at the column's position.  Escapes are numbered in
-// slab order (window-major, then row, then entry order of the segment), so the table does not depend on the thread
-// count.  Returns false, and leaves wv untouched, when more than 1/kEscDen of the stored entries would be escapes.
-namespace {
-struct WinPacked {
-  int ebase = 0;
-  std::vector<unsigned char> colhi;
-  std::vector<double> esc;
-};
-}  // namespace
-
-template <typename RowLoop>
-static bool win_pack(const std::vector<double>& hval, const std::vector<int>& rp, int nr, int nwin, long long total,
-                     const std::vector<unsigned short>& wc, std::vector<double>& wv, WinPacked& out, RowLoop parallel_rows) {
-  namespace wp = winpack;
-  // exponent window: the kCodes consecutive binades that hold the most finite normal values of the matrix
-  std::vector<long long> hist(2048, 0);
-  {
-    std::mutex mu;
-    parallel_rows([&](int a, int b) {
-      std::vector<long long> hl(2048, 0);
-      const long long k0 = (long long)hval.size() * a / nr, k1 = (long long)hval.size() * b / nr;
-      for (long long k = k0; k < k1; ++k) hl[wp::normal_exponent(hval[k])]++;
-      std::lock_guard<std::mutex> g(mu);
-      for (int e = 0; e < 2048; ++e) hist[e] += hl[e];
-    });
-  }
-  const int ebase = wp::pick_ebase(hist.data());
-  // escapes per row segment, in slab order
-  std::vector<long long> esc_off((size_t)nwin * nr + 1, 0);
-  parallel_rows([&](int a, int b) {
-    for (int w = 0; w < nwin; ++w)
-      for (int r = a; r < b; ++r) {
-        long long c = 0;
-        for (int p = rp[(size_t)w * (nr + 1) + r]; p < rp[(size_t)w * (nr + 1) + r + 1]; ++p) c += wp::code_of(wv[p], ebase) == wp::kEscape;
-        esc_off[(size_t)w * nr + r + 1] = c;
-      }
-  });
-  for (size_t i = 1; i < esc_off.size(); ++i) esc_off[i] += esc_off[i - 1];
-  const long long nesc = esc_off.back();
-  if (nesc * wp::kEscDen > total) return false;
-  out.ebase = ebase;
-  out.colhi.assign((size_t)total + 8, 0);
-  out.esc.assign((size_t)nesc, 0.0);
-  parallel_rows([&](int a, int b) {
-    for (int w = 0; w < nwin; ++w)
-      for (int r = a; r < b; ++r) {
-        const int s = rp[(size_t)w * (nr + 1) + r], kpad = rp[(size_t)w * (nr + 1) + r + 1] - s;
-        long long ei = esc_off[(size_t)w * nr + r];
-        for (int idx = 0; idx < kpad; ++idx) {   // the entry order of the kernel: step, lane, slot
-          const int st = idx >> 8, l = (idx & 255) >> 3, i = idx & 7;
-          const int ls = std::min(32, (kpad >> 3) - 32 * st);
-          const long long pc = (long long)s + idx;
-          const long long pv = (long long)s + (long long)st * 256 + (long long)(i / 2) * (2 * ls) + (long long)l * 2 + (i % 2);
-          const double v = wv[pv];
-          const unsigned col = wc[pc];
-          uint32_t slot = 0;
-          if (wp::code_of(v, ebase) == wp::kEscape) { slot = (uint32_t)ei; out.esc[(size_t)ei++] = v; }
-          const uint64_t word = wp::encode_word(v, col, ebase, slot);
-          memcpy(&wv[pv], &word, 8);
-          out.colhi[pc] = wp::encode_colhi(col);
-        }
-      }
-  });
-  return true;
 }
 
 // fn(a, b) on contiguous ranges [a, b) of nr rows, one host thread each
@@ -633,11 +552,11 @@ static void parallel_rows(int nr, const std::function<void(int, int)>& fn) {
 }
 
 // Pass 2 of build_windows: the bank-aware placement of every row segment of a CSR (rowptr, col) into the slab laid out
-// by rp.  It depends on the pattern alone, so update_matrices runs it again without values (wc = wv = nullptr) to learn
-// which entry every slot holds: wsrc[slot] = src[k] (k itself when src is null), -1 for padding.
-template <typename T>
-static void win_place(const int* rowptr, const int* col, const double* vals, const int* src, int nr, int nwin, int W,
-                      const std::vector<int>& rp, unsigned short* wc, T* wv, int* wsrc) {
+// by rp: wc[slot] = the window-local column (or a free bank for padding), wsrc[slot] = src[k] (k itself when src is
+// null), -1 for padding.  It depends on the pattern alone, so the first update_matrices runs it again (wc = nullptr) to
+// recover the slot maps that create released.
+static void win_place(const int* rowptr, const int* col, const int* src, int nr, int nwin, int W,
+                      const std::vector<int>& rp, unsigned short* wc, int* wsrc) {
   parallel_rows(nr, [&](int a, int b) {
     WinGroupScratch S;
     std::vector<std::vector<int>> seg(nwin);
@@ -645,8 +564,7 @@ static void win_place(const int* rowptr, const int* col, const double* vals, con
       for (int w = 0; w < nwin; ++w) seg[w].clear();
       for (int k = rowptr[r]; k < rowptr[r + 1]; ++k) seg[col[k] / W].push_back(k);
       for (int w = 0; w < nwin; ++w)
-        win_fill_segment<T>(col, vals, src, seg[w].data(), (int)seg[w].size(), w * W, rp[(size_t)w * (nr + 1) + r], wc, wv,
-                            wsrc, S);
+        win_fill_segment(col, src, seg[w].data(), (int)seg[w].size(), w * W, rp[(size_t)w * (nr + 1) + r], wc, wsrc, S);
     }
   });
 }
@@ -661,7 +579,7 @@ static void report_windows(const DevCsr<T>& d) {
 }
 
 template <typename T>
-void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packed) {
+void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src, bool allow_packed) {
   dst.windowed = false;
   dst.packed = false;
   if (h.nrows == 0 || h.ncols == 0) return;
@@ -677,9 +595,8 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
   const int nr = h.nrows;
   std::vector<int> rp((size_t)nwin * (nr + 1), 0);
   std::vector<long long> row_cost(nr, 0);
-  auto rows = [&](const std::function<void(int, int)>& fn) { parallel_rows(nr, fn); };
   // pass 1: padded segment lengths
-  rows([&](int a, int b) {
+  parallel_rows(nr, [&](int a, int b) {
     std::vector<int> cnt(nwin);
     for (int r = a; r < b; ++r) {
       std::fill(cnt.begin(), cnt.end(), 0);
@@ -702,8 +619,8 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
   }
   const long long total = run;
   std::vector<unsigned short> wc((size_t)total + 8, 0);
-  std::vector<T> wv((size_t)total + 8, T(0));
-  win_place<T>(h.rowptr.data(), h.col.data(), h.val.data(), nullptr, nr, nwin, W, rp, wc.data(), wv.data(), nullptr);
+  std::vector<int> wsrc((size_t)total + 8, -1);
+  win_place(h.rowptr.data(), h.col.data(), src, nr, nwin, W, rp, wc.data(), wsrc.data());
   // contiguous row chunks per CTA, balanced by padded nnz (+ per-row overhead)
   // one CTA per (row chunk, window): chunks are contiguous row ranges balanced by padded nnz
   const int nchunks = std::max(1, num_sms_ / nwin);
@@ -723,59 +640,27 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, bool allow_packe
   dst.nwin = nwin; dst.W = W; dst.nctas = nctas; dst.w_elems = total;
   dst.w_rowptr.upload(rp, stream_);
   dst.w_cta_rows.upload(cta_rows, stream_);
+  // the values go in later (update_slab), through the slot map
+  dst.w_col.upload(wc, stream_);
+  dst.d_wsrc.upload(wsrc, stream_);
+  sync();
   // fp64: the 9 B layout unless the values need too many escapes, or device equilibration will rewrite the slab values
   // in place (ruiz_apply_win_kernel works on the 10 B layout)
-  if constexpr (sizeof(T) == sizeof(double)) {
-    WinPacked pk;
-    dst.packable = allow_packed && W - 1 <= (int)winpack::kMaxCol;
-    if (dst.packable && win_pack(h.val, rp, nr, nwin, total, wc, wv, pk, rows)) {
-      dst.packed = true;
-      dst.ebase = pk.ebase;
-      dst.w_nesc = (long long)pk.esc.size();
-      dst.w_word.alloc(wv.size(), false);
-      dst.w_word.upload(reinterpret_cast<const unsigned long long*>(wv.data()), wv.size(), stream_);
-      dst.w_colhi.upload(pk.colhi, stream_);
-      dst.w_esc.upload(pk.esc, stream_);
-      sync();
-    }
-  }
-  if (!dst.packed) {
-    dst.w_col.upload(wc, stream_);
-    dst.w_val.upload(wv, stream_);
-    sync();
-  }
-  report_windows(dst);
+  dst.packable = sizeof(T) == sizeof(double) && allow_packed && W - 1 <= (int)winpack::kMaxCol;
   dst.windowed = true;
 }
 
-// Julia CSC -> (a) CSR of the transpose (zero conversion: same arrays, rebased)
-//              (b) CSR of the matrix itself (stable counting-sort transposition)
-template <typename T>
-static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, HostCsr& csr_t, bool record_src = false) {
-  const long long nr = M.nrows, nc = M.ncols;
-  if (nr < 0 || nc < 0 || nr >= (1LL << 31) - 8 || nc >= (1LL << 31) - 8)
-    throw EngineError{COSMO_B200_ERR_INVALID, "matrix dimensions out of int32 range"};
-  const long long nnz = nc ? (M.colptr[nc] - base) : 0;
-  if (nnz < 0 || nnz >= (1LL << 31) - 8) throw EngineError{COSMO_B200_ERR_INVALID, "nnz out of int32 range"};
-  const T* vals = static_cast<const T*>(M.nzval);
-  csr_t.nrows = (int)nc; csr_t.ncols = (int)nr;
-  csr_t.rowptr.resize(nc + 1);
-  csr_t.col.resize(nnz);
-  csr_t.val.resize(nnz);
-  for (long long j = 0; j <= nc; ++j) {
-    long long v = nc ? M.colptr[j] - base : 0;
-    if (v < 0 || v > nnz || (j > 0 && v < csr_t.rowptr[j - 1])) throw EngineError{COSMO_B200_ERR_INVALID, "colptr not monotone"};
-    csr_t.rowptr[j] = (int)v;
-  }
+// CSR of a matrix from the CSR of its transpose (its CSC pattern): stable counting-sort transposition, with
+// csr.src[k] = the CSC index of the entry at CSR position k
+static void csr_transpose(const HostCsr& csr_t, HostCsr& csr) {
+  const long long nr = csr_t.ncols, nc = csr_t.nrows, nnz = (long long)csr_t.col.size();
   csr.nrows = (int)nr; csr.ncols = (int)nc;
   csr.rowptr.assign(nr + 1, 0);
   csr.col.resize(nnz);
-  csr.val.resize(nnz);
-  if (record_src) csr.src.resize(nnz);
-  int* const srcp = record_src ? csr.src.data() : nullptr;
-  // Stable counting-sort transposition, parallel over column blocks: thread t counts the rows of its columns, a prefix
-  // over (row, thread) gives every thread its own slots in every row, so the scatter needs no synchronisation and the
-  // entries of a row stay ordered by column whatever the thread count (deterministic).
+  csr.src.resize(nnz);
+  // Parallel over column blocks: thread t counts the rows of its columns, a prefix over (row, thread) gives every thread
+  // its own slots in every row, so the scatter needs no synchronisation and the entries of a row stay ordered by column
+  // whatever the thread count (deterministic).
   const int nt = (int)std::max<long long>(1, std::min<long long>(std::min<long long>(32, (long long)std::thread::hardware_concurrency()),
                                                                   std::min<long long>(nnz / 200000 + 1, nc ? nc : 1)));
   std::vector<long long> cb(nt + 1, 0);                    // column block boundaries, balanced by nnz
@@ -787,7 +672,6 @@ static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, Ho
   }
   cb[nt] = nc;
   std::vector<std::vector<int>> cnt(nt);
-  std::vector<int> bad(nt, 0);
   auto run = [&](const std::function<void(int)>& fn) {
     if (nt == 1) { fn(0); return; }
     std::vector<std::thread> th;
@@ -796,15 +680,8 @@ static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, Ho
   };
   run([&](int t) {
     cnt[t].assign(nr, 0);
-    for (long long k = csr_t.rowptr[cb[t]]; k < csr_t.rowptr[cb[t + 1]]; ++k) {
-      const long long r = M.rowval[k] - base;
-      if (r < 0 || r >= nr) { bad[t] = 1; return; }
-      csr_t.col[k] = (int)r;
-      csr_t.val[k] = (double)vals[k];
-      cnt[t][r]++;
-    }
+    for (long long k = csr_t.rowptr[cb[t]]; k < csr_t.rowptr[cb[t + 1]]; ++k) cnt[t][csr_t.col[k]]++;
   });
-  for (int t = 0; t < nt; ++t) if (bad[t]) throw EngineError{COSMO_B200_ERR_INVALID, "rowval out of range"};
   for (long long r = 0; r < nr; ++r) {
     int run_sum = csr.rowptr[r];
     for (int t = 0; t < nt; ++t) { const int c = cnt[t][r]; cnt[t][r] = run_sum; run_sum += c; }   // cnt -> first slot of (t, r)
@@ -816,10 +693,37 @@ static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, Ho
       for (int k = csr_t.rowptr[j]; k < csr_t.rowptr[j + 1]; ++k) {
         const int dstk = next[csr_t.col[k]]++;
         csr.col[dstk] = (int)j;
-        csr.val[dstk] = csr_t.val[k];
-        if (srcp) srcp[dstk] = k;
+        csr.src[dstk] = k;
       }
   });
+}
+
+// Julia CSC pattern -> (a) CSR of the transpose (zero conversion: same arrays, rebased)
+//                      (b) CSR of the matrix itself, with its CSR -> CSC map (csr_transpose)
+static void csc_to_host_csrs(const cosmo_b200_csc& M, int base, HostCsr& csr, HostCsr& csr_t) {
+  const long long nr = M.nrows, nc = M.ncols;
+  if (nr < 0 || nc < 0 || nr >= (1LL << 31) - 8 || nc >= (1LL << 31) - 8)
+    throw EngineError{COSMO_B200_ERR_INVALID, "matrix dimensions out of int32 range"};
+  const long long nnz = nc ? (M.colptr[nc] - base) : 0;
+  if (nnz < 0 || nnz >= (1LL << 31) - 8) throw EngineError{COSMO_B200_ERR_INVALID, "nnz out of int32 range"};
+  csr_t.nrows = (int)nc; csr_t.ncols = (int)nr;
+  csr_t.rowptr.resize(nc + 1);
+  csr_t.col.resize(nnz);
+  for (long long j = 0; j <= nc; ++j) {
+    long long v = nc ? M.colptr[j] - base : 0;
+    if (v < 0 || v > nnz || (j > 0 && v < csr_t.rowptr[j - 1])) throw EngineError{COSMO_B200_ERR_INVALID, "colptr not monotone"};
+    csr_t.rowptr[j] = (int)v;
+  }
+  std::atomic<bool> bad{false};
+  parallel_rows((int)nc, [&](int a, int b) {
+    for (long long k = csr_t.rowptr[a]; k < csr_t.rowptr[b]; ++k) {
+      const long long r = M.rowval[k] - base;
+      if (r < 0 || r >= nr) { bad = true; return; }
+      csr_t.col[k] = (int)r;
+    }
+  });
+  if (bad) throw EngineError{COSMO_B200_ERR_INVALID, "rowval out of range"};
+  csr_transpose(csr_t, csr);
 }
 
 template <typename T>
@@ -944,20 +848,36 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
     lap("cone tables");
     // device equilibration rewrites the slab values in place, which only the 10 B slab layout allows
     const bool pack_ok = !((p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0);
+    // The host lays out the patterns; the values are written on the device the way update_matrices writes them, through
+    // value maps that are released as soon as they have been used (an engine that never updates does not keep them).
     HostCsr a, at, pp, ppt;
-    csc_to_host_csrs<T>(p.A, p.index_base, a, at);
+    csc_to_host_csrs(p.A, p.index_base, a, at);
     lap("csc -> csr (A, A')");
     build_csr(A_, a);
-    lap("upload csr A");
-    build_windows(A_, a, pack_ok);
-    lap("windows A");
     build_csr(At_, at);
-    lap("upload csr A'");
-    build_windows(At_, at, pack_ok);
+    upload_vec(At_.val, p.A.nzval, (size_t)At_.nnz);   // CSR(A') is the CSC order of A
+    A_.d_src.upload(a.src, stream_);
+    gather_csr(A_, At_.val.p);
+    A_.d_src.release();
+    lap("upload csr A, A'");
+    int ebase = 0;   // one exponent window for the packed slabs of A and A', computed when the first one needs it
+    auto fill_slab = [&](DevCsr<T>& M) {
+      if (M.packable && ebase == 0) ebase = exponent_window();
+      update_slab(M, ebase);
+      M.d_wsrc.release();
+    };
+    build_windows(A_, a, a.src.data(), pack_ok);
+    fill_slab(A_);
+    lap("windows A");
+    build_windows(At_, at, nullptr, pack_ok);
+    fill_slab(At_);
     lap("windows A'");
-    // P's CSC order is not resident: its CSR -> CSC map is kept for update_matrices (A's is derived from A')
-    csc_to_host_csrs<T>(p.P, p.index_base, pp, ppt, true);
+    // P's CSC order is not resident: its CSR -> CSC map stays on the host for update_matrices (A's is derived from A')
+    csc_to_host_csrs(p.P, p.index_base, pp, ppt);
     build_csr(P_, pp);
+    P_.d_src.upload(pp.src, stream_);
+    load_P(p.P.nzval);
+    P_.d_src.release();
     P_.h_src.swap(pp.src);
     lap("P");
     // A' and P rows are traversed by the same lane group in the fused operator kernel
@@ -1212,36 +1132,14 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
   CUDA_TRY(cudaSetDevice(device_));
   const double t0 = now_s();
   upload_value_maps();
-  auto gather = [&](DevCsr<T>& M, const T* v) {
-    matup::gather_kernel<T><<<vgrid(M.nnz), kBlock, 0, stream_>>>(M.nnz, M.d_src.p, v, M.val.p);
-    check_launch("update_matrices gather");
-  };
   if (Ax) {
     upload_vec(At_.val, Ax, (size_t)At_.nnz);   // CSR(A') is the CSC order of A
-    gather(A_, At_.val.p);
-    int ebase = 0;
-    if constexpr (sizeof(T) == sizeof(double)) {
-      if ((A_.windowed && A_.packable) || (At_.windowed && At_.packable)) {   // one exponent window for A and A'
-        DevBuf<unsigned long long> hist;
-        hist.alloc(2048);
-        matup::exp_hist_kernel<<<std::min(vgrid(At_.nnz), 4 * num_sms_), kBlock, 0, stream_>>>(At_.nnz, At_.val.p, hist.p);
-        check_launch("update_matrices exp_hist");
-        std::vector<long long> h(2048);
-        CUDA_TRY(cudaMemcpyAsync(h.data(), hist.p, 2048 * sizeof(long long), cudaMemcpyDeviceToHost, stream_));
-        sync();
-        ebase = winpack::pick_ebase(h.data());
-      }
-    }
+    gather_csr(A_, At_.val.p);
+    const int ebase = A_.packable || At_.packable ? exponent_window() : 0;   // one exponent window for A and A'
     update_slab(A_, ebase);
     update_slab(At_, ebase);
   }
-  if (Px) {
-    DevBuf<T> px;
-    px.alloc((size_t)P_.nnz, false);
-    upload_vec(px, Px, (size_t)P_.nnz);
-    gather(P_, px.p);
-    sync();
-  }
+  if (Px) load_P(Px);
   if (q) upload_vec(q_, q, n_);
   if (b) {
     upload_vec(b_, b, m_);
@@ -1261,12 +1159,47 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
   create_time_ = now_s() - t0;
 }
 
-// The value maps of update_matrices, made once and kept on the device.  Creating an engine records only the CSR(P) map
-// (P's CSC order is not resident); the others follow from the resident pattern: CSR(A) position -> CSC index by the
-// stable counting sort of csc_to_host_csrs over A' (the CSC pattern itself), and slab slot -> CSC index, -1 for
-// padding, by running build_windows' placement again on the same CSR pattern and row layout.  Padding cannot be told
-// from a stored zero by its content, but the placement is a function of the pattern, so it places every entry where
-// create placed it.  Engines that never update pay nothing for the maps, in time or memory.
+// CSR values through the CSR -> CSC map M.d_src: M.val[k] = v[src[k]]
+template <typename T>
+void Engine<T>::gather_csr(DevCsr<T>& M, const T* v) {
+  matup::gather_kernel<T><<<vgrid(M.nnz), kBlock, 0, stream_>>>(M.nnz, M.d_src.p, v, M.val.p);
+  check_launch("gather_csr");
+  sync();
+}
+
+// P's CSR values from its CSC values (host), through P_.d_src
+template <typename T>
+void Engine<T>::load_P(const void* Px) {
+  DevBuf<T> px;
+  px.alloc((size_t)P_.nnz, false);
+  upload_vec(px, Px, (size_t)P_.nnz);
+  gather_csr(P_, px.p);
+}
+
+// The window base of the packed slabs of A and A' (win_pack.h): the kCodes binades that hold the most finite normal
+// values of A, from its values in At_.val.  Integer histogram on the device, window picked on the host.
+template <typename T>
+int Engine<T>::exponent_window() {
+  if constexpr (sizeof(T) != sizeof(double)) {
+    return 0;
+  } else {
+    DevBuf<unsigned long long> hist;
+    hist.alloc(2048);
+    matup::exp_hist_kernel<<<std::min(vgrid(At_.nnz), 4 * num_sms_), kBlock, 0, stream_>>>(At_.nnz, At_.val.p, hist.p);
+    check_launch("exp_hist");
+    std::vector<long long> h(2048);
+    CUDA_TRY(cudaMemcpyAsync(h.data(), hist.p, 2048 * sizeof(long long), cudaMemcpyDeviceToHost, stream_));
+    sync();
+    return winpack::pick_ebase(h.data());
+  }
+}
+
+// The value maps of update_matrices, made by the first update and kept on the device.  Creating an engine keeps only
+// the CSR(P) map (P's CSC order is not resident); the others are derived again from the resident pattern with the
+// functions create used: CSR(A) position -> CSC index by csr_transpose of A' (the CSC pattern itself), and slab slot ->
+// CSC index, -1 for padding, by win_place on the same CSR pattern and row layout.  Padding cannot be told from a stored
+// zero by its content, but the placement is a function of the pattern, so it places every entry where create placed
+// it.  Engines that never update pay nothing for the maps, in time or memory.
 template <typename T>
 void Engine<T>::upload_value_maps() {
   if (maps_ready_) return;
@@ -1274,38 +1207,34 @@ void Engine<T>::upload_value_maps() {
     v.resize(cnt);
     if (cnt) CUDA_TRY(cudaMemcpyAsync(v.data(), d, cnt * sizeof(int), cudaMemcpyDeviceToHost, stream_));
   };
-  std::vector<int> arow, acol, atrow, atcol;
-  down(atrow, At_.rowptr.p, (size_t)n_ + 1);
-  down(atcol, At_.col.p, (size_t)At_.nnz);
-  down(arow, A_.rowptr.p, (size_t)m_ + 1);
-  if (A_.windowed) down(acol, A_.col.p, (size_t)A_.nnz);
+  HostCsr a, at;
+  at.nrows = n_; at.ncols = m_;
+  down(at.rowptr, At_.rowptr.p, (size_t)n_ + 1);
+  down(at.col, At_.col.p, (size_t)At_.nnz);
   sync();
-  std::vector<int> asrc((size_t)A_.nnz);
-  {
-    std::vector<int> next(arow.begin(), arow.end() - 1);
-    for (int j = 0; j < n_; ++j)
-      for (int k = atrow[j]; k < atrow[j + 1]; ++k) asrc[next[atcol[k]]++] = k;
-  }
-  A_.d_src.upload(asrc, stream_);
+  csr_transpose(at, a);
+  A_.d_src.upload(a.src, stream_);
   P_.d_src.upload(P_.h_src, stream_);
-  auto slab = [&](DevCsr<T>& M, const std::vector<int>& row, const std::vector<int>& col, const int* src) {
+  auto slab = [&](DevCsr<T>& M, const HostCsr& h, const int* src) {
     if (!M.windowed) return;
     std::vector<int> rp;
     down(rp, M.w_rowptr.p, (size_t)M.nwin * (M.nrows + 1));
     sync();
     std::vector<int> wsrc((size_t)M.w_elems + 8, -1);
-    win_place<T>(row.data(), col.data(), nullptr, src, M.nrows, M.nwin, M.W, rp, nullptr, nullptr, wsrc.data());
+    win_place(h.rowptr.data(), h.col.data(), src, M.nrows, M.nwin, M.W, rp, nullptr, wsrc.data());
     M.d_wsrc.upload(wsrc, stream_);
     sync();
   };
-  slab(A_, arow, acol, asrc.data());
-  slab(At_, atrow, atcol, nullptr);
+  slab(A_, a, a.src.data());
+  slab(At_, at, nullptr);
   sync();
   std::vector<int>().swap(P_.h_src);
   maps_ready_ = true;
 }
 
-// New slab values of a windowed matrix from the CSC values in At_.val, in the layout create would choose for them.
+// Slab values of a windowed matrix from the CSC values in At_.val, in the layout their escapes call for (win_pack.h).
+// create calls it on a fresh slab, which holds the columns (w_col) and no values yet; an update on a filled one, in
+// either layout.
 template <typename T>
 void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
   if (!M.windowed) return;
@@ -1316,7 +1245,7 @@ void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
       DevBuf<int> cnt;
       cnt.alloc((size_t)nseg, false);
       matup::slab_esc_count_kernel<<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, ebase, cnt.p);
-      check_launch("update_matrices esc_count");
+      check_launch("slab_esc_count");
       std::vector<int> hc((size_t)nseg);
       CUDA_TRY(cudaMemcpyAsync(hc.data(), cnt.p, (size_t)nseg * sizeof(int), cudaMemcpyDeviceToHost, stream_));
       sync();
@@ -1327,19 +1256,19 @@ void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
         DevBuf<long long> doff;
         doff.upload(off, stream_);
         if ((long long)M.w_esc.n < nesc) M.w_esc.alloc((size_t)nesc, false);
-        if (!M.packed) {   // 10 B -> 9 B: the columns come from w_col
+        if (!M.packed) {   // 10 B (or fresh) -> 9 B: the columns come from w_col
           M.w_word.alloc((size_t)M.w_elems + 8);
           M.w_colhi.alloc((size_t)M.w_elems + 8);
           matup::slab_encode_kernel<true><<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, ebase,
                                                                        doff.p, M.w_col.p, M.w_word.p, M.w_colhi.p, M.w_esc.p);
-          check_launch("update_matrices encode");
+          check_launch("slab_encode");
           sync();
           M.w_col.release();
           M.w_val.release();
         } else {
           matup::slab_encode_kernel<false><<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, ebase,
                                                                         doff.p, nullptr, M.w_word.p, M.w_colhi.p, M.w_esc.p);
-          check_launch("update_matrices encode");
+          check_launch("slab_encode");
           sync();
         }
         M.packed = true;
@@ -1351,8 +1280,7 @@ void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
       if (M.packed) {   // 9 B -> 10 B: decode the columns before the words go
         M.w_col.alloc((size_t)M.w_elems + 8);
         matup::slab_unpack_col_kernel<<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.w_word.p, M.w_colhi.p, M.w_col.p);
-        check_launch("update_matrices unpack_col");
-        M.w_val.alloc((size_t)M.w_elems + 8);
+        check_launch("slab_unpack_col");
         sync();
         M.w_word.release();
         M.w_colhi.release();
@@ -1363,8 +1291,9 @@ void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
       }
     }
   }
+  if (!M.w_val.p) M.w_val.alloc((size_t)M.w_elems + 8);   // a fresh slab, or one that was 9 B
   matup::slab_gather_kernel<T><<<grid, kBlock, 0, stream_>>>(M.nwin, M.nrows, M.w_rowptr.p, M.d_wsrc.p, At_.val.p, M.w_val.p);
-  check_launch("update_matrices slab_gather");
+  check_launch("slab_gather");
   sync();
   report_windows(M);
 }
@@ -2881,16 +2810,11 @@ int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* p, int64_t* perm, int64_t*
   try {
     if (p->m < 0 || p->n < 0 || p->A.nrows != p->m || p->A.ncols != p->n || p->P.nrows != p->n || p->P.ncols != p->n)
       throw cosmo::EngineError{COSMO_B200_ERR_INVALID, "P must be n x n and A m x n"};
-    cosmo::HostCsr a, at, pp, ppt;
-    if (p->dtype == COSMO_B200_F64) {
-      cosmo::csc_to_host_csrs<double>(p->A, p->index_base, a, at);
-      cosmo::csc_to_host_csrs<double>(p->P, p->index_base, pp, ppt);
-    } else if (p->dtype == COSMO_B200_F32) {
-      cosmo::csc_to_host_csrs<float>(p->A, p->index_base, a, at);
-      cosmo::csc_to_host_csrs<float>(p->P, p->index_base, pp, ppt);
-    } else {
+    if (p->dtype != COSMO_B200_F64 && p->dtype != COSMO_B200_F32)
       throw cosmo::EngineError{COSMO_B200_ERR_UNSUPPORTED, "dtype must be Float64 or Float32"};
-    }
+    cosmo::HostCsr a, at, pp, ppt;
+    cosmo::csc_to_host_csrs(p->A, p->index_base, a, at);
+    cosmo::csc_to_host_csrs(p->P, p->index_base, pp, ppt);
     cosmo::ldl::Symbolic S;
     cosmo::ldl::analyze((int)p->n, (int)p->m, pp.rowptr, pp.col, at.rowptr, at.col, S);
     for (int j = 0; j < S.N; ++j) {

@@ -1,12 +1,12 @@
-// mat_update.cuh -- new values of P and A in the layouts that create built (cosmo_b200_update_matrices).
+// mat_update.cuh -- the values of P and A in the layouts the host built from their patterns: the one value path of
+// engine creation and of cosmo_b200_update_matrices.
 //
 // The sparsity pattern fixes every layout: the CSR order of A and P, and the slot of every entry in the column-windowed
-// slabs (win_fill_segment places entries by column only).  create records where each stored value came from -- CSR
-// position -> CSC index, slab column position -> CSC index or -1 for padding -- and an update gathers the new CSC values
-// through those maps.  The 9 B slabs are re-encoded the way win_pack does it on the host, with the same win_pack.h
-// functions: one exponent histogram, the window base picked on the host, escapes counted per (window, row) segment and
-// numbered in slab order, so the words, the escape table and the layout decision are the ones create would produce from
-// the same values.
+// slabs (win_fill_segment places entries by column only).  Maps say where each stored value comes from -- CSR position
+// -> CSC index, slab column position -> CSC index or -1 for padding -- and the CSC values are gathered through them.
+// The 9 B slabs are encoded with the win_pack.h functions: one exponent histogram, the window base picked on the host,
+// escapes counted per (window, row) segment and numbered in slab order, so the words, the escape table and the layout
+// decision depend on the pattern and the values alone.
 // Included from engine.cu (after common.cuh).
 #pragma once
 #include "win_pack.h"
@@ -22,7 +22,7 @@ __global__ void __launch_bounds__(kBlock) gather_kernel(long long n, const int* 
     out[i] = v[src[i]];
 }
 
-// histogram of the biased exponents of the finite normal values (win_pack's exponent window); integer atomics, so the
+// histogram of the biased exponents of the finite normal values (the exponent window, pick_ebase); integer atomics, so the
 // counts do not depend on the schedule
 __global__ void __launch_bounds__(kBlock) exp_hist_kernel(long long n, const double* __restrict__ v,
                                                           unsigned long long* __restrict__ hist) {
@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(kBlock) exp_hist_kernel(long long n, const dou
 }
 
 // value position of the entry at column position `idx` of a segment of `kpad` entries starting at `s`: the
-// instruction-coalesced value order of win_fill_segment (EPL values per 16-byte load)
+// instruction-coalesced value order spmv_win_kernel loads (load8_coalesced: EPL values per 16-byte load)
 template <int EPL>
 __device__ __forceinline__ long long value_pos(long long s, int kpad, int idx) {
   const int st = idx >> 8, l = (idx & 255) >> 3, i = idx & 7;
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(kBlock) slab_esc_count_kernel(int nwin, int nr
   });
 }
 
-// 9 B words, column-high bytes and escape table of a slab (win_pack): escapes take consecutive slots from the segment's
+// 9 B words, column-high bytes and escape table of a slab (win_pack.h): escapes take consecutive slots from the segment's
 // offset in column-position order.  The window-local column comes from w_col (FROM_COL: the slab was 10 B) or is
 // decoded from the word and colhi the slab already holds (the column bits never change).
 template <bool FROM_COL>

@@ -1,4 +1,4 @@
-// win_pack.h -- the 9-byte entry of the packed fp64 column-windowed slabs (spmv_win_kernel, build_windows).
+// win_pack.h -- the 9-byte entry of the packed fp64 column-windowed slabs (spmv_win_kernel, mat_update.cuh).
 //
 // A window is at most 25 600 doubles wide, so a window-local column needs 15 bits, and the values of one matrix span
 // few binades.  A packed entry keeps the 52 mantissa bits and the sign of its value, a 4-bit exponent code and the
@@ -10,9 +10,9 @@
 //   code 15     escape: the value is esc[low 32 bits of the word], a per-matrix table of exact doubles (subnormals,
 //               Inf, NaN with its payload, every exponent outside [ebase, ebase + 13])
 // The decode is lossless: it returns the stored double bit for bit.  It touches only the high 32 bits of the word; the
-// low word (mantissa bits 0-31, or the escape index) passes through.  Plain C++ with __host__ __device__ functions,
-// so a host program can check the very functions the kernel calls, and the device re-encoder of an update
-// (mat_update.cuh) writes the words the host builder writes.
+// low word (mantissa bits 0-31, or the escape index) passes through.  The encoder runs on the device only: the slab
+// kernels of mat_update.cuh call these functions when an engine is created and when its values are updated.  They
+// are plain C++ with __host__ __device__ qualifiers, so a host program can check the very functions the kernels call.
 #pragma once
 #include <stdint.h>
 #include <string.h>

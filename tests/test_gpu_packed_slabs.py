@@ -49,10 +49,29 @@ def _count(counts, part):
 
 
 def _layouts(capfd):
-    """(layout, ebase, escapes) of every windowed matrix the last engine creation reported, A first, then A'"""
+    """(layout, ebase, escapes, windows, window width) of every windowed matrix the last engine creation reported, A
+    first, then A'"""
     err = capfd.readouterr().err
-    return [(m.group(1), int(m.group(2)), int(m.group(3)))
-            for m in re.finditer(r"\[setup\] windows .*?: (\d+ B) layout, ebase (\d+), (\d+) escapes", err)]
+    return [(m.group(3), int(m.group(4)), int(m.group(5)), int(m.group(1)), int(m.group(2)))
+            for m in re.finditer(r"\[setup\] windows (\d+) x (\d+), \d+ rows: (\d+ B) layout, ebase (\d+), (\d+) escapes", err)]
+
+
+def _assert_layout_rule(A, lay):
+    """The layouts reported for A and A', recomputed with NumPy: the exponent window is the first of the 14-binade
+    windows that hold the most finite normal values, the escapes are the stored nonzero values outside it, and a slab
+    is packed iff escapes * 256 <= its slots (every (row, window) segment padded to a multiple of 8 entries)."""
+    data = np.ascontiguousarray(A.data, dtype=np.float64)
+    e = ((data.view(np.uint64) >> np.uint64(52)) & np.uint64(0x7FF)).astype(np.int64)
+    hist = np.bincount(e[(e != 0) & (e != 0x7FF)], minlength=2048)
+    ebase = 1 + int(np.argmax(np.convolve(hist[1:2047], np.ones(14, dtype=np.int64), "valid")))
+    nesc = int(np.count_nonzero((data != 0) & ((e < ebase) | (e > ebase + 13))))
+    assert len(lay) == 2, lay
+    for M, (layout, eb, esc, nwin, W) in zip((sp.coo_matrix(A), sp.coo_matrix(A.T)), lay):
+        seg = np.bincount(M.row.astype(np.int64) * nwin + M.col // W, minlength=M.shape[0] * nwin)
+        slots = int(((seg + 7) // 8 * 8).sum())
+        assert (layout == "9 B") == (nesc * 256 <= slots), (layout, nesc, slots)
+        if layout == "9 B":
+            assert (eb, esc) == (ebase, nesc), (eb, esc, ebase, nesc)
 
 
 def _windowed_matrix(rng, values, m=20000, n=40000, per_col=30):
@@ -87,7 +106,8 @@ def test_gaussian_values_are_packed_with_escapes(tmp_path, capfd, monkeypatch):
     eng = _eye_engine(A)
     lay = _layouts(capfd)
     assert [l[0] for l in lay] == ["9 B", "9 B"], lay
-    assert all(0 < esc <= A.nnz / 256 for _, _, esc in lay), lay      # the smallest |values| escape
+    assert all(0 < esc <= A.nnz / 256 for _, _, esc, _, _ in lay), lay      # the smallest |values| escape
+    _assert_layout_rule(A, lay)
     counts = _kernel_counts(lambda: eng.spmv(0, np.ones(A.shape[1])), tmp_path)
     assert _count(counts, PACKED) > 0 and _count(counts, PLAIN) == 0, counts
     _check_products(eng, A, rng)
@@ -111,6 +131,7 @@ def test_special_values_stay_packed_and_exact(tmp_path, capfd, monkeypatch):
     eng = _eye_engine(A)
     lay = _layouts(capfd)
     assert [l[0] for l in lay] == ["9 B", "9 B"], lay
+    _assert_layout_rule(A, lay)
     # A e_j is column j exactly: every special value comes back as stored (zeros compare equal up to their sign)
     e = np.zeros(A.shape[1])
     e[j] = 1.0
@@ -151,6 +172,7 @@ def test_wide_value_range_keeps_the_10_byte_layout(tmp_path, capfd, monkeypatch)
     eng = _eye_engine(A)
     lay = _layouts(capfd)
     assert [l[0] for l in lay] == ["10 B", "10 B"], lay
+    _assert_layout_rule(A, lay)
     counts = _kernel_counts(lambda: eng.spmv(1, np.ones(A.shape[0])), tmp_path)
     assert _count(counts, PLAIN) > 0 and _count(counts, PACKED) == 0, counts
     _check_products(eng, A, rng)
@@ -189,6 +211,7 @@ def test_admm_solve_on_packed_slabs_matches_oracle(tmp_path, capfd, monkeypatch)
     eng = _engine(P, q, A, b, sets, **kw)
     lay = _layouts(capfd)
     assert [l[0] for l in lay] == ["9 B", "9 B"], lay
+    _assert_layout_rule(A, lay)
     ref = O.solve(P, q, A, b, to_oracle_cones(sets), O.Settings(kkt_solver="cg", **kw))
     outs = []
     counts = _kernel_counts(lambda: outs.append(eng.solve()), tmp_path, reps=1)
