@@ -18,24 +18,28 @@ namespace cosmo {
 
 enum { AA_F2 = 0, AA_FACC2 = 1, AA_FLAG = 2, AA_NRM2 = 3, AA_SC_COUNT = 8 };
 
-// CA.update!: f = x - g; first call after a restart only stores (g, f); otherwise the new columns
-//   G[:, j] = g - g_last,  Q[:, j] = f - f_last (orthogonalised afterwards),  then g_last = g, f_last = f.
+// CA.update! of every variant: f = x - g; after a restart only (g_last, f_last and, for Type1, x_last) are stored;
+// otherwise G[:, j] = g - g_last, F[:, j] = f - f_last and, for Type1 (Xj != nullptr), X[:, j] = x - x_last.
+// F lives in Q; the QR variant orthogonalises the new column afterwards.
 // out[0] = |f|^2 over [lo, dim)  (the safeguard's reference norm, accelerator_interface.jl:90).
 template <typename T>
-__global__ void __launch_bounds__(kBlock) aa_update_kernel(int dim, int lo, const T* __restrict__ g, const T* __restrict__ x,
-                                                           T* __restrict__ f, T* __restrict__ f_last, T* __restrict__ g_last,
-                                                           T* __restrict__ Gj, T* __restrict__ Qj, int init, RedBuf<T> rb) {
+__global__ void __launch_bounds__(kBlock) aa_hist_kernel(int dim, int lo, const T* __restrict__ g, const T* __restrict__ x,
+                                                         T* __restrict__ f, T* __restrict__ f_last, T* __restrict__ g_last,
+                                                         T* __restrict__ x_last, T* __restrict__ Gj, T* __restrict__ Fj,
+                                                         T* __restrict__ Xj, int init, RedBuf<T> rb) {
   T accS[1] = {0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dim; i += gridDim.x * blockDim.x) {
-    const T gi = g[i];
-    const T fi = x[i] - gi;
+    const T gi = g[i], xi = x[i];
+    const T fi = xi - gi;
     f[i] = fi;
     if (!init) {
       Gj[i] = gi - g_last[i];
-      Qj[i] = fi - f_last[i];
+      Fj[i] = fi - f_last[i];
+      if (Xj) Xj[i] = xi - x_last[i];
     }
     g_last[i] = gi;
     f_last[i] = fi;
+    if (x_last) x_last[i] = xi;
     if (i >= lo) accS[0] += fi * fi;
   }
   reduce_and_finalize<T, 1, 0>(accS, (const T*)nullptr, rb, NoFin());
@@ -125,32 +129,6 @@ __global__ void __launch_bounds__(kBlock) aa_apply_kernel(int dim, T* __restrict
 // column j refreshes row j and column j of M against the whole window (RollingMemory overwrites column iter mod mem).
 // ---------------------------------------------------------------------------------------------------------------
 enum { AA_GRAM_COLS = 8, AA_GRAM_NR = 3 * AA_GRAM_COLS + 2, AA_GRAM_MAX_CHUNKS = 4 };
-
-// CA.update! of the normal-equation variants: f = x - g; after a restart only (x_last, g_last, f_last) are stored;
-// otherwise G[:, j] = g - g_last, F[:, j] = f - f_last and, for Type1 (Xj != nullptr), X[:, j] = x - x_last.
-// out[0] = |f|^2 over [lo, dim) for the safeguard.
-template <typename T>
-__global__ void __launch_bounds__(kBlock) aa_hist_kernel(int dim, int lo, const T* __restrict__ g, const T* __restrict__ x,
-                                                         T* __restrict__ f, T* __restrict__ f_last, T* __restrict__ g_last,
-                                                         T* __restrict__ x_last, T* __restrict__ Gj, T* __restrict__ Fj,
-                                                         T* __restrict__ Xj, int init, RedBuf<T> rb) {
-  T accS[1] = {0};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dim; i += gridDim.x * blockDim.x) {
-    const T gi = g[i], xi = x[i];
-    const T fi = xi - gi;
-    f[i] = fi;
-    if (!init) {
-      Gj[i] = gi - g_last[i];
-      Fj[i] = fi - f_last[i];
-      if (Xj) Xj[i] = xi - x_last[i];
-    }
-    g_last[i] = gi;
-    f_last[i] = fi;
-    if (x_last) x_last[i] = xi;
-    if (i >= lo) accS[0] += fi * fi;
-  }
-  reduce_and_finalize<T, 1, 0>(accS, (const T*)nullptr, rb, NoFin());
-}
 
 // The fused Gram + right-hand-side pass over window columns c = c0 .. c0 + ncols - 1 (ncols <= 8) of A (X for
 // Type1, F for Type2) and B = F, the new column j and f; each history column is read once:

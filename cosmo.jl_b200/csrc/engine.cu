@@ -263,21 +263,19 @@ class Engine : public EngineBase {
   int aa_iter_ = 0;            // columns filled since the last restart
   bool aa_init_ = true, aa_success_ = false, aa_active_ = false;
   long long aa_accelerated_ = 0, aa_declined_ = 0;
-  // variant and activation reason (cosmo_b200_set_accelerator); the default runs aa_update / aa_accelerate above
+  // variant and activation reason (cosmo_b200_set_accelerator); the default is the QR variant above
   cosmo_b200_accelerator acc_{COSMO_B200_AA_TYPE2_QR, COSMO_B200_AA_RESTARTED_MEMORY, COSMO_B200_AA_NO_REGULARIZER,
                               COSMO_B200_AA_IMMEDIATE, 0.0, 2, 0.0};
   long long aa_rejected_ = 0, aa_rho_restarts_ = 0, aa_mem_restarts_ = 0, aa_activated_at_ = 0;
   // normal-equation variants: F is stored in aaQ_, M in aaR_ (row-major, leading dimension aa_mem_)
   DevBuf<T> aaX_, aa_xlast_, aa_nrm_, aa_gsc_, aa_gpart_;
-  int aa_j_ = 0;               // column written by the last aa_update_ne
-  bool aa_fresh_ = false;      // aa_update_ne wrote a column that aa_accelerate_ne has not used yet
-  bool aa_ne() const { return acc_.type != COSMO_B200_AA_TYPE2_QR; }
+  int aa_j_ = 0;               // column written by the last aa_update
+  bool aa_fresh_ = false;      // aa_update wrote a column that aa_accelerate has not used yet
+  bool aa_qr() const { return acc_.type == COSMO_B200_AA_TYPE2_QR; }
   void aa_prepare();
   void aa_restart() { aa_iter_ = 0; aa_init_ = true; aa_fresh_ = false; }
   void aa_update(const T* g, const T* x);
   bool aa_accelerate(T* g);
-  void aa_update_ne(const T* g, const T* x);
-  bool aa_accelerate_ne(T* g);
   // ---- state ----
   DevBuf<T> W_[2];           // operator variable, ping-pong (w / w_prev)
   int cur_ = 0, prev_ = 1;
@@ -354,8 +352,16 @@ class Engine : public EngineBase {
   // ---- helpers ----
   RedBuf<T> red(int out_slot) { return RedBuf<T>{partials_.p, sc_.p + out_slot, ticket_.p}; }
   RedBuf<T> red_ptr(T* out) { return RedBuf<T>{partials_.p, out, ticket_.p}; }
-  // K5 + K7 pass: 128-bit kernel for fp64 when every (n+m)-vector's m-part is 16-byte aligned (n even; ws_rhs too)
-  void launch_proj_rhs(const ProjRhsArgs<T>& a) {
+  // K5 + K7 pass over w: the projection (do_proj) and / or the right-hand side of admm_x! from ws_rhs (do_rhs).
+  // 128-bit kernel for fp64 when every (n+m)-vector's m-part is 16-byte aligned (n even; ws_rhs too)
+  void launch_proj_rhs(const T* w, const T* ws_rhs, bool do_proj, bool do_rhs) {
+    ProjRhsArgs<T> a;
+    a.n = n_; a.m = m_; a.w = w; a.ws_rhs = ws_rhs;
+    a.q = q_.p; a.b = b_.p; a.rho = rho_vec_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
+    a.row_class = row_class_.p; a.row_cone = row_cone_.p;
+    a.soc = SocTable<T>{soc_off_.p, soc_norm_.p};
+    a.s = s_.p; a.ls = ls_.p; a.t0 = t0_.p; a.sigma = (T)st_.sigma;
+    a.do_proj = do_proj ? 1 : 0; a.do_rhs = do_rhs ? 1 : 0;
     if constexpr (std::is_same<T, double>::value) {
       if ((a.n & 1) == 0 && ((reinterpret_cast<uintptr_t>(a.ws_rhs) & 15) == 0) && ((reinterpret_cast<uintptr_t>(a.w) & 15) == 0)) {
         const long long pairs = (a.n >> 1) + ((a.m + 1) >> 1);
@@ -405,11 +411,16 @@ class Engine : public EngineBase {
   void kkt_op_stage2(const int* done, const T* u, const T* t_in, T* c_out, bool exchange = false);
   void kkt_cg(const int* done, bool tm_ready);
   void kkt_minres(bool full);
+  // get_tolerance (kktsolver_indirect.jl:168-170): tol_constant / k^tol_exponent for the k-th inner solve
+  double inner_tol() const { return st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent); }
+  template <typename Enqueue>
+  int poll_inner(const Enqueue& enqueue);
   void set_maxit(int v);
   void compute_residuals(const T* x, const T* s, const T* mu, bool ignore_scaling, double out[5]);
   bool adapt_rho(const T* x);
   bool primal_infeasible();
   bool dual_infeasible();
+  int cone_certificates(const T* v, T eps);
   double inf_rec_[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // what the last primal_infeasible / dual_infeasible computed
   void recover_mu(const T* w_prev) {
     recover_mu_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_vec_.p, w_prev + n_, s_.p, mu_.p);
@@ -1481,14 +1492,7 @@ void Engine<T>::project_device(const T* w, bool with_rhs, const T* ws_rhs) {
     cone3_project_kernel<T><<<(n_c3_ + 127) / 128, 128, 0, stream_>>>(c3_table(), w + n_, s_.p);
     check_launch("cone3_project");
   }
-  ProjRhsArgs<T> a;
-  a.n = n_; a.m = m_; a.w = w; a.ws_rhs = ws_rhs ? ws_rhs : w + n_;
-  a.q = q_.p; a.b = b_.p; a.rho = rho_vec_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
-  a.row_class = row_class_.p; a.row_cone = row_cone_.p;
-  a.soc = SocTable<T>{soc_off_.p, soc_norm_.p};
-  a.s = s_.p; a.ls = ls_.p; a.t0 = t0_.p; a.sigma = (T)st_.sigma;
-  a.do_proj = 1; a.do_rhs = with_rhs ? 1 : 0;
-  launch_proj_rhs(a);
+  launch_proj_rhs(w, ws_rhs ? ws_rhs : w + n_, true, with_rhs);
 }
 
 // c = A' tm + P u + sigma u ; cb[n] = u'c   (second half of reduced_mul!, kktsolver_indirect.jl:61-65)
@@ -1586,7 +1590,7 @@ template <typename T>
 void Engine<T>::kkt_cg(const int* done, bool tm_ready) {
   set_maxit(n_);   // IterativeSolvers default maxiter = size(A, 2)
   if (persistent_cg_ok()) {
-    launch_persistent_cg(st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent));
+    launch_persistent_cg(inner_tol());
     return;
   }
   // c = L x0 (warm start => one product for the initial residual); tm = rho .* (A x0) is left by the previous
@@ -1596,21 +1600,30 @@ void Engine<T>::kkt_cg(const int* done, bool tm_ready) {
                 red(SC_TMP0), "spmv_A_scale");
   kkt_op_stage2(nullptr, xsol_.p, tm_.p, cb_.p, true);
   if (!p2p_) allreduce_sum(cb_.p, n_ + 1);
-  const double tol_num = st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent);
   launch_pdl(cg_init_kernel<T>, vgrid(n_), kBlock, 0, stream_, n_, (const T*)rhsb_.p, (const T*)cb_.p, r_.p, u_.p, red(SC_RES2),
-             CgInitFin<T>{sc_.p, isc_.p, (T)tol_num, p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
+             CgInitFin<T>{sc_.p, isc_.p, (T)inner_tol(), p2p_ ? xchg_seq_.p : nullptr}, p2p_, xv_);
   check_launch("cg_init");
   // NCCL collectives are capturable too: sharded runs replay the same graphs
   if (!cg_graph_[0]) build_cg_graphs(done);
-  int chunk = std::max(last_cg_iters_, 0);
-  for (;;) {
-    int left = chunk;
+  total_mults_ += 1 + poll_inner([&](int k) {
     for (int b = 3; b >= 0; --b)
-      while (left >= (1 << b)) {
+      while (k >= (1 << b)) {
         CUDA_TRY(cudaGraphLaunch(cg_graph_[b], stream_));
         launches_ += (long long)(1 << b) * (At_.windowed && P_.windowed && P_.nnz > 0 && rank_ == 0 ? 5 : 4);
-        left -= (1 << b);
+        k -= (1 << b);
       }
+  });
+}
+
+// The host loop of both iterative KKT solvers: enqueue(k) enqueues k iterations, which stop themselves on the device
+// once converged; the first chunk is the previous solve's count, then one iteration at a time until ISC_DONE is set.
+// Records the count in last_cg_iters_ and total_inner_ and returns it.
+template <typename T>
+template <typename Enqueue>
+int Engine<T>::poll_inner(const Enqueue& enqueue) {
+  int chunk = std::max(last_cg_iters_, 0);
+  for (;;) {
+    enqueue(chunk);
     CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
     sync();
     if (h_isc_[ISC_DONE]) break;
@@ -1619,7 +1632,7 @@ void Engine<T>::kkt_cg(const int* done, bool tm_ready) {
   const int iters = h_isc_[ISC_IT];
   last_cg_iters_ = iters;
   total_inner_ += iters;
-  total_mults_ += 1 + iters;
+  return iters;
 }
 
 template <typename T>
@@ -1727,15 +1740,14 @@ void Engine<T>::kkt_minres(bool full) {
   T* v_prev = mr_[0].p; T* v_curr = mr_[1].p; T* v_next = mr_[2].p;
   T* w_prev = mr_[3].p; T* w_curr = mr_[4].p; T* w_next = mr_[5].p;
   apply(nullptr, x, mr_c_.p);
-  const double tol_num = st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent);
-  minres_init_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, b, mr_c_.p, v_curr, red(SC_RES2), MinresInitFin<T>{sc_.p, isc_.p, (T)tol_num});
+  minres_init_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, b, mr_c_.p, v_curr, red(SC_RES2), MinresInitFin<T>{sc_.p, isc_.p, (T)inner_tol()});
   check_launch("minres_init");
   minres_start_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, v_curr, v_prev, w_prev, w_curr, sc_.p);
   check_launch("minres_start");
   int it_host = 0;
-  int chunk = std::max(last_cg_iters_, 0);
-  for (;;) {
-    for (int i = 0; i < chunk; ++i) {
+  // + init residual + the reference's explicit L*x0 - b (kktsolver_indirect.jl:72,151)
+  total_mults_ += 2 + poll_inner([&](int k) {
+    for (int i = 0; i < k; ++i) {
       ++it_host;
       apply(done, v_curr, mr_c_.p);
       minres_lanczos1_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, mr_c_.p, v_prev, v_curr, v_next, sc_.p, isc_.p, red(SC_H3));
@@ -1747,15 +1759,7 @@ void Engine<T>::kkt_minres(bool full) {
       T* t = v_prev; v_prev = v_curr; v_curr = v_next; v_next = t;
       t = w_prev; w_prev = w_curr; w_curr = w_next; w_next = t;
     }
-    CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-    sync();
-    if (h_isc_[ISC_DONE]) break;
-    chunk = 1;
-  }
-  const int iters = h_isc_[ISC_IT];
-  last_cg_iters_ = iters;
-  total_inner_ += iters;
-  total_mults_ += 2 + iters;   // + init residual + the reference's explicit L*x0 - b (kktsolver_indirect.jl:72,151)
+  });
   if (full) {
     CUDA_TRY(cudaMemcpyAsync(xsol_.p, mr_x_.p, n_ * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
     CUDA_TRY(cudaMemcpyAsync(nu_.p, mr_x_.p + npad, m_ * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
@@ -1844,37 +1848,12 @@ bool Engine<T>::primal_infeasible() {
   check_launch("dot_dy_b");
   cone_rows_certificate_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, 0, dy_.p, row_class_.p, box_l_.p, box_u_.p, eps, red(SC_TMP1));
   check_launch("cone_cert_primal");
-  // SOC: -v in K*  <=>  |v[2:]| <= tol - v[1]  ;  PSD: -V + tol I positive definite
-  if (n_soc_) {
-    soc_norms(dy_.p, soc_norm2_.p);
-    soc_cert_kernel<T><<<1, kBlock, 0, stream_>>>(n_soc_, soc_off_.p, soc_norm2_.p, dy_.p, eps, sc_.p + SC_TMP3);
-    check_launch("soc_cert");
-  } else {
-    CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP3, 0, sizeof(T), stream_));
-  }
-  if (n_c3_) {
-    cone3_cert_kernel<T><<<1, kBlock, 0, stream_>>>(c3_table(), dy_.p, eps, sc_.p + SC_TMP5);
-    check_launch("cone3_cert");
-  } else {
-    CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP5, 0, sizeof(T), stream_));
-  }
-  const bool psd_ok = psd_.certificate(dy_.p, /*negate=*/true, (double)eps, stream_, st_.psd_max_sweeps, launches_);
-  // the PSD verdict is a host bool of THIS rank: put it next to the device flags so that the
-  // max-allreduce makes every rank take the same decision
-  h_sc_[SC_TMP4] = psd_ok ? T(0) : T(1);
-  CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_.p + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
-  if (nranks_ > 1) {
-    allreduce_sum(sc_.p + SC_TMP0, 2);   // dy'b, box support sum
-    allreduce_max(sc_.p + SC_TMP2, 4);   // flags: rows, SOC, PSD, Exp/Pow
-  }
-  read_scalars(SC_TMP0, 6);
+  allreduce_sum(sc_.p + SC_TMP0, 2);   // dy'b, box support sum
+  const bool cone_bad = cone_certificates(dy_.p, eps) != 0;
   const double dyt_b = (double)h_sc_[SC_TMP0];
   const double box_sum = (double)h_sc_[SC_TMP1];
-  const bool cone_bad = (h_sc_[SC_TMP2] != 0) || (h_sc_[SC_TMP3] != 0) || (h_sc_[SC_TMP4] != 0) || (h_sc_[SC_TMP5] != 0);
   rec[4] = dyt_b;
   rec[5] = box_sum;
-  rec[6] = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) + (h_sc_[SC_TMP5] != 0 ? 8 : 0);
-  rec[7] = psd_.cert_unconverged;
   const double sF = (cone_bad ? INFINITY : 0.0) + box_sum - dyt_b;
   rec[0] = sF <= st_.eps_prim_inf ? 1.0 : 0.0;
   return sF <= st_.eps_prim_inf;
@@ -1915,32 +1894,46 @@ bool Engine<T>::dual_infeasible() {
   check_launch("scal_Adx");
   cone_rows_certificate_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, 1, vec_m_.p, row_class_.p, box_l_.p, box_u_.p, eps, red(SC_TMP1));
   check_launch("cone_cert_dual");
+  const bool cone_ok = cone_certificates(vec_m_.p, eps) == 0;
+  rec[0] = cone_ok ? 1.0 : 0.0;
+  return cone_ok;
+}
+
+// The cone tests of both certificates on v, after the row kernel has set the rows flag in SC_TMP2:
+// SOC (-v in K*  <=>  |v[2:]| <= tol - v[1]) into SC_TMP3, PSD (-V + tol I positive definite) into SC_TMP4, Exp/Pow
+// into SC_TMP5.  Reads SC_TMP0..5 back, records the failed families (rows 1, SOC 2, PSD 4, Exp/Pow 8) and the PSD
+// cones whose eigensolver missed psd_max_sweeps in inf_rec_[6..7], and returns the failed families.
+template <typename T>
+int Engine<T>::cone_certificates(const T* v, T eps) {
   if (n_soc_) {
-    soc_norms(vec_m_.p, soc_norm2_.p);
-    soc_cert_kernel<T><<<1, kBlock, 0, stream_>>>(n_soc_, soc_off_.p, soc_norm2_.p, vec_m_.p, eps, sc_.p + SC_TMP3);
+    soc_norms(v, soc_norm2_.p);
+    soc_cert_kernel<T><<<1, kBlock, 0, stream_>>>(n_soc_, soc_off_.p, soc_norm2_.p, v, eps, sc_.p + SC_TMP3);
     check_launch("soc_cert");
   } else {
     CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP3, 0, sizeof(T), stream_));
   }
   if (n_c3_) {
-    cone3_cert_kernel<T><<<1, kBlock, 0, stream_>>>(c3_table(), vec_m_.p, eps, sc_.p + SC_TMP5);
+    cone3_cert_kernel<T><<<1, kBlock, 0, stream_>>>(c3_table(), v, eps, sc_.p + SC_TMP5);
     check_launch("cone3_cert");
   } else {
     CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP5, 0, sizeof(T), stream_));
   }
-  const bool psd_ok = psd_.certificate(vec_m_.p, /*negate=*/true, (double)eps, stream_, st_.psd_max_sweeps, launches_);
+  const bool psd_ok = psd_.certificate(v, /*negate=*/true, (double)eps, stream_, st_.psd_max_sweeps, launches_);
+  // the PSD verdict is a host bool of THIS rank: put it next to the device flags so that the
+  // max-allreduce makes every rank take the same decision
   h_sc_[SC_TMP4] = psd_ok ? T(0) : T(1);
   CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_.p + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
-  if (nranks_ > 1) allreduce_max(sc_.p + SC_TMP2, 4);
-  read_scalars(SC_TMP2, 4);
-  rec[6] = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) + (h_sc_[SC_TMP5] != 0 ? 8 : 0);
-  rec[7] = psd_.cert_unconverged;
-  rec[0] = rec[6] == 0 ? 1.0 : 0.0;
-  return (h_sc_[SC_TMP2] == 0) && (h_sc_[SC_TMP3] == 0) && (h_sc_[SC_TMP4] == 0) && (h_sc_[SC_TMP5] == 0);
+  allreduce_max(sc_.p + SC_TMP2, 4);   // flags: rows, SOC, PSD, Exp/Pow
+  read_scalars(SC_TMP0, 6);
+  const int failed = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) +
+                     (h_sc_[SC_TMP5] != 0 ? 8 : 0);
+  inf_rec_[6] = failed;
+  inf_rec_[7] = psd_.cert_unconverged;
+  return failed;
 }
 
 // ---------------------------------------------------------------------------
-// Accelerator: AndersonAccelerator{T, Type2{QRDecomp}, RestartedMemory, NoRegularizer} (aa.cuh)
+// Accelerator: AndersonAccelerator{T, Type2{QRDecomp} | Type2{NormalEquations} | Type1, ...} (aa.cuh)
 // ---------------------------------------------------------------------------
 template <typename T>
 void Engine<T>::aa_prepare() {   // _make_accelerator!, setup.jl:10-14 (built once per dimension / memory)
@@ -1956,7 +1949,7 @@ void Engine<T>::aa_prepare() {   // _make_accelerator!, setup.jl:10-14 (built on
     if (!h_aa_.p) h_aa_.alloc(AA_SC_COUNT);
     aa_mem_ = mem;
   }
-  if (aa_ne()) {
+  if (!aa_qr()) {
     if (aa_gsc_.n == 0) {
       aa_gsc_.alloc((size_t)AA_GRAM_MAX_CHUNKS * AA_GRAM_NR);
       aa_gpart_.alloc((size_t)kMaxGrid * AA_GRAM_NR);
@@ -1973,119 +1966,82 @@ void Engine<T>::aa_prepare() {   // _make_accelerator!, setup.jl:10-14 (built on
   aa_rejected_ = aa_rho_restarts_ = aa_mem_restarts_ = aa_activated_at_ = 0;
 }
 
-// CA.update!(aa, g = w, x = w_prev): history columns + QR update by modified Gram-Schmidt
+// CA.update!(aa, g = w, x = w_prev): f = x - g; the first call after a restart only stores (g, f) (and x for Type1);
+// otherwise the history columns G_j, F_j (and X_j for Type1, aa.cuh), then for Type2{QRDecomp} the QR update of F by
+// modified Gram-Schmidt.  M of the normal-equation variants follows in aa_accelerate.
 template <typename T>
 void Engine<T>::aa_update(const T* g, const T* x) {
   const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
   const int grid = vgrid(dim);
-  if (aa_init_) {
-    aa_update_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, (T*)nullptr, (T*)nullptr, 1,
-                                                      red_ptr(aa_sc_.p + AA_F2));
-    check_launch("aa_update");
-    allreduce_sum(aa_sc_.p + AA_F2, 1);
-    aa_init_ = false;
-    return;
-  }
-  int j = aa_iter_ % aa_mem_;
-  if (j == 0 && aa_iter_ != 0) { aa_iter_ = 0; ++aa_mem_restarts_; }   // RestartedMemory: the history is full, start again
-  T* Gj = aaG_.p + (size_t)j * dim;
-  T* q = aaQ_.p + (size_t)j * dim;
-  aa_update_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, Gj, q, 0,
-                                                    red_ptr(aa_sc_.p + AA_F2));
-  check_launch("aa_update");
-  allreduce_sum(aa_sc_.p + AA_F2, 1);
-  T* Rj = aaR_.p + (size_t)j * aa_mem_;        // column j of R
-  for (int i = 0; i <= j; ++i) {
-    const T* Qp = i > 0 ? aaQ_.p + (size_t)(i - 1) * dim : nullptr;
-    const T* Qi = i < j ? aaQ_.p + (size_t)i * dim : nullptr;
-    T* out = i < j ? Rj + i : aa_sc_.p + AA_NRM2;
-    aa_mgs_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, q, Qp, i > 0 ? Rj + (i - 1) : nullptr, Qi, red_ptr(out));
-    check_launch("aa_mgs");
-    allreduce_sum(out, 1);
-  }
-  aa_normalize_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, q, aa_sc_.p + AA_NRM2, Rj + j);
-  check_launch("aa_normalize");
-  ++aa_iter_;
-}
-
-// CA.accelerate!(g = w, ...): w -= G eta with R eta = Q'f; returns was_successful(aa)
-template <typename T>
-bool Engine<T>::aa_accelerate(T* g) {
-  const int l = std::min(aa_iter_, aa_mem_);
-  if (l < std::max(st_.accelerator_min_mem, 1)) return false;
-  const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
-  const int grid = vgrid(dim);
-  for (int c0 = 0; c0 < l; c0 += 8) {
-    aa_qtf_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, aa_f_.p, aaQ_.p, (size_t)dim, c0, std::min(8, l - c0),
-                                                   red_ptr(aa_eta_.p + c0));
-    check_launch("aa_qtf");
-  }
-  allreduce_sum(aa_eta_.p, l);
-  aa_solve_kernel<T><<<1, 32, 0, stream_>>>(aaR_.p, aa_mem_, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
-  check_launch("aa_solve");
-  aa_apply_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, g, aaG_.p, (size_t)dim, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
-  check_launch("aa_apply");
-  CUDA_TRY(cudaMemcpyAsync(h_aa_.p + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
-  sync();
-  if (h_aa_[AA_FLAG] == T(0)) { ++aa_rejected_; return false; }
-  return true;
-}
-
-// CA.update! of the normal-equation variants (aa.cuh): history columns only; M follows in aa_accelerate_ne
-template <typename T>
-void Engine<T>::aa_update_ne(const T* g, const T* x) {
-  const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
-  const int grid = vgrid(dim);
   const bool type1 = acc_.type == COSMO_B200_AA_TYPE1;
-  T* xl = type1 ? aa_xlast_.p : nullptr;
-  if (aa_init_) {
-    aa_hist_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, xl, (T*)nullptr,
-                                                    (T*)nullptr, (T*)nullptr, 1, red_ptr(aa_sc_.p + AA_F2));
-    check_launch("aa_hist");
-    allreduce_sum(aa_sc_.p + AA_F2, 1);
-    aa_init_ = false;
-    aa_fresh_ = false;
-    return;
-  }
   const int j = aa_iter_ % aa_mem_;
+  // RestartedMemory: the history is full, start again (the QR variant always restarts: set_accelerator refuses rolling)
   if (acc_.memory == COSMO_B200_AA_RESTARTED_MEMORY && j == 0 && aa_iter_ != 0) { aa_iter_ = 0; ++aa_mem_restarts_; }
-  aa_hist_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, xl,
-                                                  aaG_.p + (size_t)j * dim, aaQ_.p + (size_t)j * dim,
-                                                  type1 ? aaX_.p + (size_t)j * dim : nullptr, 0, red_ptr(aa_sc_.p + AA_F2));
+  T* q = aaQ_.p + (size_t)j * dim;
+  aa_hist_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, g, x, aa_f_.p, aa_flast_.p, aa_glast_.p, type1 ? aa_xlast_.p : nullptr,
+                                                  aaG_.p + (size_t)j * dim, q, type1 ? aaX_.p + (size_t)j * dim : nullptr,
+                                                  aa_init_ ? 1 : 0, red_ptr(aa_sc_.p + AA_F2));
   check_launch("aa_hist");
   allreduce_sum(aa_sc_.p + AA_F2, 1);
+  if (aa_init_) { aa_init_ = false; return; }
+  if (aa_qr()) {
+    T* Rj = aaR_.p + (size_t)j * aa_mem_;        // column j of R
+    for (int i = 0; i <= j; ++i) {
+      const T* Qp = i > 0 ? aaQ_.p + (size_t)(i - 1) * dim : nullptr;
+      const T* Qi = i < j ? aaQ_.p + (size_t)i * dim : nullptr;
+      T* out = i < j ? Rj + i : aa_sc_.p + AA_NRM2;
+      aa_mgs_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, q, Qp, i > 0 ? Rj + (i - 1) : nullptr, Qi, red_ptr(out));
+      check_launch("aa_mgs");
+      allreduce_sum(out, 1);
+    }
+    aa_normalize_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, q, aa_sc_.p + AA_NRM2, Rj + j);
+    check_launch("aa_normalize");
+  }
   aa_j_ = j;
   ++aa_iter_;
   if (aa_iter_ >= 2 * aa_mem_) aa_iter_ -= aa_mem_;   // RollingMemory: keeps iter mod mem and min(iter, mem)
   aa_fresh_ = true;
 }
 
-// CA.accelerate! of the normal-equation variants: one fused Gram + rhs pass (ceil(l/8) launches, one allreduce), the
-// one-warp LU solve, then the candidate through aa_apply_kernel
+// CA.accelerate!(g = w, ...): w -= G eta, returns was_successful(aa).  Type2{QRDecomp} solves R eta = Q'f; the
+// normal-equation variants refresh row and column j of M in one fused Gram + rhs pass (ceil(l/8) launches, one
+// allreduce) and solve with the one-warp LU, which also keeps M current while the window is below min_mem.
 template <typename T>
-bool Engine<T>::aa_accelerate_ne(T* g) {
+bool Engine<T>::aa_accelerate(T* g) {
   if (!aa_fresh_) return false;
   aa_fresh_ = false;
   const int l = std::min(aa_iter_, aa_mem_);
+  const bool solve = l >= std::max(st_.accelerator_min_mem, 1);
   const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
   const int grid = vgrid(dim);
-  const bool type1 = acc_.type == COSMO_B200_AA_TYPE1;
-  const int nch = (l + AA_GRAM_COLS - 1) / AA_GRAM_COLS;
-  for (int ch = 0; ch < nch; ++ch) {
-    const int c0 = ch * AA_GRAM_COLS, nc = std::min((int)AA_GRAM_COLS, l - c0);
-    RedBuf<T> rb{aa_gpart_.p, aa_gsc_.p + (size_t)ch * AA_GRAM_NR, ticket_.p};
-    if (type1)
-      aa_gram_kernel<T, true><<<grid, kBlock, 0, stream_>>>(dim, lo, aaX_.p, aaQ_.p, (size_t)dim, aa_j_, c0, nc, aa_f_.p, rb);
-    else
-      aa_gram_kernel<T, false><<<grid, kBlock, 0, stream_>>>(dim, lo, aaQ_.p, aaQ_.p, (size_t)dim, aa_j_, c0, nc, aa_f_.p, rb);
-    check_launch("aa_gram");
+  if (aa_qr()) {
+    if (!solve) return false;
+    for (int c0 = 0; c0 < l; c0 += 8) {
+      aa_qtf_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, lo, aa_f_.p, aaQ_.p, (size_t)dim, c0, std::min(8, l - c0),
+                                                     red_ptr(aa_eta_.p + c0));
+      check_launch("aa_qtf");
+    }
+    allreduce_sum(aa_eta_.p, l);
+    aa_solve_kernel<T><<<1, 32, 0, stream_>>>(aaR_.p, aa_mem_, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
+    check_launch("aa_solve");
+  } else {
+    const bool type1 = acc_.type == COSMO_B200_AA_TYPE1;
+    const int nch = (l + AA_GRAM_COLS - 1) / AA_GRAM_COLS;
+    for (int ch = 0; ch < nch; ++ch) {
+      const int c0 = ch * AA_GRAM_COLS, nc = std::min((int)AA_GRAM_COLS, l - c0);
+      RedBuf<T> rb{aa_gpart_.p, aa_gsc_.p + (size_t)ch * AA_GRAM_NR, ticket_.p};
+      if (type1)
+        aa_gram_kernel<T, true><<<grid, kBlock, 0, stream_>>>(dim, lo, aaX_.p, aaQ_.p, (size_t)dim, aa_j_, c0, nc, aa_f_.p, rb);
+      else
+        aa_gram_kernel<T, false><<<grid, kBlock, 0, stream_>>>(dim, lo, aaQ_.p, aaQ_.p, (size_t)dim, aa_j_, c0, nc, aa_f_.p, rb);
+      check_launch("aa_gram");
+    }
+    allreduce_sum(aa_gsc_.p, (size_t)nch * AA_GRAM_NR);
+    aa_ne_solve_kernel<T><<<1, 32, 0, stream_>>>(aa_gsc_.p, aaR_.p, aa_nrm_.p, aa_nrm_.p + aa_mem_, aa_mem_, aa_j_, l, type1 ? 1 : 0,
+                                                 acc_.regularizer, (T)acc_.lambda, solve ? 1 : 0, aa_eta_.p, aa_sc_.p + AA_FLAG);
+    check_launch("aa_ne_solve");
+    if (!solve) return false;
   }
-  allreduce_sum(aa_gsc_.p, (size_t)nch * AA_GRAM_NR);
-  const bool solve = l >= std::max(st_.accelerator_min_mem, 1);
-  aa_ne_solve_kernel<T><<<1, 32, 0, stream_>>>(aa_gsc_.p, aaR_.p, aa_nrm_.p, aa_nrm_.p + aa_mem_, aa_mem_, aa_j_, l, type1 ? 1 : 0,
-                                               acc_.regularizer, (T)acc_.lambda, solve ? 1 : 0, aa_eta_.p, aa_sc_.p + AA_FLAG);
-  check_launch("aa_ne_solve");
-  if (!solve) return false;
   aa_apply_kernel<T><<<grid, kBlock, 0, stream_>>>(dim, g, aaG_.p, (size_t)dim, l, aa_eta_.p, aa_sc_.p + AA_FLAG);
   check_launch("aa_apply");
   CUDA_TRY(cudaMemcpyAsync(h_aa_.p + AA_FLAG, aa_sc_.p + AA_FLAG, sizeof(T), cudaMemcpyDeviceToHost, stream_));
@@ -2165,12 +2121,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
       project_device(w, true, ws_rhs);      // admm_z! fused with the right-hand side of admm_x! (one pass over w)
       t_proj_.end(stream_);
     } else {
-      ProjRhsArgs<T> a;
-      a.n = n; a.m = m; a.w = w; a.ws_rhs = ws_rhs; a.q = q_.p; a.b = b_.p; a.rho = rho_vec_.p;
-      a.box_l = box_l_.p; a.box_u = box_u_.p; a.row_class = row_class_.p; a.row_cone = row_cone_.p;
-      a.soc = SocTable<T>{soc_off_.p, soc_norm_.p};
-      a.s = s_.p; a.ls = ls_.p; a.t0 = t0_.p; a.sigma = (T)st_.sigma; a.do_proj = 0; a.do_rhs = 1;
-      launch_proj_rhs(a);
+      launch_proj_rhs(w, ws_rhs, false, true);
     }
     // the tail reads w_s from ws_rhs's buffer and writes W[dst] (elementwise, may alias)
     T* wd = W_[dst].p;
@@ -2202,13 +2153,8 @@ void Engine<T>::solve(cosmo_b200_result* out) {
         aa_activated_at_ = iter;
       }
       if (aa_active_) {
-        if (aa_ne()) {
-          aa_update_ne(W_[cur_].p, W_[prev_].p);
-          aa_success_ = aa_accelerate_ne(W_[cur_].p);
-        } else {
-          aa_update(W_[cur_].p, W_[prev_].p);
-          aa_success_ = aa_accelerate(W_[cur_].p);   // overwrites w with the candidate
-        }
+        aa_update(W_[cur_].p, W_[prev_].p);
+        aa_success_ = aa_accelerate(W_[cur_].p);   // overwrites w with the candidate
         if (aa_success_) ++aa_accelerated_;
       }
     }

@@ -10,7 +10,7 @@
 //     decomposition): ONE CTA PER CONE, matrix and eigenvectors resident in
 //     shared memory, every cone of the batch in one launch.
 //   * large cones: matrix/eigenvectors in HBM (L2-resident for N <= ~2800),
-//     one (params, columns, rows) kernel triple per Jacobi round.
+//     block Jacobi, one (pivot, columns, rows) kernel triple per round.
 // The projection keeps eigenpairs with lambda > 0 strictly (convexset.jl:250)
 // and rebuilds X+ = sum lambda_k v_k v_k' ; a cone of dim 1 is max(x, 0)
 // (convexset.jl:307-308, 404-405).
@@ -435,74 +435,6 @@ __global__ void __launch_bounds__(kBlock) psd_unscale_kernel(T* __restrict__ s, 
     s[k] = (T)((double)s[k] * f);
 }
 
-template <typename T>
-__global__ void psd_large_params_kernel(int N, int r, const T* __restrict__ A, const T* __restrict__ thr, T* __restrict__ cs,
-                                        int* __restrict__ rotated) {
-  const int Ne = (N + 1) & ~1;
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= Ne / 2) return;
-  int p, q;
-  rr_pair(Ne, r, k, p, q);
-  T c = T(1), sn = T(0);
-  if (q < N) {
-    const T apq = A[p + (long long)q * N];
-    if (tabs(apq) > *thr) {
-      sym_schur(A[p + (long long)p * N], A[q + (long long)q * N], apq, c, sn);
-      *rotated = 1;
-    }
-  }
-  cs[2 * k] = c;
-  cs[2 * k + 1] = sn;
-}
-
-// columns p,q of A and V (coalesced along i)
-template <typename T>
-__global__ void __launch_bounds__(kBlock) psd_large_cols_kernel(int N, int r, T* __restrict__ A, T* __restrict__ V,
-                                                                const T* __restrict__ cs) {
-  const int Ne = (N + 1) & ~1;
-  const int k = blockIdx.y;
-  const T sn = cs[2 * k + 1];
-  if (sn == T(0)) return;
-  const T c = cs[2 * k];
-  int p, q;
-  rr_pair(Ne, r, k, p, q);
-  T* Ap = A + (long long)p * N; T* Aq = A + (long long)q * N;
-  T* Vp = V + (long long)p * N; T* Vq = V + (long long)q * N;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
-    const T aip = Ap[i], aiq = Aq[i];
-    Ap[i] = c * aip - sn * aiq;
-    Aq[i] = sn * aip + c * aiq;
-    const T vip = Vp[i], viq = Vq[i];
-    Vp[i] = c * vip - sn * viq;
-    Vq[i] = sn * vip + c * viq;
-  }
-}
-
-// rows p,q of A: thread j handles column j for every pair (strided reads of 2 elements per pair)
-template <typename T>
-__global__ void __launch_bounds__(kBlock) psd_large_rows_kernel(int N, int r, T* __restrict__ A, const T* __restrict__ cs) {
-  const int Ne = (N + 1) & ~1;
-  const int npairs = Ne / 2;
-  extern __shared__ unsigned char smem_raw[];
-  T* scs = reinterpret_cast<T*>(smem_raw);
-  for (int k = threadIdx.x; k < 2 * npairs; k += blockDim.x) scs[k] = cs[k];
-  __syncthreads();
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= N) return;
-  T* col = A + (long long)j * N;
-  for (int k = 0; k < npairs; ++k) {
-    const T sn = scs[2 * k + 1];
-    if (sn == T(0)) continue;
-    const T c = scs[2 * k];
-    int p, q;
-    rr_pair(Ne, r, k, p, q);
-    const T apj = col[p], aqj = col[q];
-    col[p] = c * apj - sn * aqj;
-    col[q] = sn * apj + c * aqj;
-  }
-}
-
-
 // ---------------------------------------------------------------------------
 // Large cones, block Jacobi (two-sided, block size 32): per round the Nb/2 disjoint block
 // pairs (I,J) of the round-robin ordering are handled in three launches
@@ -874,7 +806,7 @@ struct PsdBatch {
   int small_maxN = 0;
   // large-cone workspace (sized for the largest cone, cones processed one after another)
   int large_maxN = 0;
-  DevBuf<T> A_d, V_d, cs_d, fro_d, thr_d, lam_large_d;
+  DevBuf<T> A_d, V_d, fro_d, thr_d, lam_large_d;
   DevBuf<int> rot_d;
   PinnedBuf<int> rot_h;
   DevBuf<unsigned long long> mx_d;   // max |entry| of the cone being projected (psd_cone_max_kernel)
@@ -918,7 +850,7 @@ struct PsdBatch {
     if (!large_h.empty()) {
       for (const auto& d : large_h) large_maxN = std::max(large_maxN, d.N);
       const size_t nn = (size_t)large_maxN * large_maxN;
-      A_d.alloc(nn, false); V_d.alloc(nn, false); cs_d.alloc(large_maxN + 2, false); fro_d.alloc(kMaxGrid, false);
+      A_d.alloc(nn, false); V_d.alloc(nn, false); fro_d.alloc(kMaxGrid, false);
       thr_d.alloc(1, false); lam_large_d.alloc(large_h.size(), false); rot_d.alloc(1, false); rot_h.alloc(1);
       mx_d.alloc(1, false); up_d.alloc(1, false);
       if (large_h.size() == 1) { Vw_d.alloc(nn, false); T_d.alloc(nn, false); }

@@ -1,5 +1,5 @@
 """gloo world-2 emulation of the sharded Gram + right-hand-side pass of the normal-equation Anderson variants
-(csrc/aa.cuh aa_gram_kernel / aa_ne_solve_kernel, Engine::aa_accelerate_ne): every rank keeps [w_x (replicated); w_s on
+(csrc/aa.cuh aa_gram_kernel / aa_ne_solve_kernel, Engine::aa_accelerate): every rank keeps [w_x (replicated); w_s on
 its rows], sums its 26 scalars per chunk of 8 columns over [lo, dim) (lo = 0 on rank 0, n elsewhere), and one
 allreduce of all chunks gives every rank the same M, rhs, eta and candidate as the unsharded restatement."""
 import os
