@@ -122,7 +122,7 @@ struct DevCsr {
   DevBuf<unsigned char> w_colhi;
   DevBuf<double> w_esc;
   long long w_elems = 0, w_nesc = 0;
-  bool packable = false;          // the 9 B layout may hold this slab (fp64, no device equilibration, 15-bit columns)
+  bool packable = false;          // the 9 B layout may hold this slab (fp64, 15-bit columns)
   // where every stored value comes from (cosmo_b200_update_matrices): CSR position -> CSC index (none when the CSR is
   // the CSC order itself, as for A'), slab column position -> CSC index of the matrix or -1 for padding.  Device copies
   // made by the first update (upload_value_maps); h_src holds the CSR(P) map from create until then.
@@ -227,7 +227,7 @@ class Engine : public EngineBase {
   // ---- problem ----
   int n_ = 0, m_ = 0, device_ = 0;
   double create_time_ = 0.0;      // engine construction (the device part of setup!)
-  bool device_scaled_ = false;    // D, E, c were computed here (equilibrate), not handed over by the host
+  bool device_scaled_ = false;    // D, E, c are computed here (equilibrate), not handed over by the host
   int auto_rho_interval_ = 0;     // adaptive_rho_interval chosen by the automatic rule (kept across solves like settings)
   cosmo_b200_settings st_;
   bool scaled_ = false;
@@ -387,7 +387,8 @@ class Engine : public EngineBase {
   void upload_vec(DevBuf<T>& dst, const void* host, size_t count);
   void download_vec(void* host, const T* src, size_t count);
   void build_csr(DevCsr<T>& dst, const HostCsr& h);
-  void build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src, bool allow_packed);
+  void build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src);
+  void write_values(const void* Px, const void* Ax, const void* q, const void* b);
   void gather_csr(DevCsr<T>& M, const T* v);
   void load_P(const void* Px);
   int exponent_window();
@@ -590,7 +591,7 @@ static void report_windows(const DevCsr<T>& d) {
 }
 
 template <typename T>
-void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src, bool allow_packed) {
+void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src) {
   dst.windowed = false;
   dst.packed = false;
   if (h.nrows == 0 || h.ncols == 0) return;
@@ -655,9 +656,9 @@ void Engine<T>::build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src, 
   dst.w_col.upload(wc, stream_);
   dst.d_wsrc.upload(wsrc, stream_);
   sync();
-  // fp64: the 9 B layout unless the values need too many escapes, or device equilibration will rewrite the slab values
-  // in place (ruiz_apply_win_kernel works on the 10 B layout)
-  dst.packable = sizeof(T) == sizeof(double) && allow_packed && W - 1 <= (int)winpack::kMaxCol;
+  // fp64: the 9 B layout when the window-local columns fit its column bits, unless the values need too many escapes
+  // (update_slab)
+  dst.packable = sizeof(T) == sizeof(double) && W - 1 <= (int)winpack::kMaxCol;
   dst.windowed = true;
 }
 
@@ -850,45 +851,30 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   if (off != m_) throw EngineError{COSMO_B200_ERR_INVALID, "sum of set dimensions != m"};
 
   // ---- matrices -----------------------------------------------------------
+  const bool dbg = getenv("COSMO_B200_SETUP_DEBUG") != nullptr;
+  double tp = now_s();
+  auto lap = [&](const char* what) {
+    if (dbg) { const double t = now_s(); fprintf(stderr, "[setup] %-22s %.3f s\n", what, t - tp); tp = t; }
+  };
+  lap("cone tables");
   {
-    const bool dbg = getenv("COSMO_B200_SETUP_DEBUG") != nullptr;
-    double tp = now_s();
-    auto lap = [&](const char* what) {
-      if (dbg) { const double t = now_s(); fprintf(stderr, "[setup] %-22s %.3f s\n", what, t - tp); tp = t; }
-    };
-    lap("cone tables");
-    // device equilibration rewrites the slab values in place, which only the 10 B slab layout allows
-    const bool pack_ok = !((p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0);
-    // The host lays out the patterns; the values are written on the device the way update_matrices writes them, through
-    // value maps that are released as soon as they have been used (an engine that never updates does not keep them).
+    // The host lays out the patterns and the value maps; write_values fills every copy on the device below, the way
+    // update_matrices does, and the maps are released after it (an engine that never updates does not keep them).
     HostCsr a, at, pp, ppt;
     csc_to_host_csrs(p.A, p.index_base, a, at);
     lap("csc -> csr (A, A')");
     build_csr(A_, a);
     build_csr(At_, at);
-    upload_vec(At_.val, p.A.nzval, (size_t)At_.nnz);   // CSR(A') is the CSC order of A
     A_.d_src.upload(a.src, stream_);
-    gather_csr(A_, At_.val.p);
-    A_.d_src.release();
-    lap("upload csr A, A'");
-    int ebase = 0;   // one exponent window for the packed slabs of A and A', computed when the first one needs it
-    auto fill_slab = [&](DevCsr<T>& M) {
-      if (M.packable && ebase == 0) ebase = exponent_window();
-      update_slab(M, ebase);
-      M.d_wsrc.release();
-    };
-    build_windows(A_, a, a.src.data(), pack_ok);
-    fill_slab(A_);
+    lap("csr A, A'");
+    build_windows(A_, a, a.src.data());
     lap("windows A");
-    build_windows(At_, at, nullptr, pack_ok);
-    fill_slab(At_);
+    build_windows(At_, at, nullptr);
     lap("windows A'");
     // P's CSC order is not resident: its CSR -> CSC map stays on the host for update_matrices (A's is derived from A')
     csc_to_host_csrs(p.P, p.index_base, pp, ppt);
     build_csr(P_, pp);
     P_.d_src.upload(pp.src, stream_);
-    load_P(p.P.nzval);
-    P_.d_src.release();
     P_.h_src.swap(pp.src);
     lap("P");
     // A' and P rows are traversed by the same lane group in the fused operator kernel
@@ -897,13 +883,19 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   }
   // ---- vectors ------------------------------------------------------------
   auto up = [&](DevBuf<T>& d, const void* h, size_t cnt) { d.alloc(cnt); if (h) upload_vec(d, h, cnt); };
-  up(q_, p.q, n_);
-  up(b_, p.b, m_);
+  q_.alloc(n_);
+  b_.alloc(m_);
   hb_.resize(m_);
-  for (int i = 0; i < m_; ++i) hb_[i] = (double)static_cast<const T*>(p.b)[i];
   scaled_ = (p.D && p.Dinv && p.E && p.Einv);
   c_ = p.c;
   if (scaled_) { up(D_, p.D, n_); up(Dinv_, p.Dinv, n_); up(E_, p.E, m_); up(Einv_, p.Einv, m_); }
+  // scaling requested but no scaling matrices handed over: the data are unscaled, equilibrate them here
+  // (setup.jl:27-33 -> scale_ruiz!); the host reads D, E, c back with cosmo_b200_get_scaling
+  device_scaled_ = (p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0;
+  if (device_scaled_) {
+    if (scaled_) throw EngineError{COSMO_B200_ERR_INVALID, "COSMO_B200_PROBLEM_EQUILIBRATE expects D = Dinv = E = Einv = NULL"};
+    hl0_ = hl_; hu0_ = hu_;
+  }
   row_class_.alloc(m_); row_cone_.alloc(m_); rho_class_.alloc(m_);
   if (m_) {
     CUDA_TRY(cudaMemcpyAsync(row_class_.p, row_class.data(), m_, cudaMemcpyHostToDevice, stream_));
@@ -939,6 +931,9 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
     c3_maxit_.upload(c3_maxit, stream_); c3_tol_.upload(c3_tol, stream_);
     sync();
   }
+  write_values(p.P.nzval, p.A.nzval, p.q, p.b);
+  A_.d_src.release(); P_.d_src.release(); A_.d_wsrc.release(); At_.d_wsrc.release();
+  lap("values");
 
   // ---- state / scratch ------------------------------------------------------
   W_[0].alloc(n_ + m_); W_[1].alloc(n_ + m_);
@@ -958,13 +953,6 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   }
   memset(&xv_, 0, sizeof(xv_));
   rho_ = st_.rho;
-  // scaling requested but no scaling matrices handed over: the data are unscaled, equilibrate them here
-  // (setup.jl:27-33 -> scale_ruiz!); the host reads D, E, c back with cosmo_b200_get_scaling
-  if ((p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0) {
-    if (scaled_) throw EngineError{COSMO_B200_ERR_INVALID, "COSMO_B200_PROBLEM_EQUILIBRATE expects D = Dinv = E = Einv = NULL"};
-    hl0_ = hl_; hu0_ = hu_;
-    equilibrate();
-  }
   classify_and_set_rho(true);
   sync();
   // QdldlKKTSolver's constructor factors K (kktsolver.jl:293-306): a non-convex P or a singular K fails the create
@@ -1064,15 +1052,11 @@ void Engine<T>::equilibrate() {
       sync();
     }
   }
-  // apply D, E, c to every copy of the data
-  if (A_.packed || At_.packed) throw EngineError{COSMO_B200_ERR_INVALID, "device equilibration of a packed (9 B) slab"};
+  // apply D, E, c to the CSR copies (A and A' both scale an entry by the product D_j E_i, so they stay equal bit for
+  // bit), q, b and the Box bounds; write_values fills the slabs from the scaled A' afterwards
   ruiz_apply_csr_kernel<T><<<wgrid(m), kBlock, 0, stream_>>>(m, A_.rowptr.p, A_.col.p, A_.val.p, E_.p, D_.p, (const T*)nullptr);
   ruiz_apply_csr_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, At_.val.p, D_.p, E_.p, (const T*)nullptr);
   ruiz_apply_csr_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.val.p, D_.p, D_.p, cdev.p);
-  if (A_.windowed)
-    ruiz_apply_win_kernel<T><<<wgrid((long long)A_.nwin * m), kBlock, 0, stream_>>>(A_.nwin, A_.W, m, n, A_.w_rowptr.p, A_.w_col.p, A_.w_val.p, E_.p, D_.p);
-  if (At_.windowed)
-    ruiz_apply_win_kernel<T><<<wgrid((long long)At_.nwin * n), kBlock, 0, stream_>>>(At_.nwin, At_.W, n, m, At_.w_rowptr.p, At_.w_col.p, At_.w_val.p, D_.p, E_.p);
   ruiz_finish_n_kernel<T><<<vgrid(n), kBlock, 0, stream_>>>(n, q_.p, D_.p, Dinv_.p, cdev.p);
   ruiz_finish_m_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, b_.p, E_.p, Einv_.p, row_class_.p, box_l_.p, box_u_.p);
   check_launch("ruiz");
@@ -1091,7 +1075,6 @@ void Engine<T>::equilibrate() {
     c_ = (double)ch;
   }
   scaled_ = true;
-  device_scaled_ = true;
 }
 
 template <typename T>
@@ -1143,12 +1126,22 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
   CUDA_TRY(cudaSetDevice(device_));
   const double t0 = now_s();
   upload_value_maps();
+  write_values(Px, Ax, q, b);
+  destroy_cg_graphs();   // the slab and escape-table pointers they captured may have changed
+  reset();
+  auto_rho_interval_ = 0;
+  if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_factor();   // reset() marked the factor dirty; a non-convex P fails here
+  create_time_ = now_s() - t0;
+}
+
+// The values of P, A, q and b (null: keep the current ones), through the value maps of mat_update.cuh, for create and
+// update_matrices alike.  An equilibrating engine scales the CSR copies, q, b and its unscaled Box bounds first; the
+// slabs come last, gathered from the final A' values, so every resident copy of A holds the same numbers.
+template <typename T>
+void Engine<T>::write_values(const void* Px, const void* Ax, const void* q, const void* b) {
   if (Ax) {
     upload_vec(At_.val, Ax, (size_t)At_.nnz);   // CSR(A') is the CSC order of A
     gather_csr(A_, At_.val.p);
-    const int ebase = A_.packable || At_.packable ? exponent_window() : 0;   // one exponent window for A and A'
-    update_slab(A_, ebase);
-    update_slab(At_, ebase);
   }
   if (Px) load_P(Px);
   if (q) upload_vec(q_, q, n_);
@@ -1162,12 +1155,12 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
     upload_vec(box_u_, u.data(), m_);
     equilibrate();
   }
+  if (Ax) {
+    const int ebase = A_.packable || At_.packable ? exponent_window() : 0;   // one exponent window for A and A'
+    update_slab(A_, ebase);
+    update_slab(At_, ebase);
+  }
   sync();
-  destroy_cg_graphs();   // the slab and escape-table pointers they captured may have changed
-  reset();
-  auto_rho_interval_ = 0;
-  if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_factor();   // reset() marked the factor dirty; a non-convex P fails here
-  create_time_ = now_s() - t0;
 }
 
 // CSR values through the CSR -> CSC map M.d_src: M.val[k] = v[src[k]]

@@ -5,9 +5,10 @@
 //     P_k = c D P0 D,   A_k = E A0 D,   q_k = c D q0,   b_k = E b0,
 // so the column / row infinity norms the loop needs are weighted row maxima of the RESIDENT CSR copies
 // (kkt_col_norms!, scaling.jl:3-8: columns of P and A = rows of P (symmetric) and of the stored A'; rows of A),
-// and the final D, E, c are applied once to every copy of the data (plain CSR of A, A', P, the column-windowed slabs,
-// q, b, Box bounds).  No scalar ever visits the host inside the loop.
-// Included from engine.cu (after spmv.cuh: CsrView, WcsrView).
+// and the final D, E, c are applied once to the CSR copies of A, A', P and to q, b, Box bounds; the column-windowed
+// slabs are filled from the scaled A' afterwards (write_values in engine.cu).  No scalar ever visits the host inside
+// the loop.
+// Included from engine.cu (after spmv.cuh: CsrView).
 #pragma once
 
 namespace cosmo {
@@ -114,37 +115,6 @@ __global__ void __launch_bounds__(kBlock) ruiz_apply_csr_kernel(int nrows, const
     const int s = rowptr[r], e = rowptr[r + 1];
     const T wr = sc * wrow[r];
     for (int k = s + lane; k < e; k += 32) val[k] *= wr * wcol[col[k]];
-  }
-}
-
-// the column-windowed slabs (build_windows / win_fill_segment in engine.cu): a row segment [s, e) of window w is a
-// sequence of 256-entry steps; in step st lane l / slot i keeps its window-local COLUMN at s + 256 st + 8 l + i and
-// its VALUE at s + 256 st + (i / EPL) (EPL ls) + l EPL + i % EPL  (EPL = 16 / sizeof(T) entries per 16-byte load,
-// ls = lanes of the step).  Global column = w W + local column; padding entries are zeros.
-template <typename T>
-__global__ void __launch_bounds__(kBlock) ruiz_apply_win_kernel(int nwin, int W, int nrows, int ncols, const int* __restrict__ w_rowptr,
-                                                                const unsigned short* __restrict__ w_col, T* __restrict__ w_val,
-                                                                const T* __restrict__ wrow, const T* __restrict__ wcol) {
-  constexpr int EPL = 16 / (int)sizeof(T);
-  const int lane = threadIdx.x & 31;
-  const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
-  const long long total = (long long)nwin * nrows;
-  for (long long wr = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; wr < total; wr += warps) {
-    const int w = (int)(wr / nrows), r = (int)(wr % nrows);
-    const int* rp = w_rowptr + (size_t)w * (nrows + 1);
-    const int s = rp[r], e = rp[r + 1];
-    const int kpad = e - s, lanes_total = kpad >> 3;
-    const T er = wrow[r];
-    for (int idx = lane; idx < kpad; idx += 32) {
-      const int st = idx >> 8, rem = idx & 255, l = rem >> 3, i = rem & 7;
-      const int ls = min(32, lanes_total - 32 * st);
-      const long long pv = (long long)s + (long long)st * 256 + (long long)(i / EPL) * (EPL * ls) + (long long)l * EPL + (i % EPL);
-      const T v = w_val[pv];
-      if (v != T(0)) {
-        const int c = w * W + (int)w_col[(long long)s + idx];
-        if (c < ncols) w_val[pv] = v * er * wcol[c];
-      }
-    }
   }
 }
 

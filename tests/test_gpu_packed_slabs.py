@@ -2,8 +2,9 @@
 slabs compute.
 
 An fp64 windowed matrix is packed (csrc/win_pack.h) unless more than 1/256 of its stored entries fall outside its best
-14 binades, or the engine equilibrates the data on the device.  The layout is read from the kernel names of a
-profiler trace (`spmv_win_kernel<double, true, ...>` is the packed kernel) and from the COSMO_B200_SETUP_DEBUG report."""
+14 binades; an engine that equilibrates on the device applies that rule to the scaled values.  The layout is read from
+the kernel names of a profiler trace (`spmv_win_kernel<double, true, ...>` is the packed kernel) and from the
+COSMO_B200_SETUP_DEBUG report."""
 import json
 import re
 
@@ -179,23 +180,45 @@ def test_wide_value_range_keeps_the_10_byte_layout(tmp_path, capfd, monkeypatch)
     eng.close()
 
 
-def test_device_equilibration_runs_the_10_byte_layout(tmp_path, capfd, monkeypatch):
-    """scale_ruiz! rewrites the slab values in place: such an engine keeps the 10 B slabs and matches the oracle"""
-    P, q, A, b, sets = cosmo_b200.problems.random_sparse_qp(30000, 4000, 0.002, seed=5)
+def _ruiz_scaled(A, D, E):
+    """E A D of a CSC matrix as the engine forms it: every entry times the product D_j E_i"""
+    S = A.copy()
+    S.data = A.data * (D[np.repeat(np.arange(A.shape[1]), np.diff(A.indptr))] * E[A.indices])
+    return S
+
+
+def test_device_equilibration_fills_the_slabs_with_the_scaled_values(tmp_path, capfd, monkeypatch):
+    """scale_ruiz! scales the CSR copies and the slabs are filled from the scaled A' afterwards: they take the layout
+    the rule picks for the scaled values and hold exactly the numbers of the CSR copies"""
+    P, q, A, b, sets = cosmo_b200.problems.random_sparse_qp(30000, 40000, 0.002, seed=5)   # A and A' windowed
+    A.sort_indices()
     monkeypatch.setenv("COSMO_B200_SETUP_DEBUG", "1")
     capfd.readouterr()
     eng = E.Engine(P, q, A, b, _tuples(sets), cosmo_b200.Settings().to_struct(), equilibrate=True)
     lay = _layouts(capfd)
-    assert lay and all(l[0] == "10 B" for l in lay), lay
     D, Ev, c = eng.scaling()
     Ps, qs, As, bs, cones, sm = O.scale_ruiz(P, q, A, b, to_oracle_cones(sets), O.Settings())
     assert np.max(np.abs(D - sm.D) / sm.D) <= 1e-13
     assert np.max(np.abs(Ev - sm.E) / sm.E) <= 1e-13
+    S = _ruiz_scaled(A, D, Ev)
+    _assert_layout_rule(S, lay)
     rng = np.random.default_rng(1)
-    x = rng.standard_normal(A.shape[1])
-    counts = _kernel_counts(lambda: eng.spmv(0, x), tmp_path)
-    assert _count(counts, PLAIN) > 0 and _count(counts, PACKED) == 0, counts
-    y = rng.standard_normal(A.shape[0])
+    x, y = rng.standard_normal(A.shape[1]), rng.standard_normal(A.shape[0])
+    for which, arg, (layout, *_) in ((0, x, lay[0]), (1, y, lay[1])):
+        want, other = (PACKED, PLAIN) if layout == "9 B" else (PLAIN, PACKED)
+        counts = _kernel_counts(lambda: eng.spmv(which, arg), tmp_path)
+        assert _count(counts, want) > 0 and _count(counts, other) == 0, (which, counts)
+    # A e_j and A' e_i are a column and a row of the slabs, on both sides of a window edge: bit for bit those of E A D
+    Sr = S.tocsr()
+    (*_, WA), (*_, WAt) = lay
+    for j in (0, WA - 1, WA, A.shape[1] - 1):
+        e = np.zeros(A.shape[1])
+        e[j] = 1.0
+        assert np.array_equal(eng.spmv(0, e), S[:, j].toarray().ravel()), j
+    for i in (0, WAt - 1, WAt, A.shape[0] - 1):
+        e = np.zeros(A.shape[0])
+        e[i] = 1.0
+        assert np.array_equal(eng.spmv(1, e), Sr[i, :].toarray().ravel()), i
     for which, got_in, ref in ((0, x, As @ x), (1, y, As.T @ y), (2, x, Ps @ x)):
         got = eng.spmv(which, got_in)
         assert np.max(np.abs(got - ref)) <= 1e-12 * max(1.0, np.max(np.abs(ref))), which

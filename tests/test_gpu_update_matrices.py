@@ -12,7 +12,7 @@ import scipy.sparse as sp
 import cosmo_b200
 from cosmo_b200 import engine as E
 from tests.gpu_helpers import _tuples
-from tests.test_gpu_packed_slabs import PACKED, PLAIN, _count, _kernel_counts, _layouts
+from tests.test_gpu_packed_slabs import PACKED, PLAIN, _assert_layout_rule, _count, _kernel_counts, _layouts, _ruiz_scaled
 
 pytestmark = pytest.mark.gpu
 
@@ -171,7 +171,7 @@ def test_windowed_fp32_update_is_bit_identical(capfd, monkeypatch):
     e2.close()
 
 
-def test_device_equilibration_update_is_bit_identical(capfd, monkeypatch):
+def test_device_equilibration_update_is_bit_identical_on_scaled_slabs(capfd, monkeypatch):
     monkeypatch.setenv("COSMO_B200_SETUP_DEBUG", "1")
     D1 = _problem(30000, 40000, 0.002, seed=9)
     P, q, A, b, sets = D1
@@ -179,7 +179,9 @@ def test_device_equilibration_update_is_bit_identical(capfd, monkeypatch):
     rng = np.random.default_rng(11)
     q2, b2 = rng.standard_normal(len(q)), b + rng.uniform(0.0, 0.5, len(b))
     e1, o1, e2, o2, lay1, lay2 = _pair(D1, (P2, q2, A2, b2, sets), _settings(scaling=10), equilibrate=True, capfd=capfd)
-    assert [l[0] for l in lay2] == ["10 B", "10 B"] and lay1 == lay2, (lay1, lay2)
+    D, Ev, _ = e2.scaling()
+    _assert_layout_rule(_ruiz_scaled(A2, D, Ev), lay2)          # the slabs are filled from the scaled values
+    assert lay1 == lay2, (lay1, lay2)
     assert not np.all(e1.scaling()[0] == 1.0)
     _assert_same(e1, o1, e2, o2)
     e1.close()
