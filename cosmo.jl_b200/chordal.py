@@ -462,6 +462,16 @@ class DecompositionInfo:
     num_overlaps: int = 0
     clique_sizes: List[int] = field(default_factory=list)
     trees: Dict[int, "CliqueTree"] = field(default_factory=dict)   # clique tree of every decomposed cone
+    # where the values of A' and b' come from (forward_arrays).  For every entry handed to the assembly of A', in that
+    # order: its row, its column and its source -- the position in the CSR data of A, -1 for the constant +1.0 and -2 for
+    # the constant -1.0 of an overlap column.  For every row of b' that takes a value of b: (row of b', row of b), and
+    # whether it is a row of a clique block, where only the nonzero values of b are written (a -0.0 arrives as +0.0).
+    a_rows: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
+    a_cols: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
+    a_src: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
+    b_new: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
+    b_old: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
+    b_clique: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=bool))
 
 
 def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
@@ -474,7 +484,11 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
     rows_new: List[np.ndarray] = []
     cols_new: List[np.ndarray] = []
     vals_new: List[np.ndarray] = []
+    src_new: List[np.ndarray] = []                               # source of every entry of vals_new (info.a_src)
     b_new: List[np.ndarray] = []
+    b_map_new: List[np.ndarray] = []
+    b_map_old: List[np.ndarray] = []
+    b_map_clique: List[np.ndarray] = []
     sets_new = []
     row_ptr = 0
     n_new = n
@@ -500,7 +514,11 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
             rows_new.append(sub.row + row_ptr)
             cols_new.append(sub.col)
             vals_new.append(sub.data)
+            src_new.append(np.arange(A.indptr[off], A.indptr[off + dim], dtype=np.int64))   # tocoo keeps the CSR order
             b_new.append(b[off:off + dim])
+            b_map_new.append(np.arange(row_ptr, row_ptr + dim, dtype=np.int64))
+            b_map_old.append(np.arange(off, off + dim, dtype=np.int64))
+            b_map_clique.append(np.zeros(dim, dtype=bool))
             sets_new.append(S)
             info.row_map_plain.append((off, row_ptr, dim))
             row_ptr += dim
@@ -533,7 +551,7 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
             loc = {int(v): a for a, v in enumerate(c)}
             par_t = tree.parent[t]
             par_loc = {int(v): a for a, v in enumerate(tree.cliques[par_t])} if par_t >= 0 else None
-            ov_rows, ov_cols, ov_vals = [], [], []
+            ov_rows, ov_cols, ov_vals, ov_src = [], [], [], []
             for bj in range(nc):
                 for ai in range(bj + 1):
                     gi, gj = int(c[ai]), int(c[bj])
@@ -545,6 +563,7 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
                         ov_rows += [new_row, starts[par_t] + svec_index(pa, pb)]
                         ov_cols += [n_new, n_new]
                         ov_vals += [1.0, -1.0]
+                        ov_src += [-1, -2]
                         n_new += 1
                     else:
                         owner[svec_index(gi, gj)] = new_row
@@ -552,6 +571,7 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
                 rows_new.append(np.array(ov_rows, dtype=np.int64))
                 cols_new.append(np.array(ov_cols, dtype=np.int64))
                 vals_new.append(np.array(ov_vals))
+                src_new.append(np.array(ov_src, dtype=np.int64))
             sets_new.append(M.PsdConeTriangle(nc * (nc + 1) // 2))
         lo, hi = int(ip[off]), int(ip[off + dim])
         sub_row = np.repeat(a_rows, row_nnz[a_rows])             # cone-local row of every entry, CSR order
@@ -559,6 +579,10 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
         rows_new.append(mapped)
         cols_new.append(A.indices[lo:hi].astype(np.int64))
         vals_new.append(A.data[lo:hi].copy())
+        src_new.append(np.arange(lo, hi, dtype=np.int64))
+        b_map_new.append(np.fromiter(owner.values(), dtype=np.int64, count=len(owner)))
+        b_map_old.append(off + np.fromiter(owner.keys(), dtype=np.int64, count=len(owner)))
+        b_map_clique.append(np.ones(len(owner), dtype=bool))
         bseg = np.zeros(row_ptr - starts[0])
         nzb = np.nonzero(b[off:off + dim])[0]
         for r in nzb:
@@ -569,6 +593,11 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
     rows_c = np.concatenate(rows_new) if rows_new else np.zeros(0, dtype=np.int64)
     cols_c = np.concatenate(cols_new) if cols_new else np.zeros(0, dtype=np.int64)
     vals_c = np.concatenate(vals_new) if vals_new else np.zeros(0)
+    info.a_rows, info.a_cols = rows_c.astype(np.int64), cols_c.astype(np.int64)
+    info.a_src = np.concatenate(src_new) if src_new else np.zeros(0, dtype=np.int64)
+    info.b_new = np.concatenate(b_map_new) if b_map_new else np.zeros(0, dtype=np.int64)
+    info.b_old = np.concatenate(b_map_old) if b_map_old else np.zeros(0, dtype=np.int64)
+    info.b_clique = np.concatenate(b_map_clique) if b_map_clique else np.zeros(0, dtype=bool)
     A2 = sp.csc_matrix((vals_c, (rows_c, cols_c)), shape=(row_ptr, n_new))
     b2 = np.concatenate(b_new) if b_new else np.zeros(0)
     P2 = sp.block_diag([sp.csc_matrix(P), sp.csc_matrix((n_new - n, n_new - n))], format="csc")
@@ -869,6 +898,93 @@ def reverse_from_arrays(d: DecompositionArrays, x2, s2, mu2):
     s[d.row] = acc
     mu[d.row] = mu2[d.mu_src]
     return x, s, mu
+
+
+@dataclass
+class ForwardArrays:
+    """Where the values of the decomposed problem come from (forward_arrays), as flat arrays.  A' in sorted CSC order:
+    entry k is A.data[a_src[k]] (A in sorted CSC order), +1.0 for a_src[k] = -1, -1.0 for -2 (overlap columns).
+    b'[i] = b[b_src[i]] for a plain row, 0.0 for b_src[i] = -1, and for a row of a clique block b_src[i] = -2 - r with r the
+    row of b: b[r], where a zero of either sign arrives as +0.0 (`decompose` writes only the nonzero values there).
+    q' = [q; 0] and P' = blockdiag(P, 0), whose stored values are P's in P's order: neither needs a map."""
+    n_orig: int
+    m_orig: int
+    n: int                     # decomposed problem
+    m: int
+    nnzA_orig: int
+    a_src: np.ndarray          # nnz(A')
+    b_src: np.ndarray          # m
+    b_uncovered: np.ndarray    # m_orig, uint8: 1 for a row of a decomposed cone that lies in no clique
+
+
+def forward_arrays(info: DecompositionInfo, A0, n2: int, m2: int) -> ForwardArrays:
+    """The value map of `decompose` as flat arrays (cosmo_b200_set_forward_map), from the row, column and source lists
+    `decompose` assembled A' and b' from.  A0: the matrix `decompose` was given; n2, m2: size of the decomposed problem.
+    A row of a decomposed cone outside every clique has no place in b': b must stay zero there (b_uncovered), or the
+    aggregate pattern, and with it the decomposition, changes."""
+    A0 = M._sorted_csc(A0)
+    nnz0 = int(A0.nnz)
+    # decompose() reads A row by row: CSR position -> sorted CSC position, by sending the positions through the same conversion
+    tag = sp.csc_matrix((np.arange(1, nnz0 + 1, dtype=np.float64), A0.indices, A0.indptr), shape=A0.shape)
+    csc_of_csr = sp.csr_matrix(tag).data.astype(np.int64) - 1
+    src = np.array(info.a_src, dtype=np.int64)
+    orig = src >= 0
+    src[orig] = csc_of_csr[src[orig]]
+    order = np.lexsort((info.a_rows, info.a_cols))             # sorted CSC order of A': by column, then row
+    r, c = info.a_rows[order], info.a_cols[order]
+    assert not np.any((np.diff(c) == 0) & (np.diff(r) == 0)), "two entries of A' share a position: the map is not one to one"
+    a_src = src[order]
+    assert np.array_equal(np.sort(a_src[a_src >= 0]), np.arange(nnz0)), "an entry of A is not used exactly once"
+    b_src = np.full(int(m2), -1, dtype=np.int64)
+    b_src[info.b_new] = np.where(info.b_clique, -2 - info.b_old, info.b_old)
+    unc = np.ones(int(info.m_orig), dtype=np.uint8)
+    unc[info.b_old] = 0
+    f = ForwardArrays(int(info.n_orig), int(info.m_orig), int(n2), int(m2), nnz0, a_src, b_src, unc)
+    validate_forward_arrays(f)
+    return f
+
+
+def validate_forward_arrays(f: ForwardArrays) -> None:
+    """Every index in range, every entry of A used exactly once, every row of b used once or marked uncovered (the checks
+    cosmo_b200_set_forward_map applies): ValueError otherwise."""
+    if min(f.n_orig, f.m_orig, f.n, f.m, f.nnzA_orig) < 0 or f.n_orig > f.n:
+        raise ValueError("forward map: bad dimensions")
+    a_src, b_src, unc = np.asarray(f.a_src), np.asarray(f.b_src), np.asarray(f.b_uncovered)
+    if b_src.shape != (f.m,) or unc.shape != (f.m_orig,) or a_src.ndim != 1:
+        raise ValueError("forward map: an array has the wrong size")
+    if len(a_src) and (a_src.min() < -2 or a_src.max() >= f.nnzA_orig):
+        raise ValueError("forward map: a_src out of range")
+    used = np.bincount(a_src[a_src >= 0], minlength=f.nnzA_orig)
+    if (used != 1).any():
+        raise ValueError("forward map: an entry of A is not used exactly once")
+    b_row = np.where(b_src < -1, -2 - b_src, b_src)           # the source row; -1: none
+    if len(b_row) and b_row.max() >= f.m_orig:
+        raise ValueError("forward map: b_src out of range")
+    used = np.bincount(b_row[b_row >= 0], minlength=f.m_orig)
+    if (used + (unc != 0) != 1).any():
+        raise ValueError("forward map: a row of b is used twice, or neither used nor marked uncovered")
+
+
+def forward_values(f: ForwardArrays, Ax=None, q=None, b=None):
+    """(A'.data, q', b') of the decomposed problem from values in the original coordinates (None stays None): what the
+    device gather of cosmo_b200_update_matrices_original computes."""
+    out = [None, None, None]
+    if Ax is not None:
+        Ax = np.asarray(Ax, dtype=np.float64) if f.nnzA_orig else np.zeros(1)
+        out[0] = np.where(f.a_src >= 0, Ax[np.maximum(f.a_src, 0)], np.where(f.a_src == -1, 1.0, -1.0))
+    if q is not None:
+        out[1] = np.concatenate([np.asarray(q, dtype=np.float64), np.zeros(f.n - f.n_orig)])
+    if b is not None:
+        b = np.asarray(b, dtype=np.float64)
+        b = b if f.m_orig else np.zeros(1)
+        clique = b[np.maximum(-2 - f.b_src, 0)]
+        out[2] = np.where(f.b_src >= 0, b[np.maximum(f.b_src, 0)], np.where((f.b_src == -1) | (clique == 0), 0.0, clique))
+    return tuple(out)
+
+
+def uncovered_rows(f: ForwardArrays, b) -> np.ndarray:
+    """rows where `b` is nonzero although no clique holds them: such a b needs a new decomposition"""
+    return np.nonzero((np.asarray(f.b_uncovered) != 0) & (np.asarray(b) != 0))[0]
 
 
 def psd_complete_from_schedule(Y: np.ndarray, c: CompletionSchedule) -> np.ndarray:

@@ -35,6 +35,7 @@
 #include "cg_persistent.cuh"
 #include "ldl.cuh"
 #include "chordal_rev.cuh"
+#include "chordal_fwd.cuh"
 #include "mat_update.cuh"
 
 namespace cosmo {
@@ -180,6 +181,9 @@ class EngineBase {
   virtual void psd_lambda_max(const void* v, double* lam) = 0;
   virtual void ldl_stats(double* out8) = 0;
   virtual void set_decomposition(const cosmo_b200_decomposition* d) = 0;
+  virtual void set_forward_map(const cosmo_b200_forward_map* f) = 0;
+  virtual void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
+                                        const void* b) = 0;
   virtual void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) = 0;
 };
 
@@ -221,6 +225,9 @@ class Engine : public EngineBase {
   void psd_lambda_max(const void* v, double* lam) override;
   void ldl_stats(double* out8) override;
   void set_decomposition(const cosmo_b200_decomposition* d) override;
+  void set_forward_map(const cosmo_b200_forward_map* f) override;
+  void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
+                                const void* b) override;
   void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) override;
 
  private:
@@ -286,6 +293,7 @@ class Engine : public EngineBase {
   bool is_optimized_ = false;
   bool have_solution_ = false;   // xs_, s_, mu_ hold what the last solve() returned (cleared by reset / warm_start)
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
+  fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
   // KKT (reduced CG)
   DevBuf<T> ls_, t0_, tm_, xsol_, rhsb_, cb_, r_, u_, nu_;
   DevBuf<T> mr_[6], mr_x_, mr_c_, mr_b_;   // MINRES Lanczos / direction vectors, solution, operator output, rhs
@@ -389,8 +397,10 @@ class Engine : public EngineBase {
   void build_csr(DevCsr<T>& dst, const HostCsr& h);
   void build_windows(DevCsr<T>& dst, const HostCsr& h, const int* src);
   void write_values(const void* Px, const void* Ax, const void* q, const void* b);
+  void upload_values(const void* Px, const void* Ax, const void* q, const void* b, DevBuf<T>& px);
+  void values_placed(const T* Px, bool A, bool b);
+  void finish_update(const T* Px, bool A, bool b, double t0);
   void gather_csr(DevCsr<T>& M, const T* v);
-  void load_P(const void* Px);
   int exponent_window();
   void update_slab(DevCsr<T>& M, int ebase);
   void upload_value_maps();
@@ -1125,8 +1135,61 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
     throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices: an equilibrating engine needs the unscaled P, A, q and b"};
   CUDA_TRY(cudaSetDevice(device_));
   const double t0 = now_s();
+  DevBuf<T> px;
+  upload_values(Px, Ax, q, b, px);
+  finish_update(Px ? px.p : nullptr, Ax != nullptr, b != nullptr, t0);
+}
+
+// The same update from values in the coordinates of the problem a chordal decomposition started from: they are staged on
+// the device, gathered through the forward map (chordal_fwd.cuh) into the resident arrays of the decomposed problem,
+// and take the value path of update_matrices from there.  Nothing is written before every check has passed.
+template <typename T>
+void Engine<T>::update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
+                                         const void* b) {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "update_matrices_original: a sharded handle holds only a slice of the data"};
+  if (!fwd_.has_map()) throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: no forward map (cosmo_b200_set_forward_map)"};
+  if ((Px && nnzP != P_.nnz) || (Ax && nnzA_orig != fwd_.nnzA_orig()))
+    throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: nnz differs from the pattern the decomposition was made for (a new pattern needs a new engine)"};
+  if (device_scaled_ && !(Px && Ax && q && b))
+    throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: an equilibrating engine needs the unscaled P, A, q and b"};
+  CUDA_TRY(cudaSetDevice(device_));
+  const double t0 = now_s();
+  DevBuf<T> px, ax, b0;
+  if (Px) px.alloc((size_t)P_.nnz, false);
+  if (Ax) ax.alloc((size_t)fwd_.nnzA_orig(), false);
+  if (b) {
+    b0.alloc((size_t)fwd_.m_orig(), false);
+    upload_vec(b0, b, (size_t)fwd_.m_orig());
+    const long long bad = fwd_.count_uncovered<T>(b0.p, stream_);
+    launches_ += 2;
+    if (bad)
+      throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: b is nonzero in " + std::to_string(bad) +
+                                                    " rows of a decomposed cone that no clique holds (the sparsity pattern, and with it the decomposition, changes: a new engine is needed)"};
+  }
+  if (Px) upload_vec(px, Px, (size_t)P_.nnz);   // P' = blockdiag(P, 0): P's values in P's order
+  if (Ax) {
+    upload_vec(ax, Ax, (size_t)fwd_.nnzA_orig());
+    fwd_.gather_values<T>(ax.p, At_.val.p, stream_);
+    ++launches_;
+  }
+  if (q) {   // q' = [q; 0]
+    upload_vec(q_, q, (size_t)fwd_.n_orig());
+    if (n_ > fwd_.n_orig()) CUDA_TRY(cudaMemsetAsync(q_.p + fwd_.n_orig(), 0, (size_t)(n_ - fwd_.n_orig()) * sizeof(T), stream_));
+  }
+  if (b) {
+    fwd_.gather_b<T>(b0.p, b_.p, stream_);
+    ++launches_;
+  }
+  sync();   // the staged host arrays have been read
+  finish_update(Px ? px.p : nullptr, Ax != nullptr, b != nullptr, t0);
+}
+
+// What follows the new values on the device, for both updates: every resident copy (values_placed), then the state of a
+// new engine.
+template <typename T>
+void Engine<T>::finish_update(const T* Px, bool A, bool b, double t0) {
   upload_value_maps();
-  write_values(Px, Ax, q, b);
+  values_placed(Px, A, b);
   destroy_cg_graphs();   // the slab and escape-table pointers they captured may have changed
   reset();
   auto_rho_interval_ = 0;
@@ -1134,20 +1197,42 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
   create_time_ = now_s() - t0;
 }
 
-// The values of P, A, q and b (null: keep the current ones), through the value maps of mat_update.cuh, for create and
-// update_matrices alike.  An equilibrating engine scales the CSR copies, q, b and its unscaled Box bounds first; the
-// slabs come last, gathered from the final A' values, so every resident copy of A holds the same numbers.
+// Host values of P, A, q and b (null: keep the current ones) to the device: A's into At_.val (CSR(A') is the CSC order of
+// A), q and b into place, P's CSC values into the scratch `px` (P's CSC order is not resident).
+template <typename T>
+void Engine<T>::upload_values(const void* Px, const void* Ax, const void* q, const void* b, DevBuf<T>& px) {
+  if (Px) {
+    px.alloc((size_t)P_.nnz, false);
+    upload_vec(px, Px, (size_t)P_.nnz);
+  }
+  if (Ax) upload_vec(At_.val, Ax, (size_t)At_.nnz);
+  if (q) upload_vec(q_, q, n_);
+  if (b) upload_vec(b_, b, m_);
+  sync();
+}
+
+// The values of P, A, q and b from host arrays, for create.
 template <typename T>
 void Engine<T>::write_values(const void* Px, const void* Ax, const void* q, const void* b) {
-  if (Ax) {
-    upload_vec(At_.val, Ax, (size_t)At_.nnz);   // CSR(A') is the CSC order of A
-    gather_csr(A_, At_.val.p);
-  }
-  if (Px) load_P(Px);
-  if (q) upload_vec(q_, q, n_);
-  if (b) {
-    upload_vec(b_, b, m_);
-    for (int i = 0; i < m_; ++i) hb_[i] = (double)static_cast<const T*>(b)[i];
+  DevBuf<T> px;
+  upload_values(Px, Ax, q, b, px);
+  values_placed(Px ? px.p : nullptr, Ax != nullptr, b != nullptr);
+}
+
+// The one value path of create and of both updates, from sources in device memory: `Px` holds P's new CSC values (null:
+// keep P), At_.val the new CSC values of A when `A` is set, b_ the new b when `b` is set (q_ needs nothing more).  They
+// go through the value maps of mat_update.cuh into the CSR copies.  An equilibrating engine scales the CSR copies, q, b
+// and its unscaled Box bounds first; the slabs come last, gathered from the final A' values, so every resident copy of A
+// holds the same numbers.
+template <typename T>
+void Engine<T>::values_placed(const T* Px, bool A, bool b) {
+  if (A) gather_csr(A_, At_.val.p);
+  if (Px) gather_csr(P_, Px);
+  if (b && !device_scaled_) {   // the host mirror of b (row classification); equilibrate() refreshes it from the scaled b
+    std::vector<T> hb(m_);
+    download_vec(hb.data(), b_.p, m_);
+    sync();
+    for (int i = 0; i < m_; ++i) hb_[i] = (double)hb[i];
   }
   if (device_scaled_) {
     std::vector<T> l(hl0_.begin(), hl0_.end()), u(hu0_.begin(), hu0_.end());
@@ -1155,7 +1240,7 @@ void Engine<T>::write_values(const void* Px, const void* Ax, const void* q, cons
     upload_vec(box_u_, u.data(), m_);
     equilibrate();
   }
-  if (Ax) {
+  if (A) {
     const int ebase = A_.packable || At_.packable ? exponent_window() : 0;   // one exponent window for A and A'
     update_slab(A_, ebase);
     update_slab(At_, ebase);
@@ -1169,15 +1254,6 @@ void Engine<T>::gather_csr(DevCsr<T>& M, const T* v) {
   matup::gather_kernel<T><<<vgrid(M.nnz), kBlock, 0, stream_>>>(M.nnz, M.d_src.p, v, M.val.p);
   check_launch("gather_csr");
   sync();
-}
-
-// P's CSR values from its CSC values (host), through P_.d_src
-template <typename T>
-void Engine<T>::load_P(const void* Px) {
-  DevBuf<T> px;
-  px.alloc((size_t)P_.nnz, false);
-  upload_vec(px, Px, (size_t)P_.nnz);
-  gather_csr(P_, px.p);
 }
 
 // The window base of the packed slabs of A and A' (win_pack.h): the kCodes binades that hold the most finite normal
@@ -2594,6 +2670,14 @@ void Engine<T>::set_decomposition(const cosmo_b200_decomposition* d) {
   else rev_.set(*d, n_, m_, stream_);
 }
 
+template <typename T>
+void Engine<T>::set_forward_map(const cosmo_b200_forward_map* f) {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "set_forward_map: a sharded handle holds only a slice of the data"};
+  CUDA_TRY(cudaSetDevice(device_));
+  if (!f) fwd_.clear();
+  else fwd_.set(*f, n_, m_, At_.nnz, stream_);
+}
+
 // reverse_scaling! + reverse_decomposition! (+ psd_completion!) of the iterates the last solve left in HBM
 template <typename T>
 void Engine<T>::reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) {
@@ -2791,6 +2875,13 @@ int cosmo_b200_comm_p2p_attach(cosmo_b200_handle* h, const void* blobs, int32_t 
 
 int cosmo_b200_set_decomposition(cosmo_b200_handle* h, const cosmo_b200_decomposition* d) {
   ABI_GUARD(h, h->impl->set_decomposition(d));
+}
+int cosmo_b200_set_forward_map(cosmo_b200_handle* h, const cosmo_b200_forward_map* f) {
+  ABI_GUARD(h, h->impl->set_forward_map(f));
+}
+int cosmo_b200_update_matrices_original(cosmo_b200_handle* h, const void* Px, int64_t nnzP, const void* Ax, int64_t nnzA_orig,
+                                        const void* q, const void* b) {
+  ABI_GUARD(h, h->impl->update_matrices_original(Px, nnzP, Ax, nnzA_orig, q, b));
 }
 int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
   ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));

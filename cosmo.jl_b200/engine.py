@@ -101,6 +101,12 @@ class DecompositionStruct(C.Structure):
                 ("n_cones", C.c_int64), ("cones", C.c_void_p)]
 
 
+class ForwardMapStruct(C.Structure):
+    _fields_ = [("n_orig", C.c_int64), ("m_orig", C.c_int64), ("n", C.c_int64), ("m", C.c_int64),
+                ("nnzA_orig", C.c_int64), ("nnzA", C.c_int64), ("a_src", C.c_void_p), ("b_src", C.c_void_p),
+                ("b_uncovered", C.c_void_p)]
+
+
 def _i64(a, keep):
     a = np.ascontiguousarray(a, dtype=np.int64)
     keep.append(a)
@@ -128,6 +134,7 @@ EXPORTS = [
     "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats", "cosmo_b200_infeasibility_test",
     "cosmo_b200_psd_lambda_max", "cosmo_b200_ldl_stats", "cosmo_b200_ldl_symbolic",
     "cosmo_b200_set_decomposition", "cosmo_b200_reverse_decomposition", "cosmo_b200_psd_complete",
+    "cosmo_b200_set_forward_map", "cosmo_b200_update_matrices_original",
 ]
 
 _lib = None
@@ -188,6 +195,8 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_set_decomposition.argtypes = [vp, C.POINTER(DecompositionStruct)]
     lib.cosmo_b200_reverse_decomposition.argtypes = [vp, C.c_int32, vp, vp, vp, i64p]
     lib.cosmo_b200_psd_complete.argtypes = [C.c_int64, C.POINTER(CompletionStruct), vp, i64p]
+    lib.cosmo_b200_set_forward_map.argtypes = [vp, C.POINTER(ForwardMapStruct)]
+    lib.cosmo_b200_update_matrices_original.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, vp]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if name not in ("cosmo_b200_destroy", "cosmo_b200_last_error"):
@@ -299,6 +308,7 @@ class Engine:
             raise EngineError(rc, (self._lib.cosmo_b200_last_error(None) or b"").decode())
         self._h = h
         self.n_orig, self.m_orig = 0, 0     # the original problem of a decomposition map (set_decomposition)
+        self._fwd_sizes = None              # (n_orig, m_orig) of the forward map (set_forward_map)
         del keep
 
     # ---- lifecycle --------------------------------------------------------
@@ -518,6 +528,33 @@ class Engine:
         self._check(self._lib.cosmo_b200_reverse_decomposition(self._h, int(bool(complete_dual)), *[_ptr(a) for a in out],
                                                                stats))
         return out[0], out[1], out[2], dict(zip(REVERSE_STATS, [int(v) for v in stats]))
+
+
+    # ---- values of the original problem onto the decomposed one ---------------
+    def set_forward_map(self, f):
+        """cosmo_b200_set_forward_map: hand over a chordal.ForwardArrays (None clears it)."""
+        if f is None:
+            self._check(self._lib.cosmo_b200_set_forward_map(self._h, None))
+            self._fwd_sizes = None
+            return
+        keep = []
+        unc = np.ascontiguousarray(f.b_uncovered, dtype=np.uint8)
+        fs = ForwardMapStruct(int(f.n_orig), int(f.m_orig), int(f.n), int(f.m), int(f.nnzA_orig), len(f.a_src),
+                              _i64(f.a_src, keep), _i64(f.b_src, keep), _ptr(unc))
+        self._check(self._lib.cosmo_b200_set_forward_map(self._h, C.byref(fs)))
+        self._fwd_sizes = (int(f.n_orig), int(f.m_orig))
+
+    def update_matrices_original(self, Px=None, Ax=None, q=None, b=None):
+        """cosmo_b200_update_matrices_original: update_matrices with the ``data`` arrays of P and A (sorted CSC), q and b
+        of the problem the chordal decomposition started from; the forward map (set_forward_map) carries them onto the
+        decomposed problem on the device."""
+        Px, Ax = [None if a is None else np.ascontiguousarray(a, dtype=self.dtype).ravel() for a in (Px, Ax)]
+        if self._fwd_sizes is not None:
+            q, b = self._vec(q, self._fwd_sizes[0]), self._vec(b, self._fwd_sizes[1])
+        else:       # without a map the engine reads none of them and answers ERR_INVALID
+            q, b = [None if a is None else np.ascontiguousarray(a, dtype=self.dtype).ravel() for a in (q, b)]
+        self._check(self._lib.cosmo_b200_update_matrices_original(
+            self._h, _ptr(Px), 0 if Px is None else Px.size, _ptr(Ax), 0 if Ax is None else Ax.size, _ptr(q), _ptr(b)))
 
 
 def psd_complete(Y, schedule):

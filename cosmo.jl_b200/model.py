@@ -464,6 +464,7 @@ class Model:
         self.times = {}
         self._dec = None          # chordal DecompositionInfo of the problem the engine holds (settings.decompose)
         self._x2 = None           # iterates of the decomposed problem (None: restart from self.x)
+        self._fwd = None          # chordal.ForwardArrays the engine holds: original values -> decomposed problem
 
     # assemble!(model, P, q, constraints; settings, x0, y0), interface.jl:30-77
     def assemble(self, P, q, constraints: Union[Constraint, Sequence[Constraint]], settings: Optional[Settings] = None,
@@ -516,6 +517,7 @@ class Model:
         self.is_scaled = False
         self._dec = None
         self._x2 = None
+        self._fwd = None
         if self.engine is not None:
             self.engine.close()
             self.engine = None
@@ -558,12 +560,15 @@ class Model:
                 raise ValueError("The dimension of b, does not agree with the model dimension, m.")
             self.b0 = b.copy()
         if self.engine is not None and getattr(self, "_dec", None) is not None:
-            # the row map of b into the clique blocks is rebuilt with the decomposition at the next optimize! (rho and
-            # the iterates of the decomposed problem restart; the reference refuses: "can not be updated if the model
-            # has been chordally decomposed before", interface.jl:192,204)
-            self._x2 = None
-            self.engine.close()
-            self.engine = None
+            # the reference refuses: "can not be updated if the model has been chordally decomposed before"
+            # (interface.jl:192,204).  Here q and b are mapped onto the decomposed problem, q' = [q; 0] and b' = b[b_src],
+            # and go to the engine as for any other model: rho and the clique iterates stay, as update! keeps them.
+            if self._decomposition_holds(b):
+                from . import chordal as _chordal
+                _, q2, b2 = _chordal.forward_values(self._fwd, None, self.q0 if q is not None else None,
+                                                    self.b0 if b is not None else None)
+                self.engine.update_qb((self.D * q2) * self.c if q is not None else None,
+                                      self.E * b2 if b is not None else None)
         elif self.engine is not None:
             qs = (self.D * self.q0) * self.c if q is not None else None
             bs = self.E * self.b0 if b is not None else None
@@ -597,10 +602,12 @@ class Model:
         if self.engine is None:
             return
         if self._dec is not None:
-            # the decomposed problem is rebuilt from the new data at the next optimize!, as update(q, b) does
-            self._x2 = None
-            self.engine.close()
-            self.engine = None
+            # the values in the original coordinates go through the forward map on the device; all four, so that an
+            # equilibrating engine can run Ruiz again.  The clique iterates stay as the next warm start.
+            if self._decomposition_holds(b):
+                self.engine.update_matrices_original(self.P0.data, self.A0.data, self.q0, self.b0)
+                if self._engine_equilibrates:
+                    self.D, self.E, self.c = self.engine.scaling()
             return
         if self._engine_equilibrates:
             # Ruiz runs again on the device from the unscaled data: every vector goes with the matrices
@@ -610,6 +617,22 @@ class Model:
             self.engine.update_matrices(new["P"].data if "P" in new else None, new["A"].data if "A" in new else None,
                                         q, b)
 
+    def _decomposition_holds(self, b) -> bool:
+        """Can the live engine of a decomposed model take the new data?  Not without the forward map, and not when the new
+        `b` is nonzero in a row of a decomposed cone that no clique holds: the aggregate sparsity pattern changes, so the
+        engine is dropped and the next optimize! decomposes again (rho and the clique iterates restart)."""
+        if self._fwd is not None:
+            if b is None:
+                return True
+            from . import chordal as _chordal
+            if not len(_chordal.uncovered_rows(self._fwd, b)):
+                return True
+        self._x2 = None
+        self._fwd = None
+        self.engine.close()
+        self.engine = None
+        return False
+
     # setup! (setup.jl:18-64): scaling + engine creation (the KKT "factorisation" analogue)
     def _setup(self):
         st = self.settings
@@ -617,6 +640,7 @@ class Model:
         if self.engine is None:
             # chordal_decomposition!(ws), chordal_decomposition.jl:1-30 (before setup!, solver.jl:88-93)
             self._dec = None
+            self._fwd = None
             P0, q0, A0, b0, sets0 = self.P0, self.q0, self.A0, self.b0, self.sets0
             if st.decompose:
                 from . import chordal as _chordal
@@ -642,6 +666,10 @@ class Model:
             self.D, self.E, self.c = D, E, c
             if self._dec is not None and st.reverse_on_device:
                 self.engine.set_decomposition(_chordal.decomposition_arrays(self._dec, n2, m2))
+            if self._dec is not None and hasattr(self.engine, "set_forward_map"):
+                # later updates of q, b, P and A keep this engine; an engine that cannot take the map is rebuilt instead
+                self._fwd = _chordal.forward_arrays(self._dec, self.A0, n2, m2)
+                self.engine.set_forward_map(self._fwd)
         else:
             self.engine.update_settings(st.to_struct())
         configure_accelerator(self.engine, st)

@@ -395,6 +395,44 @@ int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual
    stats as above.  Errors through cosmo_b200_last_error(NULL). */
 int cosmo_b200_psd_complete(int64_t N, const cosmo_b200_completion* schedule, double* Y, int64_t stats[4]);
 
+/* ---- values of the original problem onto a chordally decomposed one ------ */
+/* The way forward through the decomposition for values, an engine extension: the reference refuses to update a model
+   that has been chordally decomposed at all (update!, interface.jl:192,204), so every new q, b, P or A pays the
+   decomposition, the augmentation and the setup again.  None of them depends on the values: the decomposition is a
+   function of the sparsity pattern, and the decomposed problem (the handle's n, m, nnzA) takes its values from the
+   original one (n_orig, m_orig, nnzA_orig), 0-based, as
+     A' in CSC order with sorted rows: entry k = Ax[a_src[k]], or the constant +1.0 for a_src[k] = -1, -1.0 for -2
+        (the overlap columns); every entry of A is used exactly once;
+     b'[i] = b[b_src[i]] for a plain row, 0.0 for b_src[i] = -1, and for a row of a clique block b_src[i] = -2 - r:
+        b[r], where a zero of either sign arrives as +0.0 (the decomposition writes only the nonzero values there);
+     q' = [q; 0];   P' = blockdiag(P, 0): P's values in P's order.
+   b_uncovered[i] != 0 marks an original row of a decomposed cone that lies in no clique: b must be zero there, a
+   nonzero value changes the aggregate sparsity pattern and with it the decomposition.  Every other original row is
+   the source of exactly one row of b'. */
+typedef struct {
+  int64_t n_orig, m_orig;
+  int64_t n, m;              /* must equal the handle's n, m */
+  int64_t nnzA_orig;
+  int64_t nnzA;              /* must equal the nnz of the handle's A */
+  const int64_t* a_src;      /* nnzA */
+  const int64_t* b_src;      /* m */
+  const uint8_t* b_uncovered; /* m_orig */
+} cosmo_b200_forward_map;
+/* Checks every index and copies the map to the device (as int32 where every index fits), where it stays; NULL clears
+   it.  A size that is not the handle's, an index out of range, an entry of A used twice or not at all, a row of b used
+   twice, or a row that is neither used nor marked uncovered (or both): COSMO_B200_ERR_INVALID.  A sharded handle
+   (nranks > 1): COSMO_B200_ERR_UNSUPPORTED. */
+int cosmo_b200_set_forward_map(cosmo_b200_handle* h, const cosmo_b200_forward_map* f);
+/* cosmo_b200_update_matrices with Px (nnzP entries), Ax (nnzA_orig entries), q (n_orig) and b (m_orig) in the
+   coordinates and the CSC order of the ORIGINAL problem: they are staged on the device, gathered through the forward
+   map and enter the value path of cosmo_b200_update_matrices.  The same rules hold: NULL = leave unchanged, an
+   equilibrating engine needs all four, unscaled, and the handle ends up bit for bit in the state cosmo_b200_create
+   with the decomposed new data leaves; a decomposition map stays, reverse_decomposition needs a solve first.  No
+   forward map, nnzP or nnzA_orig that differ from the pattern, or a b that is nonzero on an uncovered row (counted on
+   the device before the first write): COSMO_B200_ERR_INVALID, and nothing has changed. */
+int cosmo_b200_update_matrices_original(cosmo_b200_handle* h, const void* Px, int64_t nnzP, const void* Ax,
+                                        int64_t nnzA_orig, const void* q, const void* b);
+
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
 int cosmo_b200_comm_unique_id(void* id128);
