@@ -19,8 +19,11 @@ Restated (not ported) from the reference:
   * compact ("clique tree based") augmentation  transformations.jl:152-374: every clique becomes a
     PsdConeTriangle block; an entry (i,j) inside the separator of a clique gets a new variable with +1 in
     the clique's row and -1 in the parent's row of the same (i,j)
+  * traditional augmentation                     transformations.jl:1-138 (compact_transformation = false):
+    A' = [A H; 0 -I], b' = [b; 0] with one column of H per row of every clique block and of every kept cone; square
+    PsdCone cones are decomposed too (clique blocks PsdCone(nc^2) over both triangles)
   * reverse_decomposition!                       chordal_decomposition.jl:129-213 (x truncated, s = sum of
-    blocks, mu = block value)
+    blocks, mu = block value; traditional: s = H s', mu = H mu' / overlap count)
   * psd_completion! / psd_complete!               chordal_decomposition.jl:215-311 (`complete_dual`): the entries
     of the dual matrix outside the pattern are chosen so that Y = -mat(mu) is positive semidefinite -- the
     maximum-determinant completion, clique by clique from the root of the clique tree
@@ -472,11 +475,60 @@ class DecompositionInfo:
     b_new: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
     b_old: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
     b_clique: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=bool))
+    # the transformation: compact (clique tree based) or traditional (A' = [A H; 0 -I]); for the traditional one the
+    # original row of every column of H (blocks and row_map_plain then point at row m_orig + column of the block's first
+    # entry, and num_overlaps counts the columns of H)
+    compact: bool = True
+    h_rows: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.int64))
 
 
-def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
-    """chordal_decomposition!(ws) for PsdConeTriangle cones (compact transformation).
-    Returns (P', q', A', b', sets', info)."""
+def _aggregate_pattern(A, b, off: int, S):
+    """find_aggregate_sparsity + row_ind_to_matrix_indices (chordal_decomposition.jl:100-115, trees.jl:655-694): the (i, j)
+    of every row of the cone at rows off.. that holds an entry of A or b, or None when the pattern with the diagonal
+    flagged covers every row (a dense cone is kept, chordal_decomposition.jl:53-60).  A: CSR."""
+    N, dim = S.sqrt_dim, S.dim
+    # straight from the row pointers (slicing the CSR matrix would copy a 50-million-row cone: C5 has N = 10 000)
+    ip = A.indptr
+    a_rows = np.nonzero(ip[off + 1:off + dim + 1] - ip[off:off + dim])[0]
+    nz_rows = np.unique(np.concatenate([a_rows, np.nonzero(b[off:off + dim])[0]]))
+    v = np.arange(N, dtype=np.int64)
+    if isinstance(S, M.PsdCone):                                # column-major: row i + N j
+        ii, jj, diag_rows = nz_rows % N, nz_rows // N, v + N * v
+    else:
+        (ii, jj), diag_rows = svec_to_ij(nz_rows), v * (v + 1) // 2 + v
+    if len(np.union1d(nz_rows, diag_rows)) >= dim:
+        return None
+    return ii, jj
+
+
+def _merged(tree: CliqueTree, merge: str) -> CliqueTree:
+    if merge == "parent_child":
+        return parent_child_merge(tree)
+    if merge == "parent_child_reference":
+        return parent_child_merge_reference(tree)
+    if merge == "clique_graph":
+        return clique_graph_merge(tree)
+    if merge != "none":
+        raise ValueError("merge must be 'none', 'parent_child', 'parent_child_reference' or 'clique_graph'")
+    return tree
+
+
+def _clique_rows(S, c: np.ndarray) -> np.ndarray:
+    """rows (cone-local) of the block of clique c, in the order of add_subblock_map! (transformations.jl:94-117): for a
+    PsdCone all (vi, vj) column-major, for a PsdConeTriangle the upper triangle column-major"""
+    c = np.asarray(c, dtype=np.int64)
+    if isinstance(S, M.PsdCone):
+        return (c[:, None] + S.sqrt_dim * c[None, :]).ravel(order="F")
+    ai, bj = svec_to_ij(np.arange(len(c) * (len(c) + 1) // 2, dtype=np.int64))
+    return c[bj] * (c[bj] + 1) // 2 + c[ai]
+
+
+def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3, compact: bool = True):
+    """chordal_decomposition!(ws).  compact = True: the clique tree based transformation of PsdConeTriangle cones; square
+    PsdCone cones stay whole (the reference defines it for triangles only, transformations.jl:267-268).  compact = False:
+    the traditional transformation of both (_decompose_traditional).  Returns (P', q', A', b', sets', info)."""
+    if not compact:
+        return _decompose_traditional(P, q, A, b, sets, merge, min_dim)
     A = sp.csr_matrix(A)
     b = np.asarray(b, dtype=np.float64)
     m, n = A.shape
@@ -496,20 +548,14 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
     Acoo_by_row = A  # csr
     for k, S in enumerate(sets):
         dim = S.dim
-        decomposable = isinstance(S, M.PsdConeTriangle) and S.sqrt_dim >= min_dim
-        if decomposable:
+        pattern = _aggregate_pattern(A, b, off, S) if isinstance(S, M.PsdConeTriangle) and S.sqrt_dim >= min_dim else None
+        if pattern is not None:
             N = S.sqrt_dim
-            # rows of the cone that hold an entry of A or b -- straight from the row pointers (slicing the CSR matrix
-            # would copy a 50-million-row cone: C5 has N = 10 000)
+            ii, jj = pattern
             ip = A.indptr
             row_nnz = ip[off + 1:off + dim + 1] - ip[off:off + dim]
             a_rows = np.nonzero(row_nnz)[0]
-            nz_rows = np.unique(np.concatenate([a_rows, np.nonzero(b[off:off + dim])[0]]))
-            ii, jj = svec_to_ij(nz_rows)
-            diag_rows = np.arange(N, dtype=np.int64) * (np.arange(N, dtype=np.int64) + 1) // 2 + np.arange(N)
-            if len(np.union1d(nz_rows, diag_rows)) >= dim:   # dense pattern: keep the cone (chordal_decomposition.jl:53-60)
-                decomposable = False
-        if not decomposable:
+        if pattern is None:
             sub = Acoo_by_row[off:off + dim].tocoo()
             rows_new.append(sub.row + row_ptr)
             cols_new.append(sub.col)
@@ -524,15 +570,7 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
             row_ptr += dim
             off += dim
             continue
-        tree = chordal_cliques(N, ii, jj)
-        if merge == "parent_child":
-            tree = parent_child_merge(tree)
-        elif merge == "parent_child_reference":
-            tree = parent_child_merge_reference(tree)
-        elif merge == "clique_graph":
-            tree = clique_graph_merge(tree)
-        elif merge != "none":
-            raise ValueError("merge must be 'none', 'parent_child', 'parent_child_reference' or 'clique_graph'")
+        tree = _merged(chordal_cliques(N, ii, jj), merge)
         # row offsets of the clique blocks
         starts = []
         for c in tree.cliques:
@@ -602,6 +640,74 @@ def decompose(P, q, A, b, sets, merge: str = "parent_child", min_dim: int = 3):
     b2 = np.concatenate(b_new) if b_new else np.zeros(0)
     P2 = sp.block_diag([sp.csc_matrix(P), sp.csc_matrix((n_new - n, n_new - n))], format="csc")
     q2 = np.concatenate([np.asarray(q, dtype=np.float64), np.zeros(n_new - n)])
+    return P2, q2, A2, b2, sets_new, info
+
+
+def _decompose_traditional(P, q, A, b, sets, merge: str, min_dim: int):
+    """find_decomposition_matrix! + augment_system! (transformations.jl:1-138): H has one column per row of a kept cone
+    (the identity) and per entry of every clique block, each with a single +1.0 in the original row it copies, and
+        A' = [A H; 0 -I],  b' = [b; 0],  P' = blockdiag(P, 0),  q' = [q; 0],
+        sets' = ZeroSet(m), then every original cone or its cliques (PsdCone(nc^2) / PsdConeTriangle(nc(nc+1)/2)).
+    Square PsdCone and PsdConeTriangle cones are decomposed; a cone whose clique tree has one clique is kept, as the
+    reference does (chordal_decomposition.jl:64-69).  The one difference from the reference's [b; 0]: a row of a
+    decomposed cone that lies in no clique gets +0.0 in b' (b is zero there, of either sign), so that new values mapped
+    through forward_arrays, which writes +0.0 there, end where this decomposition of them ends."""
+    A = sp.csr_matrix(A)
+    b = np.asarray(b, dtype=np.float64)
+    m, n = A.shape
+    info = DecompositionInfo(n, m, list(sets), compact=False)
+    h_rows: List[np.ndarray] = []
+    sets_new = [M.ZeroSet(m)]
+    covered = np.ones(m, dtype=bool)
+    col, off = 0, 0
+    for k, S in enumerate(sets):
+        dim = S.dim
+        tree = None
+        if isinstance(S, (M.PsdConeTriangle, M.PsdCone)) and S.sqrt_dim >= min_dim:
+            pattern = _aggregate_pattern(A, b, off, S)
+            if pattern is not None:
+                tree = _merged(chordal_cliques(S.sqrt_dim, *pattern), merge)
+                if len(tree.cliques) == 1:
+                    tree = None
+        if tree is None:
+            h_rows.append(np.arange(off, off + dim, dtype=np.int64))
+            info.row_map_plain.append((off, m + col, dim))
+            sets_new.append(S)
+            col += dim
+            off += dim
+            continue
+        info.cone_offsets[k] = off
+        info.trees[k] = tree
+        info.blocks[k] = []
+        covered[off:off + dim] = False
+        for c in tree.cliques:
+            rows = off + _clique_rows(S, c)
+            covered[rows] = True
+            h_rows.append(rows)
+            info.blocks[k].append((m + col, c))
+            col += len(rows)
+            nc = len(c)
+            sets_new.append(M.PsdCone(nc * nc) if isinstance(S, M.PsdCone) else M.PsdConeTriangle(nc * (nc + 1) // 2))
+        info.clique_sizes += [len(c) for c in tree.cliques]
+        off += dim
+    h = np.concatenate(h_rows) if h_rows else np.zeros(0, dtype=np.int64)
+    nH = len(h)
+    info.num_overlaps = nH
+    info.h_rows = h
+    # A in CSR order, then H (+1.0), then -I
+    a_rows = np.repeat(np.arange(m, dtype=np.int64), np.diff(A.indptr))
+    cols_h = n + np.arange(nH, dtype=np.int64)
+    info.a_rows = np.concatenate([a_rows, h, m + np.arange(nH, dtype=np.int64)])
+    info.a_cols = np.concatenate([A.indices.astype(np.int64), cols_h, cols_h])
+    info.a_src = np.concatenate([np.arange(A.nnz, dtype=np.int64), np.full(nH, -1, dtype=np.int64),
+                                 np.full(nH, -2, dtype=np.int64)])
+    vals = np.concatenate([A.data, np.ones(nH), -np.ones(nH)])
+    info.b_new = info.b_old = np.nonzero(covered)[0].astype(np.int64)
+    info.b_clique = np.zeros(len(info.b_new), dtype=bool)
+    A2 = sp.csc_matrix((vals, (info.a_rows, info.a_cols)), shape=(m + nH, n + nH))
+    b2 = np.concatenate([np.where(covered, b, 0.0), np.zeros(nH)])
+    P2 = sp.block_diag([sp.csc_matrix(P), sp.csc_matrix((nH, nH))], format="csc")
+    q2 = np.concatenate([np.asarray(q, dtype=np.float64), np.zeros(nH)])
     return P2, q2, A2, b2, sets_new, info
 
 
@@ -753,7 +859,7 @@ class CompletionSchedule:
     entries are known and stay as they are."""
     N: int
     row_offset: int            # first original row of the cone (0 for a bare matrix)
-    dim: int                   # rows of the cone: N(N+1)/2 (PsdConeTriangle); N*N (PsdCone) is refused
+    dim: int                   # rows of the cone: N(N+1)/2 (PsdConeTriangle); N*N (PsdCone) in a traditional map only
     new_of: np.ndarray         # N: old vertex -> traversal position
     steps: np.ndarray          # (n_steps, 6): lo, hi, a0, a1, k0, k1
     idx: np.ndarray
@@ -763,7 +869,8 @@ class CompletionSchedule:
 class DecompositionArrays:
     """The map of `reverse` as flat int64 arrays (decomposition_arrays): plain rows are copied; an original row of a
     decomposed cone gets s = 0.0 + the clique rows s_src[s_ptr[i]:s_ptr[i+1]] in that order and mu = mu_src[i] (the
-    last of them, the row the host loop writes last); rows in no clique stay 0."""
+    last of them, the row the host loop writes last); rows in no clique stay 0.  A traditional map (s = H s') has no
+    mu_src: mu = (0.0 + the same sum over mu') / the length of the list, and plain rows are 0.0 + the row."""
     n_orig: int
     m_orig: int
     n: int                     # decomposed problem
@@ -772,8 +879,9 @@ class DecompositionArrays:
     row: np.ndarray            # original rows of the decomposed cones, increasing
     s_ptr: np.ndarray          # len(row) + 1
     s_src: np.ndarray          # decomposed rows
-    mu_src: np.ndarray         # len(row)
+    mu_src: np.ndarray         # len(row); empty in a traditional map
     cones: List[CompletionSchedule] = field(default_factory=list)
+    traditional: bool = False  # the map of the traditional transformation (cosmo_b200_set_decomposition_noncompact)
 
 
 def completion_schedule(tree: CliqueTree, N: int, row_offset: int = 0) -> CompletionSchedule:
@@ -796,8 +904,9 @@ def completion_schedule(tree: CliqueTree, N: int, row_offset: int = 0) -> Comple
 
 
 def decomposition_arrays(info: DecompositionInfo, n: Optional[int] = None, m: Optional[int] = None) -> DecompositionArrays:
-    """Flatten `info` for the device reverse (cosmo_b200_set_decomposition).  n, m: size of the decomposed problem
-    (default: what the blocks and row map imply)."""
+    """Flatten `info` for the device reverse (cosmo_b200_set_decomposition, or cosmo_b200_set_decomposition_noncompact
+    for the traditional transformation).  n, m: size of the decomposed problem (default: what the blocks and row map
+    imply)."""
     plain = np.array(info.row_map_plain, dtype=np.int64).reshape(-1, 3)
     orig_l, src_l = [], []
     cones = []
@@ -806,15 +915,12 @@ def decomposition_arrays(info: DecompositionInfo, n: Optional[int] = None, m: Op
         S = info.sets_orig[k]
         off = info.cone_offsets[k]
         for start, c in blocks:
-            c = np.asarray(c, dtype=np.int64)
-            nc = len(c)
-            ai, bj = svec_to_ij(np.arange(nc * (nc + 1) // 2, dtype=np.int64))
-            gi, gj = c[ai], c[bj]
-            orig_l.append(off + gj * (gj + 1) // 2 + gi)
-            src_l.append(start + np.arange(nc * (nc + 1) // 2, dtype=np.int64))
-            m_imp = max(m_imp, start + nc * (nc + 1) // 2)
+            rows = off + _clique_rows(S, c)
+            orig_l.append(rows)
+            src_l.append(start + np.arange(len(rows), dtype=np.int64))
+            m_imp = max(m_imp, start + len(rows))
         sched = completion_schedule(info.trees[k], S.sqrt_dim, off)
-        sched.dim = S.dim                                      # a PsdCone would show N*N here and be refused
+        sched.dim = S.dim                                      # N*N for a PsdCone
         cones.append(sched)
     orig = np.concatenate(orig_l) if orig_l else np.zeros(0, dtype=np.int64)
     src = np.concatenate(src_l) if src_l else np.zeros(0, dtype=np.int64)
@@ -822,20 +928,23 @@ def decomposition_arrays(info: DecompositionInfo, n: Optional[int] = None, m: Op
     orig, src = orig[perm], src[perm]
     row, first, counts = np.unique(orig, return_index=True, return_counts=True)
     s_ptr = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
-    mu_src = src[s_ptr[1:] - 1] if len(row) else np.zeros(0, dtype=np.int64)
+    mu_src = src[s_ptr[1:] - 1] if len(row) and info.compact else np.zeros(0, dtype=np.int64)
     return DecompositionArrays(int(info.n_orig), int(info.m_orig), int(n if n is not None else info.n_orig + info.num_overlaps),
                                int(m if m is not None else m_imp), plain, row.astype(np.int64), s_ptr, src.astype(np.int64),
-                               mu_src.astype(np.int64), cones)
+                               mu_src.astype(np.int64), cones, traditional=not info.compact)
 
 
-def validate_schedule(c: CompletionSchedule, m_orig: Optional[int] = None) -> None:
-    """The checks cosmo_b200_set_decomposition / cosmo_b200_psd_complete apply to a schedule: ValueError if one fails."""
+def validate_schedule(c: CompletionSchedule, m_orig: Optional[int] = None, square_ok: bool = False) -> None:
+    """The checks cosmo_b200_set_decomposition / cosmo_b200_psd_complete apply to a schedule: ValueError if one fails.
+    square_ok: a schedule of a traditional map, where a cone may have the square PsdCone layout."""
     N = int(c.N)
     if N < 1:
         raise ValueError("schedule: N must be positive")
-    if m_orig is not None and c.dim == N * N and N > 1:
-        raise NotImplementedError("schedule: the square PsdCone layout is not supported")
-    if m_orig is not None and (c.dim != N * (N + 1) // 2 or not (0 <= c.row_offset and c.row_offset + c.dim <= m_orig)):
+    square = c.dim == N * N and N > 1
+    if m_orig is not None and square and not square_ok:
+        raise NotImplementedError("schedule: the square PsdCone layout is not supported by the compact transformation")
+    if m_orig is not None and ((not square and c.dim != N * (N + 1) // 2) or
+                               not (0 <= c.row_offset and c.row_offset + c.dim <= m_orig)):
         raise ValueError("schedule: cone rows out of range")
     new_of = np.asarray(c.new_of)
     if new_of.shape != (N,) or not np.array_equal(np.sort(new_of), np.arange(N)):
@@ -868,7 +977,10 @@ def validate_decomposition_arrays(d: DecompositionArrays) -> None:
         raise ValueError("decomposition: s_ptr is inconsistent")
     if len(s_src) and (s_src.min() < 0 or s_src.max() >= d.m):
         raise ValueError("decomposition: s_src out of range")
-    if mu_src.shape != row.shape or (len(row) and not np.array_equal(mu_src, s_src[s_ptr[1:] - 1])):
+    if d.traditional:
+        if len(mu_src):
+            raise ValueError("decomposition: a traditional map has no mu_src (mu is the mean over s_src)")
+    elif mu_src.shape != row.shape or (len(row) and not np.array_equal(mu_src, s_src[s_ptr[1:] - 1])):
         raise ValueError("decomposition: mu_src is not the last clique row of each row")
     cover = np.zeros(d.m_orig, dtype=np.int8)
     for old, _, dim in pl.tolist():
@@ -877,7 +989,7 @@ def validate_decomposition_arrays(d: DecompositionArrays) -> None:
     if (cover > 1).any():
         raise ValueError("decomposition: an original row is written twice")
     for c in d.cones:
-        validate_schedule(c, d.m_orig)
+        validate_schedule(c, d.m_orig, square_ok=d.traditional)
 
 
 def reverse_from_arrays(d: DecompositionArrays, x2, s2, mu2):
@@ -887,16 +999,25 @@ def reverse_from_arrays(d: DecompositionArrays, x2, s2, mu2):
     mu = np.zeros(d.m_orig)
     s2 = np.asarray(s2, dtype=np.float64)
     mu2 = np.asarray(mu2, dtype=np.float64)
+    zero = 0.0 if d.traditional else -0.0                    # -0.0 + v is v bit for bit; 0.0 + v makes a -0.0 +0.0
     for old, new, dim in np.asarray(d.plain).reshape(-1, 3).tolist():
-        s[old:old + dim] = s2[new:new + dim]
-        mu[old:old + dim] = mu2[new:new + dim]
+        s[old:old + dim] = zero + s2[new:new + dim]
+        mu[old:old + dim] = zero + mu2[new:new + dim]
     cnt = np.diff(d.s_ptr)
-    acc = np.zeros(len(d.row))
-    for t in range(int(cnt.max()) if len(cnt) else 0):       # position t of every row's list, in list order
-        has = cnt > t
-        acc[has] += s2[d.s_src[d.s_ptr[:-1][has] + t]]
-    s[d.row] = acc
-    mu[d.row] = mu2[d.mu_src]
+
+    def list_sum(v):
+        acc = np.zeros(len(d.row))
+        for t in range(int(cnt.max()) if len(cnt) else 0):   # position t of every row's list, in list order
+            has = cnt > t
+            acc[has] += v[d.s_src[d.s_ptr[:-1][has] + t]]
+        return acc
+
+    s[d.row] = list_sum(s2)
+    if d.traditional:
+        acc = list_sum(mu2)
+        mu[d.row] = np.where(cnt > 1, acc / np.maximum(cnt, 1), acc)
+    else:
+        mu[d.row] = mu2[d.mu_src]
     return x, s, mu
 
 
@@ -1019,8 +1140,24 @@ def reverse(info: DecompositionInfo, x2, s2, mu2, complete_dual: bool = False):
     """reverse_decomposition! (chordal_decomposition.jl:129-213): x = x'[1:n]; s = sum of clique blocks;
     mu = the clique block's value (overlaps carry equal values at optimality).  With `complete_dual`
     (settings.complete_dual, :146) the entries of every decomposed dual matrix outside its cliques are
-    filled by `psd_complete` so that y = -mu is in the PSD cone."""
+    filled by `psd_complete` so that y = -mu is in the PSD cone.
+    The traditional transformation (info.compact False, chordal_decomposition.jl:136-168): s = H s'[m:] and
+    mu = H mu'[m:] divided by each row's count of columns of H (rows in no clique: 0), H v summed as a sparse product
+    sums, 0.0 + the copies in column order."""
     x = np.asarray(x2)[:info.n_orig].copy()
+    if not info.compact:
+        m, h = info.m_orig, info.h_rows
+        s = np.zeros(m)
+        mu = np.zeros(m)
+        np.add.at(s, h, np.asarray(s2, dtype=np.float64)[m:m + len(h)])      # in index order: column order per row
+        np.add.at(mu, h, np.asarray(mu2, dtype=np.float64)[m:m + len(h)])
+        cnt = np.bincount(h, minlength=m)
+        over = cnt > 1
+        mu[over] /= cnt[over]
+        if complete_dual:
+            for k in info.blocks:
+                _complete_cone(mu, info.sets_orig[k], info.cone_offsets[k], info.trees[k])
+        return x, s, mu
     s = np.zeros(info.m_orig)
     mu = np.zeros(info.m_orig)
     for old, new, dim in info.row_map_plain:
@@ -1037,10 +1174,19 @@ def reverse(info: DecompositionInfo, x2, s2, mu2, complete_dual: bool = False):
                 seg = slice(start + svec_index(0, bj), start + svec_index(bj, bj) + 1)
                 s[orig] += s2[seg]
                 mu[orig] = mu2[seg]
-        if complete_dual:   # complete!(mu, ::PsdConeTriangle, ...), chordal_decomposition.jl:245-257
-            S = info.sets_orig[k]
-            N = S.sqrt_dim
-            seg = slice(off, off + S.dim)
-            Y = psd_complete(_svec_to_mat(-mu[seg], N), info.trees[k], assume_symmetric=True)
-            mu[seg] = -_mat_to_svec(Y)
+        if complete_dual:
+            _complete_cone(mu, info.sets_orig[k], off, info.trees[k])
     return x, s, mu
+
+
+def _complete_cone(mu: np.ndarray, S, off: int, tree: CliqueTree) -> None:
+    """complete!(mu, C, ...) of one decomposed cone at rows off.. (chordal_decomposition.jl:232-257), in place: a PsdCone
+    from Symmetric(mat(-mu), :U), written back to all N^2 entries; a PsdConeTriangle from its scaled upper triangle."""
+    N = S.sqrt_dim
+    seg = slice(off, off + S.dim)
+    if isinstance(S, M.PsdCone):
+        Y = psd_complete((-mu[seg]).reshape(N, N, order="F"), tree)
+        mu[seg] = -Y.ravel(order="F")
+    else:
+        Y = psd_complete(_svec_to_mat(-mu[seg], N), tree, assume_symmetric=True)
+        mu[seg] = -_mat_to_svec(Y)

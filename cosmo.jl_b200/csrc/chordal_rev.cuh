@@ -2,12 +2,16 @@
 // + psd_completion! (scaling.jl:170-179, chordal_decomposition.jl:129-311).
 //
 // The map is computed once on the host (chordal.decomposition_arrays) and handed over with
-// cosmo_b200_set_decomposition.  One reverse is:
+// cosmo_b200_set_decomposition (compact transformation) or cosmo_b200_set_decomposition_noncompact (the traditional
+// one, s = H s', chordal_decomposition.jl:136-168).  One reverse is:
 //   1. gather_kernel: x = D x'[:n_orig]; for every original row of a decomposed cone s = 0.0 + the sum of its clique
-//      rows in the host's order and mu = the last of them; plain rows are copied.  One thread per output entry, no
-//      atomics: the result is bit-identical to chordal.reverse on the same fp64 inputs.
+//      rows in the host's order; mu = the last of them (compact) or (0.0 + the same sum over mu') / their count
+//      (traditional: H mu' divided by the row's overlap count).  Plain rows are copied (compact) or are 0.0 + the
+//      row (traditional: they are rows of H s' too).  One thread per output entry, no atomics: the result is
+//      bit-identical to chordal.reverse on the same fp64 inputs.
 //   2. with complete_dual, per decomposed cone (psd_complete, chordal_decomposition.jl:262-311):
-//      a. scatter_kernel: W = mat(-mu) in the traversal numbering (dense, column-major, N x N).
+//      a. scatter_kernel: W = mat(-mu) in the traversal numbering (dense, column-major, N x N); a square PsdCone is
+//         read from its upper triangle (Symmetric(mat(-mu), :U)).
 //      b. solve_kernel, one CTA per clique: Z = W[alpha, alpha] \ W[alpha, nu] in shared memory (Cholesky; LU with
 //         partial pivoting where it fails; the pseudo-inverse through a Jacobi eigendecomposition where the LU pivot
 //         is exactly zero or Z is not finite, as numpy.linalg.solve / pinv).  Both blocks lie inside the clique, and the
@@ -15,7 +19,7 @@
 //      c. update_kernel, one cooperative launch: the cliques in traversal order, a grid barrier between two of them
 //         (clique t reads W[:lo, alpha], which the cliques before it filled); W[r, nu] = W[nu, r] = W[r, alpha] Z for the
 //         rows r < lo outside the clique.
-//      d. gather_back_kernel: mu = -svec(W) over the cone's rows.
+//      d. gather_back_kernel: mu = -svec(W) over the cone's rows (all N^2 entries of a square cone).
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
@@ -66,6 +70,7 @@ struct GatherArgs {
   const int64_t* mu_src;
   const int64_t* plain;       // 3 per block
   const int64_t* plain_pref;  // n_plain + 1
+  int traditional;            // mu is the mean over s_src (mu_src unused); plain rows are 0.0 + the row
   double* x_out;              // NULL: skipped
   double* s_out;
   double* mu_out;
@@ -94,7 +99,14 @@ __global__ void __launch_bounds__(kThreads) gather_kernel(GatherArgs<T> a) {
         for (int64_t p = a.s_ptr[i]; p < a.s_ptr[i + 1]; ++p) acc += unscale_s(a, a.s_src[p]);
         a.s_out[r] = acc;
       }
-      if (a.mu_out) a.mu_out[r] = unscale_mu(a, a.mu_src[i]);
+      if (a.mu_out && a.traditional) {
+        double acc = 0.0;
+        for (int64_t p = a.s_ptr[i]; p < a.s_ptr[i + 1]; ++p) acc += unscale_mu(a, a.s_src[p]);
+        const int64_t cnt = a.s_ptr[i + 1] - a.s_ptr[i];
+        a.mu_out[r] = cnt > 1 ? acc / (double)cnt : acc;
+      } else if (a.mu_out) {
+        a.mu_out[r] = unscale_mu(a, a.mu_src[i]);
+      }
     } else {
       const int64_t q = t - a.n_orig - a.n_rows;
       int64_t lo = 0, hi = a.n_plain - 1;            // the last block that starts at or before q
@@ -103,21 +115,32 @@ __global__ void __launch_bounds__(kThreads) gather_kernel(GatherArgs<T> a) {
         if (a.plain_pref[mid] <= q) lo = mid; else hi = mid - 1;
       }
       const int64_t k = q - a.plain_pref[lo], old = a.plain[3 * lo] + k, nw = a.plain[3 * lo + 1] + k;
-      if (a.s_out) a.s_out[old] = unscale_s(a, nw);
-      if (a.mu_out) a.mu_out[old] = unscale_mu(a, nw);
+      if (a.s_out) {                                  // 0.0 + v: a -0.0 arrives as +0.0, as H s' gives it
+        const double v = unscale_s(a, nw);
+        a.s_out[old] = a.traditional ? 0.0 + v : v;
+      }
+      if (a.mu_out) {
+        const double v = unscale_mu(a, nw);
+        a.mu_out[old] = a.traditional ? 0.0 + v : v;
+      }
     }
   }
 }
 
-// W = mat(-v) in the traversal numbering (_svec_to_mat: off-diagonal entries (y + 0) / sqrt 2)
-__global__ void __launch_bounds__(kThreads) scatter_kernel(int64_t N, const double* v, const int64_t* new_of, double* W) {
+// W = mat(-v) in the traversal numbering (_svec_to_mat: off-diagonal entries (y + 0) / sqrt 2).  A square cone
+// (column-major N x N) is read from its upper triangle, every entry y + 0 as np.triu(Y) + np.triu(Y, 1).T gives it.
+__global__ void __launch_bounds__(kThreads) scatter_kernel(int64_t N, const double* v, const int64_t* new_of, double* W,
+                                                           int square) {
   const int64_t dim = N * (N + 1) / 2;
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < dim; k += (int64_t)gridDim.x * blockDim.x) {
     int64_t i, j;
     svec_ij(k, i, j);
-    const double y = -v[k];
+    const double y = -v[square ? i + N * j : k];
     const int64_t ni = new_of[i], nj = new_of[j];
-    if (i == j) {
+    if (square) {
+      W[ni + N * nj] = y + 0.0;
+      W[nj + N * ni] = y + 0.0;
+    } else if (i == j) {
       W[ni + N * ni] = y;
     } else {
       const double w = (y + 0.0) * kInvSqrt2;
@@ -127,10 +150,15 @@ __global__ void __launch_bounds__(kThreads) scatter_kernel(int64_t N, const doub
   }
 }
 
-// v = -svec(W) (_mat_to_svec: off-diagonal entries times sqrt 2)
-__global__ void __launch_bounds__(kThreads) gather_back_kernel(int64_t N, const int64_t* new_of, const double* W, double* v) {
-  const int64_t dim = N * (N + 1) / 2;
+// v = -svec(W) (_mat_to_svec: off-diagonal entries times sqrt 2); v = -vec(W) over all N^2 entries of a square cone
+__global__ void __launch_bounds__(kThreads) gather_back_kernel(int64_t N, const int64_t* new_of, const double* W, double* v,
+                                                               int square) {
+  const int64_t dim = square ? N * N : N * (N + 1) / 2;
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < dim; k += (int64_t)gridDim.x * blockDim.x) {
+    if (square) {
+      v[k] = -W[new_of[k % N] + N * new_of[k / N]];
+      continue;
+    }
     int64_t i, j;
     svec_ij(k, i, j);
     const double y = W[new_of[j] + N * new_of[i]];
@@ -404,21 +432,25 @@ static inline void fail(int code, const std::string& msg) { throw EngineError{co
 // a validated completion schedule on the device
 struct Cone {
   int64_t N = 0, row_offset = 0, n_steps = 0, z_total = 0, max_lo = 0;
+  int square = 0;                 // the rows are the N^2 entries of a PsdCone (traditional transformation only)
   size_t smem_solve = 0, smem_update = 0;
   DevBuf<int64_t> new_of, steps, idx, z_off;
   StepTable table() const { return StepTable{n_steps, steps.p, idx.p, z_off.p}; }
 };
 
-// checks of one schedule (chordal.validate_schedule); m_orig < 0: a bare matrix
-static void check_schedule(const cosmo_b200_completion& c, int64_t m_orig, int64_t k) {
+// checks of one schedule (chordal.validate_schedule); m_orig < 0: a bare matrix.  square_ok: the traditional
+// transformation, whose cones may have the square PsdCone layout (dim = N^2).
+static void check_schedule(const cosmo_b200_completion& c, int64_t m_orig, int64_t k, bool square_ok = false) {
   const std::string where = m_orig >= 0 ? "decomposition: cone " + std::to_string(k) + ": " : "psd_complete: ";
   const int64_t N = c.N;
   if (N < 1 || N >= (1LL << 31) || !c.new_of || c.n_steps < 0 || c.n_idx < 0 || (c.n_steps && !c.steps) ||
       (c.n_idx && !c.idx))
     fail(COSMO_B200_ERR_INVALID, where + "N, the step count or an array pointer is invalid");
   if (m_orig >= 0) {
-    if (c.dim == N * N && N > 1) fail(COSMO_B200_ERR_UNSUPPORTED, where + "the square PsdCone layout is not supported");
-    if (c.dim != N * (N + 1) / 2 || c.row_offset < 0 || c.row_offset + c.dim > m_orig)
+    const bool square = c.dim == N * N && N > 1;
+    if (square && !square_ok)
+      fail(COSMO_B200_ERR_UNSUPPORTED, where + "the square PsdCone layout is not supported by the compact transformation");
+    if ((!square && c.dim != N * (N + 1) / 2) || c.row_offset < 0 || c.row_offset + c.dim > m_orig)
       fail(COSMO_B200_ERR_INVALID, where + "the rows of the cone are out of range");
   }
   std::vector<char> hit(N, 0);
@@ -444,6 +476,7 @@ static void check_schedule(const cosmo_b200_completion& c, int64_t m_orig, int64
 static void upload_cone(Cone& dst, const cosmo_b200_completion& c, cudaStream_t st) {
   dst.N = c.N;
   dst.row_offset = c.row_offset;
+  dst.square = c.dim == c.N * c.N && c.N > 1;
   dst.n_steps = c.n_steps;
   std::vector<int64_t> zoff(std::max<int64_t>(c.n_steps, 1), 0);
   int64_t z = 0, amax = 0, nnmax = 0, nkmax = 0;
@@ -523,17 +556,23 @@ class Reverse {
 
   void clear() {
     set_ = false;
+    traditional_ = false;
     cones_.clear();
   }
 
-  void set(const cosmo_b200_decomposition& d, int64_t n, int64_t m, cudaStream_t st) {
+  // traditional: the map of the traditional transformation (cosmo_b200_set_decomposition_noncompact): mu_src must be
+  // NULL, mu is the mean of the listed rows, and a cone may have the square PsdCone layout
+  void set(const cosmo_b200_decomposition& d, int64_t n, int64_t m, cudaStream_t st, bool traditional = false) {
     clear();
     if (d.n != n || d.m != m)
       fail(COSMO_B200_ERR_INVALID, "decomposition: n, m (" + std::to_string(d.n) + ", " + std::to_string(d.m) +
                                        ") are not the engine's (" + std::to_string(n) + ", " + std::to_string(m) + ")");
     if (d.n_orig < 0 || d.n_orig > n || d.m_orig < 0 || d.n_plain < 0 || d.n_rows < 0 || d.n_cones < 0 ||
-        (d.n_plain && !d.plain) || (d.n_rows && (!d.row || !d.s_ptr || !d.mu_src)) || (d.n_cones && !d.cones))
+        (d.n_plain && !d.plain) || (d.n_rows && (!d.row || !d.s_ptr || (!traditional && !d.mu_src))) ||
+        (d.n_cones && !d.cones))
       fail(COSMO_B200_ERR_INVALID, "decomposition: bad dimensions or a missing array");
+    if (traditional && d.mu_src)
+      fail(COSMO_B200_ERR_INVALID, "decomposition: mu_src must be NULL for the traditional transformation (mu is the mean)");
     // plain blocks and decomposed rows: in range, and no original row written twice
     std::vector<std::pair<int64_t, int64_t>> spans;
     std::vector<int64_t> pref(d.n_plain + 1, 0);
@@ -560,10 +599,10 @@ class Reverse {
       if (d.s_ptr[i + 1] <= d.s_ptr[i] || d.s_ptr[i + 1] > nnz) fail(COSMO_B200_ERR_INVALID, "decomposition: s_ptr is inconsistent");
       for (int64_t p = d.s_ptr[i]; p < d.s_ptr[i + 1]; ++p)
         if (d.s_src[p] < 0 || d.s_src[p] >= m) fail(COSMO_B200_ERR_INVALID, "decomposition: s_src out of range");
-      if (d.mu_src[i] != d.s_src[d.s_ptr[i + 1] - 1])
+      if (!traditional && d.mu_src[i] != d.s_src[d.s_ptr[i + 1] - 1])
         fail(COSMO_B200_ERR_INVALID, "decomposition: mu_src of row " + std::to_string(r) + " is not its last clique row");
     }
-    for (int64_t k = 0; k < d.n_cones; ++k) check_schedule(d.cones[k], d.m_orig, k);
+    for (int64_t k = 0; k < d.n_cones; ++k) check_schedule(d.cones[k], d.m_orig, k, traditional);
 
     n_orig_ = d.n_orig; m_orig_ = d.m_orig; n_rows_ = d.n_rows; n_plain_ = d.n_plain; plain_rows_ = pref[d.n_plain];
     auto up = [&](DevBuf<int64_t>& dst, const int64_t* src, int64_t count) {
@@ -575,10 +614,11 @@ class Reverse {
     up(row_, d.row, d.n_rows);
     up(s_ptr_, d.s_ptr, d.n_rows ? d.n_rows + 1 : 0);
     up(s_src_, d.s_src, nnz);
-    up(mu_src_, d.mu_src, d.n_rows);
+    up(mu_src_, d.mu_src, traditional ? 0 : d.n_rows);
     cones_ = std::vector<Cone>(d.n_cones);
     for (int64_t k = 0; k < d.n_cones; ++k) upload_cone(cones_[k], d.cones[k], st);
     CUDA_TRY(cudaStreamSynchronize(st));
+    traditional_ = traditional;
     set_ = true;
   }
 
@@ -604,16 +644,18 @@ class Reverse {
     if (hs) CUDA_TRY(cudaMemsetAsync(s_.p, 0, m_orig_ * sizeof(double), st));
     if (hmu) CUDA_TRY(cudaMemsetAsync(mu_.p, 0, m_orig_ * sizeof(double), st));
     GatherArgs<T> a{n_orig_, n_rows_, n_plain_, plain_rows_, x, s, mu, D, E, c, row_.p, s_ptr_.p, s_src_.p, mu_src_.p,
-                    plain_.p, plain_pref_.p, hx ? x_.p : nullptr, hs ? s_.p : nullptr, hmu ? mu_.p : nullptr};
+                    plain_.p, plain_pref_.p, traditional_ ? 1 : 0, hx ? x_.p : nullptr, hs ? s_.p : nullptr,
+                    hmu ? mu_.p : nullptr};
     gather_kernel<T><<<grid_for(n_orig_ + n_rows_ + plain_rows_), kThreads, 0, st>>>(a);
     CUDA_TRY(cudaGetLastError());
     if (completing) {
       for (const Cone& k : cones_) {
         double* v = mu_.p + k.row_offset;
-        scatter_kernel<<<grid_for(k.N * (k.N + 1) / 2), kThreads, 0, st>>>(k.N, v, k.new_of.p, W_.p);
+        scatter_kernel<<<grid_for(k.N * (k.N + 1) / 2), kThreads, 0, st>>>(k.N, v, k.new_of.p, W_.p, k.square);
         CUDA_TRY(cudaGetLastError());
         complete(k, W_.p, z_.p, cnt_.p, st, device);
-        gather_back_kernel<<<grid_for(k.N * (k.N + 1) / 2), kThreads, 0, st>>>(k.N, k.new_of.p, W_.p, v);
+        gather_back_kernel<<<grid_for(k.square ? k.N * k.N : k.N * (k.N + 1) / 2), kThreads, 0, st>>>(k.N, k.new_of.p, W_.p,
+                                                                                                       v, k.square);
         CUDA_TRY(cudaGetLastError());
       }
     }
@@ -638,7 +680,7 @@ class Reverse {
   double last_ms() const { return last_ms_; }
 
  private:
-  bool set_ = false;
+  bool set_ = false, traditional_ = false;
   int64_t n_orig_ = 0, m_orig_ = 0, n_rows_ = 0, n_plain_ = 0, plain_rows_ = 0;
   DevBuf<int64_t> plain_, plain_pref_, row_, s_ptr_, s_src_, mu_src_;
   std::vector<Cone> cones_;

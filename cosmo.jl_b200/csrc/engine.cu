@@ -180,7 +180,7 @@ class EngineBase {
   virtual void infeasibility_test(int which, const void* delta, double* out8) = 0;
   virtual void psd_lambda_max(const void* v, double* lam) = 0;
   virtual void ldl_stats(double* out8) = 0;
-  virtual void set_decomposition(const cosmo_b200_decomposition* d) = 0;
+  virtual void set_decomposition(const cosmo_b200_decomposition* d, bool traditional) = 0;
   virtual void set_forward_map(const cosmo_b200_forward_map* f) = 0;
   virtual void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
                                         const void* b) = 0;
@@ -224,7 +224,7 @@ class Engine : public EngineBase {
   void infeasibility_test(int which, const void* delta, double* out8) override;
   void psd_lambda_max(const void* v, double* lam) override;
   void ldl_stats(double* out8) override;
-  void set_decomposition(const cosmo_b200_decomposition* d) override;
+  void set_decomposition(const cosmo_b200_decomposition* d, bool traditional) override;
   void set_forward_map(const cosmo_b200_forward_map* f) override;
   void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
                                 const void* b) override;
@@ -2663,11 +2663,11 @@ void Engine<T>::psd_lambda_max(const void* v, double* lam) {
 }
 
 template <typename T>
-void Engine<T>::set_decomposition(const cosmo_b200_decomposition* d) {
+void Engine<T>::set_decomposition(const cosmo_b200_decomposition* d, bool traditional) {
   if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "set_decomposition: the reverse of a decomposition is single-GPU"};
   CUDA_TRY(cudaSetDevice(device_));
   if (!d) rev_.clear();
-  else rev_.set(*d, n_, m_, stream_);
+  else rev_.set(*d, n_, m_, stream_, traditional);   // either map replaces the other
 }
 
 template <typename T>
@@ -2874,7 +2874,10 @@ int cosmo_b200_comm_p2p_attach(cosmo_b200_handle* h, const void* blobs, int32_t 
 }
 
 int cosmo_b200_set_decomposition(cosmo_b200_handle* h, const cosmo_b200_decomposition* d) {
-  ABI_GUARD(h, h->impl->set_decomposition(d));
+  ABI_GUARD(h, h->impl->set_decomposition(d, false));
+}
+int cosmo_b200_set_decomposition_noncompact(cosmo_b200_handle* h, const cosmo_b200_decomposition* d) {
+  ABI_GUARD(h, h->impl->set_decomposition(d, true));
 }
 int cosmo_b200_set_forward_map(cosmo_b200_handle* h, const cosmo_b200_forward_map* f) {
   ABI_GUARD(h, h->impl->set_forward_map(f));

@@ -133,7 +133,8 @@ EXPORTS = [
     "cosmo_b200_tc_gemm_test", "cosmo_b200_psd_stats", "cosmo_b200_get_scaling",
     "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats", "cosmo_b200_infeasibility_test",
     "cosmo_b200_psd_lambda_max", "cosmo_b200_ldl_stats", "cosmo_b200_ldl_symbolic",
-    "cosmo_b200_set_decomposition", "cosmo_b200_reverse_decomposition", "cosmo_b200_psd_complete",
+    "cosmo_b200_set_decomposition", "cosmo_b200_set_decomposition_noncompact", "cosmo_b200_reverse_decomposition",
+    "cosmo_b200_psd_complete",
     "cosmo_b200_set_forward_map", "cosmo_b200_update_matrices_original",
 ]
 
@@ -193,6 +194,7 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_tc_gemm_test.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32,
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]
     lib.cosmo_b200_set_decomposition.argtypes = [vp, C.POINTER(DecompositionStruct)]
+    lib.cosmo_b200_set_decomposition_noncompact.argtypes = [vp, C.POINTER(DecompositionStruct)]
     lib.cosmo_b200_reverse_decomposition.argtypes = [vp, C.c_int32, vp, vp, vp, i64p]
     lib.cosmo_b200_psd_complete.argtypes = [C.c_int64, C.POINTER(CompletionStruct), vp, i64p]
     lib.cosmo_b200_set_forward_map.argtypes = [vp, C.POINTER(ForwardMapStruct)]
@@ -502,7 +504,8 @@ class Engine:
 
     # ---- reverse of a chordal decomposition ---------------------------------
     def set_decomposition(self, d):
-        """cosmo_b200_set_decomposition: hand over the map of a chordal.DecompositionArrays (None clears it)."""
+        """cosmo_b200_set_decomposition, or cosmo_b200_set_decomposition_noncompact for the map of the traditional
+        transformation (d.traditional): hand over the map of a chordal.DecompositionArrays (None clears it)."""
         if d is None:
             self._check(self._lib.cosmo_b200_set_decomposition(self._h, None))
             self.n_orig, self.m_orig = 0, 0
@@ -515,8 +518,9 @@ class Engine:
         ds = DecompositionStruct(int(d.n_orig), int(d.m_orig), int(d.n), int(d.m),
                                  np.asarray(d.plain).reshape(-1, 3).shape[0], _i64(d.plain, keep),
                                  len(d.row), _i64(d.row, keep), _i64(sptr, keep), _i64(d.s_src, keep),
-                                 _i64(d.mu_src, keep), len(d.cones), C.cast(cones, C.c_void_p))
-        self._check(self._lib.cosmo_b200_set_decomposition(self._h, C.byref(ds)))
+                                 None if d.traditional else _i64(d.mu_src, keep), len(d.cones), C.cast(cones, C.c_void_p))
+        setter = self._lib.cosmo_b200_set_decomposition_noncompact if d.traditional else self._lib.cosmo_b200_set_decomposition
+        self._check(setter(self._h, C.byref(ds)))
         self.n_orig, self.m_orig = int(d.n_orig), int(d.m_orig)
 
     def reverse_decomposition(self, complete_dual=False, x=True, s=True, mu=True):

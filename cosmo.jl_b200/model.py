@@ -259,12 +259,13 @@ class Settings:
     #                                                                                   ("AccuracyActivation", tol)
     safeguard: bool = True
     safeguard_tol: float = 2.0
-    # chordal decomposition of PsdConeTriangle constraints (settings.jl:50-53,129-135; host side, chordal.py).
+    # chordal decomposition of PsdConeTriangle and PsdCone constraints (settings.jl:50-53,129-135; host side, chordal.py).
     # The reference defaults to decompose = true with CliqueGraphMerge; here it is opt-in.
     decompose: bool = False
     merge_strategy: str = "CliqueGraphMerge"   # "NoMerge" | "ParentChildMerge" | "CliqueGraphMerge"
     complete_dual: bool = False
-    compact_transformation: bool = True         # the only transformation restated
+    compact_transformation: bool = True         # False: the traditional transformation A' = [A H; 0 -I], which also
+    #                                             decomposes square PsdCone constraints
     # engine-specific: reverse the decomposition (reverse_scaling!, reverse_decomposition!, psd_completion!) on the
     # device from the iterates the solve left there, instead of chordal.reverse on the host
     reverse_on_device: bool = False
@@ -644,13 +645,12 @@ class Model:
             P0, q0, A0, b0, sets0 = self.P0, self.q0, self.A0, self.b0, self.sets0
             if st.decompose:
                 from . import chordal as _chordal
-                if not st.compact_transformation:
-                    raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "only compact_transformation = true is implemented")
                 merge = {"NoMerge": "none", "ParentChildMerge": "parent_child_reference",
                          "CliqueGraphMerge": "clique_graph"}.get(st.merge_strategy)
                 if merge is None:
                     raise ValueError("unknown merge_strategy %r" % (st.merge_strategy,))
-                P2, q2, A2, b2, sets2, info = _chordal.decompose(P0, q0, A0, b0, sets0, merge=merge)
+                P2, q2, A2, b2, sets2, info = _chordal.decompose(P0, q0, A0, b0, sets0, merge=merge,
+                                                                 compact=st.compact_transformation)
                 if info.blocks:                   # at least one cone was decomposed
                     self._dec = info
                     P0, q0, A0, b0, sets0 = P2, q2, A2, b2, sets2

@@ -351,7 +351,8 @@ int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* prob, int64_t* perm, int64
 typedef struct {
   int64_t N;               /* side of the matrix */
   int64_t row_offset;      /* first row of the cone in the original problem (cosmo_b200_psd_complete ignores it) */
-  int64_t dim;             /* rows of the cone: N(N+1)/2 (PsdConeTriangle); a square PsdCone (N*N) is not supported */
+  int64_t dim;             /* rows of the cone: N(N+1)/2 (PsdConeTriangle); a square PsdCone (N*N) only in the map of
+                              cosmo_b200_set_decomposition_noncompact */
   const int64_t* new_of;   /* N: traversal position of every vertex, a permutation of 0..N-1 */
   int64_t n_steps;
   const int64_t* steps;    /* 6 * n_steps */
@@ -373,7 +374,7 @@ typedef struct {
   const int64_t* s_ptr;    /* n_rows + 1, s_ptr[0] = 0, every list non-empty */
   const int64_t* s_src;    /* s_ptr[n_rows] rows of the decomposed problem */
   const int64_t* mu_src;   /* n_rows */
-  int64_t n_cones;         /* decomposed cones (PsdConeTriangle) */
+  int64_t n_cones;         /* decomposed cones (PsdConeTriangle; PsdCone too in the traditional map) */
   const cosmo_b200_completion* cones;
 } cosmo_b200_decomposition;
 
@@ -381,6 +382,15 @@ typedef struct {
    COSMO_B200_ERR_INVALID; a cone with the square PsdCone layout (dim = N*N) and a sharded handle (nranks > 1) return
    COSMO_B200_ERR_UNSUPPORTED. */
 int cosmo_b200_set_decomposition(cosmo_b200_handle* h, const cosmo_b200_decomposition* d);
+/* The map of the traditional transformation (compact_transformation = false: A' = [A H; 0 -I], b' = [b; 0], s = H s'
+   and mu = H mu' divided by each row's overlap count, chordal_decomposition.jl:136-168), in the same struct with two
+   differences: mu_src must be NULL, and original row row[i] gets mu = (0.0 + mu'[s_src[s_ptr[i]]] + ... +
+   mu'[s_src[s_ptr[i+1]-1]]) / (s_ptr[i+1] - s_ptr[i]); a cone may have the square PsdCone layout (dim = N*N, column-major,
+   completed from its upper triangle and written back to all N*N entries).  Plain blocks point into the rows below m_orig
+   (m_orig + the column of H), and their rows are 0.0 + the row, as H s' gives them.  The same checks and errors as
+   cosmo_b200_set_decomposition; setting either map replaces the other, and cosmo_b200_reverse_decomposition runs the one
+   that is set. */
+int cosmo_b200_set_decomposition_noncompact(cosmo_b200_handle* h, const cosmo_b200_decomposition* d);
 /* reverse_scaling! + reverse_decomposition! (+ psd_completion! when complete_dual != 0) of the x, s, mu that the last
    cosmo_b200_solve left on the device: x = D x', s = s' / E, mu = (E mu') / c widened to fp64, then the map.  Writes x
    (n_orig), s and mu (m_orig) in fp64 into caller buffers; NULL skips a buffer (a NULL mu skips the completion).
