@@ -4,8 +4,8 @@ The directory is named ``cosmo.jl_b200`` (not importable as written); the
 top-level shim ``cosmo_b200.py`` registers it under the name ``cosmo_b200``.
 """
 from .engine import Engine, EngineError, default_settings, load_library, nccl_unique_id  # noqa: F401
-from .model import (Box, ComplexPsdConeTriangle, Constraint, DualExponentialCone, DualPowerCone, ExponentialCone, Model,  # noqa: F401
-                    Nonnegatives, PowerCone, PsdCone, PsdConeTriangle, Result, ResultInfo, SecondOrderCone, Settings,
+from .model import (Box, ComplexPsdConeTriangle, Constraint, CustomCone, CustomConeType, DualExponentialCone,  # noqa: F401
+                    DualPowerCone, ExponentialCone, Model, Nonnegatives, PowerCone, PsdCone, PsdConeTriangle, Result, ResultInfo, SecondOrderCone, Settings,
                     ZeroSet, assemble, optimize, ruiz_equilibrate)
 from . import problems  # noqa: F401
 from . import sharding  # noqa: F401,E402

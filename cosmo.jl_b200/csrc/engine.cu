@@ -37,6 +37,7 @@
 #include "chordal_rev.cuh"
 #include "chordal_fwd.cuh"
 #include "mat_update.cuh"
+#include "custom_cone.cuh"
 
 namespace cosmo {
 
@@ -185,6 +186,7 @@ class EngineBase {
   virtual void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
                                         const void* b) = 0;
   virtual void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) = 0;
+  virtual void custom_cone_stats(int64_t* out4) = 0;
 };
 
 template <typename T>
@@ -229,6 +231,9 @@ class Engine : public EngineBase {
   void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
                                 const void* b) override;
   void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) override;
+  void custom_cone_stats(int64_t* out4) override {
+    out4[0] = (int64_t)cust_types_.size(); out4[1] = n_cust_; out4[2] = cust_compiled_; out4[3] = cust_hits_;
+  }
 
  private:
   // ---- problem ----
@@ -263,6 +268,14 @@ class Engine : public EngineBase {
   Cone3Table<T> c3_table() const {
     return Cone3Table<T>{n_c3_, c3_off_.p, c3_kind_.p, c3_alpha_.p, c3_maxit_.p, c3_tol_.p};
   }
+  // custom cones (custom_cone.cuh): one table of all of them, grouped by type; one slice of it per type
+  std::vector<custom::TypeSlice> cust_types_;
+  int n_cust_ = 0;
+  DevBuf<int> cust_off_, cust_dim_, cust_flag_;
+  DevBuf<T> cust_params_, cust_tmp_;
+  long long cust_compiled_ = 0, cust_hits_ = 0;   // types this create compiled / found in the process-wide cache
+  void custom_project(const T* ws);
+  void custom_certificates(const T* v, T eps, int which);
   // ---- accelerator (aa.cuh) ----
   DevBuf<T> aaG_, aaQ_, aaR_, aa_eta_, aa_glast_, aa_f_, aa_flast_, aa_sc_;
   PinnedBuf<T> h_aa_;          // mirror of aa_sc_
@@ -431,7 +444,7 @@ class Engine : public EngineBase {
   bool adapt_rho(const T* x);
   bool primal_infeasible();
   bool dual_infeasible();
-  int cone_certificates(const T* v, T eps);
+  int cone_certificates(const T* v, T eps, int which);
   double inf_rec_[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // what the last primal_infeasible / dual_infeasible computed
   void recover_mu(const T* w_prev) {
     recover_mu_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_vec_.p, w_prev + n_, s_.p, mu_.p);
@@ -782,6 +795,10 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   std::vector<int> c3_off, c3_maxit;
   std::vector<unsigned char> c3_kind;
   std::vector<T> c3_alpha, c3_tol;
+  std::map<custom::Key, int> cust_index;           // type -> position in cust_keys (first appearance order)
+  std::vector<custom::Key> cust_keys;
+  std::vector<std::vector<int>> cust_off, cust_dim;
+  std::vector<std::vector<T>> cust_par;
   for (long long k = 0; k < p.n_sets; ++k) {
     const cosmo_b200_set& sdesc = p.sets[k];
     if (sdesc.dim < 0 || off + sdesc.dim > m_) throw EngineError{COSMO_B200_ERR_INVALID, "set dimensions exceed m"};
@@ -850,6 +867,28 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
         c3_alpha.push_back(is_pow ? (T)sdesc.alpha : T(0.5));
         c3_maxit.push_back(sdesc.max_iter > 0 ? sdesc.max_iter : (is_pow ? 20 : 100));   // convexset.jl:503, 631
         c3_tol.push_back(sdesc.tol > 0.0 ? (T)sdesc.tol : (T)1e-8);
+        break;
+      }
+      case COSMO_B200_CUSTOM: {
+        cls = ROW_CUSTOM;
+        const custom::Key key = custom::make_key(static_cast<const cosmo_b200_custom_cone*>(sdesc.u),
+                                                 sizeof(T) == sizeof(double) ? COSMO_B200_F64 : COSMO_B200_F32);
+        if (key.n_params > 0 && !sdesc.l)
+          throw EngineError{COSMO_B200_ERR_INVALID, "custom cone " + key.name + ": n_params > 0 but the set has no parameters (l)"};
+        if (sdesc.alpha != 0.0 || sdesc.tol != 0.0 || sdesc.max_iter != 0)
+          throw EngineError{COSMO_B200_ERR_INVALID, "custom cone " + key.name + ": alpha, tol and max_iter must be 0"};
+        if (sdesc.dim == 0) break;
+        auto it = cust_index.find(key);
+        const int t = it != cust_index.end() ? it->second : (int)cust_keys.size();
+        if (it == cust_index.end()) {
+          cust_index[key] = t;
+          cust_keys.push_back(key);
+          cust_off.emplace_back(); cust_dim.emplace_back(); cust_par.emplace_back();
+        }
+        cust_off[t].push_back((int)off);
+        cust_dim[t].push_back((int)sdesc.dim);
+        const T* par = static_cast<const T*>(sdesc.l);
+        cust_par[t].insert(cust_par[t].end(), par, par + key.n_params);
         break;
       }
       default:
@@ -939,6 +978,29 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   if (n_c3_) {
     c3_off_.upload(c3_off, stream_); c3_kind_.upload(c3_kind, stream_); c3_alpha_.upload(c3_alpha, stream_);
     c3_maxit_.upload(c3_maxit, stream_); c3_tol_.upload(c3_tol, stream_);
+    sync();
+  }
+  // custom cones: compile (or find) and load every type, then one table of all cones, type by type
+  if (!cust_keys.empty()) {
+    std::vector<int> offs, dims;
+    std::vector<T> pars;
+    for (size_t t = 0; t < cust_keys.size(); ++t) {
+      bool compiled = false;
+      custom::Entry* e = custom::cache().get(cust_keys[t], &compiled);
+      ++(compiled ? cust_compiled_ : cust_hits_);
+      custom::cache().load(e);
+      custom::TypeSlice ts;
+      ts.entry = e; ts.first = (int)offs.size(); ts.n = (int)cust_off[t].size(); ts.param_first = (long long)pars.size();
+      cust_types_.push_back(ts);
+      offs.insert(offs.end(), cust_off[t].begin(), cust_off[t].end());
+      dims.insert(dims.end(), cust_dim[t].begin(), cust_dim[t].end());
+      pars.insert(pars.end(), cust_par[t].begin(), cust_par[t].end());
+    }
+    n_cust_ = (int)offs.size();
+    cust_off_.upload(offs, stream_); cust_dim_.upload(dims, stream_);
+    if (!pars.empty()) cust_params_.upload(pars, stream_);
+    cust_flag_.alloc(n_cust_);
+    cust_tmp_.alloc(m_);
     sync();
   }
   write_values(p.P.nzval, p.A.nzval, p.q, p.b);
@@ -1561,7 +1623,46 @@ void Engine<T>::project_device(const T* w, bool with_rhs, const T* ws_rhs) {
     cone3_project_kernel<T><<<(n_c3_ + 127) / 128, 128, 0, stream_>>>(c3_table(), w + n_, s_.p);
     check_launch("cone3_project");
   }
+  if (n_cust_) custom_project(w + n_);
   launch_proj_rhs(w, ws_rhs ? ws_rhs : w + n_, true, with_rhs);
+}
+
+// s = Pi_K(w_s) on the rows of every custom cone: one launch of the type's compiled projection kernel per type
+template <typename T>
+void Engine<T>::custom_project(const T* ws) {
+  for (const custom::TypeSlice& t : cust_types_) {
+    dim3 grid, block;
+    custom::launch_dims(t.entry->key.granularity, t.n, grid, block);
+    int n = t.n;
+    const int* off = cust_off_.p + t.first;
+    const int* dim = cust_dim_.p + t.first;
+    const T* par = t.entry->key.n_params ? cust_params_.p + t.param_first : nullptr;
+    T* s = s_.p;
+    void* args[] = {&n, &off, &dim, &par, &ws, &s};
+    CUDA_TRY(cudaLaunchKernel((const void*)t.entry->project, grid, block, args, 0, stream_));
+    check_launch("custom_project");
+  }
+}
+
+// The custom-cone certificates on v into SC_TMP6 (1: some cone is not certified): in_dual(-v) for the primal test
+// (which = 0), in_pol_recc(v) for the dual one; a type without the hook certifies none of its cones
+template <typename T>
+void Engine<T>::custom_certificates(const T* v, T eps, int which) {
+  for (const custom::TypeSlice& t : cust_types_) {
+    dim3 grid, block;
+    custom::launch_dims(t.entry->key.granularity, t.n, grid, block);
+    int n = t.n, w = which;
+    const int* off = cust_off_.p + t.first;
+    const int* dim = cust_dim_.p + t.first;
+    const T* par = t.entry->key.n_params ? cust_params_.p + t.param_first : nullptr;
+    T* tmp = cust_tmp_.p;
+    int* flag = cust_flag_.p + t.first;
+    void* args[] = {&n, &off, &dim, &par, &v, &tmp, &eps, &w, &flag};
+    CUDA_TRY(cudaLaunchKernel((const void*)t.entry->cert, grid, block, args, 0, stream_));
+    check_launch("custom_cert");
+  }
+  custom_flag_fold_kernel<T><<<1, kBlock, 0, stream_>>>(n_cust_, cust_flag_.p, sc_.p + SC_TMP6);
+  check_launch("custom_fold");
 }
 
 // c = A' tm + P u + sigma u ; cb[n] = u'c   (second half of reduced_mul!, kktsolver_indirect.jl:61-65)
@@ -1918,7 +2019,7 @@ bool Engine<T>::primal_infeasible() {
   cone_rows_certificate_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, 0, dy_.p, row_class_.p, box_l_.p, box_u_.p, eps, red(SC_TMP1));
   check_launch("cone_cert_primal");
   allreduce_sum(sc_.p + SC_TMP0, 2);   // dy'b, box support sum
-  const bool cone_bad = cone_certificates(dy_.p, eps) != 0;
+  const bool cone_bad = cone_certificates(dy_.p, eps, 0) != 0;
   const double dyt_b = (double)h_sc_[SC_TMP0];
   const double box_sum = (double)h_sc_[SC_TMP1];
   rec[4] = dyt_b;
@@ -1963,17 +2064,18 @@ bool Engine<T>::dual_infeasible() {
   check_launch("scal_Adx");
   cone_rows_certificate_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, 1, vec_m_.p, row_class_.p, box_l_.p, box_u_.p, eps, red(SC_TMP1));
   check_launch("cone_cert_dual");
-  const bool cone_ok = cone_certificates(vec_m_.p, eps) == 0;
+  const bool cone_ok = cone_certificates(vec_m_.p, eps, 1) == 0;
   rec[0] = cone_ok ? 1.0 : 0.0;
   return cone_ok;
 }
 
-// The cone tests of both certificates on v, after the row kernel has set the rows flag in SC_TMP2:
-// SOC (-v in K*  <=>  |v[2:]| <= tol - v[1]) into SC_TMP3, PSD (-V + tol I positive definite) into SC_TMP4, Exp/Pow
-// into SC_TMP5.  Reads SC_TMP0..5 back, records the failed families (rows 1, SOC 2, PSD 4, Exp/Pow 8) and the PSD
-// cones whose eigensolver missed psd_max_sweeps in inf_rec_[6..7], and returns the failed families.
+// The cone tests of both certificates (which = 0: primal, 1: dual) on v, after the row kernel has set the rows flag in
+// SC_TMP2: SOC (-v in K*  <=>  |v[2:]| <= tol - v[1]) into SC_TMP3, PSD (-V + tol I positive definite) into SC_TMP4,
+// Exp/Pow into SC_TMP5, custom cones into SC_TMP6.  Reads SC_TMP0..5 (and 6) back, records the failed families (rows 1,
+// SOC 2, PSD 4, Exp/Pow 8, custom 16) and the PSD cones whose eigensolver missed psd_max_sweeps in inf_rec_[6..7], and
+// returns the failed families.
 template <typename T>
-int Engine<T>::cone_certificates(const T* v, T eps) {
+int Engine<T>::cone_certificates(const T* v, T eps, int which) {
   if (n_soc_) {
     soc_norms(v, soc_norm2_.p);
     soc_cert_kernel<T><<<1, kBlock, 0, stream_>>>(n_soc_, soc_off_.p, soc_norm2_.p, v, eps, sc_.p + SC_TMP3);
@@ -1987,15 +2089,19 @@ int Engine<T>::cone_certificates(const T* v, T eps) {
   } else {
     CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP5, 0, sizeof(T), stream_));
   }
+  // the custom flag joins the allreduce on every rank of a sharded model, whether or not the rank holds custom cones
+  const bool cust_flag = n_cust_ > 0 || nranks_ > 1;
+  if (n_cust_) custom_certificates(v, eps, which);
+  else if (cust_flag) CUDA_TRY(cudaMemsetAsync(sc_.p + SC_TMP6, 0, sizeof(T), stream_));
   const bool psd_ok = psd_.certificate(v, /*negate=*/true, (double)eps, stream_, st_.psd_max_sweeps, launches_);
   // the PSD verdict is a host bool of THIS rank: put it next to the device flags so that the
   // max-allreduce makes every rank take the same decision
   h_sc_[SC_TMP4] = psd_ok ? T(0) : T(1);
   CUDA_TRY(cudaMemcpyAsync(sc_.p + SC_TMP4, h_sc_.p + SC_TMP4, sizeof(T), cudaMemcpyHostToDevice, stream_));
-  allreduce_max(sc_.p + SC_TMP2, 4);   // flags: rows, SOC, PSD, Exp/Pow
-  read_scalars(SC_TMP0, 6);
+  allreduce_max(sc_.p + SC_TMP2, 5);   // flags: rows, SOC, PSD, Exp/Pow, custom
+  read_scalars(SC_TMP0, cust_flag ? 7 : 6);
   const int failed = (h_sc_[SC_TMP2] != 0 ? 1 : 0) + (h_sc_[SC_TMP3] != 0 ? 2 : 0) + (h_sc_[SC_TMP4] != 0 ? 4 : 0) +
-                     (h_sc_[SC_TMP5] != 0 ? 8 : 0);
+                     (h_sc_[SC_TMP5] != 0 ? 8 : 0) + (cust_flag && h_sc_[SC_TMP6] != 0 ? 16 : 0);
   inf_rec_[6] = failed;
   inf_rec_[7] = psd_.cert_unconverged;
   return failed;
@@ -2848,6 +2954,26 @@ int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* p, int64_t* perm, int64_t*
     }
     return COSMO_B200_OK;
   } catch (...) { return error_code(cosmo::g_create_error); }
+}
+int cosmo_b200_custom_cone_compile(const cosmo_b200_custom_cone* type, int32_t dtype, char* log, int64_t log_cap) {
+  if (log && log_cap > 0) log[0] = 0;
+  try {
+    bool compiled = false;
+    cosmo::custom::cache().get(cosmo::custom::make_key(type, dtype), &compiled);
+    return compiled ? 1 : 0;
+  } catch (...) {
+    const int rc = error_code(cosmo::g_create_error);
+    if (log && log_cap > 0) {
+      const size_t k = std::min<size_t>((size_t)log_cap - 1, cosmo::g_create_error.size());
+      memcpy(log, cosmo::g_create_error.data(), k);
+      log[k] = 0;
+    }
+    return rc;
+  }
+}
+int cosmo_b200_custom_cone_stats(cosmo_b200_handle* h, int64_t out[4]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->custom_cone_stats(out));
 }
 int cosmo_b200_comm_unique_id(void* id128) {
   if (!id128) return COSMO_B200_ERR_INVALID;

@@ -31,7 +31,7 @@ enum {
 enum { ISC_DONE = 0, ISC_IT = 1, ISC_MAXIT = 2, ISC_COUNT = 8 };
 
 // cone classes per row
-enum : unsigned char { ROW_ZERO = 0, ROW_NONNEG = 1, ROW_BOX = 2, ROW_SOC = 3, ROW_PSD = 4, ROW_CONE3 = 5 };
+enum : unsigned char { ROW_ZERO = 0, ROW_NONNEG = 1, ROW_BOX = 2, ROW_SOC = 3, ROW_PSD = 4, ROW_CONE3 = 5, ROW_CUSTOM = 6 };
 
 template <typename T>
 struct SocTable {          // one entry per SecondOrderCone
@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(kBlock) proj_rhs_kernel(ProjRhsArgs<T> a) {
         else if (nx <= -t) sv = T(0);
         else sv = (r == off) ? (nx + t) / T(2) : (nx + t) / (T(2) * nx) * ws;
       } else {
-        sv = a.s[r];   // PSD and Exp/Pow rows: projected by their own kernels beforehand
+        sv = a.s[r];   // PSD, Exp/Pow and custom rows: projected by their own kernels beforehand
       }
       a.s[r] = sv;
     } else {
@@ -130,7 +130,7 @@ __device__ __forceinline__ T proj_row_scalar(const ProjRhsArgs<T>& a, int r, T w
     if (nx <= -t) return T(0);
     return (r == off) ? (nx + t) / T(2) : (nx + t) / (T(2) * nx) * ws;
   }
-  return a.s[r];   // PSD and Exp/Pow rows: projected by their own kernels beforehand
+  return a.s[r];   // PSD, Exp/Pow and custom rows: projected by their own kernels beforehand
 }
 
 __global__ void __launch_bounds__(kBlock) proj_rhs_vec2_kernel(ProjRhsArgs<double> a) {

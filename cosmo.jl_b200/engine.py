@@ -18,7 +18,9 @@ from . import build as _build
 OK = 0
 ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_ALLOC, ERR_NCCL, ERR_NUMERICAL = -1, -2, -3, -4, -5, -6
 F64, F32 = 0, 1
-ZERO, NONNEG, BOX, SOC, PSD_SQUARE, PSD_TRIANGLE, EXP, DUAL_EXP, POW, DUAL_POW, PSD_TRIANGLE_COMPLEX = range(11)
+ZERO, NONNEG, BOX, SOC, PSD_SQUARE, PSD_TRIANGLE, EXP, DUAL_EXP, POW, DUAL_POW, PSD_TRIANGLE_COMPLEX, CUSTOM = range(12)
+CUSTOM_THREAD, CUSTOM_WARP, CUSTOM_BLOCK = 0, 1, 2
+CUSTOM_HAS_IN_DUAL, CUSTOM_HAS_IN_POL_RECC = 1, 2
 STATUS = {0: "Undetermined", 1: "Solved", 2: "Max_iter_reached", 3: "Time_limit_reached",
           4: "Primal_infeasible", 5: "Dual_infeasible", 6: "Unsolved"}
 KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES, KKT_LDL = 0, 1, 2, 3
@@ -43,6 +45,12 @@ class CscStruct(C.Structure):
 class SetStruct(C.Structure):
     _fields_ = [("type", C.c_int32), ("max_iter", C.c_int32), ("dim", C.c_int64), ("l", C.c_void_p), ("u", C.c_void_p),
                 ("alpha", C.c_double), ("tol", C.c_double)]
+
+
+class CustomConeStruct(C.Structure):
+    """cosmo_b200_custom_cone: a cone type whose device functions the engine compiles (include/cosmo_b200.h)."""
+    _fields_ = [("name", C.c_char_p), ("source", C.c_char_p), ("granularity", C.c_int32), ("n_params", C.c_int32),
+                ("flags", C.c_int32), ("reserved", C.c_int32)]
 
 
 class ProblemStruct(C.Structure):
@@ -136,6 +144,7 @@ EXPORTS = [
     "cosmo_b200_set_decomposition", "cosmo_b200_set_decomposition_noncompact", "cosmo_b200_reverse_decomposition",
     "cosmo_b200_psd_complete",
     "cosmo_b200_set_forward_map", "cosmo_b200_update_matrices_original",
+    "cosmo_b200_custom_cone_compile", "cosmo_b200_custom_cone_stats",
 ]
 
 _lib = None
@@ -199,12 +208,54 @@ def load_library(rebuild_if_stale=True):
     lib.cosmo_b200_psd_complete.argtypes = [C.c_int64, C.POINTER(CompletionStruct), vp, i64p]
     lib.cosmo_b200_set_forward_map.argtypes = [vp, C.POINTER(ForwardMapStruct)]
     lib.cosmo_b200_update_matrices_original.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, vp]
+    lib.cosmo_b200_custom_cone_compile.argtypes = [C.POINTER(CustomConeStruct), C.c_int32, C.c_char_p, C.c_int64]
+    lib.cosmo_b200_custom_cone_stats.argtypes = [vp, i64p]
     for name in EXPORTS:
         fn = getattr(lib, name)
         if name not in ("cosmo_b200_destroy", "cosmo_b200_last_error"):
             fn.restype = C.c_int
     _lib = lib
     return lib
+
+
+_nvrtc_ready = False
+
+
+def preload_nvrtc():
+    """Make libnvrtc.so.12 loadable for the engine's dlopen: the system's copy when the loader finds one, else the copy
+    of the `nvidia-cuda-nvrtc` wheel that PyTorch installs, loaded with RTLD_GLOBAL so that the engine's
+    dlopen("libnvrtc.so.12") finds it by its soname.  Without either, custom cones fail with ERR_UNSUPPORTED."""
+    global _nvrtc_ready
+    if _nvrtc_ready:
+        return
+    try:
+        C.CDLL("libnvrtc.so.12", mode=C.RTLD_GLOBAL)
+    except OSError:
+        try:
+            import nvidia.cuda_nvrtc as _w
+        except ImportError:
+            return
+        for d in _w.__path__:
+            path = os.path.join(d, "lib", "libnvrtc.so.12")
+            if os.path.exists(path):
+                C.CDLL(path, mode=C.RTLD_GLOBAL)
+                break
+        else:
+            return
+    _nvrtc_ready = True
+
+
+def custom_cone_compile(cone_struct: CustomConeStruct, dtype=np.float64) -> bool:
+    """cosmo_b200_custom_cone_compile: check and compile a cone type for `dtype` (no device needed).  True when this
+    call compiled it, False when it was in the process-wide cache; EngineError with the compiler log otherwise."""
+    lib = load_library()
+    preload_nvrtc()
+    log = C.create_string_buffer(1 << 16)
+    rc = lib.cosmo_b200_custom_cone_compile(C.byref(cone_struct), F64 if np.dtype(dtype) == np.float64 else F32, log,
+                                            len(log))
+    if rc < 0:
+        raise EngineError(rc, log.value.decode(errors="replace"))
+    return rc == 1
 
 
 def default_settings() -> SettingsStruct:
@@ -272,6 +323,17 @@ class Engine:
         for i, (typ, dim, l, u, *extra) in enumerate(sets):
             set_arr[i].type = int(typ)
             set_arr[i].dim = int(dim)
+            if typ == CUSTOM:
+                # u: the cone type (anything with a `struct()` -> CustomConeStruct, model.CustomConeType), l: parameters
+                preload_nvrtc()
+                cs = u.struct()
+                keep.append(cs)
+                set_arr[i].u = C.cast(C.pointer(cs), C.c_void_p)
+                if l is not None and len(l):
+                    pa = np.ascontiguousarray(l, dtype=T)
+                    keep.append(pa)
+                    set_arr[i].l = _ptr(pa)
+                continue
             if extra and extra[0]:
                 set_arr[i].alpha = float(extra[0].get("alpha", 0.0))
                 set_arr[i].max_iter = int(extra[0].get("max_iter", 0))
@@ -468,6 +530,12 @@ class Engine:
         keys = ("tc_projections", "tc_fallbacks", "tc_last_steps", "tc_last_checks", None, None, "jacobi_last_sweeps", "tc_slices")
         return {k: int(v) for k, v in zip(keys, out) if k}
 
+    def custom_cone_stats(self):
+        """cosmo_b200_custom_cone_stats, keyed by CUSTOM_CONE_STATS."""
+        out = (C.c_int64 * 4)()
+        self._check(self._lib.cosmo_b200_custom_cone_stats(self._h, out))
+        return dict(zip(CUSTOM_CONE_STATS, [int(v) for v in out]))
+
     def accelerator_stats(self):
         """Accelerator events of the last solve (cosmo_b200_accelerator_stats), keyed by ACCELERATOR_STATS."""
         out = (C.c_int64 * 6)()
@@ -576,9 +644,11 @@ def psd_complete(Y, schedule):
 
 
 # cosmo_b200_infeasibility_test's out[8]: "gate2" is |Dinv A'dy|_inf (primal) or q'dx (dual), "gate3" dy'b of the
-# normalized -dy (primal) or |Dinv P dx|_inf (dual); "families" has bit 0 rows, 1 SOC, 2 PSD, 3 Exp/Pow
+# normalized -dy (primal) or |Dinv P dx|_inf (dual); "families" has bit 0 rows, 1 SOC, 2 PSD, 3 Exp/Pow, 4 custom cones
 INFEASIBILITY_RECORD = ("verdict", "gate", "norm", "gate2", "gate3", "box_sum", "families", "psd_unconverged")
-FAMILY_ROWS, FAMILY_SOC, FAMILY_PSD, FAMILY_C3 = 1, 2, 4, 8
+FAMILY_ROWS, FAMILY_SOC, FAMILY_PSD, FAMILY_C3, FAMILY_CUSTOM = 1, 2, 4, 8, 16
+
+CUSTOM_CONE_STATS = ("types", "cones", "compilations", "cache_hits")
 
 LDL_STATS = ("N", "nnz_triu_K", "nnz_L", "levels", "solve_nodes", "factorizations", "factor_time", "symbolic_time")
 

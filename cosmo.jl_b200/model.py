@@ -147,8 +147,50 @@ class DualPowerCone(PowerCone):
     code = _eng.DUAL_POW
 
 
-# cones whose rows may only be scaled by one common factor (rectify_scaling!, convexset.jl:955-957)
-SCALAR_SCALED_CONES = (SecondOrderCone, PsdCone, PsdConeTriangle, ComplexPsdConeTriangle, ExponentialCone, PowerCone)
+class CustomConeType:
+    """A user-defined cone type: the counterpart of `struct MyCone{T} <: COSMO.AbstractConvexCone{T}` with its
+    `project!` (and optionally `in_dual` / `in_pol_recc`) methods, written as CUDA C++ device templates in namespace
+    `name` (the contract is in include/cosmo_b200.h at COSMO_B200_CUSTOM).  The engine compiles it for sm_90a when an
+    engine that uses it is created, once per process and dtype.  granularity: "thread" (one lane per cone), "warp"
+    (32 lanes) or "block" (256 lanes); n_params: values per cone; in_dual / in_pol_recc: whether `source` defines the
+    certificate hooks (without them the infeasibility checks never certify, as the reference's documentation says)."""
+    _GRAN = {"thread": _eng.CUSTOM_THREAD, "warp": _eng.CUSTOM_WARP, "block": _eng.CUSTOM_BLOCK}
+
+    def __init__(self, name: str, source: str, granularity: str = "warp", n_params: int = 0, in_dual: bool = False,
+                 in_pol_recc: bool = False):
+        if granularity not in self._GRAN:
+            raise ValueError("granularity must be one of %s" % sorted(self._GRAN))
+        self.name, self.source, self.granularity = str(name), str(source), granularity
+        self.n_params, self.in_dual, self.in_pol_recc = int(n_params), bool(in_dual), bool(in_pol_recc)
+        self._bytes = (self.name.encode(), self.source.encode())   # what struct() points to, alive with the type
+
+    def struct(self) -> "_eng.CustomConeStruct":
+        flags = (_eng.CUSTOM_HAS_IN_DUAL if self.in_dual else 0) | (_eng.CUSTOM_HAS_IN_POL_RECC if self.in_pol_recc else 0)
+        return _eng.CustomConeStruct(self._bytes[0], self._bytes[1], self._GRAN[self.granularity], self.n_params, flags, 0)
+
+    def compile(self, dtype=np.float64) -> bool:
+        """Compile for `dtype` without a device (True: compiled now, False: found in the cache)."""
+        return _eng.custom_cone_compile(self.struct(), dtype)
+
+
+class CustomCone(AbstractConvexSet):
+    """A cone of a CustomConeType, `dim` rows, with the type's n_params parameters (never scaled: scale! of a custom
+    cone is a no-op in the reference)."""
+    code = _eng.CUSTOM
+
+    def __init__(self, kind: CustomConeType, dim, params=()):
+        if dim < 0:
+            raise ValueError("dimension must be nonnegative")
+        self.kind, self.dim = kind, int(dim)
+        self.params = np.array(params, dtype=np.float64).ravel()
+        if self.params.size != kind.n_params:
+            raise ValueError("the cone type %s takes %d parameters, got %d" % (kind.name, kind.n_params, self.params.size))
+
+
+# cones whose rows may only be scaled by one common factor (rectify_scaling!, convexset.jl:952-957; a custom cone takes
+# the reference's conservative fall-back, convexset.jl:952-953)
+SCALAR_SCALED_CONES = (SecondOrderCone, PsdCone, PsdConeTriangle, ComplexPsdConeTriangle, ExponentialCone, PowerCone,
+                       CustomCone)
 # cones that cannot be split across ranks
 ATOMIC_CONES = SCALAR_SCALED_CONES
 
@@ -157,6 +199,8 @@ def set_tuple(S):
     """The (type, dim, l, u[, params]) tuple `engine.Engine` marshals into a cosmo_b200_set."""
     if isinstance(S, (ExponentialCone, PowerCone)):
         return (S.code, 3, None, None, {"alpha": getattr(S, "alpha", 0.0), "max_iter": S.MAX_ITER, "tol": S.TOL})
+    if isinstance(S, CustomCone):
+        return (S.code, S.dim, S.params, S.kind)
     return (S.code, S.dim, getattr(S, "l", None), getattr(S, "u", None))
 
 

@@ -75,6 +75,43 @@ enum {
                                           memory up to N = 48, through the large-cone path (tensor cores) beyond */
 };
 
+/* ---- custom convex cones (the reference's `AbstractConvexCone` subtypes with a `project!` method) --------------------
+   A set with type = COSMO_B200_CUSTOM is projected by CUDA C++ that the user writes.  Its cosmo_b200_set has
+   u = the const cosmo_b200_custom_cone* of its type, l = its n_params parameters in the model's element type T (NULL when
+   n_params = 0; never scaled, as scale! of a custom cone is a no-op), alpha = tol = max_iter = 0.  The engine compiles
+   each type with NVRTC (libnvrtc.so.12, loaded with dlopen on first use: without it create returns
+   COSMO_B200_ERR_UNSUPPORTED) for sm_90a when the engine is created, once per process for each (name, source,
+   granularity, n_params, flags, dtype), and launches the projection inside admm_z! after the built-in cones.
+   Custom cones sort with the exponential and power cones (class 6), take one scalar scaling per cone (Ruiz) and the
+   inequality rho.  `source` defines, in namespace `name`,
+     template <typename T> __device__ void project(T* x, long long dim, const T* p, int lane, int width);
+     template <typename T> __device__ bool in_dual(const T* x, long long dim, T tol, const T* p, int lane, int width);
+     template <typename T> __device__ bool in_pol_recc(const T* x, long long dim, T tol, const T* p, int lane, int width);
+   the last two only when flags has COSMO_B200_CUSTOM_HAS_IN_DUAL / _HAS_IN_POL_RECC.  All `width` lanes of a cone call a
+   function together (lane = 0 .. width-1); x is the cone's `dim` rows, p its parameters.  project overwrites x (which
+   holds w_s) with its projection.  The primal infeasibility certificate asks in_dual(-dy) and the dual one
+   in_pol_recc(A dx) (convexset.jl:928-936); a cone is certified when every lane returns true.  A type without the hook
+   never certifies, so such a problem runs to Max_iter_reached where the reference would raise a MethodError (its
+   documentation calls this "infeasibility detection is disabled").  No #include is needed: a prelude defines, in
+   namespace cosmo_cone, sum(v, width), max(v, width) and all(b, width) over the lanes of a cone, which every lane of
+   the cone must call. */
+#define COSMO_B200_CUSTOM 11 /* cosmo_b200_set.type */
+enum {
+  COSMO_B200_CUSTOM_THREAD = 0, /* one lane per cone */
+  COSMO_B200_CUSTOM_WARP = 1,   /* 32 lanes: one warp per cone */
+  COSMO_B200_CUSTOM_BLOCK = 2   /* 256 lanes: one thread block per cone */
+};
+#define COSMO_B200_CUSTOM_HAS_IN_DUAL 1
+#define COSMO_B200_CUSTOM_HAS_IN_POL_RECC 2
+typedef struct {
+  const char* name;    /* C identifier: the namespace of the device functions in `source` (not "cosmo_cone") */
+  const char* source;  /* CUDA C++; compiler messages name its lines as `name`(line) */
+  int32_t granularity; /* COSMO_B200_CUSTOM_THREAD | _WARP | _BLOCK */
+  int32_t n_params;    /* values of T per cone */
+  int32_t flags;       /* COSMO_B200_CUSTOM_HAS_* */
+  int32_t reserved;    /* 0 */
+} cosmo_b200_custom_cone;
+
 /* status (src/solver.jl:113,161,175,311-353) */
 enum {
   COSMO_B200_UNDETERMINED = 0,
@@ -312,7 +349,7 @@ int cosmo_b200_get_w(cosmo_b200_handle* h, void* w);
    out = {verdict (1: infeasible), last gate reached (1: norm, 2: A'dy resp. q'dx, 3: P dx (dual only), 4: cone tests),
           |E dy|_inf resp. |D dx|_inf, |Dinv A'dy|_inf resp. q'dx, dy'b of the normalized -dy resp. |Dinv P dx|_inf,
           Box support sum (primal), failed certificate families (bit 0: Zero/Nonnegatives/Box rows, 1: SOC, 2: PSD,
-          3: Exp/Pow and their duals), PSD cones whose eigensolver missed psd_max_sweeps (counted as not certified)};
+          3: Exp/Pow and their duals, 4: custom cones), PSD cones whose eigensolver missed psd_max_sweeps (counted as not certified)};
    a value that the test did not reach is NaN.  Uses the engine's dx / dy scratch vectors, as cosmo_b200_residuals
    does: call it between solves, not inside one.  With several ranks every rank calls it. */
 int cosmo_b200_infeasibility_test(cosmo_b200_handle* h, int32_t which, const void* delta, double out[8]);
@@ -453,6 +490,17 @@ int cosmo_b200_comm_init(cosmo_b200_handle* h, int32_t nranks, int32_t rank, con
    attach: maps the peers' buffers.  All ranks must be on one NVLink-connected node. */
 int cosmo_b200_comm_p2p_export(cosmo_b200_handle* h, void* blob128);
 int cosmo_b200_comm_p2p_attach(cosmo_b200_handle* h, const void* blobs, int32_t nranks);
+
+/* ---- custom cones --------------------------------------------------------- */
+/* Checks the descriptor and compiles the type for dtype (COSMO_B200_F64 | _F32) into the process-wide cache, or finds it
+   there; no device is needed.  A bad descriptor (name not an identifier, unknown granularity or flag, reserved != 0,
+   n_params < 0, no source) or a compile error: COSMO_B200_ERR_INVALID, with the NVRTC log (the user's lines as
+   `name`(line)) in cosmo_b200_last_error(NULL) and, truncated to log_cap bytes with a terminating 0, in `log` when it is
+   not NULL.  No libnvrtc.so.12: COSMO_B200_ERR_UNSUPPORTED.  Returns 1 instead of 0 when the call compiled. */
+int cosmo_b200_custom_cone_compile(const cosmo_b200_custom_cone* type, int32_t dtype, char* log, int64_t log_cap);
+/* out = {custom cone types, custom cones of this handle, compilations its create caused, types its create found in the
+   cache} */
+int cosmo_b200_custom_cone_stats(cosmo_b200_handle* h, int64_t out[4]);
 
 /* ---- diagnostics ---------------------------------------------------------- */
 /* Which path projected the large PSD cones (N > 96) so far: out = {tensor-core projections, tensor-core fallbacks to
