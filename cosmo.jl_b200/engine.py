@@ -115,6 +115,72 @@ class ForwardMapStruct(C.Structure):
                 ("b_uncovered", C.c_void_p)]
 
 
+def _signatures():
+    """(restype, argtypes) of every entry point of include/cosmo_b200.h, in the header's order."""
+    vp, i32, i64, f64, P = C.c_void_p, C.c_int32, C.c_int64, C.c_double, C.POINTER
+    rc = C.c_int
+    return {
+        "cosmo_b200_abi_version": (rc, []),
+        "cosmo_b200_default_settings": (rc, [P(SettingsStruct)]),
+        "cosmo_b200_create": (rc, [P(vp), P(ProblemStruct), P(SettingsStruct)]),
+        "cosmo_b200_destroy": (None, [vp]),
+        "cosmo_b200_last_error": (C.c_char_p, [vp]),
+        "cosmo_b200_update_settings": (rc, [vp, P(SettingsStruct)]),
+        "cosmo_b200_warm_start": (rc, [vp, vp, vp, vp]),
+        "cosmo_b200_update_qb": (rc, [vp, vp, vp]),
+        "cosmo_b200_update_matrices": (rc, [vp, vp, i64, vp, i64, vp, vp]),
+        "cosmo_b200_update_rho": (rc, [vp, vp, f64]),
+        "cosmo_b200_reset": (rc, [vp]),
+        "cosmo_b200_set_accelerator": (rc, [vp, P(AcceleratorStruct)]),
+        "cosmo_b200_accelerator_stats": (rc, [vp, P(i64)]),
+        "cosmo_b200_solve": (rc, [vp, P(ResultStruct)]),
+        "cosmo_b200_project": (rc, [vp, vp, vp]),
+        "cosmo_b200_kkt_solve": (rc, [vp, vp, vp, P(i64)]),
+        "cosmo_b200_residuals": (rc, [vp, vp, vp, vp, i32, P(f64)]),
+        "cosmo_b200_spmv": (rc, [vp, i32, vp, vp]),
+        "cosmo_b200_spmv_bench": (rc, [vp, i32, i32, P(f64), P(f64)]),
+        "cosmo_b200_get_rho_vec": (rc, [vp, vp]),
+        "cosmo_b200_get_scaling": (rc, [vp, vp, vp, P(f64)]),
+        "cosmo_b200_get_w": (rc, [vp, vp]),
+        "cosmo_b200_infeasibility_test": (rc, [vp, i32, vp, P(f64)]),
+        "cosmo_b200_psd_lambda_max": (rc, [vp, vp, P(f64)]),
+        "cosmo_b200_ldl_stats": (rc, [vp, P(f64)]),
+        "cosmo_b200_ldl_symbolic": (rc, [P(ProblemStruct), P(i64), P(i64), P(i64), P(i64)]),
+        "cosmo_b200_set_decomposition": (rc, [vp, P(DecompositionStruct)]),
+        "cosmo_b200_set_decomposition_noncompact": (rc, [vp, P(DecompositionStruct)]),
+        "cosmo_b200_reverse_decomposition": (rc, [vp, i32, vp, vp, vp, P(i64)]),
+        "cosmo_b200_psd_complete": (rc, [i64, P(CompletionStruct), vp, P(i64)]),
+        "cosmo_b200_set_forward_map": (rc, [vp, P(ForwardMapStruct)]),
+        "cosmo_b200_update_matrices_original": (rc, [vp, vp, i64, vp, i64, vp, vp]),
+        "cosmo_b200_comm_unique_id": (rc, [vp]),
+        "cosmo_b200_comm_init": (rc, [vp, i32, i32, vp]),
+        "cosmo_b200_comm_p2p_export": (rc, [vp, vp]),
+        "cosmo_b200_comm_p2p_attach": (rc, [vp, vp, i32]),
+        "cosmo_b200_custom_cone_compile": (rc, [P(CustomConeStruct), i32, C.c_char_p, i64]),
+        "cosmo_b200_custom_cone_stats": (rc, [vp, P(i64)]),
+        "cosmo_b200_psd_stats": (rc, [vp, P(i64)]),
+        "cosmo_b200_tc_gemm_test": (rc, [i32, i32, i32, i32, vp, vp, vp, i32, P(f64), P(f64)]),
+    }
+
+
+SIGNATURES = _signatures()
+EXPORTS = list(SIGNATURES)
+
+
+def _check_rc(lib, rc, h=None):
+    """EngineError unless rc is OK, with the last error of handle `h` (None: of the calls without a handle)."""
+    if rc != OK:
+        raise EngineError(rc, (lib.cosmo_b200_last_error(h) or b"").decode())
+
+
+def _keyed(lib, h, fn, *args, ctype, keys, ints=()):
+    """fn(*args, out) for an out array of len(keys) `ctype`s, checked as _check_rc does.  Returns the array as a dict in
+    the order of `keys`, without the slots whose key is None and with the values of the keys in `ints` cast to int."""
+    out = (ctype * len(keys))()
+    _check_rc(lib, fn(*args, out), h)
+    return {k: int(v) if k in ints else v for k, v in zip(keys, out) if k is not None}
+
+
 def _i64(a, keep):
     a = np.ascontiguousarray(a, dtype=np.int64)
     keep.append(a)
@@ -128,24 +194,23 @@ def completion_struct(c, keep) -> CompletionStruct:
                             len(c.idx), _i64(c.idx, keep))
 
 
+def problem_struct(P, A, dtype, index_base, keep) -> ProblemStruct:
+    """cosmo_b200_problem with dtype, index_base, m, n, P and A set from CSC matrices P and A with sorted indices
+    (values as `dtype`, indices shifted by `index_base`); the arrays it points to are appended to `keep`."""
+    prob = ProblemStruct()
+    prob.dtype = F64 if np.dtype(dtype) == np.float64 else F32
+    prob.index_base = index_base
+    prob.m, prob.n = A.shape
+    for name, M in (("P", P), ("A", A)):
+        arrs = [np.ascontiguousarray(M.indptr, dtype=np.int64) + index_base,
+                np.ascontiguousarray(M.indices, dtype=np.int64) + index_base, np.ascontiguousarray(M.data, dtype=dtype)]
+        keep.extend(arrs)
+        setattr(prob, name, CscStruct(M.shape[0], M.shape[1], *[_ptr(a) for a in arrs]))
+    return prob
+
+
 # cosmo_b200_reverse_decomposition / cosmo_b200_psd_complete stats[4]
 REVERSE_STATS = ("cones_completed", "pinv_fallbacks", "workspace_bytes", "device_us")
-
-EXPORTS = [
-    "cosmo_b200_abi_version", "cosmo_b200_default_settings", "cosmo_b200_create", "cosmo_b200_destroy",
-    "cosmo_b200_last_error", "cosmo_b200_update_settings", "cosmo_b200_warm_start", "cosmo_b200_update_qb",
-    "cosmo_b200_update_matrices",
-    "cosmo_b200_update_rho", "cosmo_b200_reset", "cosmo_b200_solve", "cosmo_b200_project", "cosmo_b200_kkt_solve",
-    "cosmo_b200_residuals", "cosmo_b200_spmv", "cosmo_b200_spmv_bench", "cosmo_b200_get_rho_vec", "cosmo_b200_get_w",
-    "cosmo_b200_comm_unique_id", "cosmo_b200_comm_init", "cosmo_b200_comm_p2p_export", "cosmo_b200_comm_p2p_attach",
-    "cosmo_b200_tc_gemm_test", "cosmo_b200_psd_stats", "cosmo_b200_get_scaling",
-    "cosmo_b200_set_accelerator", "cosmo_b200_accelerator_stats", "cosmo_b200_infeasibility_test",
-    "cosmo_b200_psd_lambda_max", "cosmo_b200_ldl_stats", "cosmo_b200_ldl_symbolic",
-    "cosmo_b200_set_decomposition", "cosmo_b200_set_decomposition_noncompact", "cosmo_b200_reverse_decomposition",
-    "cosmo_b200_psd_complete",
-    "cosmo_b200_set_forward_map", "cosmo_b200_update_matrices_original",
-    "cosmo_b200_custom_cone_compile", "cosmo_b200_custom_cone_stats",
-]
 
 _lib = None
 
@@ -165,55 +230,9 @@ def load_library(rebuild_if_stale=True):
     if not os.path.exists(path):
         raise EngineError(ERR_CUDA, "libcosmo_b200.so is missing (run `python -c 'import __graft_entry__ as g; g.build()'`)")
     lib = C.CDLL(path)
-    vp = C.c_void_p
-    lib.cosmo_b200_abi_version.restype = C.c_int
-    lib.cosmo_b200_default_settings.argtypes = [C.POINTER(SettingsStruct)]
-    lib.cosmo_b200_create.argtypes = [C.POINTER(vp), C.POINTER(ProblemStruct), C.POINTER(SettingsStruct)]
-    lib.cosmo_b200_destroy.argtypes = [vp]
-    lib.cosmo_b200_destroy.restype = None
-    lib.cosmo_b200_last_error.argtypes = [vp]
-    lib.cosmo_b200_last_error.restype = C.c_char_p
-    lib.cosmo_b200_update_settings.argtypes = [vp, C.POINTER(SettingsStruct)]
-    lib.cosmo_b200_warm_start.argtypes = [vp, vp, vp, vp]
-    lib.cosmo_b200_update_qb.argtypes = [vp, vp, vp]
-    lib.cosmo_b200_update_matrices.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, vp]
-    lib.cosmo_b200_update_rho.argtypes = [vp, vp, C.c_double]
-    lib.cosmo_b200_reset.argtypes = [vp]
-    lib.cosmo_b200_solve.argtypes = [vp, C.POINTER(ResultStruct)]
-    lib.cosmo_b200_project.argtypes = [vp, vp, vp]
-    lib.cosmo_b200_kkt_solve.argtypes = [vp, vp, vp, C.POINTER(C.c_int64)]
-    lib.cosmo_b200_residuals.argtypes = [vp, vp, vp, vp, C.c_int32, C.POINTER(C.c_double)]
-    lib.cosmo_b200_spmv.argtypes = [vp, C.c_int32, vp, vp]
-    lib.cosmo_b200_spmv_bench.argtypes = [vp, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-    lib.cosmo_b200_get_rho_vec.argtypes = [vp, vp]
-    lib.cosmo_b200_get_w.argtypes = [vp, vp]
-    lib.cosmo_b200_comm_unique_id.argtypes = [vp]
-    lib.cosmo_b200_comm_init.argtypes = [vp, C.c_int32, C.c_int32, vp]
-    lib.cosmo_b200_comm_p2p_export.argtypes = [vp, vp]
-    lib.cosmo_b200_comm_p2p_attach.argtypes = [vp, vp, C.c_int32]
-    lib.cosmo_b200_psd_stats.argtypes = [vp, C.POINTER(C.c_int64)]
-    lib.cosmo_b200_get_scaling.argtypes = [vp, vp, vp, C.POINTER(C.c_double)]
-    lib.cosmo_b200_set_accelerator.argtypes = [vp, C.POINTER(AcceleratorStruct)]
-    lib.cosmo_b200_accelerator_stats.argtypes = [vp, C.POINTER(C.c_int64)]
-    lib.cosmo_b200_infeasibility_test.argtypes = [vp, C.c_int32, vp, C.POINTER(C.c_double)]
-    lib.cosmo_b200_psd_lambda_max.argtypes = [vp, vp, C.POINTER(C.c_double)]
-    lib.cosmo_b200_ldl_stats.argtypes = [vp, C.POINTER(C.c_double)]
-    i64p = C.POINTER(C.c_int64)
-    lib.cosmo_b200_ldl_symbolic.argtypes = [C.POINTER(ProblemStruct), i64p, i64p, i64p, i64p]
-    lib.cosmo_b200_tc_gemm_test.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int32,
-                                            C.POINTER(C.c_double), C.POINTER(C.c_double)]
-    lib.cosmo_b200_set_decomposition.argtypes = [vp, C.POINTER(DecompositionStruct)]
-    lib.cosmo_b200_set_decomposition_noncompact.argtypes = [vp, C.POINTER(DecompositionStruct)]
-    lib.cosmo_b200_reverse_decomposition.argtypes = [vp, C.c_int32, vp, vp, vp, i64p]
-    lib.cosmo_b200_psd_complete.argtypes = [C.c_int64, C.POINTER(CompletionStruct), vp, i64p]
-    lib.cosmo_b200_set_forward_map.argtypes = [vp, C.POINTER(ForwardMapStruct)]
-    lib.cosmo_b200_update_matrices_original.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, vp]
-    lib.cosmo_b200_custom_cone_compile.argtypes = [C.POINTER(CustomConeStruct), C.c_int32, C.c_char_p, C.c_int64]
-    lib.cosmo_b200_custom_cone_stats.argtypes = [vp, i64p]
-    for name in EXPORTS:
+    for name, (restype, argtypes) in SIGNATURES.items():
         fn = getattr(lib, name)
-        if name not in ("cosmo_b200_destroy", "cosmo_b200_last_error"):
-            fn.restype = C.c_int
+        fn.argtypes, fn.restype = argtypes, restype
     _lib = lib
     return lib
 
@@ -273,9 +292,7 @@ def _ptr(a: Optional[np.ndarray]):
 def nccl_unique_id() -> bytes:
     buf = (C.c_char * 128)()
     lib = load_library()
-    rc = lib.cosmo_b200_comm_unique_id(C.cast(buf, C.c_void_p))
-    if rc != OK:
-        raise EngineError(rc, (lib.cosmo_b200_last_error(None) or b"").decode())
+    _check_rc(lib, lib.cosmo_b200_comm_unique_id(C.cast(buf, C.c_void_p)))
     return bytes(buf)
 
 
@@ -309,16 +326,7 @@ class Engine:
         A.sort_indices()
         self.m, self.n = A.shape
         self.n_psd = sum(1 for t in sets if t[0] in (PSD_SQUARE, PSD_TRIANGLE, PSD_TRIANGLE_COMPLEX) and int(t[1]) > 0)
-        base = 1 if julia_indexing else 0
         keep = []  # keep host arrays alive during create
-
-        def csc(M):
-            colptr = np.ascontiguousarray(M.indptr, dtype=np.int64) + base
-            rowval = np.ascontiguousarray(M.indices, dtype=np.int64) + base
-            nz = np.ascontiguousarray(M.data, dtype=T)
-            keep.extend([colptr, rowval, nz])
-            return CscStruct(M.shape[0], M.shape[1], _ptr(colptr), _ptr(rowval), _ptr(nz))
-
         set_arr = (SetStruct * max(len(sets), 1))()
         for i, (typ, dim, l, u, *extra) in enumerate(sets):
             set_arr[i].type = int(typ)
@@ -344,13 +352,9 @@ class Engine:
                 keep.extend([la, ua])
                 set_arr[i].l = _ptr(la)
                 set_arr[i].u = _ptr(ua)
-        prob = ProblemStruct()
-        prob.dtype = F64 if T == np.float64 else F32
-        prob.index_base = base
+        prob = problem_struct(P, A, T, 1 if julia_indexing else 0, keep)
         prob.device = device
         prob.flags = 1 if equilibrate else 0
-        prob.m, prob.n = self.m, self.n
-        prob.P, prob.A = csc(P), csc(A)
         qa = np.ascontiguousarray(q, dtype=T)
         ba = np.ascontiguousarray(b, dtype=T)
         keep.extend([qa, ba])
@@ -367,9 +371,7 @@ class Engine:
         prob.c = float(c)
         self.settings = settings if settings is not None else default_settings()
         h = C.c_void_p()
-        rc = self._lib.cosmo_b200_create(C.byref(h), C.byref(prob), C.byref(self.settings))
-        if rc != OK:
-            raise EngineError(rc, (self._lib.cosmo_b200_last_error(None) or b"").decode())
+        _check_rc(self._lib, self._lib.cosmo_b200_create(C.byref(h), C.byref(prob), C.byref(self.settings)))
         self._h = h
         self.n_orig, self.m_orig = 0, 0     # the original problem of a decomposition map (set_decomposition)
         self._fwd_sizes = None              # (n_orig, m_orig) of the forward map (set_forward_map)
@@ -388,16 +390,16 @@ class Engine:
             pass
 
     def _check(self, rc):
-        if rc != OK:
-            raise EngineError(rc, (self._lib.cosmo_b200_last_error(self._h) or b"").decode())
+        _check_rc(self._lib, rc, self._h)
 
-    def _vec(self, a, size):
+    def _vec(self, a, size=None):
+        """`a` as a flat contiguous array of the engine's dtype (None stays None), of length `size` if one is given."""
         if a is None:
             return None
         a = np.ascontiguousarray(a, dtype=self.dtype)
-        if a.shape != (size,):
+        if size is not None and a.shape != (size,):
             raise EngineError(ERR_INVALID, "vector has wrong length")
-        return a
+        return a.ravel()
 
     # ---- updates ------------------------------------------------------------
     def update_settings(self, settings: SettingsStruct):
@@ -416,10 +418,7 @@ class Engine:
         """cosmo_b200_update_matrices: new values of P and A on the pattern of create -- ``Px`` / ``Ax`` are the ``data``
         arrays of the CSC matrices with sorted indices -- and optionally q and b (None: unchanged).  The engine is left
         as a new Engine with these data would be; an equilibrating engine needs all four, unscaled."""
-        Px, Ax = [None if a is None else np.ascontiguousarray(a, dtype=self.dtype).ravel() for a in (Px, Ax)]
-        q, b = self._vec(q, self.n), self._vec(b, self.m)
-        self._check(self._lib.cosmo_b200_update_matrices(self._h, _ptr(Px), 0 if Px is None else Px.size, _ptr(Ax),
-                                                         0 if Ax is None else Ax.size, _ptr(q), _ptr(b)))
+        self._update_values(self._lib.cosmo_b200_update_matrices, (self.n, self.m), Px, Ax, q, b)
 
     def update_rho(self, rho_vec, rho):
         rv = self._vec(rho_vec, self.m)
@@ -523,36 +522,28 @@ class Engine:
         self._check(self._lib.cosmo_b200_get_scaling(self._h, _ptr(D), _ptr(E), C.byref(c)))
         return D.astype(np.float64), E.astype(np.float64), float(c.value)
 
+    def _read_out(self, fn, *args, ctype, keys, ints=()):
+        return _keyed(self._lib, self._h, fn, self._h, *args, ctype=ctype, keys=keys, ints=ints)
+
     def psd_stats(self):
         """Which path projected the large PSD cones so far (cosmo_b200_psd_stats)."""
-        out = (C.c_int64 * 8)()
-        self._check(self._lib.cosmo_b200_psd_stats(self._h, out))
         keys = ("tc_projections", "tc_fallbacks", "tc_last_steps", "tc_last_checks", None, None, "jacobi_last_sweeps", "tc_slices")
-        return {k: int(v) for k, v in zip(keys, out) if k}
+        return self._read_out(self._lib.cosmo_b200_psd_stats, ctype=C.c_int64, keys=keys)
 
     def custom_cone_stats(self):
         """cosmo_b200_custom_cone_stats, keyed by CUSTOM_CONE_STATS."""
-        out = (C.c_int64 * 4)()
-        self._check(self._lib.cosmo_b200_custom_cone_stats(self._h, out))
-        return dict(zip(CUSTOM_CONE_STATS, [int(v) for v in out]))
+        return self._read_out(self._lib.cosmo_b200_custom_cone_stats, ctype=C.c_int64, keys=CUSTOM_CONE_STATS)
 
     def accelerator_stats(self):
         """Accelerator events of the last solve (cosmo_b200_accelerator_stats), keyed by ACCELERATOR_STATS."""
-        out = (C.c_int64 * 6)()
-        self._check(self._lib.cosmo_b200_accelerator_stats(self._h, out))
-        return dict(zip(ACCELERATOR_STATS, [int(v) for v in out]))
-
+        return self._read_out(self._lib.cosmo_b200_accelerator_stats, ctype=C.c_int64, keys=ACCELERATOR_STATS)
 
     def infeasibility_test(self, which, delta):
         """cosmo_b200_infeasibility_test: is_primal_infeasible! (which = 0, delta = delta_y, m) or is_dual_infeasible!
         (which = 1, delta = delta_x, n) on the engine's data; returns a dict keyed by INFEASIBILITY_RECORD."""
         delta = self._vec(delta, self.m if which == 0 else self.n)
-        out = (C.c_double * 8)()
-        self._check(self._lib.cosmo_b200_infeasibility_test(self._h, int(which), _ptr(delta), out))
-        rec = dict(zip(INFEASIBILITY_RECORD, list(out)))
-        for k in ("verdict", "gate", "families", "psd_unconverged"):
-            rec[k] = int(rec[k])
-        return rec
+        return self._read_out(self._lib.cosmo_b200_infeasibility_test, int(which), _ptr(delta), ctype=C.c_double,
+                              keys=INFEASIBILITY_RECORD, ints=("verdict", "gate", "families", "psd_unconverged"))
 
     def psd_lambda_max(self, v):
         """cosmo_b200_psd_lambda_max: lambda_max of every PSD cone of mat(v) (set order) as the certificate computes it."""
@@ -563,12 +554,7 @@ class Engine:
 
     def ldl_stats(self):
         """State of the direct LDL' plugin (cosmo_b200_ldl_stats), keyed by LDL_STATS."""
-        out = (C.c_double * 8)()
-        self._check(self._lib.cosmo_b200_ldl_stats(self._h, out))
-        rec = dict(zip(LDL_STATS, list(out)))
-        for k in LDL_STATS[:6]:
-            rec[k] = int(rec[k])
-        return rec
+        return self._read_out(self._lib.cosmo_b200_ldl_stats, ctype=C.c_double, keys=LDL_STATS, ints=LDL_STATS[:6])
 
     # ---- reverse of a chordal decomposition ---------------------------------
     def set_decomposition(self, d):
@@ -596,11 +582,9 @@ class Engine:
         the last solve (a False argument skips that output: None in its place), and the stats keyed by REVERSE_STATS."""
         out = [np.empty(n, dtype=np.float64) if want else None
                for want, n in ((x, self.n_orig), (s, self.m_orig), (mu, self.m_orig))]
-        stats = (C.c_int64 * 4)()
-        self._check(self._lib.cosmo_b200_reverse_decomposition(self._h, int(bool(complete_dual)), *[_ptr(a) for a in out],
-                                                               stats))
-        return out[0], out[1], out[2], dict(zip(REVERSE_STATS, [int(v) for v in stats]))
-
+        stats = self._read_out(self._lib.cosmo_b200_reverse_decomposition, int(bool(complete_dual)),
+                               *[_ptr(a) for a in out], ctype=C.c_int64, keys=REVERSE_STATS)
+        return out[0], out[1], out[2], stats
 
     # ---- values of the original problem onto the decomposed one ---------------
     def set_forward_map(self, f):
@@ -620,13 +604,15 @@ class Engine:
         """cosmo_b200_update_matrices_original: update_matrices with the ``data`` arrays of P and A (sorted CSC), q and b
         of the problem the chordal decomposition started from; the forward map (set_forward_map) carries them onto the
         decomposed problem on the device."""
-        Px, Ax = [None if a is None else np.ascontiguousarray(a, dtype=self.dtype).ravel() for a in (Px, Ax)]
-        if self._fwd_sizes is not None:
-            q, b = self._vec(q, self._fwd_sizes[0]), self._vec(b, self._fwd_sizes[1])
-        else:       # without a map the engine reads none of them and answers ERR_INVALID
-            q, b = [None if a is None else np.ascontiguousarray(a, dtype=self.dtype).ravel() for a in (q, b)]
-        self._check(self._lib.cosmo_b200_update_matrices_original(
-            self._h, _ptr(Px), 0 if Px is None else Px.size, _ptr(Ax), 0 if Ax is None else Ax.size, _ptr(q), _ptr(b)))
+        # without a map the engine reads none of q, b and answers ERR_INVALID: their lengths go unchecked here
+        sizes = self._fwd_sizes or (None, None)
+        self._update_values(self._lib.cosmo_b200_update_matrices_original, sizes, Px, Ax, q, b)
+
+    def _update_values(self, fn, qb_sizes, Px, Ax, q, b):
+        Px, Ax = self._vec(Px), self._vec(Ax)
+        q, b = self._vec(q, qb_sizes[0]), self._vec(b, qb_sizes[1])
+        self._check(fn(self._h, _ptr(Px), 0 if Px is None else Px.size, _ptr(Ax), 0 if Ax is None else Ax.size,
+                       _ptr(q), _ptr(b)))
 
 
 def psd_complete(Y, schedule):
@@ -636,11 +622,9 @@ def psd_complete(Y, schedule):
     W = np.array(Y, dtype=np.float64, order="F", copy=True)
     keep = []
     cs = completion_struct(schedule, keep)
-    stats = (C.c_int64 * 4)()
-    rc = lib.cosmo_b200_psd_complete(int(cs.N), C.byref(cs), W.ctypes.data_as(C.c_void_p), stats)
-    if rc != OK:
-        raise EngineError(rc, (lib.cosmo_b200_last_error(None) or b"").decode())
-    return W, dict(zip(REVERSE_STATS, [int(v) for v in stats]))
+    stats = _keyed(lib, None, lib.cosmo_b200_psd_complete, int(cs.N), C.byref(cs), W.ctypes.data_as(C.c_void_p),
+                   ctype=C.c_int64, keys=REVERSE_STATS)
+    return W, stats
 
 
 # cosmo_b200_infeasibility_test's out[8]: "gate2" is |Dinv A'dy|_inf (primal) or q'dx (dual), "gate3" dy'b of the
@@ -664,22 +648,10 @@ def ldl_symbolic(P, A):
     A = sp.csc_matrix(A, dtype=np.float64)
     P.sort_indices()
     A.sort_indices()
-    m, n = A.shape
     keep = []
-
-    def csc(M):
-        arrs = [np.ascontiguousarray(M.indptr, dtype=np.int64), np.ascontiguousarray(M.indices, dtype=np.int64),
-                np.ascontiguousarray(M.data, dtype=np.float64)]
-        keep.extend(arrs)
-        return CscStruct(M.shape[0], M.shape[1], _ptr(arrs[0]), _ptr(arrs[1]), _ptr(arrs[2]))
-
-    prob = ProblemStruct()
-    prob.dtype, prob.index_base, prob.m, prob.n = F64, 0, m, n
-    prob.P, prob.A = csc(P), csc(A)
-    out = [np.zeros(n + m, dtype=np.int64) for _ in range(4)]
-    rc = lib.cosmo_b200_ldl_symbolic(C.byref(prob), *[o.ctypes.data_as(C.POINTER(C.c_int64)) for o in out])
-    if rc != OK:
-        raise EngineError(rc, (lib.cosmo_b200_last_error(None) or b"").decode())
+    prob = problem_struct(P, A, np.float64, 0, keep)
+    out = [np.zeros(prob.n + prob.m, dtype=np.int64) for _ in range(4)]
+    _check_rc(lib, lib.cosmo_b200_ldl_symbolic(C.byref(prob), *[o.ctypes.data_as(C.POINTER(C.c_int64)) for o in out]))
     return tuple(out)
 
 
@@ -694,8 +666,6 @@ def tc_gemm(A, B, slices=8, groups=0, reps=0):
     Cm = np.zeros((N, N), dtype=np.float64, order="F")
     ms = C.c_double(0.0)
     fr = (C.c_double * 2)()
-    rc = lib.cosmo_b200_tc_gemm_test(N, slices, groups, 0, A.ctypes.data, B.ctypes.data, Cm.ctypes.data, reps,
-                                     C.byref(ms), fr)
-    if rc != 0:
-        raise EngineError(rc, (lib.cosmo_b200_last_error(None) or b"").decode())
+    _check_rc(lib, lib.cosmo_b200_tc_gemm_test(N, slices, groups, 0, A.ctypes.data, B.ctypes.data, Cm.ctypes.data, reps,
+                                               C.byref(ms), fr))
     return Cm, ms.value, (fr[0], fr[1])

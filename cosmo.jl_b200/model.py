@@ -587,41 +587,13 @@ class Model:
         self.mu[:] = -y0
         self._x2 = None
 
-    # update!(model; q, b), interface.jl:187-211, extended by new values of P and A on the pattern given to set!
+    # update!(model; q, b), interface.jl:187-211, extended by new values of P and A on the pattern given to set!.  The
+    # new values go to the live engine, and the iterates of the model stay as the next warm start.  The reference
+    # refuses to update a chordally decomposed model (interface.jl:192,204); here the values are mapped onto the
+    # decomposed problem, and rho and the clique iterates stay, as update! keeps them.
     def update(self, q=None, b=None, *, P=None, A=None):
         if not self.is_assembled:
             raise RuntimeError("Model has to be assembled once before one can start updating q or b.")
-        if P is not None or A is not None:
-            self._update_matrices(q, b, P, A)
-            return
-        if q is not None:
-            q = np.asarray(q, dtype=np.float64)
-            if q.shape != (self.n,):
-                raise ValueError("The dimension of q, does not agree with the model dimension, n.")
-            self.q0 = q.copy()
-        if b is not None:
-            b = np.asarray(b, dtype=np.float64)
-            if b.shape != (self.m,):
-                raise ValueError("The dimension of b, does not agree with the model dimension, m.")
-            self.b0 = b.copy()
-        if self.engine is not None and getattr(self, "_dec", None) is not None:
-            # the reference refuses: "can not be updated if the model has been chordally decomposed before"
-            # (interface.jl:192,204).  Here q and b are mapped onto the decomposed problem, q' = [q; 0] and b' = b[b_src],
-            # and go to the engine as for any other model: rho and the clique iterates stay, as update! keeps them.
-            if self._decomposition_holds(b):
-                from . import chordal as _chordal
-                _, q2, b2 = _chordal.forward_values(self._fwd, None, self.q0 if q is not None else None,
-                                                    self.b0 if b is not None else None)
-                self.engine.update_qb((self.D * q2) * self.c if q is not None else None,
-                                      self.E * b2 if b is not None else None)
-        elif self.engine is not None:
-            qs = (self.D * self.q0) * self.c if q is not None else None
-            bs = self.E * self.b0 if b is not None else None
-            self.engine.update_qb(qs, bs)
-
-    def _update_matrices(self, q, b, P, A):
-        """update(q, b, P=, A=): the new values go to the live engine (cosmo_b200_update_matrices), which ends up as a
-        new engine with these data would be; the iterates of the model stay as the next warm start."""
         new = {}
         for name, M, old in (("P", P, self.P0), ("A", A, self.A0)):
             if M is None:
@@ -644,23 +616,30 @@ class Model:
             self.q0 = q.copy()
         if b is not None:
             self.b0 = b.copy()
-        if self.engine is None:
+        if self.engine is None or (self._dec is not None and not self._decomposition_holds(b)):
+            return
+        if not new:
+            # q and b alone, scaled on the host; a decomposed model maps them first, q' = [q; 0] and b' = b[b_src]
+            q2, b2 = self.q0, self.b0
+            if self._dec is not None:
+                from . import chordal as _chordal
+                _, q2, b2 = _chordal.forward_values(self._fwd, None, self.q0 if q is not None else None,
+                                                    self.b0 if b is not None else None)
+            self.engine.update_qb((self.D * q2) * self.c if q is not None else None,
+                                  self.E * b2 if b is not None else None)
             return
         if self._dec is not None:
             # the values in the original coordinates go through the forward map on the device; all four, so that an
-            # equilibrating engine can run Ruiz again.  The clique iterates stay as the next warm start.
-            if self._decomposition_holds(b):
-                self.engine.update_matrices_original(self.P0.data, self.A0.data, self.q0, self.b0)
-                if self._engine_equilibrates:
-                    self.D, self.E, self.c = self.engine.scaling()
-            return
-        if self._engine_equilibrates:
+            # equilibrating engine can run Ruiz again
+            self.engine.update_matrices_original(self.P0.data, self.A0.data, self.q0, self.b0)
+        elif self._engine_equilibrates:
             # Ruiz runs again on the device from the unscaled data: every vector goes with the matrices
             self.engine.update_matrices(self.P0.data, self.A0.data, self.q0, self.b0)
-            self.D, self.E, self.c = self.engine.scaling()
         else:
             self.engine.update_matrices(new["P"].data if "P" in new else None, new["A"].data if "A" in new else None,
                                         q, b)
+        if self._engine_equilibrates:
+            self.D, self.E, self.c = self.engine.scaling()
 
     def _decomposition_holds(self, b) -> bool:
         """Can the live engine of a decomposed model take the new data?  Not without the forward map, and not when the new
