@@ -246,15 +246,12 @@ class Engine : public EngineBase {
   double c_ = 1.0;
   DevCsr<T> A_, At_, P_;
   DevBuf<T> q_, b_, D_, Dinv_, E_, Einv_;
-  std::vector<double> hb_;                       // host copy of b (row classification)
-  std::vector<double> hl_, hu_;                  // host box bounds (m-length, +-inf elsewhere)
-  std::vector<double> hl0_, hu0_;                // the unscaled box bounds of an equilibrating engine (update_matrices)
-  std::vector<cosmo_b200_set> sets_;             // type + dim only
-  std::vector<int> set_off_;
   // cones
   DevBuf<unsigned char> row_class_, rho_class_;
   DevBuf<int> row_cone_;
-  DevBuf<T> box_l_, box_u_;
+  DevBuf<T> box_l_, box_u_;       // m-length, +-inf outside Box rows
+  DevBuf<T> box_l0_, box_u0_;     // the unscaled Box bounds of an equilibrating engine (Ruiz restarts from them)
+  DevBuf<int> rect_off_, rect_dim_;   // cones that rectify_set_scalings! scales by one scalar (equilibrating engine)
   int n_soc_ = 0, n_soc_chunks_ = 0;
   DevBuf<int> soc_off_, soc_dim_, soc_chunk_start_, soc_chunk_len_, soc_cone_chunk_ptr_;
   DevBuf<T> soc_norm_, soc_chunk_sum_, soc_norm2_;
@@ -303,7 +300,6 @@ class Engine : public EngineBase {
   DevBuf<T> rho_vec_;
   double rho_ = 0.1;
   std::vector<double> rho_updates_;
-  bool is_optimized_ = false;
   bool have_solution_ = false;   // xs_, s_, mu_ hold what the last solve() returned (cleared by reset / warm_start)
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
@@ -418,7 +414,8 @@ class Engine : public EngineBase {
   void update_slab(DevCsr<T>& M, int ebase);
   void upload_value_maps();
   bool maps_ready_ = false;        // d_src / d_wsrc of A_, At_, P_ are on the device
-  void classify_and_set_rho(bool reset_rho, bool rebuild_vec = true);
+  void classify_and_set_rho(bool reset_rho);
+  void write_rho_vec();
   void allreduce_sum(T* buf, size_t count);
   void allreduce_max(T* buf, size_t count);
 
@@ -788,8 +785,8 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   long long off = 0;
   std::vector<unsigned char> row_class(m_);
   std::vector<int> row_cone(m_, 0);
-  hl_.assign(m_, -INFINITY);
-  hu_.assign(m_, INFINITY);
+  std::vector<T> box_l(m_, T(-INFINITY)), box_u(m_, T(INFINITY));
+  std::vector<int> rect_off, rect_dim;
   std::vector<int> soc_off, soc_dim;
   std::vector<PsdConeDesc> psd_descs;
   std::vector<int> c3_off, c3_maxit;
@@ -802,9 +799,6 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   for (long long k = 0; k < p.n_sets; ++k) {
     const cosmo_b200_set& sdesc = p.sets[k];
     if (sdesc.dim < 0 || off + sdesc.dim > m_) throw EngineError{COSMO_B200_ERR_INVALID, "set dimensions exceed m"};
-    cosmo_b200_set keep = sdesc; keep.l = keep.u = nullptr;
-    sets_.push_back(keep);
-    set_off_.push_back((int)off);
     unsigned char cls;
     switch (sdesc.type) {
       case COSMO_B200_ZERO: cls = ROW_ZERO; break;
@@ -816,7 +810,7 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
         const T* u = static_cast<const T*>(sdesc.u);
         for (long long i = 0; i < sdesc.dim; ++i) {
           if (l[i] > u[i]) throw EngineError{COSMO_B200_ERR_INVALID, "Box set: inconsistent lower/upper bounds"};
-          hl_[off + i] = l[i]; hu_[off + i] = u[i];
+          box_l[off + i] = l[i]; box_u[off + i] = u[i];
         }
         break;
       }
@@ -895,6 +889,11 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
         throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "unsupported cone type (complex PSD): fall back to the host loop"};
     }
     for (long long i = 0; i < sdesc.dim; ++i) row_class[off + i] = cls;
+    // rectify_set_scalings! (scaling.jl:129-142) gives every other cone one scalar scaling
+    if (cls != ROW_ZERO && cls != ROW_NONNEG && cls != ROW_BOX && sdesc.dim > 0) {
+      rect_off.push_back((int)off);
+      rect_dim.push_back((int)sdesc.dim);
+    }
     off += sdesc.dim;
   }
   if (off != m_) throw EngineError{COSMO_B200_ERR_INVALID, "sum of set dimensions != m"};
@@ -934,29 +933,29 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   auto up = [&](DevBuf<T>& d, const void* h, size_t cnt) { d.alloc(cnt); if (h) upload_vec(d, h, cnt); };
   q_.alloc(n_);
   b_.alloc(m_);
-  hb_.resize(m_);
   scaled_ = (p.D && p.Dinv && p.E && p.Einv);
   c_ = p.c;
   if (scaled_) { up(D_, p.D, n_); up(Dinv_, p.Dinv, n_); up(E_, p.E, m_); up(Einv_, p.Einv, m_); }
   // scaling requested but no scaling matrices handed over: the data are unscaled, equilibrate them here
   // (setup.jl:27-33 -> scale_ruiz!); the host reads D, E, c back with cosmo_b200_get_scaling
   device_scaled_ = (p.flags & COSMO_B200_PROBLEM_EQUILIBRATE) && st_.scaling != 0;
-  if (device_scaled_) {
-    if (scaled_) throw EngineError{COSMO_B200_ERR_INVALID, "COSMO_B200_PROBLEM_EQUILIBRATE expects D = Dinv = E = Einv = NULL"};
-    hl0_ = hl_; hu0_ = hu_;
-  }
+  if (device_scaled_ && scaled_)
+    throw EngineError{COSMO_B200_ERR_INVALID, "COSMO_B200_PROBLEM_EQUILIBRATE expects D = Dinv = E = Einv = NULL"};
   row_class_.alloc(m_); row_cone_.alloc(m_); rho_class_.alloc(m_);
   if (m_) {
     CUDA_TRY(cudaMemcpyAsync(row_class_.p, row_class.data(), m_, cudaMemcpyHostToDevice, stream_));
     CUDA_TRY(cudaMemcpyAsync(row_cone_.p, row_cone.data(), m_ * sizeof(int), cudaMemcpyHostToDevice, stream_));
   }
   box_l_.alloc(m_); box_u_.alloc(m_);
-  {
-    std::vector<T> l(hl_.begin(), hl_.end()), u(hu_.begin(), hu_.end());
-    upload_vec(box_l_, l.data(), m_);
-    upload_vec(box_u_, u.data(), m_);
-    sync();
+  upload_vec(box_l_, box_l.data(), m_);
+  upload_vec(box_u_, box_u.data(), m_);
+  if (device_scaled_) {
+    box_l0_.alloc(m_, false); box_u0_.alloc(m_, false);
+    upload_vec(box_l0_, box_l.data(), m_);
+    upload_vec(box_u0_, box_u.data(), m_);
+    rect_off_.upload(rect_off, stream_); rect_dim_.upload(rect_dim, stream_);
   }
+  sync();
   // SOC tables (chunks of <= 8192 tail rows)
   n_soc_ = (int)soc_off.size();
   if (n_soc_) {
@@ -1048,34 +1047,24 @@ Engine<T>::~Engine() {
   if (stream_) cudaStreamDestroy(stream_);
 }
 
-// classify_constraints! (setup.jl:75-85; convexset.jl:62-69, 831-842) and
+// classify_constraints! (setup.jl:75-85; convexset.jl:62-69, 831-842) on the resident b and Box bounds, then
 // set_rho_vec! / update_rho_vec! (parameters.jl:3-13, 75-81)
 template <typename T>
-void Engine<T>::classify_and_set_rho(bool reset_rho, bool rebuild_vec) {
-  std::vector<unsigned char> cls(m_, 0);
-  const double big = st_.COSMO_INFTY * st_.MIN_SCALING;
-  for (size_t k = 0; k < sets_.size(); ++k) {
-    const int off = set_off_[k];
-    const long long dim = sets_[k].dim;
-    if (sets_[k].type == COSMO_B200_ZERO) {
-      for (long long i = 0; i < dim; ++i) cls[off + i] = 1;
-    } else if (sets_[k].type == COSMO_B200_NONNEG) {
-      for (long long i = 0; i < dim; ++i) if (hb_[off + i] > big) cls[off + i] = 2;
-    } else if (sets_[k].type == COSMO_B200_BOX) {
-      for (long long i = 0; i < dim; ++i) {
-        const double l = hl_[off + i], u = hu_[off + i];
-        if (l < -big && u > big) cls[off + i] = 2;
-        else if ((u - l) < st_.RHO_TOL) cls[off + i] = 1;
-      }
-    }
-  }
-  if (m_) CUDA_TRY(cudaMemcpyAsync(rho_class_.p, cls.data(), m_, cudaMemcpyHostToDevice, stream_));
-  sync();
+void Engine<T>::classify_and_set_rho(bool reset_rho) {
+  rho_class_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, row_class_.p, b_.p, box_l_.p, box_u_.p,
+                                                         st_.COSMO_INFTY * st_.MIN_SCALING, st_.RHO_TOL, rho_class_.p);
+  check_launch("rho_class");
   if (reset_rho) {
     rho_ = st_.rho;
     rho_updates_.clear();
     rho_updates_.push_back(rho_);
   }
+  write_rho_vec();
+}
+
+// rho_vec_ from rho_class_ and the current rho_; the LDL factor follows it before the next KKT solve
+template <typename T>
+void Engine<T>::write_rho_vec() {
   rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
   check_launch("rho_vec");
   ldl_dirty_ = true;
@@ -1090,62 +1079,53 @@ void Engine<T>::equilibrate() {
   DevBuf<T> cdev;
   cdev.alloc(1, false);
   ruiz_fill_kernel<T><<<vgrid(n), kBlock, 0, stream_>>>(n, D_.p, T(1));
+  check_launch("ruiz_fill");
   ruiz_fill_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, E_.p, T(1));
+  check_launch("ruiz_fill");
   ruiz_fill_kernel<T><<<1, 32, 0, stream_>>>(1, cdev.p, T(1));
+  check_launch("ruiz_fill");
   T* Dw = Dinv_.p;   // the inverse scalings double as work vectors, like in the reference (scaling.jl:37-41)
   T* Ew = Einv_.p;
   auto wgrid = [&](long long rows) { return (int)std::min<long long>((rows * 32 + kBlock - 1) / kBlock + 1, kMaxGrid); };
   for (int it = 0; it < st_.scaling; ++it) {
     // kkt_col_norms! (scaling.jl:3-8)
     ruiz_row_inf_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, P_.view(), D_.p, D_.p, cdev.p, Dw, 0);
+    check_launch("ruiz_row_inf");
     ruiz_row_inf_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, At_.view(), D_.p, E_.p, (const T*)nullptr, Dw, 1);
+    check_launch("ruiz_row_inf");
     ruiz_row_inf_kernel<T><<<wgrid(m), kBlock, 0, stream_>>>(m, A_.view(), E_.p, D_.p, (const T*)nullptr, Ew, 0);
+    check_launch("ruiz_row_inf");
     ruiz_update_kernel<T><<<vgrid(n), kBlock, 0, stream_>>>(n, Dw, D_.p, lo, hi);
+    check_launch("ruiz_update");
     ruiz_update_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, Ew, E_.p, lo, hi);
+    check_launch("ruiz_update");
     // cost scaling (scaling.jl:73-90): column norms of the newly scaled P, |q|_inf
     ruiz_row_inf_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, P_.view(), D_.p, D_.p, cdev.p, Dw, 0);
+    check_launch("ruiz_row_inf");
     ruiz_cost_kernel<T><<<1, 1024, 0, stream_>>>(n, Dw, q_.p, D_.p, cdev.p, lo, hi);
-    launches_ += 7;
+    check_launch("ruiz_cost");
   }
-  // rectify_set_scalings! (scaling.jl:129-142): one scalar per SOC / PSD / exponential / power cone
-  {
-    std::vector<int> off, dim;
-    for (size_t k = 0; k < sets_.size(); ++k) {
-      const int t = sets_[k].type;
-      if (t != COSMO_B200_ZERO && t != COSMO_B200_NONNEG && t != COSMO_B200_BOX && sets_[k].dim > 0) {
-        off.push_back(set_off_[k]);
-        dim.push_back((int)sets_[k].dim);
-      }
-    }
-    if (!off.empty()) {
-      DevBuf<int> off_d, dim_d;
-      off_d.upload(off, stream_); dim_d.upload(dim, stream_);
-      ruiz_rectify_kernel<T><<<(int)off.size(), kBlock, 0, stream_>>>(off_d.p, dim_d.p, E_.p);
-      sync();
-    }
+  // rectify_set_scalings! (scaling.jl:129-142): one scalar per cone of the table the constructor built
+  if (rect_off_.n) {
+    ruiz_rectify_kernel<T><<<(int)rect_off_.n, kBlock, 0, stream_>>>(rect_off_.p, rect_dim_.p, E_.p);
+    check_launch("ruiz_rectify");
   }
   // apply D, E, c to the CSR copies (A and A' both scale an entry by the product D_j E_i, so they stay equal bit for
   // bit), q, b and the Box bounds; write_values fills the slabs from the scaled A' afterwards
   ruiz_apply_csr_kernel<T><<<wgrid(m), kBlock, 0, stream_>>>(m, A_.rowptr.p, A_.col.p, A_.val.p, E_.p, D_.p, (const T*)nullptr);
+  check_launch("ruiz_apply_csr");
   ruiz_apply_csr_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, At_.val.p, D_.p, E_.p, (const T*)nullptr);
+  check_launch("ruiz_apply_csr");
   ruiz_apply_csr_kernel<T><<<wgrid(n), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.val.p, D_.p, D_.p, cdev.p);
+  check_launch("ruiz_apply_csr");
   ruiz_finish_n_kernel<T><<<vgrid(n), kBlock, 0, stream_>>>(n, q_.p, D_.p, Dinv_.p, cdev.p);
+  check_launch("ruiz_finish_n");
   ruiz_finish_m_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, b_.p, E_.p, Einv_.p, row_class_.p, box_l_.p, box_u_.p);
-  check_launch("ruiz");
-  // the rho classification (setup.jl:75-85) looks at the SCALED b and Box bounds: refresh the host mirrors
-  {
-    std::vector<T> hb(m), hl(m), hu(m);
-    T ch = T(1);
-    if (m) {
-      CUDA_TRY(cudaMemcpyAsync(hb.data(), b_.p, (size_t)m * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-      CUDA_TRY(cudaMemcpyAsync(hl.data(), box_l_.p, (size_t)m * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-      CUDA_TRY(cudaMemcpyAsync(hu.data(), box_u_.p, (size_t)m * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-    }
-    CUDA_TRY(cudaMemcpyAsync(&ch, cdev.p, sizeof(T), cudaMemcpyDeviceToHost, stream_));
-    sync();
-    for (int i = 0; i < m; ++i) { hb_[i] = (double)hb[i]; hl_[i] = (double)hl[i]; hu_[i] = (double)hu[i]; }
-    c_ = (double)ch;
-  }
+  check_launch("ruiz_finish_m");
+  T ch = T(1);
+  CUDA_TRY(cudaMemcpyAsync(&ch, cdev.p, sizeof(T), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  c_ = (double)ch;
   scaled_ = true;
 }
 
@@ -1178,10 +1158,8 @@ void Engine<T>::update_qb(const void* q, const void* b) {
   if (q) upload_vec(q_, q, n_);
   if (b) {
     upload_vec(b_, b, m_);
-    for (int i = 0; i < m_; ++i) hb_[i] = (double)static_cast<const T*>(b)[i];
+    classify_and_set_rho(false);
   }
-  sync();
-  if (b) classify_and_set_rho(false, !is_optimized_);
   sync();
 }
 
@@ -1290,16 +1268,9 @@ template <typename T>
 void Engine<T>::values_placed(const T* Px, bool A, bool b) {
   if (A) gather_csr(A_, At_.val.p);
   if (Px) gather_csr(P_, Px);
-  if (b && !device_scaled_) {   // the host mirror of b (row classification); equilibrate() refreshes it from the scaled b
-    std::vector<T> hb(m_);
-    download_vec(hb.data(), b_.p, m_);
-    sync();
-    for (int i = 0; i < m_; ++i) hb_[i] = (double)hb[i];
-  }
   if (device_scaled_) {
-    std::vector<T> l(hl0_.begin(), hl0_.end()), u(hu0_.begin(), hu0_.end());
-    upload_vec(box_l_, l.data(), m_);
-    upload_vec(box_u_, u.data(), m_);
+    CUDA_TRY(cudaMemcpyAsync(box_l_.p, box_l0_.p, (size_t)m_ * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+    CUDA_TRY(cudaMemcpyAsync(box_u_.p, box_u0_.p, (size_t)m_ * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
     equilibrate();
   }
   if (A) {
@@ -1459,7 +1430,6 @@ void Engine<T>::reset() {
   if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));
   kkt_counter_ = 1;
   last_cg_iters_ = 1;
-  is_optimized_ = false;
   have_solution_ = false;
   psd_.reset_warm_start();
   classify_and_set_rho(true);
@@ -1977,9 +1947,7 @@ bool Engine<T>::adapt_rho(const T* x) {
   if (new_rho > st_.adaptive_rho_tolerance * rho_ || new_rho < (1.0 / st_.adaptive_rho_tolerance) * rho_) {
     rho_ = new_rho;
     tm_valid_ = false;
-    rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
-    check_launch("rho_vec");
-    ldl_dirty_ = true;
+    write_rho_vec();
     rho_updates_.push_back(new_rho);
     return true;
   }
@@ -2274,7 +2242,6 @@ void Engine<T>::solve(cosmo_b200_result* out) {
   CUDA_TRY(cudaMemcpyAsync(W_[cur_].p, xs_.p, n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
   ws_from_mu_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, rho_vec_.p, mu_.p, s_.p, W_[cur_].p + n);
   check_launch("ws_from_mu");
-  is_optimized_ = true;
   // phase timers: on request (verbose & 2 = settings.verbose_timing) and for every problem that is not latency-bound
   {
     const bool timers = (st_.verbose & 2) != 0 || (long long)n + m >= 20000 || !psd_.large_h.empty();

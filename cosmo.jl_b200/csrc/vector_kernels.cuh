@@ -267,6 +267,31 @@ __global__ void __launch_bounds__(kBlock) ws_from_mu_kernel(int m, const T* __re
     ws[i] = T(1) / rho[i] * mu[i] + s[i];
 }
 
+// rho_class of every row (classify_constraints!, setup.jl:75-85; convexset.jl:62-69, 831-842), the table rho_vec_kernel
+// reads: 1 on Zero rows and on Box rows with u - l < RHO_TOL, 2 on loose rows (Nonnegatives with b > big, Box with
+// l < -big and u > big), 0 elsewhere.  Every comparison and u - l are taken in fp64 after widening the T values, so an
+// fp32 engine classifies the numbers it holds exactly as an fp64 statement of the rule does; NaN compares false.
+template <typename T>
+__global__ void __launch_bounds__(kBlock) rho_class_kernel(int m, const unsigned char* __restrict__ row_class,
+                                                           const T* __restrict__ b, const T* __restrict__ box_l,
+                                                           const T* __restrict__ box_u, double big, double rho_tol,
+                                                           unsigned char* __restrict__ rho_class) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+    const unsigned char cls = row_class[i];
+    unsigned char c = 0;
+    if (cls == ROW_ZERO) {
+      c = 1;
+    } else if (cls == ROW_NONNEG) {
+      if ((double)b[i] > big) c = 2;
+    } else if (cls == ROW_BOX) {
+      const double l = (double)box_l[i], u = (double)box_u[i];
+      if (l < -big && u > big) c = 2;
+      else if (u - l < rho_tol) c = 1;
+    }
+    rho_class[i] = c;
+  }
+}
+
 // rho_vec from the per-row class table        (parameters.jl:17-49, 75-81)
 //   class 0: rho ; 1: rho * RHO_EQ_OVER_RHO_INEQ ; 2: RHO_MIN
 template <typename T>
