@@ -34,6 +34,7 @@
 #include "ruiz.cuh"
 #include "cg_persistent.cuh"
 #include "ldl.cuh"
+#include "ldl_sn.cuh"
 #include "chordal_rev.cuh"
 #include "chordal_fwd.cuh"
 #include "mat_update.cuh"
@@ -181,6 +182,7 @@ class EngineBase {
   virtual void infeasibility_test(int which, const void* delta, double* out8) = 0;
   virtual void psd_lambda_max(const void* v, double* lam) = 0;
   virtual void ldl_stats(double* out8) = 0;
+  virtual void ldl_sn_stats(int64_t* out8) = 0;
   virtual void set_decomposition(const cosmo_b200_decomposition* d, bool traditional) = 0;
   virtual void set_forward_map(const cosmo_b200_forward_map* f) = 0;
   virtual void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
@@ -199,6 +201,8 @@ class Engine : public EngineBase {
       destroy_cg_graphs();
       destroy_ldl_factor_graph();
       ldl_dirty_ = true;
+      sn_factor_graph_.reset();
+      sn_dirty_ = true;
     }
     st_ = st;
   }
@@ -226,6 +230,7 @@ class Engine : public EngineBase {
   void infeasibility_test(int which, const void* delta, double* out8) override;
   void psd_lambda_max(const void* v, double* lam) override;
   void ldl_stats(double* out8) override;
+  void ldl_sn_stats(int64_t* out8) override;
   void set_decomposition(const cosmo_b200_decomposition* d, bool traditional) override;
   void set_forward_map(const cosmo_b200_forward_map* f) override;
   void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
@@ -335,6 +340,29 @@ class Engine : public EngineBase {
   void ldl_factor();
   void ldl_solve();
   void destroy_ldl_factor_graph() { ldl_factor_graph_.reset(); }
+  bool direct_kkt() const { return st_.kkt_solver == COSMO_B200_KKT_LDL || st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL; }
+  void direct_factor() {
+    if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_factor();
+    else if (st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL) sn_factor();
+  }
+  // supernodal LDL' plugin (ldl_sn.cuh): host analysis, factor and solves as captured graphs
+  struct SnBig { int s; int64_t groups, chunk; };
+  struct SnLevel { int small0 = 0, small1 = 0; size_t smem = 0; std::vector<SnBig> big; };
+  bool sn_ready_ = false;
+  bool sn_dirty_ = true;           // rho_vec_ or sigma changed since the last factorisation
+  ldl_sn::Symbolic sn_;            // the analysis; the graphs are built from it
+  std::vector<SnLevel> sn_levels_;
+  int sn_solve_nodes_ = 0, sn_factor_nodes_ = 0, sn_small_count_ = 0, sn_tiled_count_ = 0;
+  long long sn_factorizations_ = 0;
+  double sn_symbolic_s_ = 0.0, sn_factor_s_ = 0.0;
+  DevBuf<int64_t> sn_rptr_, sn_off_, sn_uptr_, sn_Ksp_, sn_Ksrc_, sn_Kpos_, sn_gptr_;
+  DevBuf<int> sn_sptr_, sn_rows_, sn_ud_, sn_up0_, sn_up1_, sn_gd_, sn_gi_, sn_perm_, sn_small_, sn_lrows_, sn_lcols_,
+      sn_bcols_, sn_flags_;
+  DevBuf<T> sn_Lx_, sn_D_, sn_Dinv_, sn_part_, sn_y_;
+  GraphExec sn_factor_graph_, sn_solve_graph_;
+  void sn_setup();
+  void sn_factor();
+  void sn_solve();
   long long kkt_counter_ = 1;   // S.iteration_counter
   int last_cg_iters_ = 1;
   // tm_ = rho .* (A xsol_), stored by the fused ADMM tail: the next CG solve of the same solve() starts from it instead
@@ -1027,10 +1055,7 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   classify_and_set_rho(true);
   sync();
   // QdldlKKTSolver's constructor factors K (kktsolver.jl:293-306): a non-convex P or a singular K fails the create
-  if (st_.kkt_solver == COSMO_B200_KKT_LDL) {
-    ldl_setup();
-    ldl_factor();
-  }
+  if (direct_kkt()) direct_factor();
   create_time_ = now_s() - t_ctor0;
   auto_rho_interval_ = 0;
 }
@@ -1068,6 +1093,7 @@ void Engine<T>::write_rho_vec() {
   rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
   check_launch("rho_vec");
   ldl_dirty_ = true;
+  sn_dirty_ = true;
 }
 
 // scale_ruiz! (scaling.jl:21-116) on the resident data; see ruiz.cuh
@@ -1233,7 +1259,7 @@ void Engine<T>::finish_update(const T* Px, bool A, bool b, double t0) {
   destroy_cg_graphs();   // the slab and escape-table pointers they captured may have changed
   reset();
   auto_rho_interval_ = 0;
-  if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_factor();   // reset() marked the factor dirty; a non-convex P fails here
+  direct_factor();   // reset() marked the factor dirty; a non-convex P fails here
   create_time_ = now_s() - t0;
 }
 
@@ -1416,6 +1442,7 @@ void Engine<T>::update_rho(const void* rho_vec, double rho) {
   if (rho_vec) upload_vec(rho_vec_, rho_vec, m_);
   rho_ = rho;
   ldl_dirty_ = true;   // update_rho! -> refactor! (kktsolver.jl:310-313), done before the next KKT solve
+  sn_dirty_ = true;
   sync();
 }
 
@@ -1452,7 +1479,7 @@ void Engine<T>::allreduce_max(T* buf, size_t count) {
 template <typename T>
 void Engine<T>::comm_init(int nranks, int rank, const void* id128) {
   if (nranks < 1 || rank < 0 || rank >= nranks) throw EngineError{COSMO_B200_ERR_INVALID, "bad rank / nranks"};
-  if (st_.kkt_solver == COSMO_B200_KKT_LDL)
+  if (direct_kkt())
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU (use CG or reduced MINRES when sharded)"};
   nranks_ = nranks; rank_ = rank;
   if (nranks == 1) return;
@@ -1686,7 +1713,7 @@ template <typename T>
 void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
   const bool lead = (rank_ == 0);
   const bool full = (st_.kkt_solver == COSMO_B200_KKT_MINRES);
-  const bool direct = (st_.kkt_solver == COSMO_B200_KKT_LDL);
+  const bool direct = direct_kkt();
   if (st_.kkt_solver != COSMO_B200_KKT_CG && st_.kkt_solver != COSMO_B200_KKT_MINRES_REDUCED && !full && !direct)
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "unknown kkt_solver"};
   if (full && nranks_ > 1)
@@ -1694,7 +1721,8 @@ void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
   const bool tm_ready = tm_valid_;
   tm_valid_ = false;
   if (full || direct) {
-    if (direct) ldl_solve();   // xsol_ = y1, nu_ = y2
+    if (direct && st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_solve();   // xsol_ = y1, nu_ = y2
+    else if (direct) sn_solve();
     else kkt_minres(true);
     if (fused_tail) {
       admm_tail_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, nu_.p, rho_vec_.p, s_.p, w_src + n_, w_dst + n_, (T)st_.alpha);
@@ -2480,7 +2508,7 @@ void Engine<T>::kkt_solve(const void* rhs, void* sol, int64_t* inner) {
   download_vec(sol, xsol_.p, n_);
   download_vec(static_cast<T*>(sol) + n_, nu_.p, m_);
   sync();
-  if (inner && st_.kkt_solver == COSMO_B200_KKT_LDL) {
+  if (inner && direct_kkt()) {
     *inner = 0;
   } else if (inner) {
     CUDA_TRY(cudaMemcpyAsync(h_isc_.p, isc_.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
@@ -2634,8 +2662,232 @@ void Engine<T>::ldl_solve() {
 
 template <typename T>
 void Engine<T>::ldl_stats(double* o) {
+  if (st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL) {   // stored entries (explicit zeros included), supernodal levels
+    o[0] = sn_.N; o[1] = (double)sn_.nnz_K; o[2] = (double)sn_.stored; o[3] = sn_.levels;
+    o[4] = sn_solve_nodes_; o[5] = (double)sn_factorizations_; o[6] = sn_factor_s_; o[7] = sn_symbolic_s_;
+    return;
+  }
   o[0] = ldl_N_; o[1] = (double)ldl_nnzK_; o[2] = (double)ldl_nnzL_; o[3] = ldl_fptr_h_.empty() ? 0 : (double)ldl_fptr_h_.size() - 1;
   o[4] = ldl_solve_nodes_; o[5] = (double)ldl_factorizations_; o[6] = ldl_factor_s_; o[7] = ldl_symbolic_s_;
+}
+
+// ---- supernodal LDL' plugin (ldl_sn.cuh) ------------------------------------------------------------------------
+// Symbolic analysis of the resident pattern (host), upload of the panels' structure and the schedules, the choice of
+// path per supernode, device buffers.
+template <typename T>
+void Engine<T>::sn_setup() {
+  CUDA_TRY(cudaSetDevice(device_));
+  const double t0 = now_s();
+  std::vector<int> Prow(n_ + 1), Pcol(P_.nnz), Arow(n_ + 1), Acol(At_.nnz);
+  CUDA_TRY(cudaMemcpyAsync(Prow.data(), P_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(Arow.data(), At_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  if (P_.nnz) CUDA_TRY(cudaMemcpyAsync(Pcol.data(), P_.col.p, P_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  if (At_.nnz) CUDA_TRY(cudaMemcpyAsync(Acol.data(), At_.col.p, At_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  ldl_sn::Symbolic& S = sn_;
+  ldl_sn::analyze(n_, m_, Prow, Pcol, Arow, Acol, S);
+  sn_symbolic_s_ = now_s() - t0;
+  const size_t ts = sizeof(T);
+  // path per supernode: the small path when the panel and its relative rows fit one CTA's shared memory; the tiled
+  // path's descendant updates split into groups of about kUpdatesPerGroup, the partial sums capped at 256 MB
+  constexpr int64_t kUpdatesPerGroup = 16;
+  sn_levels_.assign(S.levels, SnLevel());
+  std::vector<int> small;
+  int64_t part = 0;
+  sn_small_count_ = sn_tiled_count_ = 0;
+  for (int l = 0; l < S.levels; ++l) {
+    SnLevel& L = sn_levels_[l];
+    L.small0 = (int)small.size();
+    for (int k = S.lptr[l]; k < S.lptr[l + 1]; ++k) {
+      const int s = S.lcols[k];
+      const int64_t h = S.height(s), w = S.width(s);
+      const size_t bytes = (size_t)(h * w) * ts + (size_t)h * sizeof(int);
+      if (bytes <= (size_t)sn::kSmallBytes) {
+        small.push_back(s);
+        L.smem = std::max(L.smem, bytes);
+        ++sn_small_count_;
+      } else {
+        const int64_t nu = S.uptr[s + 1] - S.uptr[s];
+        int64_t g = std::max<int64_t>(1, (nu + kUpdatesPerGroup - 1) / kUpdatesPerGroup);
+        g = std::max<int64_t>(1, std::min<int64_t>(g, (int64_t)((256u << 20) / (h * w * ts))));
+        const int64_t chunk = std::max<int64_t>(1, (nu + g - 1) / g);
+        g = std::max<int64_t>(1, (nu + chunk - 1) / chunk);
+        L.big.push_back(SnBig{s, g, chunk});
+        if (nu) part = std::max(part, g * h * w);
+        ++sn_tiled_count_;
+      }
+    }
+    L.small1 = (int)small.size();
+  }
+  const int64_t N = S.N, entries = S.off.empty() ? 0 : S.off.back();
+  const double need = (double)entries * ts + (double)part * ts + (double)S.rows.size() * 4 + (double)S.Kpos.size() * 16 +
+                      (double)S.Ksrc.size() * 8 + (double)S.ud.size() * 12 + (double)S.gd.size() * 8 + (double)N * (3 * ts + 24);
+  size_t free_b = 0, total_b = 0;
+  CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+  if (need > 0.9 * (double)free_b) {
+    char b[256];
+    snprintf(b, sizeof(b), "the supernodal LDL' factor does not fit in device memory: %lld stored entries need %.2f GB, %.2f GB free",
+             (long long)S.stored, need * 1e-9, (double)free_b * 1e-9);
+    throw EngineError{COSMO_B200_ERR_ALLOC, b};
+  }
+  sn_sptr_.upload(S.sptr, stream_); sn_rptr_.upload(S.rptr, stream_); sn_rows_.upload(S.rows, stream_); sn_off_.upload(S.off, stream_);
+  sn_uptr_.upload(S.uptr, stream_); sn_ud_.upload(S.ud, stream_); sn_up0_.upload(S.up0, stream_); sn_up1_.upload(S.up1, stream_);
+  sn_Ksp_.upload(S.Ksp, stream_); sn_Ksrc_.upload(S.Ksrc, stream_); sn_Kpos_.upload(S.Kpos, stream_);
+  sn_gptr_.upload(S.gptr, stream_); sn_gd_.upload(S.gd, stream_); sn_gi_.upload(S.gi, stream_);
+  sn_perm_.upload(S.perm, stream_); sn_small_.upload(small, stream_);
+  sn_lrows_.upload(S.lrows, stream_); sn_lcols_.upload(S.lcols, stream_); sn_bcols_.upload(S.bcols, stream_);
+  sn_Lx_.alloc(std::max<int64_t>(entries, 1), false);
+  sn_part_.alloc(std::max<int64_t>(part, 1), false);
+  sn_D_.alloc(std::max<int64_t>(N, 1)); sn_Dinv_.alloc(std::max<int64_t>(N, 1)); sn_y_.alloc(std::max<int64_t>(N, 1));
+  sn_flags_.alloc(2);
+  sync();
+  CUDA_TRY(cudaFuncSetAttribute(sn::sn_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
+  CUDA_TRY(cudaFuncSetAttribute(sn::sn_fdiag_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
+  CUDA_TRY(cudaFuncSetAttribute(sn::sn_backward_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
+  ldl_ev_[0].create();
+  ldl_ev_[1].create();
+  sn_factor_graph_.reset();
+  sn_solve_graph_.reset();
+  sn_ready_ = true;
+  sn_dirty_ = true;
+}
+
+template <typename T>
+static int sn_lower_tiles(int64_t rows, int64_t cols) {   // tiles (bi >= bj) of a rows x cols panel, kTile square
+  const int64_t nrt = (rows + sn::kTile - 1) / sn::kTile, nct = (cols + sn::kTile - 1) / sn::kTile;
+  int64_t t = 0;
+  for (int64_t bj = 0; bj < nct; ++bj) t += nrt - bj;
+  return (int)t;
+}
+
+// Assemble the panels from the resident (scaled) P_, At_, rho_vec_ and sigma and factor them level by level: one
+// captured graph, replayed on every refactorisation.  Reads back the pivot counts (the plugin's only host sync).
+template <typename T>
+void Engine<T>::sn_factor() {
+  if (!sn_ready_) sn_setup();
+  const ldl_sn::Symbolic& S = sn_;
+  if (!sn_factor_graph_) {
+    int nodes = 0;
+    sn::Args<T> a;
+    a.sptr = sn_sptr_.p; a.rptr = sn_rptr_.p; a.rows = sn_rows_.p; a.off = sn_off_.p;
+    a.uptr = sn_uptr_.p; a.ud = sn_ud_.p; a.up0 = sn_up0_.p; a.up1 = sn_up1_.p;
+    a.Lx = sn_Lx_.p; a.D = sn_D_.p; a.Dinv = sn_Dinv_.p; a.flags = sn_flags_.p;
+    const int64_t entries = S.off.empty() ? 0 : S.off.back();
+    capture_graph(sn_factor_graph_, stream_, [&] {
+      ldl_reset_flags_kernel<<<1, 32, 0, stream_>>>(sn_flags_.p); ++nodes;
+      if (entries) { CUDA_TRY(cudaMemsetAsync(sn_Lx_.p, 0, entries * sizeof(T), stream_)); ++nodes; }
+      if (S.nnz_K) {
+        sn::sn_assemble_kernel<T><<<vgrid(S.nnz_K), kBlock, 0, stream_>>>(S.nnz_K, sn_Ksp_.p, sn_Ksrc_.p, sn_Kpos_.p, P_.val.p,
+                                                                          At_.val.p, rho_vec_.p, (T)st_.sigma, sn_Lx_.p);
+        ++nodes;
+      }
+      for (const SnLevel& L : sn_levels_) {
+        if (L.small1 > L.small0) {
+          const int cnt = L.small1 - L.small0;
+          sn::sn_small_kernel<T><<<std::min(cnt, kMaxGrid), kBlock, L.smem, stream_>>>(a, sn_small_.p + L.small0, cnt);
+          ++nodes;
+        }
+        for (const SnBig& B : L.big) {
+          const int s = B.s, c0 = S.sptr[s], w = S.width(s), h = S.height(s);
+          T* F = sn_Lx_.p + S.off[s];
+          const int64_t u0 = S.uptr[s], u1 = S.uptr[s + 1];
+          if (u1 > u0) {
+            sn::sn_tile_update_kernel<T><<<dim3(sn_lower_tiles<T>(h, w), (unsigned)B.groups), kBlock, 0, stream_>>>(
+                a, c0, w, h, sn_rows_.p + S.rptr[s], u0, u1, B.chunk, sn_part_.p);
+            sn::sn_tile_reduce_kernel<T><<<vgrid((int64_t)h * w), kBlock, 0, stream_>>>(F, sn_part_.p, (int)B.groups, h, w);
+            nodes += 2;
+          }
+          for (int b0 = 0; b0 < w; b0 += sn::kTile) {
+            const int nb = std::min(sn::kTile, w - b0), b1 = b0 + nb;
+            const int rows = h - b1;
+            sn::sn_diag_kernel<T><<<1, kBlock, 0, stream_>>>(a, F, c0, h, b0, nb);
+            ++nodes;
+            if (rows > 0) {
+              sn::sn_panel_kernel<T><<<(rows + sn::kPanelThreads - 1) / sn::kPanelThreads, sn::kPanelThreads, 0, stream_>>>(
+                  F, h, b0, nb);
+              ++nodes;
+            }
+            if (b1 < w) {
+              sn::sn_trail_kernel<T><<<sn_lower_tiles<T>(h - b1, w - b1), kBlock, 0, stream_>>>(F, sn_D_.p + c0 + b0, h, w, b0, b1);
+              ++nodes;
+            }
+          }
+        }
+      }
+    });
+    sn_factor_nodes_ = nodes;
+  }
+  int flags[2] = {0, 0};
+  CUDA_TRY(cudaEventRecord(ldl_ev_[0], stream_));
+  CUDA_TRY(cudaGraphLaunch(sn_factor_graph_, stream_));
+  CUDA_TRY(cudaEventRecord(ldl_ev_[1], stream_));
+  CUDA_TRY(cudaMemcpyAsync(flags, sn_flags_.p, sizeof(flags), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  launches_ += sn_factor_nodes_;
+  float ms = 0.f;
+  CUDA_TRY(cudaEventElapsedTime(&ms, ldl_ev_[0], ldl_ev_[1]));
+  sn_factor_s_ = ms * 1e-3;
+  ++sn_factorizations_;
+  if (flags[1] != 0) {
+    char b[160];
+    snprintf(b, sizeof(b), "supernodal LDL' factorisation of the KKT matrix met %d zero or non-finite pivots", flags[1]);
+    throw EngineError{COSMO_B200_ERR_NUMERICAL, b};
+  }
+  if (flags[0] != n_) throw EngineError{COSMO_B200_ERR_INVALID, "Objective function is not convex."};
+  sn_dirty_ = false;
+}
+
+// [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: the forward solve by supernodal level, the
+// backward solve by depth, replayed as one graph
+template <typename T>
+void Engine<T>::sn_solve() {
+  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the supernodal LDL' KKT solver is single-GPU"};
+  if (!sn_ready_) sn_setup();
+  if (sn_dirty_) sn_factor();
+  const ldl_sn::Symbolic& S = sn_;
+  if (!sn_solve_graph_) {
+    int nodes = 0;
+    sn::SolveArgs<T> a;
+    a.sptr = sn_sptr_.p; a.rptr = sn_rptr_.p; a.rows = sn_rows_.p; a.off = sn_off_.p;
+    a.gptr = sn_gptr_.p; a.gd = sn_gd_.p; a.gi = sn_gi_.p;
+    a.Lx = sn_Lx_.p; a.Dinv = sn_Dinv_.p; a.perm = sn_perm_.p;
+    a.rhs = ls_.p; a.y = sn_y_.p; a.out1 = xsol_.p; a.out2 = nu_.p; a.n = n_;
+    // the diagonal solves keep their part of y in shared memory up to kSmallBytes, wider supernodes work on y in place
+    auto vec_smem = [&](int wmax) { return (size_t)wmax * sizeof(T) <= (size_t)sn::kSmallBytes ? (size_t)wmax * sizeof(T) : 0; };
+    capture_graph(sn_solve_graph_, stream_, [&] {
+      for (int l = 0; l < S.levels; ++l) {
+        const int r0 = S.lrptr[l], nr = S.lrptr[l + 1] - r0, k0 = S.lptr[l], ns = S.lptr[l + 1] - k0;
+        sn::sn_gather_kernel<T><<<(int)std::min<int64_t>((nr + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid), kBlock, 0, stream_>>>(
+            a, sn_lrows_.p + r0, nr);
+        ++nodes;
+        if (nr > ns) {   // some supernode of the level is wider than one column
+          int wmax = 1;
+          for (int k = k0; k < k0 + ns; ++k) wmax = std::max(wmax, S.width(S.lcols[k]));
+          const size_t sm = vec_smem(wmax);
+          sn::sn_fdiag_kernel<T><<<std::min(ns, kMaxGrid), kBlock, sm, stream_>>>(a, sn_lcols_.p + k0, ns, sm > 0);
+          ++nodes;
+        }
+      }
+      for (size_t l = 0; l + 1 < S.bptr.size(); ++l) {
+        const int k0 = S.bptr[l], ns = S.bptr[l + 1] - k0;
+        int wmax = 1;
+        for (int k = k0; k < k0 + ns; ++k) wmax = std::max(wmax, S.width(S.bcols[k]));
+        const size_t sm = vec_smem(wmax);
+        sn::sn_backward_kernel<T><<<std::min(ns, kMaxGrid), kBlock, sm, stream_>>>(a, sn_bcols_.p + k0, ns, sm > 0);
+        ++nodes;
+      }
+    });
+    sn_solve_nodes_ = nodes;
+  }
+  CUDA_TRY(cudaGraphLaunch(sn_solve_graph_, stream_));
+  launches_ += sn_solve_nodes_;
+}
+
+template <typename T>
+void Engine<T>::ldl_sn_stats(int64_t* o) {
+  o[0] = sn_.ns; o[1] = sn_.max_width; o[2] = sn_.zeros(); o[3] = sn_.levels;
+  o[4] = sn_ready_ ? sn_small_count_ : 0; o[5] = sn_ready_ ? sn_tiled_count_ : 0; o[6] = sn_solve_nodes_;
+  o[7] = (int64_t)sn_.update_flops;
 }
 
 template <typename T>
@@ -2919,6 +3171,30 @@ int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* p, int64_t* perm, int64_t*
       colcount[j] = S.Lp[j + 1] - S.Lp[j];
       level[j] = S.level[j];
     }
+    return COSMO_B200_OK;
+  } catch (...) { return error_code(cosmo::g_create_error); }
+}
+int cosmo_b200_ldl_sn_stats(cosmo_b200_handle* h, int64_t out[8]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->ldl_sn_stats(out));
+}
+int cosmo_b200_ldl_sn_symbolic(const cosmo_b200_problem* p, int64_t* perm, int64_t* snode_ptr, int64_t* snode_parent, int64_t stats[8]) {
+  if (!p || !perm || !snode_ptr || !snode_parent || !stats) { cosmo::g_create_error = "null argument"; return COSMO_B200_ERR_INVALID; }
+  try {
+    if (p->m < 0 || p->n < 0 || p->A.nrows != p->m || p->A.ncols != p->n || p->P.nrows != p->n || p->P.ncols != p->n)
+      throw cosmo::EngineError{COSMO_B200_ERR_INVALID, "P must be n x n and A m x n"};
+    if (p->dtype != COSMO_B200_F64 && p->dtype != COSMO_B200_F32)
+      throw cosmo::EngineError{COSMO_B200_ERR_UNSUPPORTED, "dtype must be Float64 or Float32"};
+    cosmo::HostCsr a, at, pp, ppt;
+    cosmo::csc_to_host_csrs(p->A, p->index_base, a, at);
+    cosmo::csc_to_host_csrs(p->P, p->index_base, pp, ppt);
+    cosmo::ldl_sn::Symbolic S;
+    cosmo::ldl_sn::analyze((int)p->n, (int)p->m, pp.rowptr, pp.col, at.rowptr, at.col, S);
+    for (int j = 0; j < S.N; ++j) perm[j] = S.perm[j];
+    for (int s = 0; s <= S.ns; ++s) snode_ptr[s] = S.sptr[s];
+    for (int s = 0; s < S.ns; ++s) snode_parent[s] = S.sparent[s];
+    stats[0] = S.ns; stats[1] = S.max_width; stats[2] = S.stored; stats[3] = S.zeros();
+    stats[4] = S.levels; stats[5] = S.simplicial_levels; stats[6] = S.nnz_L; stats[7] = (int64_t)S.update_flops;
     return COSMO_B200_OK;
   } catch (...) { return error_code(cosmo::g_create_error); }
 }

@@ -22,25 +22,31 @@
 
 namespace cosmo {
 
-// Kx[e] = sum of the sources of entry e, in the order the host listed them
+// the sum of the sources of entry e of K, in the order the host listed them
+template <typename T>
+__device__ __forceinline__ T ldl_entry_value(int64_t e, const int64_t* __restrict__ Ksp, const int64_t* __restrict__ Ksrc,
+                                             const T* __restrict__ Pval, const T* __restrict__ Atval,
+                                             const T* __restrict__ rho, T sigma) {
+  T v = T(0);
+  for (int64_t s = Ksp[e]; s < Ksp[e + 1]; ++s) {
+    const int64_t code = Ksrc[s];
+    const int64_t idx = code >> 2;
+    switch ((int)(code & 3)) {
+      case ldl::SRC_P: v += Pval[idx]; break;
+      case ldl::SRC_AT: v += Atval[idx]; break;
+      case ldl::SRC_RHO: v += -T(1) / rho[idx]; break;
+      default: v += sigma; break;
+    }
+  }
+  return v;
+}
+
 template <typename T>
 __global__ void ldl_assemble_kernel(int64_t nnz, const int64_t* __restrict__ Ksp, const int64_t* __restrict__ Ksrc,
                                     const T* __restrict__ Pval, const T* __restrict__ Atval, const T* __restrict__ rho,
                                     T sigma, T* __restrict__ Kx) {
-  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x) {
-    T v = T(0);
-    for (int64_t s = Ksp[e]; s < Ksp[e + 1]; ++s) {
-      const int64_t code = Ksrc[s];
-      const int64_t idx = code >> 2;
-      switch ((int)(code & 3)) {
-        case ldl::SRC_P: v += Pval[idx]; break;
-        case ldl::SRC_AT: v += Atval[idx]; break;
-        case ldl::SRC_RHO: v += -T(1) / rho[idx]; break;
-        default: v += sigma; break;
-      }
-    }
-    Kx[e] = v;
-  }
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x)
+    Kx[e] = ldl_entry_value(e, Ksp, Ksrc, Pval, Atval, rho, sigma);
 }
 
 template <typename T>

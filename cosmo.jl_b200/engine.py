@@ -23,7 +23,7 @@ CUSTOM_THREAD, CUSTOM_WARP, CUSTOM_BLOCK = 0, 1, 2
 CUSTOM_HAS_IN_DUAL, CUSTOM_HAS_IN_POL_RECC = 1, 2
 STATUS = {0: "Undetermined", 1: "Solved", 2: "Max_iter_reached", 3: "Time_limit_reached",
           4: "Primal_infeasible", 5: "Dual_infeasible", 6: "Unsolved"}
-KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES, KKT_LDL = 0, 1, 2, 3
+KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES, KKT_LDL, KKT_LDL_SUPERNODAL = 0, 1, 2, 3, 4
 ACC_EMPTY, ACC_ANDERSON = 0, 1
 AA_TYPE2_QR, AA_TYPE2_NORMAL, AA_TYPE1 = 0, 1, 2
 AA_RESTARTED_MEMORY, AA_ROLLING_MEMORY = 0, 1
@@ -146,6 +146,8 @@ def _signatures():
         "cosmo_b200_psd_lambda_max": (rc, [vp, vp, P(f64)]),
         "cosmo_b200_ldl_stats": (rc, [vp, P(f64)]),
         "cosmo_b200_ldl_symbolic": (rc, [P(ProblemStruct), P(i64), P(i64), P(i64), P(i64)]),
+        "cosmo_b200_ldl_sn_stats": (rc, [vp, P(i64)]),
+        "cosmo_b200_ldl_sn_symbolic": (rc, [P(ProblemStruct), P(i64), P(i64), P(i64), P(i64)]),
         "cosmo_b200_set_decomposition": (rc, [vp, P(DecompositionStruct)]),
         "cosmo_b200_set_decomposition_noncompact": (rc, [vp, P(DecompositionStruct)]),
         "cosmo_b200_reverse_decomposition": (rc, [vp, i32, vp, vp, vp, P(i64)]),
@@ -556,6 +558,10 @@ class Engine:
         """State of the direct LDL' plugin (cosmo_b200_ldl_stats), keyed by LDL_STATS."""
         return self._read_out(self._lib.cosmo_b200_ldl_stats, ctype=C.c_double, keys=LDL_STATS, ints=LDL_STATS[:6])
 
+    def ldl_sn_stats(self):
+        """State of the supernodal LDL' plugin (cosmo_b200_ldl_sn_stats), keyed by LDL_SN_STATS."""
+        return self._read_out(self._lib.cosmo_b200_ldl_sn_stats, ctype=C.c_int64, keys=LDL_SN_STATS)
+
     # ---- reverse of a chordal decomposition ---------------------------------
     def set_decomposition(self, d):
         """cosmo_b200_set_decomposition, or cosmo_b200_set_decomposition_noncompact for the map of the traditional
@@ -636,6 +642,11 @@ CUSTOM_CONE_STATS = ("types", "cones", "compilations", "cache_hits")
 
 LDL_STATS = ("N", "nnz_triu_K", "nnz_L", "levels", "solve_nodes", "factorizations", "factor_time", "symbolic_time")
 
+LDL_SN_STATS = ("supernodes", "max_width", "explicit_zeros", "levels", "small_path", "tiled_path", "solve_nodes",
+                "update_flops")
+LDL_SN_SYMBOLIC_STATS = ("supernodes", "max_width", "stored", "explicit_zeros", "levels", "simplicial_levels", "nnz_L",
+                         "update_flops")
+
 ACCELERATOR_STATS = ("accepted", "declined", "rejected", "rho_restarts", "memory_restarts", "activated_at")
 
 
@@ -653,6 +664,27 @@ def ldl_symbolic(P, A):
     out = [np.zeros(prob.n + prob.m, dtype=np.int64) for _ in range(4)]
     _check_rc(lib, lib.cosmo_b200_ldl_symbolic(C.byref(prob), *[o.ctypes.data_as(C.POINTER(C.c_int64)) for o in out]))
     return tuple(out)
+
+
+def ldl_sn_symbolic(P, A):
+    """cosmo_b200_ldl_sn_symbolic: the supernodal symbolic analysis (no GPU needed).  Returns (perm, snode_ptr,
+    snode_parent, stats): the postordered pivots, the supernodes' column pointers and parents, and a dict keyed by
+    LDL_SN_SYMBOLIC_STATS."""
+    import scipy.sparse as sp
+    lib = load_library()
+    P = sp.csc_matrix(P, dtype=np.float64)
+    A = sp.csc_matrix(A, dtype=np.float64)
+    P.sort_indices()
+    A.sort_indices()
+    keep = []
+    prob = problem_struct(P, A, np.float64, 0, keep)
+    N = prob.n + prob.m
+    perm, sptr, spar = np.zeros(N, dtype=np.int64), np.zeros(N + 1, dtype=np.int64), np.zeros(max(N, 1), dtype=np.int64)
+    stats = _keyed(lib, None, lib.cosmo_b200_ldl_sn_symbolic, C.byref(prob),
+                   *[o.ctypes.data_as(C.POINTER(C.c_int64)) for o in (perm, sptr, spar)], ctype=C.c_int64,
+                   keys=LDL_SN_SYMBOLIC_STATS)
+    ns = stats["supernodes"]
+    return perm, sptr[:ns + 1].copy(), spar[:ns].copy(), stats
 
 
 def tc_gemm(A, B, slices=8, groups=0, reps=0):

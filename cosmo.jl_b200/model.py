@@ -266,7 +266,8 @@ class Settings:
     max_iter: int = 5000
     verbose: bool = False
     verbose_timing: bool = False             # settings.jl:43: here it forces the device phase timers (proj_time, kkt_time)
-    kkt_solver: str = "CGIndirectKKTSolver"   # the indirect family, or "DeviceLdlKKTSolver" (direct LDL' on the device)
+    kkt_solver: str = "CGIndirectKKTSolver"   # the indirect family, "DeviceLdlKKTSolver" (direct LDL' on the device) or
+    #                                          "DeviceSupernodalKKTSolver" / "MKLPardisoKKTSolver" (supernodal LDL')
     check_termination: int = 25
     check_infeasibility: int = 40
     scaling: int = 10
@@ -315,7 +316,8 @@ class Settings:
     reverse_on_device: bool = False
 
     _KKT = {"CGIndirectKKTSolver": _eng.KKT_CG, "MINRESIndirectKKTSolver": _eng.KKT_MINRES,
-            "IndirectReducedKKTSolver:MINRES": _eng.KKT_MINRES_REDUCED, "DeviceLdlKKTSolver": _eng.KKT_LDL}
+            "IndirectReducedKKTSolver:MINRES": _eng.KKT_MINRES_REDUCED, "DeviceLdlKKTSolver": _eng.KKT_LDL,
+            "DeviceSupernodalKKTSolver": _eng.KKT_LDL_SUPERNODAL, "MKLPardisoKKTSolver": _eng.KKT_LDL_SUPERNODAL}
     _AA_TYPE = {"Type2{QRDecomp}": _eng.AA_TYPE2_QR, "Type2{NormalEquations}": _eng.AA_TYPE2_NORMAL, "Type1": _eng.AA_TYPE1}
     _AA_MEMORY = {"RestartedMemory": _eng.AA_RESTARTED_MEMORY, "RollingMemory": _eng.AA_ROLLING_MEMORY}
     _AA_REG = {"NoRegularizer": _eng.AA_NO_REGULARIZER, "TikonovRegularizer": _eng.AA_TIKONOV,
@@ -356,8 +358,9 @@ class Settings:
         if self.kkt_solver not in self._KKT:
             raise _eng.EngineError(_eng.ERR_UNSUPPORTED,
                                    "kkt_solver %r is not an engine plugin: the H100 engine implements CGIndirectKKTSolver, "
-                                   "MINRESIndirectKKTSolver and, for a direct LDL' factorisation as QdldlKKTSolver does, "
-                                   "DeviceLdlKKTSolver" % self.kkt_solver)
+                                   "MINRESIndirectKKTSolver, for a direct LDL' factorisation as QdldlKKTSolver does, "
+                                   "DeviceLdlKKTSolver and, for a supernodal one as MKLPardisoKKTSolver does, "
+                                   "DeviceSupernodalKKTSolver (also selected as MKLPardisoKKTSolver)" % self.kkt_solver)
         if self.accelerator not in ("EmptyAccelerator", "AndersonAccelerator"):
             raise _eng.EngineError(_eng.ERR_UNSUPPORTED,
                                    "accelerator %r: the engine implements EmptyAccelerator and AndersonAccelerator "

@@ -107,7 +107,7 @@ def create_engine(shard: Shard, settings: M.Settings, device: int = 0, dist=None
                   dtype=np.float64) -> _eng.Engine:
     """Build the per-rank engine; with world > 1 rank 0 creates the ncclUniqueId and
     `torch.distributed` (the plumbing) broadcasts its 128 bytes."""
-    if shard.world > 1 and settings.kkt_solver == "DeviceLdlKKTSolver":
+    if shard.world > 1 and settings.to_struct().kkt_solver in (_eng.KKT_LDL, _eng.KKT_LDL_SUPERNODAL):
         raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU (use CG or reduced MINRES when sharded)")
     tuples = [M.set_tuple(S) for S in shard.sets]
     eng = _eng.Engine(shard.P, shard.q, shard.A, shard.b, tuples, settings.to_struct(), D=D,

@@ -149,8 +149,11 @@ enum {
   COSMO_B200_KKT_CG = 0,             /* CGIndirectKKTSolver      (reduced system, CG)      :3-88   */
   COSMO_B200_KKT_MINRES_REDUCED = 1, /* IndirectReducedKKTSolver(solver_type = :MINRES)    :3-88   */
   COSMO_B200_KKT_MINRES = 2,         /* MINRESIndirectKKTSolver  (full KKT, MINRES)        :90-162 */
-  COSMO_B200_KKT_LDL = 3             /* direct LDL' of the full KKT matrix on the device, the counterpart of
+  COSMO_B200_KKT_LDL = 3,            /* direct LDL' of the full KKT matrix on the device, the counterpart of
                                         QdldlKKTSolver (kktsolver.jl:285-320); single-GPU */
+  COSMO_B200_KKT_LDL_SUPERNODAL = 4  /* supernodal LDL' of the full KKT matrix on the device (dense panels), the
+                                        counterpart of the Pardiso plugins' direct solve (kktsolver_pardiso.jl);
+                                        same contract as COSMO_B200_KKT_LDL; single-GPU */
 };
 
 /* SparseMatrixCSC{T,Int64} as Julia stores it */
@@ -375,6 +378,23 @@ int cosmo_b200_ldl_stats(cosmo_b200_handle* h, double out[8]);
    permuted K (-1: root), colcount[k] = entries of column k of L below the diagonal, level[k] = 0 for a leaf, else
    1 + the largest level of its children.  Errors through cosmo_b200_last_error(NULL). */
 int cosmo_b200_ldl_symbolic(const cosmo_b200_problem* prob, int64_t* perm, int64_t* parent, int64_t* colcount, int64_t* level);
+
+/* ---- supernodal LDL' KKT plugin (kkt_solver = COSMO_B200_KKT_LDL_SUPERNODAL) ---- */
+/* The contract of COSMO_B200_KKT_LDL (factor at create, lazy refactorisation, the same errors, single-GPU), on the
+   ordering of COSMO_B200_KKT_LDL renumbered by a postorder of the elimination tree: the factor is that plugin's up to
+   a symmetric permutation.  Columns are grouped into supernodes (dense panels, relaxed amalgamation); small ones
+   factor in one CTA each, large ones tiled across CTAs.  cosmo_b200_ldl_stats answers for this plugin too (nnz_L:
+   stored entries, explicit zeros included; levels: supernodal levels).  out[8] = {supernodes, maximum width, explicit
+   zeros, supernodal levels, supernodes on the small path, supernodes on the tiled path, kernel nodes per solve,
+   flops of the descendant updates of one factorisation}; 0 where the handle never used the plugin. */
+int cosmo_b200_ldl_sn_stats(cosmo_b200_handle* h, int64_t out[8]);
+/* The supernodal symbolic analysis alone, on the host (no GPU needed).  perm (N = n + m entries): perm[k] = original
+   index of pivot k in the postordered numbering; snode_ptr (N + 1 entries, the first supernodes + 1 used): columns of
+   supernode s are [snode_ptr[s], snode_ptr[s+1]); snode_parent (N entries, the first supernodes used): the parent
+   supernode, -1 for a root.  stats = {supernodes, maximum width, stored entries, explicit zeros, supernodal levels,
+   simplicial levels, nnz(L), flops of the descendant updates}.  Errors through cosmo_b200_last_error(NULL). */
+int cosmo_b200_ldl_sn_symbolic(const cosmo_b200_problem* prob, int64_t* perm, int64_t* snode_ptr, int64_t* snode_parent,
+                               int64_t stats[8]);
 
 /* ---- reverse of a chordal decomposition (reverse_decomposition! + psd_completion!,
         chordal_decomposition.jl:129-311) ------------------------------------ */
