@@ -35,18 +35,21 @@ __global__ void __launch_bounds__(kBlock) fwd_values_kernel(long long n, const I
   }
 }
 
-// out[i] = b[src[i]]; 0 for src[i] = -1; b[-2 - src[i]] with -0.0 -> +0.0 below that
-template <typename T, typename I>
+// out[i] = b[src[i]]; 0 for src[i] = -1; b[-2 - src[i]] with -0.0 -> +0.0 below that.  With E: out[i] = O(E[i] * that),
+// the product taken in fp64 (update!(b=) of an original-coordinate fp64 b on a scaled engine)
+template <typename T, typename I, typename O>
 __global__ void __launch_bounds__(kBlock) fwd_b_kernel(long long m, const I* __restrict__ src, const T* __restrict__ b,
-                                                       T* __restrict__ out) {
+                                                       const O* __restrict__ E, O* __restrict__ out) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < m; i += (long long)gridDim.x * blockDim.x) {
     const I s = src[i];
+    T v;
     if (s >= -1) {
-      out[i] = s >= 0 ? b[s] : T(0);
+      v = s >= 0 ? b[s] : T(0);
     } else {
-      const T v = b[-2 - s];
-      out[i] = v == T(0) ? T(0) : v;
+      v = b[-2 - s];
+      if (v == T(0)) v = T(0);
     }
+    out[i] = E ? O((double)E[i] * (double)v) : O(v);
   }
 }
 
@@ -166,11 +169,11 @@ class Forward {
     CUDA_TRY(cudaGetLastError());
   }
 
-  // b' (m) from the staged b (device, m_orig)
-  template <typename T>
-  void gather_b(const T* b, T* out, cudaStream_t st) {
-    if (wide_) fwd_b_kernel<T, int64_t><<<grid_for(m_), kBlock, 0, st>>>(m_, b64_.p, b, out);
-    else fwd_b_kernel<T, int><<<grid_for(m_), kBlock, 0, st>>>(m_, b32_.p, b, out);
+  // b' (m) from the staged b (device, m_orig), times E when E is not null
+  template <typename T, typename O = T>
+  void gather_b(const T* b, O* out, cudaStream_t st, const O* E = nullptr) {
+    if (wide_) fwd_b_kernel<T, int64_t, O><<<grid_for(m_), kBlock, 0, st>>>(m_, b64_.p, b, E, out);
+    else fwd_b_kernel<T, int, O><<<grid_for(m_), kBlock, 0, st>>>(m_, b32_.p, b, E, out);
     CUDA_TRY(cudaGetLastError());
   }
 

@@ -166,6 +166,11 @@ __global__ void __launch_bounds__(kThreads) gather_back_kernel(int64_t N, const 
   }
 }
 
+// y = -mu of the reversed solution (cosmo_b200_solution)
+__global__ void __launch_bounds__(kThreads) negate_kernel(int64_t n, double* v) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) v[i] = -v[i];
+}
+
 // the bare matrix of cosmo_b200_psd_complete: its upper triangle into the traversal numbering, and back
 __global__ void __launch_bounds__(kThreads) permute_in_kernel(int64_t N, const double* Y, const int64_t* new_of, double* W) {
   for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < N * N; e += (int64_t)gridDim.x * blockDim.x) {
@@ -624,7 +629,7 @@ class Reverse {
 
   template <typename T>
   void run(const T* x, const T* s, const T* mu, const T* D, const T* E, double c, bool complete_dual, void* hx, void* hs,
-           void* hmu, int64_t* stats, cudaStream_t st, int device) {
+           void* hmu, int64_t* stats, cudaStream_t st, int device, bool negate_mu = false) {
     if (!set_) fail(COSMO_B200_ERR_INVALID, "reverse_decomposition: no decomposition map (cosmo_b200_set_decomposition)");
     ensure(x_, std::max<int64_t>(n_orig_, 1), 0);
     ensure(s_, std::max<int64_t>(m_orig_, 1), 0);
@@ -659,10 +664,14 @@ class Reverse {
         CUDA_TRY(cudaGetLastError());
       }
     }
+    if (hmu && negate_mu) {
+      negate_kernel<<<grid_for(m_orig_), kThreads, 0, st>>>(m_orig_, mu_.p);
+      CUDA_TRY(cudaGetLastError());
+    }
     CUDA_TRY(cudaEventRecord(ev_[1], st));
-    if (hx) CUDA_TRY(cudaMemcpyAsync(hx, x_.p, n_orig_ * sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (hs) CUDA_TRY(cudaMemcpyAsync(hs, s_.p, m_orig_ * sizeof(double), cudaMemcpyDeviceToHost, st));
-    if (hmu) CUDA_TRY(cudaMemcpyAsync(hmu, mu_.p, m_orig_ * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (hx) CUDA_TRY(cudaMemcpyAsync(hx, x_.p, n_orig_ * sizeof(double), cudaMemcpyDefault, st));
+    if (hs) CUDA_TRY(cudaMemcpyAsync(hs, s_.p, m_orig_ * sizeof(double), cudaMemcpyDefault, st));
+    if (hmu) CUDA_TRY(cudaMemcpyAsync(hmu, mu_.p, m_orig_ * sizeof(double), cudaMemcpyDefault, st));
     int fallbacks = 0;
     CUDA_TRY(cudaMemcpyAsync(&fallbacks, cnt_.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));

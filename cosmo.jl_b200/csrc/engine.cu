@@ -189,6 +189,11 @@ class EngineBase {
                                         const void* b) = 0;
   virtual void reverse_decomposition(int complete_dual, void* x, void* s, void* mu, int64_t* stats4) = 0;
   virtual void custom_cone_stats(int64_t* out4) = 0;
+  virtual void set_caller_stream(void* stream) = 0;
+  virtual void update_qb_original(const double* q, const double* b) = 0;
+  virtual void original_qb(double* q, double* b) = 0;
+  virtual void solution(int complete_dual, double* x, double* y, double* s) = 0;
+  virtual void rescale_iterates() = 0;
 };
 
 template <typename T>
@@ -239,6 +244,14 @@ class Engine : public EngineBase {
   void custom_cone_stats(int64_t* out4) override {
     out4[0] = (int64_t)cust_types_.size(); out4[1] = n_cust_; out4[2] = cust_compiled_; out4[3] = cust_hits_;
   }
+  void set_caller_stream(void* stream) override {
+    single_gpu("set_caller_stream");
+    caller_stream_ = static_cast<cudaStream_t>(stream);
+  }
+  void update_qb_original(const double* q, const double* b) override;
+  void original_qb(double* q, double* b) override;
+  void solution(int complete_dual, double* x, double* y, double* s) override;
+  void rescale_iterates() override;
 
  private:
   // ---- problem ----
@@ -308,6 +321,18 @@ class Engine : public EngineBase {
   bool have_solution_ = false;   // xs_, s_, mu_ hold what the last solve() returned (cleared by reset / warm_start)
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
+  rev::Reverse ident_;           // the identity map: cosmo_b200_solution of a handle without a decomposition map
+  // q and b of the last update_qb_original, fp64 in the original coordinates (allocated on first use)
+  DevBuf<double> q0_, b0_;
+  bool have_q0_ = false, have_b0_ = false;
+  // caller arrays in device memory are ordered on caller_stream_ (cosmo_b200_set_caller_stream)
+  cudaStream_t caller_stream_ = nullptr;
+  Event caller_ev_;
+  unsigned caller_arrays(std::initializer_list<const void*> ptrs);
+  void caller_written();
+  void single_gpu(const char* what) const {
+    if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, std::string(what) + ": a sharded handle holds only a slice of the data"};
+  }
   // KKT (reduced CG)
   DevBuf<T> ls_, t0_, tm_, xsol_, rhsb_, cb_, r_, u_, nu_;
   DevBuf<T> mr_[6], mr_x_, mr_c_, mr_b_;   // MINRES Lanczos / direction vectors, solution, operator output, rhs
@@ -485,12 +510,12 @@ class Engine : public EngineBase {
 template <typename T>
 void Engine<T>::upload_vec(DevBuf<T>& dst, const void* host, size_t count) {
   if (count == 0) return;
-  CUDA_TRY(cudaMemcpyAsync(dst.p, host, count * sizeof(T), cudaMemcpyHostToDevice, stream_));
+  CUDA_TRY(cudaMemcpyAsync(dst.p, host, count * sizeof(T), cudaMemcpyDefault, stream_));
 }
 template <typename T>
 void Engine<T>::download_vec(void* host, const T* src, size_t count) {
   if (count == 0) return;
-  CUDA_TRY(cudaMemcpyAsync(host, src, count * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(host, src, count * sizeof(T), cudaMemcpyDefault, stream_));
 }
 
 template <typename T>
@@ -1172,6 +1197,7 @@ void Engine<T>::get_scaling(void* D, void* E, double* c) {
 
 template <typename T>
 void Engine<T>::warm_start(const void* x, const void* s, const void* mu) {
+  caller_arrays({x, s, mu});
   have_solution_ = false;
   if (x) upload_vec(xs_, x, n_);
   if (s) upload_vec(s_, s, m_);
@@ -1181,6 +1207,7 @@ void Engine<T>::warm_start(const void* x, const void* s, const void* mu) {
 
 template <typename T>
 void Engine<T>::update_qb(const void* q, const void* b) {
+  caller_arrays({q, b});
   if (q) upload_vec(q_, q, n_);
   if (b) {
     upload_vec(b_, b, m_);
@@ -1199,7 +1226,7 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
   // Ruiz restarts from identity on the unscaled data, and the engine keeps only the scaled values
   if (device_scaled_ && !(Px && Ax && q && b))
     throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices: an equilibrating engine needs the unscaled P, A, q and b"};
-  CUDA_TRY(cudaSetDevice(device_));
+  caller_arrays({Px, Ax, q, b});
   const double t0 = now_s();
   DevBuf<T> px;
   upload_values(Px, Ax, q, b, px);
@@ -1218,7 +1245,7 @@ void Engine<T>::update_matrices_original(const void* Px, long long nnzP, const v
     throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: nnz differs from the pattern the decomposition was made for (a new pattern needs a new engine)"};
   if (device_scaled_ && !(Px && Ax && q && b))
     throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: an equilibrating engine needs the unscaled P, A, q and b"};
-  CUDA_TRY(cudaSetDevice(device_));
+  caller_arrays({Px, Ax, q, b});
   const double t0 = now_s();
   DevBuf<T> px, ax, b0;
   if (Px) px.alloc((size_t)P_.nnz, false);
@@ -2251,7 +2278,7 @@ void Engine<T>::accelerator_stats(int64_t* out) {
 template <typename T>
 void Engine<T>::solve(cosmo_b200_result* out) {
   const double t_start = now_s();
-  CUDA_TRY(cudaSetDevice(device_));
+  const unsigned dev_out = out ? caller_arrays({out->x, out->s, out->mu}) : 0u;
   const int n = n_, m = m_;
   const long long launches0 = launches_;
   total_inner_ = 0; total_mults_ = 0;
@@ -2455,6 +2482,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
     if (out->x) download_vec(out->x, W_[prev_].p, n);
     if (out->s) download_vec(out->s, s_.p, m);
     if (out->mu) download_vec(out->mu, mu_.p, m);
+    if (dev_out) caller_written();
     sync();
     out->obj_val = cost;
     out->iter = iter + safeguarding_iter;      // total_iter, solver.jl:195
@@ -3001,6 +3029,7 @@ void Engine<T>::set_forward_map(const cosmo_b200_forward_map* f) {
   CUDA_TRY(cudaSetDevice(device_));
   if (!f) fwd_.clear();
   else fwd_.set(*f, n_, m_, At_.nnz, stream_);
+  have_q0_ = have_b0_ = false;   // their sizes follow the map
 }
 
 // reverse_scaling! + reverse_decomposition! (+ psd_completion!) of the iterates the last solve left in HBM
@@ -3010,9 +3039,143 @@ void Engine<T>::reverse_decomposition(int complete_dual, void* x, void* s, void*
   if (!rev_.has_map()) throw EngineError{COSMO_B200_ERR_INVALID, "reverse_decomposition: no decomposition map (cosmo_b200_set_decomposition)"};
   if (!have_solution_)
     throw EngineError{COSMO_B200_ERR_INVALID, "reverse_decomposition: no solve since the engine was created, reset or warm-started"};
-  CUDA_TRY(cudaSetDevice(device_));
+  const unsigned dev = caller_arrays({x, s, mu});
   rev_.run<T>(xs_.p, s_.p, mu_.p, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, complete_dual != 0,
               x, s, mu, stats4, stream_, device_);
+  if (dev) caller_written();
+}
+
+// Checks the caller's array arguments before anything is written: each may be host memory, device memory of this
+// handle's device or managed memory (the copies use cudaMemcpyDefault).  When one is device or managed memory, the
+// engine stream waits for the work the caller enqueued on its stream.  Returns those arguments as a mask (bit k: the
+// k-th pointer).
+template <typename T>
+unsigned Engine<T>::caller_arrays(std::initializer_list<const void*> ptrs) {
+  CUDA_TRY(cudaSetDevice(device_));
+  unsigned dev = 0, bit = 1;
+  for (const void* p : ptrs) {
+    cudaPointerAttributes a{};
+    if (p) CUDA_TRY(cudaPointerGetAttributes(&a, p));
+    if (p && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged)) {
+      if (a.type == cudaMemoryTypeDevice && a.device != device_)
+        throw EngineError{COSMO_B200_ERR_INVALID, "an array lies in the memory of device " + std::to_string(a.device) +
+                                                      ", the engine on device " + std::to_string(device_)};
+      dev |= bit;
+    }
+    bit <<= 1;
+  }
+  if (dev) {
+    caller_ev_.create();
+    CUDA_TRY(cudaEventRecord(caller_ev_, caller_stream_));
+    CUDA_TRY(cudaStreamWaitEvent(stream_, caller_ev_, 0));
+  }
+  return dev;
+}
+
+// After the engine wrote caller device or managed memory: the caller stream waits for the engine stream.
+template <typename T>
+void Engine<T>::caller_written() {
+  caller_ev_.create();
+  CUDA_TRY(cudaEventRecord(caller_ev_, stream_));
+  CUDA_TRY(cudaStreamWaitEvent(caller_stream_, caller_ev_, 0));
+}
+
+// update!(q=, b=) in the model's coordinates, unscaled fp64: through the forward map when one is set, then scaled as the
+// host scales (scale_original_qb_kernel), then update_qb's state change.  The b is checked for uncovered rows before
+// anything is written.
+template <typename T>
+void Engine<T>::update_qb_original(const double* q, const double* b) {
+  single_gpu("update_qb_original");
+  const bool dev_b = (caller_arrays({q, b}) & 2) != 0;
+  const bool mapped = fwd_.has_map();
+  const size_t n0 = mapped ? (size_t)fwd_.n_orig() : (size_t)n_, m0 = mapped ? (size_t)fwd_.m_orig() : (size_t)m_;
+  DevBuf<double> stage;   // a host b is checked on the device before b0_ changes
+  const double* bsrc = b;
+  if (b && mapped) {
+    if (!dev_b && m0) {
+      stage.alloc(m0, false);
+      stage.upload(b, m0, stream_);
+      bsrc = stage.p;
+    }
+    const long long bad = fwd_.count_uncovered<double>(bsrc, stream_);
+    launches_ += 2;
+    if (bad)
+      throw EngineError{COSMO_B200_ERR_INVALID, "update_qb_original: b is nonzero in " + std::to_string(bad) +
+                                                    " rows of a decomposed cone that no clique holds (the sparsity pattern, and with it the decomposition, changes: a new engine is needed)"};
+  }
+  if (q) {
+    if (!q0_.p || q0_.n != n0) q0_.alloc(n0, false);
+    if (n0) CUDA_TRY(cudaMemcpyAsync(q0_.p, q, n0 * sizeof(double), cudaMemcpyDefault, stream_));
+    have_q0_ = true;
+  }
+  if (b) {
+    if (!b0_.p || b0_.n != m0) b0_.alloc(m0, false);
+    if (m0) CUDA_TRY(cudaMemcpyAsync(b0_.p, bsrc, m0 * sizeof(double), cudaMemcpyDefault, stream_));
+    have_b0_ = true;
+  }
+  const T* D = scaled_ ? D_.p : nullptr;
+  const T* E = scaled_ ? E_.p : nullptr;
+  const long long nq = q ? n_ : 0, mb = b && !mapped ? m_ : 0;
+  if (nq + mb) {
+    scale_original_qb_kernel<T><<<vgrid(nq + mb), kBlock, 0, stream_>>>(nq, (long long)n0, q0_.p, D, scaled_ ? c_ : 1.0,
+                                                                         q_.p, mb, b0_.p, E, b_.p);
+    check_launch("scale_original_qb");
+  }
+  if (b && mapped) {
+    fwd_.gather_b<double, T>(b0_.p, b_.p, stream_, E);
+    ++launches_;
+  }
+  if (b) classify_and_set_rho(false);
+  sync();
+}
+
+template <typename T>
+void Engine<T>::original_qb(double* q, double* b) {
+  single_gpu("original_qb");
+  if ((q && !have_q0_) || (b && !have_b0_))
+    throw EngineError{COSMO_B200_ERR_INVALID, "original_qb: no q or b from update_qb_original since the forward map was set"};
+  const unsigned dev = caller_arrays({q, b});
+  if (q && q0_.n) CUDA_TRY(cudaMemcpyAsync(q, q0_.p, q0_.n * sizeof(double), cudaMemcpyDefault, stream_));
+  if (b && b0_.n) CUDA_TRY(cudaMemcpyAsync(b, b0_.p, b0_.n * sizeof(double), cudaMemcpyDefault, stream_));
+  if (dev) caller_written();
+  sync();
+}
+
+// The last solution in the original coordinates: reverse_decomposition's arithmetic with a decomposition map, else the
+// same gather through the identity map (x = D x', s = s' / E, mu = (E mu') / c), with y = -mu.
+template <typename T>
+void Engine<T>::solution(int complete_dual, double* x, double* y, double* s) {
+  single_gpu("solution");
+  if (!have_solution_)
+    throw EngineError{COSMO_B200_ERR_INVALID, "solution: no solve since the engine was created, reset or warm-started"};
+  const unsigned dev = caller_arrays({x, y, s});
+  rev::Reverse* r = &rev_;
+  if (!rev_.has_map()) {
+    if (!ident_.has_map()) {
+      const int64_t plain[3] = {0, 0, m_};
+      cosmo_b200_decomposition d{};
+      d.n_orig = n_; d.m_orig = m_; d.n = n_; d.m = m_;
+      d.n_plain = m_ ? 1 : 0; d.plain = plain;
+      ident_.set(d, n_, m_, stream_);
+    }
+    r = &ident_;
+  }
+  r->run<T>(xs_.p, s_.p, mu_.p, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, complete_dual != 0,
+            x, s, y, nullptr, stream_, device_, true);
+  if (dev) caller_written();
+}
+
+// The host's round trip between two solves (reverse_scaling!, then scale_variables! of the result as the next warm
+// start) on the resident iterates; like warm_start it ends the last solution.
+template <typename T>
+void Engine<T>::rescale_iterates() {
+  single_gpu("rescale_iterates");
+  CUDA_TRY(cudaSetDevice(device_));
+  have_solution_ = false;
+  rescale_iterates_kernel<T><<<vgrid((long long)n_ + m_), kBlock, 0, stream_>>>(
+      n_, m_, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, xs_.p, s_.p, mu_.p);
+  check_launch("rescale_iterates");
+  sync();
 }
 
 }  // namespace cosmo
@@ -3255,6 +3418,15 @@ int cosmo_b200_update_matrices_original(cosmo_b200_handle* h, const void* Px, in
                                         const void* q, const void* b) {
   ABI_GUARD(h, h->impl->update_matrices_original(Px, nnzP, Ax, nnzA_orig, q, b));
 }
+int cosmo_b200_set_caller_stream(cosmo_b200_handle* h, void* stream) { ABI_GUARD(h, h->impl->set_caller_stream(stream)); }
+int cosmo_b200_update_qb_original(cosmo_b200_handle* h, const double* q, const double* b) {
+  ABI_GUARD(h, h->impl->update_qb_original(q, b));
+}
+int cosmo_b200_original_qb(cosmo_b200_handle* h, double* q, double* b) { ABI_GUARD(h, h->impl->original_qb(q, b)); }
+int cosmo_b200_solution(cosmo_b200_handle* h, int32_t complete_dual, double* x, double* y, double* s) {
+  ABI_GUARD(h, h->impl->solution(complete_dual, x, y, s));
+}
+int cosmo_b200_rescale_iterates(cosmo_b200_handle* h) { ABI_GUARD(h, h->impl->rescale_iterates()); }
 int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
   ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));
 }

@@ -61,7 +61,7 @@ struct DevBuf {
     n = 0;
   }
   void upload(const U* host, size_t count, cudaStream_t st) {
-    if (count) CUDA_TRY(cudaMemcpyAsync(p, host, count * sizeof(U), cudaMemcpyHostToDevice, st));
+    if (count) CUDA_TRY(cudaMemcpyAsync(p, host, count * sizeof(U), cudaMemcpyDefault, st));
   }
   void upload(const std::vector<U>& h, cudaStream_t st) {
     if (n < h.size()) alloc(h.size(), false);

@@ -706,4 +706,41 @@ __global__ void __launch_bounds__(kBlock) admm_tail_kernel(int m, const T* __res
   }
 }
 
+// update!(q=, b=) from the model's own fp64 values, as the host scales them: q_out = T((D q') c) with q' = [q; 0] (q has
+// n_src <= n entries) and, unless b is null, b_out = T(E b); D, E null: identity.  One rounding to T per entry.
+template <typename T>
+__global__ void __launch_bounds__(kBlock) scale_original_qb_kernel(long long n, long long n_src, const double* __restrict__ q,
+                                                                   const T* __restrict__ D, double c, T* __restrict__ q_out,
+                                                                   long long m, const double* __restrict__ b,
+                                                                   const T* __restrict__ E, T* __restrict__ b_out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n + m; i += (long long)gridDim.x * blockDim.x) {
+    if (i < n) {
+      const double v = i < n_src ? q[i] : 0.0;
+      q_out[i] = T(((D ? (double)D[i] : 1.0) * v) * c);
+    } else {
+      const long long r = i - n;
+      b_out[r] = T((E ? (double)E[r] : 1.0) * b[r]);
+    }
+  }
+}
+
+// reverse_scaling! then scale_variables! of the resident iterates, in fp64 (scaling.jl:118-123,170-179):
+// x = (D x) / D, s = E (s / E), mu = (((E mu) / c) / E) c; D, E null: identity
+template <typename T>
+__global__ void __launch_bounds__(kBlock) rescale_iterates_kernel(long long n, long long m, const T* __restrict__ D,
+                                                                  const T* __restrict__ E, double c, T* __restrict__ x,
+                                                                  T* __restrict__ s, T* __restrict__ mu) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n + m; i += (long long)gridDim.x * blockDim.x) {
+    if (i < n) {
+      const double d = D ? (double)D[i] : 1.0;
+      x[i] = T((d * (double)x[i]) / d);
+    } else {
+      const long long r = i - n;
+      const double e = E ? (double)E[r] : 1.0;
+      s[r] = T(e * ((double)s[r] / e));
+      mu[r] = T((((e * (double)mu[r]) / c) / e) * c);
+    }
+  }
+}
+
 }  // namespace cosmo

@@ -154,6 +154,11 @@ def _signatures():
         "cosmo_b200_psd_complete": (rc, [i64, P(CompletionStruct), vp, P(i64)]),
         "cosmo_b200_set_forward_map": (rc, [vp, P(ForwardMapStruct)]),
         "cosmo_b200_update_matrices_original": (rc, [vp, vp, i64, vp, i64, vp, vp]),
+        "cosmo_b200_set_caller_stream": (rc, [vp, vp]),
+        "cosmo_b200_update_qb_original": (rc, [vp, vp, vp]),
+        "cosmo_b200_original_qb": (rc, [vp, vp, vp]),
+        "cosmo_b200_solution": (rc, [vp, i32, vp, vp, vp]),
+        "cosmo_b200_rescale_iterates": (rc, [vp]),
         "cosmo_b200_comm_unique_id": (rc, [vp]),
         "cosmo_b200_comm_init": (rc, [vp, i32, i32, vp]),
         "cosmo_b200_comm_p2p_export": (rc, [vp, vp]),
@@ -287,8 +292,95 @@ def default_settings() -> SettingsStruct:
     return s
 
 
-def _ptr(a: Optional[np.ndarray]):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
+def _ptr(a):
+    """The pointer argument of a NumPy array (None stays None; a device pointer from cuda_array passes as it is)."""
+    if a is None or isinstance(a, C.c_void_p):
+        return a
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def is_cuda_array(a) -> bool:
+    return hasattr(a, "__cuda_array_interface__")
+
+
+def cuda_array(a, dtype, size=None, output=False):
+    """(device pointer, stream) of an object with ``__cuda_array_interface__`` (torch, CuPy), after the checks the C
+    calls rely on: the typestr of `dtype`, one dimension of length `size` (any length when None), C-contiguous and, for
+    an output, not read-only.  `stream` is the interface's stream field (None: no ordering is needed)."""
+    cai = a.__cuda_array_interface__
+    want = np.dtype(dtype).newbyteorder("<").str
+    if cai.get("typestr") != want:
+        raise EngineError(ERR_INVALID, "CUDA array of typestr %r where %r is needed" % (cai.get("typestr"), want))
+    shape = tuple(cai.get("shape", ()))
+    if len(shape) != 1 or (size is not None and shape[0] != size):
+        raise EngineError(ERR_INVALID, "CUDA array of shape %s where (%s,) is needed" % (shape, "n" if size is None else size))
+    strides = cai.get("strides")
+    if strides is not None and shape[0] > 1 and tuple(strides) != (np.dtype(dtype).itemsize,):
+        raise EngineError(ERR_INVALID, "CUDA array is not C-contiguous (strides %s)" % (tuple(strides),))
+    ptr, readonly = cai["data"]
+    if output and readonly:
+        raise EngineError(ERR_INVALID, "CUDA array given as an output is read-only")
+    stream = cai.get("stream")
+    if stream == 0:
+        raise EngineError(ERR_INVALID, "__cuda_array_interface__ stream 0 is not allowed (1: legacy, 2: per-thread)")
+    return ptr, stream
+
+
+def caller_stream_handle(stream):
+    """The cudaStream_t of cosmo_b200_set_caller_stream for an interface stream field: 1 is the legacy default stream
+    (NULL), 2 the per-thread default stream (cudaStreamPerThread, the same value), any other integer the stream."""
+    return None if stream == 1 else int(stream)
+
+
+_cudart_lib = None
+
+
+def _cudart():
+    """libcudart.so.12: the system's copy, else the one of the `nvidia-cuda-runtime` wheel that PyTorch installs."""
+    global _cudart_lib
+    if _cudart_lib is None:
+        try:
+            lib = C.CDLL("libcudart.so.12")
+        except OSError:
+            import nvidia.cuda_runtime as _w
+            lib = C.CDLL(os.path.join(list(_w.__path__)[0], "lib", "libcudart.so.12"))
+        lib.cudaMemcpy.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]
+        lib.cudaStreamSynchronize.argtypes = [C.c_void_p]
+        _cudart_lib = lib
+    return _cudart_lib
+
+
+def _ordered_copy(dst, src, nbytes, stream):
+    """cudaMemcpy(cudaMemcpyDefault) between a CUDA array and host memory, ordered on both sides.  Before: the array's
+    stream (the interface's stream field) is synchronised, or, when it names none (torch), the whole device, so a write
+    on any stream of this process, the caller stream of an engine included, has landed.  After: the legacy stream the
+    copy ran on is synchronised, so the data is in place for every stream when this returns."""
+    rt = _cudart()
+    rc = rt.cudaStreamSynchronize(caller_stream_handle(stream)) if stream is not None else rt.cudaDeviceSynchronize()
+    if rc == 0 and nbytes:
+        rc = rt.cudaMemcpy(dst, src, nbytes, 4) or rt.cudaStreamSynchronize(None)   # 4: cudaMemcpyDefault
+    if rc != 0:
+        raise EngineError(ERR_CUDA, "copy between a CUDA array and host memory failed (cudaError %d)" % rc)
+
+
+def copy_into(dst, src: np.ndarray):
+    """Write the host array `src` into `dst`: a CUDA array (checked by cuda_array) or a NumPy array of src's dtype."""
+    if not is_cuda_array(dst):
+        dst[...] = src
+        return
+    src = np.ascontiguousarray(src)
+    ptr, stream = cuda_array(dst, src.dtype, src.size, output=True)
+    _ordered_copy(ptr, src.ctypes.data, src.nbytes, stream)
+
+
+def to_host(a, dtype=np.float64) -> np.ndarray:
+    """A NumPy copy of a 1-D CUDA array of `dtype`, or np.asarray of anything else."""
+    if not is_cuda_array(a):
+        return np.asarray(a, dtype=dtype)
+    ptr, stream = cuda_array(a, dtype)
+    out = np.empty(a.__cuda_array_interface__["shape"][0], dtype=dtype)
+    _ordered_copy(out.ctypes.data, ptr, out.nbytes, stream)
+    return out
 
 
 def nccl_unique_id() -> bytes:
@@ -394,6 +486,32 @@ class Engine:
     def _check(self, rc):
         _check_rc(self._lib, rc, self._h)
 
+    def _arr(self, a, size=None, dtype=None, output=False):
+        """An array argument of the calls that take host or device memory.  A CUDA array passes as its device pointer
+        (checked by cuda_array; its stream, when it names one, becomes the caller stream).  A host input goes as _vec
+        makes it; a host output must be a writable C-contiguous NumPy array of the dtype and size."""
+        dtype = np.dtype(dtype or self.dtype)
+        if a is None:
+            return None
+        if is_cuda_array(a):
+            ptr, stream = cuda_array(a, dtype, size, output)
+            if stream is not None:
+                self.set_caller_stream(caller_stream_handle(stream))
+            return C.c_void_p(ptr)
+        if not output:
+            return self._vec(a, size) if dtype == self.dtype else self._vec_of(a, size, dtype)
+        if not (isinstance(a, np.ndarray) and a.dtype == dtype and a.flags.c_contiguous and a.flags.writeable
+                and a.ndim == 1 and (size is None or a.shape[0] == size)):
+            raise EngineError(ERR_INVALID, "an output must be a writable C-contiguous 1-D %s array of length %s" % (dtype, size))
+        return a
+
+    @staticmethod
+    def _vec_of(a, size, dtype):
+        a = np.ascontiguousarray(a, dtype=dtype)
+        if size is not None and a.shape != (size,):
+            raise EngineError(ERR_INVALID, "vector has wrong length")
+        return a
+
     def _vec(self, a, size=None):
         """`a` as a flat contiguous array of the engine's dtype (None stays None), of length `size` if one is given."""
         if a is None:
@@ -409,12 +527,47 @@ class Engine:
         self._check(self._lib.cosmo_b200_update_settings(self._h, C.byref(settings)))
 
     def warm_start(self, x=None, s=None, mu=None):
-        x, s, mu = self._vec(x, self.n), self._vec(s, self.m), self._vec(mu, self.m)
+        x, s, mu = self._arr(x, self.n), self._arr(s, self.m), self._arr(mu, self.m)
         self._check(self._lib.cosmo_b200_warm_start(self._h, _ptr(x), _ptr(s), _ptr(mu)))
 
     def update_qb(self, q=None, b=None):
-        q, b = self._vec(q, self.n), self._vec(b, self.m)
+        q, b = self._arr(q, self.n), self._arr(b, self.m)
         self._check(self._lib.cosmo_b200_update_qb(self._h, _ptr(q), _ptr(b)))
+
+    # ---- caller arrays in device memory ------------------------------------------
+    def set_caller_stream(self, stream=None):
+        """cosmo_b200_set_caller_stream: the cudaStream_t (an integer; None: the legacy default stream) that caller device
+        memory is ordered on, e.g. ``torch.cuda.current_stream().cuda_stream``."""
+        self._check(self._lib.cosmo_b200_set_caller_stream(self._h, None if stream is None else C.c_void_p(stream)))
+
+    def _orig_sizes(self):
+        return self._fwd_sizes or (self.n, self.m)
+
+    def update_qb_original(self, q=None, b=None):
+        """cosmo_b200_update_qb_original: update!(q=, b=) with the model's unscaled fp64 values (host or CUDA arrays;
+        None: unchanged), mapped through the forward map when one is set and scaled on the device."""
+        n0, m0 = self._orig_sizes()
+        q, b = self._arr(q, n0, np.float64), self._arr(b, m0, np.float64)
+        self._check(self._lib.cosmo_b200_update_qb_original(self._h, _ptr(q), _ptr(b)))
+
+    def original_qb(self, q=None, b=None):
+        """cosmo_b200_original_qb into the given fp64 outputs (host or CUDA arrays; None: skipped); returns (q, b)."""
+        n0, m0 = self._orig_sizes()
+        pq, pb = self._arr(q, n0, np.float64, output=True), self._arr(b, m0, np.float64, output=True)
+        self._check(self._lib.cosmo_b200_original_qb(self._h, _ptr(pq), _ptr(pb)))
+        return q, b
+
+    def solution(self, complete_dual=False, x=None, y=None, s=None):
+        """cosmo_b200_solution: the last solve's unscaled solution (x, y = -mu, s) in fp64 in the original coordinates,
+        into the given outputs (host or CUDA arrays; None: skipped).  Returns (x, y, s)."""
+        n0, m0 = (self.n_orig, self.m_orig) if self.n_orig or self.m_orig else (self.n, self.m)
+        px, py, ps = (self._arr(a, k, np.float64, output=True) for a, k in ((x, n0), (y, m0), (s, m0)))
+        self._check(self._lib.cosmo_b200_solution(self._h, int(bool(complete_dual)), _ptr(px), _ptr(py), _ptr(ps)))
+        return x, y, s
+
+    def rescale_iterates(self):
+        """cosmo_b200_rescale_iterates: the host's unscale / rescale round trip between two solves, on the device."""
+        self._check(self._lib.cosmo_b200_rescale_iterates(self._h))
 
     def update_matrices(self, Px=None, Ax=None, q=None, b=None):
         """cosmo_b200_update_matrices: new values of P and A on the pattern of create -- ``Px`` / ``Ax`` are the ``data``
@@ -447,15 +600,15 @@ class Engine:
         self._check(self._lib.cosmo_b200_comm_p2p_attach(self._h, C.cast(buf, C.c_void_p), nranks))
 
     # ---- the hot loop ----------------------------------------------------------
-    def solve(self, out_x=None, out_s=None, out_mu=None) -> SolveOutput:
-        """cosmo_b200_solve.  Output buffers may be caller-provided (e.g. pinned)."""
+    def solve(self, out_x=None, out_s=None, out_mu=None, copy_out=True) -> SolveOutput:
+        """cosmo_b200_solve.  Output buffers may be caller-provided (e.g. pinned, or CUDA arrays); copy_out=False leaves
+        the iterates on the device only (x, s, mu None)."""
         T = self.dtype
-        x = out_x if out_x is not None else np.empty(self.n, dtype=T)
-        s = out_s if out_s is not None else np.empty(self.m, dtype=T)
-        mu = out_mu if out_mu is not None else np.empty(self.m, dtype=T)
+        x, s, mu = ((o if o is not None or not copy_out else np.empty(k, dtype=T))
+                    for o, k in ((out_x, self.n), (out_s, self.m), (out_mu, self.m)))
         rho_updates = np.zeros(256, dtype=np.float64)
         r = ResultStruct()
-        r.x, r.s, r.mu = _ptr(x), _ptr(s), _ptr(mu)
+        r.x, r.s, r.mu = (_ptr(self._arr(a, k, output=True)) for a, k in ((x, self.n), (s, self.m), (mu, self.m)))
         r.rho_updates = _ptr(rho_updates)
         r.rho_updates_cap = rho_updates.shape[0]
         self._check(self._lib.cosmo_b200_solve(self._h, C.byref(r)))
@@ -585,11 +738,13 @@ class Engine:
 
     def reverse_decomposition(self, complete_dual=False, x=True, s=True, mu=True):
         """cosmo_b200_reverse_decomposition: the unscaled (x, s, mu) of the original problem in fp64 from the iterates of
-        the last solve (a False argument skips that output: None in its place), and the stats keyed by REVERSE_STATS."""
-        out = [np.empty(n, dtype=np.float64) if want else None
+        the last solve (a False argument skips that output: None in its place; an fp64 array, host or CUDA, is written
+        into), and the stats keyed by REVERSE_STATS."""
+        out = [(np.empty(n, dtype=np.float64) if want else None) if isinstance(want, bool) else want
                for want, n in ((x, self.n_orig), (s, self.m_orig), (mu, self.m_orig))]
-        stats = self._read_out(self._lib.cosmo_b200_reverse_decomposition, int(bool(complete_dual)),
-                               *[_ptr(a) for a in out], ctype=C.c_int64, keys=REVERSE_STATS)
+        ptrs = [_ptr(self._arr(a, n, np.float64, output=True)) for a, n in zip(out, (self.n_orig, self.m_orig, self.m_orig))]
+        stats = self._read_out(self._lib.cosmo_b200_reverse_decomposition, int(bool(complete_dual)), *ptrs,
+                               ctype=C.c_int64, keys=REVERSE_STATS)
         return out[0], out[1], out[2], stats
 
     # ---- values of the original problem onto the decomposed one ---------------
@@ -615,10 +770,11 @@ class Engine:
         self._update_values(self._lib.cosmo_b200_update_matrices_original, sizes, Px, Ax, q, b)
 
     def _update_values(self, fn, qb_sizes, Px, Ax, q, b):
-        Px, Ax = self._vec(Px), self._vec(Ax)
-        q, b = self._vec(q, qb_sizes[0]), self._vec(b, qb_sizes[1])
-        self._check(fn(self._h, _ptr(Px), 0 if Px is None else Px.size, _ptr(Ax), 0 if Ax is None else Ax.size,
-                       _ptr(q), _ptr(b)))
+        nnz = [0 if a is None else a.__cuda_array_interface__["shape"][0] if is_cuda_array(a) else None for a in (Px, Ax)]
+        Px, Ax = self._arr(Px), self._arr(Ax)
+        q, b = self._arr(q, qb_sizes[0]), self._arr(b, qb_sizes[1])
+        nnz = [a.size if k is None else k for a, k in zip((Px, Ax), nnz)]
+        self._check(fn(self._h, _ptr(Px), nnz[0], _ptr(Ax), nnz[1], _ptr(q), _ptr(b)))
 
 
 def psd_complete(Y, schedule):

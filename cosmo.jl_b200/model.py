@@ -513,6 +513,55 @@ class Model:
         self._dec = None          # chordal DecompositionInfo of the problem the engine holds (settings.decompose)
         self._x2 = None           # iterates of the decomposed problem (None: restart from self.x)
         self._fwd = None          # chordal.ForwardArrays the engine holds: original values -> decomposed problem
+        self._q0 = self._b0 = None
+        self._qb_on_device = [False, False]   # q0 / b0 came as CUDA arrays: the engine holds them (original_qb)
+        self._solution_on_device = False      # optimize(solution="device"): x, s, mu live only in the engine
+
+    # q0 and b0 after update(q=, b=) with CUDA arrays are read back from the engine only when something reads them
+    @property
+    def q0(self):
+        if self._qb_on_device[0]:
+            self._fetch_qb()
+        return self._q0
+
+    @q0.setter
+    def q0(self, v):
+        self._q0, self._qb_on_device[0] = v, False
+
+    @property
+    def b0(self):
+        if self._qb_on_device[1]:
+            self._fetch_qb()
+        return self._b0
+
+    @b0.setter
+    def b0(self, v):
+        self._b0, self._qb_on_device[1] = v, False
+
+    def _fetch_qb(self):
+        if not any(self._qb_on_device):
+            return
+        want = [np.empty(k) if dev else None for dev, k in zip(self._qb_on_device, (self.n, self.m))]
+        q, b = self.engine.original_qb(*want)
+        if q is not None:
+            self.q0 = q
+        if b is not None:
+            self.b0 = b
+
+    def _fetch_solution(self):
+        """x, s, mu of a solve that left them on the device, to the host (before the engine loses them)."""
+        if not self._solution_on_device:
+            return
+        self._solution_on_device = False
+        x, y, s = self._device_solution(np.empty(self.n), np.empty(self.m), np.empty(self.m))
+        self.x, self.s, self.mu = x, s, -y
+        self._x2 = None   # the clique iterates stay in the engine: a decomposed model restarts from x
+
+    def _device_solution(self, x, y, s):
+        if self._dec is not None and not self.engine.n_orig:   # reverse on the device, with or without reverse_on_device
+            from . import chordal as _chordal
+            self.engine.set_decomposition(_chordal.decomposition_arrays(self._dec, len(self.D), len(self.E)))
+        return self.engine.solution(self.settings.complete_dual, x, y, s)
 
     # assemble!(model, P, q, constraints; settings, x0, y0), interface.jl:30-77
     def assemble(self, P, q, constraints: Union[Constraint, Sequence[Constraint]], settings: Optional[Settings] = None,
@@ -566,6 +615,7 @@ class Model:
         self._dec = None
         self._x2 = None
         self._fwd = None
+        self._solution_on_device = False
         if self.engine is not None:
             self.engine.close()
             self.engine = None
@@ -575,11 +625,13 @@ class Model:
         x0 = np.asarray(x0, dtype=np.float64)
         if x0.shape != (self.n,):
             raise ValueError("Dimension of warm starting vector doesn't match the length of index range ind.")
+        self._fetch_solution()
         self.x[:] = x0
         self.s[:] = self.b0 - self.A0 @ self.x   # s0 = b - A x0 (interface.jl:131-147)
         self._x2 = None                           # a decomposed model restarts from this point (see _setup)
 
     def warm_start_slack(self, s0):
+        self._fetch_solution()
         self.s[:] = s0
         self._x2 = None
 
@@ -587,16 +639,37 @@ class Model:
         y0 = np.asarray(y0, dtype=np.float64)
         if y0.shape != (self.m,):
             raise ValueError("Dimension of warm starting vector doesn't match the length of index range ind.")
+        self._fetch_solution()
         self.mu[:] = -y0
         self._x2 = None
 
     # update!(model; q, b), interface.jl:187-211, extended by new values of P and A on the pattern given to set!.  The
     # new values go to the live engine, and the iterates of the model stay as the next warm start.  The reference
     # refuses to update a chordally decomposed model (interface.jl:192,204); here the values are mapped onto the
-    # decomposed problem, and rho and the clique iterates stay, as update! keeps them.
+    # decomposed problem, and rho and the clique iterates stay, as update! keeps them.  q and b may be CUDA arrays
+    # (__cuda_array_interface__, fp64): with a live engine and no new P or A they go to the engine without a host copy
+    # (update_qb_original), else they are copied to the host first.
     def update(self, q=None, b=None, *, P=None, A=None):
         if not self.is_assembled:
             raise RuntimeError("Model has to be assembled once before one can start updating q or b.")
+        if _eng.is_cuda_array(q) or _eng.is_cuda_array(b):
+            for v, k, name in ((q, self.n, "q"), (b, self.m, "b")):
+                if _eng.is_cuda_array(v) and tuple(v.__cuda_array_interface__["shape"]) != (k,):
+                    raise ValueError("The dimension of %s, does not agree with the model dimension, %s." % (name, "nm"[name == "b"]))
+            if P is None and A is None and self.engine is not None and (self._dec is None or self._fwd is not None):
+                try:
+                    self.engine.update_qb_original(q, b)
+                except _eng.EngineError as e:
+                    if e.code != _eng.ERR_INVALID or self._dec is None or b is None:
+                        raise
+                    # b is nonzero on a row no clique holds: the host route below drops the engine
+                    pass
+                else:
+                    for k, v in enumerate((q, b)):
+                        if v is not None:
+                            self._qb_on_device[k] = True
+                    return
+            q, b = (None if v is None else _eng.to_host(v) for v in (q, b))
         new = {}
         for name, M, old in (("P", P, self.P0), ("A", A, self.A0)):
             if M is None:
@@ -615,6 +688,8 @@ class Model:
             if b.shape != (self.m,):
                 raise ValueError("The dimension of b, does not agree with the model dimension, m.")
         self.P0, self.A0 = new.get("P", self.P0), new.get("A", self.A0)
+        if new:
+            self._fetch_solution()   # new matrices reset the engine's iterates; the next solve warm-starts from the host
         if q is not None:
             self.q0 = q.copy()
         if b is not None:
@@ -654,6 +729,8 @@ class Model:
             from . import chordal as _chordal
             if not len(_chordal.uncovered_rows(self._fwd, b)):
                 return True
+        self._fetch_qb()          # what lives only in the engine goes to the host before it is closed
+        self._fetch_solution()
         self._x2 = None
         self._fwd = None
         self.engine.close()
@@ -700,7 +777,11 @@ class Model:
             self.engine.update_settings(st.to_struct())
         configure_accelerator(self.engine, st)
         # scale_variables! (scaling.jl:118-123)
-        if self._dec is not None:
+        if self._solution_on_device:
+            # the last solution never left the device: the same unscale / rescale round trip, in place
+            self._solution_on_device = False
+            self.engine.rescale_iterates()
+        elif self._dec is not None:
             # The decomposed problem keeps its own iterates between solves.  A warm start given in the ORIGINAL
             # coordinates enters through x only (the clique copies of s and mu start from zero): the reference
             # re-allocates all variables after the decomposition (pre_allocate_variables!, chordal_decomposition.jl:29),
@@ -714,17 +795,28 @@ class Model:
             self.engine.warm_start(self.x / self.D, self.E * self.s, (self.mu / self.E) * self.c)
         return time.perf_counter() - t0
 
-    # optimize!(model), solver.jl:78-203
-    def optimize(self) -> Result:
+    # optimize!(model), solver.jl:78-203.  solution="device" leaves the solution on the device: Result.x, .y, .s are
+    # None, solution_into() writes it into caller arrays, and the next optimize starts from it without a host round trip.
+    def optimize(self, solution: str = "host") -> Result:
         if not self.is_assembled:
             raise RuntimeError("The model has to be assembled! / set! before optimize!() can be called.")
+        if solution not in ("host", "device"):
+            raise ValueError("solution must be \"host\" or \"device\"")
         t0 = time.perf_counter()
         setup_time = self._setup()
         if self.settings.time_limit != 0 or (self.settings.adaptive_rho and self.settings.adaptive_rho_interval == 0):
             st = self.settings.to_struct()           # both rules count setup! (solver.jl:119,244-256,349)
             st.setup_time = setup_time
             self.engine.update_settings(st)
-        out = self.engine.solve()
+        out = self.engine.solve() if solution == "host" else self.engine.solve(copy_out=False)
+        times = dict(out.times)
+        times["setup_time"] = setup_time
+        info = ResultInfo(out.r_prim, out.r_dual, out.max_norm_prim, out.max_norm_dual, list(out.rho_updates))
+        if solution == "device":
+            self._solution_on_device = True
+            times["solver_time"] = time.perf_counter() - t0
+            return Result(None, None, None, out.obj_val, out.iter, out.safeguarding_iter, out.status, info, times,
+                          kkt_inner_iterations=out.kkt_inner_iterations, kernel_launches=out.kernel_launches)
         # reverse_scaling! (scaling.jl:170-179)
         x = self.D * out.x.astype(np.float64)
         s = out.s.astype(np.float64) / self.E
@@ -737,12 +829,20 @@ class Model:
             else:
                 x, s, mu = _chordal.reverse(self._dec, x, s, mu, complete_dual=self.settings.complete_dual)
         self.x, self.s, self.mu = x.copy(), s.copy(), mu.copy()
-        times = dict(out.times)
-        times["setup_time"] = setup_time
         times["solver_time"] = time.perf_counter() - t0
-        info = ResultInfo(out.r_prim, out.r_dual, out.max_norm_prim, out.max_norm_dual, list(out.rho_updates))
         return Result(x, -mu, s, out.obj_val, out.iter, out.safeguarding_iter, out.status, info, times,
                       kkt_inner_iterations=out.kkt_inner_iterations, kernel_launches=out.kernel_launches)
+
+    def solution_into(self, x=None, y=None, s=None):
+        """The last solution (x, y, s of Result, completed as settings.complete_dual asks) into caller fp64 arrays, CUDA
+        (__cuda_array_interface__) or NumPy; None skips one.  After optimize(solution="device") it is reversed on the
+        device straight into them (a decomposed model without reverse_on_device gets the device map for it)."""
+        if self._solution_on_device:
+            self._device_solution(x, y, s)
+            return
+        for dst, src in ((x, self.x), (y, -self.mu), (s, self.s)):
+            if dst is not None:
+                _eng.copy_into(dst, src)
 
     def empty_model(self):  # empty_model!, interface.jl:84-100
         if self.engine is not None:

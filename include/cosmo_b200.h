@@ -15,9 +15,11 @@
  *       AbstractConvexSet  project!(x, set)          (src/convexset.jl:885-891)
  *
  * Conventions
- *   - plain pointers and sizes only; every array argument is a HOST pointer
- *     owned by the caller (Julia GC memory under GC.@preserve). The engine
- *     copies inputs to HBM inside the call and never keeps a host pointer.
+ *   - plain pointers and sizes only; array arguments are owned by the caller
+ *     (Julia GC memory under GC.@preserve, or a CuArray). The engine copies
+ *     inputs to HBM inside the call and never keeps a caller pointer.  Array
+ *     arguments are HOST pointers, except where "host or device" is said
+ *     (see "Caller arrays in device memory" below).
  *   - matrices arrive exactly as Julia stores them: SparseMatrixCSC{T,Int64},
  *     1-based colptr/rowval (`index_base = 1`); `index_base = 0` accepts
  *     SciPy-style 0-based int64 arrays.
@@ -499,6 +501,40 @@ int cosmo_b200_set_forward_map(cosmo_b200_handle* h, const cosmo_b200_forward_ma
    the device before the first write): COSMO_B200_ERR_INVALID, and nothing has changed. */
 int cosmo_b200_update_matrices_original(cosmo_b200_handle* h, const void* Px, int64_t nnzP, const void* Ax,
                                         int64_t nnzA_orig, const void* q, const void* b);
+
+/* ---- caller arrays in device memory --------------------------------------- */
+/* Host or device: every array of cosmo_b200_warm_start, _update_qb, _update_matrices and _update_matrices_original, the
+   x, s, mu buffers of cosmo_b200_result, the outputs of cosmo_b200_reverse_decomposition and the arrays of the entry
+   points below may point to host memory, to device memory on the handle's device or to managed memory (copies use
+   cudaMemcpyDefault, so a host pointer takes the path it always took).  A pointer in device memory of another device:
+   COSMO_B200_ERR_INVALID, and nothing is written.  "Caller device memory" means device or managed memory: when a call
+   reads it, the engine stream first waits on an event recorded on the caller stream; when a call writes it, the caller
+   stream waits on the engine stream before the call returns (the call is synchronous as before; no cudaDeviceSynchronize).  The entry points below refuse a sharded handle
+   (nranks > 1) with COSMO_B200_ERR_UNSUPPORTED. */
+/* The stream that caller device memory is ordered on (NULL: the legacy default stream, which is also the initial one;
+   cudaStreamPerThread is accepted).  Kept until the next call. */
+int cosmo_b200_set_caller_stream(cosmo_b200_handle* h, void* stream);
+/* update!(model, q=, b=) in the model's own coordinates, unscaled, in fp64 (NULL = unchanged): with a forward map
+   (cosmo_b200_set_forward_map) q has n_orig and b m_orig entries and become q' = [q; 0], b' = b[b_src] as there; without
+   one they have n and m.  The device then forms (D q') c and E b' in fp64, rounded once to the element type, and changes
+   the state as cosmo_b200_update_qb does (rho classes recomputed from a new b; iterates and rho kept).  A b that is
+   nonzero on an uncovered row of the forward map: COSMO_B200_ERR_INVALID, and nothing has changed.  The handle keeps the
+   fp64 q and b it was given on the device (8 (n_orig + m_orig) bytes, allocated on first use) for
+   cosmo_b200_original_qb. */
+int cosmo_b200_update_qb_original(cosmo_b200_handle* h, const double* q, const double* b);
+/* Reads back the q and b last given to cosmo_b200_update_qb_original (NULL skips one); one that was never given, or was
+   given before the forward map changed its sizes: COSMO_B200_ERR_INVALID. */
+int cosmo_b200_original_qb(cosmo_b200_handle* h, double* q, double* b);
+/* The last solve's solution in the original, unscaled coordinates, in fp64: x (n_orig), y = -mu and s (m_orig); any
+   pointer may be NULL.  With a decomposition map this is cosmo_b200_reverse_decomposition's arithmetic (the completion
+   when complete_dual != 0); without one it is reverse_scaling!: x = D x', s = s' / E, mu = (E mu') / c after widening,
+   with n_orig = n and m_orig = m.  No solve since create / reset / warm_start / rescale_iterates: COSMO_B200_ERR_INVALID. */
+int cosmo_b200_solution(cosmo_b200_handle* h, int32_t complete_dual, double* x, double* y, double* s);
+/* reverse_scaling! followed by scale_variables! on the resident iterates, in fp64 and then rounded to the element type:
+   x' <- (D x') / D, s' <- E (s' / E), mu' <- (((E mu') / c) / E) c: the round trip the host applies between two solves
+   when it hands the unscaled solution back as the next warm start.  Like cosmo_b200_warm_start, it ends the solution
+   that cosmo_b200_solution and cosmo_b200_reverse_decomposition read. */
+int cosmo_b200_rescale_iterates(cosmo_b200_handle* h);
 
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
