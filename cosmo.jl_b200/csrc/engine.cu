@@ -39,6 +39,7 @@
 #include "chordal_fwd.cuh"
 #include "mat_update.cuh"
 #include "custom_cone.cuh"
+#include "polish.cuh"
 
 namespace cosmo {
 
@@ -194,6 +195,7 @@ class EngineBase {
   virtual void original_qb(double* q, double* b) = 0;
   virtual void solution(int complete_dual, double* x, double* y, double* s) = 0;
   virtual void rescale_iterates() = 0;
+  virtual void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) = 0;
 };
 
 template <typename T>
@@ -252,6 +254,7 @@ class Engine : public EngineBase {
   void original_qb(double* q, double* b) override;
   void solution(int complete_dual, double* x, double* y, double* s) override;
   void rescale_iterates() override;
+  void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) override;
 
  private:
   // ---- problem ----
@@ -319,6 +322,14 @@ class Engine : public EngineBase {
   double rho_ = 0.1;
   std::vector<double> rho_updates_;
   bool have_solution_ = false;   // xs_, s_, mu_ hold what the last solve() returned (cleared by reset / warm_start)
+  int last_status_ = COSMO_B200_UNDETERMINED;   // status of the last solve()
+  bool conic_rows_ = false;      // a set other than ZeroSet, Nonnegatives and Box has rows (polishing does not apply)
+  // solution polishing (polish.cuh): scratch allocated by the first polish and kept
+  DevBuf<T> pol_zx_, pol_znu_, pol_rhs_, pol_px_, pol_w_, pol_s_, pol_mu_, pol_rho_;
+  DevBuf<unsigned char> pol_kind_;
+  DevBuf<int> pol_cnt_;
+  void polish_residual(double* max2);
+  void emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y, double* s);
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
   rev::Reverse ident_;           // the identity map: cosmo_b200_solution of a handle without a decomposition map
@@ -424,13 +435,13 @@ class Engine : public EngineBase {
   RedBuf<T> red_ptr(T* out) { return RedBuf<T>{partials_.p, out, ticket_.p}; }
   // K5 + K7 pass over w: the projection (do_proj) and / or the right-hand side of admm_x! from ws_rhs (do_rhs).
   // 128-bit kernel for fp64 when every (n+m)-vector's m-part is 16-byte aligned (n even; ws_rhs too)
-  void launch_proj_rhs(const T* w, const T* ws_rhs, bool do_proj, bool do_rhs) {
+  void launch_proj_rhs(const T* w, const T* ws_rhs, bool do_proj, bool do_rhs, T* s_out = nullptr) {
     ProjRhsArgs<T> a;
     a.n = n_; a.m = m_; a.w = w; a.ws_rhs = ws_rhs;
     a.q = q_.p; a.b = b_.p; a.rho = rho_vec_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
     a.row_class = row_class_.p; a.row_cone = row_cone_.p;
     a.soc = SocTable<T>{soc_off_.p, soc_norm_.p};
-    a.s = s_.p; a.ls = ls_.p; a.t0 = t0_.p; a.sigma = (T)st_.sigma;
+    a.s = s_out ? s_out : s_.p; a.ls = ls_.p; a.t0 = t0_.p; a.sigma = (T)st_.sigma;
     a.do_proj = do_proj ? 1 : 0; a.do_rhs = do_rhs ? 1 : 0;
     if constexpr (std::is_same<T, double>::value) {
       if ((a.n & 1) == 0 && ((reinterpret_cast<uintptr_t>(a.ws_rhs) & 15) == 0) && ((reinterpret_cast<uintptr_t>(a.w) & 15) == 0)) {
@@ -950,6 +961,7 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
     off += sdesc.dim;
   }
   if (off != m_) throw EngineError{COSMO_B200_ERR_INVALID, "sum of set dimensions != m"};
+  conic_rows_ = !rect_off.empty();
 
   // ---- matrices -----------------------------------------------------------
   const bool dbg = getenv("COSMO_B200_SETUP_DEBUG") != nullptr;
@@ -2478,6 +2490,7 @@ void Engine<T>::solve(cosmo_b200_result* out) {
   // x = view(w_prev, 1:n): keep it for the next warm start and hand it out
   CUDA_TRY(cudaMemcpyAsync(xs_.p, W_[prev_].p, n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
   have_solution_ = true;
+  last_status_ = status;
   if (out) {
     if (out->x) download_vec(out->x, W_[prev_].p, n);
     if (out->s) download_vec(out->s, s_.p, m);
@@ -3148,6 +3161,14 @@ void Engine<T>::solution(int complete_dual, double* x, double* y, double* s) {
   single_gpu("solution");
   if (!have_solution_)
     throw EngineError{COSMO_B200_ERR_INVALID, "solution: no solve since the engine was created, reset or warm-started"};
+  emit_solution(xs_.p, s_.p, mu_.p, complete_dual, x, y, s);
+}
+
+// (xsrc, ssrc, musrc) in the resident coordinates into the caller's fp64 x, y = -mu, s: through the decomposition map
+// when one is set, else through the identity map
+template <typename T>
+void Engine<T>::emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y,
+                              double* s) {
   const unsigned dev = caller_arrays({x, y, s});
   rev::Reverse* r = &rev_;
   if (!rev_.has_map()) {
@@ -3160,7 +3181,7 @@ void Engine<T>::solution(int complete_dual, double* x, double* y, double* s) {
     }
     r = &ident_;
   }
-  r->run<T>(xs_.p, s_.p, mu_.p, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, complete_dual != 0,
+  r->run<T>(xsrc, ssrc, musrc, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, complete_dual != 0,
             x, s, y, nullptr, stream_, device_, true);
   if (dev) caller_written();
 }
@@ -3175,6 +3196,128 @@ void Engine<T>::rescale_iterates() {
   rescale_iterates_kernel<T><<<vgrid((long long)n_ + m_), kBlock, 0, stream_>>>(
       n_, m_, scaled_ ? D_.p : nullptr, scaled_ ? E_.p : nullptr, scaled_ ? c_ : 1.0, xs_.p, s_.p, mu_.p);
   check_launch("rescale_iterates");
+  sync();
+}
+
+// r^ - K_A z of the exact reduced system (polish.cuh) into ls_, the right-hand side of the next refinement solve:
+// P x, then the x rows over A' nu and the s rows over A x.  max2 (optional) = {|r_x|_inf, |r_s|_inf}.
+template <typename T>
+void Engine<T>::polish_residual(double* max2) {
+  const int n = n_, m = m_;
+  launch_spmv(P_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n, EpiStore<T>{nullptr, pol_px_.p}, red(SC_TMP6),
+              "spmv_polish_P");
+  launch_spmv(At_, pol_znu_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n,
+              EpiPolishResX<T>{nullptr, ls_.p, q_.p, pol_px_.p}, red(SC_TMP6), "spmv_polish_res_x");
+  launch_spmv(A_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m,
+              EpiPolishResS<T>{nullptr, ls_.p + n, pol_rhs_.p, pol_kind_.p}, red(SC_TMP7), "spmv_polish_res_s");
+  if (max2) {
+    read_scalars(SC_TMP6, 2);
+    max2[0] = (double)h_sc_[SC_TMP6];
+    max2[1] = (double)h_sc_[SC_TMP7];
+  }
+}
+
+// Solution polishing (DESIGN.md §3i): active set from the resident (x, s, mu), the regularised reduced KKT system
+// factored by the direct plugin, iterative refinement, the candidate and its acceptance.  The resident iterates, rho,
+// sigma and the solve's statistics are left as the solve left them; the factor is marked dirty.
+template <typename T>
+void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out) {
+  const cosmo_b200_polish_settings p = ps ? *ps : cosmo_b200_polish_settings{1e-6, 3, 0};
+  if (!(p.delta > 0.0) || !std::isfinite(p.delta) || p.refine_iter < 0 || p.refine_iter > 100 || p.reserved != 0)
+    throw EngineError{COSMO_B200_ERR_INVALID, "polish: delta must be finite and > 0, refine_iter in 0 .. 100, reserved 0"};
+  single_gpu("polish");
+  if (!direct_kkt())
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "polish: needs a direct KKT plugin (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver)"};
+  if (!have_solution_)
+    throw EngineError{COSMO_B200_ERR_INVALID, "polish: no solve since the engine was created, reset or warm-started"};
+  CUDA_TRY(cudaSetDevice(device_));
+  out[0] = -1.0; out[1] = out[2] = out[3] = 0.0;
+  for (int k = 4; k < 8; ++k) out[k] = NAN;
+  if (conic_rows_ || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE || last_status_ == COSMO_B200_DUAL_INFEASIBLE ||
+      last_status_ == COSMO_B200_UNSOLVED) {
+    emit_solution(xs_.p, s_.p, mu_.p, 0, x, y, s);
+    return;
+  }
+  const int n = n_, m = m_;
+  if (!pol_kind_.p) {
+    pol_zx_.alloc(std::max(n, 1)); pol_px_.alloc(std::max(n, 1)); pol_w_.alloc((size_t)n + m + 1);
+    pol_znu_.alloc(std::max(m, 1)); pol_rhs_.alloc(std::max(m, 1)); pol_s_.alloc(std::max(m, 1));
+    pol_mu_.alloc(std::max(m, 1)); pol_rho_.alloc(std::max(m, 1));
+    pol_kind_.alloc(std::max(m, 1)); pol_cnt_.alloc(POLISH_CNT_COUNT);
+  }
+  // the solve's rho vector and sigma come back whatever happens below; the factor then follows them again
+  const double sigma0 = st_.sigma;
+  CUDA_TRY(cudaMemcpyAsync(pol_rho_.p, rho_vec_.p, m * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  auto set_factor_values = [&](double sigma) {
+    st_.sigma = sigma;   // baked into the captured factor graphs
+    destroy_ldl_factor_graph();
+    sn_factor_graph_.reset();
+    ldl_dirty_ = true;
+    sn_dirty_ = true;
+  };
+  auto restore = [&] {
+    set_factor_values(sigma0);
+    CUDA_TRY(cudaMemcpyAsync(rho_vec_.p, pol_rho_.p, m * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  };
+  bool polished = false;
+  try {
+    CUDA_TRY(cudaMemsetAsync(pol_cnt_.p, 0, POLISH_CNT_COUNT * sizeof(int), stream_));
+    PolishClassifyArgs<T> a;
+    a.n = n; a.m = m; a.row_class = row_class_.p; a.box_l = box_l_.p; a.box_u = box_u_.p; a.b = b_.p; a.q = q_.p;
+    a.s = s_.p; a.mu = mu_.p; a.x = xs_.p; a.delta = (T)p.delta;
+    a.kind = pol_kind_.p; a.rhs = pol_rhs_.p; a.rho = rho_vec_.p; a.ls = ls_.p; a.counts = pol_cnt_.p;
+    polish_classify_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(a);
+    check_launch("polish_classify");
+    int cnt[POLISH_CNT_COUNT] = {0, 0, 0, 0};
+    CUDA_TRY(cudaMemcpyAsync(cnt, pol_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+    set_factor_values(p.delta);
+    bool factored = true;
+    try {
+      direct_factor();
+    } catch (const EngineError& e) {
+      if (e.code == COSMO_B200_ERR_CUDA) throw;
+      factored = false;   // zero or non-finite pivots, or the wrong inertia: not an error, the polish is rejected
+    }
+    out[0] = 0.0;
+    out[1] = cnt[POLISH_CNT_LOWER]; out[2] = cnt[POLISH_CNT_UPPER]; out[3] = cnt[POLISH_CNT_EQ];
+    if (factored) {
+      auto plugin_solve = [&] {   // [xsol_; nu_] = K~ \ ls_
+        if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_solve();
+        else sn_solve();
+      };
+      for (int k = 0; k <= p.refine_iter; ++k) {
+        if (k > 0) polish_residual(nullptr);
+        plugin_solve();
+        polish_update_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, xsol_.p, nu_.p, pol_zx_.p,
+                                                                                  pol_znu_.p, k == 0 ? 1 : 0);
+        check_launch("polish_update");
+      }
+      double rmax[2];
+      polish_residual(rmax);
+      // the candidate: x_p, s_p = Pi_K(b - A x_p), mu_p = the clipped -nu
+      launch_spmv(A_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m, EpiPolishSlack<T>{nullptr, pol_w_.p + n, b_.p},
+                  red(SC_TMP6), "spmv_polish_slack");
+      launch_proj_rhs(pol_w_.p, nullptr, true, false, pol_s_.p);
+      polish_finish_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, pol_kind_.p, pol_znu_.p, pol_mu_.p);
+      check_launch("polish_finish");
+      double cand[5], unp[5];
+      compute_residuals(pol_zx_.p, pol_s_.p, pol_mu_.p, false, cand);
+      compute_residuals(xs_.p, s_.p, mu_.p, false, unp);
+      const double u = (double)std::numeric_limits<T>::epsilon() / 2.0;
+      bool finite = std::isfinite(rmax[0]) && std::isfinite(rmax[1]);
+      for (double v : cand) finite = finite && std::isfinite(v);
+      polished = finite && cand[0] <= std::max(unp[0], 10.0 * u * (1.0 + cand[2])) &&
+                 cand[1] <= std::max(unp[1], 10.0 * u * (1.0 + cand[3]));
+      out[0] = polished ? 1.0 : 0.0;
+      out[4] = cand[0]; out[5] = cand[1]; out[6] = cand[4]; out[7] = std::max(rmax[0], rmax[1]);
+    }
+  } catch (...) {
+    try { restore(); } catch (...) {}
+    throw;
+  }
+  restore();
+  if (polished) emit_solution(pol_zx_.p, pol_s_.p, pol_mu_.p, 0, x, y, s);
+  else emit_solution(xs_.p, s_.p, mu_.p, 0, x, y, s);
   sync();
 }
 
@@ -3427,6 +3570,11 @@ int cosmo_b200_solution(cosmo_b200_handle* h, int32_t complete_dual, double* x, 
   ABI_GUARD(h, h->impl->solution(complete_dual, x, y, s));
 }
 int cosmo_b200_rescale_iterates(cosmo_b200_handle* h) { ABI_GUARD(h, h->impl->rescale_iterates()); }
+int cosmo_b200_polish(cosmo_b200_handle* h, const cosmo_b200_polish_settings* ps, double* x, double* y, double* s,
+                      double out[8]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->polish(ps, x, y, s, out));
+}
 int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
   ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));
 }

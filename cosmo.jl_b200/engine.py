@@ -115,6 +115,14 @@ class ForwardMapStruct(C.Structure):
                 ("b_uncovered", C.c_void_p)]
 
 
+class PolishSettings(C.Structure):
+    _fields_ = [("delta", C.c_double), ("refine_iter", C.c_int32), ("reserved", C.c_int32)]
+
+
+POLISH_STATUS = {1: "Polished", 0: "Unpolished", -1: "Not_applicable"}
+POLISH_STATS = ("status", "n_lower", "n_upper", "n_equality", "r_prim", "r_dual", "obj_val", "refine_residual")
+
+
 def _signatures():
     """(restype, argtypes) of every entry point of include/cosmo_b200.h, in the header's order."""
     vp, i32, i64, f64, P = C.c_void_p, C.c_int32, C.c_int64, C.c_double, C.POINTER
@@ -159,6 +167,7 @@ def _signatures():
         "cosmo_b200_original_qb": (rc, [vp, vp, vp]),
         "cosmo_b200_solution": (rc, [vp, i32, vp, vp, vp]),
         "cosmo_b200_rescale_iterates": (rc, [vp]),
+        "cosmo_b200_polish": (rc, [vp, P(PolishSettings), vp, vp, vp, P(f64)]),
         "cosmo_b200_comm_unique_id": (rc, [vp]),
         "cosmo_b200_comm_init": (rc, [vp, i32, i32, vp]),
         "cosmo_b200_comm_p2p_export": (rc, [vp, vp]),
@@ -568,6 +577,18 @@ class Engine:
     def rescale_iterates(self):
         """cosmo_b200_rescale_iterates: the host's unscale / rescale round trip between two solves, on the device."""
         self._check(self._lib.cosmo_b200_rescale_iterates(self._h))
+
+    def polish(self, delta=1e-6, refine_iter=3, x=None, y=None, s=None):
+        """cosmo_b200_polish: polish the last solve's solution through the direct LDL' plugin.  Like solution(), x, y, s
+        are fp64 outputs in the original coordinates (host or CUDA arrays; None: skipped) and receive the polished
+        solution on stats["status"] == 1, the unpolished one otherwise.  Returns (x, y, s, stats), stats keyed by
+        POLISH_STATS (status 1 polished, 0 rejected, -1 not applicable; the counts as ints)."""
+        n0, m0 = (self.n_orig, self.m_orig) if self.n_orig or self.m_orig else (self.n, self.m)
+        px, py, ps = (self._arr(a, k, np.float64, output=True) for a, k in ((x, n0), (y, m0), (s, m0)))
+        st = PolishSettings(float(delta), int(refine_iter), 0)
+        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_polish, self._h, C.byref(st), _ptr(px), _ptr(py), _ptr(ps),
+                       ctype=C.c_double, keys=POLISH_STATS, ints=POLISH_STATS[:4])
+        return x, y, s, stats
 
     def update_matrices(self, Px=None, Ax=None, q=None, b=None):
         """cosmo_b200_update_matrices: new values of P and A on the pattern of create -- ``Px`` / ``Ax`` are the ``data``

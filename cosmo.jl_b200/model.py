@@ -314,6 +314,11 @@ class Settings:
     # engine-specific: reverse the decomposition (reverse_scaling!, reverse_decomposition!, psd_completion!) on the
     # device from the iterates the solve left there, instead of chordal.reverse on the host
     reverse_on_device: bool = False
+    # engine extension: polish the solution of a QP or LP after the solve (cosmo_b200_polish, DESIGN.md §3i): an
+    # active-set KKT solve with iterative refinement through the direct plugin, kept only when its residuals are no worse
+    polish: bool = False
+    polish_delta: float = 1e-6
+    polish_refine_iter: int = 3
 
     _KKT = {"CGIndirectKKTSolver": _eng.KKT_CG, "MINRESIndirectKKTSolver": _eng.KKT_MINRES,
             "IndirectReducedKKTSolver:MINRES": _eng.KKT_MINRES_REDUCED, "DeviceLdlKKTSolver": _eng.KKT_LDL,
@@ -365,6 +370,12 @@ class Settings:
             raise _eng.EngineError(_eng.ERR_UNSUPPORTED,
                                    "accelerator %r: the engine implements EmptyAccelerator and AndersonAccelerator "
                                    "(variant in accelerator_type / _memory / _regularizer)" % self.accelerator)
+        if self.polish:
+            if self._KKT[self.kkt_solver] not in (_eng.KKT_LDL, _eng.KKT_LDL_SUPERNODAL):
+                raise _eng.EngineError(_eng.ERR_UNSUPPORTED, "polish needs a direct KKT solver (DeviceLdlKKTSolver or "
+                                                             "DeviceSupernodalKKTSolver), not %r" % self.kkt_solver)
+            if not (0.0 < self.polish_delta < float("inf")) or not 0 <= self.polish_refine_iter <= 100:
+                raise _eng.EngineError(_eng.ERR_INVALID, "polish_delta must be finite and > 0, polish_refine_iter in 0 .. 100")
         if self.accelerator == "AndersonAccelerator":
             self.accelerator_struct()
             if self.accelerator_mem <= 2:
@@ -409,6 +420,7 @@ class Result:
     times: dict
     kkt_inner_iterations: int = 0
     kernel_launches: int = 0
+    polish: str = "Not_run"     # "Not_run" | "Polished" | "Unpolished" | "Not_applicable" (Settings.polish)
 
 
 # ---------------------------------------------------------------------------
@@ -802,6 +814,8 @@ class Model:
             raise RuntimeError("The model has to be assembled! / set! before optimize!() can be called.")
         if solution not in ("host", "device"):
             raise ValueError("solution must be \"host\" or \"device\"")
+        if solution == "device" and self.settings.polish:
+            raise ValueError("polish=True needs solution=\"host\"; with the solution on the device call Engine.polish")
         t0 = time.perf_counter()
         setup_time = self._setup()
         if self.settings.time_limit != 0 or (self.settings.adaptive_rho and self.settings.adaptive_rho_interval == 0):
@@ -828,10 +842,25 @@ class Model:
                 x, s, mu, _ = self.engine.reverse_decomposition(complete_dual=self.settings.complete_dual)
             else:
                 x, s, mu = _chordal.reverse(self._dec, x, s, mu, complete_dual=self.settings.complete_dual)
+        # the model's warm-start iterates stay the ADMM ones: a re-solve after a polished solve is the same as after an
+        # unpolished one
         self.x, self.s, self.mu = x.copy(), s.copy(), mu.copy()
+        y, obj_val, polish = -mu, out.obj_val, "Not_run"
+        if self.settings.polish:
+            tp = time.perf_counter()
+            if self._dec is not None:     # the decomposed problem has PSD cones: no finite active set
+                polish = "Not_applicable"
+            else:
+                xp, yp, sp_ = np.empty(self.n), np.empty(self.m), np.empty(self.m)
+                _, _, _, pst = self.engine.polish(self.settings.polish_delta, self.settings.polish_refine_iter, xp, yp, sp_)
+                polish = _eng.POLISH_STATUS[pst["status"]]
+                if pst["status"] == 1:
+                    x, y, s, obj_val = xp, yp, sp_, pst["obj_val"]
+                    info.r_prim, info.r_dual = pst["r_prim"], pst["r_dual"]
+            times["polish_time"] = time.perf_counter() - tp
         times["solver_time"] = time.perf_counter() - t0
-        return Result(x, -mu, s, out.obj_val, out.iter, out.safeguarding_iter, out.status, info, times,
-                      kkt_inner_iterations=out.kkt_inner_iterations, kernel_launches=out.kernel_launches)
+        return Result(x, y, s, obj_val, out.iter, out.safeguarding_iter, out.status, info, times,
+                      kkt_inner_iterations=out.kkt_inner_iterations, kernel_launches=out.kernel_launches, polish=polish)
 
     def solution_into(self, x=None, y=None, s=None):
         """The last solution (x, y, s of Result, completed as settings.complete_dual asks) into caller fp64 arrays, CUDA

@@ -536,6 +536,38 @@ int cosmo_b200_solution(cosmo_b200_handle* h, int32_t complete_dual, double* x, 
    that cosmo_b200_solution and cosmo_b200_reverse_decomposition read. */
 int cosmo_b200_rescale_iterates(cosmo_b200_handle* h);
 
+/* ---- solution polishing (QPs and LPs) ------------------------------------- */
+/* An engine extension beyond the reference (like cosmo_b200_update_matrices): nothing changes unless it is called.
+   From the last solve's (x, s, mu) it guesses the active rows (ZeroSet rows and Box rows with l = u always; a
+   Nonnegatives row when s < -mu; a Box row at l when s - l < -mu, else at u when u - s < mu), solves the equality-
+   constrained KKT system of that guess through the handle's direct LDL' plugin with the diagonal sigma = delta,
+   rho = 1/delta on the active rows and rho = delta elsewhere, refines it refine_iter times against the exact reduced
+   system, and keeps the candidate (x_p, s_p = Pi_K(b - A x_p), mu_p = the multipliers clipped into the normal cone of
+   each active row) only when everything is finite and each of its residuals r_prim, r_dual (compute_residuals, unscaled
+   as the termination test unscales them) is at most max(the last solve's, 10 u (1 + the candidate's max_norm)), with u
+   the unit roundoff of the element type.  DESIGN.md §3i. */
+typedef struct {
+  double delta;        /* regularisation delta > 0, finite (1e-6) */
+  int32_t refine_iter; /* iterative-refinement steps, 0 .. 100 (3) */
+  int32_t reserved;    /* 0 */
+} cosmo_b200_polish_settings;
+/* NULL ps = defaults.  x (n_orig), y, s (m_orig) in fp64, host or device, with the arithmetic and the caller-memory rules
+   of cosmo_b200_solution (complete_dual = 0); any may be NULL.  out = {status, lower-active rows, upper-active rows,
+   equality rows, r_prim, r_dual, obj_val of the candidate, |r|_inf of the exact reduced system (scaled) after the last
+   refinement step}.  status 1: polished, the buffers get the candidate.  0: rejected (the candidate failed the rule, or
+   the regularised factorisation met a zero pivot or the wrong inertia; the values are then NaN): not an error, the
+   buffers get the unpolished solution.  -1: not applicable (a set other than ZeroSet, Nonnegatives and Box, or the last
+   solve ended Primal_infeasible, Dual_infeasible or Unsolved): the buffers get the unpolished solution, the counts are 0
+   and the values NaN.  Bad ps, out NULL, or no solve since create / reset / warm_start / rescale_iterates:
+   COSMO_B200_ERR_INVALID.  An indirect plugin (CG, MINRES) or a sharded handle: COSMO_B200_ERR_UNSUPPORTED.
+   State: the handle stays as the solve left it -- w, x, s, mu, rho, the rho vector, the rho updates, the KKT counter,
+   the accelerator history and the solution that cosmo_b200_solution reads.  sigma and the rho vector of the solve are
+   restored and the factor is marked dirty, so the next KKT solve refactors from them; only the factorisation counters
+   of cosmo_b200_ldl_stats / cosmo_b200_ldl_sn_stats move.  Scratch of about 3 n + 6 m values of the element type and
+   one byte per row is allocated by the first call and kept. */
+int cosmo_b200_polish(cosmo_b200_handle* h, const cosmo_b200_polish_settings* ps, double* x, double* y, double* s,
+                      double out[8]);
+
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
 int cosmo_b200_comm_unique_id(void* id128);
