@@ -1,0 +1,73 @@
+"""torch.autograd for polished QP and LP solves on the device (DESIGN.md §3j).
+
+``solve_qp(engine, Px, q, Ax, b)`` puts new values of P, q, A and b into a live engine (``Engine.update_matrices``),
+solves, polishes and returns the polished unscaled solution ``(x, y, s)`` as CUDA tensors; its backward pass is one
+``Engine.adjoint`` into CUDA tensors.  Nothing leaves the device.
+
+The engine is created by the caller with a direct KKT solver (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver), on the
+pattern of P and A, without host scaling (scaling 0, or ``equilibrate=True``), so that ``update_matrices`` takes the
+unscaled data.  ``Px`` and ``Ax`` are the ``data`` arrays of P and A in sorted CSC order, all four inputs CUDA tensors of
+the engine's dtype.  The Box bounds are not inputs of ``update_matrices`` and get no gradient here (``Engine.adjoint``
+returns them).  The derivative is that of the polished solution map on its active set: exact where the active set is
+stable, one-sided at weakly active rows.
+
+The backward pass reads the point and the factor the engine keeps from the last polish.  When the engine has run
+another ``solve_qp`` since this pass's forward (as ``torch.autograd.gradcheck`` does between them), the backward pass
+first solves and polishes this pass's data again; the solve is deterministic, so it differentiates the same point.
+Between a forward pass and its backward pass the engine must not be used other than through ``solve_qp``.
+"""
+import torch
+
+from .engine import EngineError
+
+
+def _solve_and_polish(engine, Px, q, Ax, b):
+    """update_matrices, solve and polish into new CUDA tensors; returns (x, y, s) and tags the engine with this call."""
+    dev = q.device
+    engine.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
+    engine.update_matrices(Px.detach().contiguous(), Ax.detach().contiguous(), q.detach().contiguous(),
+                           b.detach().contiguous())
+    engine.solve(copy_out=False)
+    f64 = dict(dtype=torch.float64, device=dev)
+    x, y, s = torch.empty(engine.n, **f64), torch.empty(engine.m, **f64), torch.empty(engine.m, **f64)
+    _, _, _, st = engine.polish(x=x, y=y, s=s)
+    if st["status"] != 1:
+        raise EngineError(st["status"], "solve_qp: the solution could not be polished (status %d), so it has no "
+                                        "derivative here" % st["status"])
+    engine._solve_qp_call = getattr(engine, "_solve_qp_call", 0) + 1
+    return x, y, s
+
+
+class _SolveQP(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, engine, refine_iter, Px, q, Ax, b):
+        x, y, s = _solve_and_polish(engine, Px, q, Ax, b)
+        ctx.engine, ctx.refine_iter, ctx.device, ctx.call = engine, refine_iter, q.device, engine._solve_qp_call
+        ctx.dtypes = (Px.dtype, q.dtype, Ax.dtype, b.dtype)
+        ctx.save_for_backward(Px, q, Ax, b)
+        return x, y, s
+
+    @staticmethod
+    def backward(ctx, gx, gy, gs):
+        eng = ctx.engine
+        dev = ctx.device
+        if eng._solve_qp_call != ctx.call:   # the engine has polished other data since: this pass's point again
+            _solve_and_polish(eng, *ctx.saved_tensors)
+            ctx.call = eng._solve_qp_call
+        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
+        f64 = dict(dtype=torch.float64, device=dev)
+        dq, db = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64)
+        dPx, dAx = torch.empty(eng.nnzP, **f64), torch.empty(eng.nnzA, **f64)
+        dl, du = torch.empty(eng.m, **f64), torch.empty(eng.m, **f64)
+        g = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (gx, gy, gs)]
+        _, st = eng.adjoint(*g, refine_iter=ctx.refine_iter, dq=dq, db=db, dPx=dPx, dAx=dAx, dl=dl, du=du)
+        if st["status"] != 1:
+            raise EngineError(st["status"], "solve_qp: the adjoint did not apply (status %d)" % st["status"])
+        tP, tq, tA, tb = ctx.dtypes
+        return None, None, dPx.to(tP), dq.to(tq), dAx.to(tA), db.to(tb)
+
+
+def solve_qp(engine, Px, q, Ax, b, refine_iter=3):
+    """The polished solution (x, y, s) of the engine's problem with the data (Px, q, Ax, b), differentiable with respect
+    to all four (see the module docstring)."""
+    return _SolveQP.apply(engine, refine_iter, Px, q, Ax, b)

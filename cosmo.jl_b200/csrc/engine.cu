@@ -40,6 +40,7 @@
 #include "mat_update.cuh"
 #include "custom_cone.cuh"
 #include "polish.cuh"
+#include "adjoint.cuh"
 
 namespace cosmo {
 
@@ -196,6 +197,8 @@ class EngineBase {
   virtual void solution(int complete_dual, double* x, double* y, double* s) = 0;
   virtual void rescale_iterates() = 0;
   virtual void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) = 0;
+  virtual void adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db,
+                       double* dPx, double* dAx, double* dl, double* du, double* out4) = 0;
 };
 
 template <typename T>
@@ -204,6 +207,7 @@ class Engine : public EngineBase {
   Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st);
   ~Engine() override;
   void update_settings(const cosmo_b200_settings& st) override {
+    drop_polish_record();
     if (st.sigma != st_.sigma) {   // sigma is baked into the captured kernel arguments
       destroy_cg_graphs();
       destroy_ldl_factor_graph();
@@ -255,6 +259,8 @@ class Engine : public EngineBase {
   void solution(int complete_dual, double* x, double* y, double* s) override;
   void rescale_iterates() override;
   void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) override;
+  void adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db, double* dPx,
+               double* dAx, double* dl, double* du, double* out4) override;
 
  private:
   // ---- problem ----
@@ -325,10 +331,24 @@ class Engine : public EngineBase {
   int last_status_ = COSMO_B200_UNDETERMINED;   // status of the last solve()
   bool conic_rows_ = false;      // a set other than ZeroSet, Nonnegatives and Box has rows (polishing does not apply)
   // solution polishing (polish.cuh): scratch allocated by the first polish and kept
-  DevBuf<T> pol_zx_, pol_znu_, pol_rhs_, pol_px_, pol_w_, pol_s_, pol_mu_, pol_rho_;
+  DevBuf<T> pol_zx_, pol_znu_, pol_rhs_, pol_px_, pol_w_, pol_s_, pol_mu_, pol_rho_, pol_nq_;
   DevBuf<unsigned char> pol_kind_;
   DevBuf<int> pol_cnt_;
-  void polish_residual(double* max2);
+  void polish_residual(const T* zx, const T* znu, const T* rx, const T* rs, double* max2);
+  // The record of the last polish, read by the adjoint (adjoint.cuh): its status, and with status 1 the plugin's
+  // factorisation count after it, while the factor still holds that polish's K~.  Every entry point that factors or
+  // changes the data, sigma, rho or the iterates drops it.
+  static constexpr int kNoPolishRecord = -2;
+  int pol_rec_status_ = kNoPolishRecord;
+  long long pol_rec_factors_ = -1;
+  void drop_polish_record() { pol_rec_status_ = kNoPolishRecord; }
+  long long direct_factorizations() const {
+    return st_.kkt_solver == COSMO_B200_KKT_LDL ? ldl_factorizations_ : sn_factorizations_;
+  }
+  // adjoint scratch, allocated by the first adjoint and kept: its own z (pol_zx_ / pol_znu_ hold the polished point the
+  // gradients read), the kept right-hand side, gs~ and two counters
+  DevBuf<T> adj_zx_, adj_zv_, adj_rx_, adj_rs_, adj_gs_;
+  DevBuf<int> adj_cnt_;
   void emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y, double* s);
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
@@ -374,7 +394,7 @@ class Engine : public EngineBase {
   Event ldl_ev_[2];
   void ldl_setup();
   void ldl_factor();
-  void ldl_solve();
+  void ldl_solve(bool kept_factor = false);
   void destroy_ldl_factor_graph() { ldl_factor_graph_.reset(); }
   bool direct_kkt() const { return st_.kkt_solver == COSMO_B200_KKT_LDL || st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL; }
   void direct_factor() {
@@ -398,7 +418,7 @@ class Engine : public EngineBase {
   GraphExec sn_factor_graph_, sn_solve_graph_;
   void sn_setup();
   void sn_factor();
-  void sn_solve();
+  void sn_solve(bool kept_factor = false);
   long long kkt_counter_ = 1;   // S.iteration_counter
   int last_cg_iters_ = 1;
   // tm_ = rho .* (A xsol_), stored by the fused ADMM tail: the next CG solve of the same solve() starts from it instead
@@ -1209,6 +1229,7 @@ void Engine<T>::get_scaling(void* D, void* E, double* c) {
 
 template <typename T>
 void Engine<T>::warm_start(const void* x, const void* s, const void* mu) {
+  drop_polish_record();
   caller_arrays({x, s, mu});
   have_solution_ = false;
   if (x) upload_vec(xs_, x, n_);
@@ -1219,6 +1240,7 @@ void Engine<T>::warm_start(const void* x, const void* s, const void* mu) {
 
 template <typename T>
 void Engine<T>::update_qb(const void* q, const void* b) {
+  drop_polish_record();
   caller_arrays({q, b});
   if (q) upload_vec(q_, q, n_);
   if (b) {
@@ -1232,6 +1254,7 @@ void Engine<T>::update_qb(const void* q, const void* b) {
 // settings leaves (mat_update.cuh): same scaling, rho vector, zero iterates, KKT call counter at 1, a fresh factor.
 template <typename T>
 void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, long long nnzA, const void* q, const void* b) {
+  drop_polish_record();
   if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "update_matrices: a sharded handle holds only a slice of the data"};
   if ((Px && nnzP != P_.nnz) || (Ax && nnzA != At_.nnz))
     throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices: nnz differs from the pattern given at create (a new pattern needs a new engine)"};
@@ -1251,6 +1274,7 @@ void Engine<T>::update_matrices(const void* Px, long long nnzP, const void* Ax, 
 template <typename T>
 void Engine<T>::update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
                                          const void* b) {
+  drop_polish_record();
   if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "update_matrices_original: a sharded handle holds only a slice of the data"};
   if (!fwd_.has_map()) throw EngineError{COSMO_B200_ERR_INVALID, "update_matrices_original: no forward map (cosmo_b200_set_forward_map)"};
   if ((Px && nnzP != P_.nnz) || (Ax && nnzA_orig != fwd_.nnzA_orig()))
@@ -1478,6 +1502,7 @@ void Engine<T>::update_slab(DevCsr<T>& M, int ebase) {
 
 template <typename T>
 void Engine<T>::update_rho(const void* rho_vec, double rho) {
+  drop_polish_record();
   if (rho_vec) upload_vec(rho_vec_, rho_vec, m_);
   rho_ = rho;
   ldl_dirty_ = true;   // update_rho! -> refactor! (kktsolver.jl:310-313), done before the next KKT solve
@@ -1487,6 +1512,7 @@ void Engine<T>::update_rho(const void* rho_vec, double rho) {
 
 template <typename T>
 void Engine<T>::reset() {
+  drop_polish_record();
   CUDA_TRY(cudaMemsetAsync(xs_.p, 0, std::max(n_, 1) * sizeof(T), stream_));
   CUDA_TRY(cudaMemsetAsync(s_.p, 0, std::max(m_, 1) * sizeof(T), stream_));
   CUDA_TRY(cudaMemsetAsync(mu_.p, 0, std::max(m_, 1) * sizeof(T), stream_));
@@ -2262,6 +2288,7 @@ bool Engine<T>::aa_accelerate(T* g) {
 
 template <typename T>
 void Engine<T>::set_accelerator(const cosmo_b200_accelerator* a) {
+  drop_polish_record();
   if (!a) {
     acc_ = cosmo_b200_accelerator{COSMO_B200_AA_TYPE2_QR, COSMO_B200_AA_RESTARTED_MEMORY, COSMO_B200_AA_NO_REGULARIZER,
                                   COSMO_B200_AA_IMMEDIATE, 0.0, 2, 0.0};
@@ -2290,6 +2317,7 @@ void Engine<T>::accelerator_stats(int64_t* out) {
 template <typename T>
 void Engine<T>::solve(cosmo_b200_result* out) {
   const double t_start = now_s();
+  drop_polish_record();
   const unsigned dev_out = out ? caller_arrays({out->x, out->s, out->mu}) : 0u;
   const int n = n_, m = m_;
   const long long launches0 = launches_;
@@ -2540,6 +2568,7 @@ void Engine<T>::project(const void* ws, void* s_out) {
 
 template <typename T>
 void Engine<T>::kkt_solve(const void* rhs, void* sol, int64_t* inner) {
+  drop_polish_record();
   CUDA_TRY(cudaSetDevice(device_));
   tm_valid_ = false;
   upload_vec(ls_, rhs, (size_t)n_ + m_);
@@ -2668,12 +2697,14 @@ void Engine<T>::ldl_factor() {
   ldl_dirty_ = false;
 }
 
-// [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: forward and backward levels replayed as one graph
+// [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: forward and backward levels replayed as one graph.
+// kept_factor: solve with the factor in memory even when it is marked dirty (the adjoint, with the factor of a polish);
+// the solve reads only the factor, ls_ and the permutation, never sigma or the rho vector.
 template <typename T>
-void Engine<T>::ldl_solve() {
+void Engine<T>::ldl_solve(bool kept_factor) {
   if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU"};
   if (!ldl_ready_) ldl_setup();
-  if (ldl_dirty_) ldl_factor();
+  if (ldl_dirty_ && !kept_factor) ldl_factor();
   if (!ldl_solve_graph_) {
     int nodes = 0;
     capture_graph(ldl_solve_graph_, stream_, [&] {
@@ -2879,12 +2910,12 @@ void Engine<T>::sn_factor() {
 }
 
 // [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: the forward solve by supernodal level, the
-// backward solve by depth, replayed as one graph
+// backward solve by depth, replayed as one graph (kept_factor as for ldl_solve)
 template <typename T>
-void Engine<T>::sn_solve() {
+void Engine<T>::sn_solve(bool kept_factor) {
   if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the supernodal LDL' KKT solver is single-GPU"};
   if (!sn_ready_) sn_setup();
-  if (sn_dirty_) sn_factor();
+  if (sn_dirty_ && !kept_factor) sn_factor();
   const ldl_sn::Symbolic& S = sn_;
   if (!sn_solve_graph_) {
     int nodes = 0;
@@ -3098,6 +3129,7 @@ void Engine<T>::caller_written() {
 // anything is written.
 template <typename T>
 void Engine<T>::update_qb_original(const double* q, const double* b) {
+  drop_polish_record();
   single_gpu("update_qb_original");
   const bool dev_b = (caller_arrays({q, b}) & 2) != 0;
   const bool mapped = fwd_.has_map();
@@ -3190,6 +3222,7 @@ void Engine<T>::emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int 
 // start) on the resident iterates; like warm_start it ends the last solution.
 template <typename T>
 void Engine<T>::rescale_iterates() {
+  drop_polish_record();
   single_gpu("rescale_iterates");
   CUDA_TRY(cudaSetDevice(device_));
   have_solution_ = false;
@@ -3199,17 +3232,18 @@ void Engine<T>::rescale_iterates() {
   sync();
 }
 
-// r^ - K_A z of the exact reduced system (polish.cuh) into ls_, the right-hand side of the next refinement solve:
-// P x, then the x rows over A' nu and the s rows over A x.  max2 (optional) = {|r_x|_inf, |r_s|_inf}.
+// r^ - K_A z of the exact reduced system (polish.cuh) into ls_, the right-hand side of the next refinement solve, for
+// z = (zx, znu) and r^ = (rx, rs on the active rows): P x, then the x rows over A' nu and the s rows over A x.  max2
+// (optional) = {|r_x|_inf, |r_s|_inf}.
 template <typename T>
-void Engine<T>::polish_residual(double* max2) {
+void Engine<T>::polish_residual(const T* zx, const T* znu, const T* rx, const T* rs, double* max2) {
   const int n = n_, m = m_;
-  launch_spmv(P_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n, EpiStore<T>{nullptr, pol_px_.p}, red(SC_TMP6),
+  launch_spmv(P_, zx, (const DevCsr<T>*)nullptr, (const T*)nullptr, n, EpiStore<T>{nullptr, pol_px_.p}, red(SC_TMP6),
               "spmv_polish_P");
-  launch_spmv(At_, pol_znu_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n,
-              EpiPolishResX<T>{nullptr, ls_.p, q_.p, pol_px_.p}, red(SC_TMP6), "spmv_polish_res_x");
-  launch_spmv(A_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m,
-              EpiPolishResS<T>{nullptr, ls_.p + n, pol_rhs_.p, pol_kind_.p}, red(SC_TMP7), "spmv_polish_res_s");
+  launch_spmv(At_, znu, (const DevCsr<T>*)nullptr, (const T*)nullptr, n,
+              EpiPolishResX<T>{nullptr, ls_.p, rx, pol_px_.p}, red(SC_TMP6), "spmv_polish_res_x");
+  launch_spmv(A_, zx, (const DevCsr<T>*)nullptr, (const T*)nullptr, m,
+              EpiPolishResS<T>{nullptr, ls_.p + n, rs, pol_kind_.p}, red(SC_TMP7), "spmv_polish_res_s");
   if (max2) {
     read_scalars(SC_TMP6, 2);
     max2[0] = (double)h_sc_[SC_TMP6];
@@ -3231,11 +3265,13 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
   if (!have_solution_)
     throw EngineError{COSMO_B200_ERR_INVALID, "polish: no solve since the engine was created, reset or warm-started"};
   CUDA_TRY(cudaSetDevice(device_));
+  drop_polish_record();   // a polish that fails leaves none
   out[0] = -1.0; out[1] = out[2] = out[3] = 0.0;
   for (int k = 4; k < 8; ++k) out[k] = NAN;
   if (conic_rows_ || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE || last_status_ == COSMO_B200_DUAL_INFEASIBLE ||
       last_status_ == COSMO_B200_UNSOLVED) {
     emit_solution(xs_.p, s_.p, mu_.p, 0, x, y, s);
+    pol_rec_status_ = -1;
     return;
   }
   const int n = n_, m = m_;
@@ -3243,7 +3279,7 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
     pol_zx_.alloc(std::max(n, 1)); pol_px_.alloc(std::max(n, 1)); pol_w_.alloc((size_t)n + m + 1);
     pol_znu_.alloc(std::max(m, 1)); pol_rhs_.alloc(std::max(m, 1)); pol_s_.alloc(std::max(m, 1));
     pol_mu_.alloc(std::max(m, 1)); pol_rho_.alloc(std::max(m, 1));
-    pol_kind_.alloc(std::max(m, 1)); pol_cnt_.alloc(POLISH_CNT_COUNT);
+    pol_kind_.alloc(std::max(m, 1)); pol_cnt_.alloc(POLISH_CNT_COUNT); pol_nq_.alloc(std::max(n, 1));
   }
   // the solve's rho vector and sigma come back whatever happens below; the factor then follows them again
   const double sigma0 = st_.sigma;
@@ -3265,7 +3301,7 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
     PolishClassifyArgs<T> a;
     a.n = n; a.m = m; a.row_class = row_class_.p; a.box_l = box_l_.p; a.box_u = box_u_.p; a.b = b_.p; a.q = q_.p;
     a.s = s_.p; a.mu = mu_.p; a.x = xs_.p; a.delta = (T)p.delta;
-    a.kind = pol_kind_.p; a.rhs = pol_rhs_.p; a.rho = rho_vec_.p; a.ls = ls_.p; a.counts = pol_cnt_.p;
+    a.kind = pol_kind_.p; a.rhs = pol_rhs_.p; a.rho = rho_vec_.p; a.ls = ls_.p; a.counts = pol_cnt_.p; a.nq = pol_nq_.p;
     polish_classify_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(a);
     check_launch("polish_classify");
     int cnt[POLISH_CNT_COUNT] = {0, 0, 0, 0};
@@ -3286,14 +3322,14 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
         else sn_solve();
       };
       for (int k = 0; k <= p.refine_iter; ++k) {
-        if (k > 0) polish_residual(nullptr);
+        if (k > 0) polish_residual(pol_zx_.p, pol_znu_.p, pol_nq_.p, pol_rhs_.p, nullptr);
         plugin_solve();
         polish_update_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, xsol_.p, nu_.p, pol_zx_.p,
                                                                                   pol_znu_.p, k == 0 ? 1 : 0);
         check_launch("polish_update");
       }
       double rmax[2];
-      polish_residual(rmax);
+      polish_residual(pol_zx_.p, pol_znu_.p, pol_nq_.p, pol_rhs_.p, rmax);
       // the candidate: x_p, s_p = Pi_K(b - A x_p), mu_p = the clipped -nu
       launch_spmv(A_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m, EpiPolishSlack<T>{nullptr, pol_w_.p + n, b_.p},
                   red(SC_TMP6), "spmv_polish_slack");
@@ -3319,6 +3355,125 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
   if (polished) emit_solution(pol_zx_.p, pol_s_.p, pol_mu_.p, 0, x, y, s);
   else emit_solution(xs_.p, s_.p, mu_.p, 0, x, y, s);
   sync();
+  // restore() marked the factor dirty but did not refactor: it still holds this polish's K~ for the adjoint
+  pol_rec_status_ = polished ? 1 : 0;
+  pol_rec_factors_ = direct_factorizations();
+}
+
+// Derivatives of the polished solution (DESIGN.md §3j, adjoint.cuh): the right-hand side from the incoming gradients,
+// refine_iter + 1 solves with the factor the polish left and its refinement against the exact K_A, then the gradients
+// of q, b, the Box bounds, P and A.  Nothing is factored; the iterates, the solution, rho, the statistics and the polish
+// record stay as they are.
+template <typename T>
+void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db,
+                        double* dPx, double* dAx, double* dl, double* du, double* out) {
+  if (refine_iter < 0 || refine_iter > 100) throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: refine_iter in 0 .. 100"};
+  single_gpu("adjoint");
+  if (!direct_kkt())
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "adjoint: needs a direct KKT plugin (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver)"};
+  if (pol_rec_status_ == kNoPolishRecord)
+    throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: no polish since the last solve, update, reset or warm start"};
+  if (pol_rec_status_ == 1 && pol_rec_factors_ != direct_factorizations())
+    throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: the factor of the last polish has been replaced"};
+  const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
+  const int n = n_, m = m_;
+  const long long nnzP = P_.nnz, nnzA = At_.nnz;
+  struct Out { double* p; long long count; };
+  const Out outs[6] = {{dq, n}, {db, m}, {dPx, nnzP}, {dAx, nnzA}, {dl, m}, {du, m}};
+  out[0] = pol_rec_status_; out[1] = out[2] = 0.0; out[3] = NAN;
+  if (pol_rec_status_ != 1) {
+    for (int k = 0; k < 6; ++k) {
+      if (!outs[k].p || !outs[k].count) continue;
+      if (dev & (8u << k)) {
+        adjoint_nan_kernel<<<vgrid(outs[k].count), kBlock, 0, stream_>>>(outs[k].count, outs[k].p);
+        check_launch("adjoint_nan");
+      } else {
+        std::fill(outs[k].p, outs[k].p + outs[k].count, std::numeric_limits<double>::quiet_NaN());
+      }
+    }
+    if (dev) caller_written();
+    sync();
+    return;
+  }
+  if (!adj_cnt_.p) {
+    adj_zx_.alloc(std::max(n, 1)); adj_rx_.alloc(std::max(n, 1));
+    adj_zv_.alloc(std::max(m, 1)); adj_rs_.alloc(std::max(m, 1)); adj_gs_.alloc(std::max(m, 1));
+    adj_cnt_.alloc(ADJ_CNT_COUNT);
+  }
+  // host arrays are staged through one fp64 device buffer; device arrays are read and written in place
+  const double* ins[3] = {dx, dy, ds};
+  const long long in_count[3] = {n, m, m};
+  long long stage_n = 0;
+  for (int k = 0; k < 3; ++k) if (ins[k] && !(dev & (1u << k))) stage_n += in_count[k];
+  for (int k = 0; k < 6; ++k) if (outs[k].p && !(dev & (8u << k))) stage_n += outs[k].count;
+  DevBuf<double> stage;
+  if (stage_n) stage.alloc((size_t)stage_n, false);
+  long long off = 0;
+  const double* din[3];
+  for (int k = 0; k < 3; ++k) {
+    din[k] = ins[k];
+    if (ins[k] && !(dev & (1u << k))) {
+      if (in_count[k]) CUDA_TRY(cudaMemcpyAsync(stage.p + off, ins[k], in_count[k] * sizeof(double), cudaMemcpyHostToDevice, stream_));
+      din[k] = stage.p + off;
+      off += in_count[k];
+    }
+  }
+  double* dout[6];
+  for (int k = 0; k < 6; ++k) {
+    dout[k] = outs[k].p;
+    if (outs[k].p && !(dev & (8u << k))) {
+      dout[k] = stage.p + off;
+      off += outs[k].count;
+    }
+  }
+  const T* D = scaled_ ? D_.p : nullptr;
+  const T* Ev = scaled_ ? E_.p : nullptr;
+  const double c = scaled_ ? c_ : 1.0;
+  // right-hand side: s rows and gs~, then the x rows over A' gs~, into ls_ and the kept copies
+  adjoint_rhs_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, din[1], din[2], Ev, c, adj_gs_.p, adj_rs_.p, ls_.p);
+  check_launch("adjoint_rhs");
+  launch_spmv(At_, adj_gs_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n, EpiAdjointRhsX<T>{nullptr, adj_rx_.p, ls_.p, din[0], D},
+              red(SC_TMP6), "spmv_adjoint_rhs_x");
+  // the first solve from z = 0, then refine_iter steps against the exact K_A, v masked off the active rows
+  for (int k = 0; k <= refine_iter; ++k) {
+    if (k > 0) polish_residual(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, nullptr);
+    if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_solve(true);
+    else sn_solve(true);
+    polish_update_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, xsol_.p, nu_.p, adj_zx_.p,
+                                                                              adj_zv_.p, k == 0 ? 1 : 0);
+    check_launch("polish_update");
+  }
+  double rmax[2];
+  polish_residual(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, rmax);
+  // gradients
+  CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
+  AdjointVecArgs<T> a;
+  a.n = n; a.m = m; a.kind = pol_kind_.p; a.row_class = row_class_.p; a.u = adj_zx_.p; a.v = adj_zv_.p; a.gs = adj_gs_.p;
+  a.mu_p = pol_mu_.p; a.D = D; a.E = Ev; a.c = c;
+  a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5]; a.counts = adj_cnt_.p;
+  adjoint_grad_vec_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(a);
+  check_launch("adjoint_grad_vec");
+  if (dout[2] && nnzP) {
+    if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only, not the slab maps
+    adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.d_src.p, adj_zx_.p,
+                                                                             pol_zx_.p, D, c, dout[2]);
+    check_launch("adjoint_grad_P");
+  }
+  if (dout[3] && nnzA) {
+    adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, adj_zx_.p, pol_zx_.p,
+                                                                             adj_zv_.p, pol_mu_.p, adj_gs_.p, D, Ev, dout[3]);
+    check_launch("adjoint_grad_A");
+  }
+  int cnt[ADJ_CNT_COUNT] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+  for (int k = 0; k < 6; ++k)
+    if (outs[k].p && dout[k] != outs[k].p && outs[k].count)
+      CUDA_TRY(cudaMemcpyAsync(outs[k].p, dout[k], outs[k].count * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  if (dev) caller_written();
+  sync();
+  out[1] = cnt[ADJ_CNT_ACTIVE];
+  out[2] = cnt[ADJ_CNT_WEAK];
+  out[3] = std::max(rmax[0], rmax[1]);
 }
 
 }  // namespace cosmo
@@ -3574,6 +3729,11 @@ int cosmo_b200_polish(cosmo_b200_handle* h, const cosmo_b200_polish_settings* ps
                       double out[8]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->polish(ps, x, y, s, out));
+}
+int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* dx, const double* dy, const double* ds,
+                       double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double out[4]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->adjoint(refine_iter, dx, dy, ds, dq, db, dPx, dAx, dl, du, out));
 }
 int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
   ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));

@@ -38,6 +38,7 @@ struct PolishClassifyArgs {
   const T* x;            // resident x
   T* ls;                 // out: the first right-hand side [-q + delta x; rhs + delta mu on the active rows] (n + m)
   int* counts;           // POLISH_CNT_COUNT ints, zero on entry
+  T* nq;                 // out: -q, the x rows of the exact right-hand side (n)
 };
 
 // Row classification (DESIGN §3i step 1) and the first right-hand side, one thread per entry of [x; s].  The first
@@ -59,6 +60,7 @@ __global__ void __launch_bounds__(kBlock) polish_classify_kernel(PolishClassifyA
     unsigned char kd = POLISH_INACTIVE;
     if (idx < a.n) {
       a.ls[idx] = a.delta * a.x[idx] - a.q[idx];
+      a.nq[idx] = -a.q[idx];
     } else if (idx < total) {
       const int r = idx - a.n;
       const unsigned char cls = a.row_class[r];
@@ -123,23 +125,26 @@ __global__ void __launch_bounds__(kBlock) polish_finish_kernel(int m, const unsi
 }
 
 // ---- SpMV epilogues of the refinement residual and the candidate slack --------------------------------------------
-// x rows of r^ - K_A z over A' nu (px = P x precomputed):  r_x = -q - P x - A' nu,   max0 = |r_x|_inf
+// x rows of r^ - K_A z over A' nu (px = P x precomputed):  r_x = rx - P x - A' nu,   max0 = |r_x|_inf.  rx is -q for the
+// polish (the negation is exact, so this is -q - P x - A' nu bit for bit) and the adjoint's right-hand side for
+// cosmo_b200_adjoint (adjoint.cuh).
 template <typename T>
 struct EpiPolishResX {
   static constexpr int NS = 0, NM = 1;
   const int* done;
   T* out;
-  const T* q;
+  const T* rx;
   const T* px;
   __device__ void row(int r, T atnu, T*, T* accM) const {
-    const T v = -q[r] - (px[r] + atnu);
+    const T v = rx[r] - (px[r] + atnu);
     out[r] = v;
     accM[0] = nanmax(accM[0], tabs(v));
   }
   __device__ void operator()(T*) const {}
 };
 
-// s rows over A x:  r_s = rhs - A x on the active rows, 0 elsewhere,   max0 = |r_s|_inf
+// s rows over A x:  r_s = rhs - A x on the active rows, 0 elsewhere,   max0 = |r_s|_inf (rhs: b - sbar for the polish,
+// the adjoint's s rows for cosmo_b200_adjoint)
 template <typename T>
 struct EpiPolishResS {
   static constexpr int NS = 0, NM = 1;

@@ -121,6 +121,8 @@ class PolishSettings(C.Structure):
 
 POLISH_STATUS = {1: "Polished", 0: "Unpolished", -1: "Not_applicable"}
 POLISH_STATS = ("status", "n_lower", "n_upper", "n_equality", "r_prim", "r_dual", "obj_val", "refine_residual")
+# cosmo_b200_adjoint's out[4]
+ADJOINT_STATS = ("status", "n_active", "n_weak", "refine_residual")
 
 
 def _signatures():
@@ -168,6 +170,7 @@ def _signatures():
         "cosmo_b200_solution": (rc, [vp, i32, vp, vp, vp]),
         "cosmo_b200_rescale_iterates": (rc, [vp]),
         "cosmo_b200_polish": (rc, [vp, P(PolishSettings), vp, vp, vp, P(f64)]),
+        "cosmo_b200_adjoint": (rc, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_comm_unique_id": (rc, [vp]),
         "cosmo_b200_comm_init": (rc, [vp, i32, i32, vp]),
         "cosmo_b200_comm_p2p_export": (rc, [vp, vp]),
@@ -428,6 +431,7 @@ class Engine:
         P.sort_indices()
         A.sort_indices()
         self.m, self.n = A.shape
+        self.nnzP, self.nnzA = len(P.data), len(A.data)
         self.n_psd = sum(1 for t in sets if t[0] in (PSD_SQUARE, PSD_TRIANGLE, PSD_TRIANGLE_COMPLEX) and int(t[1]) > 0)
         keep = []  # keep host arrays alive during create
         set_arr = (SetStruct * max(len(sets), 1))()
@@ -589,6 +593,20 @@ class Engine:
         stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_polish, self._h, C.byref(st), _ptr(px), _ptr(py), _ptr(ps),
                        ctype=C.c_double, keys=POLISH_STATS, ints=POLISH_STATS[:4])
         return x, y, s, stats
+
+    def adjoint(self, dx=None, dy=None, ds=None, refine_iter=3, dq=None, db=None, dPx=None, dAx=None, dl=None, du=None):
+        """cosmo_b200_adjoint: the gradients of a loss with respect to the data from its gradients dx, dy, ds with
+        respect to the last polished solution (fp64, host or CUDA arrays; None: zero).  dq (n), db, dl, du (m), dPx and
+        dAx (the ``data`` order of P and A as given to create / update_matrices) are fp64 outputs, host or CUDA arrays;
+        None allocates a NumPy array.  Returns ((dq, db, dPx, dAx, dl, du), stats), stats keyed by ADJOINT_STATS (status 1
+        computed, 0 the polish was rejected, -1 it did not apply, the outputs then NaN; the counts as ints)."""
+        gx, gy, gs = (self._arr(a, k, np.float64) for a, k in ((dx, self.n), (dy, self.m), (ds, self.m)))
+        sizes = (self.n, self.m, self.nnzP, self.nnzA, self.m, self.m)
+        outs = [np.empty(k) if a is None else a for a, k in zip((dq, db, dPx, dAx, dl, du), sizes)]
+        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
+        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_adjoint, self._h, int(refine_iter), _ptr(gx), _ptr(gy),
+                       _ptr(gs), *ptrs, ctype=C.c_double, keys=ADJOINT_STATS, ints=ADJOINT_STATS[:3])
+        return tuple(outs), stats
 
     def update_matrices(self, Px=None, Ax=None, q=None, b=None):
         """cosmo_b200_update_matrices: new values of P and A on the pattern of create -- ``Px`` / ``Ax`` are the ``data``

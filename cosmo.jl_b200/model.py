@@ -528,6 +528,7 @@ class Model:
         self._q0 = self._b0 = None
         self._qb_on_device = [False, False]   # q0 / b0 came as CUDA arrays: the engine holds them (original_qb)
         self._solution_on_device = False      # optimize(solution="device"): x, s, mu live only in the engine
+        self._polished = False                # the last optimize() polished: the engine can differentiate it (adjoint)
 
     # q0 and b0 after update(q=, b=) with CUDA arrays are read back from the engine only when something reads them
     @property
@@ -628,6 +629,7 @@ class Model:
         self._x2 = None
         self._fwd = None
         self._solution_on_device = False
+        self._polished = False
         if self.engine is not None:
             self.engine.close()
             self.engine = None
@@ -664,6 +666,7 @@ class Model:
     def update(self, q=None, b=None, *, P=None, A=None):
         if not self.is_assembled:
             raise RuntimeError("Model has to be assembled once before one can start updating q or b.")
+        self._polished = False
         if _eng.is_cuda_array(q) or _eng.is_cuda_array(b):
             for v, k, name in ((q, self.n, "q"), (b, self.m, "b")):
                 if _eng.is_cuda_array(v) and tuple(v.__cuda_array_interface__["shape"]) != (k,):
@@ -817,6 +820,7 @@ class Model:
         if solution == "device" and self.settings.polish:
             raise ValueError("polish=True needs solution=\"host\"; with the solution on the device call Engine.polish")
         t0 = time.perf_counter()
+        self._polished = False
         setup_time = self._setup()
         if self.settings.time_limit != 0 or (self.settings.adaptive_rho and self.settings.adaptive_rho_interval == 0):
             st = self.settings.to_struct()           # both rules count setup! (solver.jl:119,244-256,349)
@@ -855,12 +859,29 @@ class Model:
                 _, _, _, pst = self.engine.polish(self.settings.polish_delta, self.settings.polish_refine_iter, xp, yp, sp_)
                 polish = _eng.POLISH_STATUS[pst["status"]]
                 if pst["status"] == 1:
+                    self._polished = True
                     x, y, s, obj_val = xp, yp, sp_, pst["obj_val"]
                     info.r_prim, info.r_dual = pst["r_prim"], pst["r_dual"]
             times["polish_time"] = time.perf_counter() - tp
         times["solver_time"] = time.perf_counter() - t0
         return Result(x, y, s, obj_val, out.iter, out.safeguarding_iter, out.status, info, times,
                       kkt_inner_iterations=out.kkt_inner_iterations, kernel_launches=out.kernel_launches, polish=polish)
+
+    def adjoint(self, dx=None, dy=None, ds=None, refine_iter=3):
+        """Gradients of a scalar loss with respect to the data, from its gradients dx (n), dy, ds (m) with respect to the
+        polished solution (x, y, s) of the last optimize() (None: zero), through cosmo_b200_adjoint (DESIGN.md §3j).
+        Returns a dict in the coordinates update() takes: "P" and "A" as CSC matrices on the patterns of P0 and A0 (set!
+        form A x + s = b; "P" is the symmetrised gradient: moving both stored (i, j) and (j, i) by e changes the loss by
+        2 e dP_ij), "q", "b", and "l", "u", m-vectors zero off Box rows, plus "stats" (Engine.ADJOINT_STATS).  ValueError
+        unless the last optimize() returned polish == "Polished"."""
+        if not self._polished or self.engine is None:
+            raise ValueError("adjoint needs the last optimize() to have returned polish == \"Polished\" "
+                             "(Settings(polish=True) and a direct KKT solver)")
+        (dq, db, dPx, dAx, dl, du), st = self.engine.adjoint(dx, dy, ds, refine_iter)
+        P0, A0 = self.P0, self.A0
+        return {"P": sp.csc_matrix((dPx, P0.indices, P0.indptr), shape=P0.shape),
+                "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
+                "q": dq, "b": db, "l": dl, "u": du, "stats": st}
 
     def solution_into(self, x=None, y=None, s=None):
         """The last solution (x, y, s of Result, completed as settings.complete_dual asks) into caller fp64 arrays, CUDA

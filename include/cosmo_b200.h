@@ -568,6 +568,33 @@ typedef struct {
 int cosmo_b200_polish(cosmo_b200_handle* h, const cosmo_b200_polish_settings* ps, double* x, double* y, double* s,
                       double out[8]);
 
+/* ---- derivatives of a polished solution ------------------------------------ */
+/* An engine extension beyond the reference, like cosmo_b200_polish: nothing changes unless it is called.  Given the
+   gradients dx (n), dy, ds (m) of a scalar loss with respect to the last polished solution (x, y, s) of
+   cosmo_b200_polish, it returns the gradients of that loss with respect to the data, in the unscaled set! form
+   A x + s = b, y = -mu, on the active set A of the polish (at an accepted polish P x + q + A_A' y_A = 0 and
+   A_A x = b_A - sbar_A):  with K_A [u; v] = [dx - A' ds; dy on A], v = 0 off A,
+     dq = -u,  db = v + ds,  dP_ij = -(u_i x_j + x_i u_j) / 2 (symmetrised: moving both stored (i, j) and (j, i) by e
+     changes the loss by 2 e dP_ij),  dA_rj = -(y_r u_j + v_r x_j) - ds_r x_j,
+     dl_r = -v_r on lower-active Box rows, du_r = -v_r on upper-active ones, dl_r = du_r = -v_r / 2 on Box rows with
+     l = u, 0 on every other row.
+   The system is solved in the engine's scaled coordinates with the factor of the regularised K~ the polish left in the
+   direct plugin, from z = 0, then refined refine_iter (0 .. 100) times against the exact K_A; nothing is factored.
+   dPx (nnz P) is in the CSC order of P given to create / update_matrices, dAx (nnz A) in that of A; dq (n), db, dl, du
+   (m) are vectors.  All are fp64, host or device, under the caller-memory rules of cosmo_b200_solution; a NULL input
+   is zero, a NULL output is skipped.  out = {status, active rows, weakly active rows (lower- or upper-active rows whose
+   clipped multiplier is 0: the derivative there is one-sided), |r|_inf of the scaled adjoint system after the last
+   step}.  status 1: the gradients are written.  0: the last polish was rejected; -1: it did not apply (conic rows,
+   an infeasible or unsolved solve): the outputs are NaN, the counts 0 and the residual NaN.  No polish since the last
+   solve, kkt_solve, warm_start, update_qb(_original), update_matrices(_original), update_rho, update_settings,
+   set_accelerator, reset or rescale_iterates, or a factor replaced since the polish: COSMO_B200_ERR_INVALID.  An
+   indirect plugin or a sharded handle: COSMO_B200_ERR_UNSUPPORTED.  The iterates, the solution, rho, the statistics
+   and the polish record stay as they are, so two calls give bit-identical results.  Scratch of about 2 n + 3 m values
+   of the element type is allocated by the first call and kept; host arrays are staged through a buffer of their size.
+   DESIGN.md §3j. */
+int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* dx, const double* dy, const double* ds,
+                       double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double out[4]);
+
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
 int cosmo_b200_comm_unique_id(void* id128);
