@@ -1,4 +1,4 @@
-"""torch.autograd for polished QP and LP solves on the device (DESIGN.md §3j).
+"""torch.autograd for solves on the device: polished QPs and LPs (DESIGN.md §3j) and conic problems (§3k).
 
 ``solve_qp(engine, Px, q, Ax, b)`` puts new values of P, q, A and b into a live engine (``Engine.update_matrices``),
 solves, polishes and returns the polished unscaled solution ``(x, y, s)`` as CUDA tensors; its backward pass is one
@@ -71,3 +71,61 @@ def solve_qp(engine, Px, q, Ax, b, refine_iter=3):
     """The polished solution (x, y, s) of the engine's problem with the data (Px, q, Ax, b), differentiable with respect
     to all four (see the module docstring)."""
     return _SolveQP.apply(engine, refine_iter, Px, q, Ax, b)
+
+
+def _solve(engine, Px, q, Ax, b):
+    """update_matrices and solve, then the unscaled solution into new CUDA tensors; returns (x, y, s) and tags the engine
+    with this call."""
+    dev = q.device
+    engine.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
+    engine.update_matrices(Px.detach().contiguous(), Ax.detach().contiguous(), q.detach().contiguous(),
+                           b.detach().contiguous())
+    out = engine.solve(copy_out=False)
+    if out.status != "Solved":
+        raise EngineError(0, "solve_conic: the solve ended %s, not Solved, so its solution has no derivative here"
+                          % out.status)
+    f64 = dict(dtype=torch.float64, device=dev)
+    x, y, s = torch.empty(engine.n, **f64), torch.empty(engine.m, **f64), torch.empty(engine.m, **f64)
+    engine.solution(x=x, y=y, s=s)
+    engine._solve_conic_call = getattr(engine, "_solve_conic_call", 0) + 1
+    return x, y, s
+
+
+class _SolveConic(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, engine, settings, Px, q, Ax, b):
+        x, y, s = _solve(engine, Px, q, Ax, b)
+        ctx.engine, ctx.settings, ctx.device, ctx.call = engine, settings, q.device, engine._solve_conic_call
+        ctx.dtypes = (Px.dtype, q.dtype, Ax.dtype, b.dtype)
+        ctx.save_for_backward(Px, q, Ax, b)
+        return x, y, s
+
+    @staticmethod
+    def backward(ctx, gx, gy, gs):
+        eng = ctx.engine
+        dev = ctx.device
+        if eng._solve_conic_call != ctx.call:   # the engine has solved other data since: this pass's point again
+            _solve(eng, *ctx.saved_tensors)
+            ctx.call = eng._solve_conic_call
+        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
+        f64 = dict(dtype=torch.float64, device=dev)
+        dq, db = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64)
+        dPx, dAx = torch.empty(eng.nnzP, **f64), torch.empty(eng.nnzA, **f64)
+        g = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (gx, gy, gs)]
+        _, st = eng.solve_adjoint(*g, dq=dq, db=db, dPx=dPx, dAx=dAx, **ctx.settings)
+        if st["status"] != 1:
+            raise EngineError(st["status"], "solve_conic: the solve adjoint did not apply or converge (status %d)"
+                              % st["status"])
+        tP, tq, tA, tb = ctx.dtypes
+        return None, None, dPx.to(tP), dq.to(tq), dAx.to(tA), db.to(tb)
+
+
+def solve_conic(engine, Px, q, Ax, b, **adjoint_settings):
+    """The solution (x, y, s) of the engine's problem with the data (Px, q, Ax, b), differentiable with respect to all four
+    through Engine.solve_adjoint (DESIGN.md §3k): any cone but Exp/Pow, custom and complex PSD cones, any single-GPU
+    KKT solver.  The engine is created as for solve_qp (on the pattern of P and A, without host scaling); the forward
+    pass raises unless the solve ends Solved.  adjoint_settings (tol, max_iter, restart, kkt_tol) go to
+    Engine.solve_adjoint.  The derivative is that of the solution map at the solve's point, exact as the solve's
+    tolerance goes to 0.  The engine rules of solve_qp apply: between a forward pass and its backward pass it is used
+    only through solve_conic, and a backward pass after other solves re-solves its own data first."""
+    return _SolveConic.apply(engine, dict(adjoint_settings), Px, q, Ax, b)

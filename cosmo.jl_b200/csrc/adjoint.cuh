@@ -129,7 +129,7 @@ __global__ void __launch_bounds__(kBlock) adjoint_grad_P_kernel(int n, const int
 }
 
 // dA over CSR(A') (its value order is A's CSC order), one warp per column j of A:
-//   dA_rj = E_r D_j (-(y_r u_j + v_r x_j) - gs~_r x_j),   y = -mu_p
+//   dA_rj = E_r D_j (-(y_r u_j + v_r x_j) - gs~_r x_j),   y = -mu_p  (gs null: no gs~ term; the solve adjoint)
 template <typename T>
 __global__ void __launch_bounds__(kBlock) adjoint_grad_A_kernel(int n, const int* __restrict__ rowptr, const int* __restrict__ col,
                                                                 const T* __restrict__ u, const T* __restrict__ x,
@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(kBlock) adjoint_grad_A_kernel(int n, const int
     for (int k = rowptr[j] + lane; k < rowptr[j + 1]; k += 32) {
       const int r = col[k];
       const double y = -(double)mu_p[r];
-      const double g = -(y * uj + (double)v[r] * xj) - (double)gs[r] * xj;
+      const double g = -(y * uj + (double)v[r] * xj) - (gs ? (double)gs[r] * xj : 0.0);
       dAx[k] = (E ? (double)E[r] * dj : dj) * g;
     }
   }

@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(kBlock) cg_persistent_kernel(CgPersistArgs<T> 
   T res2, rhs2;
   fold_partials2(a.partA, res2, rhs2);
   T res = sqrt(res2), prev = T(1);
-  const T tol = a.tol_num / sqrt(rhs2);
+  const T tol = inner_abstol(a.tol_num, sqrt(rhs2));
   int it = 0;
 
   while (!(res <= tol) && it < maxit) {

@@ -41,6 +41,7 @@
 #include "custom_cone.cuh"
 #include "polish.cuh"
 #include "adjoint.cuh"
+#include "solve_adjoint.cuh"
 
 namespace cosmo {
 
@@ -199,6 +200,9 @@ class EngineBase {
   virtual void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) = 0;
   virtual void adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db,
                        double* dPx, double* dAx, double* dl, double* du, double* out4) = 0;
+  virtual void solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy,
+                             const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
+                             double* out8) = 0;
 };
 
 template <typename T>
@@ -261,6 +265,8 @@ class Engine : public EngineBase {
   void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) override;
   void adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db, double* dPx,
                double* dAx, double* dl, double* du, double* out4) override;
+  void solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy, const double* ds,
+                     double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double* out8) override;
 
  private:
   // ---- problem ----
@@ -349,6 +355,29 @@ class Engine : public EngineBase {
   // gradients read), the kept right-hand side, gs~ and two counters
   DevBuf<T> adj_zx_, adj_zv_, adj_rx_, adj_rs_, adj_gs_;
   DevBuf<int> adj_cnt_;
+  // fp64 caller arrays of the two adjoints: dev holds their caller_arrays bits, the inputs first, then the outputs.  Host
+  // arrays are staged through `stage`, device arrays are read and written in place.
+  struct F64Out { double* p; long long count; };
+  void stage_f64(unsigned dev, const double* const* ins, const long long* in_count, int nin, const F64Out* outs, int nout,
+                 DevBuf<double>& stage, const double** din, double** dout);
+  void unstage_f64(const F64Out* outs, double* const* dout, int nout);
+  void nan_f64(unsigned dev, int nin, const F64Out* outs, int nout);
+  // solve adjoint (solve_adjoint.cuh): scratch allocated by the first call and kept -- the Krylov basis with lam and gw,
+  // the point w_s, two m-vectors for Dpi, the row flags, the SOC norms and x'h, the eigenpairs of the PSD cones (small
+  // cones first, then large ones) and three N x N work matrices for the largest large cone, the saved plugin state
+  int sa_restart_ = 0;
+  DevBuf<T> sa_V_, sa_ws_, sa_h_, sa_dh_, sa_soc_r_, sa_psd_q_, sa_psd_lam_, sa_psd_work_, sa_save_;
+  DevBuf<unsigned char> sa_flag_;
+  DevBuf<double> sa_part_, sa_hd_, sa_soc_dot_;
+  DevBuf<long long> sa_q_off_;
+  DevBuf<int> sa_lam_off_, sa_cnt_;
+  std::vector<long long> sa_large_q_off_;
+  std::vector<int> sa_large_lam_off_;
+  void sa_alloc(int restart);
+  void sa_dots(const T* V, long long ldv, int k, const T* w, double* out);
+  void sa_dpi(const T* h, T* out);
+  void sa_kkt(const T* lam);
+  void sa_operator(const T* lam, T* out);
   void emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y, double* s);
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
@@ -420,6 +449,7 @@ class Engine : public EngineBase {
   void sn_factor();
   void sn_solve(bool kept_factor = false);
   long long kkt_counter_ = 1;   // S.iteration_counter
+  double kkt_tol_fixed_ = 0.0;  // > 0: the fixed relative tolerance of the solve adjoint's inner solves (inner_tol)
   int last_cg_iters_ = 1;
   // tm_ = rho .* (A xsol_), stored by the fused ADMM tail: the next CG solve of the same solve() starts from it instead
   // of recomputing the product.  It never outlives one solve() call: solve() and kkt_solve() clear it on entry (so
@@ -517,7 +547,13 @@ class Engine : public EngineBase {
   void kkt_cg(const int* done, bool tm_ready);
   void kkt_minres(bool full);
   // get_tolerance (kktsolver_indirect.jl:168-170): tol_constant / k^tol_exponent for the k-th inner solve
-  double inner_tol() const { return st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent); }
+  // (negative: kkt_tol_fixed_ as a relative tolerance, inner_abstol in vector_kernels.cuh)
+  double inner_tol() const {
+    return kkt_tol_fixed_ > 0.0 ? -kkt_tol_fixed_ : st_.tol_constant / pow((double)kkt_counter_, st_.tol_exponent);
+  }
+  // the iteration cap of an inner solve: the reference's size of the system, at least 1000 for the fixed tolerance of
+  // the solve adjoint (rounding makes small, ill-conditioned systems need more than size-many steps to reach it)
+  int inner_maxit(int size) const { return kkt_tol_fixed_ > 0.0 ? std::max(size, 1000) : size; }
   template <typename Enqueue>
   int poll_inner(const Enqueue& enqueue);
   void set_maxit(int v);
@@ -1821,7 +1857,7 @@ void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
 // cg!(previous_solution, L, y1; abstol = tol_k/|y1|, reltol = 0) (kktsolver_indirect.jl:70)
 template <typename T>
 void Engine<T>::kkt_cg(const int* done, bool tm_ready) {
-  set_maxit(n_);   // IterativeSolvers default maxiter = size(A, 2)
+  set_maxit(inner_maxit(n_));   // IterativeSolvers default maxiter = size(A, 2)
   if (persistent_cg_ok()) {
     launch_persistent_cg(inner_tol());
     return;
@@ -1952,7 +1988,7 @@ void Engine<T>::kkt_minres(bool full) {
   const int* done = isc_.p + ISC_DONE;
   T* x = full ? mr_x_.p : xsol_.p;
   const T* b = full ? mr_b_.p : rhsb_.p;
-  set_maxit(full ? n_ + m_ : n_);
+  set_maxit(inner_maxit(full ? n_ + m_ : n_));
   if (full) {
     CUDA_TRY(cudaMemcpyAsync(mr_b_.p, ls_.p, n_ * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
     CUDA_TRY(cudaMemcpyAsync(mr_b_.p + npad, ls_.p + n_, m_ * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
@@ -3378,21 +3414,10 @@ void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, con
   const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
   const int n = n_, m = m_;
   const long long nnzP = P_.nnz, nnzA = At_.nnz;
-  struct Out { double* p; long long count; };
-  const Out outs[6] = {{dq, n}, {db, m}, {dPx, nnzP}, {dAx, nnzA}, {dl, m}, {du, m}};
+  const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, nnzP}, {dAx, nnzA}, {dl, m}, {du, m}};
   out[0] = pol_rec_status_; out[1] = out[2] = 0.0; out[3] = NAN;
   if (pol_rec_status_ != 1) {
-    for (int k = 0; k < 6; ++k) {
-      if (!outs[k].p || !outs[k].count) continue;
-      if (dev & (8u << k)) {
-        adjoint_nan_kernel<<<vgrid(outs[k].count), kBlock, 0, stream_>>>(outs[k].count, outs[k].p);
-        check_launch("adjoint_nan");
-      } else {
-        std::fill(outs[k].p, outs[k].p + outs[k].count, std::numeric_limits<double>::quiet_NaN());
-      }
-    }
-    if (dev) caller_written();
-    sync();
+    nan_f64(dev, 3, outs, 6);
     return;
   }
   if (!adj_cnt_.p) {
@@ -3400,32 +3425,12 @@ void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, con
     adj_zv_.alloc(std::max(m, 1)); adj_rs_.alloc(std::max(m, 1)); adj_gs_.alloc(std::max(m, 1));
     adj_cnt_.alloc(ADJ_CNT_COUNT);
   }
-  // host arrays are staged through one fp64 device buffer; device arrays are read and written in place
   const double* ins[3] = {dx, dy, ds};
   const long long in_count[3] = {n, m, m};
-  long long stage_n = 0;
-  for (int k = 0; k < 3; ++k) if (ins[k] && !(dev & (1u << k))) stage_n += in_count[k];
-  for (int k = 0; k < 6; ++k) if (outs[k].p && !(dev & (8u << k))) stage_n += outs[k].count;
   DevBuf<double> stage;
-  if (stage_n) stage.alloc((size_t)stage_n, false);
-  long long off = 0;
   const double* din[3];
-  for (int k = 0; k < 3; ++k) {
-    din[k] = ins[k];
-    if (ins[k] && !(dev & (1u << k))) {
-      if (in_count[k]) CUDA_TRY(cudaMemcpyAsync(stage.p + off, ins[k], in_count[k] * sizeof(double), cudaMemcpyHostToDevice, stream_));
-      din[k] = stage.p + off;
-      off += in_count[k];
-    }
-  }
   double* dout[6];
-  for (int k = 0; k < 6; ++k) {
-    dout[k] = outs[k].p;
-    if (outs[k].p && !(dev & (8u << k))) {
-      dout[k] = stage.p + off;
-      off += outs[k].count;
-    }
-  }
+  stage_f64(dev, ins, in_count, 3, outs, 6, stage, din, dout);
   const T* D = scaled_ ? D_.p : nullptr;
   const T* Ev = scaled_ ? E_.p : nullptr;
   const double c = scaled_ ? c_ : 1.0;
@@ -3466,14 +3471,443 @@ void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, con
   }
   int cnt[ADJ_CNT_COUNT] = {0, 0};
   CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
-  for (int k = 0; k < 6; ++k)
-    if (outs[k].p && dout[k] != outs[k].p && outs[k].count)
-      CUDA_TRY(cudaMemcpyAsync(outs[k].p, dout[k], outs[k].count * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  unstage_f64(outs, dout, 6);
   if (dev) caller_written();
   sync();
   out[1] = cnt[ADJ_CNT_ACTIVE];
   out[2] = cnt[ADJ_CNT_WEAK];
   out[3] = std::max(rmax[0], rmax[1]);
+}
+
+template <typename T>
+void Engine<T>::stage_f64(unsigned dev, const double* const* ins, const long long* in_count, int nin, const F64Out* outs,
+                          int nout, DevBuf<double>& stage, const double** din, double** dout) {
+  long long stage_n = 0;
+  for (int k = 0; k < nin; ++k) if (ins[k] && !(dev & (1u << k))) stage_n += in_count[k];
+  for (int k = 0; k < nout; ++k) if (outs[k].p && !(dev & (1u << (nin + k)))) stage_n += outs[k].count;
+  if (stage_n) stage.alloc((size_t)stage_n, false);
+  long long off = 0;
+  for (int k = 0; k < nin; ++k) {
+    din[k] = ins[k];
+    if (ins[k] && !(dev & (1u << k))) {
+      if (in_count[k]) CUDA_TRY(cudaMemcpyAsync(stage.p + off, ins[k], in_count[k] * sizeof(double), cudaMemcpyHostToDevice, stream_));
+      din[k] = stage.p + off;
+      off += in_count[k];
+    }
+  }
+  for (int k = 0; k < nout; ++k) {
+    dout[k] = outs[k].p;
+    if (outs[k].p && !(dev & (1u << (nin + k)))) {
+      dout[k] = stage.p + off;
+      off += outs[k].count;
+    }
+  }
+}
+
+template <typename T>
+void Engine<T>::unstage_f64(const F64Out* outs, double* const* dout, int nout) {
+  for (int k = 0; k < nout; ++k)
+    if (outs[k].p && dout[k] != outs[k].p && outs[k].count)
+      CUDA_TRY(cudaMemcpyAsync(outs[k].p, dout[k], outs[k].count * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+}
+
+// NaN into every output of a call whose status is not 1, then the caller-stream handshake and a synchronise
+template <typename T>
+void Engine<T>::nan_f64(unsigned dev, int nin, const F64Out* outs, int nout) {
+  for (int k = 0; k < nout; ++k) {
+    if (!outs[k].p || !outs[k].count) continue;
+    if (dev & (1u << (nin + k))) {
+      adjoint_nan_kernel<<<vgrid(outs[k].count), kBlock, 0, stream_>>>(outs[k].count, outs[k].p);
+      check_launch("adjoint_nan");
+    } else {
+      std::fill(outs[k].p, outs[k].p + outs[k].count, std::numeric_limits<double>::quiet_NaN());
+    }
+  }
+  if (dev) caller_written();
+  sync();
+}
+
+// ---- solve adjoint (DESIGN.md §3k, solve_adjoint.cuh) ---------------------------------------------------------------
+template <typename T>
+void Engine<T>::sa_alloc(int restart) {
+  const long long L = (long long)n_ + m_;
+  const int m1 = std::max(m_, 1);
+  if (restart > sa_restart_) {
+    sa_restart_ = 0;   // until the three buffers below are in place
+    sa_V_.alloc((size_t)(restart + 3) * std::max<long long>(L, 1), false);   // restart + 1 basis columns, lam, gw
+    sa_part_.alloc((size_t)264 * (restart + 1), false);
+    sa_hd_.alloc((size_t)3 * (restart + 1) + 2, false);
+    sa_restart_ = restart;
+  }
+  const size_t save = (size_t)std::max(n_, 1) + (mr_x_.p ? mr_x_.n : 0);   // xsol_ and the full MINRES warm start
+  if (sa_save_.n < save) sa_save_.alloc(save, false);
+  if (sa_cnt_.p) return;
+  sa_ws_.alloc(m1, false); sa_h_.alloc(m1); sa_dh_.alloc(m1); sa_flag_.alloc(m1);
+  sa_cnt_.alloc(SA_CNT_COUNT);
+  if (n_soc_) { sa_soc_r_.alloc(n_soc_); sa_soc_dot_.alloc((size_t)n_soc_ + std::max(n_soc_chunks_, 1)); }
+  if (!psd_.empty()) {
+    std::vector<long long> q_off;
+    std::vector<int> lam_off;
+    sa_large_q_off_.clear();
+    sa_large_lam_off_.clear();
+    long long q = 0;
+    int l = 0, large_max = 0;
+    for (const PsdConeDesc& d : psd_.small_h) { q_off.push_back(q); lam_off.push_back(l); q += (long long)d.N * d.N; l += d.N; }
+    for (const PsdConeDesc& d : psd_.large_h) {
+      sa_large_q_off_.push_back(q); sa_large_lam_off_.push_back(l);
+      q += (long long)d.N * d.N; l += d.N;
+      large_max = std::max(large_max, d.N);
+    }
+    sa_psd_q_.alloc((size_t)q, false);
+    sa_psd_lam_.alloc((size_t)l, false);
+    if (!q_off.empty()) { sa_q_off_.upload(q_off, stream_); sa_lam_off_.upload(lam_off, stream_); }
+    if (large_max) sa_psd_work_.alloc((size_t)3 * large_max * large_max, false);
+    // the attribute belongs to the function on the device: raise it to the worst case of kPsdSmallMax once
+    const size_t ld_max = (size_t)(kPsdSmallMax | 1);
+    CUDA_TRY(cudaFuncSetAttribute(sa_psd_small_apply_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)(2 * ld_max * kPsdSmallMax * sizeof(T))));
+    sync();
+  }
+}
+
+// out[0 .. k) = V_c'w for the k columns V_c = V + c ldv: fixed-order block partials folded in order
+template <typename T>
+void Engine<T>::sa_dots(const T* V, long long ldv, int k, const T* w, double* out) {
+  const long long L = (long long)n_ + m_;
+  const int nb = (int)std::min<long long>(std::max<long long>((L + kBlock - 1) / kBlock, 1), 264);
+  sa_dots_kernel<T><<<dim3(nb, k), kBlock, 0, stream_>>>(L, V, ldv, w, sa_part_.p);
+  check_launch("sa_dots");
+  sa_fold_kernel<<<(k + 127) / 128, 128, 0, stream_>>>(k, nb, sa_part_.p, out);
+  check_launch("sa_fold");
+}
+
+// out = Dpi h at the point sa_ws_ (m-vectors): the rows and SOC cones elementwise after the per-cone x'h, the small PSD
+// cones one CTA each, each large cone by four bj_gemm_kernel products around a Hadamard kernel
+template <typename T>
+void Engine<T>::sa_dpi(const T* h, T* out) {
+  if (n_soc_) {
+    if (n_soc_chunks_) {
+      sa_soc_dot_chunk_kernel<T><<<n_soc_chunks_, kBlock, 0, stream_>>>(sa_ws_.p, h, soc_chunk_start_.p, soc_chunk_len_.p,
+                                                                       sa_soc_dot_.p + n_soc_);
+      check_launch("sa_soc_dot_chunk");
+    }
+    sa_soc_dot_final_kernel<<<(n_soc_ + 127) / 128, 128, 0, stream_>>>(sa_soc_dot_.p + n_soc_, soc_cone_chunk_ptr_.p, n_soc_,
+                                                                        sa_soc_dot_.p);
+    check_launch("sa_soc_dot_final");
+  }
+  sa_dpi_rows_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, row_class_.p, row_cone_.p, sa_flag_.p, soc_off_.p, sa_ws_.p,
+                                                           sa_soc_r_.p, sa_soc_dot_.p, h, out);
+  check_launch("sa_dpi_rows");
+  if (!psd_.small_h.empty()) {
+    const size_t ld = (size_t)(psd_.small_maxN | 1);
+    sa_psd_small_apply_kernel<T><<<(int)psd_.small_h.size(), kBlock, 2 * ld * psd_.small_maxN * sizeof(T), stream_>>>(
+        psd_.small_d.p, sa_q_off_.p, sa_lam_off_.p, sa_psd_q_.p, sa_psd_lam_.p, h, out);
+    check_launch("sa_psd_small_apply");
+  }
+  for (size_t k = 0; k < psd_.large_h.size(); ++k) {
+    const PsdConeDesc& d = psd_.large_h[k];
+    const int N = d.N;
+    const long long NN = (long long)N * N;
+    T* H = sa_psd_work_.p;
+    T* W1 = H + NN;
+    T* W2 = W1 + NN;
+    const T* Q = sa_psd_q_.p + sa_large_q_off_[k];
+    const T* lam = sa_psd_lam_.p + sa_large_lam_off_[k];
+    const int g = vgrid(NN);
+    const dim3 gg((N + 127) / 128, (N + 127) / 128);
+    sa_psd_load_kernel<T><<<g, kBlock, 0, stream_>>>(d, h, H);
+    check_launch("sa_psd_load");
+    bj_gemm_kernel<T, false><<<gg, kBlock, 0, stream_>>>(N, H, Q, W1);    // W1 = H Q
+    check_launch("bj_gemm");
+    bj_gemm_kernel<T, true><<<gg, kBlock, 0, stream_>>>(N, Q, W1, H);     // H = Q' W1
+    check_launch("bj_gemm");
+    sa_psd_hadamard_kernel<T><<<g, kBlock, 0, stream_>>>(N, lam, Q, H, W2);   // H = Gamma o H, W2 = Q'
+    check_launch("sa_psd_hadamard");
+    bj_gemm_kernel<T, false><<<gg, kBlock, 0, stream_>>>(N, H, W2, W1);   // W1 = H Q'
+    check_launch("bj_gemm");
+    bj_gemm_kernel<T, false><<<gg, kBlock, 0, stream_>>>(N, Q, W1, H);    // H = Q W1
+    check_launch("bj_gemm");
+    sa_psd_store_kernel<T><<<g, kBlock, 0, stream_>>>(d, H, out);
+    check_launch("sa_psd_store");
+  }
+}
+
+// [xsol_; nu_] = K^-1 [lam_x; -lam_s / rho] through the plugin (kkt_core), each solve from zero
+template <typename T>
+void Engine<T>::sa_kkt(const T* lam) {
+  const int n = n_, m = m_;
+  CUDA_TRY(cudaMemsetAsync(xsol_.p, 0, std::max(n, 1) * sizeof(T), stream_));
+  if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));
+  sa_op_rhs_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, lam, rho_vec_.p, ls_.p, t0_.p);
+  check_launch("sa_op_rhs");
+  tm_valid_ = false;
+  kkt_core(false, nullptr, nullptr);
+}
+
+// out = (I - M') lam = lam - [sigma a; b + Dpi(lam_s - 2 b)],  [a; b] = K^-1 [lam_x; -lam_s / rho]
+template <typename T>
+void Engine<T>::sa_operator(const T* lam, T* out) {
+  const int n = n_, m = m_;
+  sa_kkt(lam);
+  sa_op_mid_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, lam + n, nu_.p, sa_h_.p);
+  check_launch("sa_op_mid");
+  sa_dpi(sa_h_.p, sa_dh_.p);
+  sa_op_out_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, lam, xsol_.p, nu_.p, sa_dh_.p, (T)st_.sigma, out);
+  check_launch("sa_op_out");
+}
+
+// Derivatives of the last solve's solution through the fixed point of the iteration (DESIGN.md §3k): the Jacobian data
+// of the point, the right-hand side gw, GMRES(restart) on (I - M') lam = gw, one more plugin solve for [u; v] and the
+// gradients.  The iterates, the solution, rho, the statistics and the polish record stay as they are; the plugin state
+// the inner solves move (the CG warm start, the KKT counter, the inner iteration state) is put back.
+template <typename T>
+void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy,
+                              const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
+                              double* out) {
+  cosmo_b200_solve_adjoint_settings p{0.0, 500, 30, 1e-12, 0};
+  if (as) p = *as;
+  if (!(p.tol >= 0.0 && p.tol < 1.0) || p.max_iter < 1 || p.restart < 1 || p.restart > 200 ||
+      !(p.kkt_tol > 0.0 && p.kkt_tol < 1.0) || p.reserved != 0)
+    throw EngineError{COSMO_B200_ERR_INVALID, "solve_adjoint: tol in [0, 1), max_iter >= 1, restart in 1 .. 200, kkt_tol in (0, 1), reserved 0"};
+  single_gpu("solve_adjoint");
+  if (fwd_.has_map() || rev_.has_map())
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "solve_adjoint: gradients through a forward or decomposition map are not supported"};
+  if (!have_solution_)
+    throw EngineError{COSMO_B200_ERR_INVALID, "solve_adjoint: no solve since the engine was created, reset or warm-started"};
+  CUDA_TRY(cudaSetDevice(device_));
+  const double tol = p.tol > 0.0 ? p.tol : (sizeof(T) == sizeof(double) ? 1e-10 : 1e-5);
+  const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
+  const int n = n_, m = m_;
+  const long long L = (long long)n + m;
+  const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, P_.nnz}, {dAx, At_.nnz}, {dl, m}, {du, m}};
+  for (int k = 1; k < 8; ++k) out[k] = 0.0;
+  out[2] = NAN;
+  bool complex_psd = false;
+  for (const PsdConeDesc& d : psd_.small_h) complex_psd = complex_psd || d.triangle == 2;
+  for (const PsdConeDesc& d : psd_.large_h) complex_psd = complex_psd || d.triangle == 2;
+  if (n_c3_ || n_cust_ || complex_psd || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
+      last_status_ == COSMO_B200_DUAL_INFEASIBLE || last_status_ == COSMO_B200_UNSOLVED) {
+    out[0] = -1.0;
+    nan_f64(dev, 3, outs, 6);
+    return;
+  }
+  const int R = p.restart;
+  sa_alloc(R);
+  // ---- the plugin state the inner solves move, saved and put back at the end
+  const long long kkt_counter0 = kkt_counter_, total_inner0 = total_inner_, total_mults0 = total_mults_;
+  const long long persist0 = persist_solves_;
+  const bool tm_valid0 = tm_valid_;
+  const int last_cg_iters0 = last_cg_iters_, cur_maxit0 = cur_maxit_, psd_sweeps0 = psd_.last_sweeps;
+  const bool had_mr_x = mr_x_.p != nullptr;
+  int isc0[ISC_COUNT];
+  CUDA_TRY(cudaMemcpyAsync(isc0, isc_.p, sizeof(isc0), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(sa_save_.p, xsol_.p, std::max(n, 1) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  if (had_mr_x) CUDA_TRY(cudaMemcpyAsync(sa_save_.p + std::max(n, 1), mr_x_.p, mr_x_.n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  sync();
+  auto restore = [&] {
+    CUDA_TRY(cudaMemcpyAsync(xsol_.p, sa_save_.p, std::max(n, 1) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+    if (had_mr_x) CUDA_TRY(cudaMemcpyAsync(mr_x_.p, sa_save_.p + std::max(n, 1), mr_x_.n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+    else if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));   // as a first allocation leaves it
+    CUDA_TRY(cudaMemcpyAsync(isc_.p, isc0, sizeof(isc0), cudaMemcpyHostToDevice, stream_));
+    sync();
+    h_isc_[ISC_MAXIT] = isc0[ISC_MAXIT];
+    kkt_counter_ = kkt_counter0; total_inner_ = total_inner0; total_mults_ = total_mults0; persist_solves_ = persist0;
+    tm_valid_ = tm_valid0; last_cg_iters_ = last_cg_iters0; cur_maxit_ = cur_maxit0; psd_.last_sweeps = psd_sweeps0;
+    kkt_tol_fixed_ = 0.0;
+  };
+  try {
+    const double* ins[3] = {dx, dy, ds};
+    const long long in_count[3] = {n, m, m};
+    DevBuf<double> stage;
+    const double* din[3];
+    double* dout[6];
+    stage_f64(dev, ins, in_count, 3, outs, 6, stage, din, dout);
+    const T* D = scaled_ ? D_.p : nullptr;
+    const T* Ev = scaled_ ? E_.p : nullptr;
+    const double c = scaled_ ? c_ : 1.0;
+    // ---- the point w_s = s + mu / rho and its Jacobian data
+    CUDA_TRY(cudaMemsetAsync(sa_cnt_.p, 0, SA_CNT_COUNT * sizeof(int), stream_));
+    ws_from_mu_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, rho_vec_.p, mu_.p, s_.p, sa_ws_.p);
+    check_launch("ws_from_mu");
+    sa_row_flags_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_ws_.p, box_l_.p, box_u_.p, sa_flag_.p, sa_cnt_.p);
+    check_launch("sa_row_flags");
+    if (n_soc_) {
+      soc_norms(sa_ws_.p, sa_soc_r_.p);
+      sa_soc_kink_kernel<T><<<vgrid(n_soc_), kBlock, 0, stream_>>>(n_soc_, soc_off_.p, sa_ws_.p, sa_soc_r_.p, sa_cnt_.p);
+      check_launch("sa_soc_kink");
+    }
+    const int sweeps = st_.psd_max_sweeps > 0 ? st_.psd_max_sweeps : 30;
+    int psd_unconverged = 0;
+    if (!psd_.small_h.empty()) {
+      PsdEigOut<T> eo;
+      eo.Q = sa_psd_q_.p; eo.lam = sa_psd_lam_.p; eo.q_off = sa_q_off_.p; eo.lam_off = sa_lam_off_.p;
+      eo.kinks = sa_cnt_.p + SA_CNT_PSD;
+      psd_small_kernel<T><<<(int)psd_.small_h.size(), kBlock, psd_.small_smem(), stream_>>>(
+          psd_.small_d.p, sa_ws_.p, nullptr, 2, nullptr, sweeps, sa_cnt_.p + SA_CNT_PSD_UNCONVERGED, eo);
+      check_launch("psd_small_eig");
+    }
+    for (size_t k = 0; k < psd_.large_h.size(); ++k) {
+      const PsdConeDesc& d = psd_.large_h[k];
+      if (!psd_.large_eig(d, sa_ws_.p, stream_, sweeps, launches_, /*allow_warm=*/false, /*certificate=*/false,
+                          /*no_throw=*/true)) {
+        ++psd_unconverged;
+        continue;
+      }
+      CUDA_TRY(cudaMemcpyAsync(sa_psd_q_.p + sa_large_q_off_[k], psd_.V_d.p, (size_t)d.N * d.N * sizeof(T),
+                               cudaMemcpyDeviceToDevice, stream_));
+      sa_psd_large_eig_kernel<T><<<1, kBlock, 0, stream_>>>(d.N, psd_.A_d.p, psd_.up_d.p, psd_.mx_d.p,
+                                                             sa_psd_lam_.p + sa_large_lam_off_[k], sa_cnt_.p);
+      check_launch("sa_psd_large_eig");
+    }
+    int cnt[SA_CNT_COUNT];
+    CUDA_TRY(cudaMemcpyAsync(cnt, sa_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+    sync();
+    psd_unconverged += cnt[SA_CNT_PSD_UNCONVERGED];
+    out[4] = cnt[SA_CNT_ROWS]; out[5] = cnt[SA_CNT_SOC]; out[6] = cnt[SA_CNT_PSD]; out[7] = psd_unconverged;
+    // ---- GMRES(R) on (I - M') lam = gw; the basis V_0 .. V_R, then lam and gw, in sa_V_
+    T* V = sa_V_.p;
+    T* lam = V + (long long)(R + 1) * L;
+    T* gw = lam + L;
+    double* h1 = sa_hd_.p;            // the two CGS passes, |w|^2, then the update coefficients y
+    double* h2 = h1 + (R + 1);
+    double* nrm2 = h2 + (R + 1);
+    double* yd = nrm2 + 1;
+    kkt_tol_fixed_ = p.kkt_tol;
+    int isc_start[ISC_COUNT];
+    CUDA_TRY(cudaMemcpyAsync(isc_start, isc_.p, sizeof(isc_start), cudaMemcpyDeviceToHost, stream_));
+    const long long inner_start = total_inner_;
+    long long apps = 0;
+    bool converged = false;
+    double rel = NAN;
+    if (psd_unconverged == 0) {
+      sa_gw_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, din[0], din[1], din[2], D, Ev, c, rho_vec_.p, gw, sa_h_.p);
+      check_launch("sa_gw");
+      sa_dpi(sa_h_.p, sa_dh_.p);
+      sa_gw_s_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, din[1], Ev, c, rho_vec_.p, sa_dh_.p, gw + n);
+      check_launch("sa_gw_s");
+      CUDA_TRY(cudaMemsetAsync(lam, 0, L * sizeof(T), stream_));
+      sa_dots(gw, L, 1, gw, nrm2);
+      double g2 = 0.0;
+      CUDA_TRY(cudaMemcpyAsync(&g2, nrm2, sizeof(double), cudaMemcpyDeviceToHost, stream_));
+      sync();
+      const double gnorm = sqrt(g2);
+      if (!(gnorm > 0.0)) {
+        converged = gnorm == 0.0;   // gw = 0: lam = 0
+        rel = converged ? 0.0 : NAN;
+      } else {
+        // r_0 = gw (lam = 0): V_0 = gw / |gw|
+        CUDA_TRY(cudaMemcpyAsync(V, gw, L * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+        sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, V);
+        check_launch("sa_normalise");
+        double beta = gnorm;
+        std::vector<double> H((size_t)(R + 1) * R), cs(R), sn(R), g(R + 1), y(R), hh(2 * (R + 1) + 1);
+        for (;;) {
+          std::fill(g.begin(), g.end(), 0.0);
+          g[0] = beta;
+          int k = 0;
+          while (k < R && apps + 1 < p.max_iter) {   // one application stays for the explicit residual
+            T* w = V + (long long)(k + 1) * L;
+            sa_operator(V + (long long)k * L, w);
+            ++apps;
+            // CGS2: two classical Gram-Schmidt passes against V_0 .. V_k, then |w|
+            sa_dots(V, L, k + 1, w, h1);
+            sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k + 1, h1, -1.0, w);
+            check_launch("sa_axpy");
+            sa_dots(V, L, k + 1, w, h2);
+            sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k + 1, h2, -1.0, w);
+            check_launch("sa_axpy");
+            sa_dots(w, L, 1, w, nrm2);
+            sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, w);
+            check_launch("sa_normalise");
+            CUDA_TRY(cudaMemcpyAsync(hh.data(), h1, hh.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+            sync();
+            double* col = H.data() + (size_t)k * (R + 1);
+            for (int i = 0; i <= k; ++i) col[i] = hh[i] + hh[R + 1 + i];
+            col[k + 1] = sqrt(hh[2 * (R + 1)]);
+            const bool breakdown = !(col[k + 1] > 0.0);
+            for (int i = 0; i < k; ++i) {   // the previous Givens rotations
+              const double a = col[i], b = col[i + 1];
+              col[i] = cs[i] * a + sn[i] * b;
+              col[i + 1] = -sn[i] * a + cs[i] * b;
+            }
+            const double r = std::hypot(col[k], col[k + 1]);
+            cs[k] = r > 0.0 ? col[k] / r : 1.0;
+            sn[k] = r > 0.0 ? col[k + 1] / r : 0.0;
+            col[k] = r;
+            col[k + 1] = 0.0;
+            g[k + 1] = -sn[k] * g[k];
+            g[k] = cs[k] * g[k];
+            ++k;
+            if (breakdown || fabs(g[k]) <= tol * gnorm) break;
+          }
+          if (k > 0) {   // lam += V y, H y = g by back substitution
+            for (int i = k - 1; i >= 0; --i) {
+              double v = g[i];
+              for (int j = i + 1; j < k; ++j) v -= H[(size_t)j * (R + 1) + i] * y[j];
+              y[i] = v / H[(size_t)i * (R + 1) + i];
+            }
+            CUDA_TRY(cudaMemcpyAsync(yd, y.data(), k * sizeof(double), cudaMemcpyHostToDevice, stream_));
+            sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k, yd, 1.0, lam);
+            check_launch("sa_axpy");
+          }
+          // the explicit residual r = gw - (I - M') lam into V_0
+          sa_operator(lam, V);
+          ++apps;
+          sa_residual_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, gw, V);
+          check_launch("sa_residual");
+          sa_dots(V, L, 1, V, nrm2);
+          double r2 = 0.0;
+          CUDA_TRY(cudaMemcpyAsync(&r2, nrm2, sizeof(double), cudaMemcpyDeviceToHost, stream_));
+          sync();
+          beta = sqrt(r2);
+          rel = beta / gnorm;
+          if (rel <= tol) { converged = true; break; }
+          if (!(rel == rel) || apps + 1 >= p.max_iter) break;
+          sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, V);
+          check_launch("sa_normalise");
+        }
+      }
+    }
+    out[1] = (double)apps;
+    out[2] = rel;
+    if (!converged) {
+      out[0] = 0.0;
+    } else {
+      // ---- [u; v] = K^-1 [lam_x; -lam_s / rho] into xsol_ / nu_, then the gradients
+      sa_kkt(lam);
+      SolveAdjointVecArgs<T> a;
+      a.n = n; a.m = m; a.row_class = row_class_.p; a.flag = sa_flag_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
+      a.u = xsol_.p; a.v = nu_.p; a.lam_s = lam + n; a.rho = rho_vec_.p; a.gy = din[1]; a.gs = din[2];
+      a.D = D; a.E = Ev; a.c = c;
+      a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5];
+      solve_adjoint_grad_vec_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(a);
+      check_launch("solve_adjoint_grad_vec");
+      if (dout[2] && P_.nnz) {
+        if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only, not the slab maps
+        adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.d_src.p, xsol_.p,
+                                                                                 xs_.p, D, c, dout[2]);
+        check_launch("adjoint_grad_P");
+      }
+      if (dout[3] && At_.nnz) {
+        adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, xsol_.p, xs_.p,
+                                                                                 nu_.p, mu_.p, nullptr, D, Ev, dout[3]);
+        check_launch("adjoint_grad_A");
+      }
+      unstage_f64(outs, dout, 6);
+      out[0] = 1.0;
+    }
+    int isc_end[ISC_COUNT];
+    CUDA_TRY(cudaMemcpyAsync(isc_end, isc_.p, sizeof(isc_end), cudaMemcpyDeviceToHost, stream_));
+    sync();
+    out[3] = direct_kkt() ? 0.0 : (double)(total_inner_ - inner_start + (isc_end[ISC_TOTAL] - isc_start[ISC_TOTAL]));
+    restore();
+    if (!converged) nan_f64(dev, 3, outs, 6);
+    else if (dev) caller_written();
+    sync();
+  } catch (...) {
+    restore();
+    throw;
+  }
 }
 
 }  // namespace cosmo
@@ -3734,6 +4168,12 @@ int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* 
                        double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double out[4]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->adjoint(refine_iter, dx, dy, ds, dq, db, dPx, dAx, dl, du, out));
+}
+int cosmo_b200_solve_adjoint(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dx,
+                             const double* dy, const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl,
+                             double* du, double out[8]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->solve_adjoint(as, dx, dy, ds, dq, db, dPx, dAx, dl, du, out));
 }
 int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
   ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));

@@ -117,7 +117,10 @@ __global__ void __launch_bounds__(kBlock) psd_embedding_store_kernel(PsdConeDesc
 
 // ---------------------------------------------------------------------------
 // Small cones: one CTA per cone, everything in shared memory.
-//   mode 0: s[cone] = Pi_PSD(ws[cone]);  mode 1: lam_max[cone] = max eigenvalue of mat(ws[cone])
+//   mode 0: s[cone] = Pi_PSD(ws[cone]);  mode 1: lam_max[cone] = max eigenvalue of mat(ws[cone]);
+//   mode 2: the eigenpairs of mat(ws[cone]) (symmetrised as in mode 0) into eig (the Jacobian of the projection,
+//           solve_adjoint.cuh): Q column-major at eig.Q + eig.q_off[cone], the eigenvalues at eig.lam + eig.lam_off[cone],
+//           and the cone counted in eig.kinks when an eigenvalue is within 64 u (1 + max |w_s|) of 0
 // mode 0 symmetrizes a square cone as project! does (symmetrize_upper!); mode 1 reads its upper triangle only, as the
 // certificate is_pos_def! -> cholesky!(Hermitian(X)) does (convexset.jl:324-336, algebra.jl:226-233): delta y and
 // A delta x are not symmetric on the rows of a square cone in general.  In mode 1 a cone whose Jacobi sweeps did not
@@ -125,9 +128,19 @@ __global__ void __launch_bounds__(kBlock) psd_embedding_store_kernel(PsdConeDesc
 // underestimate lambda_max) and increments *fail_flag.
 // ---------------------------------------------------------------------------
 template <typename T>
+struct PsdEigOut {
+  T* Q = nullptr;
+  T* lam = nullptr;
+  const long long* q_off = nullptr;
+  const int* lam_off = nullptr;
+  int* kinks = nullptr;
+};
+
+template <typename T>
 __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __restrict__ descs, const T* __restrict__ ws,
                                                            T* __restrict__ s, int mode, T* __restrict__ lam_max,
-                                                           int max_sweeps, int* __restrict__ fail_flag) {
+                                                           int max_sweeps, int* __restrict__ fail_flag,
+                                                           PsdEigOut<T> eig = PsdEigOut<T>()) {
   extern __shared__ unsigned char smem_raw[];
   const PsdConeDesc d = descs[blockIdx.x];
   const int N = d.N;
@@ -135,8 +148,15 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
   if (N == 1) {
     if (threadIdx.x == 0) {
       const T v = x[0];
-      if (mode == 0) s[d.off] = (v > T(0)) ? v : ((v != v) ? v : T(0));
-      else lam_max[blockIdx.x] = v;
+      if (mode == 0) {
+        s[d.off] = (v > T(0)) ? v : ((v != v) ? v : T(0));
+      } else if (mode == 1) {
+        lam_max[blockIdx.x] = v;
+      } else {
+        eig.Q[eig.q_off[blockIdx.x]] = T(1);
+        eig.lam[eig.lam_off[blockIdx.x]] = v;
+        if (tabs(v) <= (T)(64.0 * PsdEps<T>::v) * (T(1) + tabs(v))) atomicAdd(eig.kinks, 1);
+      }
     }
     return;
   }
@@ -178,6 +198,7 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
   __syncthreads();
   mx = red[0];
   for (int w = 1; w < kWarpsPerBlock; ++w) mx = fmax(mx, red[w]);
+  const T mx_in = mx;
   const int pe = pow2_exponent(mx) & ~1;          // even: sqrt(lambda 2^-pe) = sqrt(lambda) 2^(-pe/2) exactly
   const T down = (T)ldexp(1.0, -pe), up = (T)ldexp(1.0, pe);
   __syncthreads();
@@ -258,6 +279,24 @@ __global__ void __launch_bounds__(kBlock) psd_small_kernel(const PsdConeDesc* __
     __syncthreads();
   }
   if (!converged && threadIdx.x == 0 && fail_flag) atomicAdd(fail_flag, 1);
+
+  if (mode == 2) {
+    T* Q = eig.Q + eig.q_off[blockIdx.x];
+    T* lam = eig.lam + eig.lam_off[blockIdx.x];
+    const T band = (T)(64.0 * PsdEps<T>::v) * (T(1) + mx_in);
+    bool kink = false;
+    for (int e = threadIdx.x; e < N * N; e += blockDim.x) {
+      const int i = e % N, k = e / N;
+      Q[e] = V[i + k * ld];
+      if (i == 0) {
+        const T l = A[k + k * ld] * up;
+        lam[k] = l;
+        kink = kink || tabs(l) <= band;
+      }
+    }
+    if (__syncthreads_or(kink) && threadIdx.x == 0) atomicAdd(eig.kinks, 1);
+    return;
+  }
 
   if (mode == 1) {
     if (!converged) {
@@ -891,9 +930,10 @@ struct PsdBatch {
   }
 
   // eigen-decompose one large cone into A_d (diagonal = eigenvalues) and V_d (block Jacobi).  certificate: load a
-  // square cone from its upper triangle and return false instead of throwing ERR_NUMERICAL when max_sweeps is not enough.
+  // square cone from its upper triangle and return false instead of throwing ERR_NUMERICAL when max_sweeps is not enough;
+  // no_throw alone: the latter only (the eigenpairs of the projection's matrix, solve_adjoint.cuh).
   bool large_eig(const PsdConeDesc& d, const T* ws, cudaStream_t st, int max_sweeps, long long& launches,
-                 bool allow_warm = false, bool certificate = false) {
+                 bool allow_warm = false, bool certificate = false, bool no_throw = false) {
     const int N = d.N;
     int Nb = (N + kBjB - 1) / kBjB;
     if (Nb & 1) ++Nb;                                 // even number of blocks (zero padding decouples)
@@ -934,7 +974,7 @@ struct PsdBatch {
     if (getenv("COSMO_B200_PSD_DEBUG")) fprintf(stderr, "[psd] N=%d warm=%d sweeps=%d\n", N, (int)warm, sweep);
     CUDA_TRY(cudaGetLastError());
     if (!converged) {
-      if (certificate) return false;
+      if (certificate || no_throw) return false;
       throw EngineError{COSMO_B200_ERR_NUMERICAL, "block Jacobi eigensolver did not converge within psd_max_sweeps"};
     }
     if (allow_warm && Vw_d.p) {

@@ -358,6 +358,14 @@ __global__ void __launch_bounds__(kBlock) p2p_push_kernel(P2pView<T> v, const T*
   }
 }
 
+// Absolute tolerance of an inner KKT solve whose right-hand side (or initial residual) has norm nrm: tol_num > 0 is the
+// reference's tol_k / nrm; tol_num < 0 asks for the fixed relative tolerance -tol_num nrm (the inner solves of
+// cosmo_b200_solve_adjoint).
+template <typename T>
+__device__ __forceinline__ T inner_abstol(T tol_num, T nrm) {
+  return tol_num < T(0) ? -tol_num * nrm : tol_num / nrm;
+}
+
 template <typename T>
 struct CgInitFin {
   T* sc; int* isc; T tol_num;
@@ -365,7 +373,7 @@ struct CgInitFin {
   __device__ void operator()(T* out) const {   // out[0] = |r|^2, out[1] = |rhs|^2
     const T res = sqrt(out[0]);
     const T rhsn = sqrt(out[1]);
-    const T tol = tol_num / rhsn;              // abstol = get_tolerance(S)/norm(y1), reltol = 0
+    const T tol = inner_abstol(tol_num, rhsn);  // abstol = get_tolerance(S)/norm(y1), reltol = 0
     sc[SC_RES] = res;
     sc[SC_PREV] = T(1);
     sc[SC_TOL] = tol;
@@ -551,7 +559,7 @@ struct MinresInitFin {
   __device__ void operator()(T* out) const {   // out[0] = |b - L x|^2
     const T res = sqrt(out[0]);
     sc[SC_RES] = res;
-    sc[SC_TOL] = tol_num / res;                // abstol = get_tolerance(S) / init_residual, reltol = 0
+    sc[SC_TOL] = inner_abstol(tol_num, res);   // abstol = get_tolerance(S) / init_residual, reltol = 0
     sc[SC_H1] = sc[SC_H2] = sc[SC_H3] = sc[SC_H4] = T(0);
     sc[SC_RHS_1] = res; sc[SC_RHS_2] = T(0);
     sc[SC_C_PREV] = T(1); sc[SC_S_PREV] = T(0); sc[SC_C_CURR] = T(1); sc[SC_S_CURR] = T(0);

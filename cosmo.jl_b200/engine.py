@@ -125,6 +125,16 @@ POLISH_STATS = ("status", "n_lower", "n_upper", "n_equality", "r_prim", "r_dual"
 ADJOINT_STATS = ("status", "n_active", "n_weak", "refine_residual")
 
 
+class SolveAdjointSettings(C.Structure):
+    _fields_ = [("tol", C.c_double), ("max_iter", C.c_int32), ("restart", C.c_int32), ("kkt_tol", C.c_double),
+                ("reserved", C.c_int64)]
+
+
+# cosmo_b200_solve_adjoint's out[8]
+SOLVE_ADJOINT_STATS = ("status", "operator_applications", "residual", "inner_iterations", "rows_near_kink",
+                       "soc_near_kink", "psd_near_kink", "psd_unconverged")
+
+
 def _signatures():
     """(restype, argtypes) of every entry point of include/cosmo_b200.h, in the header's order."""
     vp, i32, i64, f64, P = C.c_void_p, C.c_int32, C.c_int64, C.c_double, C.POINTER
@@ -171,6 +181,7 @@ def _signatures():
         "cosmo_b200_rescale_iterates": (rc, [vp]),
         "cosmo_b200_polish": (rc, [vp, P(PolishSettings), vp, vp, vp, P(f64)]),
         "cosmo_b200_adjoint": (rc, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
+        "cosmo_b200_solve_adjoint": (rc, [vp, P(SolveAdjointSettings), vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_comm_unique_id": (rc, [vp]),
         "cosmo_b200_comm_init": (rc, [vp, i32, i32, vp]),
         "cosmo_b200_comm_p2p_export": (rc, [vp, vp]),
@@ -606,6 +617,23 @@ class Engine:
         ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
         stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_adjoint, self._h, int(refine_iter), _ptr(gx), _ptr(gy),
                        _ptr(gs), *ptrs, ctype=C.c_double, keys=ADJOINT_STATS, ints=ADJOINT_STATS[:3])
+        return tuple(outs), stats
+
+    def solve_adjoint(self, dx=None, dy=None, ds=None, tol=0.0, max_iter=500, restart=30, kkt_tol=1e-12, dq=None,
+                      db=None, dPx=None, dAx=None, dl=None, du=None):
+        """cosmo_b200_solve_adjoint: the gradients of a loss with respect to the data from its gradients dx, dy, ds with
+        respect to the last solve's solution (x, y, s), through the fixed point of the iteration (DESIGN.md §3k); every
+        cone but Exp/Pow, custom and complex PSD cones, every single-GPU KKT plugin.  Inputs and outputs as for
+        ``adjoint``.  Returns ((dq, db, dPx, dAx, dl, du), stats), stats keyed by SOLVE_ADJOINT_STATS (status 1 computed,
+        0 GMRES or a PSD eigensolve did not converge, -1 not applicable, the outputs then NaN; the counts as ints)."""
+        gx, gy, gs = (self._arr(a, k, np.float64) for a, k in ((dx, self.n), (dy, self.m), (ds, self.m)))
+        sizes = (self.n, self.m, self.nnzP, self.nnzA, self.m, self.m)
+        outs = [np.empty(k) if a is None else a for a, k in zip((dq, db, dPx, dAx, dl, du), sizes)]
+        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
+        st = SolveAdjointSettings(float(tol), int(max_iter), int(restart), float(kkt_tol), 0)
+        ints = tuple(k for k in SOLVE_ADJOINT_STATS if k != "residual")
+        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_solve_adjoint, self._h, C.byref(st), _ptr(gx), _ptr(gy),
+                       _ptr(gs), *ptrs, ctype=C.c_double, keys=SOLVE_ADJOINT_STATS, ints=ints)
         return tuple(outs), stats
 
     def update_matrices(self, Px=None, Ax=None, q=None, b=None):

@@ -883,6 +883,23 @@ class Model:
                 "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
                 "q": dq, "b": db, "l": dl, "u": du, "stats": st}
 
+    def solve_adjoint(self, dx=None, dy=None, ds=None, tol=0.0, max_iter=500, restart=30, kkt_tol=1e-12):
+        """Gradients of a scalar loss with respect to the data, from its gradients dx (n), dy, ds (m) with respect to the
+        solution (x, y, s) of the last optimize() (None: zero), through cosmo_b200_solve_adjoint (DESIGN.md §3k): the
+        derivative of the solution map through the fixed point of the iteration, for ZeroSet, Nonnegatives, Box, SOC and
+        real PSD constraints and every KKT solver.  Returns the dict of adjoint() ("P", "A", "q", "b", "l", "u") plus
+        "stats" (Engine.SOLVE_ADJOINT_STATS).  ValueError before the first optimize() and when the last one decomposed
+        the problem (decompose=True with at least one decomposed cone)."""
+        if self.engine is None:
+            raise ValueError("solve_adjoint needs a solve: call optimize() first")
+        if self._dec is not None:
+            raise ValueError("solve_adjoint does not map gradients through a chordal decomposition (decompose=True)")
+        (dq, db, dPx, dAx, dl, du), st = self.engine.solve_adjoint(dx, dy, ds, tol, max_iter, restart, kkt_tol)
+        P0, A0 = self.P0, self.A0
+        return {"P": sp.csc_matrix((dPx, P0.indices, P0.indptr), shape=P0.shape),
+                "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
+                "q": dq, "b": db, "l": dl, "u": du, "stats": st}
+
     def solution_into(self, x=None, y=None, s=None):
         """The last solution (x, y, s of Result, completed as settings.complete_dual asks) into caller fp64 arrays, CUDA
         (__cuda_array_interface__) or NumPy; None skips one.  After optimize(solution="device") it is reversed on the

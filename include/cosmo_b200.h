@@ -595,6 +595,52 @@ int cosmo_b200_polish(cosmo_b200_handle* h, const cosmo_b200_polish_settings* ps
 int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* dx, const double* dy, const double* ds,
                        double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double out[4]);
 
+/* ---- derivatives of a conic solution --------------------------------------- */
+/* An engine extension beyond the reference, like cosmo_b200_adjoint, for every cone the engine differentiates: ZeroSet,
+   Nonnegatives, Box, SecondOrderCone, PsdCone and PsdConeTriangle (real), with every single-GPU KKT plugin.  Given the
+   gradients dx (n), dy, ds (m) of a scalar loss with respect to the last solve's solution (x, y = -mu, s), it returns
+   the gradients of that loss with respect to the data of the unscaled set! form A x + s = b, by the adjoint of the
+   fixed point of the ADMM iteration.  In the engine's scaled coordinates, with w_s = s + mu ./ rho, Dpi the Jacobian
+   of the projection at w_s (symmetric) and K = [P + sigma I, A'; A, -diag(1 ./ rho)]:
+     gw = [dx~; Dpi(ds~ + rho .* dy~) - rho .* dy~],  (I - M') lam = gw  with
+     (I - M') lam = lam - [sigma a; b + Dpi(lam_s - 2 b)],  [a; b] = K \ [lam_x; -lam_s ./ rho]  (GMRES),
+     [u; v] = K \ [lam_x; -lam_s ./ rho],
+     dq = -u,  db = v,  dP_ij = -(u_i x_j + x_i u_j) / 2 (symmetrised as in cosmo_b200_adjoint),  dA_rj = -(v_r x_j + y_r u_j),
+     on Box rows with w_s <= l: dl_r = lam_s,r - 2 v_r + ds~_r + rho_r dy~_r, with w_s >= u the same value in du_r,
+     half to each on rows with l = u; 0 on every other row,
+   mapped back with D, E and c as cosmo_b200_adjoint maps them.  The result depends on the problem only, not on rho,
+   sigma or alpha, up to the accuracy of the solve.  At a kink of a projection (a row at its bound, |xbar| = |t| in a
+   SOC, a zero eigenvalue of a PSD cone) the derivative is one-sided.  DESIGN.md §3k. */
+typedef struct {
+  double tol;        /* relative GMRES residual |gw - (I - M') lam| / |gw|; 0: 1e-10 in fp64, 1e-5 in fp32 */
+  int32_t max_iter;  /* operator applications, >= 1 (500); the explicit residual of each restart counts */
+  int32_t restart;   /* Krylov dimension, 1 .. 200 (30) */
+  double kkt_tol;    /* fixed relative tolerance of the CG / MINRES inner solves, in (0, 1) (1e-12); each starts at 0 */
+  int64_t reserved;  /* 0 */
+} cosmo_b200_solve_adjoint_settings;
+/* NULL as = defaults.  dPx (nnz P) is in the CSC order of P given to create / update_matrices, dAx (nnz A) in that of A;
+   dq (n), db, dl, du (m) are vectors.  All are fp64, host or device, under the caller-memory rules of
+   cosmo_b200_solution; a NULL input is zero, a NULL output is skipped.  out = {status, operator applications, the
+   explicit final relative residual, inner KKT iterations (0 for the direct plugins), Nonnegatives and Box rows near a
+   kink, SOC cones near a kink, PSD cones near a kink, PSD cones whose eigensolver missed psd_max_sweeps}; near a kink
+   means within 64 u (1 + |w_s| of the cone), u the unit roundoff of the element type.  status 1: the gradients are
+   written.  0: GMRES did not reach tol within max_iter, or a PSD eigensolve did not converge: the outputs are NaN.
+   -1: not applicable (an Exp / Pow cone or a dual, a custom cone, a complex PsdConeTriangle, or the last solve ended
+   Primal_infeasible, Dual_infeasible or Unsolved): the outputs are NaN.  Bad settings, out NULL, or no solve since
+   create / reset / warm_start / rescale_iterates: COSMO_B200_ERR_INVALID.  A sharded handle, or a handle with a forward
+   map or decomposition map: COSMO_B200_ERR_UNSUPPORTED.  A Krylov basis that does not fit: COSMO_B200_ERR_ALLOC.
+   State: the iterates, the solution, rho, the rho vector, the rho updates, the accelerator history and the polish
+   record stay as the solve left them.  The plugin state the inner solves move -- the CG / MINRES warm start, the KKT
+   call counter and the inner-iteration state -- is put back, so the next solve is bit for bit the solve of a handle
+   that never ran this call; a direct plugin whose factor is marked dirty refactors here instead of in the next solve
+   (only the factorisation counters move, and the factor a polish left for cosmo_b200_adjoint is replaced).  Two calls
+   give bit-identical results.  Scratch allocated by the first call and kept: (restart + 3)(n + m) + 3 m values of the
+   element type, m flag bytes, N^2 + N values per PSD cone and 3 N^2 for the largest PSD cone with N > 96.  Host arrays
+   are staged through a buffer of their size. */
+int cosmo_b200_solve_adjoint(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dx,
+                             const double* dy, const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl,
+                             double* du, double out[8]);
+
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
 int cosmo_b200_comm_unique_id(void* id128);
