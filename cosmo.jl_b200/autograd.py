@@ -1,4 +1,4 @@
-"""torch.autograd for solves on the device: polished QPs and LPs (DESIGN.md §3j) and conic problems (§3k).
+"""torch.autograd for solves on the device: polished QPs and LPs (DESIGN.md §3j) and conic problems (§3k, §3l).
 
 ``solve_qp(engine, Px, q, Ax, b)`` puts new values of P, q, A and b into a live engine (``Engine.update_matrices``),
 solves, polishes and returns the polished unscaled solution ``(x, y, s)`` as CUDA tensors; its backward pass is one
@@ -15,6 +15,11 @@ The backward pass reads the point and the factor the engine keeps from the last 
 another ``solve_qp`` since this pass's forward (as ``torch.autograd.gradcheck`` does between them), the backward pass
 first solves and polishes this pass's data again; the solve is deterministic, so it differentiates the same point.
 Between a forward pass and its backward pass the engine must not be used other than through ``solve_qp``.
+
+``solve_conic(engine, Px, q, Ax, b)`` does the same for any solve the fixed-point derivatives cover, without a polish:
+its backward pass is one ``Engine.solve_adjoint`` and its forward-mode product (``torch.autograd.forward_ad``,
+``gradcheck(check_forward_ad=True)``) one ``Engine.solve_derivative``, both into CUDA tensors.  The ``torch.func``
+transforms (``jvp``, ``jacfwd``, ``vmap``) are not supported: they need the ``setup_context`` form of the Function.
 """
 import torch
 
@@ -98,7 +103,25 @@ class _SolveConic(torch.autograd.Function):
         ctx.engine, ctx.settings, ctx.device, ctx.call = engine, settings, q.device, engine._solve_conic_call
         ctx.dtypes = (Px.dtype, q.dtype, Ax.dtype, b.dtype)
         ctx.save_for_backward(Px, q, Ax, b)
+        ctx.save_for_forward(Px, q, Ax, b)
         return x, y, s
+
+    @staticmethod
+    def jvp(ctx, _engine, _settings, tPx, tq, tAx, tb):
+        eng = ctx.engine
+        dev = ctx.device
+        if eng._solve_conic_call != ctx.call:   # the engine has solved other data since: this pass's point again
+            _solve(eng, *ctx.saved_tensors)
+            ctx.call = eng._solve_conic_call
+        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
+        f64 = dict(dtype=torch.float64, device=dev)
+        dx, dy, ds = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64), torch.empty(eng.m, **f64)
+        d = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (tPx, tq, tAx, tb)]
+        _, st = eng.solve_derivative(d[0], d[1], d[2], d[3], dx=dx, dy=dy, ds=ds, **ctx.settings)
+        if st["status"] != 1:
+            raise EngineError(st["status"], "solve_conic: the solve derivative did not apply or converge (status %d)"
+                              % st["status"])
+        return dx, dy, ds
 
     @staticmethod
     def backward(ctx, gx, gy, gs):
@@ -125,7 +148,8 @@ def solve_conic(engine, Px, q, Ax, b, **adjoint_settings):
     through Engine.solve_adjoint (DESIGN.md §3k): any cone but Exp/Pow, custom and complex PSD cones, any single-GPU
     KKT solver.  The engine is created as for solve_qp (on the pattern of P and A, without host scaling); the forward
     pass raises unless the solve ends Solved.  adjoint_settings (tol, max_iter, restart, kkt_tol) go to
-    Engine.solve_adjoint.  The derivative is that of the solution map at the solve's point, exact as the solve's
-    tolerance goes to 0.  The engine rules of solve_qp apply: between a forward pass and its backward pass it is used
-    only through solve_conic, and a backward pass after other solves re-solves its own data first."""
+    Engine.solve_adjoint and Engine.solve_derivative.  The derivative is that of the solution map at the solve's point,
+    exact as the solve's tolerance goes to 0.  The engine rules of solve_qp apply: between a forward pass and its
+    backward pass (or its forward-mode product) it is used only through solve_conic, and a derivative after other
+    solves re-solves its own data first."""
     return _SolveConic.apply(engine, dict(adjoint_settings), Px, q, Ax, b)

@@ -203,6 +203,9 @@ class EngineBase {
   virtual void solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy,
                              const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
                              double* out8) = 0;
+  virtual void solve_derivative(const cosmo_b200_solve_adjoint_settings* as, const double* dPx, const double* dq,
+                                const double* dAx, const double* db, const double* dl, const double* du, double* dx,
+                                double* dy, double* ds, double* out8) = 0;
 };
 
 template <typename T>
@@ -267,6 +270,9 @@ class Engine : public EngineBase {
                double* dAx, double* dl, double* du, double* out4) override;
   void solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy, const double* ds,
                      double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double* out8) override;
+  void solve_derivative(const cosmo_b200_solve_adjoint_settings* as, const double* dPx, const double* dq, const double* dAx,
+                        const double* db, const double* dl, const double* du, double* dx, double* dy, double* ds,
+                        double* out8) override;
 
  private:
   // ---- problem ----
@@ -376,8 +382,33 @@ class Engine : public EngineBase {
   void sa_alloc(int restart);
   void sa_dots(const T* V, long long ldv, int k, const T* w, double* out);
   void sa_dpi(const T* h, T* out);
+  template <class Rhs>
+  void sa_kkt_with(Rhs&& rhs);
   void sa_kkt(const T* lam);
   void sa_operator(const T* lam, T* out);
+  // the steps both derivatives through the fixed point share: the checks of a call, the plugin state the inner solves
+  // move (saved and put back), the Jacobian data of the point and GMRES(restart) on an operator
+  struct SaSaved {
+    long long kkt_counter, total_inner, total_mults, persist;
+    bool tm_valid, had_mr_x;
+    int last_cg_iters, cur_maxit, psd_sweeps;
+    int isc[ISC_COUNT];
+  };
+  cosmo_b200_solve_adjoint_settings sa_settings(const cosmo_b200_solve_adjoint_settings* as, const char* who);
+  bool sa_not_applicable() const;
+  SaSaved sa_save();
+  void sa_restore(const SaSaved& sv);
+  int sa_point(double* out);
+  template <class Op>
+  bool sa_gmres(Op&& op, int R, int max_iter, double tol, long long& apps, double& rel);
+  template <class Rhs, class Op, class Emit>
+  void sa_run(const cosmo_b200_solve_adjoint_settings& p, unsigned dev, const double* const* ins, const long long* in_count,
+              int nin, const F64Out* outs, int nout, double* out, Rhs&& rhs, Op&& op, Emit&& emit);
+  // solve derivative (DESIGN.md §3l): dPi of the Box bound directions, the CSR(A) -> CSC map of A's values when the
+  // value maps are not resident (derived once and kept)
+  DevBuf<T> sd_dpi_;
+  DevBuf<int> sd_amap_;
+  void sd_operator(const T* v, T* out);
   void emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y, double* s);
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
   fwd::Forward fwd_;             // where the values of the decomposed problem come from (cosmo_b200_set_forward_map)
@@ -3632,16 +3663,26 @@ void Engine<T>::sa_dpi(const T* h, T* out) {
   }
 }
 
-// [xsol_; nu_] = K^-1 [lam_x; -lam_s / rho] through the plugin (kkt_core), each solve from zero
+// [xsol_; nu_] = K^-1 [ls_x; ls_s] through the plugin (kkt_core), each solve from zero; `rhs` launches the kernels that
+// write ls_ and t0_ = rho .* ls_s
+template <typename T>
+template <class Rhs>
+void Engine<T>::sa_kkt_with(Rhs&& rhs) {
+  CUDA_TRY(cudaMemsetAsync(xsol_.p, 0, std::max(n_, 1) * sizeof(T), stream_));
+  if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));
+  rhs();
+  tm_valid_ = false;
+  kkt_core(false, nullptr, nullptr);
+}
+
+// [xsol_; nu_] = K^-1 [lam_x; -lam_s / rho]
 template <typename T>
 void Engine<T>::sa_kkt(const T* lam) {
   const int n = n_, m = m_;
-  CUDA_TRY(cudaMemsetAsync(xsol_.p, 0, std::max(n, 1) * sizeof(T), stream_));
-  if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));
-  sa_op_rhs_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, lam, rho_vec_.p, ls_.p, t0_.p);
-  check_launch("sa_op_rhs");
-  tm_valid_ = false;
-  kkt_core(false, nullptr, nullptr);
+  sa_kkt_with([&] {
+    sa_op_rhs_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, lam, rho_vec_.p, ls_.p, t0_.p);
+    check_launch("sa_op_rhs");
+  });
 }
 
 // out = (I - M') lam = lam - [sigma a; b + Dpi(lam_s - 2 b)],  [a; b] = K^-1 [lam_x; -lam_s / rho]
@@ -3656,122 +3697,233 @@ void Engine<T>::sa_operator(const T* lam, T* out) {
   check_launch("sa_op_out");
 }
 
-// Derivatives of the last solve's solution through the fixed point of the iteration (DESIGN.md §3k): the Jacobian data
-// of the point, the right-hand side gw, GMRES(restart) on (I - M') lam = gw, one more plugin solve for [u; v] and the
-// gradients.  The iterates, the solution, rho, the statistics and the polish record stay as they are; the plugin state
-// the inner solves move (the CG warm start, the KKT counter, the inner iteration state) is put back.
+// The settings of a call through the fixed point (NULL: the defaults), checked, and the refusals both derivatives share
 template <typename T>
-void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy,
-                              const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
-                              double* out) {
+cosmo_b200_solve_adjoint_settings Engine<T>::sa_settings(const cosmo_b200_solve_adjoint_settings* as, const char* who) {
+  const std::string w(who);
   cosmo_b200_solve_adjoint_settings p{0.0, 500, 30, 1e-12, 0};
   if (as) p = *as;
   if (!(p.tol >= 0.0 && p.tol < 1.0) || p.max_iter < 1 || p.restart < 1 || p.restart > 200 ||
       !(p.kkt_tol > 0.0 && p.kkt_tol < 1.0) || p.reserved != 0)
-    throw EngineError{COSMO_B200_ERR_INVALID, "solve_adjoint: tol in [0, 1), max_iter >= 1, restart in 1 .. 200, kkt_tol in (0, 1), reserved 0"};
-  single_gpu("solve_adjoint");
+    throw EngineError{COSMO_B200_ERR_INVALID, w + ": tol in [0, 1), max_iter >= 1, restart in 1 .. 200, kkt_tol in (0, 1), reserved 0"};
+  single_gpu(who);
   if (fwd_.has_map() || rev_.has_map())
-    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "solve_adjoint: gradients through a forward or decomposition map are not supported"};
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, w + ": derivatives through a forward or decomposition map are not supported"};
   if (!have_solution_)
-    throw EngineError{COSMO_B200_ERR_INVALID, "solve_adjoint: no solve since the engine was created, reset or warm-started"};
+    throw EngineError{COSMO_B200_ERR_INVALID, w + ": no solve since the engine was created, reset or warm-started"};
   CUDA_TRY(cudaSetDevice(device_));
-  const double tol = p.tol > 0.0 ? p.tol : (sizeof(T) == sizeof(double) ? 1e-10 : 1e-5);
-  const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
-  const int n = n_, m = m_;
-  const long long L = (long long)n + m;
-  const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, P_.nnz}, {dAx, At_.nnz}, {dl, m}, {du, m}};
-  for (int k = 1; k < 8; ++k) out[k] = 0.0;
-  out[2] = NAN;
+  return p;
+}
+
+// status -1: a cone without a Jacobian here, or a last solve without a solution
+template <typename T>
+bool Engine<T>::sa_not_applicable() const {
   bool complex_psd = false;
   for (const PsdConeDesc& d : psd_.small_h) complex_psd = complex_psd || d.triangle == 2;
   for (const PsdConeDesc& d : psd_.large_h) complex_psd = complex_psd || d.triangle == 2;
-  if (n_c3_ || n_cust_ || complex_psd || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
-      last_status_ == COSMO_B200_DUAL_INFEASIBLE || last_status_ == COSMO_B200_UNSOLVED) {
-    out[0] = -1.0;
-    nan_f64(dev, 3, outs, 6);
-    return;
+  return n_c3_ || n_cust_ || complex_psd || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
+         last_status_ == COSMO_B200_DUAL_INFEASIBLE || last_status_ == COSMO_B200_UNSOLVED;
+}
+
+// the plugin state the inner solves move: the warm starts (xsol_ and the full MINRES one into sa_save_), the inner
+// iteration state and the counters
+template <typename T>
+typename Engine<T>::SaSaved Engine<T>::sa_save() {
+  SaSaved sv;
+  sv.kkt_counter = kkt_counter_; sv.total_inner = total_inner_; sv.total_mults = total_mults_;
+  sv.persist = persist_solves_;
+  sv.tm_valid = tm_valid_;
+  sv.last_cg_iters = last_cg_iters_; sv.cur_maxit = cur_maxit_; sv.psd_sweeps = psd_.last_sweeps;
+  sv.had_mr_x = mr_x_.p != nullptr;
+  CUDA_TRY(cudaMemcpyAsync(sv.isc, isc_.p, sizeof(sv.isc), cudaMemcpyDeviceToHost, stream_));
+  CUDA_TRY(cudaMemcpyAsync(sa_save_.p, xsol_.p, std::max(n_, 1) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  if (sv.had_mr_x) CUDA_TRY(cudaMemcpyAsync(sa_save_.p + std::max(n_, 1), mr_x_.p, mr_x_.n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  sync();
+  return sv;
+}
+
+template <typename T>
+void Engine<T>::sa_restore(const SaSaved& sv) {
+  CUDA_TRY(cudaMemcpyAsync(xsol_.p, sa_save_.p, std::max(n_, 1) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  if (sv.had_mr_x) CUDA_TRY(cudaMemcpyAsync(mr_x_.p, sa_save_.p + std::max(n_, 1), mr_x_.n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  else if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));   // as a first allocation leaves it
+  CUDA_TRY(cudaMemcpyAsync(isc_.p, sv.isc, sizeof(sv.isc), cudaMemcpyHostToDevice, stream_));
+  sync();
+  h_isc_[ISC_MAXIT] = sv.isc[ISC_MAXIT];
+  kkt_counter_ = sv.kkt_counter; total_inner_ = sv.total_inner; total_mults_ = sv.total_mults; persist_solves_ = sv.persist;
+  tm_valid_ = sv.tm_valid; last_cg_iters_ = sv.last_cg_iters; cur_maxit_ = sv.cur_maxit; psd_.last_sweeps = sv.psd_sweeps;
+  kkt_tol_fixed_ = 0.0;
+}
+
+// The point w_s = s + mu / rho and its Jacobian data: the row flags, the SOC norms, the eigenpairs of every PSD cone,
+// and the kink counts into out[4 .. 7].  Returns the PSD cones whose eigensolve did not converge.
+template <typename T>
+int Engine<T>::sa_point(double* out) {
+  const int m = m_;
+  CUDA_TRY(cudaMemsetAsync(sa_cnt_.p, 0, SA_CNT_COUNT * sizeof(int), stream_));
+  ws_from_mu_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, rho_vec_.p, mu_.p, s_.p, sa_ws_.p);
+  check_launch("ws_from_mu");
+  sa_row_flags_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_ws_.p, box_l_.p, box_u_.p, sa_flag_.p, sa_cnt_.p);
+  check_launch("sa_row_flags");
+  if (n_soc_) {
+    soc_norms(sa_ws_.p, sa_soc_r_.p);
+    sa_soc_kink_kernel<T><<<vgrid(n_soc_), kBlock, 0, stream_>>>(n_soc_, soc_off_.p, sa_ws_.p, sa_soc_r_.p, sa_cnt_.p);
+    check_launch("sa_soc_kink");
   }
+  const int sweeps = st_.psd_max_sweeps > 0 ? st_.psd_max_sweeps : 30;
+  int psd_unconverged = 0;
+  if (!psd_.small_h.empty()) {
+    PsdEigOut<T> eo;
+    eo.Q = sa_psd_q_.p; eo.lam = sa_psd_lam_.p; eo.q_off = sa_q_off_.p; eo.lam_off = sa_lam_off_.p;
+    eo.kinks = sa_cnt_.p + SA_CNT_PSD;
+    psd_small_kernel<T><<<(int)psd_.small_h.size(), kBlock, psd_.small_smem(), stream_>>>(
+        psd_.small_d.p, sa_ws_.p, nullptr, 2, nullptr, sweeps, sa_cnt_.p + SA_CNT_PSD_UNCONVERGED, eo);
+    check_launch("psd_small_eig");
+  }
+  for (size_t k = 0; k < psd_.large_h.size(); ++k) {
+    const PsdConeDesc& d = psd_.large_h[k];
+    if (!psd_.large_eig(d, sa_ws_.p, stream_, sweeps, launches_, /*allow_warm=*/false, /*certificate=*/false,
+                        /*no_throw=*/true)) {
+      ++psd_unconverged;
+      continue;
+    }
+    CUDA_TRY(cudaMemcpyAsync(sa_psd_q_.p + sa_large_q_off_[k], psd_.V_d.p, (size_t)d.N * d.N * sizeof(T),
+                             cudaMemcpyDeviceToDevice, stream_));
+    sa_psd_large_eig_kernel<T><<<1, kBlock, 0, stream_>>>(d.N, psd_.A_d.p, psd_.up_d.p, psd_.mx_d.p,
+                                                           sa_psd_lam_.p + sa_large_lam_off_[k], sa_cnt_.p);
+    check_launch("sa_psd_large_eig");
+  }
+  int cnt[SA_CNT_COUNT];
+  CUDA_TRY(cudaMemcpyAsync(cnt, sa_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  psd_unconverged += cnt[SA_CNT_PSD_UNCONVERGED];
+  out[4] = cnt[SA_CNT_ROWS]; out[5] = cnt[SA_CNT_SOC]; out[6] = cnt[SA_CNT_PSD]; out[7] = psd_unconverged;
+  return psd_unconverged;
+}
+
+// GMRES(R) on op(z) = r from z = 0: the basis V_0 .. V_R, then z, then r, in sa_V_ (r written by the caller).  CGS2
+// Arnoldi with fixed-order dot products on the device, the Hessenberg system and its Givens rotations on the host in
+// fp64, and the explicit residual r - op(z) at every restart.  `apps` counts the operator applications (the explicit
+// residuals included), `rel` is the last explicit relative residual.  Returns whether it reached tol.
+template <typename T>
+template <class Op>
+bool Engine<T>::sa_gmres(Op&& op, int R, int max_iter, double tol, long long& apps, double& rel) {
+  const long long L = (long long)n_ + m_;
+  T* V = sa_V_.p;
+  T* z = V + (long long)(R + 1) * L;
+  const T* rhs = z + L;
+  double* h1 = sa_hd_.p;            // the two CGS passes, |w|^2, then the update coefficients y
+  double* h2 = h1 + (R + 1);
+  double* nrm2 = h2 + (R + 1);
+  double* yd = nrm2 + 1;
+  bool converged = false;
+  CUDA_TRY(cudaMemsetAsync(z, 0, L * sizeof(T), stream_));
+  sa_dots(rhs, L, 1, rhs, nrm2);
+  double g2 = 0.0;
+  CUDA_TRY(cudaMemcpyAsync(&g2, nrm2, sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  const double gnorm = sqrt(g2);
+  if (!(gnorm > 0.0)) {
+    converged = gnorm == 0.0;   // r = 0: z = 0
+    rel = converged ? 0.0 : NAN;
+    return converged;
+  }
+  // r_0 = r (z = 0): V_0 = r / |r|
+  CUDA_TRY(cudaMemcpyAsync(V, rhs, L * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, V);
+  check_launch("sa_normalise");
+  double beta = gnorm;
+  std::vector<double> H((size_t)(R + 1) * R), cs(R), sn(R), g(R + 1), y(R), hh(2 * (R + 1) + 1);
+  for (;;) {
+    std::fill(g.begin(), g.end(), 0.0);
+    g[0] = beta;
+    int k = 0;
+    while (k < R && apps + 1 < max_iter) {   // one application stays for the explicit residual
+      T* w = V + (long long)(k + 1) * L;
+      op(V + (long long)k * L, w);
+      ++apps;
+      // CGS2: two classical Gram-Schmidt passes against V_0 .. V_k, then |w|
+      sa_dots(V, L, k + 1, w, h1);
+      sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k + 1, h1, -1.0, w);
+      check_launch("sa_axpy");
+      sa_dots(V, L, k + 1, w, h2);
+      sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k + 1, h2, -1.0, w);
+      check_launch("sa_axpy");
+      sa_dots(w, L, 1, w, nrm2);
+      sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, w);
+      check_launch("sa_normalise");
+      CUDA_TRY(cudaMemcpyAsync(hh.data(), h1, hh.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+      sync();
+      double* col = H.data() + (size_t)k * (R + 1);
+      for (int i = 0; i <= k; ++i) col[i] = hh[i] + hh[R + 1 + i];
+      col[k + 1] = sqrt(hh[2 * (R + 1)]);
+      const bool breakdown = !(col[k + 1] > 0.0);
+      for (int i = 0; i < k; ++i) {   // the previous Givens rotations
+        const double a = col[i], b = col[i + 1];
+        col[i] = cs[i] * a + sn[i] * b;
+        col[i + 1] = -sn[i] * a + cs[i] * b;
+      }
+      const double r = std::hypot(col[k], col[k + 1]);
+      cs[k] = r > 0.0 ? col[k] / r : 1.0;
+      sn[k] = r > 0.0 ? col[k + 1] / r : 0.0;
+      col[k] = r;
+      col[k + 1] = 0.0;
+      g[k + 1] = -sn[k] * g[k];
+      g[k] = cs[k] * g[k];
+      ++k;
+      if (breakdown || fabs(g[k]) <= tol * gnorm) break;
+    }
+    if (k > 0) {   // z += V y, H y = g by back substitution
+      for (int i = k - 1; i >= 0; --i) {
+        double v = g[i];
+        for (int j = i + 1; j < k; ++j) v -= H[(size_t)j * (R + 1) + i] * y[j];
+        y[i] = v / H[(size_t)i * (R + 1) + i];
+      }
+      CUDA_TRY(cudaMemcpyAsync(yd, y.data(), k * sizeof(double), cudaMemcpyHostToDevice, stream_));
+      sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k, yd, 1.0, z);
+      check_launch("sa_axpy");
+    }
+    // the explicit residual r - op(z) into V_0
+    op(z, V);
+    ++apps;
+    sa_residual_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, rhs, V);
+    check_launch("sa_residual");
+    sa_dots(V, L, 1, V, nrm2);
+    double r2 = 0.0;
+    CUDA_TRY(cudaMemcpyAsync(&r2, nrm2, sizeof(double), cudaMemcpyDeviceToHost, stream_));
+    sync();
+    beta = sqrt(r2);
+    rel = beta / gnorm;
+    if (rel <= tol) { converged = true; break; }
+    if (!(rel == rel) || apps + 1 >= max_iter) break;
+    sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, V);
+    check_launch("sa_normalise");
+  }
+  return converged;
+}
+
+// One call through the fixed point (DESIGN.md §3k, §3l): the plugin state saved, the caller arrays staged, the Jacobian
+// data of the point, then `rhs(din, r)` writes the right-hand side r, GMRES solves op(z) = r, and on convergence
+// `emit(din, dout, z)` writes the outputs.  out[0 .. 3] are the status, the operator applications, the residual and the
+// inner KKT iterations; the plugin state is put back and the outputs are NaN unless the status is 1.
+template <typename T>
+template <class Rhs, class Op, class Emit>
+void Engine<T>::sa_run(const cosmo_b200_solve_adjoint_settings& p, unsigned dev, const double* const* ins,
+                       const long long* in_count, int nin, const F64Out* outs, int nout, double* out, Rhs&& rhs, Op&& op,
+                       Emit&& emit) {
+  const double tol = p.tol > 0.0 ? p.tol : (sizeof(T) == sizeof(double) ? 1e-10 : 1e-5);
+  const long long L = (long long)n_ + m_;
   const int R = p.restart;
   sa_alloc(R);
-  // ---- the plugin state the inner solves move, saved and put back at the end
-  const long long kkt_counter0 = kkt_counter_, total_inner0 = total_inner_, total_mults0 = total_mults_;
-  const long long persist0 = persist_solves_;
-  const bool tm_valid0 = tm_valid_;
-  const int last_cg_iters0 = last_cg_iters_, cur_maxit0 = cur_maxit_, psd_sweeps0 = psd_.last_sweeps;
-  const bool had_mr_x = mr_x_.p != nullptr;
-  int isc0[ISC_COUNT];
-  CUDA_TRY(cudaMemcpyAsync(isc0, isc_.p, sizeof(isc0), cudaMemcpyDeviceToHost, stream_));
-  CUDA_TRY(cudaMemcpyAsync(sa_save_.p, xsol_.p, std::max(n, 1) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-  if (had_mr_x) CUDA_TRY(cudaMemcpyAsync(sa_save_.p + std::max(n, 1), mr_x_.p, mr_x_.n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-  sync();
-  auto restore = [&] {
-    CUDA_TRY(cudaMemcpyAsync(xsol_.p, sa_save_.p, std::max(n, 1) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-    if (had_mr_x) CUDA_TRY(cudaMemcpyAsync(mr_x_.p, sa_save_.p + std::max(n, 1), mr_x_.n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-    else if (mr_x_.p) CUDA_TRY(cudaMemsetAsync(mr_x_.p, 0, mr_x_.n * sizeof(T), stream_));   // as a first allocation leaves it
-    CUDA_TRY(cudaMemcpyAsync(isc_.p, isc0, sizeof(isc0), cudaMemcpyHostToDevice, stream_));
-    sync();
-    h_isc_[ISC_MAXIT] = isc0[ISC_MAXIT];
-    kkt_counter_ = kkt_counter0; total_inner_ = total_inner0; total_mults_ = total_mults0; persist_solves_ = persist0;
-    tm_valid_ = tm_valid0; last_cg_iters_ = last_cg_iters0; cur_maxit_ = cur_maxit0; psd_.last_sweeps = psd_sweeps0;
-    kkt_tol_fixed_ = 0.0;
-  };
+  const SaSaved sv = sa_save();
   try {
-    const double* ins[3] = {dx, dy, ds};
-    const long long in_count[3] = {n, m, m};
     DevBuf<double> stage;
-    const double* din[3];
-    double* dout[6];
-    stage_f64(dev, ins, in_count, 3, outs, 6, stage, din, dout);
-    const T* D = scaled_ ? D_.p : nullptr;
-    const T* Ev = scaled_ ? E_.p : nullptr;
-    const double c = scaled_ ? c_ : 1.0;
-    // ---- the point w_s = s + mu / rho and its Jacobian data
-    CUDA_TRY(cudaMemsetAsync(sa_cnt_.p, 0, SA_CNT_COUNT * sizeof(int), stream_));
-    ws_from_mu_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, rho_vec_.p, mu_.p, s_.p, sa_ws_.p);
-    check_launch("ws_from_mu");
-    sa_row_flags_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_ws_.p, box_l_.p, box_u_.p, sa_flag_.p, sa_cnt_.p);
-    check_launch("sa_row_flags");
-    if (n_soc_) {
-      soc_norms(sa_ws_.p, sa_soc_r_.p);
-      sa_soc_kink_kernel<T><<<vgrid(n_soc_), kBlock, 0, stream_>>>(n_soc_, soc_off_.p, sa_ws_.p, sa_soc_r_.p, sa_cnt_.p);
-      check_launch("sa_soc_kink");
-    }
-    const int sweeps = st_.psd_max_sweeps > 0 ? st_.psd_max_sweeps : 30;
-    int psd_unconverged = 0;
-    if (!psd_.small_h.empty()) {
-      PsdEigOut<T> eo;
-      eo.Q = sa_psd_q_.p; eo.lam = sa_psd_lam_.p; eo.q_off = sa_q_off_.p; eo.lam_off = sa_lam_off_.p;
-      eo.kinks = sa_cnt_.p + SA_CNT_PSD;
-      psd_small_kernel<T><<<(int)psd_.small_h.size(), kBlock, psd_.small_smem(), stream_>>>(
-          psd_.small_d.p, sa_ws_.p, nullptr, 2, nullptr, sweeps, sa_cnt_.p + SA_CNT_PSD_UNCONVERGED, eo);
-      check_launch("psd_small_eig");
-    }
-    for (size_t k = 0; k < psd_.large_h.size(); ++k) {
-      const PsdConeDesc& d = psd_.large_h[k];
-      if (!psd_.large_eig(d, sa_ws_.p, stream_, sweeps, launches_, /*allow_warm=*/false, /*certificate=*/false,
-                          /*no_throw=*/true)) {
-        ++psd_unconverged;
-        continue;
-      }
-      CUDA_TRY(cudaMemcpyAsync(sa_psd_q_.p + sa_large_q_off_[k], psd_.V_d.p, (size_t)d.N * d.N * sizeof(T),
-                               cudaMemcpyDeviceToDevice, stream_));
-      sa_psd_large_eig_kernel<T><<<1, kBlock, 0, stream_>>>(d.N, psd_.A_d.p, psd_.up_d.p, psd_.mx_d.p,
-                                                             sa_psd_lam_.p + sa_large_lam_off_[k], sa_cnt_.p);
-      check_launch("sa_psd_large_eig");
-    }
-    int cnt[SA_CNT_COUNT];
-    CUDA_TRY(cudaMemcpyAsync(cnt, sa_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
-    sync();
-    psd_unconverged += cnt[SA_CNT_PSD_UNCONVERGED];
-    out[4] = cnt[SA_CNT_ROWS]; out[5] = cnt[SA_CNT_SOC]; out[6] = cnt[SA_CNT_PSD]; out[7] = psd_unconverged;
-    // ---- GMRES(R) on (I - M') lam = gw; the basis V_0 .. V_R, then lam and gw, in sa_V_
-    T* V = sa_V_.p;
-    T* lam = V + (long long)(R + 1) * L;
-    T* gw = lam + L;
-    double* h1 = sa_hd_.p;            // the two CGS passes, |w|^2, then the update coefficients y
-    double* h2 = h1 + (R + 1);
-    double* nrm2 = h2 + (R + 1);
-    double* yd = nrm2 + 1;
+    const double* din[8];
+    double* dout[8];
+    stage_f64(dev, ins, in_count, nin, outs, nout, stage, din, dout);
+    const int psd_unconverged = sa_point(out);
+    T* z = sa_V_.p + (long long)(R + 1) * L;
+    T* r = z + L;
     kkt_tol_fixed_ = p.kkt_tol;
     int isc_start[ISC_COUNT];
     CUDA_TRY(cudaMemcpyAsync(isc_start, isc_.p, sizeof(isc_start), cudaMemcpyDeviceToHost, stream_));
@@ -3780,134 +3932,177 @@ void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const
     bool converged = false;
     double rel = NAN;
     if (psd_unconverged == 0) {
-      sa_gw_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, din[0], din[1], din[2], D, Ev, c, rho_vec_.p, gw, sa_h_.p);
-      check_launch("sa_gw");
-      sa_dpi(sa_h_.p, sa_dh_.p);
-      sa_gw_s_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, din[1], Ev, c, rho_vec_.p, sa_dh_.p, gw + n);
-      check_launch("sa_gw_s");
-      CUDA_TRY(cudaMemsetAsync(lam, 0, L * sizeof(T), stream_));
-      sa_dots(gw, L, 1, gw, nrm2);
-      double g2 = 0.0;
-      CUDA_TRY(cudaMemcpyAsync(&g2, nrm2, sizeof(double), cudaMemcpyDeviceToHost, stream_));
-      sync();
-      const double gnorm = sqrt(g2);
-      if (!(gnorm > 0.0)) {
-        converged = gnorm == 0.0;   // gw = 0: lam = 0
-        rel = converged ? 0.0 : NAN;
-      } else {
-        // r_0 = gw (lam = 0): V_0 = gw / |gw|
-        CUDA_TRY(cudaMemcpyAsync(V, gw, L * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-        sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, V);
-        check_launch("sa_normalise");
-        double beta = gnorm;
-        std::vector<double> H((size_t)(R + 1) * R), cs(R), sn(R), g(R + 1), y(R), hh(2 * (R + 1) + 1);
-        for (;;) {
-          std::fill(g.begin(), g.end(), 0.0);
-          g[0] = beta;
-          int k = 0;
-          while (k < R && apps + 1 < p.max_iter) {   // one application stays for the explicit residual
-            T* w = V + (long long)(k + 1) * L;
-            sa_operator(V + (long long)k * L, w);
-            ++apps;
-            // CGS2: two classical Gram-Schmidt passes against V_0 .. V_k, then |w|
-            sa_dots(V, L, k + 1, w, h1);
-            sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k + 1, h1, -1.0, w);
-            check_launch("sa_axpy");
-            sa_dots(V, L, k + 1, w, h2);
-            sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k + 1, h2, -1.0, w);
-            check_launch("sa_axpy");
-            sa_dots(w, L, 1, w, nrm2);
-            sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, w);
-            check_launch("sa_normalise");
-            CUDA_TRY(cudaMemcpyAsync(hh.data(), h1, hh.size() * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-            sync();
-            double* col = H.data() + (size_t)k * (R + 1);
-            for (int i = 0; i <= k; ++i) col[i] = hh[i] + hh[R + 1 + i];
-            col[k + 1] = sqrt(hh[2 * (R + 1)]);
-            const bool breakdown = !(col[k + 1] > 0.0);
-            for (int i = 0; i < k; ++i) {   // the previous Givens rotations
-              const double a = col[i], b = col[i + 1];
-              col[i] = cs[i] * a + sn[i] * b;
-              col[i + 1] = -sn[i] * a + cs[i] * b;
-            }
-            const double r = std::hypot(col[k], col[k + 1]);
-            cs[k] = r > 0.0 ? col[k] / r : 1.0;
-            sn[k] = r > 0.0 ? col[k + 1] / r : 0.0;
-            col[k] = r;
-            col[k + 1] = 0.0;
-            g[k + 1] = -sn[k] * g[k];
-            g[k] = cs[k] * g[k];
-            ++k;
-            if (breakdown || fabs(g[k]) <= tol * gnorm) break;
-          }
-          if (k > 0) {   // lam += V y, H y = g by back substitution
-            for (int i = k - 1; i >= 0; --i) {
-              double v = g[i];
-              for (int j = i + 1; j < k; ++j) v -= H[(size_t)j * (R + 1) + i] * y[j];
-              y[i] = v / H[(size_t)i * (R + 1) + i];
-            }
-            CUDA_TRY(cudaMemcpyAsync(yd, y.data(), k * sizeof(double), cudaMemcpyHostToDevice, stream_));
-            sa_axpy_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, V, L, k, yd, 1.0, lam);
-            check_launch("sa_axpy");
-          }
-          // the explicit residual r = gw - (I - M') lam into V_0
-          sa_operator(lam, V);
-          ++apps;
-          sa_residual_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, gw, V);
-          check_launch("sa_residual");
-          sa_dots(V, L, 1, V, nrm2);
-          double r2 = 0.0;
-          CUDA_TRY(cudaMemcpyAsync(&r2, nrm2, sizeof(double), cudaMemcpyDeviceToHost, stream_));
-          sync();
-          beta = sqrt(r2);
-          rel = beta / gnorm;
-          if (rel <= tol) { converged = true; break; }
-          if (!(rel == rel) || apps + 1 >= p.max_iter) break;
-          sa_normalise_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(L, nrm2, V);
-          check_launch("sa_normalise");
-        }
-      }
+      rhs(din, r);
+      converged = sa_gmres(op, R, p.max_iter, tol, apps, rel);
     }
     out[1] = (double)apps;
     out[2] = rel;
     if (!converged) {
       out[0] = 0.0;
     } else {
-      // ---- [u; v] = K^-1 [lam_x; -lam_s / rho] into xsol_ / nu_, then the gradients
-      sa_kkt(lam);
-      SolveAdjointVecArgs<T> a;
-      a.n = n; a.m = m; a.row_class = row_class_.p; a.flag = sa_flag_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
-      a.u = xsol_.p; a.v = nu_.p; a.lam_s = lam + n; a.rho = rho_vec_.p; a.gy = din[1]; a.gs = din[2];
-      a.D = D; a.E = Ev; a.c = c;
-      a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5];
-      solve_adjoint_grad_vec_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(a);
-      check_launch("solve_adjoint_grad_vec");
-      if (dout[2] && P_.nnz) {
-        if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only, not the slab maps
-        adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.d_src.p, xsol_.p,
-                                                                                 xs_.p, D, c, dout[2]);
-        check_launch("adjoint_grad_P");
-      }
-      if (dout[3] && At_.nnz) {
-        adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, xsol_.p, xs_.p,
-                                                                                 nu_.p, mu_.p, nullptr, D, Ev, dout[3]);
-        check_launch("adjoint_grad_A");
-      }
-      unstage_f64(outs, dout, 6);
+      emit(din, dout, z);
+      unstage_f64(outs, dout, nout);
       out[0] = 1.0;
     }
     int isc_end[ISC_COUNT];
     CUDA_TRY(cudaMemcpyAsync(isc_end, isc_.p, sizeof(isc_end), cudaMemcpyDeviceToHost, stream_));
     sync();
     out[3] = direct_kkt() ? 0.0 : (double)(total_inner_ - inner_start + (isc_end[ISC_TOTAL] - isc_start[ISC_TOTAL]));
-    restore();
-    if (!converged) nan_f64(dev, 3, outs, 6);
+    sa_restore(sv);
+    if (!converged) nan_f64(dev, nin, outs, nout);
     else if (dev) caller_written();
     sync();
   } catch (...) {
-    restore();
+    sa_restore(sv);
     throw;
   }
+}
+
+// Derivatives of the last solve's solution through the fixed point of the iteration (DESIGN.md §3k): the Jacobian data
+// of the point, the right-hand side gw, GMRES(restart) on (I - M') lam = gw, one more plugin solve for [u; v] and the
+// gradients.  The iterates, the solution, rho, the statistics and the polish record stay as they are; the plugin state
+// the inner solves move (the CG warm start, the KKT counter, the inner iteration state) is put back.
+template <typename T>
+void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy,
+                              const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
+                              double* out) {
+  const cosmo_b200_solve_adjoint_settings p = sa_settings(as, "solve_adjoint");
+  const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
+  const int n = n_, m = m_;
+  const long long L = (long long)n + m;
+  const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, P_.nnz}, {dAx, At_.nnz}, {dl, m}, {du, m}};
+  for (int k = 1; k < 8; ++k) out[k] = 0.0;
+  out[2] = NAN;
+  if (sa_not_applicable()) {
+    out[0] = -1.0;
+    nan_f64(dev, 3, outs, 6);
+    return;
+  }
+  const double* ins[3] = {dx, dy, ds};
+  const long long in_count[3] = {n, m, m};
+  const T* D = scaled_ ? D_.p : nullptr;
+  const T* Ev = scaled_ ? E_.p : nullptr;
+  const double c = scaled_ ? c_ : 1.0;
+  // gw = [dx~; Dpi(ds~ + rho dy~) - rho dy~]
+  auto rhs = [&](const double* const* din, T* gw) {
+    sa_gw_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, din[0], din[1], din[2], D, Ev, c, rho_vec_.p, gw, sa_h_.p);
+    check_launch("sa_gw");
+    sa_dpi(sa_h_.p, sa_dh_.p);
+    sa_gw_s_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, din[1], Ev, c, rho_vec_.p, sa_dh_.p, gw + n);
+    check_launch("sa_gw_s");
+  };
+  auto op = [&](const T* v, T* w) { sa_operator(v, w); };
+  // [u; v] = K^-1 [lam_x; -lam_s / rho] into xsol_ / nu_, then the gradients
+  auto emit = [&](const double* const* din, double* const* dout, const T* lam) {
+    sa_kkt(lam);
+    SolveAdjointVecArgs<T> a;
+    a.n = n; a.m = m; a.row_class = row_class_.p; a.flag = sa_flag_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
+    a.u = xsol_.p; a.v = nu_.p; a.lam_s = lam + n; a.rho = rho_vec_.p; a.gy = din[1]; a.gs = din[2];
+    a.D = D; a.E = Ev; a.c = c;
+    a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5];
+    solve_adjoint_grad_vec_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(a);
+    check_launch("solve_adjoint_grad_vec");
+    if (dout[2] && P_.nnz) {
+      if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only, not the slab maps
+      adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.d_src.p, xsol_.p,
+                                                                               xs_.p, D, c, dout[2]);
+      check_launch("adjoint_grad_P");
+    }
+    if (dout[3] && At_.nnz) {
+      adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, xsol_.p, xs_.p,
+                                                                               nu_.p, mu_.p, nullptr, D, Ev, dout[3]);
+      check_launch("adjoint_grad_A");
+    }
+  };
+  sa_run(p, dev, ins, in_count, 3, outs, 6, out, rhs, op, emit);
+}
+
+// (I - M) v = [v_x - a; v_s + b / rho - h],  h = Dpi v_s,  [a; b] = K^-1 [sigma v_x; v_s - 2 h]
+template <typename T>
+void Engine<T>::sd_operator(const T* v, T* out) {
+  const int n = n_, m = m_;
+  sa_dpi(v + n, sa_h_.p);
+  sa_kkt_with([&] {
+    sd_op_rhs_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, v, sa_h_.p, (T)st_.sigma, rho_vec_.p, ls_.p, t0_.p);
+    check_launch("sd_op_rhs");
+  });
+  sd_op_out_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, v, xsol_.p, nu_.p, sa_h_.p, rho_vec_.p, out);
+  check_launch("sd_op_out");
+}
+
+// The forward derivative of the last solve's solution along a data direction (DESIGN.md §3l): the Jacobian data of the
+// point as solve_adjoint forms them, t = [x'; dPi - nu' / rho] from one plugin solve over the direction passes,
+// GMRES(restart) on (I - M) w' = t, and the outputs from w' and one more Jacobian application.  State as solve_adjoint.
+template <typename T>
+void Engine<T>::solve_derivative(const cosmo_b200_solve_adjoint_settings* as, const double* dPx, const double* dq,
+                                 const double* dAx, const double* db, const double* dl, const double* du, double* dx,
+                                 double* dy, double* ds, double* out) {
+  const cosmo_b200_solve_adjoint_settings p = sa_settings(as, "solve_derivative");
+  const unsigned dev = caller_arrays({dPx, dq, dAx, db, dl, du, dx, dy, ds});
+  const int n = n_, m = m_;
+  const long long L = (long long)n + m;
+  const F64Out outs[3] = {{dx, n}, {dy, m}, {ds, m}};
+  for (int k = 1; k < 8; ++k) out[k] = 0.0;
+  out[2] = NAN;
+  if (sa_not_applicable()) {
+    out[0] = -1.0;
+    nan_f64(dev, 6, outs, 3);
+    return;
+  }
+  const double* ins[6] = {dPx, dq, dAx, db, dl, du};
+  const long long in_count[6] = {P_.nnz, n, At_.nnz, m, m, m};
+  const T* D = scaled_ ? D_.p : nullptr;
+  const T* Ev = scaled_ ? E_.p : nullptr;
+  const double c = scaled_ ? c_ : 1.0;
+  if (m && !sd_dpi_.p) sd_dpi_.alloc(m);
+  // t from [x'; nu'] = K^-1 [-dq~ - dP~ x~ - dA~' y~; db~ - 2 dPi - dA~ x~]
+  auto rhs = [&](const double* const* din, T* t) {
+    const int* amap = nullptr;
+    if (din[2] && At_.nnz) {
+      if (A_.d_src.p) {
+        amap = A_.d_src.p;   // the value maps of update_matrices are resident
+      } else {
+        if (!sd_amap_.p) {
+          sd_amap_.alloc((size_t)At_.nnz, false);
+          sd_amap_kernel<<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, A_.rowptr.p, A_.col.p,
+                                                                           sd_amap_.p);
+          check_launch("sd_amap");
+        }
+        amap = sd_amap_.p;
+      }
+    }
+    if (din[0] && P_.nnz && !maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only
+    sa_kkt_with([&] {
+      if (m) {
+        sd_box_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_flag_.p, box_l_.p, box_u_.p, din[4], din[5], Ev,
+                                                           sd_dpi_.p);
+        check_launch("sd_box");
+      }
+      if (n) {
+        sd_rhs_x_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(
+            n, P_.rowptr.p, P_.col.p, P_.d_src.p, At_.rowptr.p, At_.col.p, P_.nnz ? din[0] : nullptr, din[1],
+            At_.nnz ? din[2] : nullptr, xs_.p, mu_.p, D, Ev, c, ls_.p);
+        check_launch("sd_rhs_x");
+      }
+      if (m) {
+        sd_rhs_s_kernel<T><<<vgrid((long long)m * 32), kBlock, 0, stream_>>>(m, A_.rowptr.p, A_.col.p, amap, amap ? din[2] : nullptr,
+                                                                             din[3], sd_dpi_.p, xs_.p, D, Ev, rho_vec_.p,
+                                                                             ls_.p + n, t0_.p);
+        check_launch("sd_rhs_s");
+      }
+    });
+    sd_t_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, xsol_.p, nu_.p, sd_dpi_.p, rho_vec_.p, t);
+    check_launch("sd_t");
+  };
+  auto op = [&](const T* v, T* w) { sd_operator(v, w); };
+  // dx = D w'_x, ds = (Dpi w'_s + dPi) / E, dy = -E rho (w'_s - s~') / c
+  auto emit = [&](const double* const*, double* const* dout, const T* w) {
+    sa_dpi(w + n, sa_dh_.p);
+    sd_out_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, w, sa_dh_.p, sd_dpi_.p, rho_vec_.p, D, Ev, c, dout[0], dout[1],
+                                                       dout[2]);
+    check_launch("sd_out");
+  };
+  sa_run(p, dev, ins, in_count, 6, outs, 3, out, rhs, op, emit);
 }
 
 }  // namespace cosmo
@@ -4174,6 +4369,12 @@ int cosmo_b200_solve_adjoint(cosmo_b200_handle* h, const cosmo_b200_solve_adjoin
                              double* du, double out[8]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->solve_adjoint(as, dx, dy, ds, dq, db, dPx, dAx, dl, du, out));
+}
+int cosmo_b200_solve_derivative(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dPx,
+                                const double* dq, const double* dAx, const double* db, const double* dl, const double* du,
+                                double* dx, double* dy, double* ds, double out[8]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->solve_derivative(as, dPx, dq, dAx, db, dl, du, dx, dy, ds, out));
 }
 int cosmo_b200_reverse_decomposition(cosmo_b200_handle* h, int32_t complete_dual, void* x, void* s, void* mu, int64_t stats[4]) {
   ABI_GUARD(h, h->impl->reverse_decomposition(complete_dual, x, s, mu, stats));

@@ -1,5 +1,5 @@
 // solve_adjoint.cuh -- derivatives of a conic solution through the fixed point of the ADMM iteration
-// (cosmo_b200_solve_adjoint, DESIGN.md §3k).
+// (cosmo_b200_solve_adjoint, DESIGN.md §3k, and its forward counterpart cosmo_b200_solve_derivative, §3l).
 //
 // In the engine's scaled coordinates an alpha = 1 step of the iteration is
 //   T1(w) = [x~; Pi(w_s) - nu/rho],  [x~; nu] = K^-1 [sigma w_x - q; b - 2 Pi(w_s) + w_s],  K = [P + sigma I, A'; A, -1/rho]
@@ -453,6 +453,174 @@ __global__ void __launch_bounds__(kBlock) solve_adjoint_grad_vec_kernel(SolveAdj
     }
     if (a.dl) a.dl[r] = lo;
     if (a.du) a.du[r] = up;
+  }
+}
+
+// ---- the forward derivative (cosmo_b200_solve_derivative, DESIGN.md §3l) -----------------------------------------
+// The transpose of the operator above: for a data direction (dP, dq, dA, db, dl, du), scaled as the data are,
+//   t = [x'; dPi - nu' / rho],  [x'; nu'] = K^-1 [-dq - dP x - dA' y; db - 2 dPi - dA x],  (I - M) w' = t  (GMRES),
+//   (I - M) v = [v_x - a; v_s + b / rho - h],  h = Dpi v_s,  [a; b] = K^-1 [sigma v_x; v_s - 2 h],
+//   x' = w'_x,  s' = Dpi w'_s + dPi,  y' = -rho (w'_s - s'),
+// with dPi the Box term of the bound directions.  The direction passes below each write every output once, summing
+// a warp's lanes through the fixed xor tree.
+
+// map[p] = k for the CSR(A) position p of the CSC entry k, one warp per column j of A (row j of A', whose value order
+// is A's CSC order): the row r of the entry, then j found by binary search among the ascending columns of CSR(A) row r
+__global__ void __launch_bounds__(kBlock) sd_amap_kernel(int n, const int* __restrict__ at_rowptr, const int* __restrict__ at_col,
+                                                         const int* __restrict__ a_rowptr, const int* __restrict__ a_col,
+                                                         int* __restrict__ map) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += warps) {
+    for (int k = at_rowptr[j] + lane; k < at_rowptr[j + 1]; k += 32) {
+      const int r = at_col[k];
+      int lo = a_rowptr[r], hi = a_rowptr[r + 1] - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a_col[mid] < j) lo = mid + 1;
+        else hi = mid;
+      }
+      map[lo] = k;
+    }
+  }
+}
+
+// dPi of the Box rows from the scaled bound directions E dl, E du: dl~ where w_s <= l, du~ where w_s >= u, their mean
+// on clamped rows with l = u, 0 on every other row (the transpose of solve_adjoint_grad_vec_kernel's split)
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_box_kernel(int m, const unsigned char* __restrict__ row_class,
+                                                        const unsigned char* __restrict__ flag, const T* __restrict__ box_l,
+                                                        const T* __restrict__ box_u, const double* __restrict__ dl,
+                                                        const double* __restrict__ du, const T* __restrict__ E,
+                                                        T* __restrict__ dpi) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < m; r += gridDim.x * blockDim.x) {
+    double v = 0.0;
+    const unsigned char f = flag[r];
+    if (row_class[r] == ROW_BOX && (f == SA_ROW_LOWER || f == SA_ROW_UPPER)) {
+      const double e = E ? (double)E[r] : 1.0;
+      const double lo = dl ? e * dl[r] : 0.0, up = du ? e * du[r] : 0.0;
+      if (box_l[r] == box_u[r]) v = 0.5 * (lo + up);
+      else v = f == SA_ROW_LOWER ? lo : up;
+    }
+    dpi[r] = (T)v;
+  }
+}
+
+// ls_x = -c D_i dq_i - (dP~ x~)_i - (dA~' y~)_i, one warp per i over CSR(P) row i and CSR(A') row i (y = -mu):
+//   dP~_ij = c D_i D_j dPx[src[k]],  dA~'_ir = E_r D_i dAx[k]  (A''s value order is A's CSC order)
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_rhs_x_kernel(int n, const int* __restrict__ p_rowptr, const int* __restrict__ p_col,
+                                                          const int* __restrict__ p_src, const int* __restrict__ at_rowptr,
+                                                          const int* __restrict__ at_col, const double* __restrict__ dPx,
+                                                          const double* __restrict__ dq, const double* __restrict__ dAx,
+                                                          const T* __restrict__ x, const T* __restrict__ mu,
+                                                          const T* __restrict__ D, const T* __restrict__ E, double c,
+                                                          T* __restrict__ ls) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+    double px = 0.0, ay = 0.0;
+    if (dPx)
+      for (int k = p_rowptr[i] + lane; k < p_rowptr[i + 1]; k += 32) {
+        const int j = p_col[k];
+        px += (D ? (double)D[j] : 1.0) * dPx[p_src[k]] * (double)x[j];
+      }
+    if (dAx)
+      for (int k = at_rowptr[i] + lane; k < at_rowptr[i + 1]; k += 32) {
+        const int r = at_col[k];
+        ay -= (E ? (double)E[r] : 1.0) * dAx[k] * (double)mu[r];
+      }
+    px = warp_sum(px);
+    ay = warp_sum(ay);
+    if (lane == 0) {
+      const double di = D ? (double)D[i] : 1.0;
+      ls[i] = (T)(-di * ((dq ? c * dq[i] : 0.0) + c * px + ay));
+    }
+  }
+}
+
+// ls_s = E_r db_r - 2 dPi_r - (dA~ x~)_r, one warp per CSR(A) row r (map: CSR position -> CSC index), t0 = rho .* ls_s
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_rhs_s_kernel(int m, const int* __restrict__ a_rowptr, const int* __restrict__ a_col,
+                                                          const int* __restrict__ map, const double* __restrict__ dAx,
+                                                          const double* __restrict__ db, const T* __restrict__ dpi,
+                                                          const T* __restrict__ x, const T* __restrict__ D,
+                                                          const T* __restrict__ E, const T* __restrict__ rho,
+                                                          T* __restrict__ ls_s, T* __restrict__ t0) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < m; r += warps) {
+    const double e = E ? (double)E[r] : 1.0;
+    double acc = 0.0;
+    if (dAx)
+      for (int k = a_rowptr[r] + lane; k < a_rowptr[r + 1]; k += 32) {
+        const int j = a_col[k];
+        acc += e * (D ? (double)D[j] : 1.0) * dAx[map[k]] * (double)x[j];
+      }
+    acc = warp_sum(acc);
+    if (lane == 0) {
+      const T v = (T)((db ? e * db[r] : 0.0) - 2.0 * (double)dpi[r] - acc);
+      ls_s[r] = v;
+      t0[r] = rho[r] * v;
+    }
+  }
+}
+
+// t = [x'; dPi - nu' / rho] from [x'; nu'] = K^-1 [ls_x; ls_s]
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_t_kernel(int n, int m, const T* __restrict__ xsol, const T* __restrict__ nu,
+                                                      const T* __restrict__ dpi, const T* __restrict__ rho, T* __restrict__ t) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < (long long)n + m; k += (long long)gridDim.x * blockDim.x)
+    t[k] = k < n ? xsol[k] : dpi[k - n] - nu[k - n] / rho[k - n];
+}
+
+// ls = [sigma v_x; v_s - 2 h], t0 = rho .* ls_s (h = Dpi v_s)
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_op_rhs_kernel(int n, int m, const T* __restrict__ v, const T* __restrict__ h, T sigma,
+                                                           const T* __restrict__ rho, T* __restrict__ ls, T* __restrict__ t0) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < (long long)n + m; k += (long long)gridDim.x * blockDim.x) {
+    if (k < n) {
+      ls[k] = sigma * v[k];
+    } else {
+      const long long r = k - n;
+      const T w = v[k] - T(2) * h[r];
+      ls[k] = w;
+      t0[r] = rho[r] * w;
+    }
+  }
+}
+
+// out = (I - M) v = [v_x - a; v_s + b / rho - h]
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_op_out_kernel(int n, int m, const T* __restrict__ v, const T* __restrict__ a,
+                                                           const T* __restrict__ b, const T* __restrict__ h,
+                                                           const T* __restrict__ rho, T* __restrict__ out) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < (long long)n + m; k += (long long)gridDim.x * blockDim.x) {
+    if (k < n) {
+      out[k] = v[k] - a[k];
+    } else {
+      const long long r = k - n;
+      out[k] = v[k] + b[r] / rho[r] - h[r];
+    }
+  }
+}
+
+// the outputs, unscaled: dx = D w'_x,  ds = s~' / E,  dy = -E rho (w'_s - s~') / c  with s~' = Dpi w'_s + dPi
+template <typename T>
+__global__ void __launch_bounds__(kBlock) sd_out_kernel(int n, int m, const T* __restrict__ w, const T* __restrict__ dh,
+                                                        const T* __restrict__ dpi, const T* __restrict__ rho,
+                                                        const T* __restrict__ D, const T* __restrict__ E, double c,
+                                                        double* __restrict__ dx, double* __restrict__ dy, double* __restrict__ ds) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < (long long)n + m; k += (long long)gridDim.x * blockDim.x) {
+    if (k < n) {
+      if (dx) dx[k] = (D ? (double)D[k] : 1.0) * (double)w[k];
+      continue;
+    }
+    const long long r = k - n;
+    const double e = E ? (double)E[r] : 1.0;
+    const double st = (double)dh[r] + (double)dpi[r];
+    if (ds) ds[r] = st / e;
+    if (dy) dy[r] = -e * (double)rho[r] * ((double)w[k] - st) / c;
   }
 }
 

@@ -182,6 +182,7 @@ def _signatures():
         "cosmo_b200_polish": (rc, [vp, P(PolishSettings), vp, vp, vp, P(f64)]),
         "cosmo_b200_adjoint": (rc, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_solve_adjoint": (rc, [vp, P(SolveAdjointSettings), vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
+        "cosmo_b200_solve_derivative": (rc, [vp, P(SolveAdjointSettings), vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_comm_unique_id": (rc, [vp]),
         "cosmo_b200_comm_init": (rc, [vp, i32, i32, vp]),
         "cosmo_b200_comm_p2p_export": (rc, [vp, vp]),
@@ -634,6 +635,24 @@ class Engine:
         ints = tuple(k for k in SOLVE_ADJOINT_STATS if k != "residual")
         stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_solve_adjoint, self._h, C.byref(st), _ptr(gx), _ptr(gy),
                        _ptr(gs), *ptrs, ctype=C.c_double, keys=SOLVE_ADJOINT_STATS, ints=ints)
+        return tuple(outs), stats
+
+    def solve_derivative(self, dPx=None, dq=None, dAx=None, db=None, dl=None, du=None, tol=0.0, max_iter=500, restart=30,
+                         kkt_tol=1e-12, dx=None, dy=None, ds=None):
+        """cosmo_b200_solve_derivative: the directional derivatives (dx, dy, ds) of the last solve's solution along the
+        data direction dPx, dAx (the ``data`` order of P and A as given to create / update_matrices), dq (n), db, dl, du
+        (m), through the fixed point of the iteration (DESIGN.md §3l): the forward counterpart of ``solve_adjoint``, with
+        its settings.  Inputs are fp64 host or CUDA arrays (None: zero); dx (n), dy, ds (m) are fp64 outputs, host or
+        CUDA arrays, None allocates a NumPy array.  Returns ((dx, dy, ds), stats), stats keyed by SOLVE_ADJOINT_STATS
+        (status 1 computed, 0 GMRES or a PSD eigensolve did not converge, -1 not applicable, the outputs then NaN)."""
+        sizes = (self.nnzP, self.n, self.nnzA, self.m, self.m, self.m)
+        ins = [self._arr(a, k, np.float64) for a, k in zip((dPx, dq, dAx, db, dl, du), sizes)]
+        outs = [np.empty(k) if a is None else a for a, k in zip((dx, dy, ds), (self.n, self.m, self.m))]
+        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, (self.n, self.m, self.m))]
+        st = SolveAdjointSettings(float(tol), int(max_iter), int(restart), float(kkt_tol), 0)
+        ints = tuple(k for k in SOLVE_ADJOINT_STATS if k != "residual")
+        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_solve_derivative, self._h, C.byref(st),
+                       *(_ptr(a) for a in ins), *ptrs, ctype=C.c_double, keys=SOLVE_ADJOINT_STATS, ints=ints)
         return tuple(outs), stats
 
     def update_matrices(self, Px=None, Ax=None, q=None, b=None):

@@ -900,6 +900,24 @@ class Model:
                 "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
                 "q": dq, "b": db, "l": dl, "u": du, "stats": st}
 
+    def solve_derivative(self, dP=None, dq=None, dA=None, db=None, dl=None, du=None, tol=0.0, max_iter=500, restart=30,
+                         kkt_tol=1e-12):
+        """Directional derivatives of the solution (x, y, s) of the last optimize() along a data direction, through
+        cosmo_b200_solve_derivative (DESIGN.md §3l): the forward counterpart of solve_adjoint(), in its coordinates.
+        "dP" and "dA" are sparse matrices on the patterns of P0 and A0 (their values are read in the CSC order of those
+        patterns; P0 stores both triangles, so a symmetric direction moves (i, j) and (j, i) together), "dq" an n-vector,
+        "db", "dl", "du" m-vectors (dl, du are read on Box rows only); None is zero.  Returns a dict of "x", "y", "s" and
+        "stats" (Engine.SOLVE_ADJOINT_STATS).  ValueError before the first optimize() and when the last one decomposed the
+        problem, as solve_adjoint()."""
+        if self.engine is None:
+            raise ValueError("solve_derivative needs a solve: call optimize() first")
+        if self._dec is not None:
+            raise ValueError("solve_derivative does not map directions through a chordal decomposition (decompose=True)")
+        dPx = None if dP is None else _pattern_values(dP, self.P0, "dP")
+        dAx = None if dA is None else _pattern_values(dA, self.A0, "dA")
+        (dx, dy, ds), st = self.engine.solve_derivative(dPx, dq, dAx, db, dl, du, tol, max_iter, restart, kkt_tol)
+        return {"x": dx, "y": dy, "s": ds, "stats": st}
+
     def solution_into(self, x=None, y=None, s=None):
         """The last solution (x, y, s of Result, completed as settings.complete_dual asks) into caller fp64 arrays, CUDA
         (__cuda_array_interface__) or NumPy; None skips one.  After optimize(solution="device") it is reversed on the
@@ -915,6 +933,19 @@ class Model:
         if self.engine is not None:
             self.engine.close()
         self.__init__(self.dtype, self.device)
+
+
+def _pattern_values(D, M, name):
+    """The values of the sparse matrix D at the stored entries of the CSC matrix M, in M's data order (entries of D off
+    M's pattern: ValueError)."""
+    D = sp.csc_matrix(D, dtype=np.float64)
+    if D.shape != M.shape:
+        raise ValueError("%s must be %d x %d" % (name, *M.shape))
+    rows, cols = M.indices, np.repeat(np.arange(M.shape[1]), np.diff(M.indptr))
+    vals = np.asarray(D[rows, cols]).ravel()
+    if not np.isclose(np.abs(vals).sum(), np.abs(D.data).sum(), rtol=1e-12, atol=0.0):
+        raise ValueError("%s has entries off the pattern of the model's matrix" % name)
+    return vals
 
 
 def configure_accelerator(engine, st: Settings):

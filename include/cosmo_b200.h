@@ -640,6 +640,28 @@ typedef struct {
 int cosmo_b200_solve_adjoint(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dx,
                              const double* dy, const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl,
                              double* du, double out[8]);
+/* The forward counterpart of cosmo_b200_solve_adjoint: the Jacobian-vector product of the same solution map.  Given a
+   direction (dPx, dq, dAx, db, dl, du) of the data of the unscaled set! form, it returns the directional derivatives
+   dx (n), dy, ds (m) of the last solve's solution (x, y = -mu, s).  With the direction scaled as the data are
+   (c D dP D, c D dq, E dA D, E db, E dl, E du), w_s, Dpi and K as above:
+     dPi = dl_r on Box rows with w_s <= l, du_r with w_s >= u, (dl_r + du_r) / 2 on those with l = u, 0 elsewhere,
+     [x'; nu'] = K \ [-dq - dP x - dA' y; db - 2 dPi - dA x],  t = [x'; dPi - nu' ./ rho],
+     (I - M) w' = t  with  (I - M) v = [v_x - a; v_s + b ./ rho - h],  h = Dpi v_s,  [a; b] = K \ [sigma v_x; v_s - 2 h]
+     (GMRES),
+     dx = w'_x,  ds = Dpi w'_s + dPi,  dy = -rho .* (w'_s - ds),
+   mapped back as cosmo_b200_solution maps the solution (x = D x~, s = s~ ./ E, y = E y~ / c).  One plugin solve for t,
+   then one plugin solve and one Jacobian application per operator application, as in cosmo_b200_solve_adjoint, whose
+   transpose this is: <g, J d> = <J' g, d> to the accuracy of the two GMRES solves.  dP is read through the stored
+   pattern of P (both triangles when both are stored); a symmetric direction is the one the adjoint's symmetrised dPx
+   describes.  The settings, the status codes, out (the GMRES residual is |t - (I - M) w'| / |t|), the errors and the
+   untouched state are those of cosmo_b200_solve_adjoint; two calls give bit-identical results.  The inputs dPx (nnz P,
+   the CSC order of P given to create / update_matrices), dq (n), dAx (nnz A, A's CSC order), db, dl, du (m) and the
+   outputs are fp64, host or device, under the caller-memory rules of cosmo_b200_solution; a NULL input is zero, a NULL
+   output is skipped.  Scratch kept besides solve_adjoint's: m values of the element type, and one int per nonzero of A
+   for the CSR -> CSC map of A's values when update_matrices has not made it resident.  DESIGN.md §3l. */
+int cosmo_b200_solve_derivative(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dPx,
+                                const double* dq, const double* dAx, const double* db, const double* dl, const double* du,
+                                double* dx, double* dy, double* ds, double out[8]);
 
 /* ---- multi-GPU (one process per GPU; rows sharded, n-vectors replicated) -- */
 /* 128-byte ncclUniqueId created on rank 0 and broadcast by the host plumbing */
