@@ -145,8 +145,8 @@ class _SolveConic(torch.autograd.Function):
 
 def solve_conic(engine, Px, q, Ax, b, **adjoint_settings):
     """The solution (x, y, s) of the engine's problem with the data (Px, q, Ax, b), differentiable with respect to all four
-    through Engine.solve_adjoint (DESIGN.md §3k): any cone but Exp/Pow, custom and complex PSD cones, any single-GPU
-    KKT solver.  The engine is created as for solve_qp (on the pattern of P and A, without host scaling); the forward
+    through Engine.solve_adjoint (DESIGN.md §3k): any cone but Exp/Pow, complex PSD and custom cones whose type has no
+    Jacobian hook, any single-GPU KKT solver.  The engine is created as for solve_qp (on the pattern of P and A, without host scaling); the forward
     pass raises unless the solve ends Solved.  adjoint_settings (tol, max_iter, restart, kkt_tol) go to
     Engine.solve_adjoint and Engine.solve_derivative.  The derivative is that of the solution map at the solve's point,
     exact as the solve's tolerance goes to 0.  The engine rules of solve_qp apply: between a forward pass and its

@@ -2,12 +2,16 @@
 //
 // The reference lets a user add a cone by subtyping AbstractConvexCone and defining project! (and optionally in_dual /
 // in_pol_recc for the infeasibility certificates, convexset.jl:919-958).  Here the same three functions are CUDA device
-// templates: each type is compiled with NVRTC for sm_90a together with a small prelude and two generated wrapper
-// kernels, loaded with cudaLibraryLoadData and launched on the engine stream like any other cone kernel.
+// templates, with an optional fourth for the Jacobian of the projection: each type is compiled with NVRTC for sm_90a
+// together with a small prelude and two or three generated wrapper kernels, loaded with cudaLibraryLoadData and launched
+// on the engine stream like any other cone kernel.
 //   cosmo_custom_project: copies a cone's w_s rows into s, synchronises the cone's lanes and calls NAME::project;
 //   cosmo_custom_cert:    copies -v (primal certificate) or v (dual) into a scratch vector, calls the hook and writes
 //                         flag[cone] = 0 when every lane certified, 1 otherwise; custom_flag_fold_kernel folds the flags
-//                         of all types into one scalar in a fixed order.
+//                         of all types into one scalar in a fixed order;
+//   cosmo_custom_jacobian: (types with COSMO_B200_CUSTOM_HAS_JACOBIAN) copies a cone's rows of a direction h into out,
+//                         synchronises the lanes and calls NAME::jacobian(w_s, Pi(w_s), out): out = DPi(w_s) h, for
+//                         the derivatives through the fixed point (solve_adjoint.cuh).
 // The compiled cubins live in one process-wide cache keyed by the descriptor's contents and the dtype, so every engine
 // (and every rank of a sharded model) of a process compiles a type once.  NVRTC is loaded with dlopen on first use, so
 // that an engine without custom cones neither needs nor loads it.
@@ -86,7 +90,7 @@ inline Key make_key(const cosmo_b200_custom_cone* d, int dtype) {
   if (name == "cosmo_cone") throw EngineError{COSMO_B200_ERR_INVALID, "custom cone: the name cosmo_cone is the prelude's"};
   if (d->granularity < COSMO_B200_CUSTOM_THREAD || d->granularity > COSMO_B200_CUSTOM_BLOCK)
     throw EngineError{COSMO_B200_ERR_INVALID, "custom cone " + name + ": unknown granularity"};
-  if (d->flags & ~(COSMO_B200_CUSTOM_HAS_IN_DUAL | COSMO_B200_CUSTOM_HAS_IN_POL_RECC))
+  if (d->flags & ~(COSMO_B200_CUSTOM_HAS_IN_DUAL | COSMO_B200_CUSTOM_HAS_IN_POL_RECC | COSMO_B200_CUSTOM_HAS_JACOBIAN))
     throw EngineError{COSMO_B200_ERR_INVALID, "custom cone " + name + ": unknown flag"};
   if (d->reserved != 0) throw EngineError{COSMO_B200_ERR_INVALID, "custom cone " + name + ": reserved must be 0"};
   if (d->n_params < 0) throw EngineError{COSMO_B200_ERR_INVALID, "custom cone " + name + ": n_params < 0"};
@@ -182,6 +186,20 @@ extern "C" __global__ void cosmo_custom_cert(int ncones, const int* off, const i
   ok = cosmo_cone::all(ok, width);
   if (lane == 0) flag[cone] = ok ? 0 : 1;
 }
+
+#if COSMO_CONE_FLAGS & 8
+// out = DPi(ws) h on the rows of every cone, ps = Pi(ws) at the same point
+extern "C" __global__ void cosmo_custom_jacobian(int ncones, const int* off, const int* dim, const COSMO_CONE_T* params,
+                                                 const COSMO_CONE_T* ws, const COSMO_CONE_T* ps, const COSMO_CONE_T* h,
+                                                 COSMO_CONE_T* out) {
+  COSMO_CONE_LOCATE
+  COSMO_CONE_T* x = out + off[cone];
+  const COSMO_CONE_T* src = h + off[cone];
+  for (long long i = lane; i < d; i += width) x[i] = src[i];
+  cosmo_cone::sync(width);
+  COSMO_CONE_NAME::jacobian<COSMO_CONE_T>(ws + off[cone], ps + off[cone], x, d, p, lane, width);
+}
+#endif
 )WRAP";
 
 inline std::string generated_source(const Key& k) {
@@ -204,6 +222,7 @@ struct Entry {
   std::vector<char> cubin;
   cudaLibrary_t lib = nullptr;          // loaded on the first engine that uses the type (needs a device)
   cudaKernel_t project = nullptr, cert = nullptr;
+  cudaKernel_t jac = nullptr;           // types with COSMO_B200_CUSTOM_HAS_JACOBIAN only
 };
 
 // One per process.  Entries are never removed or unloaded: a type compiled once stays usable by later engines.
@@ -230,6 +249,7 @@ class Cache {
     CUDA_TRY(cudaLibraryLoadData(&lib, e->cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0));
     CUDA_TRY(cudaLibraryGetKernel(&e->project, lib, "cosmo_custom_project"));
     CUDA_TRY(cudaLibraryGetKernel(&e->cert, lib, "cosmo_custom_cert"));
+    if (e->key.flags & COSMO_B200_CUSTOM_HAS_JACOBIAN) CUDA_TRY(cudaLibraryGetKernel(&e->jac, lib, "cosmo_custom_jacobian"));
     e->lib = lib;
   }
 

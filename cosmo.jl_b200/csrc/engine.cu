@@ -310,7 +310,7 @@ class Engine : public EngineBase {
   DevBuf<int> cust_off_, cust_dim_, cust_flag_;
   DevBuf<T> cust_params_, cust_tmp_;
   long long cust_compiled_ = 0, cust_hits_ = 0;   // types this create compiled / found in the process-wide cache
-  void custom_project(const T* ws);
+  void custom_project(const T* ws, T* out);
   void custom_certificates(const T* v, T eps, int which);
   // ---- accelerator (aa.cuh) ----
   DevBuf<T> aaG_, aaQ_, aaR_, aa_eta_, aa_glast_, aa_f_, aa_flast_, aa_sc_;
@@ -370,9 +370,10 @@ class Engine : public EngineBase {
   void nan_f64(unsigned dev, int nin, const F64Out* outs, int nout);
   // solve adjoint (solve_adjoint.cuh): scratch allocated by the first call and kept -- the Krylov basis with lam and gw,
   // the point w_s, two m-vectors for Dpi, the row flags, the SOC norms and x'h, the eigenpairs of the PSD cones (small
-  // cones first, then large ones) and three N x N work matrices for the largest large cone, the saved plugin state
+  // cones first, then large ones) and three N x N work matrices for the largest large cone, the saved plugin state, and
+  // Pi(w_s) on the rows of the custom cones for their Jacobian hooks
   int sa_restart_ = 0;
-  DevBuf<T> sa_V_, sa_ws_, sa_h_, sa_dh_, sa_soc_r_, sa_psd_q_, sa_psd_lam_, sa_psd_work_, sa_save_;
+  DevBuf<T> sa_V_, sa_ws_, sa_h_, sa_dh_, sa_soc_r_, sa_psd_q_, sa_psd_lam_, sa_psd_work_, sa_save_, sa_cust_s_;
   DevBuf<unsigned char> sa_flag_;
   DevBuf<double> sa_part_, sa_hd_, sa_soc_dot_;
   DevBuf<long long> sa_q_off_;
@@ -1752,13 +1753,13 @@ void Engine<T>::project_device(const T* w, bool with_rhs, const T* ws_rhs) {
     cone3_project_kernel<T><<<(n_c3_ + 127) / 128, 128, 0, stream_>>>(c3_table(), w + n_, s_.p);
     check_launch("cone3_project");
   }
-  if (n_cust_) custom_project(w + n_);
+  if (n_cust_) custom_project(w + n_, s_.p);
   launch_proj_rhs(w, ws_rhs ? ws_rhs : w + n_, true, with_rhs);
 }
 
-// s = Pi_K(w_s) on the rows of every custom cone: one launch of the type's compiled projection kernel per type
+// out = Pi_K(w_s) on the rows of every custom cone: one launch of the type's compiled projection kernel per type
 template <typename T>
-void Engine<T>::custom_project(const T* ws) {
+void Engine<T>::custom_project(const T* ws, T* out) {
   for (const custom::TypeSlice& t : cust_types_) {
     dim3 grid, block;
     custom::launch_dims(t.entry->key.granularity, t.n, grid, block);
@@ -1766,8 +1767,7 @@ void Engine<T>::custom_project(const T* ws) {
     const int* off = cust_off_.p + t.first;
     const int* dim = cust_dim_.p + t.first;
     const T* par = t.entry->key.n_params ? cust_params_.p + t.param_first : nullptr;
-    T* s = s_.p;
-    void* args[] = {&n, &off, &dim, &par, &ws, &s};
+    void* args[] = {&n, &off, &dim, &par, &ws, &out};
     CUDA_TRY(cudaLaunchKernel((const void*)t.entry->project, grid, block, args, 0, stream_));
     check_launch("custom_project");
   }
@@ -3576,6 +3576,7 @@ void Engine<T>::sa_alloc(int restart) {
   sa_ws_.alloc(m1, false); sa_h_.alloc(m1); sa_dh_.alloc(m1); sa_flag_.alloc(m1);
   sa_cnt_.alloc(SA_CNT_COUNT);
   if (n_soc_) { sa_soc_r_.alloc(n_soc_); sa_soc_dot_.alloc((size_t)n_soc_ + std::max(n_soc_chunks_, 1)); }
+  if (n_cust_) sa_cust_s_.alloc(m1, false);
   if (!psd_.empty()) {
     std::vector<long long> q_off;
     std::vector<int> lam_off;
@@ -3613,7 +3614,8 @@ void Engine<T>::sa_dots(const T* V, long long ldv, int k, const T* w, double* ou
 }
 
 // out = Dpi h at the point sa_ws_ (m-vectors): the rows and SOC cones elementwise after the per-cone x'h, the small PSD
-// cones one CTA each, each large cone by four bj_gemm_kernel products around a Hadamard kernel
+// cones one CTA each, each large cone by four bj_gemm_kernel products around a Hadamard kernel, the custom cones by one
+// launch of their type's Jacobian hook per type (at sa_ws_ and its projection sa_cust_s_)
 template <typename T>
 void Engine<T>::sa_dpi(const T* h, T* out) {
   if (n_soc_) {
@@ -3660,6 +3662,19 @@ void Engine<T>::sa_dpi(const T* h, T* out) {
     check_launch("bj_gemm");
     sa_psd_store_kernel<T><<<g, kBlock, 0, stream_>>>(d, H, out);
     check_launch("sa_psd_store");
+  }
+  for (const custom::TypeSlice& t : cust_types_) {
+    dim3 grid, block;
+    custom::launch_dims(t.entry->key.granularity, t.n, grid, block);
+    int n = t.n;
+    const int* off = cust_off_.p + t.first;
+    const int* dim = cust_dim_.p + t.first;
+    const T* par = t.entry->key.n_params ? cust_params_.p + t.param_first : nullptr;
+    const T* ws = sa_ws_.p;
+    const T* ps = sa_cust_s_.p;
+    void* args[] = {&n, &off, &dim, &par, &ws, &ps, &h, &out};
+    CUDA_TRY(cudaLaunchKernel((const void*)t.entry->jac, grid, block, args, 0, stream_));
+    check_launch("custom_jacobian");
   }
 }
 
@@ -3715,13 +3730,15 @@ cosmo_b200_solve_adjoint_settings Engine<T>::sa_settings(const cosmo_b200_solve_
   return p;
 }
 
-// status -1: a cone without a Jacobian here, or a last solve without a solution
+// status -1: a cone without a Jacobian here (a custom type without the hook among them), or a last solve without a
+// solution
 template <typename T>
 bool Engine<T>::sa_not_applicable() const {
-  bool complex_psd = false;
+  bool complex_psd = false, hookless = false;
   for (const PsdConeDesc& d : psd_.small_h) complex_psd = complex_psd || d.triangle == 2;
   for (const PsdConeDesc& d : psd_.large_h) complex_psd = complex_psd || d.triangle == 2;
-  return n_c3_ || n_cust_ || complex_psd || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
+  for (const custom::TypeSlice& t : cust_types_) hookless = hookless || !t.entry->jac;
+  return n_c3_ || hookless || complex_psd || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
          last_status_ == COSMO_B200_DUAL_INFEASIBLE || last_status_ == COSMO_B200_UNSOLVED;
 }
 
@@ -3756,7 +3773,8 @@ void Engine<T>::sa_restore(const SaSaved& sv) {
 }
 
 // The point w_s = s + mu / rho and its Jacobian data: the row flags, the SOC norms, the eigenpairs of every PSD cone,
-// and the kink counts into out[4 .. 7].  Returns the PSD cones whose eigensolve did not converge.
+// the projection of the custom cones' rows, and the kink counts into out[4 .. 7] (custom cones are not counted).
+// Returns the PSD cones whose eigensolve did not converge.
 template <typename T>
 int Engine<T>::sa_point(double* out) {
   const int m = m_;
@@ -3765,6 +3783,7 @@ int Engine<T>::sa_point(double* out) {
   check_launch("ws_from_mu");
   sa_row_flags_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_ws_.p, box_l_.p, box_u_.p, sa_flag_.p, sa_cnt_.p);
   check_launch("sa_row_flags");
+  if (n_cust_) custom_project(sa_ws_.p, sa_cust_s_.p);
   if (n_soc_) {
     soc_norms(sa_ws_.p, sa_soc_r_.p);
     sa_soc_kink_kernel<T><<<vgrid(n_soc_), kBlock, 0, stream_>>>(n_soc_, soc_off_.p, sa_ws_.p, sa_soc_r_.p, sa_cnt_.p);

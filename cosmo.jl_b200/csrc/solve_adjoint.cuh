@@ -111,7 +111,8 @@ __global__ void sa_soc_dot_final_kernel(const double* __restrict__ chunk_dot, co
   dot[k] = v;
 }
 
-// out = Dpi h on every row outside the PSD cones (those are written by the PSD kernels):
+// out = Dpi h on every row outside the PSD and custom cones (those are written by the PSD kernels and the custom cones'
+// Jacobian hooks):
 //   ZeroSet 0;  Nonnegatives, Box: h strictly inside, 0 outside;
 //   SOC (t, xbar), r = |xbar|: h if r <= t, 0 if r <= -t, else
 //     1/2 [h_t + xbar'hbar / r ;  xbar h_t / r + (1 + t/r) hbar - (t/r) xbar (xbar'hbar) / r^2]
@@ -123,7 +124,7 @@ __global__ void __launch_bounds__(kBlock) sa_dpi_rows_kernel(int m, const unsign
                                                              const T* __restrict__ h, T* __restrict__ out) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
     const unsigned char cls = row_class[i];
-    if (cls == ROW_PSD) continue;
+    if (cls == ROW_PSD || cls == ROW_CUSTOM) continue;
     T v = T(0);
     if (cls == ROW_NONNEG || cls == ROW_BOX) {
       v = flag[i] == SA_ROW_IN ? h[i] : T(0);

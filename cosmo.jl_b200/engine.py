@@ -21,6 +21,7 @@ F64, F32 = 0, 1
 ZERO, NONNEG, BOX, SOC, PSD_SQUARE, PSD_TRIANGLE, EXP, DUAL_EXP, POW, DUAL_POW, PSD_TRIANGLE_COMPLEX, CUSTOM = range(12)
 CUSTOM_THREAD, CUSTOM_WARP, CUSTOM_BLOCK = 0, 1, 2
 CUSTOM_HAS_IN_DUAL, CUSTOM_HAS_IN_POL_RECC = 1, 2
+CUSTOM_HAS_JACOBIAN = 8
 STATUS = {0: "Undetermined", 1: "Solved", 2: "Max_iter_reached", 3: "Time_limit_reached",
           4: "Primal_infeasible", 5: "Dual_infeasible", 6: "Unsolved"}
 KKT_CG, KKT_MINRES_REDUCED, KKT_MINRES, KKT_LDL, KKT_LDL_SUPERNODAL = 0, 1, 2, 3, 4
@@ -624,7 +625,7 @@ class Engine:
                       db=None, dPx=None, dAx=None, dl=None, du=None):
         """cosmo_b200_solve_adjoint: the gradients of a loss with respect to the data from its gradients dx, dy, ds with
         respect to the last solve's solution (x, y, s), through the fixed point of the iteration (DESIGN.md §3k); every
-        cone but Exp/Pow, custom and complex PSD cones, every single-GPU KKT plugin.  Inputs and outputs as for
+        cone but Exp/Pow, complex PSD and custom cones whose type has no Jacobian hook, every single-GPU KKT plugin.  Inputs and outputs as for
         ``adjoint``.  Returns ((dq, db, dPx, dAx, dl, du), stats), stats keyed by SOLVE_ADJOINT_STATS (status 1 computed,
         0 GMRES or a PSD eigensolve did not converge, -1 not applicable, the outputs then NaN; the counts as ints)."""
         gx, gy, gs = (self._arr(a, k, np.float64) for a, k in ((dx, self.n), (dy, self.m), (ds, self.m)))

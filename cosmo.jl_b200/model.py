@@ -153,19 +153,23 @@ class CustomConeType:
     `name` (the contract is in include/cosmo_b200.h at COSMO_B200_CUSTOM).  The engine compiles it for sm_90a when an
     engine that uses it is created, once per process and dtype.  granularity: "thread" (one lane per cone), "warp"
     (32 lanes) or "block" (256 lanes); n_params: values per cone; in_dual / in_pol_recc: whether `source` defines the
-    certificate hooks (without them the infeasibility checks never certify, as the reference's documentation says)."""
+    certificate hooks (without them the infeasibility checks never certify, as the reference's documentation says);
+    jacobian: whether `source` defines the Jacobian of its projection, `jacobian(w, s, h, dim, p, lane, width)`, which
+    solve_adjoint / solve_derivative (and autograd.solve_conic) need to differentiate through the cone."""
     _GRAN = {"thread": _eng.CUSTOM_THREAD, "warp": _eng.CUSTOM_WARP, "block": _eng.CUSTOM_BLOCK}
 
     def __init__(self, name: str, source: str, granularity: str = "warp", n_params: int = 0, in_dual: bool = False,
-                 in_pol_recc: bool = False):
+                 in_pol_recc: bool = False, jacobian: bool = False):
         if granularity not in self._GRAN:
             raise ValueError("granularity must be one of %s" % sorted(self._GRAN))
         self.name, self.source, self.granularity = str(name), str(source), granularity
         self.n_params, self.in_dual, self.in_pol_recc = int(n_params), bool(in_dual), bool(in_pol_recc)
+        self.jacobian = bool(jacobian)
         self._bytes = (self.name.encode(), self.source.encode())   # what struct() points to, alive with the type
 
     def struct(self) -> "_eng.CustomConeStruct":
-        flags = (_eng.CUSTOM_HAS_IN_DUAL if self.in_dual else 0) | (_eng.CUSTOM_HAS_IN_POL_RECC if self.in_pol_recc else 0)
+        flags = (_eng.CUSTOM_HAS_IN_DUAL if self.in_dual else 0) | (_eng.CUSTOM_HAS_IN_POL_RECC if self.in_pol_recc else 0) | \
+            (_eng.CUSTOM_HAS_JACOBIAN if self.jacobian else 0)
         return _eng.CustomConeStruct(self._bytes[0], self._bytes[1], self._GRAN[self.granularity], self.n_params, flags, 0)
 
     def compile(self, dtype=np.float64) -> bool:
@@ -886,8 +890,8 @@ class Model:
     def solve_adjoint(self, dx=None, dy=None, ds=None, tol=0.0, max_iter=500, restart=30, kkt_tol=1e-12):
         """Gradients of a scalar loss with respect to the data, from its gradients dx (n), dy, ds (m) with respect to the
         solution (x, y, s) of the last optimize() (None: zero), through cosmo_b200_solve_adjoint (DESIGN.md §3k): the
-        derivative of the solution map through the fixed point of the iteration, for ZeroSet, Nonnegatives, Box, SOC and
-        real PSD constraints and every KKT solver.  Returns the dict of adjoint() ("P", "A", "q", "b", "l", "u") plus
+        derivative of the solution map through the fixed point of the iteration, for ZeroSet, Nonnegatives, Box, SOC,
+        real PSD constraints and custom cones whose type has a Jacobian hook, and every KKT solver.  Returns the dict of adjoint() ("P", "A", "q", "b", "l", "u") plus
         "stats" (Engine.SOLVE_ADJOINT_STATS).  ValueError before the first optimize() and when the last one decomposed
         the problem (decompose=True with at least one decomposed cone)."""
         if self.engine is None:

@@ -96,7 +96,16 @@ enum {
    never certifies, so such a problem runs to Max_iter_reached where the reference would raise a MethodError (its
    documentation calls this "infeasibility detection is disabled").  No #include is needed: a prelude defines, in
    namespace cosmo_cone, sum(v, width), max(v, width) and all(b, width) over the lanes of a cone, which every lane of
-   the cone must call. */
+   the cone must call, and sync(width), which orders the lanes' memory accesses.
+   With COSMO_B200_CUSTOM_HAS_JACOBIAN the source also defines
+     template <typename T> __device__ void jacobian(const T* w, const T* s, T* h, long long dim, const T* p, int lane, int width);
+   which cosmo_b200_solve_adjoint and cosmo_b200_solve_derivative use to differentiate through the cone: w is the cone's
+   rows of the point w_s = s + mu ./ rho, s = project(w) (computed by the type's own project at that point), and h holds
+   a direction that the hook overwrites with DPi(w) h.  All lanes call it together, as the other hooks.  The hook must be
+   linear in h and symmetric (<g, DPi h> = <DPi g, h>: the Jacobian of the projection onto a closed convex set is
+   symmetric wherever it exists, and the engine uses the one hook for both Dpi and Dpi'), and deterministic (the prelude's
+   reductions, no atomics).  At a kink it may return any element of the generalised Jacobian, as the built-in cones do.
+   A type without the flag makes both derivative calls return status -1. */
 #define COSMO_B200_CUSTOM 11 /* cosmo_b200_set.type */
 enum {
   COSMO_B200_CUSTOM_THREAD = 0, /* one lane per cone */
@@ -105,6 +114,8 @@ enum {
 };
 #define COSMO_B200_CUSTOM_HAS_IN_DUAL 1
 #define COSMO_B200_CUSTOM_HAS_IN_POL_RECC 2
+/* 4 is unassigned */
+#define COSMO_B200_CUSTOM_HAS_JACOBIAN 8
 typedef struct {
   const char* name;    /* C identifier: the namespace of the device functions in `source` (not "cosmo_cone") */
   const char* source;  /* CUDA C++; compiler messages name its lines as `name`(line) */
@@ -597,7 +608,8 @@ int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* 
 
 /* ---- derivatives of a conic solution --------------------------------------- */
 /* An engine extension beyond the reference, like cosmo_b200_adjoint, for every cone the engine differentiates: ZeroSet,
-   Nonnegatives, Box, SecondOrderCone, PsdCone and PsdConeTriangle (real), with every single-GPU KKT plugin.  Given the
+   Nonnegatives, Box, SecondOrderCone, PsdCone and PsdConeTriangle (real), and custom cones whose type has
+   COSMO_B200_CUSTOM_HAS_JACOBIAN, with every single-GPU KKT plugin.  Given the
    gradients dx (n), dy, ds (m) of a scalar loss with respect to the last solve's solution (x, y = -mu, s), it returns
    the gradients of that loss with respect to the data of the unscaled set! form A x + s = b, by the adjoint of the
    fixed point of the ADMM iteration.  In the engine's scaled coordinates, with w_s = s + mu ./ rho, Dpi the Jacobian
@@ -625,8 +637,9 @@ typedef struct {
    kink, SOC cones near a kink, PSD cones near a kink, PSD cones whose eigensolver missed psd_max_sweeps}; near a kink
    means within 64 u (1 + |w_s| of the cone), u the unit roundoff of the element type.  status 1: the gradients are
    written.  0: GMRES did not reach tol within max_iter, or a PSD eigensolve did not converge: the outputs are NaN.
-   -1: not applicable (an Exp / Pow cone or a dual, a custom cone, a complex PsdConeTriangle, or the last solve ended
-   Primal_infeasible, Dual_infeasible or Unsolved): the outputs are NaN.  Bad settings, out NULL, or no solve since
+   -1: not applicable (an Exp / Pow cone or a dual, a custom cone whose type lacks COSMO_B200_CUSTOM_HAS_JACOBIAN, a
+   complex PsdConeTriangle, or the last solve ended Primal_infeasible, Dual_infeasible or Unsolved): the outputs are NaN.
+   Custom cones with the hook are differentiated through it; they are not counted in the kink diagnostics out[4 .. 7].  Bad settings, out NULL, or no solve since
    create / reset / warm_start / rescale_iterates: COSMO_B200_ERR_INVALID.  A sharded handle, or a handle with a forward
    map or decomposition map: COSMO_B200_ERR_UNSUPPORTED.  A Krylov basis that does not fit: COSMO_B200_ERR_ALLOC.
    State: the iterates, the solution, rho, the rho vector, the rho updates, the accelerator history and the polish
@@ -635,7 +648,8 @@ typedef struct {
    that never ran this call; a direct plugin whose factor is marked dirty refactors here instead of in the next solve
    (only the factorisation counters move, and the factor a polish left for cosmo_b200_adjoint is replaced).  Two calls
    give bit-identical results.  Scratch allocated by the first call and kept: (restart + 3)(n + m) + 3 m values of the
-   element type, m flag bytes, N^2 + N values per PSD cone and 3 N^2 for the largest PSD cone with N > 96.  Host arrays
+   element type, m flag bytes, N^2 + N values per PSD cone, 3 N^2 for the largest PSD cone with N > 96, and m more values
+   when the handle has custom cones (their projection at w_s, for the Jacobian hook).  Host arrays
    are staged through a buffer of their size. */
 int cosmo_b200_solve_adjoint(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dx,
                              const double* dy, const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl,
