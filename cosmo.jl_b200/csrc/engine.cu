@@ -206,6 +206,7 @@ class EngineBase {
   virtual void solve_derivative(const cosmo_b200_solve_adjoint_settings* as, const double* dPx, const double* dq,
                                 const double* dAx, const double* db, const double* dl, const double* du, double* dx,
                                 double* dy, double* ds, double* out8) = 0;
+  virtual void project_jacobian(const void* ws, const void* dir, void* out, int64_t* counts4) = 0;
 };
 
 template <typename T>
@@ -273,6 +274,7 @@ class Engine : public EngineBase {
   void solve_derivative(const cosmo_b200_solve_adjoint_settings* as, const double* dPx, const double* dq, const double* dAx,
                         const double* db, const double* dl, const double* du, double* dx, double* dy, double* ds,
                         double* out8) override;
+  void project_jacobian(const void* ws, const void* dir, void* out, int64_t* counts4) override;
 
  private:
   // ---- problem ----
@@ -381,6 +383,7 @@ class Engine : public EngineBase {
   std::vector<long long> sa_large_q_off_;
   std::vector<int> sa_large_lam_off_;
   void sa_alloc(int restart);
+  void sa_alloc_point();
   void sa_dots(const T* V, long long ldv, int k, const T* w, double* out);
   void sa_dpi(const T* h, T* out);
   template <class Rhs>
@@ -396,10 +399,12 @@ class Engine : public EngineBase {
     int isc[ISC_COUNT];
   };
   cosmo_b200_solve_adjoint_settings sa_settings(const cosmo_b200_solve_adjoint_settings* as, const char* who);
+  bool sa_cone_without_jacobian() const;
   bool sa_not_applicable() const;
   SaSaved sa_save();
   void sa_restore(const SaSaved& sv);
   int sa_point(double* out);
+  int sa_point_data(double* out);
   template <class Op>
   bool sa_gmres(Op&& op, int R, int max_iter, double tol, long long& apps, double& rel);
   template <class Rhs, class Op, class Emit>
@@ -3562,7 +3567,6 @@ void Engine<T>::nan_f64(unsigned dev, int nin, const F64Out* outs, int nout) {
 template <typename T>
 void Engine<T>::sa_alloc(int restart) {
   const long long L = (long long)n_ + m_;
-  const int m1 = std::max(m_, 1);
   if (restart > sa_restart_) {
     sa_restart_ = 0;   // until the three buffers below are in place
     sa_V_.alloc((size_t)(restart + 3) * std::max<long long>(L, 1), false);   // restart + 1 basis columns, lam, gw
@@ -3572,6 +3576,13 @@ void Engine<T>::sa_alloc(int restart) {
   }
   const size_t save = (size_t)std::max(n_, 1) + (mr_x_.p ? mr_x_.n : 0);   // xsol_ and the full MINRES warm start
   if (sa_save_.n < save) sa_save_.alloc(save, false);
+  sa_alloc_point();
+}
+
+// the buffers of the point and its Jacobian data (everything sa_point_data and sa_dpi use), allocated once
+template <typename T>
+void Engine<T>::sa_alloc_point() {
+  const int m1 = std::max(m_, 1);
   if (sa_cnt_.p) return;
   sa_ws_.alloc(m1, false); sa_h_.alloc(m1); sa_dh_.alloc(m1); sa_flag_.alloc(m1);
   sa_cnt_.alloc(SA_CNT_COUNT);
@@ -3621,11 +3632,12 @@ void Engine<T>::sa_dpi(const T* h, T* out) {
   if (n_soc_) {
     if (n_soc_chunks_) {
       sa_soc_dot_chunk_kernel<T><<<n_soc_chunks_, kBlock, 0, stream_>>>(sa_ws_.p, h, soc_chunk_start_.p, soc_chunk_len_.p,
+                                                                       soc_cone_chunk_ptr_.p, n_soc_, sa_soc_r_.p,
                                                                        sa_soc_dot_.p + n_soc_);
       check_launch("sa_soc_dot_chunk");
     }
-    sa_soc_dot_final_kernel<<<(n_soc_ + 127) / 128, 128, 0, stream_>>>(sa_soc_dot_.p + n_soc_, soc_cone_chunk_ptr_.p, n_soc_,
-                                                                        sa_soc_dot_.p);
+    sa_soc_dot_final_kernel<T><<<(n_soc_ + 127) / 128, 128, 0, stream_>>>(sa_soc_dot_.p + n_soc_, soc_cone_chunk_ptr_.p, n_soc_,
+                                                                           sa_soc_r_.p, sa_soc_dot_.p);
     check_launch("sa_soc_dot_final");
   }
   sa_dpi_rows_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, row_class_.p, row_cone_.p, sa_flag_.p, soc_off_.p, sa_ws_.p,
@@ -3730,15 +3742,20 @@ cosmo_b200_solve_adjoint_settings Engine<T>::sa_settings(const cosmo_b200_solve_
   return p;
 }
 
-// status -1: a cone without a Jacobian here (a custom type without the hook among them), or a last solve without a
-// solution
+// a cone without a Jacobian here: Exp/Pow cones and their duals, complex PSD cones, custom types without the hook
 template <typename T>
-bool Engine<T>::sa_not_applicable() const {
+bool Engine<T>::sa_cone_without_jacobian() const {
   bool complex_psd = false, hookless = false;
   for (const PsdConeDesc& d : psd_.small_h) complex_psd = complex_psd || d.triangle == 2;
   for (const PsdConeDesc& d : psd_.large_h) complex_psd = complex_psd || d.triangle == 2;
   for (const custom::TypeSlice& t : cust_types_) hookless = hookless || !t.entry->jac;
-  return n_c3_ || hookless || complex_psd || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
+  return n_c3_ || hookless || complex_psd;
+}
+
+// status -1: a cone without a Jacobian here, or a last solve without a solution
+template <typename T>
+bool Engine<T>::sa_not_applicable() const {
+  return sa_cone_without_jacobian() || last_status_ == COSMO_B200_PRIMAL_INFEASIBLE ||
          last_status_ == COSMO_B200_DUAL_INFEASIBLE || last_status_ == COSMO_B200_UNSOLVED;
 }
 
@@ -3772,15 +3789,22 @@ void Engine<T>::sa_restore(const SaSaved& sv) {
   kkt_tol_fixed_ = 0.0;
 }
 
-// The point w_s = s + mu / rho and its Jacobian data: the row flags, the SOC norms, the eigenpairs of every PSD cone,
-// the projection of the custom cones' rows, and the kink counts into out[4 .. 7] (custom cones are not counted).
-// Returns the PSD cones whose eigensolve did not converge.
+// The point w_s = s + mu / rho into sa_ws_ and its Jacobian data (sa_point_data).  Returns the PSD cones whose
+// eigensolve did not converge.
 template <typename T>
 int Engine<T>::sa_point(double* out) {
+  ws_from_mu_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_vec_.p, mu_.p, s_.p, sa_ws_.p);
+  check_launch("ws_from_mu");
+  return sa_point_data(out);
+}
+
+// The Jacobian data of the point sa_ws_ holds: the row flags, the SOC norms, the eigenpairs of every PSD cone, the
+// projection of the custom cones' rows, and the kink counts into out[4 .. 7] (custom cones are not counted).  Returns
+// the PSD cones whose eigensolve did not converge.
+template <typename T>
+int Engine<T>::sa_point_data(double* out) {
   const int m = m_;
   CUDA_TRY(cudaMemsetAsync(sa_cnt_.p, 0, SA_CNT_COUNT * sizeof(int), stream_));
-  ws_from_mu_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, rho_vec_.p, mu_.p, s_.p, sa_ws_.p);
-  check_launch("ws_from_mu");
   sa_row_flags_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_ws_.p, box_l_.p, box_u_.p, sa_flag_.p, sa_cnt_.p);
   check_launch("sa_row_flags");
   if (n_cust_) custom_project(sa_ws_.p, sa_cust_s_.p);
@@ -4124,6 +4148,37 @@ void Engine<T>::solve_derivative(const cosmo_b200_solve_adjoint_settings* as, co
   sa_run(p, dev, ins, in_count, 6, outs, 3, out, rhs, op, emit);
 }
 
+// out = DPi(w_s) dir in the coordinates project() takes: the Jacobian data of w_s formed as solve_adjoint forms them at
+// its point (sa_point_data), then one sa_dpi.  counts = the kink counts and the PSD cones whose eigensolve missed
+// psd_max_sweeps (out is then all NaN).  Needs no solve; the iterates, the solution, rho and the plugin state are not
+// touched, and the GMRES scratch is not allocated.
+template <typename T>
+void Engine<T>::project_jacobian(const void* ws, const void* dir, void* out, int64_t* counts) {
+  single_gpu("project_jacobian");
+  if (sa_cone_without_jacobian())
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED,
+                      "project_jacobian: no Jacobian for Exp/Pow cones, complex PSD cones or custom types without the hook"};
+  CUDA_TRY(cudaSetDevice(device_));
+  for (int k = 0; k < 4; ++k) counts[k] = 0;
+  if (!m_) return;
+  sa_alloc_point();
+  upload_vec(sa_ws_, ws, m_);
+  upload_vec(sa_h_, dir, m_);
+  const int sweeps = psd_.last_sweeps;   // what the last solve's projections reported
+  double o[8];
+  const int unconverged = sa_point_data(o);
+  psd_.last_sweeps = sweeps;
+  if (unconverged) {
+    ruiz_fill_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, sa_dh_.p, std::numeric_limits<T>::quiet_NaN());
+    check_launch("project_jacobian_nan");
+  } else {
+    sa_dpi(sa_h_.p, sa_dh_.p);
+  }
+  download_vec(out, sa_dh_.p, m_);
+  sync();
+  for (int k = 0; k < 4; ++k) counts[k] = (int64_t)o[4 + k];
+}
+
 }  // namespace cosmo
 
 // ============================================================================
@@ -4211,6 +4266,10 @@ int cosmo_b200_solve(cosmo_b200_handle* h, cosmo_b200_result* out) { ABI_GUARD(h
 int cosmo_b200_project(cosmo_b200_handle* h, const void* w_s, void* s_out) {
   if (!w_s || !s_out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->project(w_s, s_out));
+}
+int cosmo_b200_project_jacobian(cosmo_b200_handle* h, const void* w_s, const void* dir, void* out, int64_t counts[4]) {
+  if (!w_s || !dir || !out || !counts) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->project_jacobian(w_s, dir, out, counts));
 }
 int cosmo_b200_kkt_solve(cosmo_b200_handle* h, const void* rhs, void* sol, int64_t* inner) {
   if (!rhs || !sol) return COSMO_B200_ERR_INVALID;

@@ -81,16 +81,31 @@ __global__ void __launch_bounds__(kBlock) sa_soc_kink_kernel(int ncones, const i
   }
 }
 
-// xbar'h per chunk of a SOC tail (fixed-order block tree), the partials the next kernel folds per cone
+// The SOC terms are formed from dhat = xbar'hbar / r, summed with xbar scaled by 2^-e, e = pow2_exponent(r) (exact):
+// every scaled entry is below 1 in magnitude, so the sum neither overflows nor underflows where h does not, whatever
+// the scale of w_s (an unscaled xbar'hbar overflows at |w_s| |h| > 2^1024 and flushes to 0 below 2^-1074)
+__device__ __forceinline__ int sa_soc_exponent(double r) { return pow2_exponent<double>(r); }
+
+// 2^-e xbar'h per chunk of a SOC tail (fixed-order block tree), the partials the next kernel folds per cone; the cone
+// of chunk c is the last k with cone_chunk_ptr[k] <= c
 template <typename T>
 __global__ void __launch_bounds__(kBlock) sa_soc_dot_chunk_kernel(const T* __restrict__ ws, const T* __restrict__ h,
                                                                   const int* __restrict__ chunk_start,
-                                                                  const int* __restrict__ chunk_len, double* __restrict__ chunk_dot) {
+                                                                  const int* __restrict__ chunk_len,
+                                                                  const int* __restrict__ cone_chunk_ptr, int ncones,
+                                                                  const T* __restrict__ norm, double* __restrict__ chunk_dot) {
   __shared__ double sm[kWarpsPerBlock];
   const int c = blockIdx.x;
   const int start = chunk_start[c], len = chunk_len[c];
+  int lo = 0, hi = ncones - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (cone_chunk_ptr[mid] <= c) lo = mid;
+    else hi = mid - 1;
+  }
+  const double down = ldexp(1.0, -sa_soc_exponent((double)norm[lo]));
   double acc = 0.0;
-  for (int i = threadIdx.x; i < len; i += blockDim.x) acc += (double)ws[start + i] * (double)h[start + i];
+  for (int i = threadIdx.x; i < len; i += blockDim.x) acc += ((double)ws[start + i] * down) * (double)h[start + i];
   acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = acc;
   __syncthreads();
@@ -101,26 +116,29 @@ __global__ void __launch_bounds__(kBlock) sa_soc_dot_chunk_kernel(const T* __res
   }
 }
 
-// dot[k] = sum of cone k's chunk partials in chunk order
+// dhat[k] = (sum of cone k's chunk partials in chunk order) / (2^-e r), 0 when r = 0 (no branch reads it then)
+template <typename T>
 __global__ void sa_soc_dot_final_kernel(const double* __restrict__ chunk_dot, const int* __restrict__ cone_chunk_ptr, int ncones,
-                                        double* __restrict__ dot) {
+                                        const T* __restrict__ norm, double* __restrict__ dhat) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= ncones) return;
   double v = 0.0;
   for (int c = cone_chunk_ptr[k]; c < cone_chunk_ptr[k + 1]; ++c) v += chunk_dot[c];
-  dot[k] = v;
+  const double r = (double)norm[k];
+  const double rs = ldexp(r, -sa_soc_exponent(r));
+  dhat[k] = rs > 0.0 ? v / rs : 0.0;
 }
 
 // out = Dpi h on every row outside the PSD and custom cones (those are written by the PSD kernels and the custom cones'
 // Jacobian hooks):
 //   ZeroSet 0;  Nonnegatives, Box: h strictly inside, 0 outside;
-//   SOC (t, xbar), r = |xbar|: h if r <= t, 0 if r <= -t, else
-//     1/2 [h_t + xbar'hbar / r ;  xbar h_t / r + (1 + t/r) hbar - (t/r) xbar (xbar'hbar) / r^2]
+//   SOC (t, xbar), r = |xbar|, dhat = xbar'hbar / r: h if r <= t, 0 if r <= -t, else
+//     1/2 [h_t + dhat ;  (xbar / r) h_t + (1 + t/r) hbar - (t/r) (xbar / r) dhat]
 template <typename T>
 __global__ void __launch_bounds__(kBlock) sa_dpi_rows_kernel(int m, const unsigned char* __restrict__ row_class,
                                                              const int* __restrict__ row_cone, const unsigned char* __restrict__ flag,
                                                              const int* __restrict__ soc_off, const T* __restrict__ ws,
-                                                             const T* __restrict__ soc_r, const double* __restrict__ soc_dot,
+                                                             const T* __restrict__ soc_r, const double* __restrict__ soc_dhat,
                                                              const T* __restrict__ h, T* __restrict__ out) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
     const unsigned char cls = row_class[i];
@@ -135,12 +153,12 @@ __global__ void __launch_bounds__(kBlock) sa_dpi_rows_kernel(int m, const unsign
       if (r <= t) {
         v = h[i];
       } else if (r > -t) {
-        const double d = soc_dot[k];
+        const double d = soc_dhat[k];
         if (i == off) {
-          v = (T)(0.5 * ((double)h[off] + d / r));
+          v = (T)(0.5 * ((double)h[off] + d));
         } else {
-          const double xi = (double)ws[i], tr = t / r;
-          v = (T)(0.5 * (xi / r * (double)h[off] + (1.0 + tr) * (double)h[i] - tr * xi * d / (r * r)));
+          const double xr = (double)ws[i] / r, tr = t / r;
+          v = (T)(0.5 * (xr * (double)h[off] + (1.0 + tr) * (double)h[i] - tr * xr * d));
         }
       }
     }

@@ -134,6 +134,8 @@ class SolveAdjointSettings(C.Structure):
 # cosmo_b200_solve_adjoint's out[8]
 SOLVE_ADJOINT_STATS = ("status", "operator_applications", "residual", "inner_iterations", "rows_near_kink",
                        "soc_near_kink", "psd_near_kink", "psd_unconverged")
+# cosmo_b200_project_jacobian's counts[4]
+PROJECT_JACOBIAN_STATS = ("rows_near_kink", "soc_near_kink", "psd_near_kink", "psd_unconverged")
 
 
 def _signatures():
@@ -156,6 +158,7 @@ def _signatures():
         "cosmo_b200_accelerator_stats": (rc, [vp, P(i64)]),
         "cosmo_b200_solve": (rc, [vp, P(ResultStruct)]),
         "cosmo_b200_project": (rc, [vp, vp, vp]),
+        "cosmo_b200_project_jacobian": (rc, [vp, vp, vp, vp, P(i64)]),
         "cosmo_b200_kkt_solve": (rc, [vp, vp, vp, P(i64)]),
         "cosmo_b200_residuals": (rc, [vp, vp, vp, vp, i32, P(f64)]),
         "cosmo_b200_spmv": (rc, [vp, i32, vp, vp]),
@@ -719,6 +722,17 @@ class Engine:
         out = np.empty(self.m, dtype=self.dtype)
         self._check(self._lib.cosmo_b200_project(self._h, _ptr(w_s), _ptr(out)))
         return out
+
+    def project_jacobian(self, w_s, h, out=None):
+        """cosmo_b200_project_jacobian: DPi(w_s) h on the engine's cones, in the coordinates ``project`` takes (the
+        Jacobian solve_adjoint and solve_derivative apply, DESIGN.md §3k).  w_s and h are host or CUDA arrays of m values;
+        out a host or CUDA output of the engine's dtype, None allocates a NumPy array.  Returns (out, counts), counts keyed
+        by PROJECT_JACOBIAN_STATS (out is all NaN when a PSD eigensolve missed psd_max_sweeps)."""
+        out = np.empty(self.m, dtype=self.dtype) if out is None else out
+        w, d, o = self._arr(w_s, self.m), self._arr(h, self.m), self._arr(out, self.m, output=True)
+        counts = _keyed(self._lib, self._h, self._lib.cosmo_b200_project_jacobian, self._h, _ptr(w), _ptr(d), _ptr(o),
+                        ctype=C.c_int64, keys=PROJECT_JACOBIAN_STATS)
+        return out, counts
 
     def kkt_solve(self, rhs):
         rhs = self._vec(rhs, self.n + self.m)

@@ -341,6 +341,13 @@ int cosmo_b200_solve(cosmo_b200_handle* h, cosmo_b200_result* out);
 /* ---- plugin-granularity entry points (also the parity-test hooks) -------- */
 /* project!(s, C): s_out = Pi_K(w_s) (convexset.jl:885-891) */
 int cosmo_b200_project(cosmo_b200_handle* h, const void* w_s, void* s_out);
+/* out = DPi(w_s) dir on the handle's cones, in the coordinates cosmo_b200_project takes; counts = {rows, SOC cones,
+   PSD cones near a kink, PSD cones whose eigensolve missed psd_max_sweeps (out is then all NaN)}.  Arrays of m values
+   of the handle's dtype, host or device memory; no solve needed, and the iterates, the solution, rho and the plugin
+   state are not touched.  The Jacobian solve_adjoint and solve_derivative apply (DESIGN.md §3k), so a custom type's
+   `jacobian` hook can be checked against finite differences of cosmo_b200_project.  ERR_UNSUPPORTED for Exp/Pow
+   cones and their duals, complex PSD cones, custom types without the hook and sharded handles. */
+int cosmo_b200_project_jacobian(cosmo_b200_handle* h, const void* w_s, const void* dir, void* out, int64_t counts[4]);
 /* solve!(kkt_solver, sol, rhs): rhs, sol in R^{n+m} (kktsolver_indirect.jl:36-88,123-162) */
 int cosmo_b200_kkt_solve(cosmo_b200_handle* h, const void* rhs, void* sol, int64_t* inner_iterations);
 /* calculate_residuals! + max_res_component_norm + calculate_cost! (residuals.jl:30-96,143-147)

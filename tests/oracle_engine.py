@@ -3,7 +3,7 @@
 It exists to exercise, without a GPU, the Python side of everything that normally talks to the CUDA engine: the host
 glue of Model (scaling, decomposition, warm starts) and the bodies of the GPU tests themselves (so a typo in a GPU
 test is found by the CPU run, not at the next GPU run).  It implements the part of the call surface those users need:
-ctor, update_settings, warm_start, update_qb, project, solve, w, rho_vec, scaling, close, and the infeasibility hooks
+ctor, update_settings, warm_start, update_qb, project, project_jacobian, solve, w, rho_vec, scaling, close, and the infeasibility hooks
 infeasibility_test and psd_lambda_max."""
 import numpy as np
 import scipy.sparse as sp
@@ -82,6 +82,18 @@ class OracleEngine:
         out = np.array(ws, dtype=float).copy()
         O.project(out, self.cones)
         return out.astype(self.dtype)
+
+    def project_jacobian(self, w_s, h, out=None):
+        """Dpi(w_s) h from the double-double reference, with its kink counts (no eigensolve misses here)"""
+        from tests import projection_jacobian_reference as R
+        w = np.asarray(w_s, dtype=float)
+        u = 2.0 ** -24 if self.dtype == np.float32 else 2.0 ** -53
+        res = R.dpi(w, self.cones, np.asarray(h, dtype=float)).astype(self.dtype)
+        if out is not None:
+            out[:] = res
+            res = out
+        counts = dict(zip(E.PROJECT_JACOBIAN_STATS, R.kink_counts(w, self.cones, u) + (0,)))
+        return res, counts
 
     def solve(self):
         st = self.st

@@ -1,6 +1,7 @@
 """Dry run of GPU test bodies on the CPU: the CUDA engine is replaced by the oracle-backed stand-in of
 tests/oracle_engine.py and the functions of tests/test_gpu_parity.py, tests/test_gpu_float32.py and
-tests/test_gpu_scale_edges.py and tests/test_gpu_infeasibility.py are called directly.  What this checks is the
+tests/test_gpu_scale_edges.py, tests/test_gpu_infeasibility.py and tests/test_gpu_projection_jacobian.py are called
+directly.  What this checks is the
 Python side of those tests (imports, helpers, fixtures, the host glue they drive) -- a NameError in a GPU test would
 otherwise only show up on the next GPU run.  Assertion failures are tolerated where the stand-in legitimately differs
 from the engine (it ignores the D/E unscaling of the termination test); every other exception fails the test."""
@@ -39,7 +40,12 @@ CASES = ["test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_t
          "test_gpu_infeasibility::test_psd_lambda_max_homogeneity_ladder",
          "test_gpu_infeasibility::test_unconverged_eigensolver_is_not_certified",
          "test_gpu_infeasibility::test_reference_infeasible_problems_status_and_iterations",
-         "test_gpu_infeasibility::test_reference_infeasible_problems_float32"]
+         "test_gpu_infeasibility::test_reference_infeasible_problems_float32",
+         "test_gpu_projection_jacobian::test_psd_size_and_spectrum_sweep",
+         "test_gpu_projection_jacobian::test_psd_sweep_float32", "test_gpu_projection_jacobian::test_soc_sweep",
+         "test_gpu_projection_jacobian::test_rows_bit_exact", "test_gpu_projection_jacobian::test_properties_per_path",
+         "test_gpu_projection_jacobian::test_scale_ladder", "test_gpu_projection_jacobian::test_path_boundary_96_97",
+         "test_gpu_projection_jacobian::test_kink_counts"]
 MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_through_the_clique_batch",
              "test_project_exp_pow_cones", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
              "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_project_psd_small_batch_float32",
@@ -47,7 +53,10 @@ MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_s
              "test_gpu_infeasibility::test_gates_reached_on_either_side_pin_E_D_and_c",
              "test_gpu_infeasibility::test_rows_at_the_tolerance_edge",
              "test_gpu_infeasibility::test_soc_exact_boundary_points_are_certified",
-             "test_gpu_infeasibility::test_composite_bitmask_names_exactly_the_failing_family"}
+             "test_gpu_infeasibility::test_composite_bitmask_names_exactly_the_failing_family",
+             "test_gpu_projection_jacobian::test_psd_size_and_spectrum_sweep",
+             "test_gpu_projection_jacobian::test_soc_sweep", "test_gpu_projection_jacobian::test_rows_bit_exact",
+             "test_gpu_projection_jacobian::test_kink_counts"}
 
 
 def _calls(fn):
