@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <limits>
 
 namespace cosmo {
@@ -19,6 +20,9 @@ constexpr int kBlock = 256;           // threads per block for every reducing ke
 constexpr int kWarpsPerBlock = kBlock / 32;
 constexpr int kMaxGrid = 132 * 8;     // 132 SMs x 8 resident 256-thread blocks
 constexpr int kMaxRed = 8;            // max reduction slots per kernel
+
+// grid of a kBlock-thread grid-stride loop over n elements
+inline int vgrid(long long n) { return (int)std::min<long long>(std::max<long long>((n + kBlock - 1) / kBlock, 1), kMaxGrid); }
 
 template <typename T>
 struct CsrView {

@@ -19,7 +19,7 @@
 #include <atomic>
 #include <functional>
 #include <thread>
-#include <chrono>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -46,10 +46,6 @@
 namespace cosmo {
 
 static thread_local std::string g_create_error;
-
-static inline double now_s() {
-  return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
 
 // ---- NCCL through dlopen (the single-GPU path has no NCCL dependency) --------
 struct NcclUniqueId { char internal[128]; };
@@ -216,12 +212,9 @@ class Engine : public EngineBase {
   ~Engine() override;
   void update_settings(const cosmo_b200_settings& st) override {
     drop_polish_record();
-    if (st.sigma != st_.sigma) {   // sigma is baked into the captured kernel arguments
+    if (st.sigma != st_.sigma) {   // sigma is baked into the captured CG kernel arguments and enters every factor
       destroy_cg_graphs();
-      destroy_ldl_factor_graph();
-      ldl_dirty_ = true;
-      sn_factor_graph_.reset();
-      sn_dirty_ = true;
+      invalidate_factors();
     }
     st_ = st;
   }
@@ -248,8 +241,17 @@ class Engine : public EngineBase {
   void accelerator_stats(int64_t* out6) override;
   void infeasibility_test(int which, const void* delta, double* out8) override;
   void psd_lambda_max(const void* v, double* lam) override;
-  void ldl_stats(double* out8) override;
-  void ldl_sn_stats(int64_t* out8) override;
+  // the supernodal plugin's when it is the KKT solver, otherwise the simplicial one's; zeros from a plugin never built
+  void ldl_stats(double* out8) override {
+    const DirectPlugin<T>* d = st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL ? (const DirectPlugin<T>*)supernodal_.get()
+                                                                                 : simplicial_.get();
+    if (d) d->stats(out8);
+    else std::fill(out8, out8 + 8, 0.0);
+  }
+  void ldl_sn_stats(int64_t* out8) override {
+    if (supernodal_) supernodal_->sn_stats(out8);
+    else std::fill(out8, out8 + 8, (int64_t)0);
+  }
   void set_decomposition(const cosmo_b200_decomposition* d, bool traditional) override;
   void set_forward_map(const cosmo_b200_forward_map* f) override;
   void update_matrices_original(const void* Px, long long nnzP, const void* Ax, long long nnzA_orig, const void* q,
@@ -356,9 +358,9 @@ class Engine : public EngineBase {
   int pol_rec_status_ = kNoPolishRecord;
   long long pol_rec_factors_ = -1;
   void drop_polish_record() { pol_rec_status_ = kNoPolishRecord; }
-  long long direct_factorizations() const {
-    return st_.kkt_solver == COSMO_B200_KKT_LDL ? ldl_factorizations_ : sn_factorizations_;
-  }
+  // refine_iter + 1 solves of K~ z = r^ with the factor in memory, each followed by polish_update_kernel, with the
+  // residual r^ - K_A z between them and at the end (max2 as for polish_residual)
+  void refine_with_factor(T* zx, T* znu, const T* rx, const T* rs, int refine_iter, double* max2);
   // adjoint scratch, allocated by the first adjoint and kept: its own z (pol_zx_ / pol_znu_ hold the polished point the
   // gradients read), the kept right-hand side, gs~ and two counters
   DevBuf<T> adj_zx_, adj_zv_, adj_rx_, adj_rs_, adj_gs_;
@@ -445,46 +447,28 @@ class Engine : public EngineBase {
   void cg_iteration_launches(const int* done);
   void build_cg_graphs(const int* done);
   void destroy_cg_graphs();
-  // direct LDL' plugin (ldl.cuh): symbolic analysis on the host, factor and solves as captured graphs
-  bool ldl_ready_ = false;
-  bool ldl_dirty_ = true;          // rho_vec_ or sigma changed since the last factorisation
-  std::vector<ldl::Segment> ldl_fseg_, ldl_bseg_;
-  std::vector<int> ldl_fptr_h_, ldl_bptr_h_;
-  int ldl_N_ = 0, ldl_ws_ctas_ = 1, ldl_solve_nodes_ = 0, ldl_factor_nodes_ = 0;
-  long long ldl_nnzK_ = 0, ldl_nnzL_ = 0, ldl_factorizations_ = 0;
-  double ldl_symbolic_s_ = 0.0, ldl_factor_s_ = 0.0;
-  DevBuf<int64_t> ldl_Kp_, ldl_Ksp_, ldl_Ksrc_, ldl_Lp_, ldl_Rp_, ldl_Rmap_;
-  DevBuf<int> ldl_Ki_, ldl_Li_, ldl_Rj_, ldl_fcols_, ldl_fptr_, ldl_bcols_, ldl_bptr_, ldl_perm_, ldl_flags_;
-  DevBuf<T> ldl_Kx_, ldl_Lx_, ldl_Rx_, ldl_D_, ldl_Dinv_, ldl_ws_, ldl_y_;
-  GraphExec ldl_factor_graph_, ldl_solve_graph_;
-  Event ldl_ev_[2];
-  void ldl_setup();
-  void ldl_factor();
-  void ldl_solve(bool kept_factor = false);
-  void destroy_ldl_factor_graph() { ldl_factor_graph_.reset(); }
+  // direct LDL' plugins (ldl.cuh, ldl_sn.cuh), each created on first use and kept across update_settings, so that a
+  // switch back finds its factor as it was
+  std::unique_ptr<LdlPlugin<T>> simplicial_;
+  std::unique_ptr<SnPlugin<T>> supernodal_;
   bool direct_kkt() const { return st_.kkt_solver == COSMO_B200_KKT_LDL || st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL; }
-  void direct_factor() {
-    if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_factor();
-    else if (st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL) sn_factor();
+  // the plugin of the current kkt_solver, null for the iterative ones
+  DirectPlugin<T>* direct_plugin() {
+    if (st_.kkt_solver == COSMO_B200_KKT_LDL) return created(simplicial_);
+    if (st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL) return created(supernodal_);
+    return nullptr;
   }
-  // supernodal LDL' plugin (ldl_sn.cuh): host analysis, factor and solves as captured graphs
-  struct SnBig { int s; int64_t groups, chunk; };
-  struct SnLevel { int small0 = 0, small1 = 0; size_t smem = 0; std::vector<SnBig> big; };
-  bool sn_ready_ = false;
-  bool sn_dirty_ = true;           // rho_vec_ or sigma changed since the last factorisation
-  ldl_sn::Symbolic sn_;            // the analysis; the graphs are built from it
-  std::vector<SnLevel> sn_levels_;
-  int sn_solve_nodes_ = 0, sn_factor_nodes_ = 0, sn_small_count_ = 0, sn_tiled_count_ = 0;
-  long long sn_factorizations_ = 0;
-  double sn_symbolic_s_ = 0.0, sn_factor_s_ = 0.0;
-  DevBuf<int64_t> sn_rptr_, sn_off_, sn_uptr_, sn_Ksp_, sn_Ksrc_, sn_Kpos_, sn_gptr_;
-  DevBuf<int> sn_sptr_, sn_rows_, sn_ud_, sn_up0_, sn_up1_, sn_gd_, sn_gi_, sn_perm_, sn_small_, sn_lrows_, sn_lcols_,
-      sn_bcols_, sn_flags_;
-  DevBuf<T> sn_Lx_, sn_D_, sn_Dinv_, sn_part_, sn_y_;
-  GraphExec sn_factor_graph_, sn_solve_graph_;
-  void sn_setup();
-  void sn_factor();
-  void sn_solve(bool kept_factor = false);
+  template <class Plugin>
+  Plugin* created(std::unique_ptr<Plugin>& p) {
+    if (!p) p.reset(new Plugin(DirectWiring<T>{n_, m_, device_, num_sms_, stream_, P_.view(), At_.view(), P_.nnz, At_.nnz,
+                                               rho_vec_.p, ls_.p, xsol_.p, nu_.p, &nranks_, &launches_}));
+    return p.get();
+  }
+  // rho_vec_ or sigma changed: every factor follows before its plugin's next solve
+  void invalidate_factors() {
+    if (simplicial_) simplicial_->invalidate();
+    if (supernodal_) supernodal_->invalidate();
+  }
   long long kkt_counter_ = 1;   // S.iteration_counter
   double kkt_tol_fixed_ = 0.0;  // > 0: the fixed relative tolerance of the solve adjoint's inner solves (inner_tol)
   int last_cg_iters_ = 1;
@@ -541,7 +525,6 @@ class Engine : public EngineBase {
     proj_rhs_kernel<T><<<vgrid((long long)a.n + a.m), kBlock, 0, stream_>>>(a);
     check_launch("proj_rhs");
   }
-  static int vgrid(long long n) { return (int)std::min<long long>(std::max<long long>((n + kBlock - 1) / kBlock, 1), kMaxGrid); }
   static int sgrid(long long rows, int lanes) {
     long long per = kBlock / lanes;
     return (int)std::min<long long>(std::max<long long>((rows + per - 1) / per, 1), kMaxGrid);
@@ -1185,7 +1168,7 @@ Engine<T>::Engine(const cosmo_b200_problem& p, const cosmo_b200_settings& st) : 
   classify_and_set_rho(true);
   sync();
   // QdldlKKTSolver's constructor factors K (kktsolver.jl:293-306): a non-convex P or a singular K fails the create
-  if (direct_kkt()) direct_factor();
+  if (DirectPlugin<T>* d = direct_plugin()) d->factor(st_.sigma);
   create_time_ = now_s() - t_ctor0;
   auto_rho_interval_ = 0;
 }
@@ -1222,8 +1205,7 @@ template <typename T>
 void Engine<T>::write_rho_vec() {
   rho_vec_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, rho_class_.p, (T)rho_, (T)st_.RHO_EQ_OVER_RHO_INEQ, (T)st_.RHO_MIN, rho_vec_.p);
   check_launch("rho_vec");
-  ldl_dirty_ = true;
-  sn_dirty_ = true;
+  invalidate_factors();
 }
 
 // scale_ruiz! (scaling.jl:21-116) on the resident data; see ruiz.cuh
@@ -1395,7 +1377,7 @@ void Engine<T>::finish_update(const T* Px, bool A, bool b, double t0) {
   destroy_cg_graphs();   // the slab and escape-table pointers they captured may have changed
   reset();
   auto_rho_interval_ = 0;
-  direct_factor();   // reset() marked the factor dirty; a non-convex P fails here
+  if (DirectPlugin<T>* d = direct_plugin()) d->factor(st_.sigma);   // a non-convex P fails here
   create_time_ = now_s() - t0;
 }
 
@@ -1578,8 +1560,7 @@ void Engine<T>::update_rho(const void* rho_vec, double rho) {
   drop_polish_record();
   if (rho_vec) upload_vec(rho_vec_, rho_vec, m_);
   rho_ = rho;
-  ldl_dirty_ = true;   // update_rho! -> refactor! (kktsolver.jl:310-313), done before the next KKT solve
-  sn_dirty_ = true;
+  invalidate_factors();   // update_rho! -> refactor! (kktsolver.jl:310-313), done before the next KKT solve
   sync();
 }
 
@@ -1858,8 +1839,7 @@ void Engine<T>::kkt_core(bool fused_tail, const T* w_src, T* w_dst) {
   const bool tm_ready = tm_valid_;
   tm_valid_ = false;
   if (full || direct) {
-    if (direct && st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_solve();   // xsol_ = y1, nu_ = y2
-    else if (direct) sn_solve();
+    if (direct) direct_plugin()->solve(st_.sigma, false);   // xsol_ = y1, nu_ = y2
     else kkt_minres(true);
     if (fused_tail) {
       admm_tail_kernel<T><<<vgrid(m_), kBlock, 0, stream_>>>(m_, nu_.p, rho_vec_.p, s_.p, w_src + n_, w_dst + n_, (T)st_.alpha);
@@ -2659,381 +2639,6 @@ void Engine<T>::kkt_solve(const void* rhs, void* sol, int64_t* inner) {
   }
 }
 
-// ---- direct LDL' plugin (ldl.cuh) -----------------------------------------------------------------------------
-// Symbolic analysis of the resident pattern (host), upload of L's structure and the schedules, device buffers.
-template <typename T>
-void Engine<T>::ldl_setup() {
-  CUDA_TRY(cudaSetDevice(device_));
-  const double t0 = now_s();
-  std::vector<int> Prow(n_ + 1), Pcol(P_.nnz), Arow(n_ + 1), Acol(At_.nnz);
-  CUDA_TRY(cudaMemcpyAsync(Prow.data(), P_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  CUDA_TRY(cudaMemcpyAsync(Arow.data(), At_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  if (P_.nnz) CUDA_TRY(cudaMemcpyAsync(Pcol.data(), P_.col.p, P_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  if (At_.nnz) CUDA_TRY(cudaMemcpyAsync(Acol.data(), At_.col.p, At_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  sync();
-  ldl::Symbolic S;
-  ldl::analyze(n_, m_, Prow, Pcol, Arow, Acol, S);
-  ldl_symbolic_s_ = now_s() - t0;
-  const int N = S.N;
-  ldl_N_ = N;
-  ldl_nnzK_ = S.nnz_triu_K();
-  ldl_nnzL_ = S.nnz_L();
-  // one dense workspace of length N per resident factor CTA: as many CTAs as the widest level, at most two per SM
-  int maxw = 1;
-  for (const ldl::Segment& s : S.fseg)
-    if (!s.run) maxw = std::max(maxw, S.fptr[s.l1] - S.fptr[s.l0]);
-  ldl_ws_ctas_ = std::max(1, std::min(maxw, 2 * num_sms_));
-  const double ts = (double)sizeof(T);
-  const double need = (double)ldl_nnzL_ * (2 * ts + 4 + 4 + 8) + (double)ldl_nnzK_ * (ts + 4 + 8) + (double)S.Ksrc.size() * 8 +
-                      (double)(N + 1) * 8 * 3 + (double)N * (ts * 3 + 4 * 5) + (double)ldl_ws_ctas_ * N * ts;
-  size_t free_b = 0, total_b = 0;
-  CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
-  if (need > 0.9 * (double)free_b) {
-    char b[256];
-    snprintf(b, sizeof(b), "the direct LDL' factor does not fit in device memory: nnz(L) = %lld needs %.2f GB, %.2f GB free",
-             ldl_nnzL_, need * 1e-9, (double)free_b * 1e-9);
-    throw EngineError{COSMO_B200_ERR_ALLOC, b};
-  }
-  ldl_Kp_.upload(S.Kp, stream_); ldl_Ki_.upload(S.Ki, stream_); ldl_Ksp_.upload(S.Ksp, stream_); ldl_Ksrc_.upload(S.Ksrc, stream_);
-  ldl_Lp_.upload(S.Lp, stream_); ldl_Li_.upload(S.Li, stream_);
-  ldl_Rp_.upload(S.Rp, stream_); ldl_Rj_.upload(S.Rj, stream_); ldl_Rmap_.upload(S.Rmap, stream_);
-  ldl_fcols_.upload(S.fcols, stream_); ldl_fptr_.upload(S.fptr, stream_);
-  ldl_bcols_.upload(S.bcols, stream_); ldl_bptr_.upload(S.bptr, stream_);
-  ldl_perm_.upload(S.perm, stream_);
-  ldl_Kx_.alloc(std::max<long long>(ldl_nnzK_, 1), false);
-  ldl_Lx_.alloc(std::max<long long>(ldl_nnzL_, 1), false);
-  ldl_Rx_.alloc(std::max<long long>(ldl_nnzL_, 1), false);
-  ldl_D_.alloc(std::max(N, 1)); ldl_Dinv_.alloc(std::max(N, 1)); ldl_y_.alloc(std::max(N, 1));
-  ldl_ws_.alloc((size_t)ldl_ws_ctas_ * std::max(N, 1));   // zeroed: every column clears what it touched
-  ldl_flags_.alloc(2);
-  sync();
-  ldl_fseg_ = S.fseg; ldl_bseg_ = S.bseg;
-  ldl_fptr_h_ = S.fptr; ldl_bptr_h_ = S.bptr;
-  ldl_ev_[0].create();
-  ldl_ev_[1].create();
-  destroy_ldl_factor_graph();
-  ldl_solve_graph_.reset();
-  ldl_ready_ = true;
-  ldl_dirty_ = true;
-}
-
-// Assemble K from the resident (scaled) P_, At_, rho_vec_ and sigma and factor it: one captured graph, replayed on
-// every refactorisation.  Reads back the pivot counts (the only host synchronisation of the plugin).
-template <typename T>
-void Engine<T>::ldl_factor() {
-  if (!ldl_ready_) ldl_setup();
-  if (!ldl_factor_graph_) {
-    int nodes = 0;
-    capture_graph(ldl_factor_graph_, stream_, [&] {
-      ldl_reset_flags_kernel<<<1, 32, 0, stream_>>>(ldl_flags_.p); ++nodes;
-      ldl_assemble_kernel<T><<<vgrid(ldl_nnzK_), kBlock, 0, stream_>>>(ldl_nnzK_, ldl_Ksp_.p, ldl_Ksrc_.p, P_.val.p, At_.val.p,
-                                                                       rho_vec_.p, (T)st_.sigma, ldl_Kx_.p);
-      ++nodes;
-      LdlFactorArgs<T> a;
-      a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p;
-      a.Kp = ldl_Kp_.p; a.Ki = ldl_Ki_.p; a.Kx = ldl_Kx_.p;
-      a.Lp = ldl_Lp_.p; a.Li = ldl_Li_.p; a.Lx = ldl_Lx_.p;
-      a.Rp = ldl_Rp_.p; a.Rj = ldl_Rj_.p; a.Rmap = ldl_Rmap_.p;
-      a.D = ldl_D_.p; a.Dinv = ldl_Dinv_.p; a.ws = ldl_ws_.p; a.N = ldl_N_; a.flags = ldl_flags_.p;
-      for (const ldl::Segment& s : ldl_fseg_) {
-        a.l0 = s.l0; a.l1 = s.l1;
-        const int grid = s.run ? 1 : std::min(ldl_fptr_h_[s.l1] - ldl_fptr_h_[s.l0], ldl_ws_ctas_);
-        ldl_factor_kernel<T><<<grid, kBlock, 0, stream_>>>(a);
-        ++nodes;
-      }
-      if (ldl_nnzL_) {
-        ldl_csr_gather_kernel<T><<<vgrid(ldl_nnzL_), kBlock, 0, stream_>>>(ldl_nnzL_, ldl_Rmap_.p, ldl_Lx_.p, ldl_Rx_.p);
-        ++nodes;
-      }
-    });
-    ldl_factor_nodes_ = nodes;
-  }
-  int flags[2] = {0, 0};
-  CUDA_TRY(cudaEventRecord(ldl_ev_[0], stream_));
-  CUDA_TRY(cudaGraphLaunch(ldl_factor_graph_, stream_));
-  CUDA_TRY(cudaEventRecord(ldl_ev_[1], stream_));
-  CUDA_TRY(cudaMemcpyAsync(flags, ldl_flags_.p, sizeof(flags), cudaMemcpyDeviceToHost, stream_));
-  sync();
-  launches_ += ldl_factor_nodes_;
-  float ms = 0.f;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ldl_ev_[0], ldl_ev_[1]));
-  ldl_factor_s_ = ms * 1e-3;
-  ++ldl_factorizations_;
-  if (flags[1] != 0) {
-    char b[160];
-    snprintf(b, sizeof(b), "LDL' factorisation of the KKT matrix met %d zero or non-finite pivots", flags[1]);
-    throw EngineError{COSMO_B200_ERR_NUMERICAL, b};
-  }
-  // positive_inertia(ldlfact) == n (kktsolver.jl:300-303)
-  if (flags[0] != n_) throw EngineError{COSMO_B200_ERR_INVALID, "Objective function is not convex."};
-  ldl_dirty_ = false;
-}
-
-// [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: forward and backward levels replayed as one graph.
-// kept_factor: solve with the factor in memory even when it is marked dirty (the adjoint, with the factor of a polish);
-// the solve reads only the factor, ls_ and the permutation, never sigma or the rho vector.
-template <typename T>
-void Engine<T>::ldl_solve(bool kept_factor) {
-  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the direct LDL' KKT solver is single-GPU"};
-  if (!ldl_ready_) ldl_setup();
-  if (ldl_dirty_ && !kept_factor) ldl_factor();
-  if (!ldl_solve_graph_) {
-    int nodes = 0;
-    capture_graph(ldl_solve_graph_, stream_, [&] {
-      LdlSolveArgs<T> a;
-      a.Dinv = ldl_Dinv_.p; a.perm = ldl_perm_.p; a.rhs = ls_.p; a.y = ldl_y_.p; a.out1 = xsol_.p; a.out2 = nu_.p; a.n = n_;
-      auto grid = [&](const std::vector<int>& ptr, const ldl::Segment& s) {
-        return s.run ? 1 : (int)std::min<long long>(((long long)ptr[s.l1] - ptr[s.l0] + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid);
-      };
-      a.cols = ldl_fcols_.p; a.lptr = ldl_fptr_.p; a.ptr = ldl_Rp_.p; a.idx = ldl_Rj_.p; a.val = ldl_Rx_.p;
-      for (const ldl::Segment& s : ldl_fseg_) {
-        a.l0 = s.l0; a.l1 = s.l1;
-        ldl_forward_kernel<T><<<grid(ldl_fptr_h_, s), kBlock, 0, stream_>>>(a);
-        ++nodes;
-      }
-      a.cols = ldl_bcols_.p; a.lptr = ldl_bptr_.p; a.ptr = ldl_Lp_.p; a.idx = ldl_Li_.p; a.val = ldl_Lx_.p;
-      for (const ldl::Segment& s : ldl_bseg_) {
-        a.l0 = s.l0; a.l1 = s.l1;
-        ldl_backward_kernel<T><<<grid(ldl_bptr_h_, s), kBlock, 0, stream_>>>(a);
-        ++nodes;
-      }
-    });
-    ldl_solve_nodes_ = nodes;
-  }
-  CUDA_TRY(cudaGraphLaunch(ldl_solve_graph_, stream_));
-  launches_ += ldl_solve_nodes_;
-}
-
-template <typename T>
-void Engine<T>::ldl_stats(double* o) {
-  if (st_.kkt_solver == COSMO_B200_KKT_LDL_SUPERNODAL) {   // stored entries (explicit zeros included), supernodal levels
-    o[0] = sn_.N; o[1] = (double)sn_.nnz_K; o[2] = (double)sn_.stored; o[3] = sn_.levels;
-    o[4] = sn_solve_nodes_; o[5] = (double)sn_factorizations_; o[6] = sn_factor_s_; o[7] = sn_symbolic_s_;
-    return;
-  }
-  o[0] = ldl_N_; o[1] = (double)ldl_nnzK_; o[2] = (double)ldl_nnzL_; o[3] = ldl_fptr_h_.empty() ? 0 : (double)ldl_fptr_h_.size() - 1;
-  o[4] = ldl_solve_nodes_; o[5] = (double)ldl_factorizations_; o[6] = ldl_factor_s_; o[7] = ldl_symbolic_s_;
-}
-
-// ---- supernodal LDL' plugin (ldl_sn.cuh) ------------------------------------------------------------------------
-// Symbolic analysis of the resident pattern (host), upload of the panels' structure and the schedules, the choice of
-// path per supernode, device buffers.
-template <typename T>
-void Engine<T>::sn_setup() {
-  CUDA_TRY(cudaSetDevice(device_));
-  const double t0 = now_s();
-  std::vector<int> Prow(n_ + 1), Pcol(P_.nnz), Arow(n_ + 1), Acol(At_.nnz);
-  CUDA_TRY(cudaMemcpyAsync(Prow.data(), P_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  CUDA_TRY(cudaMemcpyAsync(Arow.data(), At_.rowptr.p, (n_ + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  if (P_.nnz) CUDA_TRY(cudaMemcpyAsync(Pcol.data(), P_.col.p, P_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  if (At_.nnz) CUDA_TRY(cudaMemcpyAsync(Acol.data(), At_.col.p, At_.nnz * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-  sync();
-  ldl_sn::Symbolic& S = sn_;
-  ldl_sn::analyze(n_, m_, Prow, Pcol, Arow, Acol, S);
-  sn_symbolic_s_ = now_s() - t0;
-  const size_t ts = sizeof(T);
-  // path per supernode: the small path when the panel and its relative rows fit one CTA's shared memory; the tiled
-  // path's descendant updates split into groups of about kUpdatesPerGroup, the partial sums capped at 256 MB
-  constexpr int64_t kUpdatesPerGroup = 16;
-  sn_levels_.assign(S.levels, SnLevel());
-  std::vector<int> small;
-  int64_t part = 0;
-  sn_small_count_ = sn_tiled_count_ = 0;
-  for (int l = 0; l < S.levels; ++l) {
-    SnLevel& L = sn_levels_[l];
-    L.small0 = (int)small.size();
-    for (int k = S.lptr[l]; k < S.lptr[l + 1]; ++k) {
-      const int s = S.lcols[k];
-      const int64_t h = S.height(s), w = S.width(s);
-      const size_t bytes = (size_t)(h * w) * ts + (size_t)h * sizeof(int);
-      if (bytes <= (size_t)sn::kSmallBytes) {
-        small.push_back(s);
-        L.smem = std::max(L.smem, bytes);
-        ++sn_small_count_;
-      } else {
-        const int64_t nu = S.uptr[s + 1] - S.uptr[s];
-        int64_t g = std::max<int64_t>(1, (nu + kUpdatesPerGroup - 1) / kUpdatesPerGroup);
-        g = std::max<int64_t>(1, std::min<int64_t>(g, (int64_t)((256u << 20) / (h * w * ts))));
-        const int64_t chunk = std::max<int64_t>(1, (nu + g - 1) / g);
-        g = std::max<int64_t>(1, (nu + chunk - 1) / chunk);
-        L.big.push_back(SnBig{s, g, chunk});
-        if (nu) part = std::max(part, g * h * w);
-        ++sn_tiled_count_;
-      }
-    }
-    L.small1 = (int)small.size();
-  }
-  const int64_t N = S.N, entries = S.off.empty() ? 0 : S.off.back();
-  const double need = (double)entries * ts + (double)part * ts + (double)S.rows.size() * 4 + (double)S.Kpos.size() * 16 +
-                      (double)S.Ksrc.size() * 8 + (double)S.ud.size() * 12 + (double)S.gd.size() * 8 + (double)N * (3 * ts + 24);
-  size_t free_b = 0, total_b = 0;
-  CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
-  if (need > 0.9 * (double)free_b) {
-    char b[256];
-    snprintf(b, sizeof(b), "the supernodal LDL' factor does not fit in device memory: %lld stored entries need %.2f GB, %.2f GB free",
-             (long long)S.stored, need * 1e-9, (double)free_b * 1e-9);
-    throw EngineError{COSMO_B200_ERR_ALLOC, b};
-  }
-  sn_sptr_.upload(S.sptr, stream_); sn_rptr_.upload(S.rptr, stream_); sn_rows_.upload(S.rows, stream_); sn_off_.upload(S.off, stream_);
-  sn_uptr_.upload(S.uptr, stream_); sn_ud_.upload(S.ud, stream_); sn_up0_.upload(S.up0, stream_); sn_up1_.upload(S.up1, stream_);
-  sn_Ksp_.upload(S.Ksp, stream_); sn_Ksrc_.upload(S.Ksrc, stream_); sn_Kpos_.upload(S.Kpos, stream_);
-  sn_gptr_.upload(S.gptr, stream_); sn_gd_.upload(S.gd, stream_); sn_gi_.upload(S.gi, stream_);
-  sn_perm_.upload(S.perm, stream_); sn_small_.upload(small, stream_);
-  sn_lrows_.upload(S.lrows, stream_); sn_lcols_.upload(S.lcols, stream_); sn_bcols_.upload(S.bcols, stream_);
-  sn_Lx_.alloc(std::max<int64_t>(entries, 1), false);
-  sn_part_.alloc(std::max<int64_t>(part, 1), false);
-  sn_D_.alloc(std::max<int64_t>(N, 1)); sn_Dinv_.alloc(std::max<int64_t>(N, 1)); sn_y_.alloc(std::max<int64_t>(N, 1));
-  sn_flags_.alloc(2);
-  sync();
-  CUDA_TRY(cudaFuncSetAttribute(sn::sn_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
-  CUDA_TRY(cudaFuncSetAttribute(sn::sn_fdiag_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
-  CUDA_TRY(cudaFuncSetAttribute(sn::sn_backward_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
-  ldl_ev_[0].create();
-  ldl_ev_[1].create();
-  sn_factor_graph_.reset();
-  sn_solve_graph_.reset();
-  sn_ready_ = true;
-  sn_dirty_ = true;
-}
-
-template <typename T>
-static int sn_lower_tiles(int64_t rows, int64_t cols) {   // tiles (bi >= bj) of a rows x cols panel, kTile square
-  const int64_t nrt = (rows + sn::kTile - 1) / sn::kTile, nct = (cols + sn::kTile - 1) / sn::kTile;
-  int64_t t = 0;
-  for (int64_t bj = 0; bj < nct; ++bj) t += nrt - bj;
-  return (int)t;
-}
-
-// Assemble the panels from the resident (scaled) P_, At_, rho_vec_ and sigma and factor them level by level: one
-// captured graph, replayed on every refactorisation.  Reads back the pivot counts (the plugin's only host sync).
-template <typename T>
-void Engine<T>::sn_factor() {
-  if (!sn_ready_) sn_setup();
-  const ldl_sn::Symbolic& S = sn_;
-  if (!sn_factor_graph_) {
-    int nodes = 0;
-    sn::Args<T> a;
-    a.sptr = sn_sptr_.p; a.rptr = sn_rptr_.p; a.rows = sn_rows_.p; a.off = sn_off_.p;
-    a.uptr = sn_uptr_.p; a.ud = sn_ud_.p; a.up0 = sn_up0_.p; a.up1 = sn_up1_.p;
-    a.Lx = sn_Lx_.p; a.D = sn_D_.p; a.Dinv = sn_Dinv_.p; a.flags = sn_flags_.p;
-    const int64_t entries = S.off.empty() ? 0 : S.off.back();
-    capture_graph(sn_factor_graph_, stream_, [&] {
-      ldl_reset_flags_kernel<<<1, 32, 0, stream_>>>(sn_flags_.p); ++nodes;
-      if (entries) { CUDA_TRY(cudaMemsetAsync(sn_Lx_.p, 0, entries * sizeof(T), stream_)); ++nodes; }
-      if (S.nnz_K) {
-        sn::sn_assemble_kernel<T><<<vgrid(S.nnz_K), kBlock, 0, stream_>>>(S.nnz_K, sn_Ksp_.p, sn_Ksrc_.p, sn_Kpos_.p, P_.val.p,
-                                                                          At_.val.p, rho_vec_.p, (T)st_.sigma, sn_Lx_.p);
-        ++nodes;
-      }
-      for (const SnLevel& L : sn_levels_) {
-        if (L.small1 > L.small0) {
-          const int cnt = L.small1 - L.small0;
-          sn::sn_small_kernel<T><<<std::min(cnt, kMaxGrid), kBlock, L.smem, stream_>>>(a, sn_small_.p + L.small0, cnt);
-          ++nodes;
-        }
-        for (const SnBig& B : L.big) {
-          const int s = B.s, c0 = S.sptr[s], w = S.width(s), h = S.height(s);
-          T* F = sn_Lx_.p + S.off[s];
-          const int64_t u0 = S.uptr[s], u1 = S.uptr[s + 1];
-          if (u1 > u0) {
-            sn::sn_tile_update_kernel<T><<<dim3(sn_lower_tiles<T>(h, w), (unsigned)B.groups), kBlock, 0, stream_>>>(
-                a, c0, w, h, sn_rows_.p + S.rptr[s], u0, u1, B.chunk, sn_part_.p);
-            sn::sn_tile_reduce_kernel<T><<<vgrid((int64_t)h * w), kBlock, 0, stream_>>>(F, sn_part_.p, (int)B.groups, h, w);
-            nodes += 2;
-          }
-          for (int b0 = 0; b0 < w; b0 += sn::kTile) {
-            const int nb = std::min(sn::kTile, w - b0), b1 = b0 + nb;
-            const int rows = h - b1;
-            sn::sn_diag_kernel<T><<<1, kBlock, 0, stream_>>>(a, F, c0, h, b0, nb);
-            ++nodes;
-            if (rows > 0) {
-              sn::sn_panel_kernel<T><<<(rows + sn::kPanelThreads - 1) / sn::kPanelThreads, sn::kPanelThreads, 0, stream_>>>(
-                  F, h, b0, nb);
-              ++nodes;
-            }
-            if (b1 < w) {
-              sn::sn_trail_kernel<T><<<sn_lower_tiles<T>(h - b1, w - b1), kBlock, 0, stream_>>>(F, sn_D_.p + c0 + b0, h, w, b0, b1);
-              ++nodes;
-            }
-          }
-        }
-      }
-    });
-    sn_factor_nodes_ = nodes;
-  }
-  int flags[2] = {0, 0};
-  CUDA_TRY(cudaEventRecord(ldl_ev_[0], stream_));
-  CUDA_TRY(cudaGraphLaunch(sn_factor_graph_, stream_));
-  CUDA_TRY(cudaEventRecord(ldl_ev_[1], stream_));
-  CUDA_TRY(cudaMemcpyAsync(flags, sn_flags_.p, sizeof(flags), cudaMemcpyDeviceToHost, stream_));
-  sync();
-  launches_ += sn_factor_nodes_;
-  float ms = 0.f;
-  CUDA_TRY(cudaEventElapsedTime(&ms, ldl_ev_[0], ldl_ev_[1]));
-  sn_factor_s_ = ms * 1e-3;
-  ++sn_factorizations_;
-  if (flags[1] != 0) {
-    char b[160];
-    snprintf(b, sizeof(b), "supernodal LDL' factorisation of the KKT matrix met %d zero or non-finite pivots", flags[1]);
-    throw EngineError{COSMO_B200_ERR_NUMERICAL, b};
-  }
-  if (flags[0] != n_) throw EngineError{COSMO_B200_ERR_INVALID, "Objective function is not convex."};
-  sn_dirty_ = false;
-}
-
-// [y1; y2] = K \ [x1; x2] with ls_ = [x1; x2], xsol_ = y1, nu_ = y2: the forward solve by supernodal level, the
-// backward solve by depth, replayed as one graph (kept_factor as for ldl_solve)
-template <typename T>
-void Engine<T>::sn_solve(bool kept_factor) {
-  if (nranks_ > 1) throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "the supernodal LDL' KKT solver is single-GPU"};
-  if (!sn_ready_) sn_setup();
-  if (sn_dirty_ && !kept_factor) sn_factor();
-  const ldl_sn::Symbolic& S = sn_;
-  if (!sn_solve_graph_) {
-    int nodes = 0;
-    sn::SolveArgs<T> a;
-    a.sptr = sn_sptr_.p; a.rptr = sn_rptr_.p; a.rows = sn_rows_.p; a.off = sn_off_.p;
-    a.gptr = sn_gptr_.p; a.gd = sn_gd_.p; a.gi = sn_gi_.p;
-    a.Lx = sn_Lx_.p; a.Dinv = sn_Dinv_.p; a.perm = sn_perm_.p;
-    a.rhs = ls_.p; a.y = sn_y_.p; a.out1 = xsol_.p; a.out2 = nu_.p; a.n = n_;
-    // the diagonal solves keep their part of y in shared memory up to kSmallBytes, wider supernodes work on y in place
-    auto vec_smem = [&](int wmax) { return (size_t)wmax * sizeof(T) <= (size_t)sn::kSmallBytes ? (size_t)wmax * sizeof(T) : 0; };
-    capture_graph(sn_solve_graph_, stream_, [&] {
-      for (int l = 0; l < S.levels; ++l) {
-        const int r0 = S.lrptr[l], nr = S.lrptr[l + 1] - r0, k0 = S.lptr[l], ns = S.lptr[l + 1] - k0;
-        sn::sn_gather_kernel<T><<<(int)std::min<int64_t>((nr + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid), kBlock, 0, stream_>>>(
-            a, sn_lrows_.p + r0, nr);
-        ++nodes;
-        if (nr > ns) {   // some supernode of the level is wider than one column
-          int wmax = 1;
-          for (int k = k0; k < k0 + ns; ++k) wmax = std::max(wmax, S.width(S.lcols[k]));
-          const size_t sm = vec_smem(wmax);
-          sn::sn_fdiag_kernel<T><<<std::min(ns, kMaxGrid), kBlock, sm, stream_>>>(a, sn_lcols_.p + k0, ns, sm > 0);
-          ++nodes;
-        }
-      }
-      for (size_t l = 0; l + 1 < S.bptr.size(); ++l) {
-        const int k0 = S.bptr[l], ns = S.bptr[l + 1] - k0;
-        int wmax = 1;
-        for (int k = k0; k < k0 + ns; ++k) wmax = std::max(wmax, S.width(S.bcols[k]));
-        const size_t sm = vec_smem(wmax);
-        sn::sn_backward_kernel<T><<<std::min(ns, kMaxGrid), kBlock, sm, stream_>>>(a, sn_bcols_.p + k0, ns, sm > 0);
-        ++nodes;
-      }
-    });
-    sn_solve_nodes_ = nodes;
-  }
-  CUDA_TRY(cudaGraphLaunch(sn_solve_graph_, stream_));
-  launches_ += sn_solve_nodes_;
-}
-
-template <typename T>
-void Engine<T>::ldl_sn_stats(int64_t* o) {
-  o[0] = sn_.ns; o[1] = sn_.max_width; o[2] = sn_.zeros(); o[3] = sn_.levels;
-  o[4] = sn_ready_ ? sn_small_count_ : 0; o[5] = sn_ready_ ? sn_tiled_count_ : 0; o[6] = sn_solve_nodes_;
-  o[7] = (int64_t)sn_.update_flops;
-}
-
 template <typename T>
 void Engine<T>::residuals(const void* x, const void* s, const void* mu, int ignore_scaling, double* out) {
   CUDA_TRY(cudaSetDevice(device_));
@@ -3353,18 +2958,10 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
     pol_mu_.alloc(std::max(m, 1)); pol_rho_.alloc(std::max(m, 1));
     pol_kind_.alloc(std::max(m, 1)); pol_cnt_.alloc(POLISH_CNT_COUNT); pol_nq_.alloc(std::max(n, 1));
   }
-  // the solve's rho vector and sigma come back whatever happens below; the factor then follows them again
-  const double sigma0 = st_.sigma;
+  // the solve's rho vector comes back whatever happens below; the factor then follows it and the solve's sigma again
   CUDA_TRY(cudaMemcpyAsync(pol_rho_.p, rho_vec_.p, m * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-  auto set_factor_values = [&](double sigma) {
-    st_.sigma = sigma;   // baked into the captured factor graphs
-    destroy_ldl_factor_graph();
-    sn_factor_graph_.reset();
-    ldl_dirty_ = true;
-    sn_dirty_ = true;
-  };
   auto restore = [&] {
-    set_factor_values(sigma0);
+    invalidate_factors();
     CUDA_TRY(cudaMemcpyAsync(rho_vec_.p, pol_rho_.p, m * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
   };
   bool polished = false;
@@ -3378,10 +2975,9 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
     check_launch("polish_classify");
     int cnt[POLISH_CNT_COUNT] = {0, 0, 0, 0};
     CUDA_TRY(cudaMemcpyAsync(cnt, pol_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
-    set_factor_values(p.delta);
     bool factored = true;
     try {
-      direct_factor();
+      direct_plugin()->factor(p.delta);
     } catch (const EngineError& e) {
       if (e.code == COSMO_B200_ERR_CUDA) throw;
       factored = false;   // zero or non-finite pivots, or the wrong inertia: not an error, the polish is rejected
@@ -3389,19 +2985,8 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
     out[0] = 0.0;
     out[1] = cnt[POLISH_CNT_LOWER]; out[2] = cnt[POLISH_CNT_UPPER]; out[3] = cnt[POLISH_CNT_EQ];
     if (factored) {
-      auto plugin_solve = [&] {   // [xsol_; nu_] = K~ \ ls_
-        if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_solve();
-        else sn_solve();
-      };
-      for (int k = 0; k <= p.refine_iter; ++k) {
-        if (k > 0) polish_residual(pol_zx_.p, pol_znu_.p, pol_nq_.p, pol_rhs_.p, nullptr);
-        plugin_solve();
-        polish_update_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, xsol_.p, nu_.p, pol_zx_.p,
-                                                                                  pol_znu_.p, k == 0 ? 1 : 0);
-        check_launch("polish_update");
-      }
       double rmax[2];
-      polish_residual(pol_zx_.p, pol_znu_.p, pol_nq_.p, pol_rhs_.p, rmax);
+      refine_with_factor(pol_zx_.p, pol_znu_.p, pol_nq_.p, pol_rhs_.p, p.refine_iter, rmax);
       // the candidate: x_p, s_p = Pi_K(b - A x_p), mu_p = the clipped -nu
       launch_spmv(A_, pol_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m, EpiPolishSlack<T>{nullptr, pol_w_.p + n, b_.p},
                   red(SC_TMP6), "spmv_polish_slack");
@@ -3429,7 +3014,20 @@ void Engine<T>::polish(const cosmo_b200_polish_settings* ps, double* x, double* 
   sync();
   // restore() marked the factor dirty but did not refactor: it still holds this polish's K~ for the adjoint
   pol_rec_status_ = polished ? 1 : 0;
-  pol_rec_factors_ = direct_factorizations();
+  pol_rec_factors_ = direct_plugin()->factorizations();
+}
+
+template <typename T>
+void Engine<T>::refine_with_factor(T* zx, T* znu, const T* rx, const T* rs, int refine_iter, double* max2) {
+  DirectPlugin<T>* d = direct_plugin();
+  for (int k = 0; k <= refine_iter; ++k) {
+    if (k > 0) polish_residual(zx, znu, rx, rs, nullptr);
+    d->solve(st_.sigma, true);   // [xsol_; nu_] = K~ \ ls_
+    polish_update_kernel<T><<<vgrid((long long)n_ + m_), kBlock, 0, stream_>>>(n_, m_, pol_kind_.p, xsol_.p, nu_.p, zx, znu,
+                                                                                k == 0 ? 1 : 0);
+    check_launch("polish_update");
+  }
+  polish_residual(zx, znu, rx, rs, max2);
 }
 
 // Derivatives of the polished solution (DESIGN.md §3j, adjoint.cuh): the right-hand side from the incoming gradients,
@@ -3445,7 +3043,7 @@ void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, con
     throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "adjoint: needs a direct KKT plugin (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver)"};
   if (pol_rec_status_ == kNoPolishRecord)
     throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: no polish since the last solve, update, reset or warm start"};
-  if (pol_rec_status_ == 1 && pol_rec_factors_ != direct_factorizations())
+  if (pol_rec_status_ == 1 && pol_rec_factors_ != direct_plugin()->factorizations())
     throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: the factor of the last polish has been replaced"};
   const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
   const int n = n_, m = m_;
@@ -3476,16 +3074,8 @@ void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, con
   launch_spmv(At_, adj_gs_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n, EpiAdjointRhsX<T>{nullptr, adj_rx_.p, ls_.p, din[0], D},
               red(SC_TMP6), "spmv_adjoint_rhs_x");
   // the first solve from z = 0, then refine_iter steps against the exact K_A, v masked off the active rows
-  for (int k = 0; k <= refine_iter; ++k) {
-    if (k > 0) polish_residual(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, nullptr);
-    if (st_.kkt_solver == COSMO_B200_KKT_LDL) ldl_solve(true);
-    else sn_solve(true);
-    polish_update_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, xsol_.p, nu_.p, adj_zx_.p,
-                                                                              adj_zv_.p, k == 0 ? 1 : 0);
-    check_launch("polish_update");
-  }
   double rmax[2];
-  polish_residual(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, rmax);
+  refine_with_factor(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, refine_iter, rmax);
   // gradients
   CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
   AdjointVecArgs<T> a;

@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 #include <stdio.h>
 
+#include <chrono>
 #include <string>
 #include <utility>
 #include <vector>
@@ -14,6 +15,10 @@
 #include "../../include/cosmo_b200.h"
 
 namespace cosmo {
+
+inline double now_s() {
+  return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
 
 struct EngineError {
   int code;
@@ -119,16 +124,20 @@ void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cu
   CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
 }
 
-// Stream-capture what `launches()` enqueues on `st` into `out`.
+// Stream-capture what `launches()` enqueues on `st` into `out`; returns the number of nodes (launches, copies, memsets)
+// the graph holds.
 template <typename F>
-void capture_graph(GraphExec& out, cudaStream_t st, F&& launches) {
+size_t capture_graph(GraphExec& out, cudaStream_t st, F&& launches) {
   out.reset();
   cudaGraph_t graph = nullptr;
   CUDA_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   launches();
   CUDA_TRY(cudaStreamEndCapture(st, &graph));
+  size_t nodes = 0;
+  CUDA_TRY(cudaGraphGetNodes(graph, nullptr, &nodes));
   CUDA_TRY(cudaGraphInstantiate(&out.g, graph, 0));
   CUDA_TRY(cudaGraphDestroy(graph));
+  return nodes;
 }
 
 }  // namespace cosmo

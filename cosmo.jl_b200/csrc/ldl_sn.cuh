@@ -363,5 +363,176 @@ __global__ void __launch_bounds__(kBlock) sn_backward_kernel(SolveArgs<T> a, con
   }
 }
 
+// tiles (bi >= bj) of a rows x cols panel, kTile square
+inline int lower_tile_count(int64_t rows, int64_t cols) {
+  const int64_t nrt = (rows + kTile - 1) / kTile, nct = (cols + kTile - 1) / kTile;
+  int64_t t = 0;
+  for (int64_t bj = 0; bj < nct; ++bj) t += nrt - bj;
+  return (int)t;
+}
+
 }  // namespace sn
+
+// The supernodal plugin (DESIGN §3c′): the analysis of ldl_sn_symbolic.h, the choice of path per supernode, the factor
+// by supernodal level and the solves by level and depth.
+template <typename T>
+class SnPlugin : public DirectPlugin<T> {
+ public:
+  explicit SnPlugin(const DirectWiring<T>& w) : DirectPlugin<T>(w, "supernodal LDL'", "supernodal LDL'") {}
+
+  // cosmo_b200_ldl_sn_stats
+  void sn_stats(int64_t* o) const {
+    o[0] = S_.ns; o[1] = S_.max_width; o[2] = S_.zeros(); o[3] = S_.levels;
+    o[4] = this->ready_ ? small_count_ : 0; o[5] = this->ready_ ? tiled_count_ : 0; o[6] = this->solve_nodes_;
+    o[7] = (int64_t)S_.update_flops;
+  }
+
+ private:
+  using DirectPlugin<T>::w_;
+  struct Big { int s; int64_t groups, chunk; };
+  struct Level { int small0 = 0, small1 = 0; size_t smem = 0; std::vector<Big> big; };
+
+  void build(const std::vector<int>& Prow, const std::vector<int>& Pcol, const std::vector<int>& Arow,
+             const std::vector<int>& Acol, double t0) override {
+    ldl_sn::Symbolic& S = S_;
+    ldl_sn::analyze(w_.n, w_.m, Prow, Pcol, Arow, Acol, S);
+    this->symbolic_s_ = now_s() - t0;
+    cudaStream_t st = w_.stream;
+    const size_t ts = sizeof(T);
+    // path per supernode: the small path when the panel and its relative rows fit one CTA's shared memory; the tiled
+    // path's descendant updates split into groups of about kUpdatesPerGroup, the partial sums capped at 256 MB
+    constexpr int64_t kUpdatesPerGroup = 16;
+    levels_.assign(S.levels, Level());
+    std::vector<int> small;
+    int64_t part = 0;
+    small_count_ = tiled_count_ = 0;
+    for (int l = 0; l < S.levels; ++l) {
+      Level& L = levels_[l];
+      L.small0 = (int)small.size();
+      for (int k = S.lptr[l]; k < S.lptr[l + 1]; ++k) {
+        const int s = S.lcols[k];
+        const int64_t h = S.height(s), w = S.width(s);
+        const size_t bytes = (size_t)(h * w) * ts + (size_t)h * sizeof(int);
+        if (bytes <= (size_t)sn::kSmallBytes) {
+          small.push_back(s);
+          L.smem = std::max(L.smem, bytes);
+          ++small_count_;
+        } else {
+          const int64_t nu = S.uptr[s + 1] - S.uptr[s];
+          int64_t g = std::max<int64_t>(1, (nu + kUpdatesPerGroup - 1) / kUpdatesPerGroup);
+          g = std::max<int64_t>(1, std::min<int64_t>(g, (int64_t)((256u << 20) / (h * w * ts))));
+          const int64_t chunk = std::max<int64_t>(1, (nu + g - 1) / g);
+          g = std::max<int64_t>(1, (nu + chunk - 1) / chunk);
+          L.big.push_back(Big{s, g, chunk});
+          if (nu) part = std::max(part, g * h * w);
+          ++tiled_count_;
+        }
+      }
+      L.small1 = (int)small.size();
+    }
+    const int64_t N = S.N, entries = S.off.empty() ? 0 : S.off.back();
+    const double need = (double)entries * ts + (double)part * ts + (double)S.rows.size() * 4 + (double)S.Kpos.size() * 16 +
+                        (double)S.Ksrc.size() * 8 + (double)S.ud.size() * 12 + (double)S.gd.size() * 8 + (double)N * (3 * ts + 24);
+    this->fit(need, std::to_string((long long)S.stored) + " stored entries need");
+    sptr_.upload(S.sptr, st); rptr_.upload(S.rptr, st); rows_.upload(S.rows, st); off_.upload(S.off, st);
+    uptr_.upload(S.uptr, st); ud_.upload(S.ud, st); up0_.upload(S.up0, st); up1_.upload(S.up1, st);
+    Ksp_.upload(S.Ksp, st); Ksrc_.upload(S.Ksrc, st); Kpos_.upload(S.Kpos, st);
+    gptr_.upload(S.gptr, st); gd_.upload(S.gd, st); gi_.upload(S.gi, st);
+    perm_.upload(S.perm, st); small_.upload(small, st);
+    lrows_.upload(S.lrows, st); lcols_.upload(S.lcols, st); bcols_.upload(S.bcols, st);
+    Lx_.alloc(std::max<int64_t>(entries, 1), false);
+    part_.alloc(std::max<int64_t>(part, 1), false);
+    D_.alloc(std::max<int64_t>(N, 1)); Dinv_.alloc(std::max<int64_t>(N, 1)); y_.alloc(std::max<int64_t>(N, 1));
+    this->sync();
+    CUDA_TRY(cudaFuncSetAttribute(sn::sn_small_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
+    CUDA_TRY(cudaFuncSetAttribute(sn::sn_fdiag_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
+    CUDA_TRY(cudaFuncSetAttribute(sn::sn_backward_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sn::kSmallBytes));
+  }
+
+  // memset and assembly of the panels, then level by level the small supernodes in one launch and each tiled one in
+  // its own sequence of launches
+  void capture_factor(T sigma) override {
+    const ldl_sn::Symbolic& S = S_;
+    cudaStream_t st = w_.stream;
+    sn::Args<T> a;
+    a.sptr = sptr_.p; a.rptr = rptr_.p; a.rows = rows_.p; a.off = off_.p;
+    a.uptr = uptr_.p; a.ud = ud_.p; a.up0 = up0_.p; a.up1 = up1_.p;
+    a.Lx = Lx_.p; a.D = D_.p; a.Dinv = Dinv_.p; a.flags = this->flags_.p;
+    const int64_t entries = S.off.empty() ? 0 : S.off.back();
+    if (entries) CUDA_TRY(cudaMemsetAsync(Lx_.p, 0, entries * sizeof(T), st));
+    if (S.nnz_K)
+      sn::sn_assemble_kernel<T><<<vgrid(S.nnz_K), kBlock, 0, st>>>(S.nnz_K, Ksp_.p, Ksrc_.p, Kpos_.p, w_.P.val, w_.At.val,
+                                                                   w_.rho, sigma, Lx_.p);
+    for (const Level& L : levels_) {
+      if (L.small1 > L.small0) {
+        const int cnt = L.small1 - L.small0;
+        sn::sn_small_kernel<T><<<std::min(cnt, kMaxGrid), kBlock, L.smem, st>>>(a, small_.p + L.small0, cnt);
+      }
+      for (const Big& B : L.big) {
+        const int s = B.s, c0 = S.sptr[s], w = S.width(s), h = S.height(s);
+        T* F = Lx_.p + S.off[s];
+        const int64_t u0 = S.uptr[s], u1 = S.uptr[s + 1];
+        if (u1 > u0) {
+          sn::sn_tile_update_kernel<T><<<dim3(sn::lower_tile_count(h, w), (unsigned)B.groups), kBlock, 0, st>>>(
+              a, c0, w, h, rows_.p + S.rptr[s], u0, u1, B.chunk, part_.p);
+          sn::sn_tile_reduce_kernel<T><<<vgrid((int64_t)h * w), kBlock, 0, st>>>(F, part_.p, (int)B.groups, h, w);
+        }
+        for (int b0 = 0; b0 < w; b0 += sn::kTile) {
+          const int nb = std::min(sn::kTile, w - b0), b1 = b0 + nb;
+          const int rows = h - b1;
+          sn::sn_diag_kernel<T><<<1, kBlock, 0, st>>>(a, F, c0, h, b0, nb);
+          if (rows > 0)
+            sn::sn_panel_kernel<T><<<(rows + sn::kPanelThreads - 1) / sn::kPanelThreads, sn::kPanelThreads, 0, st>>>(
+                F, h, b0, nb);
+          if (b1 < w)
+            sn::sn_trail_kernel<T><<<sn::lower_tile_count(h - b1, w - b1), kBlock, 0, st>>>(F, D_.p + c0 + b0, h, w, b0, b1);
+        }
+      }
+    }
+  }
+
+  // the forward solve by supernodal level, the backward solve by depth
+  void capture_solve() override {
+    const ldl_sn::Symbolic& S = S_;
+    cudaStream_t st = w_.stream;
+    sn::SolveArgs<T> a;
+    a.sptr = sptr_.p; a.rptr = rptr_.p; a.rows = rows_.p; a.off = off_.p;
+    a.gptr = gptr_.p; a.gd = gd_.p; a.gi = gi_.p;
+    a.Lx = Lx_.p; a.Dinv = Dinv_.p; a.perm = perm_.p;
+    a.rhs = w_.rhs; a.y = y_.p; a.out1 = w_.y1; a.out2 = w_.y2; a.n = w_.n;
+    // the diagonal solves keep their part of y in shared memory up to kSmallBytes, wider supernodes work on y in place
+    auto vec_smem = [&](int wmax) { return (size_t)wmax * sizeof(T) <= (size_t)sn::kSmallBytes ? (size_t)wmax * sizeof(T) : 0; };
+    for (int l = 0; l < S.levels; ++l) {
+      const int r0 = S.lrptr[l], nr = S.lrptr[l + 1] - r0, k0 = S.lptr[l], ns = S.lptr[l + 1] - k0;
+      sn::sn_gather_kernel<T><<<(int)std::min<int64_t>((nr + kWarpsPerBlock - 1) / kWarpsPerBlock, kMaxGrid), kBlock, 0, st>>>(
+          a, lrows_.p + r0, nr);
+      if (nr > ns) {   // some supernode of the level is wider than one column
+        int wmax = 1;
+        for (int k = k0; k < k0 + ns; ++k) wmax = std::max(wmax, S.width(S.lcols[k]));
+        const size_t sm = vec_smem(wmax);
+        sn::sn_fdiag_kernel<T><<<std::min(ns, kMaxGrid), kBlock, sm, st>>>(a, lcols_.p + k0, ns, sm > 0);
+      }
+    }
+    for (size_t l = 0; l + 1 < S.bptr.size(); ++l) {
+      const int k0 = S.bptr[l], ns = S.bptr[l + 1] - k0;
+      int wmax = 1;
+      for (int k = k0; k < k0 + ns; ++k) wmax = std::max(wmax, S.width(S.bcols[k]));
+      const size_t sm = vec_smem(wmax);
+      sn::sn_backward_kernel<T><<<std::min(ns, kMaxGrid), kBlock, sm, st>>>(a, bcols_.p + k0, ns, sm > 0);
+    }
+  }
+
+  // stored entries (explicit zeros included), supernodal levels
+  void stats_row(double* o) const override {
+    o[0] = S_.N; o[1] = (double)S_.nnz_K; o[2] = (double)S_.stored; o[3] = S_.levels;
+  }
+
+  ldl_sn::Symbolic S_;   // the analysis; the graphs are built from it
+  std::vector<Level> levels_;
+  int small_count_ = 0, tiled_count_ = 0;
+  DevBuf<int64_t> rptr_, off_, uptr_, Ksp_, Ksrc_, Kpos_, gptr_;
+  DevBuf<int> sptr_, rows_, ud_, up0_, up1_, gd_, gi_, perm_, small_, lrows_, lcols_, bcols_;
+  DevBuf<T> Lx_, D_, Dinv_, part_, y_;
+};
+
 }  // namespace cosmo
