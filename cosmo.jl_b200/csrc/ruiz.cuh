@@ -103,7 +103,11 @@ __global__ void __launch_bounds__(kBlock) ruiz_rectify_kernel(const int* __restr
   }
 }
 
-// val[k] *= scal * wrow[r] * wcol[col[k]]   (plain CSR copy)
+// val[k] *= scal * (wrow[r] * wcol[col[k]])   (plain CSR copy)
+// The product wrow[r] * wcol[col[k]] is taken first: for P (both triangles stored, wrow = wcol = D) it is D_i D_j on
+// both sides of the diagonal, bit for bit, so the scaled P is exactly symmetric, as the reference makes it with
+// symmetrize_full! (scaling.jl:99).  Scaling (scal * D_i) first would round P_ij and P_ji differently.  Without scal the
+// factor is exactly 1 and A, A' get E_i D_j.
 template <typename T>
 __global__ void __launch_bounds__(kBlock) ruiz_apply_csr_kernel(int nrows, const int* __restrict__ rowptr, const int* __restrict__ col,
                                                                 T* __restrict__ val, const T* __restrict__ wrow,
@@ -113,8 +117,8 @@ __global__ void __launch_bounds__(kBlock) ruiz_apply_csr_kernel(int nrows, const
   const T sc = scal ? *scal : T(1);
   for (int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < nrows; r += warps) {
     const int s = rowptr[r], e = rowptr[r + 1];
-    const T wr = sc * wrow[r];
-    for (int k = s + lane; k < e; k += 32) val[k] *= wr * wcol[col[k]];
+    const T wr = wrow[r];
+    for (int k = s + lane; k < e; k += 32) val[k] *= sc * (wr * wcol[col[k]]);
   }
 }
 

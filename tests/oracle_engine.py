@@ -3,8 +3,8 @@
 It exists to exercise, without a GPU, the Python side of everything that normally talks to the CUDA engine: the host
 glue of Model (scaling, decomposition, warm starts) and the bodies of the GPU tests themselves (so a typo in a GPU
 test is found by the CPU run, not at the next GPU run).  It implements the part of the call surface those users need:
-ctor, update_settings, warm_start, update_qb, project, project_jacobian, solve, w, rho_vec, scaling, close, and the infeasibility hooks
-infeasibility_test and psd_lambda_max."""
+ctor, update_settings, warm_start, update_qb, update_matrices, project, project_jacobian, solve, w, rho_vec, scaling,
+spmv, residuals, close, and the infeasibility hooks infeasibility_test and psd_lambda_max."""
 import numpy as np
 import scipy.sparse as sp
 
@@ -42,6 +42,7 @@ class OracleEngine:
 
     def __init__(self, P, q, A, b, sets, settings=None, D=None, E=None, c=1.0, dtype=np.float64, device=0, julia_indexing=True,
                  equilibrate=False):
+        self._args = (P, q, A, b, sets, settings, D, E, c, dtype, device, julia_indexing, equilibrate)
         self.P, self.q = sp.csc_matrix(P), np.array(q, dtype=float)
         self.A, self.b = sp.csc_matrix(A), np.array(b, dtype=float)
         self.m, self.n = self.A.shape
@@ -52,9 +53,11 @@ class OracleEngine:
         self._scal = (np.ones(self.n), np.ones(self.m), 1.0) if D is None else (np.array(D), np.array(E), float(c))
         if equilibrate and D is None and settings is not None and settings.scaling != 0:
             # like the engine: unscaled data + scaling requested -> equilibrate here (scale_ruiz!)
-            ost = O.Settings(scaling=int(settings.scaling), MIN_SCALING=settings.MIN_SCALING)
+            ost = O.Settings(scaling=int(settings.scaling), MIN_SCALING=settings.MIN_SCALING, MAX_SCALING=settings.MAX_SCALING)
             Ps, qs, As, bs, cones, sm = O.scale_ruiz(self.P, self.q, self.A, self.b, self.cones, ost)
-            self.P, self.q, self.A, self.b, self.cones = sp.csc_matrix(Ps), qs, sp.csc_matrix(As), bs, cones
+            Ps = sp.csc_matrix(Ps)
+            Ps = sp.csc_matrix((Ps + Ps.T) / 2)      # symmetrize_full!, scaling.jl:99
+            self.P, self.q, self.A, self.b, self.cones = Ps, qs, sp.csc_matrix(As), bs, cones
             self._scal = (sm.D, sm.E, sm.c)
             self.scaled = True
         self._w = self._rho = self._warm = None
@@ -77,6 +80,34 @@ class OracleEngine:
             self.q = np.array(q, dtype=float)
         if b is not None:
             self.b = np.array(b, dtype=float)
+
+    def update_matrices(self, Px=None, Ax=None, q=None, b=None):
+        """new values on the pattern of create: the stand-in is rebuilt from the new unscaled data"""
+        P, q0, A, b0, *rest = self._args
+        P, A = sp.csc_matrix(P, copy=True), sp.csc_matrix(A, copy=True)
+        P.sort_indices()
+        A.sort_indices()
+        if Px is not None:
+            P.data = np.array(Px, dtype=float)
+        if Ax is not None:
+            A.data = np.array(Ax, dtype=float)
+        OracleEngine.instances.remove(self)
+        self.__init__(P, q0 if q is None else q, A, b0 if b is None else b, *rest)
+
+    def spmv(self, which, x):
+        x = np.asarray(x, dtype=float)
+        M = {0: self.A, 1: self.A.T, 2: self.P}[which]
+        return (M @ x).astype(self.dtype)
+
+    def residuals(self, x, s, mu, ignore_scaling=False):
+        """(r_prim, r_dual, max_norm_prim, max_norm_dual, cost) of the resident (scaled) data, unscaled unless
+        ignore_scaling, as cosmo_b200_residuals"""
+        x, s, mu = (np.asarray(v, dtype=float) for v in (x, s, mu))
+        D, Em, c = self._scal if not ignore_scaling else (np.ones(self.n), np.ones(self.m), 1.0)
+        Ax, Px, Aty = self.A @ x, self.P @ x, self.A.T @ mu
+        nrm = lambda v: float(np.max(np.abs(v))) if v.size else 0.0
+        return (nrm((Ax + s - self.b) / Em), nrm((Px + self.q - Aty) / D / c), max(nrm(Ax / Em), nrm(s / Em), nrm(self.b / Em)),
+                max(nrm(Px / D / c), nrm(Aty / D / c), nrm(self.q / D / c)), (0.5 * x @ Px + self.q @ x) / self._scal[2])
 
     def project(self, ws):
         out = np.array(ws, dtype=float).copy()
@@ -172,6 +203,14 @@ class OracleEngine:
         return self._w
 
     def rho_vec(self):
+        if self._rho is None and self.st is not None:     # before a solve: set_rho_vec! on the resident data
+            ost = O.Settings(rho=self.st.rho, RHO_MIN=self.st.RHO_MIN, RHO_TOL=self.st.RHO_TOL,
+                             RHO_EQ_OVER_RHO_INEQ=self.st.RHO_EQ_OVER_RHO_INEQ, COSMO_INFTY=self.st.COSMO_INFTY,
+                             MIN_SCALING=self.st.MIN_SCALING)
+            O.classify_constraints(self.cones, self.b, ost)
+            rv = np.full(self.m, ost.rho)
+            O.apply_constraint_rho_scaling(rv, self.cones, ost)
+            return rv.astype(self.dtype)
         return self._rho
 
     def close(self):

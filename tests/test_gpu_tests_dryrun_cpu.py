@@ -1,7 +1,7 @@
 """Dry run of GPU test bodies on the CPU: the CUDA engine is replaced by the oracle-backed stand-in of
 tests/oracle_engine.py and the functions of tests/test_gpu_parity.py, tests/test_gpu_float32.py and
-tests/test_gpu_scale_edges.py, tests/test_gpu_infeasibility.py and tests/test_gpu_projection_jacobian.py are called
-directly.  What this checks is the
+tests/test_gpu_scale_edges.py, tests/test_gpu_infeasibility.py, tests/test_gpu_projection_jacobian.py and
+tests/test_gpu_ruiz.py are called directly.  What this checks is the
 Python side of those tests (imports, helpers, fixtures, the host glue they drive) -- a NameError in a GPU test would
 otherwise only show up on the next GPU run.  Assertion failures are tolerated where the stand-in legitimately differs
 from the engine (it ignores the D/E unscaling of the termination test); every other exception fails the test."""
@@ -45,7 +45,12 @@ CASES = ["test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_t
          "test_gpu_projection_jacobian::test_psd_sweep_float32", "test_gpu_projection_jacobian::test_soc_sweep",
          "test_gpu_projection_jacobian::test_rows_bit_exact", "test_gpu_projection_jacobian::test_properties_per_path",
          "test_gpu_projection_jacobian::test_scale_ladder", "test_gpu_projection_jacobian::test_path_boundary_96_97",
-         "test_gpu_projection_jacobian::test_kink_counts"]
+         "test_gpu_projection_jacobian::test_kink_counts",
+         "test_gpu_ruiz::test_clip_edges_at_the_first_pass", "test_gpu_ruiz::test_zero_rows_and_columns_keep_the_scale_one",
+         "test_gpu_ruiz::test_cost_scaling_guard", "test_gpu_ruiz::test_dynamic_range_clips_in_every_pass",
+         "test_gpu_ruiz::test_every_rectified_family", "test_gpu_ruiz::test_box_bounds_and_row_classes",
+         "test_gpu_ruiz::test_long_rows_and_n_above_1024", "test_gpu_ruiz::test_wide_qp_slabs_hold_the_scaled_values",
+         "test_gpu_ruiz::test_scaled_P_is_symmetric", "test_gpu_ruiz::test_update_matrices_reproduces_a_fresh_engine"]
 MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_through_the_clique_batch",
              "test_project_exp_pow_cones", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
              "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_project_psd_small_batch_float32",
@@ -56,7 +61,11 @@ MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_s
              "test_gpu_infeasibility::test_composite_bitmask_names_exactly_the_failing_family",
              "test_gpu_projection_jacobian::test_psd_size_and_spectrum_sweep",
              "test_gpu_projection_jacobian::test_soc_sweep", "test_gpu_projection_jacobian::test_rows_bit_exact",
-             "test_gpu_projection_jacobian::test_kink_counts"}
+             "test_gpu_projection_jacobian::test_kink_counts",
+             "test_gpu_ruiz::test_clip_edges_at_the_first_pass", "test_gpu_ruiz::test_zero_rows_and_columns_keep_the_scale_one",
+             "test_gpu_ruiz::test_cost_scaling_guard", "test_gpu_ruiz::test_scaled_P_is_symmetric",
+             "test_gpu_ruiz::test_every_rectified_family",
+             "test_gpu_ruiz::test_update_matrices_reproduces_a_fresh_engine"}
 
 
 def _calls(fn):
