@@ -2,7 +2,8 @@
 
 ``solve_qp(engine, Px, q, Ax, b)`` puts new values of P, q, A and b into a live engine (``Engine.update_matrices``),
 solves, polishes and returns the polished unscaled solution ``(x, y, s)`` as CUDA tensors; its backward pass is one
-``Engine.adjoint`` into CUDA tensors.  Nothing leaves the device.
+``Engine.adjoint`` and its forward-mode product (``torch.autograd.forward_ad``, ``gradcheck(check_forward_ad=True)``)
+one ``Engine.derivative``, both into CUDA tensors.  Nothing leaves the device.
 
 The engine is created by the caller with a direct KKT solver (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver), on the
 pattern of P and A, without host scaling (scaling 0, or ``equilibrate=True``), so that ``update_matrices`` takes the
@@ -11,10 +12,11 @@ the engine's dtype.  The Box bounds are not inputs of ``update_matrices`` and ge
 returns them).  The derivative is that of the polished solution map on its active set: exact where the active set is
 stable, one-sided at weakly active rows.
 
-The backward pass reads the point and the factor the engine keeps from the last polish.  When the engine has run
-another ``solve_qp`` since this pass's forward (as ``torch.autograd.gradcheck`` does between them), the backward pass
-first solves and polishes this pass's data again; the solve is deterministic, so it differentiates the same point.
-Between a forward pass and its backward pass the engine must not be used other than through ``solve_qp``.
+The backward pass and the forward-mode product read the point and the factor the engine keeps from the last polish.
+When the engine has run another ``solve_qp`` since this pass's forward (as ``torch.autograd.gradcheck`` does between
+them), they first solve and polish this pass's data again; the solve is deterministic, so they differentiate the same
+point.  Between a forward pass and its backward pass (or its forward-mode product) the engine must not be used other
+than through ``solve_qp``.
 
 ``solve_conic(engine, Px, q, Ax, b)`` does the same for any solve the fixed-point derivatives cover, without a polish:
 its backward pass is one ``Engine.solve_adjoint`` and its forward-mode product (``torch.autograd.forward_ad``,
@@ -50,7 +52,24 @@ class _SolveQP(torch.autograd.Function):
         ctx.engine, ctx.refine_iter, ctx.device, ctx.call = engine, refine_iter, q.device, engine._solve_qp_call
         ctx.dtypes = (Px.dtype, q.dtype, Ax.dtype, b.dtype)
         ctx.save_for_backward(Px, q, Ax, b)
+        ctx.save_for_forward(Px, q, Ax, b)
         return x, y, s
+
+    @staticmethod
+    def jvp(ctx, _engine, _refine_iter, tPx, tq, tAx, tb):
+        eng = ctx.engine
+        dev = ctx.device
+        if eng._solve_qp_call != ctx.call:   # the engine has polished other data since: this pass's point again
+            _solve_and_polish(eng, *ctx.saved_tensors)
+            ctx.call = eng._solve_qp_call
+        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
+        f64 = dict(dtype=torch.float64, device=dev)
+        dx, dy, ds = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64), torch.empty(eng.m, **f64)
+        d = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (tPx, tq, tAx, tb)]
+        _, st = eng.derivative(d[0], d[1], d[2], d[3], refine_iter=ctx.refine_iter, dx=dx, dy=dy, ds=ds)
+        if st["status"] != 1:
+            raise EngineError(st["status"], "solve_qp: the derivative did not apply (status %d)" % st["status"])
+        return dx, dy, ds
 
     @staticmethod
     def backward(ctx, gx, gy, gs):

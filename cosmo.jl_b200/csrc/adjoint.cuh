@@ -51,6 +51,26 @@ struct EpiAdjointRhsX {
   __device__ void operator()(T*) const {}
 };
 
+// Adds the block's active rows and its weakly active ones (lower- or upper-active rows whose clipped multiplier is 0:
+// the derivative there is one-sided) to counts, for row r of the polish (r outside 0 .. m: none).  Every thread of the
+// block calls it once per round (__syncthreads_count).
+template <typename T>
+__device__ __forceinline__ void adj_count_rows(int r, int m, const unsigned char* __restrict__ kind,
+                                               const T* __restrict__ mu_p, int* __restrict__ counts) {
+  bool active = false, weak = false;
+  if (r >= 0 && r < m) {
+    const unsigned char kd = kind[r];
+    active = kd != POLISH_INACTIVE;
+    weak = (kd == POLISH_LOWER || kd == POLISH_UPPER) && mu_p[r] == T(0);
+  }
+  const int na = __syncthreads_count(active);
+  const int nw = __syncthreads_count(weak);
+  if (threadIdx.x == 0) {
+    if (na) atomicAdd(counts + ADJ_CNT_ACTIVE, na);
+    if (nw) atomicAdd(counts + ADJ_CNT_WEAK, nw);
+  }
+}
+
 template <typename T>
 struct AdjointVecArgs {
   int n, m;
@@ -80,7 +100,6 @@ __global__ void __launch_bounds__(kBlock) adjoint_grad_vec_kernel(AdjointVecArgs
   // every thread of the block runs the same number of rounds (__syncthreads_count below)
   const int rounds = (total + stride - 1) / stride;
   for (int k = 0, idx = blockIdx.x * blockDim.x + threadIdx.x; k < rounds; ++k, idx += stride) {
-    bool active = false, weak = false;
     if (idx < a.n) {
       if (a.dq) a.dq[idx] = -(a.D ? a.c * (double)a.D[idx] : a.c) * (double)a.u[idx];
     } else if (idx < total) {
@@ -97,15 +116,8 @@ __global__ void __launch_bounds__(kBlock) adjoint_grad_vec_kernel(AdjointVecArgs
       }
       if (a.dl) a.dl[r] = lo;
       if (a.du) a.du[r] = up;
-      active = kd != POLISH_INACTIVE;
-      weak = (kd == POLISH_LOWER || kd == POLISH_UPPER) && a.mu_p[r] == T(0);
     }
-    const int na = __syncthreads_count(active);
-    const int nw = __syncthreads_count(weak);
-    if (threadIdx.x == 0) {
-      if (na) atomicAdd(a.counts + ADJ_CNT_ACTIVE, na);
-      if (nw) atomicAdd(a.counts + ADJ_CNT_WEAK, nw);
-    }
+    adj_count_rows(idx - a.n, a.m, a.kind, a.mu_p, a.counts);
   }
 }
 
@@ -146,6 +158,81 @@ __global__ void __launch_bounds__(kBlock) adjoint_grad_A_kernel(int n, const int
       const double g = -(y * uj + (double)v[r] * xj) - (gs ? (double)gs[r] * xj : 0.0);
       dAx[k] = (E ? (double)E[r] * dj : dj) * g;
     }
+  }
+}
+
+// ---- the forward derivative (cosmo_b200_derivative, DESIGN.md §3j) -----------------------------------------------
+// The transpose of the adjoint above, with the same K_A, factor and refinement:
+//   K_A [x'; y'_A] = [-dq~ - dP~ x~ - dA~' y~; e - sbar'~ on A],   y' = 0 off A,   e = E db - dA~ x~,   s~' = e - A~ x'.
+// The x rows are sd_rhs_x_kernel's (solve_adjoint.cuh) at the polished point, s~' is one SpMV pass with
+// EpiPolishSlack; the two kernels below form the s rows and write the outputs.
+
+// s rows of the right-hand side, one warp per CSR(A) row r (map: CSR position -> CSC index of A's values):
+//   e_r = E_r db_r - (dA~ x~)_r on every row, kept in e for s~',
+//   r_s = e_r - sbar'_r on the active rows, 0 elsewhere, kept in rs and written into ls_s for the first solve,
+// with sbar' the scaled bound direction: E dl on lower-active Box rows, E du on upper-active ones, E (dl + du) / 2 on
+// Box rows with l = u (the transpose of adjoint_grad_vec_kernel's half split), 0 on ZeroSet and Nonnegatives rows.
+// dAx, db, dl, du null: zero.
+template <typename T>
+__global__ void __launch_bounds__(kBlock) derivative_rhs_s_kernel(int m, const int* __restrict__ a_rowptr, const int* __restrict__ a_col,
+                                                                  const int* __restrict__ map, const double* __restrict__ dAx,
+                                                                  const double* __restrict__ db, const double* __restrict__ dl,
+                                                                  const double* __restrict__ du, const unsigned char* __restrict__ kind,
+                                                                  const unsigned char* __restrict__ row_class,
+                                                                  const T* __restrict__ x, const T* __restrict__ D,
+                                                                  const T* __restrict__ E, T* __restrict__ e_out,
+                                                                  T* __restrict__ rs, T* __restrict__ ls_s) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < m; r += warps) {
+    const double e = E ? (double)E[r] : 1.0;
+    double acc = 0.0;
+    if (dAx)
+      for (int k = a_rowptr[r] + lane; k < a_rowptr[r + 1]; k += 32) {
+        const int j = a_col[k];
+        acc += e * (D ? (double)D[j] : 1.0) * dAx[map[k]] * (double)x[j];
+      }
+    acc = warp_sum(acc);
+    if (lane == 0) {
+      const double er = (db ? e * db[r] : 0.0) - acc;
+      const unsigned char kd = kind[r];
+      double sb = 0.0;
+      if (row_class[r] == ROW_BOX) {
+        const double lo = dl ? e * dl[r] : 0.0, up = du ? e * du[r] : 0.0;
+        if (kd == POLISH_LOWER) sb = lo;
+        else if (kd == POLISH_UPPER) sb = up;
+        else if (kd == POLISH_EQUALITY) sb = 0.5 * (lo + up);
+      }
+      const T v = kd != POLISH_INACTIVE ? (T)(er - sb) : T(0);
+      e_out[r] = (T)er;
+      rs[r] = v;
+      ls_s[r] = v;
+    }
+  }
+}
+
+// the outputs, unscaled as cosmo_b200_solution unscales the solution: dx = D x~',  dy = E y~' / c on the active rows
+// and 0 elsewhere,  ds = s~' / E; counts the rows as adjoint_grad_vec_kernel does.  One thread per entry of [x; s].
+template <typename T>
+__global__ void __launch_bounds__(kBlock) derivative_out_kernel(int n, int m, const unsigned char* __restrict__ kind,
+                                                                const T* __restrict__ mu_p, const T* __restrict__ xd,
+                                                                const T* __restrict__ yd, const T* __restrict__ sd,
+                                                                const T* __restrict__ D, const T* __restrict__ E, double c,
+                                                                double* __restrict__ dx, double* __restrict__ dy,
+                                                                double* __restrict__ ds, int* __restrict__ counts) {
+  const int total = n + m;
+  // the loop bound is the block's first index, so every thread of the block runs the same rounds (adj_count_rows)
+  for (int first = blockIdx.x * blockDim.x; first < total; first += gridDim.x * blockDim.x) {
+    const int idx = first + threadIdx.x;
+    if (idx < n) {
+      if (dx) dx[idx] = (D ? (double)D[idx] : 1.0) * (double)xd[idx];
+    } else if (idx < total) {
+      const int r = idx - n;
+      const double e = E ? (double)E[r] : 1.0;
+      if (dy) dy[r] = kind[r] != POLISH_INACTIVE ? e * (double)yd[r] / c : 0.0;
+      if (ds) ds[r] = (double)sd[r] / e;
+    }
+    adj_count_rows(idx - n, m, kind, mu_p, counts);
   }
 }
 

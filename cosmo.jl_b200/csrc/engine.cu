@@ -196,6 +196,8 @@ class EngineBase {
   virtual void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) = 0;
   virtual void adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db,
                        double* dPx, double* dAx, double* dl, double* du, double* out4) = 0;
+  virtual void derivative(int refine_iter, const double* dPx, const double* dq, const double* dAx, const double* db,
+                          const double* dl, const double* du, double* dx, double* dy, double* ds, double* out4) = 0;
   virtual void solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy,
                              const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
                              double* out8) = 0;
@@ -271,6 +273,8 @@ class Engine : public EngineBase {
   void polish(const cosmo_b200_polish_settings* ps, double* x, double* y, double* s, double* out8) override;
   void adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db, double* dPx,
                double* dAx, double* dl, double* du, double* out4) override;
+  void derivative(int refine_iter, const double* dPx, const double* dq, const double* dAx, const double* db,
+                  const double* dl, const double* du, double* dx, double* dy, double* ds, double* out4) override;
   void solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const double* dx, const double* dy, const double* ds,
                      double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double* out8) override;
   void solve_derivative(const cosmo_b200_solve_adjoint_settings* as, const double* dPx, const double* dq, const double* dAx,
@@ -361,8 +365,8 @@ class Engine : public EngineBase {
   // refine_iter + 1 solves of K~ z = r^ with the factor in memory, each followed by polish_update_kernel, with the
   // residual r^ - K_A z between them and at the end (max2 as for polish_residual)
   void refine_with_factor(T* zx, T* znu, const T* rx, const T* rs, int refine_iter, double* max2);
-  // adjoint scratch, allocated by the first adjoint and kept: its own z (pol_zx_ / pol_znu_ hold the polished point the
-  // gradients read), the kept right-hand side, gs~ and two counters
+  // adjoint scratch, allocated by the first adjoint or derivative and kept: its own z (pol_zx_ / pol_znu_ hold the
+  // polished point the gradients read), the kept right-hand side, gs~ (the derivative's e) and two counters
   DevBuf<T> adj_zx_, adj_zv_, adj_rx_, adj_rs_, adj_gs_;
   DevBuf<int> adj_cnt_;
   // fp64 caller arrays of the two adjoints: dev holds their caller_arrays bits, the inputs first, then the outputs.  Host
@@ -372,6 +376,10 @@ class Engine : public EngineBase {
                  DevBuf<double>& stage, const double** din, double** dout);
   void unstage_f64(const F64Out* outs, double* const* dout, int nout);
   void nan_f64(unsigned dev, int nin, const F64Out* outs, int nout);
+  // the two calls on the polish record (adjoint, derivative): the checks of a call, then out = {status, 0, 0, NaN}
+  // with NaN outputs and false unless the status is 1, else the scratch allocated and true
+  void adj_check(int refine_iter, const char* who);
+  bool adj_begin(unsigned dev, int nin, const F64Out* outs, int nout, double* out);
   // solve adjoint (solve_adjoint.cuh): scratch allocated by the first call and kept -- the Krylov basis with lam and gw,
   // the point w_s, two m-vectors for Dpi, the row flags, the SOC norms and x'h, the eigenpairs of the PSD cones (small
   // cones first, then large ones) and three N x N work matrices for the largest large cone, the saved plugin state, and
@@ -416,6 +424,7 @@ class Engine : public EngineBase {
   // value maps are not resident (derived once and kept)
   DevBuf<T> sd_dpi_;
   DevBuf<int> sd_amap_;
+  const int* a_value_map();
   void sd_operator(const T* v, T* out);
   void emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y, double* s);
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
@@ -3037,28 +3046,12 @@ void Engine<T>::refine_with_factor(T* zx, T* znu, const T* rx, const T* rs, int 
 template <typename T>
 void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db,
                         double* dPx, double* dAx, double* dl, double* du, double* out) {
-  if (refine_iter < 0 || refine_iter > 100) throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: refine_iter in 0 .. 100"};
-  single_gpu("adjoint");
-  if (!direct_kkt())
-    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, "adjoint: needs a direct KKT plugin (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver)"};
-  if (pol_rec_status_ == kNoPolishRecord)
-    throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: no polish since the last solve, update, reset or warm start"};
-  if (pol_rec_status_ == 1 && pol_rec_factors_ != direct_plugin()->factorizations())
-    throw EngineError{COSMO_B200_ERR_INVALID, "adjoint: the factor of the last polish has been replaced"};
+  adj_check(refine_iter, "adjoint");
   const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
   const int n = n_, m = m_;
   const long long nnzP = P_.nnz, nnzA = At_.nnz;
   const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, nnzP}, {dAx, nnzA}, {dl, m}, {du, m}};
-  out[0] = pol_rec_status_; out[1] = out[2] = 0.0; out[3] = NAN;
-  if (pol_rec_status_ != 1) {
-    nan_f64(dev, 3, outs, 6);
-    return;
-  }
-  if (!adj_cnt_.p) {
-    adj_zx_.alloc(std::max(n, 1)); adj_rx_.alloc(std::max(n, 1));
-    adj_zv_.alloc(std::max(m, 1)); adj_rs_.alloc(std::max(m, 1)); adj_gs_.alloc(std::max(m, 1));
-    adj_cnt_.alloc(ADJ_CNT_COUNT);
-  }
+  if (!adj_begin(dev, 3, outs, 6, out)) return;
   const double* ins[3] = {dx, dy, ds};
   const long long in_count[3] = {n, m, m};
   DevBuf<double> stage;
@@ -3098,6 +3091,93 @@ void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, con
   int cnt[ADJ_CNT_COUNT] = {0, 0};
   CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
   unstage_f64(outs, dout, 6);
+  if (dev) caller_written();
+  sync();
+  out[1] = cnt[ADJ_CNT_ACTIVE];
+  out[2] = cnt[ADJ_CNT_WEAK];
+  out[3] = std::max(rmax[0], rmax[1]);
+}
+
+template <typename T>
+void Engine<T>::adj_check(int refine_iter, const char* who) {
+  const std::string w(who);
+  if (refine_iter < 0 || refine_iter > 100) throw EngineError{COSMO_B200_ERR_INVALID, w + ": refine_iter in 0 .. 100"};
+  single_gpu(who);
+  if (!direct_kkt())
+    throw EngineError{COSMO_B200_ERR_UNSUPPORTED, w + ": needs a direct KKT plugin (DeviceLdlKKTSolver or DeviceSupernodalKKTSolver)"};
+  if (pol_rec_status_ == kNoPolishRecord)
+    throw EngineError{COSMO_B200_ERR_INVALID, w + ": no polish since the last solve, update, reset or warm start"};
+  if (pol_rec_status_ == 1 && pol_rec_factors_ != direct_plugin()->factorizations())
+    throw EngineError{COSMO_B200_ERR_INVALID, w + ": the factor of the last polish has been replaced"};
+}
+
+template <typename T>
+bool Engine<T>::adj_begin(unsigned dev, int nin, const F64Out* outs, int nout, double* out) {
+  out[0] = pol_rec_status_; out[1] = out[2] = 0.0; out[3] = NAN;
+  if (pol_rec_status_ != 1) {
+    nan_f64(dev, nin, outs, nout);
+    return false;
+  }
+  if (!adj_cnt_.p) {
+    const int n = n_, m = m_;
+    adj_zx_.alloc(std::max(n, 1)); adj_rx_.alloc(std::max(n, 1));
+    adj_zv_.alloc(std::max(m, 1)); adj_rs_.alloc(std::max(m, 1)); adj_gs_.alloc(std::max(m, 1));
+    adj_cnt_.alloc(ADJ_CNT_COUNT);
+  }
+  return true;
+}
+
+// The forward derivative of the polished solution along a data direction (DESIGN.md §3j, adjoint.cuh): the transpose
+// of adjoint() -- the right-hand side from the direction at the polished point, the same refine_iter + 1 solves with
+// the factor the polish left, then s~' = e - A~ x~' and the unscaled outputs.  Checks, statuses and the untouched
+// state are adjoint()'s.
+template <typename T>
+void Engine<T>::derivative(int refine_iter, const double* dPx, const double* dq, const double* dAx, const double* db,
+                           const double* dl, const double* du, double* dx, double* dy, double* ds, double* out) {
+  adj_check(refine_iter, "derivative");
+  const unsigned dev = caller_arrays({dPx, dq, dAx, db, dl, du, dx, dy, ds});
+  const int n = n_, m = m_;
+  const F64Out outs[3] = {{dx, n}, {dy, m}, {ds, m}};
+  if (!adj_begin(dev, 6, outs, 3, out)) return;
+  const double* ins[6] = {dPx, dq, dAx, db, dl, du};
+  const long long in_count[6] = {P_.nnz, n, At_.nnz, m, m, m};
+  DevBuf<double> stage;
+  const double* din[6];
+  double* dout[3];
+  stage_f64(dev, ins, in_count, 6, outs, 3, stage, din, dout);
+  const T* D = scaled_ ? D_.p : nullptr;
+  const T* Ev = scaled_ ? E_.p : nullptr;
+  const double c = scaled_ ? c_ : 1.0;
+  // x rows -dq~ - dP~ x~ - dA~' y~ at the polished point into the kept rx and ls_
+  if (din[0] && P_.nnz && !maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only
+  if (n) {
+    sd_rhs_x_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(
+        n, P_.rowptr.p, P_.col.p, P_.d_src.p, At_.rowptr.p, At_.col.p, P_.nnz ? din[0] : nullptr, din[1],
+        At_.nnz ? din[2] : nullptr, pol_zx_.p, pol_mu_.p, D, Ev, c, adj_rx_.p);
+    check_launch("sd_rhs_x");
+    CUDA_TRY(cudaMemcpyAsync(ls_.p, adj_rx_.p, n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+  }
+  // s rows on the active rows into the kept rs and ls_, e on every row into adj_gs_
+  if (m) {
+    const int* amap = din[2] && At_.nnz ? a_value_map() : nullptr;
+    derivative_rhs_s_kernel<T><<<vgrid((long long)m * 32), kBlock, 0, stream_>>>(
+        m, A_.rowptr.p, A_.col.p, amap, amap ? din[2] : nullptr, din[3], din[4], din[5], pol_kind_.p, row_class_.p,
+        pol_zx_.p, D, Ev, adj_gs_.p, adj_rs_.p, ls_.p + n);
+    check_launch("derivative_rhs_s");
+  }
+  double rmax[2];
+  refine_with_factor(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, refine_iter, rmax);
+  // s~' = e - A~ x~' into adj_rs_, whose right-hand side the refinement no longer reads
+  launch_spmv(A_, adj_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m, EpiPolishSlack<T>{nullptr, adj_rs_.p, adj_gs_.p},
+              red(SC_TMP6), "spmv_derivative_slack");
+  CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
+  derivative_out_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, pol_mu_.p, adj_zx_.p, adj_zv_.p,
+                                                                          adj_rs_.p, D, Ev, c, dout[0], dout[1], dout[2],
+                                                                          adj_cnt_.p);
+  check_launch("derivative_out");
+  int cnt[ADJ_CNT_COUNT] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+  unstage_f64(outs, dout, 3);
   if (dev) caller_written();
   sync();
   out[1] = cnt[ADJ_CNT_ACTIVE];
@@ -3650,6 +3730,20 @@ void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const
   sa_run(p, dev, ins, in_count, 3, outs, 6, out, rhs, op, emit);
 }
 
+// The CSR(A) -> CSC map of A's values, for the derivatives' dA~ x~ passes over CSR(A): the value map of update_matrices
+// when it is resident, else one derived on the device by the first call and kept
+template <typename T>
+const int* Engine<T>::a_value_map() {
+  if (A_.d_src.p) return A_.d_src.p;
+  if (!sd_amap_.p) {
+    sd_amap_.alloc((size_t)At_.nnz, false);
+    sd_amap_kernel<<<vgrid((long long)n_ * 32), kBlock, 0, stream_>>>(n_, At_.rowptr.p, At_.col.p, A_.rowptr.p, A_.col.p,
+                                                                      sd_amap_.p);
+    check_launch("sd_amap");
+  }
+  return sd_amap_.p;
+}
+
 // (I - M) v = [v_x - a; v_s + b / rho - h],  h = Dpi v_s,  [a; b] = K^-1 [sigma v_x; v_s - 2 h]
 template <typename T>
 void Engine<T>::sd_operator(const T* v, T* out) {
@@ -3690,20 +3784,7 @@ void Engine<T>::solve_derivative(const cosmo_b200_solve_adjoint_settings* as, co
   if (m && !sd_dpi_.p) sd_dpi_.alloc(m);
   // t from [x'; nu'] = K^-1 [-dq~ - dP~ x~ - dA~' y~; db~ - 2 dPi - dA~ x~]
   auto rhs = [&](const double* const* din, T* t) {
-    const int* amap = nullptr;
-    if (din[2] && At_.nnz) {
-      if (A_.d_src.p) {
-        amap = A_.d_src.p;   // the value maps of update_matrices are resident
-      } else {
-        if (!sd_amap_.p) {
-          sd_amap_.alloc((size_t)At_.nnz, false);
-          sd_amap_kernel<<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, A_.rowptr.p, A_.col.p,
-                                                                           sd_amap_.p);
-          check_launch("sd_amap");
-        }
-        amap = sd_amap_.p;
-      }
-    }
+    const int* amap = din[2] && At_.nnz ? a_value_map() : nullptr;
     if (din[0] && P_.nnz && !maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only
     sa_kkt_with([&] {
       if (m) {
@@ -4031,6 +4112,12 @@ int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* 
                        double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double out[4]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->adjoint(refine_iter, dx, dy, ds, dq, db, dPx, dAx, dl, du, out));
+}
+int cosmo_b200_derivative(cosmo_b200_handle* h, int32_t refine_iter, const double* dPx, const double* dq,
+                          const double* dAx, const double* db, const double* dl, const double* du, double* dx, double* dy,
+                          double* ds, double out[4]) {
+  if (!out) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->derivative(refine_iter, dPx, dq, dAx, db, dl, du, dx, dy, ds, out));
 }
 int cosmo_b200_solve_adjoint(cosmo_b200_handle* h, const cosmo_b200_solve_adjoint_settings* as, const double* dx,
                              const double* dy, const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl,

@@ -185,6 +185,7 @@ def _signatures():
         "cosmo_b200_rescale_iterates": (rc, [vp]),
         "cosmo_b200_polish": (rc, [vp, P(PolishSettings), vp, vp, vp, P(f64)]),
         "cosmo_b200_adjoint": (rc, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
+        "cosmo_b200_derivative": (rc, [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_solve_adjoint": (rc, [vp, P(SolveAdjointSettings), vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_solve_derivative": (rc, [vp, P(SolveAdjointSettings), vp, vp, vp, vp, vp, vp, vp, vp, vp, P(f64)]),
         "cosmo_b200_comm_unique_id": (rc, [vp]),
@@ -622,6 +623,22 @@ class Engine:
         ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
         stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_adjoint, self._h, int(refine_iter), _ptr(gx), _ptr(gy),
                        _ptr(gs), *ptrs, ctype=C.c_double, keys=ADJOINT_STATS, ints=ADJOINT_STATS[:3])
+        return tuple(outs), stats
+
+    def derivative(self, dPx=None, dq=None, dAx=None, db=None, dl=None, du=None, refine_iter=3, dx=None, dy=None,
+                   ds=None):
+        """cosmo_b200_derivative: the directional derivatives (dx, dy, ds) of the last polished solution along the data
+        direction dPx, dAx (the ``data`` order of P and A as given to create / update_matrices), dq (n), db, dl, du (m),
+        on the polish's active set (DESIGN.md §3j): the forward counterpart of ``adjoint``.  Inputs are fp64 host or
+        CUDA arrays (None: zero); dx (n), dy, ds (m) are fp64 outputs, host or CUDA arrays, None allocates a NumPy
+        array.  Returns ((dx, dy, ds), stats), stats keyed by ADJOINT_STATS (status 1 computed, 0 the polish was
+        rejected, -1 it did not apply, the outputs then NaN; the counts as ints)."""
+        sizes = (self.nnzP, self.n, self.nnzA, self.m, self.m, self.m)
+        ins = [self._arr(a, k, np.float64) for a, k in zip((dPx, dq, dAx, db, dl, du), sizes)]
+        outs = [np.empty(k) if a is None else a for a, k in zip((dx, dy, ds), (self.n, self.m, self.m))]
+        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, (self.n, self.m, self.m))]
+        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_derivative, self._h, int(refine_iter),
+                       *(_ptr(a) for a in ins), *ptrs, ctype=C.c_double, keys=ADJOINT_STATS, ints=ADJOINT_STATS[:3])
         return tuple(outs), stats
 
     def solve_adjoint(self, dx=None, dy=None, ds=None, tol=0.0, max_iter=500, restart=30, kkt_tol=1e-12, dq=None,

@@ -887,6 +887,21 @@ class Model:
                 "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
                 "q": dq, "b": db, "l": dl, "u": du, "stats": st}
 
+    def derivative(self, dP=None, dq=None, dA=None, db=None, dl=None, du=None, refine_iter=3):
+        """Directional derivatives of the polished solution (x, y, s) of the last optimize() along a data direction,
+        through cosmo_b200_derivative (DESIGN.md §3j): the forward counterpart of adjoint(), in its coordinates.  "dP"
+        and "dA" are sparse matrices on the patterns of P0 and A0 (read as solve_derivative() reads them), "dq" an
+        n-vector, "db", "dl", "du" m-vectors (dl, du are read on active Box rows only); None is zero.  Returns a dict of
+        "x", "y", "s" and "stats" (Engine.ADJOINT_STATS).  ValueError unless the last optimize() returned
+        polish == "Polished", as adjoint()."""
+        if not self._polished or self.engine is None:
+            raise ValueError("derivative needs the last optimize() to have returned polish == \"Polished\" "
+                             "(Settings(polish=True) and a direct KKT solver)")
+        dPx = None if dP is None else _pattern_values(dP, self.P0, "dP")
+        dAx = None if dA is None else _pattern_values(dA, self.A0, "dA")
+        (dx, dy, ds), st = self.engine.derivative(dPx, dq, dAx, db, dl, du, refine_iter)
+        return {"x": dx, "y": dy, "s": ds, "stats": st}
+
     def solve_adjoint(self, dx=None, dy=None, ds=None, tol=0.0, max_iter=500, restart=30, kkt_tol=1e-12):
         """Gradients of a scalar loss with respect to the data, from its gradients dx (n), dy, ds (m) with respect to the
         solution (x, y, s) of the last optimize() (None: zero), through cosmo_b200_solve_adjoint (DESIGN.md §3k): the

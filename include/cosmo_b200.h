@@ -612,6 +612,27 @@ int cosmo_b200_polish(cosmo_b200_handle* h, const cosmo_b200_polish_settings* ps
    DESIGN.md §3j. */
 int cosmo_b200_adjoint(cosmo_b200_handle* h, int32_t refine_iter, const double* dx, const double* dy, const double* ds,
                        double* dq, double* db, double* dPx, double* dAx, double* dl, double* du, double out[4]);
+/* The forward counterpart of cosmo_b200_adjoint: the Jacobian-vector product of the same polished solution map.  Given
+   a direction (dPx, dq, dAx, db, dl, du) of the data of the unscaled set! form, it returns the directional derivatives
+   dx (n), dy, ds (m) of the last polished solution (x, y, s), with the active set A held fixed:
+     K_A [dx; dy_A] = [-dq - dP x - dA' y; db_A - dsbar_A - dA_A x],  dy = 0 off A,  ds = db - dA x - A dx (every row),
+     dsbar_r = dl_r on lower-active Box rows, du_r on upper-active ones, (dl_r + du_r) / 2 on Box rows with l = u, 0 on
+     every other row (the transpose of the adjoint's half split).
+   With the direction scaled as the data are (c D dP D, c D dq, E dA D, E db, E dl, E du), the system is solved in the
+   engine's scaled coordinates with the factor the polish left, from z = 0, then refined refine_iter (0 .. 100) times
+   against the exact K_A, and the outputs are mapped back as cosmo_b200_solution maps the solution (x = D x~,
+   s = s~ ./ E, y = E y~ / c).  On the active rows ds equals dsbar up to the refinement residual.  <g, J d> = <J' g, d>
+   with cosmo_b200_adjoint to the accuracy of the refined solves.  dP is read through the stored pattern of P (both
+   triangles when both are stored); a symmetric direction is the one the adjoint's symmetrised dPx describes.  The
+   inputs dPx (nnz P, the CSC order of P given to create / update_matrices), dq (n), dAx (nnz A, A's CSC order), db, dl,
+   du (m) and the outputs are fp64, host or device, under the caller-memory rules of cosmo_b200_solution; a NULL input
+   is zero, a NULL output is skipped.  out, the statuses (the outputs are NaN unless it is 1), the errors and the
+   untouched state are those of cosmo_b200_adjoint; two calls give bit-identical results, and nothing is factored.
+   Scratch is cosmo_b200_adjoint's, plus one int per nonzero of A for the CSR -> CSC map of A's values when
+   update_matrices has not made it resident (shared with cosmo_b200_solve_derivative).  DESIGN.md §3j. */
+int cosmo_b200_derivative(cosmo_b200_handle* h, int32_t refine_iter, const double* dPx, const double* dq,
+                          const double* dAx, const double* db, const double* dl, const double* du, double* dx, double* dy,
+                          double* ds, double out[4]);
 
 /* ---- derivatives of a conic solution --------------------------------------- */
 /* An engine extension beyond the reference, like cosmo_b200_adjoint, for every cone the engine differentiates: ZeroSet,
