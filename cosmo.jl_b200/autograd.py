@@ -23,6 +23,9 @@ its backward pass is one ``Engine.solve_adjoint`` and its forward-mode product (
 ``gradcheck(check_forward_ad=True)``) one ``Engine.solve_derivative``, both into CUDA tensors.  The ``torch.func``
 transforms (``jvp``, ``jacfwd``, ``vmap``) are not supported: they need the ``setup_context`` form of the Function.
 """
+import dataclasses
+from typing import Callable
+
 import torch
 
 from .engine import EngineError
@@ -45,58 +48,6 @@ def _solve_and_polish(engine, Px, q, Ax, b):
     return x, y, s
 
 
-class _SolveQP(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, engine, refine_iter, Px, q, Ax, b):
-        x, y, s = _solve_and_polish(engine, Px, q, Ax, b)
-        ctx.engine, ctx.refine_iter, ctx.device, ctx.call = engine, refine_iter, q.device, engine._solve_qp_call
-        ctx.dtypes = (Px.dtype, q.dtype, Ax.dtype, b.dtype)
-        ctx.save_for_backward(Px, q, Ax, b)
-        ctx.save_for_forward(Px, q, Ax, b)
-        return x, y, s
-
-    @staticmethod
-    def jvp(ctx, _engine, _refine_iter, tPx, tq, tAx, tb):
-        eng = ctx.engine
-        dev = ctx.device
-        if eng._solve_qp_call != ctx.call:   # the engine has polished other data since: this pass's point again
-            _solve_and_polish(eng, *ctx.saved_tensors)
-            ctx.call = eng._solve_qp_call
-        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
-        f64 = dict(dtype=torch.float64, device=dev)
-        dx, dy, ds = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64), torch.empty(eng.m, **f64)
-        d = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (tPx, tq, tAx, tb)]
-        _, st = eng.derivative(d[0], d[1], d[2], d[3], refine_iter=ctx.refine_iter, dx=dx, dy=dy, ds=ds)
-        if st["status"] != 1:
-            raise EngineError(st["status"], "solve_qp: the derivative did not apply (status %d)" % st["status"])
-        return dx, dy, ds
-
-    @staticmethod
-    def backward(ctx, gx, gy, gs):
-        eng = ctx.engine
-        dev = ctx.device
-        if eng._solve_qp_call != ctx.call:   # the engine has polished other data since: this pass's point again
-            _solve_and_polish(eng, *ctx.saved_tensors)
-            ctx.call = eng._solve_qp_call
-        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
-        f64 = dict(dtype=torch.float64, device=dev)
-        dq, db = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64)
-        dPx, dAx = torch.empty(eng.nnzP, **f64), torch.empty(eng.nnzA, **f64)
-        dl, du = torch.empty(eng.m, **f64), torch.empty(eng.m, **f64)
-        g = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (gx, gy, gs)]
-        _, st = eng.adjoint(*g, refine_iter=ctx.refine_iter, dq=dq, db=db, dPx=dPx, dAx=dAx, dl=dl, du=du)
-        if st["status"] != 1:
-            raise EngineError(st["status"], "solve_qp: the adjoint did not apply (status %d)" % st["status"])
-        tP, tq, tA, tb = ctx.dtypes
-        return None, None, dPx.to(tP), dq.to(tq), dAx.to(tA), db.to(tb)
-
-
-def solve_qp(engine, Px, q, Ax, b, refine_iter=3):
-    """The polished solution (x, y, s) of the engine's problem with the data (Px, q, Ax, b), differentiable with respect
-    to all four (see the module docstring)."""
-    return _SolveQP.apply(engine, refine_iter, Px, q, Ax, b)
-
-
 def _solve(engine, Px, q, Ax, b):
     """update_matrices and solve, then the unscaled solution into new CUDA tensors; returns (x, y, s) and tags the engine
     with this call."""
@@ -115,51 +66,83 @@ def _solve(engine, Px, q, Ax, b):
     return x, y, s
 
 
-class _SolveConic(torch.autograd.Function):
+@dataclasses.dataclass(frozen=True)
+class _Mode:
+    """What solve_qp and solve_conic differ in: the forward solve, the engine attribute that counts its calls, the
+    forward derivative (engine, options, direction, dx, dy, ds) and the adjoint (engine, options, gradients, dq, db, dPx,
+    dAx), each returning the engine call's (outputs, stats), and the errors of those two when their status is not 1."""
+    solve: Callable
+    counter: str
+    derivative: Callable
+    adjoint: Callable
+    derivative_error: str
+    adjoint_error: str
+
+
+def _at_forward_point(ctx):
+    """ctx's engine, solved at the data of ctx's forward pass again when it has solved other data since, with the
+    current stream as its caller stream; and the options of the fp64 output tensors."""
+    eng, mode = ctx.engine, ctx.mode
+    if getattr(eng, mode.counter) != ctx.call:   # the engine has solved other data since: this pass's point again
+        mode.solve(eng, *ctx.saved_tensors)
+        ctx.call = getattr(eng, mode.counter)
+    eng.set_caller_stream(torch.cuda.current_stream(ctx.device).cuda_stream)
+    return eng, dict(dtype=torch.float64, device=ctx.device)
+
+
+class _Solve(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, engine, settings, Px, q, Ax, b):
-        x, y, s = _solve(engine, Px, q, Ax, b)
-        ctx.engine, ctx.settings, ctx.device, ctx.call = engine, settings, q.device, engine._solve_conic_call
+    def forward(ctx, mode, engine, options, Px, q, Ax, b):
+        x, y, s = mode.solve(engine, Px, q, Ax, b)
+        ctx.mode, ctx.engine, ctx.options, ctx.device = mode, engine, options, q.device
+        ctx.call = getattr(engine, mode.counter)
         ctx.dtypes = (Px.dtype, q.dtype, Ax.dtype, b.dtype)
         ctx.save_for_backward(Px, q, Ax, b)
         ctx.save_for_forward(Px, q, Ax, b)
         return x, y, s
 
     @staticmethod
-    def jvp(ctx, _engine, _settings, tPx, tq, tAx, tb):
-        eng = ctx.engine
-        dev = ctx.device
-        if eng._solve_conic_call != ctx.call:   # the engine has solved other data since: this pass's point again
-            _solve(eng, *ctx.saved_tensors)
-            ctx.call = eng._solve_conic_call
-        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
-        f64 = dict(dtype=torch.float64, device=dev)
+    def jvp(ctx, _mode, _engine, _options, tPx, tq, tAx, tb):
+        eng, f64 = _at_forward_point(ctx)
         dx, dy, ds = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64), torch.empty(eng.m, **f64)
         d = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (tPx, tq, tAx, tb)]
-        _, st = eng.solve_derivative(d[0], d[1], d[2], d[3], dx=dx, dy=dy, ds=ds, **ctx.settings)
+        _, st = ctx.mode.derivative(eng, ctx.options, d, dx, dy, ds)
         if st["status"] != 1:
-            raise EngineError(st["status"], "solve_conic: the solve derivative did not apply or converge (status %d)"
-                              % st["status"])
+            raise EngineError(st["status"], ctx.mode.derivative_error % st["status"])
         return dx, dy, ds
 
     @staticmethod
     def backward(ctx, gx, gy, gs):
-        eng = ctx.engine
-        dev = ctx.device
-        if eng._solve_conic_call != ctx.call:   # the engine has solved other data since: this pass's point again
-            _solve(eng, *ctx.saved_tensors)
-            ctx.call = eng._solve_conic_call
-        eng.set_caller_stream(torch.cuda.current_stream(dev).cuda_stream)
-        f64 = dict(dtype=torch.float64, device=dev)
+        eng, f64 = _at_forward_point(ctx)
         dq, db = torch.empty(eng.n, **f64), torch.empty(eng.m, **f64)
         dPx, dAx = torch.empty(eng.nnzP, **f64), torch.empty(eng.nnzA, **f64)
         g = [None if t is None else t.detach().to(torch.float64).contiguous() for t in (gx, gy, gs)]
-        _, st = eng.solve_adjoint(*g, dq=dq, db=db, dPx=dPx, dAx=dAx, **ctx.settings)
+        _, st = ctx.mode.adjoint(eng, ctx.options, g, dq, db, dPx, dAx)
         if st["status"] != 1:
-            raise EngineError(st["status"], "solve_conic: the solve adjoint did not apply or converge (status %d)"
-                              % st["status"])
+            raise EngineError(st["status"], ctx.mode.adjoint_error % st["status"])
         tP, tq, tA, tb = ctx.dtypes
-        return None, None, dPx.to(tP), dq.to(tq), dAx.to(tA), db.to(tb)
+        return None, None, None, dPx.to(tP), dq.to(tq), dAx.to(tA), db.to(tb)
+
+
+# dl and du: CUDA tensors for the polished adjoint, the NumPy arrays Engine.solve_adjoint allocates for the conic one
+_QP = _Mode(
+    _solve_and_polish, "_solve_qp_call",
+    lambda eng, refine_iter, d, dx, dy, ds: eng.derivative(*d, refine_iter=refine_iter, dx=dx, dy=dy, ds=ds),
+    lambda eng, refine_iter, g, dq, db, dPx, dAx: eng.adjoint(
+        *g, refine_iter=refine_iter, dq=dq, db=db, dPx=dPx, dAx=dAx, dl=torch.empty_like(db), du=torch.empty_like(db)),
+    "solve_qp: the derivative did not apply (status %d)", "solve_qp: the adjoint did not apply (status %d)")
+_CONIC = _Mode(
+    _solve, "_solve_conic_call",
+    lambda eng, settings, d, dx, dy, ds: eng.solve_derivative(*d, dx=dx, dy=dy, ds=ds, **settings),
+    lambda eng, settings, g, dq, db, dPx, dAx: eng.solve_adjoint(*g, dq=dq, db=db, dPx=dPx, dAx=dAx, **settings),
+    "solve_conic: the solve derivative did not apply or converge (status %d)",
+    "solve_conic: the solve adjoint did not apply or converge (status %d)")
+
+
+def solve_qp(engine, Px, q, Ax, b, refine_iter=3):
+    """The polished solution (x, y, s) of the engine's problem with the data (Px, q, Ax, b), differentiable with respect
+    to all four (see the module docstring)."""
+    return _Solve.apply(_QP, engine, refine_iter, Px, q, Ax, b)
 
 
 def solve_conic(engine, Px, q, Ax, b, **adjoint_settings):
@@ -171,4 +154,4 @@ def solve_conic(engine, Px, q, Ax, b, **adjoint_settings):
     exact as the solve's tolerance goes to 0.  The engine rules of solve_qp apply: between a forward pass and its
     backward pass (or its forward-mode product) it is used only through solve_conic, and a derivative after other
     solves re-solves its own data first."""
-    return _SolveConic.apply(engine, dict(adjoint_settings), Px, q, Ax, b)
+    return _Solve.apply(_CONIC, engine, dict(adjoint_settings), Px, q, Ax, b)

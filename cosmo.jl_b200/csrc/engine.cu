@@ -365,21 +365,47 @@ class Engine : public EngineBase {
   // refine_iter + 1 solves of K~ z = r^ with the factor in memory, each followed by polish_update_kernel, with the
   // residual r^ - K_A z between them and at the end (max2 as for polish_residual)
   void refine_with_factor(T* zx, T* znu, const T* rx, const T* rs, int refine_iter, double* max2);
-  // adjoint scratch, allocated by the first adjoint or derivative and kept: its own z (pol_zx_ / pol_znu_ hold the
-  // polished point the gradients read), the kept right-hand side, gs~ (the derivative's e) and two counters
+  // adjoint scratch, allocated by the first adjoint or derivative with status 1 and kept: its own z (pol_zx_ / pol_znu_
+  // hold the polished point the gradients read), the kept right-hand side, gs~ (the derivative's e) and two counters
   DevBuf<T> adj_zx_, adj_zv_, adj_rx_, adj_rs_, adj_gs_;
   DevBuf<int> adj_cnt_;
-  // fp64 caller arrays of the two adjoints: dev holds their caller_arrays bits, the inputs first, then the outputs.  Host
-  // arrays are staged through `stage`, device arrays are read and written in place.
-  struct F64Out { double* p; long long count; };
-  void stage_f64(unsigned dev, const double* const* ins, const long long* in_count, int nin, const F64Out* outs, int nout,
-                 DevBuf<double>& stage, const double** din, double** dout);
-  void unstage_f64(const F64Out* outs, double* const* dout, int nout);
-  void nan_f64(unsigned dev, int nin, const F64Out* outs, int nout);
-  // the two calls on the polish record (adjoint, derivative): the checks of a call, then out = {status, 0, 0, NaN}
-  // with NaN outputs and false unless the status is 1, else the scratch allocated and true
+  void adj_alloc();
+  // the checks of the two calls on the polish record (adjoint, derivative)
   void adj_check(int refine_iter, const char* who);
-  bool adj_begin(unsigned dev, int nin, const F64Out* outs, int nout, double* out);
+  // The fp64 caller arrays of a derivative call: dev holds their caller_arrays bits, the inputs first, then the outputs.
+  // Host arrays are staged through a device buffer, device arrays are read and written in place.  reverse_io: the
+  // gradients dx, dy, ds of the solution in, those of the data out; forward_io: a data direction in, dx, dy, ds out.
+  struct F64Io {
+    unsigned dev;
+    int nin, nout;
+    const double* in[6];
+    long long in_count[6];
+    double* out[6];
+    long long out_count[6];
+  };
+  F64Io reverse_io(const double* dx, const double* dy, const double* ds, double* dq, double* db, double* dPx, double* dAx,
+                   double* dl, double* du) {
+    return F64Io{caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du}), 3, 6, {dx, dy, ds}, {n_, m_, m_},
+                 {dq, db, dPx, dAx, dl, du}, {n_, m_, P_.nnz, At_.nnz, m_, m_}};
+  }
+  F64Io forward_io(const double* dPx, const double* dq, const double* dAx, const double* db, const double* dl,
+                   const double* du, double* dx, double* dy, double* ds) {
+    return F64Io{caller_arrays({dPx, dq, dAx, db, dl, du, dx, dy, ds}), 6, 3, {dPx, dq, dAx, db, dl, du},
+                 {P_.nnz, n_, At_.nnz, m_, m_, m_}, {dx, dy, ds}, {n_, m_, m_}};
+  }
+  void stage_f64(const F64Io& io, DevBuf<double>& stage, const double** din, double** dout);
+  void unstage_f64(const F64Io& io, double* const* dout);
+  void nan_f64(const F64Io& io);
+  // the frame of the four derivative calls (adjoint, derivative, solve_adjoint, solve_derivative): out[0] = status, the
+  // outputs NaN unless it is 1, else the arrays staged around body(din, dout), which returns false for status 0
+  template <class Body>
+  void derivative_frame(const F64Io& io, int status, double* out, Body&& body);
+  // dP and dA of the two reverse calls (adjoint.cuh): from u, x, v, mu and gs (NULL: no gs~ term) into dPx / dAx (NULL:
+  // skipped)
+  void emit_matrix_grads(const T* u, const T* x, const T* v, const T* mu, const T* gs, double* dPx, double* dAx);
+  // D, E and c of the scaling, or none (NULL, NULL, 1) on an unscaled engine
+  struct Scaling { const T* D; const T* E; double c; };
+  Scaling scaling() const { return scaled_ ? Scaling{D_.p, E_.p, c_} : Scaling{nullptr, nullptr, 1.0}; }
   // solve adjoint (solve_adjoint.cuh): scratch allocated by the first call and kept -- the Krylov basis with lam and gw,
   // the point w_s, two m-vectors for Dpi, the row flags, the SOC norms and x'h, the eigenpairs of the PSD cones (small
   // cones first, then large ones) and three N x N work matrices for the largest large cone, the saved plugin state, and
@@ -401,7 +427,7 @@ class Engine : public EngineBase {
   void sa_kkt(const T* lam);
   void sa_operator(const T* lam, T* out);
   // the steps both derivatives through the fixed point share: the checks of a call, the plugin state the inner solves
-  // move (saved and put back), the Jacobian data of the point and GMRES(restart) on an operator
+  // move (saved and put back), the Jacobian data of the point and GMRES(restart) on an operator, driven by sa_run
   struct SaSaved {
     long long kkt_counter, total_inner, total_mults, persist;
     bool tm_valid, had_mr_x;
@@ -418,13 +444,17 @@ class Engine : public EngineBase {
   template <class Op>
   bool sa_gmres(Op&& op, int R, int max_iter, double tol, long long& apps, double& rel);
   template <class Rhs, class Op, class Emit>
-  void sa_run(const cosmo_b200_solve_adjoint_settings& p, unsigned dev, const double* const* ins, const long long* in_count,
-              int nin, const F64Out* outs, int nout, double* out, Rhs&& rhs, Op&& op, Emit&& emit);
+  void sa_run(const cosmo_b200_solve_adjoint_settings& p, const F64Io& io, double* out, Rhs&& rhs, Op&& op, Emit&& emit);
   // solve derivative (DESIGN.md §3l): dPi of the Box bound directions, the CSR(A) -> CSC map of A's values when the
   // value maps are not resident (derived once and kept)
   DevBuf<T> sd_dpi_;
   DevBuf<int> sd_amap_;
   const int* a_value_map();
+  // the CSR(P) -> CSC map of P's values: uploaded on its own, without the slab maps, when they are not resident
+  const int* p_value_map() {
+    if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);
+    return P_.d_src.p;
+  }
   void sd_operator(const T* v, T* out);
   void emit_solution(const T* xsrc, const T* ssrc, const T* musrc, int complete_dual, double* x, double* y, double* s);
   rev::Reverse rev_;             // map of a chordal decomposition (cosmo_b200_set_decomposition)
@@ -3039,6 +3069,26 @@ void Engine<T>::refine_with_factor(T* zx, T* znu, const T* rx, const T* rs, int 
   polish_residual(zx, znu, rx, rs, max2);
 }
 
+// The frame of the four derivative calls.  out[0] = status.  Unless it is 1 the outputs are set to NaN; with 1 the
+// caller arrays are staged, body(din, dout) runs on the staged pointers, and its outputs are copied back, or set to NaN
+// with status 0 when it returns false.  Ends with the caller-stream handshake and a synchronise.
+template <typename T>
+template <class Body>
+void Engine<T>::derivative_frame(const F64Io& io, int status, double* out, Body&& body) {
+  out[0] = status;
+  DevBuf<double> stage;   // the copies back read it until the synchronise
+  if (status == 1) {
+    const double* din[6];
+    double* dout[6];
+    stage_f64(io, stage, din, dout);
+    if (body(din, dout)) unstage_f64(io, dout);
+    else out[0] = 0.0;
+  }
+  if (out[0] != 1.0) nan_f64(io);
+  if (io.dev) caller_written();
+  sync();
+}
+
 // Derivatives of the polished solution (DESIGN.md §3j, adjoint.cuh): the right-hand side from the incoming gradients,
 // refine_iter + 1 solves with the factor the polish left and its refinement against the exact K_A, then the gradients
 // of q, b, the Box bounds, P and A.  Nothing is factored; the iterates, the solution, rho, the statistics and the polish
@@ -3047,52 +3097,33 @@ template <typename T>
 void Engine<T>::adjoint(int refine_iter, const double* dx, const double* dy, const double* ds, double* dq, double* db,
                         double* dPx, double* dAx, double* dl, double* du, double* out) {
   adj_check(refine_iter, "adjoint");
-  const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
+  const F64Io io = reverse_io(dx, dy, ds, dq, db, dPx, dAx, dl, du);
   const int n = n_, m = m_;
-  const long long nnzP = P_.nnz, nnzA = At_.nnz;
-  const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, nnzP}, {dAx, nnzA}, {dl, m}, {du, m}};
-  if (!adj_begin(dev, 3, outs, 6, out)) return;
-  const double* ins[3] = {dx, dy, ds};
-  const long long in_count[3] = {n, m, m};
-  DevBuf<double> stage;
-  const double* din[3];
-  double* dout[6];
-  stage_f64(dev, ins, in_count, 3, outs, 6, stage, din, dout);
-  const T* D = scaled_ ? D_.p : nullptr;
-  const T* Ev = scaled_ ? E_.p : nullptr;
-  const double c = scaled_ ? c_ : 1.0;
-  // right-hand side: s rows and gs~, then the x rows over A' gs~, into ls_ and the kept copies
-  adjoint_rhs_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, din[1], din[2], Ev, c, adj_gs_.p, adj_rs_.p, ls_.p);
-  check_launch("adjoint_rhs");
-  launch_spmv(At_, adj_gs_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n, EpiAdjointRhsX<T>{nullptr, adj_rx_.p, ls_.p, din[0], D},
-              red(SC_TMP6), "spmv_adjoint_rhs_x");
-  // the first solve from z = 0, then refine_iter steps against the exact K_A, v masked off the active rows
-  double rmax[2];
-  refine_with_factor(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, refine_iter, rmax);
-  // gradients
-  CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
-  AdjointVecArgs<T> a;
-  a.n = n; a.m = m; a.kind = pol_kind_.p; a.row_class = row_class_.p; a.u = adj_zx_.p; a.v = adj_zv_.p; a.gs = adj_gs_.p;
-  a.mu_p = pol_mu_.p; a.D = D; a.E = Ev; a.c = c;
-  a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5]; a.counts = adj_cnt_.p;
-  adjoint_grad_vec_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(a);
-  check_launch("adjoint_grad_vec");
-  if (dout[2] && nnzP) {
-    if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only, not the slab maps
-    adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.d_src.p, adj_zx_.p,
-                                                                             pol_zx_.p, D, c, dout[2]);
-    check_launch("adjoint_grad_P");
-  }
-  if (dout[3] && nnzA) {
-    adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, adj_zx_.p, pol_zx_.p,
-                                                                             adj_zv_.p, pol_mu_.p, adj_gs_.p, D, Ev, dout[3]);
-    check_launch("adjoint_grad_A");
-  }
+  const Scaling sc = scaling();
   int cnt[ADJ_CNT_COUNT] = {0, 0};
-  CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
-  unstage_f64(outs, dout, 6);
-  if (dev) caller_written();
-  sync();
+  double rmax[2] = {NAN, NAN};   // out[1 .. 3] = 0, 0, NaN unless the status is 1
+  derivative_frame(io, pol_rec_status_, out, [&](const double* const* din, double* const* dout) {
+    adj_alloc();
+    // right-hand side: s rows and gs~, then the x rows over A' gs~, into ls_ and the kept copies
+    adjoint_rhs_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, din[1], din[2], sc.E, sc.c, adj_gs_.p,
+                                                            adj_rs_.p, ls_.p);
+    check_launch("adjoint_rhs");
+    launch_spmv(At_, adj_gs_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, n,
+                EpiAdjointRhsX<T>{nullptr, adj_rx_.p, ls_.p, din[0], sc.D}, red(SC_TMP6), "spmv_adjoint_rhs_x");
+    // the first solve from z = 0, then refine_iter steps against the exact K_A, v masked off the active rows
+    refine_with_factor(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, refine_iter, rmax);
+    // gradients
+    CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
+    AdjointVecArgs<T> a;
+    a.n = n; a.m = m; a.kind = pol_kind_.p; a.row_class = row_class_.p; a.u = adj_zx_.p; a.v = adj_zv_.p; a.gs = adj_gs_.p;
+    a.mu_p = pol_mu_.p; a.D = sc.D; a.E = sc.E; a.c = sc.c;
+    a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5]; a.counts = adj_cnt_.p;
+    adjoint_grad_vec_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(a);
+    check_launch("adjoint_grad_vec");
+    emit_matrix_grads(adj_zx_.p, pol_zx_.p, adj_zv_.p, pol_mu_.p, adj_gs_.p, dout[2], dout[3]);
+    CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+    return true;
+  });
   out[1] = cnt[ADJ_CNT_ACTIVE];
   out[2] = cnt[ADJ_CNT_WEAK];
   out[3] = std::max(rmax[0], rmax[1]);
@@ -3112,19 +3143,12 @@ void Engine<T>::adj_check(int refine_iter, const char* who) {
 }
 
 template <typename T>
-bool Engine<T>::adj_begin(unsigned dev, int nin, const F64Out* outs, int nout, double* out) {
-  out[0] = pol_rec_status_; out[1] = out[2] = 0.0; out[3] = NAN;
-  if (pol_rec_status_ != 1) {
-    nan_f64(dev, nin, outs, nout);
-    return false;
-  }
-  if (!adj_cnt_.p) {
-    const int n = n_, m = m_;
-    adj_zx_.alloc(std::max(n, 1)); adj_rx_.alloc(std::max(n, 1));
-    adj_zv_.alloc(std::max(m, 1)); adj_rs_.alloc(std::max(m, 1)); adj_gs_.alloc(std::max(m, 1));
-    adj_cnt_.alloc(ADJ_CNT_COUNT);
-  }
-  return true;
+void Engine<T>::adj_alloc() {
+  if (adj_cnt_.p) return;
+  const int n = n_, m = m_;
+  adj_zx_.alloc(std::max(n, 1)); adj_rx_.alloc(std::max(n, 1));
+  adj_zv_.alloc(std::max(m, 1)); adj_rs_.alloc(std::max(m, 1)); adj_gs_.alloc(std::max(m, 1));
+  adj_cnt_.alloc(ADJ_CNT_COUNT);
 }
 
 // The forward derivative of the polished solution along a data direction (DESIGN.md §3j, adjoint.cuh): the transpose
@@ -3135,102 +3159,110 @@ template <typename T>
 void Engine<T>::derivative(int refine_iter, const double* dPx, const double* dq, const double* dAx, const double* db,
                            const double* dl, const double* du, double* dx, double* dy, double* ds, double* out) {
   adj_check(refine_iter, "derivative");
-  const unsigned dev = caller_arrays({dPx, dq, dAx, db, dl, du, dx, dy, ds});
+  const F64Io io = forward_io(dPx, dq, dAx, db, dl, du, dx, dy, ds);
   const int n = n_, m = m_;
-  const F64Out outs[3] = {{dx, n}, {dy, m}, {ds, m}};
-  if (!adj_begin(dev, 6, outs, 3, out)) return;
-  const double* ins[6] = {dPx, dq, dAx, db, dl, du};
-  const long long in_count[6] = {P_.nnz, n, At_.nnz, m, m, m};
-  DevBuf<double> stage;
-  const double* din[6];
-  double* dout[3];
-  stage_f64(dev, ins, in_count, 6, outs, 3, stage, din, dout);
-  const T* D = scaled_ ? D_.p : nullptr;
-  const T* Ev = scaled_ ? E_.p : nullptr;
-  const double c = scaled_ ? c_ : 1.0;
-  // x rows -dq~ - dP~ x~ - dA~' y~ at the polished point into the kept rx and ls_
-  if (din[0] && P_.nnz && !maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only
-  if (n) {
-    sd_rhs_x_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(
-        n, P_.rowptr.p, P_.col.p, P_.d_src.p, At_.rowptr.p, At_.col.p, P_.nnz ? din[0] : nullptr, din[1],
-        At_.nnz ? din[2] : nullptr, pol_zx_.p, pol_mu_.p, D, Ev, c, adj_rx_.p);
-    check_launch("sd_rhs_x");
-    CUDA_TRY(cudaMemcpyAsync(ls_.p, adj_rx_.p, n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-  }
-  // s rows on the active rows into the kept rs and ls_, e on every row into adj_gs_
-  if (m) {
-    const int* amap = din[2] && At_.nnz ? a_value_map() : nullptr;
-    derivative_rhs_s_kernel<T><<<vgrid((long long)m * 32), kBlock, 0, stream_>>>(
-        m, A_.rowptr.p, A_.col.p, amap, amap ? din[2] : nullptr, din[3], din[4], din[5], pol_kind_.p, row_class_.p,
-        pol_zx_.p, D, Ev, adj_gs_.p, adj_rs_.p, ls_.p + n);
-    check_launch("derivative_rhs_s");
-  }
-  double rmax[2];
-  refine_with_factor(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, refine_iter, rmax);
-  // s~' = e - A~ x~' into adj_rs_, whose right-hand side the refinement no longer reads
-  launch_spmv(A_, adj_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m, EpiPolishSlack<T>{nullptr, adj_rs_.p, adj_gs_.p},
-              red(SC_TMP6), "spmv_derivative_slack");
-  CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
-  derivative_out_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, pol_mu_.p, adj_zx_.p, adj_zv_.p,
-                                                                          adj_rs_.p, D, Ev, c, dout[0], dout[1], dout[2],
-                                                                          adj_cnt_.p);
-  check_launch("derivative_out");
+  const Scaling sc = scaling();
   int cnt[ADJ_CNT_COUNT] = {0, 0};
-  CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
-  unstage_f64(outs, dout, 3);
-  if (dev) caller_written();
-  sync();
+  double rmax[2] = {NAN, NAN};   // out[1 .. 3] = 0, 0, NaN unless the status is 1
+  derivative_frame(io, pol_rec_status_, out, [&](const double* const* din, double* const* dout) {
+    adj_alloc();
+    // x rows -dq~ - dP~ x~ - dA~' y~ at the polished point into the kept rx and ls_
+    const int* pmap = din[0] && P_.nnz ? p_value_map() : nullptr;
+    if (n) {
+      sd_rhs_x_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(
+          n, P_.rowptr.p, P_.col.p, pmap, At_.rowptr.p, At_.col.p, pmap ? din[0] : nullptr, din[1],
+          At_.nnz ? din[2] : nullptr, pol_zx_.p, pol_mu_.p, sc.D, sc.E, sc.c, adj_rx_.p);
+      check_launch("sd_rhs_x");
+      CUDA_TRY(cudaMemcpyAsync(ls_.p, adj_rx_.p, n * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+    }
+    // s rows on the active rows into the kept rs and ls_, e on every row into adj_gs_
+    if (m) {
+      const int* amap = din[2] && At_.nnz ? a_value_map() : nullptr;
+      derivative_rhs_s_kernel<T><<<vgrid((long long)m * 32), kBlock, 0, stream_>>>(
+          m, A_.rowptr.p, A_.col.p, amap, amap ? din[2] : nullptr, din[3], din[4], din[5], pol_kind_.p, row_class_.p,
+          pol_zx_.p, sc.D, sc.E, adj_gs_.p, adj_rs_.p, ls_.p + n);
+      check_launch("derivative_rhs_s");
+    }
+    refine_with_factor(adj_zx_.p, adj_zv_.p, adj_rx_.p, adj_rs_.p, refine_iter, rmax);
+    // s~' = e - A~ x~' into adj_rs_, whose right-hand side the refinement no longer reads
+    launch_spmv(A_, adj_zx_.p, (const DevCsr<T>*)nullptr, (const T*)nullptr, m, EpiPolishSlack<T>{nullptr, adj_rs_.p, adj_gs_.p},
+                red(SC_TMP6), "spmv_derivative_slack");
+    CUDA_TRY(cudaMemsetAsync(adj_cnt_.p, 0, ADJ_CNT_COUNT * sizeof(int), stream_));
+    derivative_out_kernel<T><<<vgrid((long long)n + m), kBlock, 0, stream_>>>(n, m, pol_kind_.p, pol_mu_.p, adj_zx_.p,
+                                                                            adj_zv_.p, adj_rs_.p, sc.D, sc.E, sc.c,
+                                                                            dout[0], dout[1], dout[2], adj_cnt_.p);
+    check_launch("derivative_out");
+    CUDA_TRY(cudaMemcpyAsync(cnt, adj_cnt_.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream_));
+    return true;
+  });
   out[1] = cnt[ADJ_CNT_ACTIVE];
   out[2] = cnt[ADJ_CNT_WEAK];
   out[3] = std::max(rmax[0], rmax[1]);
 }
 
 template <typename T>
-void Engine<T>::stage_f64(unsigned dev, const double* const* ins, const long long* in_count, int nin, const F64Out* outs,
-                          int nout, DevBuf<double>& stage, const double** din, double** dout) {
+void Engine<T>::stage_f64(const F64Io& io, DevBuf<double>& stage, const double** din, double** dout) {
   long long stage_n = 0;
-  for (int k = 0; k < nin; ++k) if (ins[k] && !(dev & (1u << k))) stage_n += in_count[k];
-  for (int k = 0; k < nout; ++k) if (outs[k].p && !(dev & (1u << (nin + k)))) stage_n += outs[k].count;
+  for (int k = 0; k < io.nin; ++k) if (io.in[k] && !(io.dev & (1u << k))) stage_n += io.in_count[k];
+  for (int k = 0; k < io.nout; ++k) if (io.out[k] && !(io.dev & (1u << (io.nin + k)))) stage_n += io.out_count[k];
   if (stage_n) stage.alloc((size_t)stage_n, false);
   long long off = 0;
-  for (int k = 0; k < nin; ++k) {
-    din[k] = ins[k];
-    if (ins[k] && !(dev & (1u << k))) {
-      if (in_count[k]) CUDA_TRY(cudaMemcpyAsync(stage.p + off, ins[k], in_count[k] * sizeof(double), cudaMemcpyHostToDevice, stream_));
+  for (int k = 0; k < io.nin; ++k) {
+    din[k] = io.in[k];
+    if (io.in[k] && !(io.dev & (1u << k))) {
+      if (io.in_count[k])
+        CUDA_TRY(cudaMemcpyAsync(stage.p + off, io.in[k], io.in_count[k] * sizeof(double), cudaMemcpyHostToDevice, stream_));
       din[k] = stage.p + off;
-      off += in_count[k];
+      off += io.in_count[k];
     }
   }
-  for (int k = 0; k < nout; ++k) {
-    dout[k] = outs[k].p;
-    if (outs[k].p && !(dev & (1u << (nin + k)))) {
+  for (int k = 0; k < io.nout; ++k) {
+    dout[k] = io.out[k];
+    if (io.out[k] && !(io.dev & (1u << (io.nin + k)))) {
       dout[k] = stage.p + off;
-      off += outs[k].count;
+      off += io.out_count[k];
     }
   }
 }
 
 template <typename T>
-void Engine<T>::unstage_f64(const F64Out* outs, double* const* dout, int nout) {
-  for (int k = 0; k < nout; ++k)
-    if (outs[k].p && dout[k] != outs[k].p && outs[k].count)
-      CUDA_TRY(cudaMemcpyAsync(outs[k].p, dout[k], outs[k].count * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+void Engine<T>::unstage_f64(const F64Io& io, double* const* dout) {
+  for (int k = 0; k < io.nout; ++k)
+    if (io.out[k] && dout[k] != io.out[k] && io.out_count[k])
+      CUDA_TRY(cudaMemcpyAsync(io.out[k], dout[k], io.out_count[k] * sizeof(double), cudaMemcpyDeviceToHost, stream_));
 }
 
-// NaN into every output of a call whose status is not 1, then the caller-stream handshake and a synchronise
+// NaN into every output: a kernel into device memory, a fill of host memory
 template <typename T>
-void Engine<T>::nan_f64(unsigned dev, int nin, const F64Out* outs, int nout) {
-  for (int k = 0; k < nout; ++k) {
-    if (!outs[k].p || !outs[k].count) continue;
-    if (dev & (1u << (nin + k))) {
-      adjoint_nan_kernel<<<vgrid(outs[k].count), kBlock, 0, stream_>>>(outs[k].count, outs[k].p);
+void Engine<T>::nan_f64(const F64Io& io) {
+  for (int k = 0; k < io.nout; ++k) {
+    if (!io.out[k] || !io.out_count[k]) continue;
+    if (io.dev & (1u << (io.nin + k))) {
+      adjoint_nan_kernel<<<vgrid(io.out_count[k]), kBlock, 0, stream_>>>(io.out_count[k], io.out[k]);
       check_launch("adjoint_nan");
     } else {
-      std::fill(outs[k].p, outs[k].p + outs[k].count, std::numeric_limits<double>::quiet_NaN());
+      std::fill(io.out[k], io.out[k] + io.out_count[k], std::numeric_limits<double>::quiet_NaN());
     }
   }
-  if (dev) caller_written();
-  sync();
+}
+
+// dP over CSR(P) and dA over CSR(A') into dPx / dAx, at the point x with the adjoint solution [u; v], the multipliers
+// mu and gs~ (NULL for the solve adjoint)
+template <typename T>
+void Engine<T>::emit_matrix_grads(const T* u, const T* x, const T* v, const T* mu, const T* gs, double* dPx, double* dAx) {
+  const int n = n_;
+  const Scaling sc = scaling();
+  if (dPx && P_.nnz) {
+    const int* pmap = p_value_map();
+    adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, pmap, u, x, sc.D,
+                                                                             sc.c, dPx);
+    check_launch("adjoint_grad_P");
+  }
+  if (dAx && At_.nnz) {
+    adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, u, x, v, mu, gs,
+                                                                             sc.D, sc.E, dAx);
+    check_launch("adjoint_grad_A");
+  }
 }
 
 // ---- solve adjoint (DESIGN.md §3k, solve_adjoint.cuh) ---------------------------------------------------------------
@@ -3615,60 +3647,51 @@ bool Engine<T>::sa_gmres(Op&& op, int R, int max_iter, double tol, long long& ap
   return converged;
 }
 
-// One call through the fixed point (DESIGN.md §3k, §3l): the plugin state saved, the caller arrays staged, the Jacobian
-// data of the point, then `rhs(din, r)` writes the right-hand side r, GMRES solves op(z) = r, and on convergence
-// `emit(din, dout, z)` writes the outputs.  out[0 .. 3] are the status, the operator applications, the residual and the
-// inner KKT iterations; the plugin state is put back and the outputs are NaN unless the status is 1.
+// One call through the fixed point (DESIGN.md §3k, §3l) in the derivative frame, status -1 when sa_not_applicable():
+// the plugin state saved, the Jacobian data of the point, then `rhs(din, r)` writes the right-hand side r, GMRES solves
+// op(z) = r, and on convergence `emit(din, dout, z)` writes the outputs.  out[1 .. 3] are the operator applications,
+// the residual and the inner KKT iterations; the plugin state is put back and the outputs are NaN unless the status is 1.
 template <typename T>
 template <class Rhs, class Op, class Emit>
-void Engine<T>::sa_run(const cosmo_b200_solve_adjoint_settings& p, unsigned dev, const double* const* ins,
-                       const long long* in_count, int nin, const F64Out* outs, int nout, double* out, Rhs&& rhs, Op&& op,
+void Engine<T>::sa_run(const cosmo_b200_solve_adjoint_settings& p, const F64Io& io, double* out, Rhs&& rhs, Op&& op,
                        Emit&& emit) {
-  const double tol = p.tol > 0.0 ? p.tol : (sizeof(T) == sizeof(double) ? 1e-10 : 1e-5);
-  const long long L = (long long)n_ + m_;
-  const int R = p.restart;
-  sa_alloc(R);
-  const SaSaved sv = sa_save();
-  try {
-    DevBuf<double> stage;
-    const double* din[8];
-    double* dout[8];
-    stage_f64(dev, ins, in_count, nin, outs, nout, stage, din, dout);
-    const int psd_unconverged = sa_point(out);
-    T* z = sa_V_.p + (long long)(R + 1) * L;
-    T* r = z + L;
-    kkt_tol_fixed_ = p.kkt_tol;
-    int isc_start[ISC_COUNT];
-    CUDA_TRY(cudaMemcpyAsync(isc_start, isc_.p, sizeof(isc_start), cudaMemcpyDeviceToHost, stream_));
-    const long long inner_start = total_inner_;
-    long long apps = 0;
+  for (int k = 1; k < 8; ++k) out[k] = 0.0;
+  out[2] = NAN;
+  derivative_frame(io, sa_not_applicable() ? -1 : 1, out, [&](const double* const* din, double* const* dout) {
+    const double tol = p.tol > 0.0 ? p.tol : (sizeof(T) == sizeof(double) ? 1e-10 : 1e-5);
+    const long long L = (long long)n_ + m_;
+    const int R = p.restart;
+    sa_alloc(R);
+    const SaSaved sv = sa_save();
     bool converged = false;
-    double rel = NAN;
-    if (psd_unconverged == 0) {
-      rhs(din, r);
-      converged = sa_gmres(op, R, p.max_iter, tol, apps, rel);
+    try {
+      const int psd_unconverged = sa_point(out);
+      T* z = sa_V_.p + (long long)(R + 1) * L;
+      T* r = z + L;
+      kkt_tol_fixed_ = p.kkt_tol;
+      int isc_start[ISC_COUNT];
+      CUDA_TRY(cudaMemcpyAsync(isc_start, isc_.p, sizeof(isc_start), cudaMemcpyDeviceToHost, stream_));
+      const long long inner_start = total_inner_;
+      long long apps = 0;
+      double rel = NAN;
+      if (psd_unconverged == 0) {
+        rhs(din, r);
+        converged = sa_gmres(op, R, p.max_iter, tol, apps, rel);
+      }
+      out[1] = (double)apps;
+      out[2] = rel;
+      if (converged) emit(din, dout, z);
+      int isc_end[ISC_COUNT];
+      CUDA_TRY(cudaMemcpyAsync(isc_end, isc_.p, sizeof(isc_end), cudaMemcpyDeviceToHost, stream_));
+      sync();
+      out[3] = direct_kkt() ? 0.0 : (double)(total_inner_ - inner_start + (isc_end[ISC_TOTAL] - isc_start[ISC_TOTAL]));
+      sa_restore(sv);
+    } catch (...) {
+      sa_restore(sv);
+      throw;
     }
-    out[1] = (double)apps;
-    out[2] = rel;
-    if (!converged) {
-      out[0] = 0.0;
-    } else {
-      emit(din, dout, z);
-      unstage_f64(outs, dout, nout);
-      out[0] = 1.0;
-    }
-    int isc_end[ISC_COUNT];
-    CUDA_TRY(cudaMemcpyAsync(isc_end, isc_.p, sizeof(isc_end), cudaMemcpyDeviceToHost, stream_));
-    sync();
-    out[3] = direct_kkt() ? 0.0 : (double)(total_inner_ - inner_start + (isc_end[ISC_TOTAL] - isc_start[ISC_TOTAL]));
-    sa_restore(sv);
-    if (!converged) nan_f64(dev, nin, outs, nout);
-    else if (dev) caller_written();
-    sync();
-  } catch (...) {
-    sa_restore(sv);
-    throw;
-  }
+    return converged;
+  });
 }
 
 // Derivatives of the last solve's solution through the fixed point of the iteration (DESIGN.md §3k): the Jacobian data
@@ -3680,28 +3703,16 @@ void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const
                               const double* ds, double* dq, double* db, double* dPx, double* dAx, double* dl, double* du,
                               double* out) {
   const cosmo_b200_solve_adjoint_settings p = sa_settings(as, "solve_adjoint");
-  const unsigned dev = caller_arrays({dx, dy, ds, dq, db, dPx, dAx, dl, du});
+  const F64Io io = reverse_io(dx, dy, ds, dq, db, dPx, dAx, dl, du);
   const int n = n_, m = m_;
   const long long L = (long long)n + m;
-  const F64Out outs[6] = {{dq, n}, {db, m}, {dPx, P_.nnz}, {dAx, At_.nnz}, {dl, m}, {du, m}};
-  for (int k = 1; k < 8; ++k) out[k] = 0.0;
-  out[2] = NAN;
-  if (sa_not_applicable()) {
-    out[0] = -1.0;
-    nan_f64(dev, 3, outs, 6);
-    return;
-  }
-  const double* ins[3] = {dx, dy, ds};
-  const long long in_count[3] = {n, m, m};
-  const T* D = scaled_ ? D_.p : nullptr;
-  const T* Ev = scaled_ ? E_.p : nullptr;
-  const double c = scaled_ ? c_ : 1.0;
+  const Scaling sc = scaling();
   // gw = [dx~; Dpi(ds~ + rho dy~) - rho dy~]
   auto rhs = [&](const double* const* din, T* gw) {
-    sa_gw_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, din[0], din[1], din[2], D, Ev, c, rho_vec_.p, gw, sa_h_.p);
+    sa_gw_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, din[0], din[1], din[2], sc.D, sc.E, sc.c, rho_vec_.p, gw, sa_h_.p);
     check_launch("sa_gw");
     sa_dpi(sa_h_.p, sa_dh_.p);
-    sa_gw_s_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, din[1], Ev, c, rho_vec_.p, sa_dh_.p, gw + n);
+    sa_gw_s_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, din[1], sc.E, sc.c, rho_vec_.p, sa_dh_.p, gw + n);
     check_launch("sa_gw_s");
   };
   auto op = [&](const T* v, T* w) { sa_operator(v, w); };
@@ -3711,23 +3722,13 @@ void Engine<T>::solve_adjoint(const cosmo_b200_solve_adjoint_settings* as, const
     SolveAdjointVecArgs<T> a;
     a.n = n; a.m = m; a.row_class = row_class_.p; a.flag = sa_flag_.p; a.box_l = box_l_.p; a.box_u = box_u_.p;
     a.u = xsol_.p; a.v = nu_.p; a.lam_s = lam + n; a.rho = rho_vec_.p; a.gy = din[1]; a.gs = din[2];
-    a.D = D; a.E = Ev; a.c = c;
+    a.D = sc.D; a.E = sc.E; a.c = sc.c;
     a.dq = dout[0]; a.db = dout[1]; a.dl = dout[4]; a.du = dout[5];
     solve_adjoint_grad_vec_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(a);
     check_launch("solve_adjoint_grad_vec");
-    if (dout[2] && P_.nnz) {
-      if (!maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only, not the slab maps
-      adjoint_grad_P_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, P_.rowptr.p, P_.col.p, P_.d_src.p, xsol_.p,
-                                                                               xs_.p, D, c, dout[2]);
-      check_launch("adjoint_grad_P");
-    }
-    if (dout[3] && At_.nnz) {
-      adjoint_grad_A_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(n, At_.rowptr.p, At_.col.p, xsol_.p, xs_.p,
-                                                                               nu_.p, mu_.p, nullptr, D, Ev, dout[3]);
-      check_launch("adjoint_grad_A");
-    }
+    emit_matrix_grads(xsol_.p, xs_.p, nu_.p, mu_.p, nullptr, dout[2], dout[3]);
   };
-  sa_run(p, dev, ins, in_count, 3, outs, 6, out, rhs, op, emit);
+  sa_run(p, io, out, rhs, op, emit);
 }
 
 // The CSR(A) -> CSC map of A's values, for the derivatives' dA~ x~ passes over CSR(A): the value map of update_matrices
@@ -3765,42 +3766,30 @@ void Engine<T>::solve_derivative(const cosmo_b200_solve_adjoint_settings* as, co
                                  const double* dAx, const double* db, const double* dl, const double* du, double* dx,
                                  double* dy, double* ds, double* out) {
   const cosmo_b200_solve_adjoint_settings p = sa_settings(as, "solve_derivative");
-  const unsigned dev = caller_arrays({dPx, dq, dAx, db, dl, du, dx, dy, ds});
+  const F64Io io = forward_io(dPx, dq, dAx, db, dl, du, dx, dy, ds);
   const int n = n_, m = m_;
   const long long L = (long long)n + m;
-  const F64Out outs[3] = {{dx, n}, {dy, m}, {ds, m}};
-  for (int k = 1; k < 8; ++k) out[k] = 0.0;
-  out[2] = NAN;
-  if (sa_not_applicable()) {
-    out[0] = -1.0;
-    nan_f64(dev, 6, outs, 3);
-    return;
-  }
-  const double* ins[6] = {dPx, dq, dAx, db, dl, du};
-  const long long in_count[6] = {P_.nnz, n, At_.nnz, m, m, m};
-  const T* D = scaled_ ? D_.p : nullptr;
-  const T* Ev = scaled_ ? E_.p : nullptr;
-  const double c = scaled_ ? c_ : 1.0;
-  if (m && !sd_dpi_.p) sd_dpi_.alloc(m);
+  const Scaling sc = scaling();
   // t from [x'; nu'] = K^-1 [-dq~ - dP~ x~ - dA~' y~; db~ - 2 dPi - dA~ x~]
   auto rhs = [&](const double* const* din, T* t) {
+    if (m && !sd_dpi_.p) sd_dpi_.alloc(m);
     const int* amap = din[2] && At_.nnz ? a_value_map() : nullptr;
-    if (din[0] && P_.nnz && !maps_ready_ && !P_.d_src.p) P_.d_src.upload(P_.h_src, stream_);   // P's value map only
+    const int* pmap = din[0] && P_.nnz ? p_value_map() : nullptr;
     sa_kkt_with([&] {
       if (m) {
-        sd_box_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_flag_.p, box_l_.p, box_u_.p, din[4], din[5], Ev,
+        sd_box_kernel<T><<<vgrid(m), kBlock, 0, stream_>>>(m, row_class_.p, sa_flag_.p, box_l_.p, box_u_.p, din[4], din[5], sc.E,
                                                            sd_dpi_.p);
         check_launch("sd_box");
       }
       if (n) {
         sd_rhs_x_kernel<T><<<vgrid((long long)n * 32), kBlock, 0, stream_>>>(
-            n, P_.rowptr.p, P_.col.p, P_.d_src.p, At_.rowptr.p, At_.col.p, P_.nnz ? din[0] : nullptr, din[1],
-            At_.nnz ? din[2] : nullptr, xs_.p, mu_.p, D, Ev, c, ls_.p);
+            n, P_.rowptr.p, P_.col.p, pmap, At_.rowptr.p, At_.col.p, pmap ? din[0] : nullptr, din[1],
+            At_.nnz ? din[2] : nullptr, xs_.p, mu_.p, sc.D, sc.E, sc.c, ls_.p);
         check_launch("sd_rhs_x");
       }
       if (m) {
         sd_rhs_s_kernel<T><<<vgrid((long long)m * 32), kBlock, 0, stream_>>>(m, A_.rowptr.p, A_.col.p, amap, amap ? din[2] : nullptr,
-                                                                             din[3], sd_dpi_.p, xs_.p, D, Ev, rho_vec_.p,
+                                                                             din[3], sd_dpi_.p, xs_.p, sc.D, sc.E, rho_vec_.p,
                                                                              ls_.p + n, t0_.p);
         check_launch("sd_rhs_s");
       }
@@ -3812,11 +3801,11 @@ void Engine<T>::solve_derivative(const cosmo_b200_solve_adjoint_settings* as, co
   // dx = D w'_x, ds = (Dpi w'_s + dPi) / E, dy = -E rho (w'_s - s~') / c
   auto emit = [&](const double* const*, double* const* dout, const T* w) {
     sa_dpi(w + n, sa_dh_.p);
-    sd_out_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, w, sa_dh_.p, sd_dpi_.p, rho_vec_.p, D, Ev, c, dout[0], dout[1],
-                                                       dout[2]);
+    sd_out_kernel<T><<<vgrid(L), kBlock, 0, stream_>>>(n, m, w, sa_dh_.p, sd_dpi_.p, rho_vec_.p, sc.D, sc.E, sc.c, dout[0],
+                                                       dout[1], dout[2]);
     check_launch("sd_out");
   };
-  sa_run(p, dev, ins, in_count, 6, outs, 3, out, rhs, op, emit);
+  sa_run(p, io, out, rhs, op, emit);
 }
 
 // out = DPi(w_s) dir in the coordinates project() takes: the Jacobian data of w_s formed as solve_adjoint forms them at

@@ -134,6 +134,7 @@ class SolveAdjointSettings(C.Structure):
 # cosmo_b200_solve_adjoint's out[8]
 SOLVE_ADJOINT_STATS = ("status", "operator_applications", "residual", "inner_iterations", "rows_near_kink",
                        "soc_near_kink", "psd_near_kink", "psd_unconverged")
+_SOLVE_ADJOINT_INTS = tuple(k for k in SOLVE_ADJOINT_STATS if k != "residual")
 # cosmo_b200_project_jacobian's counts[4]
 PROJECT_JACOBIAN_STATS = ("rows_near_kink", "soc_near_kink", "psd_near_kink", "psd_unconverged")
 
@@ -611,19 +612,38 @@ class Engine:
                        ctype=C.c_double, keys=POLISH_STATS, ints=POLISH_STATS[:4])
         return x, y, s, stats
 
+    def _reverse(self, fn, lead, grads, outs, keys, ints):
+        """fn(handle, *lead, dx, dy, ds, dq, db, dPx, dAx, dl, du, out) of the two reverse calls: `grads` (dx, dy, ds) are
+        fp64 inputs, `outs` (dq, db, dPx, dAx, dl, du) fp64 outputs, None allocating a NumPy array.  Returns (the outputs,
+        the stats keyed by `keys`, the values of `ints` as ints)."""
+        n, m = self.n, self.m
+        gx, gy, gs = (self._arr(a, k, np.float64) for a, k in zip(grads, (n, m, m)))
+        sizes = (n, m, self.nnzP, self.nnzA, m, m)
+        outs = [np.empty(k) if a is None else a for a, k in zip(outs, sizes)]
+        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
+        stats = _keyed(self._lib, self._h, fn, self._h, *lead, _ptr(gx), _ptr(gy), _ptr(gs), *ptrs, ctype=C.c_double,
+                       keys=keys, ints=ints)
+        return tuple(outs), stats
+
+    def _forward(self, fn, lead, dirs, outs, keys, ints):
+        """fn(handle, *lead, dPx, dq, dAx, db, dl, du, dx, dy, ds, out) of the two forward calls: `dirs` (dPx, dq, dAx, db,
+        dl, du) are fp64 inputs, `outs` (dx, dy, ds) fp64 outputs, None allocating a NumPy array.  Returns as _reverse."""
+        n, m = self.n, self.m
+        ins = [self._arr(a, k, np.float64) for a, k in zip(dirs, (self.nnzP, n, self.nnzA, m, m, m))]
+        outs = [np.empty(k) if a is None else a for a, k in zip(outs, (n, m, m))]
+        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, (n, m, m))]
+        stats = _keyed(self._lib, self._h, fn, self._h, *lead, *(_ptr(a) for a in ins), *ptrs, ctype=C.c_double,
+                       keys=keys, ints=ints)
+        return tuple(outs), stats
+
     def adjoint(self, dx=None, dy=None, ds=None, refine_iter=3, dq=None, db=None, dPx=None, dAx=None, dl=None, du=None):
         """cosmo_b200_adjoint: the gradients of a loss with respect to the data from its gradients dx, dy, ds with
         respect to the last polished solution (fp64, host or CUDA arrays; None: zero).  dq (n), db, dl, du (m), dPx and
         dAx (the ``data`` order of P and A as given to create / update_matrices) are fp64 outputs, host or CUDA arrays;
         None allocates a NumPy array.  Returns ((dq, db, dPx, dAx, dl, du), stats), stats keyed by ADJOINT_STATS (status 1
         computed, 0 the polish was rejected, -1 it did not apply, the outputs then NaN; the counts as ints)."""
-        gx, gy, gs = (self._arr(a, k, np.float64) for a, k in ((dx, self.n), (dy, self.m), (ds, self.m)))
-        sizes = (self.n, self.m, self.nnzP, self.nnzA, self.m, self.m)
-        outs = [np.empty(k) if a is None else a for a, k in zip((dq, db, dPx, dAx, dl, du), sizes)]
-        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
-        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_adjoint, self._h, int(refine_iter), _ptr(gx), _ptr(gy),
-                       _ptr(gs), *ptrs, ctype=C.c_double, keys=ADJOINT_STATS, ints=ADJOINT_STATS[:3])
-        return tuple(outs), stats
+        return self._reverse(self._lib.cosmo_b200_adjoint, (int(refine_iter),), (dx, dy, ds), (dq, db, dPx, dAx, dl, du),
+                             ADJOINT_STATS, ADJOINT_STATS[:3])
 
     def derivative(self, dPx=None, dq=None, dAx=None, db=None, dl=None, du=None, refine_iter=3, dx=None, dy=None,
                    ds=None):
@@ -633,13 +653,8 @@ class Engine:
         CUDA arrays (None: zero); dx (n), dy, ds (m) are fp64 outputs, host or CUDA arrays, None allocates a NumPy
         array.  Returns ((dx, dy, ds), stats), stats keyed by ADJOINT_STATS (status 1 computed, 0 the polish was
         rejected, -1 it did not apply, the outputs then NaN; the counts as ints)."""
-        sizes = (self.nnzP, self.n, self.nnzA, self.m, self.m, self.m)
-        ins = [self._arr(a, k, np.float64) for a, k in zip((dPx, dq, dAx, db, dl, du), sizes)]
-        outs = [np.empty(k) if a is None else a for a, k in zip((dx, dy, ds), (self.n, self.m, self.m))]
-        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, (self.n, self.m, self.m))]
-        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_derivative, self._h, int(refine_iter),
-                       *(_ptr(a) for a in ins), *ptrs, ctype=C.c_double, keys=ADJOINT_STATS, ints=ADJOINT_STATS[:3])
-        return tuple(outs), stats
+        return self._forward(self._lib.cosmo_b200_derivative, (int(refine_iter),), (dPx, dq, dAx, db, dl, du), (dx, dy, ds),
+                             ADJOINT_STATS, ADJOINT_STATS[:3])
 
     def solve_adjoint(self, dx=None, dy=None, ds=None, tol=0.0, max_iter=500, restart=30, kkt_tol=1e-12, dq=None,
                       db=None, dPx=None, dAx=None, dl=None, du=None):
@@ -648,15 +663,9 @@ class Engine:
         cone but Exp/Pow, complex PSD and custom cones whose type has no Jacobian hook, every single-GPU KKT plugin.  Inputs and outputs as for
         ``adjoint``.  Returns ((dq, db, dPx, dAx, dl, du), stats), stats keyed by SOLVE_ADJOINT_STATS (status 1 computed,
         0 GMRES or a PSD eigensolve did not converge, -1 not applicable, the outputs then NaN; the counts as ints)."""
-        gx, gy, gs = (self._arr(a, k, np.float64) for a, k in ((dx, self.n), (dy, self.m), (ds, self.m)))
-        sizes = (self.n, self.m, self.nnzP, self.nnzA, self.m, self.m)
-        outs = [np.empty(k) if a is None else a for a, k in zip((dq, db, dPx, dAx, dl, du), sizes)]
-        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, sizes)]
         st = SolveAdjointSettings(float(tol), int(max_iter), int(restart), float(kkt_tol), 0)
-        ints = tuple(k for k in SOLVE_ADJOINT_STATS if k != "residual")
-        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_solve_adjoint, self._h, C.byref(st), _ptr(gx), _ptr(gy),
-                       _ptr(gs), *ptrs, ctype=C.c_double, keys=SOLVE_ADJOINT_STATS, ints=ints)
-        return tuple(outs), stats
+        return self._reverse(self._lib.cosmo_b200_solve_adjoint, (C.byref(st),), (dx, dy, ds), (dq, db, dPx, dAx, dl, du),
+                             SOLVE_ADJOINT_STATS, _SOLVE_ADJOINT_INTS)
 
     def solve_derivative(self, dPx=None, dq=None, dAx=None, db=None, dl=None, du=None, tol=0.0, max_iter=500, restart=30,
                          kkt_tol=1e-12, dx=None, dy=None, ds=None):
@@ -666,15 +675,9 @@ class Engine:
         its settings.  Inputs are fp64 host or CUDA arrays (None: zero); dx (n), dy, ds (m) are fp64 outputs, host or
         CUDA arrays, None allocates a NumPy array.  Returns ((dx, dy, ds), stats), stats keyed by SOLVE_ADJOINT_STATS
         (status 1 computed, 0 GMRES or a PSD eigensolve did not converge, -1 not applicable, the outputs then NaN)."""
-        sizes = (self.nnzP, self.n, self.nnzA, self.m, self.m, self.m)
-        ins = [self._arr(a, k, np.float64) for a, k in zip((dPx, dq, dAx, db, dl, du), sizes)]
-        outs = [np.empty(k) if a is None else a for a, k in zip((dx, dy, ds), (self.n, self.m, self.m))]
-        ptrs = [_ptr(self._arr(a, k, np.float64, output=True)) for a, k in zip(outs, (self.n, self.m, self.m))]
         st = SolveAdjointSettings(float(tol), int(max_iter), int(restart), float(kkt_tol), 0)
-        ints = tuple(k for k in SOLVE_ADJOINT_STATS if k != "residual")
-        stats = _keyed(self._lib, self._h, self._lib.cosmo_b200_solve_derivative, self._h, C.byref(st),
-                       *(_ptr(a) for a in ins), *ptrs, ctype=C.c_double, keys=SOLVE_ADJOINT_STATS, ints=ints)
-        return tuple(outs), stats
+        return self._forward(self._lib.cosmo_b200_solve_derivative, (C.byref(st),), (dPx, dq, dAx, db, dl, du),
+                             (dx, dy, ds), SOLVE_ADJOINT_STATS, _SOLVE_ADJOINT_INTS)
 
     def update_matrices(self, Px=None, Ax=None, q=None, b=None):
         """cosmo_b200_update_matrices: new values of P and A on the pattern of create -- ``Px`` / ``Ax`` are the ``data``

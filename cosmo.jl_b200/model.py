@@ -881,11 +881,7 @@ class Model:
         if not self._polished or self.engine is None:
             raise ValueError("adjoint needs the last optimize() to have returned polish == \"Polished\" "
                              "(Settings(polish=True) and a direct KKT solver)")
-        (dq, db, dPx, dAx, dl, du), st = self.engine.adjoint(dx, dy, ds, refine_iter)
-        P0, A0 = self.P0, self.A0
-        return {"P": sp.csc_matrix((dPx, P0.indices, P0.indptr), shape=P0.shape),
-                "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
-                "q": dq, "b": db, "l": dl, "u": du, "stats": st}
+        return self._data_grads(*self.engine.adjoint(dx, dy, ds, refine_iter))
 
     def derivative(self, dP=None, dq=None, dA=None, db=None, dl=None, du=None, refine_iter=3):
         """Directional derivatives of the polished solution (x, y, s) of the last optimize() along a data direction,
@@ -897,8 +893,7 @@ class Model:
         if not self._polished or self.engine is None:
             raise ValueError("derivative needs the last optimize() to have returned polish == \"Polished\" "
                              "(Settings(polish=True) and a direct KKT solver)")
-        dPx = None if dP is None else _pattern_values(dP, self.P0, "dP")
-        dAx = None if dA is None else _pattern_values(dA, self.A0, "dA")
+        dPx, dAx = self._direction_values(dP, dA)
         (dx, dy, ds), st = self.engine.derivative(dPx, dq, dAx, db, dl, du, refine_iter)
         return {"x": dx, "y": dy, "s": ds, "stats": st}
 
@@ -913,11 +908,7 @@ class Model:
             raise ValueError("solve_adjoint needs a solve: call optimize() first")
         if self._dec is not None:
             raise ValueError("solve_adjoint does not map gradients through a chordal decomposition (decompose=True)")
-        (dq, db, dPx, dAx, dl, du), st = self.engine.solve_adjoint(dx, dy, ds, tol, max_iter, restart, kkt_tol)
-        P0, A0 = self.P0, self.A0
-        return {"P": sp.csc_matrix((dPx, P0.indices, P0.indptr), shape=P0.shape),
-                "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
-                "q": dq, "b": db, "l": dl, "u": du, "stats": st}
+        return self._data_grads(*self.engine.solve_adjoint(dx, dy, ds, tol, max_iter, restart, kkt_tol))
 
     def solve_derivative(self, dP=None, dq=None, dA=None, db=None, dl=None, du=None, tol=0.0, max_iter=500, restart=30,
                          kkt_tol=1e-12):
@@ -932,10 +923,22 @@ class Model:
             raise ValueError("solve_derivative needs a solve: call optimize() first")
         if self._dec is not None:
             raise ValueError("solve_derivative does not map directions through a chordal decomposition (decompose=True)")
-        dPx = None if dP is None else _pattern_values(dP, self.P0, "dP")
-        dAx = None if dA is None else _pattern_values(dA, self.A0, "dA")
+        dPx, dAx = self._direction_values(dP, dA)
         (dx, dy, ds), st = self.engine.solve_derivative(dPx, dq, dAx, db, dl, du, tol, max_iter, restart, kkt_tol)
         return {"x": dx, "y": dy, "s": ds, "stats": st}
+
+    def _data_grads(self, grads, st):
+        """The dict of adjoint() and solve_adjoint() from the engine's (dq, db, dPx, dAx, dl, du) and stats."""
+        dq, db, dPx, dAx, dl, du = grads
+        P0, A0 = self.P0, self.A0
+        return {"P": sp.csc_matrix((dPx, P0.indices, P0.indptr), shape=P0.shape),
+                "A": sp.csc_matrix((dAx, A0.indices, A0.indptr), shape=A0.shape),
+                "q": dq, "b": db, "l": dl, "u": du, "stats": st}
+
+    def _direction_values(self, dP, dA):
+        """dP and dA of derivative() and solve_derivative() as values on the patterns of P0 and A0 (None stays None)."""
+        return (None if dP is None else _pattern_values(dP, self.P0, "dP"),
+                None if dA is None else _pattern_values(dA, self.A0, "dA"))
 
     def solution_into(self, x=None, y=None, s=None):
         """The last solution (x, y, s of Result, completed as settings.complete_dual asks) into caller fp64 arrays, CUDA
