@@ -12,22 +12,64 @@
 // inner products run over [lo, dim) with lo = 0 on rank 0 and lo = n elsewhere, followed by an allreduce, so
 // every rank holds the same R and eta and applies the same update to its copy of w_x.
 #pragma once
+#include <cmath>
+
 #include "common.cuh"
 
 namespace cosmo {
 
-enum { AA_F2 = 0, AA_FACC2 = 1, AA_FLAG = 2, AA_NRM2 = 3, AA_SC_COUNT = 8 };
+// AA_F2 and AA_FACC2 hold the AA_SSQ scaled sums of squares of aa_ssq_add each
+enum { AA_SSQ = 3, AA_F2 = 0, AA_FACC2 = AA_SSQ, AA_FLAG = 2 * AA_SSQ, AA_NRM2 = AA_FLAG + 1, AA_SC_COUNT = 8 };
+
+// The safeguard's two norms |f|_2 and |f_acc|_2 (accelerator_interface.jl:90,120-123) are the reference's norm(f, 2),
+// which rescales and neither overflows nor underflows.  A plain sum of squares in T overflows once |f|_2 passes
+// sqrt(max(T)) (1.8e19 in float32), and the test nrm_f_acc > tol * nrm_f then never declines.  So each entry goes to
+// one of three sums of squares by its magnitude, with the thresholds and power-of-two scales of LAPACK's dnrm2 (Blue's
+// algorithm, la_constants.f90): x^2 for tsml <= |x| <= tbig, (x sbig)^2 above, (x ssml)^2 below.  Scaling by a power of
+// two is exact, no sum overflows or underflows to zero for any finite entry of T, and the three are plain sums, so a
+// sharded allreduce adds them like any other.  aa_norm combines them on the host.  A NaN entry lands in the middle sum.
+template <typename T> struct AaBlue;
+template <> struct AaBlue<double> {
+  static constexpr double tsml = 0x1p-511, tbig = 0x1p486, ssml = 0x1p537, sbig = 0x1p-538;
+};
+template <> struct AaBlue<float> {
+  static constexpr float tsml = 0x1p-63f, tbig = 0x1p52f, ssml = 0x1p75f, sbig = 0x1p-76f;
+};
+
+template <typename T>
+__device__ __forceinline__ void aa_ssq_add(T (&acc)[AA_SSQ], T x) {
+  const T a = tabs(x);
+  if (a > AaBlue<T>::tbig) {
+    const T y = x * AaBlue<T>::sbig;
+    acc[1] += y * y;
+  } else if (a < AaBlue<T>::tsml) {
+    const T y = x * AaBlue<T>::ssml;
+    acc[2] += y * y;
+  } else {
+    acc[0] += x * x;
+  }
+}
+
+// |x|_2 from the AA_SSQ sums of aa_ssq_add, in double.  Only the middle sum is set for every vector whose entries lie in
+// [tsml, tbig] or are zero, and the result is then sqrt of that sum, as a single sum of squares gives.  NaN when a sum is.
+template <typename T>
+inline double aa_norm(const T* s) {
+  const double mid = sqrt((double)s[0]), big = sqrt((double)s[1]) / (double)AaBlue<T>::sbig,
+               sml = sqrt((double)s[2]) / (double)AaBlue<T>::ssml;
+  if (mid != mid || big != big || sml != sml) return NAN;
+  return std::hypot(std::hypot(mid, big), sml);
+}
 
 // CA.update! of every variant: f = x - g; after a restart only (g_last, f_last and, for Type1, x_last) are stored;
 // otherwise G[:, j] = g - g_last, F[:, j] = f - f_last and, for Type1 (Xj != nullptr), X[:, j] = x - x_last.
 // F lives in Q; the QR variant orthogonalises the new column afterwards.
-// out[0] = |f|^2 over [lo, dim)  (the safeguard's reference norm, accelerator_interface.jl:90).
+// out[0:AA_SSQ] = the scaled sums of squares of f over [lo, dim) (the safeguard's reference norm, accelerator_interface.jl:90).
 template <typename T>
 __global__ void __launch_bounds__(kBlock) aa_hist_kernel(int dim, int lo, const T* __restrict__ g, const T* __restrict__ x,
                                                          T* __restrict__ f, T* __restrict__ f_last, T* __restrict__ g_last,
                                                          T* __restrict__ x_last, T* __restrict__ Gj, T* __restrict__ Fj,
                                                          T* __restrict__ Xj, int init, RedBuf<T> rb) {
-  T accS[1] = {0};
+  T accS[AA_SSQ] = {0, 0, 0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dim; i += gridDim.x * blockDim.x) {
     const T gi = g[i], xi = x[i];
     const T fi = xi - gi;
@@ -40,9 +82,9 @@ __global__ void __launch_bounds__(kBlock) aa_hist_kernel(int dim, int lo, const 
     g_last[i] = gi;
     f_last[i] = fi;
     if (x_last) x_last[i] = xi;
-    if (i >= lo) accS[0] += fi * fi;
+    if (i >= lo) aa_ssq_add(accS, fi);
   }
-  reduce_and_finalize<T, 1, 0>(accS, (const T*)nullptr, rb, NoFin());
+  reduce_and_finalize<T, AA_SSQ, 0>(accS, (const T*)nullptr, rb, NoFin());
 }
 
 // One modified Gram-Schmidt step on the new column q:
@@ -243,17 +285,18 @@ __global__ void __launch_bounds__(32) aa_ne_solve_kernel(const T* __restrict__ g
   flag[0] = ok ? T(1) : T(0);
 }
 
-// compute_accelerated_res_norm! (accelerator_interface.jl:120-123): f = w_prev - w, out[0] = |f|^2
+// compute_accelerated_res_norm! (accelerator_interface.jl:120-123): f = w_prev - w, out[0:AA_SSQ] = the scaled sums of
+// squares of f (aa_ssq_add)
 template <typename T>
 __global__ void __launch_bounds__(kBlock) aa_res_kernel(int dim, int lo, const T* __restrict__ w_prev, const T* __restrict__ w,
                                                         T* __restrict__ f, RedBuf<T> rb) {
-  T accS[1] = {0};
+  T accS[AA_SSQ] = {0, 0, 0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dim; i += gridDim.x * blockDim.x) {
     const T fi = w_prev[i] - w[i];
     f[i] = fi;
-    if (i >= lo) accS[0] += fi * fi;
+    if (i >= lo) aa_ssq_add(accS, fi);
   }
-  reduce_and_finalize<T, 1, 0>(accS, (const T*)nullptr, rb, NoFin());
+  reduce_and_finalize<T, AA_SSQ, 0>(accS, (const T*)nullptr, rb, NoFin());
 }
 
 }  // namespace cosmo

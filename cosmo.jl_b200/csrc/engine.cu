@@ -178,6 +178,8 @@ class EngineBase {
   virtual void p2p_attach(const void* blobs, int nranks) = 0;
   virtual void set_accelerator(const cosmo_b200_accelerator* acc) = 0;
   virtual void accelerator_stats(int64_t* out6) = 0;
+  virtual void accelerator_probe(long long K, const void* g, const void* x, const void* w_next, void* cand, double* eta,
+                                 int64_t* info, double* safeguard) = 0;
   virtual void infeasibility_test(int which, const void* delta, double* out8) = 0;
   virtual void psd_lambda_max(const void* v, double* lam) = 0;
   virtual void ldl_stats(double* out8) = 0;
@@ -241,6 +243,8 @@ class Engine : public EngineBase {
   void p2p_attach(const void* blobs, int nranks) override;
   void set_accelerator(const cosmo_b200_accelerator* acc) override;
   void accelerator_stats(int64_t* out6) override;
+  void accelerator_probe(long long K, const void* g, const void* x, const void* w_next, void* cand, double* eta, int64_t* info,
+                         double* safeguard) override;
   void infeasibility_test(int which, const void* delta, double* out8) override;
   void psd_lambda_max(const void* v, double* lam) override;
   // the supernodal plugin's when it is the KKT solver, otherwise the simplicial one's; zeros from a plugin never built
@@ -340,6 +344,7 @@ class Engine : public EngineBase {
   void aa_restart() { aa_iter_ = 0; aa_init_ = true; aa_fresh_ = false; }
   void aa_update(const T* g, const T* x);
   bool aa_accelerate(T* g);
+  bool aa_safeguard_declines(const T* w_prev, const T* w, double* nrm2);
   // ---- state ----
   DevBuf<T> W_[2];           // operator variable, ping-pong (w / w_prev)
   int cur_ = 0, prev_ = 1;
@@ -2309,7 +2314,7 @@ void Engine<T>::aa_update(const T* g, const T* x) {
                                                   aaG_.p + (size_t)j * dim, q, type1 ? aaX_.p + (size_t)j * dim : nullptr,
                                                   aa_init_ ? 1 : 0, red_ptr(aa_sc_.p + AA_F2));
   check_launch("aa_hist");
-  allreduce_sum(aa_sc_.p + AA_F2, 1);
+  allreduce_sum(aa_sc_.p + AA_F2, AA_SSQ);
   if (aa_init_) { aa_init_ = false; return; }
   if (aa_qr()) {
     T* Rj = aaR_.p + (size_t)j * aa_mem_;        // column j of R
@@ -2375,6 +2380,77 @@ bool Engine<T>::aa_accelerate(T* g) {
   sync();
   if (h_aa_[AA_FLAG] == T(0)) { ++aa_rejected_; return false; }
   return true;
+}
+
+// The safeguard of acceleration_post! (accelerator_interface.jl:85-97,120-123), for the solve loop and the probe:
+// f_acc = w_prev - w (into aa_f_), declined when |f_acc|_2 > safeguard_tol |f|_2 with f the residual of the last
+// aa_update.  Both norms are overflow-safe (aa_norm); nrm2 = {|f|_2, |f_acc|_2}.
+template <typename T>
+bool Engine<T>::aa_safeguard_declines(const T* w_prev, const T* w, double* nrm2) {
+  const int dim = n_ + m_, lo = (rank_ == 0) ? 0 : n_;
+  aa_res_kernel<T><<<vgrid(dim), kBlock, 0, stream_>>>(dim, lo, w_prev, w, aa_f_.p, red_ptr(aa_sc_.p + AA_FACC2));
+  check_launch("aa_res");
+  allreduce_sum(aa_sc_.p + AA_FACC2, AA_SSQ);
+  CUDA_TRY(cudaMemcpyAsync(h_aa_.p, aa_sc_.p, 2 * AA_SSQ * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+  sync();
+  nrm2[0] = aa_norm(h_aa_.p + AA_F2);
+  nrm2[1] = aa_norm(h_aa_.p + AA_FACC2);
+  return nrm2[1] > nrm2[0] * st_.safeguard_tol;
+}
+
+// The accelerator on K caller pairs (g_k, x_k), from a restart: aa_update(g_k, x_k), then aa_accelerate on the engine's
+// copy of g_k, and with w_next the safeguard of the candidate against w_next_k.  The accelerator state is rebuilt at the
+// start of every accelerated solve (aa_prepare); what the last solve reported -- the counters of accelerator_stats and
+// the activation flags -- is put back afterwards, and the iterates, rho and the plugin state are not touched.
+template <typename T>
+void Engine<T>::accelerator_probe(long long K, const void* g, const void* x, const void* w_next, void* cand, double* eta,
+                                  int64_t* info, double* sg) {
+  single_gpu("accelerator_probe");
+  if (K < 0) throw EngineError{COSMO_B200_ERR_INVALID, "accelerator_probe: K must not be negative"};
+  CUDA_TRY(cudaSetDevice(device_));
+  const size_t dim = (size_t)n_ + m_;
+  const long long saved[6] = {aa_accelerated_, aa_declined_, aa_rejected_, aa_rho_restarts_, aa_mem_restarts_, aa_activated_at_};
+  const bool saved_active = aa_active_, saved_success = aa_success_;
+  aa_prepare();
+  DevBuf<T> buf;
+  buf.alloc(3 * dim);
+  T* gk = buf.p;
+  T* xk = buf.p + dim;
+  T* wn = buf.p + 2 * dim;
+  std::vector<T> h_eta(32);
+  const int min_mem = std::max(st_.accelerator_min_mem, 1);
+  for (long long k = 0; k < K; ++k) {
+    const size_t off = (size_t)k * dim * sizeof(T);
+    CUDA_TRY(cudaMemcpyAsync(gk, (const char*)g + off, dim * sizeof(T), cudaMemcpyDefault, stream_));
+    CUDA_TRY(cudaMemcpyAsync(xk, (const char*)x + off, dim * sizeof(T), cudaMemcpyDefault, stream_));
+    aa_update(gk, xk);
+    const bool fresh = aa_fresh_;
+    const int l = fresh ? std::min(aa_iter_, aa_mem_) : 0;
+    const bool formed = fresh && l >= min_mem;
+    const bool accepted = aa_accelerate(gk);
+    for (int c = 0; c < 32; ++c) eta[k * 32 + c] = NAN;
+    if (accepted) {
+      CUDA_TRY(cudaMemcpyAsync(h_eta.data(), aa_eta_.p, l * sizeof(T), cudaMemcpyDeviceToHost, stream_));
+      sync();
+      for (int c = 0; c < l; ++c) eta[k * 32 + c] = (double)h_eta[c];
+    }
+    info[4 * k] = formed ? 1 : 0;
+    info[4 * k + 1] = accepted ? 1 : 0;
+    info[4 * k + 2] = l;
+    info[4 * k + 3] = fresh ? aa_j_ : -1;
+    CUDA_TRY(cudaMemcpyAsync((char*)cand + off, gk, dim * sizeof(T), cudaMemcpyDefault, stream_));
+    if (w_next) {
+      CUDA_TRY(cudaMemcpyAsync(wn, (const char*)w_next + off, dim * sizeof(T), cudaMemcpyDefault, stream_));
+      double nrm[2];
+      sg[3 * k] = aa_safeguard_declines(gk, wn, nrm) ? 1.0 : 0.0;
+      sg[3 * k + 1] = nrm[0];
+      sg[3 * k + 2] = nrm[1];
+    }
+  }
+  sync();
+  aa_accelerated_ = saved[0]; aa_declined_ = saved[1]; aa_rejected_ = saved[2];
+  aa_rho_restarts_ = saved[3]; aa_mem_restarts_ = saved[4]; aa_activated_at_ = saved[5];
+  aa_active_ = saved_active; aa_success_ = saved_success;
 }
 
 template <typename T>
@@ -2530,16 +2606,10 @@ void Engine<T>::solve(cosmo_b200_result* out) {
     prev_ = src; cur_ = dst;
     // acceleration_post! (accelerator_interface.jl:85-114): safeguard the accelerated candidate
     if (use_aa && aa_active_ && aa_success_ && st_.safeguard) {
-      const int dim = n + m, lo = (rank_ == 0) ? 0 : n;
-      aa_res_kernel<T><<<vgrid(dim), kBlock, 0, stream_>>>(dim, lo, W_[prev_].p, W_[cur_].p, aa_f_.p, red_ptr(aa_sc_.p + AA_FACC2));
-      check_launch("aa_res");
-      allreduce_sum(aa_sc_.p + AA_FACC2, 1);
-      CUDA_TRY(cudaMemcpyAsync(h_aa_.p, aa_sc_.p, 2 * sizeof(T), cudaMemcpyDeviceToHost, stream_));
-      sync();
-      const double nrm_f = sqrt((double)h_aa_[AA_F2]), nrm_f_acc = sqrt((double)h_aa_[AA_FACC2]);
-      if (nrm_f_acc > nrm_f * st_.safeguard_tol) {
+      double nrm[2];
+      if (aa_safeguard_declines(W_[prev_].p, W_[cur_].p, nrm)) {
         // decline: w_prev = w = g_last, then one plain ADMM step from there (:100-106)
-        CUDA_TRY(cudaMemcpyAsync(W_[prev_].p, aa_glast_.p, (size_t)dim * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
+        CUDA_TRY(cudaMemcpyAsync(W_[prev_].p, aa_glast_.p, (size_t)(n + m) * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
         xw_step(prev_, cur_, true, nullptr);
         ++safeguarding_iter;
         ++aa_declined_;
@@ -3965,6 +4035,11 @@ int cosmo_b200_set_accelerator(cosmo_b200_handle* h, const cosmo_b200_accelerato
 int cosmo_b200_accelerator_stats(cosmo_b200_handle* h, int64_t out[6]) {
   if (!out) return COSMO_B200_ERR_INVALID;
   ABI_GUARD(h, h->impl->accelerator_stats(out));
+}
+int cosmo_b200_accelerator_probe(cosmo_b200_handle* h, int64_t K, const void* g, const void* x, const void* w_next, void* cand,
+                                 double* eta, int64_t* info, double* safeguard) {
+  if (K > 0 && (!g || !x || !cand || !eta || !info || (w_next && !safeguard))) return COSMO_B200_ERR_INVALID;
+  ABI_GUARD(h, h->impl->accelerator_probe(K, g, x, w_next, cand, eta, info, safeguard));
 }
 int cosmo_b200_infeasibility_test(cosmo_b200_handle* h, int32_t which, const void* delta, double out[8]) {
   if (!delta || !out) return COSMO_B200_ERR_INVALID;

@@ -157,6 +157,7 @@ def _signatures():
         "cosmo_b200_reset": (rc, [vp]),
         "cosmo_b200_set_accelerator": (rc, [vp, P(AcceleratorStruct)]),
         "cosmo_b200_accelerator_stats": (rc, [vp, P(i64)]),
+        "cosmo_b200_accelerator_probe": (rc, [vp, i64, vp, vp, vp, vp, P(f64), P(i64), P(f64)]),
         "cosmo_b200_solve": (rc, [vp, P(ResultStruct)]),
         "cosmo_b200_project": (rc, [vp, vp, vp]),
         "cosmo_b200_project_jacobian": (rc, [vp, vp, vp, vp, P(i64)]),
@@ -813,6 +814,33 @@ class Engine:
     def accelerator_stats(self):
         """Accelerator events of the last solve (cosmo_b200_accelerator_stats), keyed by ACCELERATOR_STATS."""
         return self._read_out(self._lib.cosmo_b200_accelerator_stats, ctype=C.c_int64, keys=ACCELERATOR_STATS)
+
+    def accelerator_probe(self, g, x, w_next=None):
+        """cosmo_b200_accelerator_probe: the accelerator of this engine (set_accelerator, accelerator_mem, min_mem,
+        safeguard_tol) run from a restart on the K pairs g[k], x[k] (K x (n+m) arrays of the engine's dtype), each an
+        update followed by an accelerate on a copy of g[k]; w_next[k], when given, is safeguarded against.  Returns a
+        dict: "cand" (K x (n+m), g[k] bit for bit unless accepted), "eta" (K x 32 fp64 in physical column order, NaN past
+        l and unless accepted), "formed", "accepted", "l", "j" (int arrays of K; j = -1: no column written) and, with
+        w_next, "declined" (bool), "nrm_f" and "nrm_f_acc".  Leaves the solve state as it was."""
+        dim = self.n + self.m
+        g = np.ascontiguousarray(g, dtype=self.dtype).reshape(-1, dim)
+        x = np.ascontiguousarray(x, dtype=self.dtype).reshape(-1, dim)
+        K = g.shape[0]
+        if x.shape[0] != K:
+            raise EngineError(ERR_INVALID, "g and x must hold the same number of vectors")
+        wn = None if w_next is None else np.ascontiguousarray(w_next, dtype=self.dtype).reshape(K, dim)
+        cand = np.empty((K, dim), dtype=self.dtype)
+        eta = np.empty((max(K, 1), 32))
+        info = np.zeros((max(K, 1), 4), dtype=np.int64)
+        sg = np.full((max(K, 1), 3), np.nan)
+        self._check(self._lib.cosmo_b200_accelerator_probe(
+            self._h, K, _ptr(g), _ptr(x), _ptr(wn), _ptr(cand), eta.ctypes.data_as(C.POINTER(C.c_double)),
+            info.ctypes.data_as(C.POINTER(C.c_int64)), sg.ctypes.data_as(C.POINTER(C.c_double))))
+        out = {"cand": cand, "eta": eta[:K], "formed": info[:K, 0], "accepted": info[:K, 1], "l": info[:K, 2],
+               "j": info[:K, 3]}
+        if wn is not None:
+            out.update(declined=sg[:K, 0] == 1.0, nrm_f=sg[:K, 1], nrm_f_acc=sg[:K, 2])
+        return out
 
     def infeasibility_test(self, which, delta):
         """cosmo_b200_infeasibility_test: is_primal_infeasible! (which = 0, delta = delta_y, m) or is_dual_infeasible!

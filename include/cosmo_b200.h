@@ -334,6 +334,17 @@ int cosmo_b200_set_accelerator(cosmo_b200_handle* h, const cosmo_b200_accelerato
    (singular, non-finite or |eta| > 1e4), restarts after a rho adaptation, memory restarts, iteration at which the
    accelerator became active (0: never)} */
 int cosmo_b200_accelerator_stats(cosmo_b200_handle* h, int64_t out[6]);
+/* Test hook: the handle's accelerator (cosmo_b200_set_accelerator; accelerator_mem, accelerator_min_mem and
+   safeguard_tol of the settings) run from a restart on K caller pairs.  Pair k is update!(g_k, x_k) followed by
+   accelerate! on a copy of g_k.  g, x and w_next hold K vectors of n+m values of the handle's dtype one after another,
+   host or device memory; w_next may be NULL.  Per pair: cand[k] = the candidate (g_k bit for bit when none was formed
+   or it was rejected); eta[32 k + c] = the coefficient of physical history column c, as fp64, NaN past l and everywhere
+   unless the candidate was accepted; info[4 k + 0..3] = {formed, accepted, l, physical column written (-1: none)};
+   with w_next, safeguard[3 k + 0..2] = {declined, |f_k|_2, |cand_k - w_next_k|_2}, the test of the solve loop.  The
+   iterates, rho, the plugin state, accelerator_stats and the next solve are not changed.  ERR_UNSUPPORTED for sharded
+   handles. */
+int cosmo_b200_accelerator_probe(cosmo_b200_handle* h, int64_t K, const void* g, const void* x, const void* w_next, void* cand,
+                                 double* eta, int64_t* info, double* safeguard);
 
 /* ---- the hot loop (solver.jl:125-167) ------------------------------------ */
 int cosmo_b200_solve(cosmo_b200_handle* h, cosmo_b200_result* out);

@@ -4,7 +4,8 @@ It exists to exercise, without a GPU, the Python side of everything that normall
 glue of Model (scaling, decomposition, warm starts) and the bodies of the GPU tests themselves (so a typo in a GPU
 test is found by the CPU run, not at the next GPU run).  It implements the part of the call surface those users need:
 ctor, update_settings, warm_start, update_qb, update_matrices, project, project_jacobian, solve, w, rho_vec, scaling,
-spmv, residuals, close, and the infeasibility hooks infeasibility_test and psd_lambda_max."""
+spmv, residuals, close, the infeasibility hooks infeasibility_test and psd_lambda_max, and set_accelerator with the
+accelerator_probe hook."""
 import numpy as np
 import scipy.sparse as sp
 
@@ -61,6 +62,7 @@ class OracleEngine:
             self._scal = (sm.D, sm.E, sm.c)
             self.scaled = True
         self._w = self._rho = self._warm = None
+        self._acc = None
         OracleEngine.instances.append(self)
 
     def scaling(self):
@@ -143,6 +145,62 @@ class OracleEngine:
         out.rho, out.rho_updates, out.times = 0.1, list(r.info.rho_updates), {"iter_time_device": 0.0}
         out.kkt_inner_iterations = out.kkt_multiplications = out.kernel_launches = 0
         return out
+
+    def set_accelerator(self, acc):
+        self._acc = acc
+
+    def accelerator_probe(self, g, x, w_next=None):
+        """cosmo_b200_accelerator_probe through the two fp64 restatements: oracle.cosmo_oracle.AndersonAccelerator for
+        Type2{QRDecomp}, tests/anderson_variants.NormalEquationsAccelerator for the others"""
+        from cosmo_b200 import model as M
+        from tests import anderson_variants as V
+        names = lambda table, v: {i: k for k, i in table.items()}[v]
+        a = self._acc
+        t = "Type2{QRDecomp}" if a is None else names(M.Settings._AA_TYPE, a.type)
+        memory = "RestartedMemory" if a is None else names(M.Settings._AA_MEMORY, a.memory)
+        reg = "NoRegularizer" if a is None else names(M.Settings._AA_REG, a.regularizer)
+        lam = 0.0 if a is None else float(self.dtype.type(a.lambda_))
+        dim = self.n + self.m
+        g = np.asarray(g, dtype=self.dtype).reshape(-1, dim)
+        x = np.asarray(x, dtype=self.dtype).reshape(-1, dim)
+        K = g.shape[0]
+        if x.shape[0] != K:
+            raise E.EngineError(E.ERR_INVALID, "g and x must hold the same number of vectors")
+        if t == "Type2{QRDecomp}":
+            aa = O.AndersonAccelerator(dim, self.st.accelerator_mem, self.st.accelerator_min_mem)
+        else:
+            aa = V.NormalEquationsAccelerator(dim, self.st.accelerator_mem, self.st.accelerator_min_mem,
+                                              type1=t == "Type1", rolling=memory == "RollingMemory", regularizer=reg,
+                                              lam=lam)
+        out = {"cand": g.copy(), "eta": np.full((K, 32), np.nan), "formed": np.zeros(K, dtype=np.int64),
+               "accepted": np.zeros(K, dtype=np.int64), "l": np.zeros(K, dtype=np.int64), "j": np.full(K, -1, dtype=np.int64)}
+        sg = np.full((K, 3), np.nan)
+        with np.errstate(all="ignore"):
+            for k in range(K):
+                gk, xk = g[k].astype(float), x[k].astype(float)
+                init = aa.init_phase
+                rejected = len([e for e in aa.log if e[1] == "acc_failed"])
+                aa.update(gk, xk, k)
+                j = aa.j if hasattr(aa, "j") else (aa.iter - 1) % aa.mem
+                l = 0 if init else min(aa.iter, aa.mem)
+                cand = gk.copy()
+                aa.accelerate(cand, xk, k)
+                formed = aa.success or len([e for e in aa.log if e[1] == "acc_failed"]) > rejected
+                out["formed"][k], out["accepted"][k], out["l"][k] = formed, aa.success, l
+                out["j"][k] = -1 if init else j
+                if aa.success:
+                    out["cand"][k] = cand.astype(self.dtype)
+                    out["eta"][k, :l] = aa.eta[:l]
+                if w_next is not None:
+                    wn = np.asarray(w_next, dtype=self.dtype).reshape(K, dim)[k].astype(float)
+                    nf, nacc = np.linalg.norm(aa.f), np.linalg.norm(out["cand"][k].astype(float) - wn)
+                    sg[k] = (float(nacc > nf * self.st.safeguard_tol), nf, nacc)
+        if w_next is not None:
+            out.update(declined=sg[:, 0] == 1.0, nrm_f=sg[:, 1], nrm_f_acc=sg[:, 2])
+        return out
+
+    def accelerator_stats(self):
+        return dict.fromkeys(E.ACCELERATOR_STATS, 0)
 
     def infeasibility_test(self, which, delta):
         """cosmo_b200_infeasibility_test through the oracle's scaled_norm / in_dual / in_pol_recc / support_function"""

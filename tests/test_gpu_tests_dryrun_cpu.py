@@ -1,7 +1,7 @@
 """Dry run of GPU test bodies on the CPU: the CUDA engine is replaced by the oracle-backed stand-in of
 tests/oracle_engine.py and the functions of tests/test_gpu_parity.py, tests/test_gpu_float32.py and
 tests/test_gpu_scale_edges.py, tests/test_gpu_infeasibility.py, tests/test_gpu_projection_jacobian.py and
-tests/test_gpu_ruiz.py are called directly.  What this checks is the
+tests/test_gpu_ruiz.py and tests/test_gpu_anderson.py are called directly.  What this checks is the
 Python side of those tests (imports, helpers, fixtures, the host glue they drive) -- a NameError in a GPU test would
 otherwise only show up on the next GPU run.  Assertion failures are tolerated where the stand-in legitimately differs
 from the engine (it ignores the D/E unscaling of the termination test); every other exception fails the test."""
@@ -50,7 +50,15 @@ CASES = ["test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_t
          "test_gpu_ruiz::test_cost_scaling_guard", "test_gpu_ruiz::test_dynamic_range_clips_in_every_pass",
          "test_gpu_ruiz::test_every_rectified_family", "test_gpu_ruiz::test_box_bounds_and_row_classes",
          "test_gpu_ruiz::test_long_rows_and_n_above_1024", "test_gpu_ruiz::test_wide_qp_slabs_hold_the_scaled_values",
-         "test_gpu_ruiz::test_scaled_P_is_symmetric", "test_gpu_ruiz::test_update_matrices_reproduces_a_fresh_engine"]
+         "test_gpu_ruiz::test_scaled_P_is_symmetric", "test_gpu_ruiz::test_update_matrices_reproduces_a_fresh_engine",
+         "test_gpu_anderson::test_windows_and_dimensions", "test_gpu_anderson::test_prescribed_condition",
+         "test_gpu_anderson::test_grid_stride_wrap", "test_gpu_anderson::test_min_mem_above_the_window",
+         "test_gpu_anderson::test_exact_duplicate_differences", "test_gpu_anderson::test_eta_norm_rule",
+         "test_gpu_anderson::test_non_finite_inputs", "test_gpu_anderson::test_pivot_ties_of_opposite_sign",
+         "test_gpu_anderson::test_safeguard_norms_over_the_whole_range",
+         "test_gpu_anderson::test_overflowing_squares_never_accept_non_finite",
+         "test_gpu_anderson::test_power_of_two_ladder_and_determinism",
+         "test_gpu_anderson::test_probe_leaves_the_solve_state_untouched", "test_gpu_anderson::test_report_worst_ratios"]
 MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_sdp_through_the_clique_batch",
              "test_project_exp_pow_cones", "test_soc_branches", "test_complex_psd_cone_projection_and_least_eigenvalue",
              "test_gpu_float32::test_clamp_cones_bit_exact_float32", "test_gpu_float32::test_project_psd_small_batch_float32",
@@ -65,7 +73,10 @@ MUST_PASS = {"test_engine_matches_committed_golden_iterates", "test_g6_chordal_s
              "test_gpu_ruiz::test_clip_edges_at_the_first_pass", "test_gpu_ruiz::test_zero_rows_and_columns_keep_the_scale_one",
              "test_gpu_ruiz::test_cost_scaling_guard", "test_gpu_ruiz::test_scaled_P_is_symmetric",
              "test_gpu_ruiz::test_every_rectified_family",
-             "test_gpu_ruiz::test_update_matrices_reproduces_a_fresh_engine"}
+             "test_gpu_ruiz::test_update_matrices_reproduces_a_fresh_engine",
+             "test_gpu_anderson::test_windows_and_dimensions", "test_gpu_anderson::test_min_mem_above_the_window",
+             "test_gpu_anderson::test_exact_duplicate_differences", "test_gpu_anderson::test_eta_norm_rule",
+             "test_gpu_anderson::test_non_finite_inputs", "test_gpu_anderson::test_pivot_ties_of_opposite_sign"}
 
 
 def _calls(fn):
